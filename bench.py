@@ -5,7 +5,7 @@
   python bench.py --impl reference [...]                         the reference arm: the CPU decoder on the host cores
 
 A "step" = one pass of the hot path over one batch: every rank decodes its shard of independent streams
-(N = 1: BASELINE configs[1], 4096 x 64 KiB synthetic-text streams; N > 1: configs[2], 8192 streams per GPU -- weak scaling: the
+(N = 1: BASELINE configs[1], 4096 x 64 KiB synthetic-text streams; N > 1: configs[2], 4096 streams per GPU -- weak scaling: the
 per-GPU batch is fixed as N grows).
 `value` times K steps with inputs resident in HBM (CUDA events on the launching stream, max over ranks);
 `e2e` repeats the measurement through the host-buffer C-ABI call (pinned host memory, H2D + D2H inside the timed
@@ -32,7 +32,7 @@ sys.path.insert(0, ROOT)
 
 STREAM_BYTES = 65536
 STREAMS_PER_GPU = 4096           # N = 1 (BASELINE configs[1])
-STREAMS_PER_GPU_SCALING = 8192   # N > 1 (BASELINE configs[2]: 65536 streams at 8 GPUs)
+STREAMS_PER_GPU_SCALING = 4096   # N > 1 (BASELINE configs[2]: 32768 streams at 8 GPUs; one 16-lane pass on an 80 GB H100)
 METRIC = "decompressed MB/s (batched 64KiB streams)"
 UNIT = "MB/s"
 
@@ -44,12 +44,12 @@ def _peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3), not a measured figure"
 
 
 class ClockSampler(threading.Thread):
-    """SM clock / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe): NVML in-process every
-    ~10 ms when nvidia_ml_py is importable, else the `nvidia-smi --query-gpu` line the recipe gives (one call ~0.1 s)."""
+    """SM clock / throttle reasons sampled DURING the timed region: NVML in-process every ~10 ms when nvidia_ml_py is
+    importable, else one `nvidia-smi --query-gpu` line per sample (one call ~0.1 s)."""
 
     def __init__(self, index, uuid=None):
         super().__init__(daemon=True)
@@ -181,7 +181,7 @@ def run_reference_arm(args):
     """--impl reference: the reference's CPU implementation of the path (the oracle port: the Rust crate cannot be compiled in
     this image) on all host threads, same workload / metric.  Every step decodes the same fixed sample (2048 streams) after one
     untimed warm pass per thread pool; the line reports the MEDIAN step (a CPU arm on a shared host moves a lot between
-    boxes: the median of >= 5 steps and the fixed sample are what keep it comparable) and the single-thread figure."""
+    boxes: the median step and the fixed sample are what keep it comparable) and the single-thread figure."""
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
         return 0
@@ -193,7 +193,7 @@ def run_reference_arm(args):
     enc, eoff, elen = O.encode_batch(blob, off, ln, O.options(), threads)
     for _ in range(max(1, args.warmup)):
         O.decode_batch(enc, eoff, elen, off, ln, threads)
-    steps = max(5, args.steps)
+    steps = args.steps
     ts = []
     for _ in range(steps):
         t0 = time.perf_counter()
@@ -258,7 +258,7 @@ def _compact(out, eoff, out_len):
     return comp, coff, out_len.astype(np.uint64)
 
 
-def measure_populations(eng, torch, dev, stream, blob, off, ln, steps=3):
+def measure_populations(eng, torch, dev, stream, blob, off, ln, steps):
     """SURVEY 8d: the same raw streams under the other encodings.  Inputs are produced by the product's own GPU encoder (Z: the
     library's greedy LZ77 command generator + the GPU command-list encoder)."""
     import divans_b200
@@ -306,7 +306,7 @@ def run_entropy(args, eng, rank, world, dev):
         out_len, status = eng.encode_batch_host(blob, off, ln, out, eoff, cap, divans_b200.encode_options())
         assert (status == 0).all()
         comp, coff, clen = _compact(out, eoff, out_len)
-        ms, kms, ok = _device_decode_ms(eng, torch, dev, stream, comp, coff, clen, blob, off, ln, max(2, args.steps // 3))
+        ms, kms, ok = _device_decode_ms(eng, torch, dev, stream, comp, coff, clen, blob, off, ln, args.steps)
         t = torch.tensor([ms], dtype=torch.float64, device=dev)
         if world > 1:
             dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -315,7 +315,7 @@ def run_entropy(args, eng, rank, world, dev):
         tot_bytes += world * n * sb
         tot_ms += ms
     if rank == 0:
-        print(json.dumps({"metric": METRIC, "value": tot_bytes / tot_ms / 1e3, "unit": UNIT, "n_gpus": world, "steps": max(2, args.steps // 3),
+        print(json.dumps({"metric": METRIC, "value": tot_bytes / tot_ms / 1e3, "unit": UNIT, "n_gpus": world, "steps": args.steps,
                           "warmup": 2, "ms_per_step": tot_ms, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "i16/u64",
                           "data": "synthetic",
                           "config": {"workload": "entropy sweep (BASELINE configs[4]): %d x 1 MiB Bernoulli-bit streams per GPU, p in {0.5, 0.9, 0.99}, "
@@ -326,19 +326,40 @@ def run_entropy(args, eng, rank, world, dev):
     return 0
 
 
+DUMP_SAMPLE_STREAMS = 64   # 64 x 64 KiB decoded bytes as float32 = 16 MiB
+
+
+def dump_outputs(d, d_out, d_out_len, d_status, off):
+    """What a caller of the device decode receives, as float arrays: every stream's out_len and status, and the decoded bytes
+    of a fixed, seeded sample of the streams (the whole output is 256 MiB of bytes at the default size)."""
+    os.makedirs(d, exist_ok=True)
+    n = len(off)
+    pick = np.sort(np.random.default_rng(0).choice(n, size=min(n, DUMP_SAMPLE_STREAMS), replace=False))
+    out = d_out.cpu().numpy()
+    sample = np.stack([out[int(off[i]): int(off[i]) + STREAM_BYTES] for i in pick]).astype(np.float32)
+    np.save(os.path.join(d, "decoded_sample.npy"), sample)
+    np.save(os.path.join(d, "decoded_sample_streams.npy"), pick.astype(np.float64))
+    np.save(os.path.join(d, "out_len.npy"), d_out_len.cpu().numpy().astype(np.float64))
+    np.save(os.path.join(d, "status.npy"), d_status.cpu().numpy().astype(np.float32))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours")
-    ap.add_argument("--streams", type=int, default=0, help="streams per GPU (default: 4096 at N=1, 8192 at N>1)")
+    ap.add_argument("--streams", type=int, default=0, help="streams per GPU (default: 4096)")
     ap.add_argument("--workload", default="text", choices=["text", "entropy"])
     ap.add_argument("--skip-populations", action="store_true")
     ap.add_argument("--lanes", type=int, default=int(os.environ.get("DIVANS_B200_LPS", "0")), help="lanes per stream: 16 / 8 (v2 engine), 32 / 116 (round-1 kernels); 0 = by batch size")
     ap.add_argument("--cpu-sample", type=int, default=0, help="streams in the cpu_baseline sample (0 = auto)")
     ap.add_argument("--skip-cpu", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one decoded (rank 0's shard) as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.impl == "reference":
         return run_reference_arm(args)
 
@@ -359,7 +380,7 @@ def main():
 
     if not args.streams:
         args.streams = STREAMS_PER_GPU if world == 1 else STREAMS_PER_GPU_SCALING
-    eng = divans_b200.Engine(local_rank, 0, args.lanes)   # 0: the library picks 16 lanes per stream while the batch is resident, else 8
+    eng = divans_b200.Engine(local_rank, 0, args.lanes)   # 0: the library picks the layout by batch size
     if args.workload == "entropy":
         return run_entropy(args, eng, rank, world, dev)
     n = args.streams
@@ -412,6 +433,8 @@ def main():
     barrier()
     clocks = sampler.stop()
     dev_ms = ev0.elapsed_time(ev1)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, d_out, d_out_len, d_status, off)
     launches = eng.launch_count - launches0
     # the decode kernel's own duration (CUDA events inside the library, on the same stream), one extra untimed pass
     for _ in range(3):
@@ -420,10 +443,10 @@ def main():
         main_ms.append(eng.last_main_kernel_ms())
     kern_ms = float(np.median(main_ms))
 
-    # ---- the other encodings of the same raw streams (rank 0's shard; device-resident, 3 steps each) ----
+    # ---- the other encodings of the same raw streams (rank 0's shard; device-resident, --steps steps each) ----
     populations = None
     if rank == 0 and not args.skip_populations:
-        populations = measure_populations(eng, torch, dev, stream, blob, off, ln)
+        populations = measure_populations(eng, torch, dev, stream, blob, off, ln, args.steps)
 
     # ---- supplementary: the GPU encoder on the same shard, raw inputs resident in HBM (BASELINE configs[3] shape) ----
     d_raw = torch.from_numpy(blob).to(dev)
@@ -449,7 +472,7 @@ def main():
         ee1.record(stream)
         torch.cuda.synchronize()
         return ee0.elapsed_time(ee1) / enc_steps, eng.last_main_kernel_ms(), int(d_elen.sum())
-    enc_steps = 3
+    enc_steps = args.steps
     enc_ms, enc_model_ms, _ = run_encode(divans_b200.encode_options(), comp_bytes)                       # reference defaults
     enc2_ms, enc2_model_ms, enc2_bytes = run_encode(divans_b200.encode_options(dynamic_context_mixing=2))   # BASELINE configs[3] option
     del d_eout
@@ -465,7 +488,7 @@ def main():
         eng.decode_batch_host(h_in_np[0], coff, clen, h_out_np, off, ln)
     barrier()
     t0 = time.perf_counter()
-    sync_steps = 3
+    sync_steps = args.steps
     for _ in range(sync_steps):
         out_len_h, status_h = eng.decode_batch_host(h_in_np[0], coff, clen, h_out_np, off, ln)
     torch.cuda.synchronize()
@@ -475,7 +498,7 @@ def main():
         eng.decode_batch_host_async(h_in_np[k], coff, clen, h_out_np_l[k], off, ln).wait()
     h_out_np_l[1][:out_bytes] = 0
     barrier()
-    e2e_steps = max(4, args.steps)
+    e2e_steps = args.steps
     t0 = time.perf_counter()
     pend, results = [], []
     for k in range(e2e_steps):
@@ -518,7 +541,7 @@ def main():
             job_len = np.concatenate([g_len[r].cpu().numpy() for r in range(world)])
             job_cap = np.full(job_len.size, STREAM_BYTES, np.int64)
             del g_comp
-        sc_steps = 3
+        sc_steps = args.steps
         for k in range(1 + sc_steps):
             barrier()
             t0 = time.perf_counter()
@@ -579,7 +602,7 @@ def main():
                                    "encoding (1 PredictionMode + 1 Literal command)" % (n, 1 if world == 1 else 2),
                        "streams_per_gpu": n, "stream_bytes": STREAM_BYTES, "compressed_bytes_per_gpu": comp_bytes,
                        "lanes_per_stream": args.lanes, "parallelism": "dp%d (streams sharded, no data-path collective)" % world,
-                       "l2_policy": "inputs+outputs+model state per step (>0.39 GB + prior arena) exceed the 126 MB L2; no explicit flush",
+                       "l2_policy": "inputs+outputs+model state per step (>0.39 GB + prior arena) exceed the 50 MB L2; no explicit flush",
                        "input_generator": generator},
             "e2e": {"value": e2e_v, "unit": UNIT, "h2d_bytes_per_step": comp_bytes + 4 * 8 * n, "d2h_bytes_per_step": out_bytes + 12 * n,
                     "steps": e2e_steps, "api": "divans_b200_decode_batch_host_async / _wait (two batches in flight, pinned host buffers)",

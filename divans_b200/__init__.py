@@ -1,6 +1,6 @@
-"""divans_b200 -- host-side Python mirror of the B200-native divANS engine.
+"""divans_b200 -- host-side Python mirror of the H100-native divANS engine.
 
-The compute lives in ``lib/libdivans_b200.so`` (hand-written sm_100a CUDA behind a C ABI, see
+The compute lives in ``lib/libdivans_b200.so`` (hand-written sm_90a CUDA behind a C ABI, see
 ``include/divans_b200.h``).  This module only loads it and mirrors the reference's operator surface:
 
 * :class:`DivansDecompressorReader`  -- reference ``src/reader.rs:298-320`` (``new(reader, buffer_size, skip_crc, multithread)``)
@@ -197,14 +197,14 @@ def encode_options(**kw):
 
 
 class Engine:
-    """Batch engine bound to one GPU.  ``lanes_per_stream``: 0 = by batch size (16, or 8 beyond ~4700 streams), 16 / 8 = the round-2
+    """Batch engine bound to one GPU.  ``lanes_per_stream``: 0 = by batch size (16, or 8 where their residency holds the batch in fewer passes; never on an 80 GB H100, whose slot memory caps both), 16 / 8 = the round-2
     engine with two / four streams per warp, 32 / 116 = the round-1 kernels (include/divans_b200.h)."""
 
     def __init__(self, device=0, max_resident=0, lanes_per_stream=0):
         self._L = load_library()
         self._h = self._L.divans_b200_create(int(device), int(max_resident), int(lanes_per_stream))
         if not self._h:
-            raise DivansError("divans_b200_create(device=%d) failed: no usable sm_100a CUDA device (no CPU fallback)" % device)
+            raise DivansError("divans_b200_create(device=%d) failed: no usable sm_90a CUDA device (no CPU fallback)" % device)
         self.device = device
         self._inflight = {}     # ticket -> every buffer the C side still reads or writes for that pipelined batch
 

@@ -2,7 +2,7 @@
 //   LPG = 16: two streams per warp, lane j of a group holds CDF element j;
 //   LPG = 8:  four streams per warp, lane j holds elements 2j and 2j+1 packed in one register (c[2j] | c[2j+1] << 16).
 //
-// What bounds the decoder (profiles/r2_*): with 4096 streams a B200 has fewer than 7 streams per warp scheduler, each one a
+// What bounds the decoder: with 4096 streams a GPU of ~130-150 SMs has fewer than 8 streams per warp scheduler, each one a
 // serial dependency chain -- a warp issues one instruction every 5-6 cycles, so the time of a batch is
 //     bytes per stream x (warp instructions per byte) x ~5.5 cycles     (until the issue slots run out, at larger batches)
 // and the levers are the instructions in the per-byte loop and the streams that share each of them.  v2 versus the
@@ -22,7 +22,7 @@
 //     stores of last_8_literals;
 //   * LPG = 8: blend and rescale (frequentist_cdf.rs:74-85) are one packed add / one packed subtract for two elements.
 // (An L1 prefetch of the 16 candidate priors of the next low nibble -- contiguous thanks to lit_index_lo -- was built and
-// measured: prefetch.global.L1 only reaches L2 on this part, profiles/r2_ubench_prefetch_l1.txt; it is not in the loop.)
+// measured on the part this engine was first tuned on: prefetch.global.L1 only reached L2 there; it is not in the loop.)
 // Decode only.
 #pragma once
 #include "dv_engine_kernel.cuh"
@@ -257,8 +257,8 @@ __device__ __forceinline__ void rans_pair_v2(uint64_t &a, uint64_t &b, const uin
                                              const uint32_t el, const uint32_t ml, const int l, FastK &f) {
     uint64_t xa = rans_advance_v2<LPG>(a, eh, mh, h), xb = rans_advance_v2<LPG>(b, el, ml, l);
     const bool na = xa < (1ull << 31), nb = xb < (1ull << 31);
-    // two streams per warp: no state refills in 78 % of the bytes, the branch pays (46.6 -> 45.6 ms for 4096 streams); four
-    // streams per warp: 61 %, the predicated form is the faster one (73.6 vs 75.1 ms for 8192) -- profiles/r2_v12_ab.txt
+    // two streams per warp: no state refills in 78 % of the bytes, the branch pays; four streams per warp: 61 %, the
+    // predicated form is the faster one
     if (LPG == 8 || __any_sync(FULL, na || nb)) {
         if (na) { xa = (xa << 32) | (uint64_t)f.wnext; f.wi = min(f.wi + 1, f.wmax); f.wnext = ld_stream_u32(f.wbase + f.wi); }
         if (nb) { xb = (xb << 32) | (uint64_t)f.wnext; f.wi = min(f.wi + 1, f.wmax); f.wnext = ld_stream_u32(f.wbase + f.wi); }
@@ -500,10 +500,9 @@ __device__ __forceinline__ bool literal_fast_v2(St &s, Next &nx, const G2 g, con
                 touch_l1(mk_ptr(lo_tab + row_l * 32u + (LPG == 16 ? li * 32u : li * 64u), slot_hi), smem_dummy);
                 if (LPG == 8) touch_l1(mk_ptr(lo_tab + row_l * 32u + li * 64u + 32u, slot_hi), smem_dummy);
             }
-// (16 lanes per stream: not unrolled -- the literal loop itself times the same with 1, 2 or 4 bytes per trip, 45.1-46.8 ms over
-            // two rounds each, but the command path, which is instruction-fetch bound, takes 119 ms with the smaller kernel instead
-            // of 129, profiles/r2_v18_variants.txt.  8 lanes per stream: two bytes per trip, 73.4 vs 76.3 ms for 8192 streams,
-            // profiles/r2_v19_ab8.txt)
+// (16 lanes per stream: not unrolled -- the literal loop itself times the same with 1, 2 or 4 bytes per trip, but the
+            // command path, which is instruction-fetch bound, is faster with the smaller kernel.  8 lanes per stream: two bytes
+            // per trip)
 #pragma unroll (LPG == 16 ? 1 : 2)
             for (uint32_t i = 0; i < m; i++) {
                 // -- high nibble: search (speculative: the prior is almost always one this stream has written)

@@ -7,8 +7,9 @@
 namespace dv {
 
 constexpr int DEC2_BLOCK_THREADS = 32;          // one warp per block: blocks spread evenly over the SMs
-constexpr int DEC2_MIN_BLOCKS = 16;             // 4 one-warp blocks per scheduler partition (16 K registers each): <= 128 registers.  (144 registers = 3 per
-                                                // partition = 12 per SM: 3552 resident 16-lane streams, measured 66 ms for 4096 -- a second wave)
+constexpr int DEC2_MIN_BLOCKS = 16;             // 4 one-warp blocks per scheduler partition (16 K registers each): <= 128 registers, 32 resident
+                                                // 16-lane streams per SM (4224 on an H100's 132 SMs).  (144 registers = 3 per partition = 12 per
+                                                // SM: 3168 resident 16-lane streams, a second wave for 4096)
 
 template <int LPG, bool PF>
 __global__ void __launch_bounds__(DEC2_BLOCK_THREADS, DEC2_MIN_BLOCKS) decode_kernel_v2(DecodeParams p) {

@@ -1,7 +1,7 @@
 // dv_capi.cu -- the C ABI of libdivans_b200.so: batch engine context + the reference's FFI surface as a drop-in.
 //
 // Host side only marshals: offsets/lengths tables, H2D/D2H copies, kernel launches.  All model/entropy work runs in
-// the sm_100a kernels (dv_kernels.cu); there is no CPU decode path in this library.
+// the sm_90a kernels (dv_kernels.cu); there is no CPU decode path in this library.
 #include <cuda_runtime.h>
 #include <stdarg.h>
 #include <stdio.h>
@@ -39,7 +39,7 @@ struct divans_b200_ctx {
     cudaStream_t stream = nullptr;
     uint8_t *d_arena = nullptr; size_t arena_slots = 0;   // 16 MiB aligned view of d_arena_raw
     uint8_t *d_arena_raw = nullptr;
-    bool auto_lanes = false;         // lanes_per_stream 0: 16 lanes while the batch fits their residency, else 8 (twice the resident streams)
+    bool auto_lanes = false;         // lanes_per_stream 0: 16 lanes, or 8 where their residency holds the batch in fewer passes
     int last_lanes = 0;              // layout the most recent decode call used
     uint32_t cap16 = 0, cap8 = 0;    // resident streams of the two v2 layouts
     bool prefetch = false;           // v2 engine: touch the candidate priors of the next nibble (env DIVANS_B200_PREFETCH, default off)
@@ -81,6 +81,8 @@ struct divans_b200_ctx {
 
 static bool ck(divans_b200_ctx *c, cudaError_t e, const char *what) {
     if (e == cudaSuccess) return true;
+    // a failed allocation is reported here; clear it, or the launch check of the next call on this context reports it again
+    if (e == cudaErrorMemoryAllocation) cudaGetLastError();
     char buf[512];
     snprintf(buf, sizeof buf, "divans_b200: %s failed: %s", what, cudaGetErrorString(e));
     if (c) c->err = buf;
@@ -115,8 +117,8 @@ extern "C" divans_b200_ctx *divans_b200_create(int device, uint32_t max_resident
         fprintf(stderr, "divans_b200: no usable CUDA device %d -- this library has no CPU path\n", device);
         delete ctx; return nullptr;
     }
-    if (prop.major < 10) {
-        fprintf(stderr, "divans_b200: device %d is sm_%d%d; the kernels are built for sm_100a only\n", device, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) {   // sm_90a code runs on compute capability 9.0 only
+        fprintf(stderr, "divans_b200: device %d is sm_%d%d; the kernels are built for sm_90a only\n", device, prop.major, prop.minor);
         delete ctx; return nullptr;
     }
     ctx->sm_count = prop.multiProcessorCount;
@@ -137,7 +139,9 @@ extern "C" divans_b200_ctx *divans_b200_create(int device, uint32_t max_resident
     uint32_t auto_res = (uint32_t)ctx->sm_count * (uint32_t)per_sm * groups_per_block;
     size_t free_b = 0, total_b = 0;
     cudaMemGetInfo(&free_b, &total_b);
-    uint32_t mem_cap = (uint32_t)((free_b * 8 / 10) / SLOT_STRIDE);   // leave room for batch buffers
+    // Leave room for batch buffers.  85 %: on an 80 GB H100 the full 16-lane residency (132 SMs x 32 streams, 66 GiB of slots)
+    // must fit, or a 4096-stream batch would leave a second wave behind.
+    uint32_t mem_cap = (uint32_t)((free_b * 17 / 20) / SLOT_STRIDE);
     if (auto_res > mem_cap) auto_res = mem_cap;
     ctx->max_resident = max_resident ? (max_resident < auto_res ? max_resident : auto_res) : auto_res;
     if (ctx->max_resident < groups_per_block) ctx->max_resident = groups_per_block;
@@ -180,7 +184,7 @@ extern "C" void divans_b200_destroy(divans_b200_ctx *ctx) {
     if (ctx->stream) cudaStreamDestroy(ctx->stream);
     delete ctx;
 }
-// bumped whenever a decode kernel changes: profiles/traffic.json (an ncu capture) is only quoted by bench.py for the version it measured
+// bumped whenever a decode kernel changes: bench.py quotes a stored DRAM-traffic capture (profiles/traffic.json) only for the version it measured
 #define DV_KERNEL_VERSION "r2.11-v2-signtags"
 extern "C" const char *divans_b200_kernel_version(void) { return DV_KERNEL_VERSION; }
 extern "C" const char *divans_b200_last_error(divans_b200_ctx *ctx) { return ctx ? ctx->err.c_str() : "null context"; }
@@ -235,9 +239,13 @@ static DivansResult decode_device_nolock(divans_b200_ctx *ctx, size_t n, const u
         cap = (uint32_t)ctx->sm_count * (uint32_t)std::max(1, decode_max_blocks_per_sm16_blend()) * gpb;
         if (cap > ctx->max_resident) cap = std::max(ctx->max_resident / gpb * gpb, gpb);   // (memory / caller limits of the context)
     } else if (ctx->engine == 0) {
-        // a batch that fits the 16-lane layout's residency runs there (fewer instructions per stream on the critical path of a
-        // half-empty GPU); a larger one takes 8 lanes per stream: twice the streams in flight instead of a second wave
-        if (ctx->auto_lanes) lanes = n <= ctx->cap16 ? 16 : 8;
+        // 16 lanes per stream unless 8 hold the batch in fewer passes.  At equal residency 8 lanes is the slower layout (half the
+        // warps per scheduler); it only pays where registers, not slot memory, cap residency: there it keeps twice the streams in
+        // flight.  On an 80 GB H100 both layouts are capped by slot memory (cap8 ~ cap16), so 16 lanes run every batch size.
+        if (ctx->auto_lanes) {
+            const uint64_t passes16 = (n + ctx->cap16 - 1) / ctx->cap16, passes8 = (n + ctx->cap8 - 1) / ctx->cap8;
+            lanes = passes8 < passes16 ? 8 : 16;
+        }
         gpb = (uint32_t)decode_groups_per_block_v2(lanes); cap = lanes == 16 ? ctx->cap16 : ctx->cap8;
     }
     ctx->last_lanes = lanes;
@@ -418,19 +426,24 @@ extern "C" DivansResult divans_b200_decode_batch_host_async(divans_b200_ctx *ctx
 // ---- encoder ----
 static inline int pack_speed(const int16_t sp[2]) { return (int)((uint32_t)(uint16_t)sp[0] | ((uint32_t)(uint16_t)sp[1] << 16)); }
 
+// Arena slots the encoder's model pass uses for n streams: whole blocks of 16-lane groups, capped by its residency.
+constexpr uint32_t ENCODE_GROUPS_PER_BLOCK = DECODE_BLOCK_THREADS / 16;
+static size_t encode_slots(const divans_b200_ctx *ctx, size_t n) {
+    int per_sm = encode_max_blocks_per_sm(); if (per_sm < 1) per_sm = 1;
+    uint32_t max_res = (uint32_t)ctx->sm_count * (uint32_t)per_sm * ENCODE_GROUPS_PER_BLOCK;
+    if (ctx->max_resident < max_res) max_res = ctx->max_resident;
+    const uint32_t resident = (uint32_t)(n < max_res ? n : max_res);
+    return (size_t)((resident + ENCODE_GROUPS_PER_BLOCK - 1) / ENCODE_GROUPS_PER_BLOCK) * ENCODE_GROUPS_PER_BLOCK;
+}
+
 // One launch set over n streams whose inputs/outputs already sit in HBM.  `cmd_cap`/`lit_cap`: log entries per stream,
 // `replay_stride`: bytes of replay window per resident slot.
 static DivansResult encode_device_internal(divans_b200_ctx *ctx, size_t n, int raw_mode, const uint8_t *d_in, const uint64_t *d_in_off,
                                            const uint64_t *d_in_len, uint32_t cmd_cap, uint32_t lit_cap, uint64_t replay_stride,
                                            uint8_t *d_out, const uint64_t *d_out_off, const uint64_t *d_out_cap, uint64_t *d_out_len,
                                            int32_t *d_status, const divans_b200_encode_options *o, cudaStream_t st) {
-    const uint32_t gpb = DECODE_BLOCK_THREADS / 16;
-    int per_sm = encode_max_blocks_per_sm(); if (per_sm < 1) per_sm = 1;
-    uint32_t max_res = (uint32_t)ctx->sm_count * (uint32_t)per_sm * gpb;
-    if (ctx->max_resident < max_res) max_res = ctx->max_resident;
-    uint32_t resident = (uint32_t)(n < max_res ? n : max_res);
-    uint32_t blocks = (resident + gpb - 1) / gpb;
-    size_t slots = (size_t)blocks * gpb;
+    const size_t slots = encode_slots(ctx, n);
+    const uint32_t blocks = (uint32_t)(slots / ENCODE_GROUPS_PER_BLOCK);
     if (ensure_arena(ctx, slots) != DIVANS_SUCCESS) return DIVANS_FAILURE;
     const uint32_t cmd_chunks = (cmd_cap + NUM_SYMBOLS_BEFORE_FLUSH - 1) / NUM_SYMBOLS_BEFORE_FLUSH;
     const uint32_t lit_chunks = (lit_cap + NUM_SYMBOLS_BEFORE_FLUSH - 1) / NUM_SYMBOLS_BEFORE_FLUSH;
@@ -548,6 +561,8 @@ static DivansResult encode_host_common(divans_b200_ctx *ctx, size_t n, int raw_m
         }
     }
     const uint8_t *src = raw_mode ? in : staged.data();
+    // the slots first: the symbol logs are sized from what is left (on an 80 GB GPU the slots take most of the memory)
+    if (ensure_arena(ctx, encode_slots(ctx, n)) != DIVANS_SUCCESS) return DIVANS_FAILURE;
     size_t free_b = 0, total_b = 0;
     cudaMemGetInfo(&free_b, &total_b);
     const uint64_t budget = (uint64_t)(free_b + ctx->sf_cap * 4) * 6 / 10;

@@ -1,4 +1,4 @@
-// dv_common.cuh -- shared definitions for the sm_100a divANS kernels.
+// dv_common.cuh -- shared definitions for the sm_90a divANS kernels.
 //
 // Data layout in HBM (per resident "slot" = the private model state of one stream while a lane-group
 // decodes/encodes it; slots are recycled from stream to stream):

@@ -1,4 +1,4 @@
-// dv_encode.cu -- sm_100a kernels of the divANS batch ENCODER (SURVEY 8a "next": GPU encoder, BASELINE config 4).
+// dv_encode.cu -- sm_90a kernels of the divANS batch ENCODER (SURVEY 8a "next": GPU encoder, BASELINE config 4).
 //
 // The reference's encoder (codec/mod.rs:280-560 + ans.rs:289-378) interleaves three things per stream: the adaptive
 // model walk, a reverse rANS pass every 65536 symbols, and the mux.  They are separate passes here:

@@ -1,4 +1,4 @@
-// dv_engine.cuh -- lock-step warp engine for the divANS command codec (sm_100a).
+// dv_engine.cuh -- lock-step warp engine for the divANS command codec (sm_90a).
 //
 // A warp runs two streams (one per 16-lane group) in LOCK STEP: every loop iteration the whole warp, converged under
 // the compile-time mask 0xffffffff, codes exactly one nibble per group ("nibble core": CDF load, bin search by ballot,
@@ -152,7 +152,7 @@ struct G2 {            // lane geometry of one lane-group (16 lanes: one CDF ele
 
 // The group's cold state, found from scratch.  The out-of-line helpers below use this instead of taking pointers into it: a
 // generic pointer to shared memory costs two special-register reads to build, and the compiler builds the arguments of those
-// (rare) calls at the head of every iteration of the main loop (~25 instructions per iteration, profiles/r2_v6_z4096).
+// (rare) calls at the head of every iteration of the main loop (~25 instructions per iteration).
 __device__ __forceinline__ Cold *cold_of_group(const G2 g) {
     extern __shared__ __align__(16) uint8_t dv_dynamic_smem[];
     return reinterpret_cast<Cold *>(dv_dynamic_smem + (unsigned)g.grp * ((sizeof(Cold) + 15) / 16 * 16));

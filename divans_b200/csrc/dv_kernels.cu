@@ -1,4 +1,4 @@
-// dv_kernels.cu -- sm_100a kernels of the divANS batch engine: framing/CRC pre-pass and the stream decoder.
+// dv_kernels.cu -- sm_90a kernels of the divANS batch engine: framing/CRC pre-pass and the stream decoder.
 #include "dv_core.cuh"
 
 namespace dv {

@@ -5,10 +5,8 @@
 namespace dv {
 constexpr int DECODE_BLOCK_THREADS = 64;
 
-// Resident blocks per SM of a stream kernel (register-limited).  (L1 and shared memory share 256 KB per SM and the driver gives
-// these kernels a 100 KB carve-out although they use ~2.3 KB per block.  Asking for less through
-// cudaFuncAttributePreferredSharedMemoryCarveout brought nothing: 16 % left the configuration ncu reports at 100 KB and the
-// time unchanged, 28 % was 1-4 % slower -- profiles/r2_v8_sweep.txt -- so no preference is set.)
+// Resident blocks per SM of a stream kernel (register-limited; the kernels use ~2.3 KB of shared memory per block, so no
+// shared-memory carve-out preference is set).
 template <typename K> static inline int stream_kernel_blocks_per_sm(K kernel, int threads, size_t dyn_smem) {
     int nb = 0;
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kernel, threads, dyn_smem);

@@ -1,4 +1,4 @@
-// dv_model.cuh -- the divANS model + rANS coder as warp-level device code (sm_100a).
+// dv_model.cuh -- the divANS model + rANS coder as warp-level device code (sm_90a).
 //
 // One 16-lane group owns one stream: lane i (0..15) of the group holds element i of whichever 16-entry adaptive
 // CDF is being coded, so the reference's per-symbol work becomes

@@ -1,5 +1,5 @@
 /*
- * divans_b200.h -- C ABI of the B200-native divANS entropy engine (libdivans_b200.so).
+ * divans_b200.h -- C ABI of the H100-native divANS entropy engine (libdivans_b200.so).
  *
  * Two surfaces:
  *  (1) the reference's own C FFI, symbol for symbol (reference: src/ffi/mod.rs, c/divans/ffi.h), so a
@@ -7,7 +7,7 @@
  *  (2) a batch extension (ours, additive) -- the shape the GPU wants: N independent streams per call,
  *      either from host buffers (end-to-end path, copies included) or device-resident.
  *
- * Every stream is decoded/encoded by hand-written sm_100a CUDA kernels; there is no CPU fallback:
+ * Every stream is decoded/encoded by hand-written sm_90a CUDA kernels; there is no CPU fallback:
  * if no CUDA device / context can be had, constructors return NULL and batch calls return
  * DIVANS_FAILURE after printing the CUDA error to stderr.
  */
@@ -124,8 +124,9 @@ typedef struct divans_b200_ctx divans_b200_ctx;
 /* per-stream status values are DivansResult codes (0 ok, 1 truncated input, 2 output capacity too small, 3 corrupt) */
 
 /* device = CUDA ordinal; max_resident = cap on concurrently resident streams (0 = auto: sized to the GPU);
- * lanes_per_stream: 0 = by batch size (16 lanes per stream while the batch fits their residency, 8 beyond it); 16 = two
- * streams per warp, one CDF element per lane; 8 = four streams per warp, two elements per lane (twice the resident streams) --
+ * lanes_per_stream: 0 = by batch size (16 lanes per stream, 8 when their residency holds the batch in fewer passes); 16 = two
+ * streams per warp, one CDF element per lane; 8 = four streams per warp, two elements per lane (up to twice the resident
+ * streams where registers, not slot memory, limit residency) --
  * all three the round-2 engine; 32 = round-1 kernel, one warp owns one stream (the upper half-warp mirrors the lower);
  * 116 = the round-1 16-lane kernel (A/B measurements). */
 divans_b200_ctx *divans_b200_create(int device, uint32_t max_resident, uint32_t lanes_per_stream);

@@ -1,17 +1,17 @@
 #!/usr/bin/env python3
-"""Regenerate tests/golden/*.  Run in the build container only (needs /root/reference/testdata).
+"""Regenerate tests/golden/*.  Usage: make_golden.py <reference tree> (reads its testdata/).
 
 The reference holds no compressed golden vectors (SURVEY section 4), so the fixtures are made by feeding the
 reference's own IR fixtures (testdata/*.ir, the input of src/bin/integration_test.rs:76-108) through the oracle
 encoder; the EXPECTED OUTPUT side is pinned by the reference's raw testdata files (sha256 below), i.e. by real
 reference data, not by the oracle.  Each entry: <name>.divans + an index line in golden.json.
 """
-import hashlib, json, os, sys
+import hashlib, json, lzma, os, sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(os.path.dirname(HERE)))
 from oracle import oracle_py as O
 
-REF = "/root/reference/testdata/"
+REF = os.path.join(sys.argv[1], "testdata", "")
 CASES = [
     # name, ir file, raw file, options
     ("alice29_ir", "alice29.ir", "alice29", dict()),
@@ -38,3 +38,5 @@ for name, ir, rawf, opts in CASES:
                       raw_sha256=hashlib.sha256(raw).hexdigest(), divans_len=len(enc), divans_sha256=hashlib.sha256(enc).hexdigest()))
     print(name, len(enc), len(raw))
 json.dump(index, open(os.path.join(HERE, "golden.json"), "w"), indent=1)
+# one of the reference IR fixtures itself, for the tests of the IR text parser on a real file
+open(os.path.join(HERE, "asyoulik.ir.xz"), "wb").write(lzma.compress(open(REF + "asyoulik.ir", "rb").read(), preset=9 | lzma.PRESET_EXTREME))

@@ -7,7 +7,7 @@ import os
 import numpy as np
 import pytest
 
-REF = "/root/reference/testdata/"
+GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 
 def test_crc32c_known_answers(oracle):
@@ -174,26 +174,42 @@ def test_encoder_is_deterministic_against_golden(oracle, golden):
     assert rc == 0 and oracle.encode_raw(raw) == enc
 
 
-@pytest.mark.skipif(not os.path.exists(REF), reason="reference tree not mounted (GPU box)")
-def test_ir_fixtures_recode_to_raw(oracle):
-    # reference src/bin/integration_test.rs:76-108
-    for name in ["alice29", "asyoulik", "random_then_unicode", "ends_with_truncated_dictionary"]:
-        raw = open(REF + name, "rb").read()
-        c = oracle.Commands.from_ir(open(REF + name + ".ir", "rb").read())
+def _golden_cmds(oracle, golden, name):
+    """the command list a golden fixture was encoded from (tests/golden/make_golden.py: one of the reference's IR fixtures),
+    recovered by decoding it; its plaintext is pinned by the sha256 of the reference's raw file"""
+    e = [g for g in golden if g["name"] == name][0]
+    enc = open(e["path"], "rb").read()
+    rc, raw, c = oracle.decode_cmds(enc, out_cap=e["raw_len"] + 64)
+    assert rc == 0 and hashlib.sha256(raw).hexdigest() == e["raw_sha256"], name
+    assert c.encode(oracle.options(**e["options"])) == enc, name      # the recovered list is the one that was encoded
+    return e, raw, c
+
+
+def test_ir_fixtures_recode_to_raw(oracle, golden):
+    # reference src/bin/integration_test.rs:76-108.  Two of the IR fixtures are stored (the small one as text, asyoulik.ir
+    # xz-compressed) and go through the IR text parser; the others are held by the golden streams made from them
+    import lzma
+    c = oracle.Commands.from_ir(open(os.path.join(GOLD, "ends_with_truncated_dictionary.ir"), "rb").read())
+    rc, rec = c.recode(c.window or 22)
+    assert rc == 0 and rec == open(os.path.join(GOLD, "ends_with_truncated_dictionary"), "rb").read()
+    e = [g for g in golden if g["name"] == "asyoulik_ir_mix2"][0]
+    c = oracle.Commands.from_ir(lzma.decompress(open(os.path.join(GOLD, "asyoulik.ir.xz"), "rb").read()))
+    rc, rec = c.recode(c.window or 22)
+    assert rc == 0 and hashlib.sha256(rec).hexdigest() == e["raw_sha256"]
+    assert c.encode(oracle.options(**e["options"])) == open(e["path"], "rb").read()
+    for name in ["alice29_ir", "asyoulik_ir_mix2", "random_then_unicode_ir", "truncated_dictionary"]:
+        e, raw, c = _golden_cmds(oracle, golden, name)
         rc, rec = c.recode(c.window or 22)
-        assert rc == 0 and rec == raw
+        assert rc == 0 and rec == raw, name
 
 
-@pytest.mark.skipif(not os.path.exists(REF), reason="reference tree not mounted (GPU box)")
-def test_ratio_ceilings(oracle):
+def test_ratio_ceilings(oracle, golden):
     # reference src/bin/integration_test.rs:235-236 (alice29 <= 0.34 with brotli commands, <= 0.46 literal-only),
     # src/bin/benchmark.rs:430-443 (random_then_unicode IR <= 0.6)
-    raw = open(REF + "alice29", "rb").read()
+    _, raw, c = _golden_cmds(oracle, golden, "alice29_ir")
     assert len(oracle.encode_raw(raw)) / len(raw) <= 0.46
-    c = oracle.Commands.from_ir(open(REF + "alice29.ir", "rb").read())
     assert len(c.encode(oracle.options(dynamic_context_mixing=1))) / len(raw) <= 0.34
-    raw = open(REF + "random_then_unicode", "rb").read()
-    c = oracle.Commands.from_ir(open(REF + "random_then_unicode.ir", "rb").read())
+    _, raw, c = _golden_cmds(oracle, golden, "random_then_unicode_ir")
     assert len(c.encode()) / len(raw) <= 0.6
 
 
@@ -257,9 +273,6 @@ def test_random_ir_roundtrip(oracle):
 # ---------------------------------------------------------------------------------------------------------------
 # The one compressed stream the reference tree holds (wasm/wasm.html:98-107): whole-bitstream pin of the oracle.
 # ---------------------------------------------------------------------------------------------------------------
-GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
-
-
 def _wasm_vector():
     import json
     vec = open(os.path.join(GOLD, "ref_wasm_example.divans"), "rb").read()
@@ -268,14 +281,9 @@ def _wasm_vector():
 
 
 def test_reference_held_stream_fixture_is_the_reference_bytes():
-    # the committed fixture equals what wasm/wasm.html holds (checked whenever the reference tree is mounted)
-    import re
+    # the committed fixture is the byte array of the reference's wasm/wasm.html (tests/golden/extract_wasm_vector.py)
     vec, meta = _wasm_vector()
     assert len(vec) == 113 and hashlib.sha256(vec).hexdigest() == meta["divans_sha256"]
-    html = "/root/reference/wasm/wasm.html"
-    if os.path.exists(html):
-        m = re.search(r"_example_dv_file\s*=\s*\[(.*?)\]", open(html).read(), re.S)
-        assert bytes(int(x, 16) for x in re.findall(r"0x([0-9a-fA-F]{2})", m.group(1))) == vec
 
 
 def test_reference_held_stream_decodes_under_its_model_revision(oracle):

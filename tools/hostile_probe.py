@@ -1,8 +1,9 @@
 """Dev probe (not collected by pytest): corrupted streams with the CRC check skipped must come back with a status, never
 hang or fault.  Run under `timeout`."""
-import sys, numpy as np
-sys.path.insert(0, "/root/repo")
-sys.path.insert(0, "/root/repo/tests")
+import os, sys, numpy as np
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
 import divans_b200
 from divans_b200 import synth
 from oracle import oracle_py as O

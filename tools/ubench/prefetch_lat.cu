@@ -1,5 +1,5 @@
-// Micro-benchmark (dev tool): does prefetch.global.L1 shorten a later dependent load on sm_100a, and what do the load
-// latencies look like?  One warp, one lane measuring with clock64.  Build: nvcc -gencode arch=compute_100a,code=sm_100a
+// Micro-benchmark (dev tool): does prefetch.global.L1 shorten a later dependent load on sm_90a, and what do the load
+// latencies look like?  One warp, one lane measuring with clock64.  Build: nvcc -gencode arch=compute_90a,code=sm_90a
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
