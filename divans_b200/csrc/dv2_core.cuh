@@ -50,6 +50,8 @@ __device__ __forceinline__ void touch_l1(const void *p, const uint32_t smem_dumm
 __device__ __forceinline__ uint32_t ld_stream_u32(const void *p) { uint32_t v; asm volatile("ld.global.cs.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory"); return v; }
 __device__ __forceinline__ void st_stream_u64(const void *p, unsigned long long v) { asm volatile("st.global.cs.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory"); }
 __device__ __forceinline__ void st_u8(const void *p, uint32_t v) { asm volatile("st.global.u8 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
+__device__ __forceinline__ uint32_t ld_shared_u8(const uint32_t a) { uint32_t v; asm volatile("ld.shared.u8 %0, [%1];" : "=r"(v) : "r"(a) : "memory"); return v; }
+__device__ __forceinline__ void st_shared_u8(const uint32_t a, const uint32_t v) { asm volatile("st.shared.u8 [%0], %1;" ::"r"(a), "r"(v) : "memory"); }
 
 // tag bits of this lane's element(s): element i carries bit i of the 16-bit generation in its bit 15
 template <int LPG> __device__ __forceinline__ uint32_t lane_tag(const uint32_t gen, const int li) {
@@ -178,8 +180,13 @@ __device__ __forceinline__ int nibble_core_v2(St &s, const Next &nx, const G2 g)
 // class = lut1[byte before] in 0..7 (codec/literal.rs:87-117, codec/interface.rs:199-238): the context of the next byte AND the
 // class that the byte after it will need, in one 16-bit load.  Rebuilt by the group when the prediction mode, the context
 // map or the literal block type changed.
+// LSB6 and MSB6 have no classes (lut1 is all zeros, codec/interface.rs:210-217): for them the 16-lane plain loop reads the
+// context from T2S[byte] = T2[byte * 8] & 0xff, 256 bytes per stream in SHARED memory (`t2s`: its shared address, 0 = none).
 // ---------------------------------------------------------------------------------------------------------------
-static __device__ __noinline__ void build_t2(const G2 g, uint8_t *slot, const uint8_t *tables, uint32_t pred_mode, uint32_t btype_last) {
+constexpr int T2S_BYTES = 256;
+__device__ __forceinline__ bool t2s_mode(const uint32_t pred_mode) { return pred_mode < 2; }   // LSB6, MSB6
+static __device__ __noinline__ void build_t2(const G2 g, uint8_t *slot, const uint8_t *tables, uint32_t pred_mode, uint32_t btype_last,
+                                             const uint32_t t2s) {
     const uint8_t *lut0 = tables + TB_CTX + 512 * pred_mode, *lut1 = lut0 + 256;
     const uint8_t *lcm = slot + OFF_LCM + (btype_last << 6);
     uint32_t *t2 = reinterpret_cast<uint32_t *>(slot + OFF_T2);
@@ -187,6 +194,8 @@ static __device__ __noinline__ void build_t2(const G2 g, uint8_t *slot, const ui
         const uint32_t byte = w >> 2, a = lut0[byte], k = (w & 3) * 2, cls = (uint32_t)(lut1[byte] & 7u) << 8;
         t2[w] = ((uint32_t)lcm[a | k] | cls) | (((uint32_t)lcm[a | (k + 1)] | cls) << 16);
     }
+    if (t2s && t2s_mode(pred_mode))
+        for (uint32_t b = (uint32_t)g.l16; b < (uint32_t)T2S_BYTES; b += (uint32_t)g.nl) st_shared_u8(t2s + b, lcm[lut0[b]]);
     __syncwarp(g.gmask);
 }
 
@@ -420,8 +429,9 @@ __device__ __forceinline__ void literal_mix_loop16(St &s, const G2 g, const bool
 // Returns false (nothing done) when some group cannot take the fast loop: dynamic context mixing, per-context mixing values, the
 // flat prior, wide speeds, untagged priors, or the first 7 bytes of a literal that began within 8 bytes of the ring start -- the
 // caller then codes one nibble per group through the generic core and the state machine.
+// `t2s`: shared address of this group's T2S (16 lanes per stream), else 0.
 template <int LPG, bool PF>
-__device__ __forceinline__ bool literal_fast_v2(St &s, Next &nx, const G2 g, const bool active, const uint32_t smem_dummy) {
+__device__ __forceinline__ bool literal_fast_v2(St &s, Next &nx, const G2 g, const bool active, const uint32_t smem_dummy, const uint32_t t2s) {
     uint32_t n = active ? s.lit_left : 0xffffffffu;
     if (LPG == 8) n = min(n, __shfl_xor_sync(FULL, n, 8));
     n = min(n, __shfl_xor_sync(FULL, n, 16));
@@ -429,7 +439,7 @@ __device__ __forceinline__ bool literal_fast_v2(St &s, Next &nx, const G2 g, con
     // dynamic context mixing >= 2 with one mixing value for the whole map (16 lanes per stream): its own loop
     if (LPG == 16 && __all_sync(FULL, !active || (s.mixing_trait && s.lit_cfg >= 0 && s.speeds_small && s.tagged &&
                                                   !(s.c->lit_quirk && s.c->lit_total - s.lit_left < 7u)))) {
-        if (active && s.c->t2_dirty) { build_t2(g, s.slot, s.tables, s.pred_mode, s.btype_last); s.c->t2_dirty = false; }
+        if (active && s.c->t2_dirty) { build_t2(g, s.slot, s.tables, s.pred_mode, s.btype_last, t2s); s.c->t2_dirty = false; }
         __syncwarp();
         literal_mix_loop16(s, g, active, n);
         if (active) enter_lit_nibble<false, true, true>(s, nx);
@@ -441,8 +451,11 @@ __device__ __forceinline__ bool literal_fast_v2(St &s, Next &nx, const G2 g, con
     if (!__all_sync(FULL, !active || (!s.mixing_trait && s.lit_cfg >= 0 && !(s.lit_cfg & 0x800) && s.speeds_small && s.tagged &&
                                       !(s.c->lit_quirk && s.c->lit_total - s.lit_left < 7u)))) return false;
     {
-        if (active && s.c->t2_dirty) { build_t2(g, s.slot, s.tables, s.pred_mode, s.btype_last); s.c->t2_dirty = false; }
+        if (active && s.c->t2_dirty) { build_t2(g, s.slot, s.tables, s.pred_mode, s.btype_last, t2s); s.c->t2_dirty = false; }
         __syncwarp();
+        // every group in LSB6 / MSB6 (16 lanes): the context comes from T2S in shared memory (a dummy group reads garbage
+        // contexts, which still address inside its own slot)
+        const bool small = LPG == 16 && __all_sync(FULL, !active || t2s_mode(s.pred_mode));
         const int li = g.l16;
         const int cfg = active ? s.lit_cfg : mm_cfg(4);
         const uint32_t mm = (cfg & 0x100) ? 0xffu : 0u, o1 = (cfg & 0x200) ? 0xfu : 0u, fc = (cfg & 0x400) ? 0xfu : 0u;
@@ -542,7 +555,7 @@ __device__ __forceinline__ bool literal_fast_v2(St &s, Next &nx, const G2 g, con
                 if (st_lane && (ap & 7u) == 7u) st_stream_u64(dbase + (done + i) - 7, l8);
                 ap++;
                 // -- context and priors of the next byte (get_prev_word_context, codec/literal.rs:87-117, through T2)
-                const uint32_t cv = ld_u16g(mk_ptr(t2 + (cur * 8u + pcp) * 2u, slot_hi));
+                const uint32_t cv = small ? ld_shared_u8(t2s + cur) : ld_u16g(mk_ptr(t2 + (cur * 8u + pcp) * 2u, slot_hi));
                 ctx = cv & 0xffu; pcp = cv >> 8;
                 ssb = (uint32_t)(l8 >> sh) & 0xffu;
                 idx_h = ctx * 256u + (ssb & mm & (~o1 & 0xffu));

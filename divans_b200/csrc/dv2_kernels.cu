@@ -14,12 +14,16 @@ constexpr int DEC2_MIN_BLOCKS = 16;             // 4 one-warp blocks per schedul
 template <int LPG, bool PF>
 __global__ void __launch_bounds__(DEC2_BLOCK_THREADS, DEC2_MIN_BLOCKS) decode_kernel_v2(DecodeParams p) {
     extern __shared__ __align__(16) uint8_t smem[];
-    // one dummy word per lane behind the groups' cold state: destination of the L1-touching async copies (dv2_core.cuh)
-    const uint32_t smem_dummy = PF ? (uint32_t)__cvta_generic_to_shared(smem + (DEC2_BLOCK_THREADS / LPG) * SMEM_BYTES_PER_GROUP_V2) + 4u * threadIdx.x : 0u;
     const int lane = threadIdx.x & 31;
     const int warp_in_block = threadIdx.x >> 5;
     constexpr int GPW = 32 / LPG;
     const int group_in_block = warp_in_block * GPW + lane / LPG;
+    // behind the groups' cold state: 16 lanes per stream, each group's T2S (dv2_core.cuh); then one dummy word per lane, the
+    // destination of the L1-touching async copies
+    constexpr uint32_t T2S_OFF = (DEC2_BLOCK_THREADS / LPG) * SMEM_BYTES_PER_GROUP_V2;
+    constexpr uint32_t DUMMY_OFF = T2S_OFF + (LPG == 16 ? (DEC2_BLOCK_THREADS / LPG) * T2S_BYTES : 0);
+    const uint32_t t2s = LPG == 16 ? (uint32_t)__cvta_generic_to_shared(smem + T2S_OFF) + (uint32_t)group_in_block * T2S_BYTES : 0u;
+    const uint32_t smem_dummy = PF ? (uint32_t)__cvta_generic_to_shared(smem + DUMMY_OFF) + 4u * threadIdx.x : 0u;
     const uint32_t slot = blockIdx.x * (DEC2_BLOCK_THREADS / LPG) + group_in_block;
     G2 g;
     g.l16 = lane & (LPG - 1);
@@ -96,7 +100,7 @@ __global__ void __launch_bounds__(DEC2_BLOCK_THREADS, DEC2_MIN_BLOCKS) decode_ke
         }
         // ---- whole literal bytes while every group is at a byte boundary of a literal (or out of work) ----
         const bool lit = s.state == S_LIT_HI;
-        if (__any_sync(FULL, lit) && __all_sync(FULL, lit || s.state == S_DONE) && literal_fast_v2<LPG, PF>(s, nx, g, lit, smem_dummy)) {   // (the cheaper, usually false test first)
+        if (__any_sync(FULL, lit) && __all_sync(FULL, lit || s.state == S_DONE) && literal_fast_v2<LPG, PF>(s, nx, g, lit, smem_dummy, t2s)) {   // (the cheaper, usually false test first)
             if (lit) {
                 if (s.cur.underflow) s.status = ST_NEED_INPUT;
                 if (s.lit_left == 0 && s.status == ST_OK) { swap_coders(s, g); enter_cmd_type<false>(s, nx); }
@@ -128,8 +132,11 @@ __global__ void __launch_bounds__(DEC2_BLOCK_THREADS, DEC2_MIN_BLOCKS) decode_ke
     if (g.store0) *reinterpret_cast<uint32_t *>(s.slot + OFF_HDR) = s.c->gen_ctr;
 }
 
-// per block: the groups' cold state (+ one dummy word per thread, the target of the candidate-touch prefetch, when that is compiled in)
-template <int LPG, bool PF> static size_t smem_v2() { return (size_t)(DEC2_BLOCK_THREADS / LPG) * SMEM_BYTES_PER_GROUP_V2 + (PF ? 4 * DEC2_BLOCK_THREADS : 0); }
+// per block: the groups' cold state, 16 lanes per stream their T2S (+ one dummy word per thread, the target of the candidate-touch
+// prefetch, when that is compiled in)
+template <int LPG, bool PF> static size_t smem_v2() {
+    return (size_t)(DEC2_BLOCK_THREADS / LPG) * (SMEM_BYTES_PER_GROUP_V2 + (LPG == 16 ? T2S_BYTES : 0)) + (PF ? 4 * DEC2_BLOCK_THREADS : 0);
+}
 template <int LPG, bool PF> static void launch_v2(const DecodeParams &p, uint32_t n_blocks, cudaStream_t st) {
     decode_kernel_v2<LPG, PF><<<n_blocks, DEC2_BLOCK_THREADS, smem_v2<LPG, PF>(), st>>>(p);
 }

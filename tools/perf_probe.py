@@ -1,12 +1,51 @@
 """Dev probe (not a test, not the bench): device time of decode/encode for several stream populations.
-  python tools/perf_probe.py [n_streams] [--l-only] [--lz-all] [--decode-once]     (DIVANS_B200_LPS selects the lane layout)"""
-import os, sys, time, numpy as np
+  python tools/perf_probe.py [n_streams] [--l-only] [--lz-all] [--decode-once]     (DIVANS_B200_LPS selects the lane layout)
+  python tools/perf_probe.py --sweep [n1,n2,...]     literal-only text decode kernel time per decoded byte per stream, by batch size
+                                                     (default 132,528,1056,2112,4224: 1/8 to 4 warps per scheduler on 132 SMs)"""
+import os, subprocess, sys, time, numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import divans_b200
 from divans_b200 import synth
 
 once = "--decode-once" in sys.argv
+
+
+def sweep(sizes):
+    """Is the literal loop bound by its dependency chain (time per byte flat in the warps per scheduler), by issue (time grows
+    with them), or by memory (a step where the batch's literal priors, ~28 KB per stream, outgrow the L2)?"""
+    import torch
+    prop = torch.cuda.get_device_properties(0)
+    try:
+        card = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                              capture_output=True, text=True, timeout=20).stdout.strip()
+    except Exception as e:
+        card = "%s (nvidia-smi: %s)" % (prop.name, e)
+    print("card: %s | %d SMs | kernel %s" % (card, prop.multi_processor_count, divans_b200.kernel_version()), flush=True)
+    eng = divans_b200.Engine(0, 0, 16)
+    blob, off, ln = synth.text_streams(max(sizes), 65536, seed=3)
+    raws_all = [blob[int(o):int(o + l)].tobytes() for o, l in zip(off, ln)]
+    for n in sizes:
+        raws = raws_all[:n]
+        streams = eng.encode(raws, divans_b200.encode_options())
+        caps = [len(r) + 64 for r in raws]
+        ms = []
+        for _ in range(4):
+            res = eng.decode(streams, caps)
+            ms.append(eng.last_main_kernel_ms())
+        ok = all(st == 0 and out == r for (st, out), r in zip(res, raws))
+        kms = float(np.median(ms[1:]))
+        wps = (n / 2) / (prop.multi_processor_count * 4)   # 16 lanes per stream: two streams per warp
+        print("streams %5d  warps/scheduler %5.2f  decode kernel %8.2f ms (min %8.2f max %8.2f)  %7.1f ns/byte/stream  ok=%s"
+              % (n, wps, kms, min(ms[1:]), max(ms[1:]), kms * 1e6 / 65536, ok), flush=True)
+    eng.close()
+
+
+if "--sweep" in sys.argv:
+    i = sys.argv.index("--sweep")
+    spec = sys.argv[i + 1] if i + 1 < len(sys.argv) and not sys.argv[i + 1].startswith("--") else "132,528,1056,2112,4224"
+    sweep([int(x) for x in spec.split(",")])
+    sys.exit(0)
 
 def run(name, raws, opts, eng, cmds=None):
     streams = eng.encode(cmds if cmds is not None else raws, opts, cmds=cmds is not None)
