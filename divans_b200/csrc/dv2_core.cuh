@@ -20,9 +20,9 @@
 //     ONE fix-up per quotient;
 //   * the next payload word of the eager-refill coder is always in a register; decoded literals leave as aligned 8-byte
 //     stores of last_8_literals;
-//   * LPG = 8: blend and rescale (frequentist_cdf.rs:74-85) are one packed add / one packed subtract for two elements.
-// (An L1 prefetch of the 16 candidate priors of the next low nibble -- contiguous thanks to lit_index_lo -- was built and
-// measured on the part this engine was first tuned on: prefetch.global.L1 only reached L2 there; it is not in the loop.)
+//   * LPG = 8: blend and rescale (frequentist_cdf.rs:74-85) are one packed add / one packed subtract for two elements;
+//   * literal priors in a dense order (lit_index_hi / lit_index_lo, dv_common.cuh): the priors a stream uses share cache lines,
+//     so that the hot priors of the resident streams stay in L1.
 // Decode only.
 #pragma once
 #include "dv_engine_kernel.cuh"
@@ -41,11 +41,6 @@ __device__ __forceinline__ int ld_s16g(const void *p) { int v; asm volatile("ld.
 __device__ __forceinline__ uint32_t ld_u8g(const void *p) { uint32_t v; asm volatile("ld.global.u8 %0, [%1];" : "=r"(v) : "l"(p) : "memory"); return v; }
 __device__ __forceinline__ void st_u32(const void *p, uint32_t v) { asm volatile("st.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
 __device__ __forceinline__ void st_u16(const void *p, uint32_t v) { asm volatile("st.global.u16 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
-// asynchronous 4-byte copy global -> shared through L1 (LDGSTS): used only for its side effect -- the line is brought into L1
-// (or at least requested from L2) long before the dependent load needs it; nobody ever waits for the copy itself
-__device__ __forceinline__ void touch_l1(const void *p, const uint32_t smem_dummy) {
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_dummy), "l"(p) : "memory");
-}
 // streaming accesses (touched once: payload words, decoded output): evict-first, so that they do not push the priors out of L2
 __device__ __forceinline__ uint32_t ld_stream_u32(const void *p) { uint32_t v; asm volatile("ld.global.cs.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory"); return v; }
 __device__ __forceinline__ void st_stream_u64(const void *p, unsigned long long v) { asm volatile("st.global.cs.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory"); }
@@ -335,7 +330,7 @@ __device__ __forceinline__ void literal_mix_loop16(St &s, const G2 g, const bool
     const int li = g.l16;
     const int cfg = active ? s.lit_cfg : mm_cfg(4);
     const uint32_t mm = (cfg & 0x100) ? 0xffu : 0u, o1 = (cfg & 0x200) ? 0xfu : 0u, fc = (cfg & 0x400) ? 0xfu : 0u;
-    const uint32_t sh = (uint32_t)(cfg >> 2) & 63u, which = (uint32_t)cfg & 3u;
+    const uint32_t sh = (uint32_t)(cfg >> 2) & 63u, which = (uint32_t)cfg & 3u, mhi = mm & (~o1 & 0xffu);
     const bool ro = (cfg & 0x800) != 0;                                      // mixing value 2: the stride prior is read, never adapted
     FastK f;
     f.inc = !active ? 0x10 : ro ? 0 : (int)(short)(s.ad_stride & 0xffff); f.lim = !active ? 0x2000 : ro ? 0x7fff : (s.ad_stride >> 16);
@@ -375,7 +370,7 @@ __device__ __forceinline__ void literal_mix_loop16(St &s, const G2 g, const bool
         m = min(m, __shfl_xor_sync(FULL, m, 16));
         if (m == 0) break;
         uint32_t ssb = (uint32_t)(l8 >> sh) & 0xffu;
-        const char *nbh = mk_ptr(hi_tab + (ctx * 256u + (ssb & mm & (~o1 & 0xffu))) * 32u, slot_hi), *cmh = mk_ptr(cmb + ctx * 32u, slot_hi);
+        const char *nbh = mk_ptr(hi_tab + lit_index_hi(which, ctx, ssb & mhi) * 32u, slot_hi), *cmh = mk_ptr(cmb + ctx * 32u, slot_hi);
         __syncwarp();
         MixV vh = mixv_load(nbh, cmh, li);
         for (uint32_t i = 0; i < m; i++) {
@@ -384,8 +379,8 @@ __device__ __forceinline__ void literal_mix_loop16(St &s, const G2 g, const bool
             if ((okh & gm) == gm) { vh.c &= 0x7fffu; vh.maxv &= 0x7fffu; } else { vh.c = defe; vh.maxv = 64u; }
             const MixS sh_ = mixv_search(k.a, vh, wh.norm, bsel);
             const uint32_t h = (uint32_t)sh_.sym;
-            const uint32_t ib = (mm & ssb) | ((~mm & 0xffu) & ctx), ic = (h & fc) | ((ctx & o1) << 4);
-            const char *const nbl = mk_ptr(lo_tab + (((ic >> 4) << 12) | (ib << 4) | (ic & 15u)) * 32u, slot_hi), *const cml = mk_ptr(cmb + (256u + h + 16u * ctx) * 32u, slot_hi);
+            const uint32_t ib = (mm & ssb) | ((~mm & 0xffu) & ctx), ic = (h & fc) + ((ctx & o1) << 4);
+            const char *const nbl = mk_ptr(lo_tab + lit_index_lo(which, ic, ib) * 32u, slot_hi), *const cml = mk_ptr(cmb + (256u + h + 16u * ctx) * 32u, slot_hi);
             __syncwarp();
             MixV vl = mixv_load(nbl, cml, li);
             mixv_finish(k.a, vh, sh_, wh, nbh, cmh, g, f, ch_inc, ch_lim);
@@ -400,7 +395,7 @@ __device__ __forceinline__ void literal_mix_loop16(St &s, const G2 g, const bool
             const uint32_t cv = ld_u16g(mk_ptr(t2 + (cur * 8u + pcp) * 2u, slot_hi));
             ctx = cv & 0xffu; pcp = cv >> 8;
             ssb = (uint32_t)(l8 >> sh) & 0xffu;
-            nbh = mk_ptr(hi_tab + (ctx * 256u + (ssb & mm & (~o1 & 0xffu))) * 32u, slot_hi); cmh = mk_ptr(cmb + ctx * 32u, slot_hi);
+            nbh = mk_ptr(hi_tab + lit_index_hi(which, ctx, ssb & mhi) * 32u, slot_hi); cmh = mk_ptr(cmb + ctx * 32u, slot_hi);
             __syncwarp();
             vh = mixv_load(nbh, cmh, li);   // speculative on the last byte: inside the slot
             mixv_finish(k.b, vl, sl_, wl, nbl, cml, g, f, cl_inc, cl_lim);
@@ -423,15 +418,12 @@ __device__ __forceinline__ void literal_mix_loop16(St &s, const G2 g, const bool
 // Converged literal fast path: code_nibble_array (codec/literal.rs:261-394) for whole bytes of every stream of the warp.
 // `active`: this group really is at the start of a literal byte.  A group that has run out of streams rides along as a dummy
 // (it codes garbage against its own slot and stores no output) so that its warp-mates keep the fast loop.
-// PF: touch the 16 candidate priors of the next nibble as soon as everything but that nibble's predecessor is known -- the low
-// nibble's candidates (one per value of the high nibble) are 512 contiguous bytes (lit_index_lo), the high nibble's (one per
-// value of the low nibble just being decoded) go through T2 per candidate.
 // Returns false (nothing done) when some group cannot take the fast loop: dynamic context mixing, per-context mixing values, the
 // flat prior, wide speeds, untagged priors, or the first 7 bytes of a literal that began within 8 bytes of the ring start -- the
 // caller then codes one nibble per group through the generic core and the state machine.
 // `t2s`: shared address of this group's T2S (16 lanes per stream), else 0.
-template <int LPG, bool PF>
-__device__ __forceinline__ bool literal_fast_v2(St &s, Next &nx, const G2 g, const bool active, const uint32_t smem_dummy, const uint32_t t2s) {
+template <int LPG>
+__device__ __forceinline__ bool literal_fast_v2(St &s, Next &nx, const G2 g, const bool active, const uint32_t t2s) {
     uint32_t n = active ? s.lit_left : 0xffffffffu;
     if (LPG == 8) n = min(n, __shfl_xor_sync(FULL, n, 8));
     n = min(n, __shfl_xor_sync(FULL, n, 16));
@@ -459,7 +451,7 @@ __device__ __forceinline__ bool literal_fast_v2(St &s, Next &nx, const G2 g, con
         const int li = g.l16;
         const int cfg = active ? s.lit_cfg : mm_cfg(4);
         const uint32_t mm = (cfg & 0x100) ? 0xffu : 0u, o1 = (cfg & 0x200) ? 0xfu : 0u, fc = (cfg & 0x400) ? 0xfu : 0u;
-        const uint32_t sh = (uint32_t)(cfg >> 2) & 63u, which = (uint32_t)cfg & 3u;
+        const uint32_t sh = (uint32_t)(cfg >> 2) & 63u, which = (uint32_t)cfg & 3u, mhi = mm & (~o1 & 0xffu);
         FastK f;
         f.inc = active ? (int)(short)(s.ad_stride & 0xffff) : 0x10; f.lim = active ? (s.ad_stride >> 16) : 0x2000;
         f.incp = (uint32_t)f.inc * 0x10001u;
@@ -503,16 +495,12 @@ __device__ __forceinline__ bool literal_fast_v2(St &s, Next &nx, const G2 g, con
             m = min(m, __shfl_xor_sync(FULL, m, 16));
             if (m == 0) break;   // unreachable: the literal coder codes nibbles in pairs, sym_count stays even
             // ---- priors of the first byte ----
+            // (low nibble: index_c = (high nibble & fc) + ((ctx & o1) << 4), index_b = ib -- all but the high nibble known a byte ahead)
             uint32_t ssb = (uint32_t)(l8 >> sh) & 0xffu;
-            uint32_t idx_h = ctx * 256u + (ssb & mm & (~o1 & 0xffu));
-            uint32_t row_l = ((ctx & o1) << 12) | (((mm & ssb) | ((~mm & 0xffu) & ctx)) << 4);
-            const char *ph = mk_ptr(hi_tab + idx_h * 32u, slot_hi);
+            uint32_t cl = (ctx & o1) << 4, ib = (mm & ssb) | ((~mm & 0xffu) & ctx);
+            const char *ph = mk_ptr(hi_tab + lit_index_hi(which, ctx, ssb & mhi) * 32u, slot_hi);
             __syncwarp();
             uint32_t eh = load_elems<LPG>(ph, li), mh = ld_u16g(ph + 30);
-            if (PF) {
-                touch_l1(mk_ptr(lo_tab + row_l * 32u + (LPG == 16 ? li * 32u : li * 64u), slot_hi), smem_dummy);
-                if (LPG == 8) touch_l1(mk_ptr(lo_tab + row_l * 32u + li * 64u + 32u, slot_hi), smem_dummy);
-            }
 // (16 lanes per stream: not unrolled -- the literal loop itself times the same with 1, 2 or 4 bytes per trip, but the
             // command path, which is instruction-fetch bound, is faster with the smaller kernel.  8 lanes per stream: two bytes
             // per trip)
@@ -526,18 +514,8 @@ __device__ __forceinline__ bool literal_fast_v2(St &s, Next &nx, const G2 g, con
                     if ((okh & gm) != gm) { eh_v = defe; mh_v = 64u; }
                     h = search_v2<LPG>(k.a, eh_v, mh_v, bsel);
                 }
-                if (PF) {   // candidates of the NEXT byte's high-nibble prior: this byte = (h, j) for every j
-#pragma unroll
-                    for (int q = 0; q < 16 / LPG; q++) {
-                        const uint32_t cj = ((uint32_t)h << 4) | (uint32_t)(LPG == 16 ? li : 2 * li + q);
-                        const uint32_t cvj = ld_u16g(mk_ptr(t2 + (cj * 8u + pcp) * 2u, slot_hi)) & 0xffu;
-                        const uint32_t sj = (uint32_t)(((l8 >> 8) | ((unsigned long long)cj << 56)) >> sh) & 0xffu;
-                        touch_l1(mk_ptr(hi_tab + (cvj * 256u + (sj & mm & (~o1 & 0xffu))) * 32u, slot_hi), smem_dummy);
-                    }
-                }
                 // -- low nibble: prior
-                const uint32_t idx_l = row_l + ((uint32_t)h & fc);
-                const char *const pl = mk_ptr(lo_tab + idx_l * 32u, slot_hi);
+                const char *const pl = mk_ptr(lo_tab + lit_index_lo(which, ((uint32_t)h & fc) + cl, ib) * 32u, slot_hi);
                 __syncwarp();
                 const uint32_t el = load_elems<LPG>(pl, li), ml = ld_u16g(pl + 30);
                 // -- high nibble: blend (this prior may be the next one to be loaded)
@@ -558,15 +536,10 @@ __device__ __forceinline__ bool literal_fast_v2(St &s, Next &nx, const G2 g, con
                 const uint32_t cv = small ? ld_shared_u8(t2s + cur) : ld_u16g(mk_ptr(t2 + (cur * 8u + pcp) * 2u, slot_hi));
                 ctx = cv & 0xffu; pcp = cv >> 8;
                 ssb = (uint32_t)(l8 >> sh) & 0xffu;
-                idx_h = ctx * 256u + (ssb & mm & (~o1 & 0xffu));
-                ph = mk_ptr(hi_tab + idx_h * 32u, slot_hi);
+                ph = mk_ptr(hi_tab + lit_index_hi(which, ctx, ssb & mhi) * 32u, slot_hi);
                 __syncwarp();
                 eh = load_elems<LPG>(ph, li); mh = ld_u16g(ph + 30);   // speculative on the last byte: inside the slot
-                row_l = ((ctx & o1) << 12) | (((mm & ssb) | ((~mm & 0xffu) & ctx)) << 4);
-                if (PF) {
-                    touch_l1(mk_ptr(lo_tab + row_l * 32u + (LPG == 16 ? li * 32u : li * 64u), slot_hi), smem_dummy);
-                    if (LPG == 8) touch_l1(mk_ptr(lo_tab + row_l * 32u + li * 64u + 32u, slot_hi), smem_dummy);
-                }
+                cl = (ctx & o1) << 4; ib = (mm & ssb) | ((~mm & 0xffu) & ctx);
                 // -- low nibble: blend; then the rANS steps of both nibbles (state a before b: the order of the payload words)
                 blend_store_v2<LPG>(el_v, ml_v, l, pl, g, f);
                 rans_pair_v2<LPG>(k.a, k.b, eh_v, mh_v, h, el_v, ml_v, l, f);

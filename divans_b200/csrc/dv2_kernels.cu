@@ -3,7 +3,6 @@
 // the same command state machine (dv_engine_kernel.cuh, transition<false, true>) as the round-1 decoders.
 #include "dv2_core.cuh"
 
-#include <algorithm>
 namespace dv {
 
 constexpr int DEC2_BLOCK_THREADS = 32;          // one warp per block: blocks spread evenly over the SMs
@@ -11,19 +10,16 @@ constexpr int DEC2_MIN_BLOCKS = 16;             // 4 one-warp blocks per schedul
                                                 // 16-lane streams per SM (4224 on an H100's 132 SMs).  (144 registers = 3 per partition = 12 per
                                                 // SM: 3168 resident 16-lane streams, a second wave for 4096)
 
-template <int LPG, bool PF>
+template <int LPG>
 __global__ void __launch_bounds__(DEC2_BLOCK_THREADS, DEC2_MIN_BLOCKS) decode_kernel_v2(DecodeParams p) {
     extern __shared__ __align__(16) uint8_t smem[];
     const int lane = threadIdx.x & 31;
     const int warp_in_block = threadIdx.x >> 5;
     constexpr int GPW = 32 / LPG;
     const int group_in_block = warp_in_block * GPW + lane / LPG;
-    // behind the groups' cold state: 16 lanes per stream, each group's T2S (dv2_core.cuh); then one dummy word per lane, the
-    // destination of the L1-touching async copies
+    // behind the groups' cold state: 16 lanes per stream, each group's T2S (dv2_core.cuh)
     constexpr uint32_t T2S_OFF = (DEC2_BLOCK_THREADS / LPG) * SMEM_BYTES_PER_GROUP_V2;
-    constexpr uint32_t DUMMY_OFF = T2S_OFF + (LPG == 16 ? (DEC2_BLOCK_THREADS / LPG) * T2S_BYTES : 0);
     const uint32_t t2s = LPG == 16 ? (uint32_t)__cvta_generic_to_shared(smem + T2S_OFF) + (uint32_t)group_in_block * T2S_BYTES : 0u;
-    const uint32_t smem_dummy = PF ? (uint32_t)__cvta_generic_to_shared(smem + DUMMY_OFF) + 4u * threadIdx.x : 0u;
     const uint32_t slot = blockIdx.x * (DEC2_BLOCK_THREADS / LPG) + group_in_block;
     G2 g;
     g.l16 = lane & (LPG - 1);
@@ -100,7 +96,7 @@ __global__ void __launch_bounds__(DEC2_BLOCK_THREADS, DEC2_MIN_BLOCKS) decode_ke
         }
         // ---- whole literal bytes while every group is at a byte boundary of a literal (or out of work) ----
         const bool lit = s.state == S_LIT_HI;
-        if (__any_sync(FULL, lit) && __all_sync(FULL, lit || s.state == S_DONE) && literal_fast_v2<LPG, PF>(s, nx, g, lit, smem_dummy, t2s)) {   // (the cheaper, usually false test first)
+        if (__any_sync(FULL, lit) && __all_sync(FULL, lit || s.state == S_DONE) && literal_fast_v2<LPG>(s, nx, g, lit, t2s)) {   // (the cheaper, usually false test first)
             if (lit) {
                 if (s.cur.underflow) s.status = ST_NEED_INPUT;
                 if (s.lit_left == 0 && s.status == ST_OK) { swap_coders(s, g); enter_cmd_type<false>(s, nx); }
@@ -132,22 +128,16 @@ __global__ void __launch_bounds__(DEC2_BLOCK_THREADS, DEC2_MIN_BLOCKS) decode_ke
     if (g.store0) *reinterpret_cast<uint32_t *>(s.slot + OFF_HDR) = s.c->gen_ctr;
 }
 
-// per block: the groups' cold state, 16 lanes per stream their T2S (+ one dummy word per thread, the target of the candidate-touch
-// prefetch, when that is compiled in)
-template <int LPG, bool PF> static size_t smem_v2() {
-    return (size_t)(DEC2_BLOCK_THREADS / LPG) * (SMEM_BYTES_PER_GROUP_V2 + (LPG == 16 ? T2S_BYTES : 0)) + (PF ? 4 * DEC2_BLOCK_THREADS : 0);
+// per block: the groups' cold state, 16 lanes per stream their T2S
+template <int LPG> static size_t smem_v2() {
+    return (size_t)(DEC2_BLOCK_THREADS / LPG) * (SMEM_BYTES_PER_GROUP_V2 + (LPG == 16 ? T2S_BYTES : 0));
 }
-template <int LPG, bool PF> static void launch_v2(const DecodeParams &p, uint32_t n_blocks, cudaStream_t st) {
-    decode_kernel_v2<LPG, PF><<<n_blocks, DEC2_BLOCK_THREADS, smem_v2<LPG, PF>(), st>>>(p);
+template <int LPG> static void launch_v2(const DecodeParams &p, uint32_t n_blocks, cudaStream_t st) {
+    decode_kernel_v2<LPG><<<n_blocks, DEC2_BLOCK_THREADS, smem_v2<LPG>(), st>>>(p);
 }
-template <int LPG, bool PF> static int tune_v2() { return stream_kernel_blocks_per_sm(decode_kernel_v2<LPG, PF>, DEC2_BLOCK_THREADS, smem_v2<LPG, PF>()); }
-template <int LPG> static int max_blocks_v2() {
-    const int nb = std::min(tune_v2<LPG, false>(), tune_v2<LPG, true>());
-    return nb;
-}
-void launch_decode_v2(int lanes_per_stream, bool prefetch, const DecodeParams &p, uint32_t n_blocks, cudaStream_t st) {
-    if (lanes_per_stream == 8) { if (prefetch) launch_v2<8, true>(p, n_blocks, st); else launch_v2<8, false>(p, n_blocks, st); }
-    else { if (prefetch) launch_v2<16, true>(p, n_blocks, st); else launch_v2<16, false>(p, n_blocks, st); }
+template <int LPG> static int max_blocks_v2() { return stream_kernel_blocks_per_sm(decode_kernel_v2<LPG>, DEC2_BLOCK_THREADS, smem_v2<LPG>()); }
+void launch_decode_v2(int lanes_per_stream, const DecodeParams &p, uint32_t n_blocks, cudaStream_t st) {
+    if (lanes_per_stream == 8) launch_v2<8>(p, n_blocks, st); else launch_v2<16>(p, n_blocks, st);
 }
 int decode_max_blocks_per_sm_v2(int lanes_per_stream) { return lanes_per_stream == 8 ? max_blocks_v2<8>() : max_blocks_v2<16>(); }
 int decode_groups_per_block_v2(int lanes_per_stream) { return DEC2_BLOCK_THREADS / lanes_per_stream; }

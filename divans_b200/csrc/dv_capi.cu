@@ -42,7 +42,6 @@ struct divans_b200_ctx {
     bool auto_lanes = false;         // lanes_per_stream 0: 16 lanes, or 8 where their residency holds the batch in fewer passes
     int last_lanes = 0;              // layout the most recent decode call used
     uint32_t cap16 = 0, cap8 = 0;    // resident streams of the two v2 layouts
-    bool prefetch = false;           // v2 engine: touch the candidate priors of the next nibble (env DIVANS_B200_PREFETCH, default off)
     int engine = 0;                  // 0: v2 (dv2_kernels.cu, lanes 16 or 8), 1: round-1 kernels (dv_kernels.cu, lanes 16 or 32)
     uint8_t *d_tables = nullptr;
     uint32_t *d_counter = nullptr;
@@ -111,7 +110,6 @@ extern "C" divans_b200_ctx *divans_b200_create(int device, uint32_t max_resident
     ctx->engine = (lanes_per_stream == 32 || lanes_per_stream == 116) ? 1 : 0;
     ctx->auto_lanes = lanes_per_stream == 0;
     ctx->lanes_per_stream = lanes_per_stream == 8 ? 8 : (lanes_per_stream == 32 ? 32 : 16);
-    { const char *e = getenv("DIVANS_B200_PREFETCH"); ctx->prefetch = e && atoi(e) != 0; }
     cudaDeviceProp prop;
     if (!ck(ctx, cudaSetDevice(device), "cudaSetDevice") || !ck(ctx, cudaGetDeviceProperties(&prop, device), "cudaGetDeviceProperties")) {
         fprintf(stderr, "divans_b200: no usable CUDA device %d -- this library has no CPU path\n", device);
@@ -185,7 +183,7 @@ extern "C" void divans_b200_destroy(divans_b200_ctx *ctx) {
     delete ctx;
 }
 // bumped whenever a decode kernel changes: bench.py quotes a stored DRAM-traffic capture (profiles/traffic.json) only for the version it measured
-#define DV_KERNEL_VERSION "r2.12-v2-t2s"
+#define DV_KERNEL_VERSION "r2.13-v2-dense-priors"
 extern "C" const char *divans_b200_kernel_version(void) { return DV_KERNEL_VERSION; }
 extern "C" const char *divans_b200_last_error(divans_b200_ctx *ctx) { return ctx ? ctx->err.c_str() : "null context"; }
 extern "C" int divans_b200_last_lanes(divans_b200_ctx *ctx) { return ctx ? ctx->last_lanes : 0; }
@@ -269,7 +267,7 @@ static DivansResult decode_device_nolock(divans_b200_ctx *ctx, size_t n, const u
     launch_frame(fp, ctx->d_payload, (uint64_t)ctx->payload_cap, st);
     if (dbg) { CK(cudaStreamSynchronize(st)); fprintf(stderr, "divans_b200[debug]: frame kernel ok (n=%zu)\n", n); }
     CK(cudaEventRecord(ctx->evm, st));
-    if (!skip_decode) { if (blend) launch_decode16_blend(dp, blocks, st); else if (ctx->engine == 0) launch_decode_v2(lanes, ctx->prefetch, dp, blocks, st); else if (ctx->lanes_per_stream == 16) launch_decode16(dp, blocks, st); else launch_decode32(dp, blocks, st); }
+    if (!skip_decode) { if (blend) launch_decode16_blend(dp, blocks, st); else if (ctx->engine == 0) launch_decode_v2(lanes, dp, blocks, st); else if (ctx->lanes_per_stream == 16) launch_decode16(dp, blocks, st); else launch_decode32(dp, blocks, st); }
     if (dbg) { CK(cudaStreamSynchronize(st)); fprintf(stderr, "divans_b200[debug]: decode kernel ok (blocks=%u, lps=%d)\n", blocks, ctx->lanes_per_stream); }
     CK(cudaEventRecord(ctx->ev1, st));
     CK(cudaEventRecord(ctx->ev_busy, st)); ctx->busy_recorded = true;

@@ -8,10 +8,10 @@
 //
 // A CDF is 16 x int16 = 32 B = one DRAM sector; lane i of a 16-lane group owns element i.
 // The in-memory order of priors is NOT on the wire (reference: src/priors.rs:211-237 only fixes the index rule),
-// so the literal tables are laid out [which][index_c][index_b]: one (which, index_c) "slab" is 256 consecutive
-// CDFs (8 KiB) and is default-initialised lazily by the kernel the first time the stream's context map / mixing
-// mask makes it reachable -- no 12.6 MB memset per stream (the reference default-initialises all of it,
-// codec/interface.rs:728-729).
+// so the round-1 engines lay the literal tables out [which][index_c][index_b]: one (which, index_c) "slab" is 256
+// consecutive CDFs (8 KiB) and is default-initialised lazily by the kernel the first time the stream's context map /
+// mixing mask makes it reachable -- no 12.6 MB memset per stream (the reference default-initialises all of it,
+// codec/interface.rs:728-729).  The v2 engine orders each which-block by lit_index_hi / lit_index_lo (below).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -47,9 +47,23 @@ constexpr uint64_t OFF_SLOT_END = OFF_HDR + 64;
 // the slot + offset), i.e. ONE 32-bit add in the decode loop instead of 64-bit pointer arithmetic (dv2_core.cuh).
 constexpr uint64_t SLOT_STRIDE = 16ull << 20;
 static_assert(OFF_SLOT_END <= SLOT_STRIDE, "slot layout exceeds the slot stride");
-// low-nibble prior index of the v2 engine: [which][index_c >> 4][index_b][index_c & 15]
+// Literal prior order of the v2 engine: the CDF index of prior (index_c, index_b) inside the 65536-CDF block of `which` (the
+// block itself starts at which << 16; all three blocks use the same order).  Every v2 access to LIT_HI / LIT_LO -- the generic
+// path and both fast loops -- goes through these two functions, so they cannot disagree.  The order is chosen so that the priors
+// one stream actually uses share cache lines (a 128-byte line holds 4 CDFs):
+//   high nibble: row (index_c - (index_b & 63)) & 255, column index_b.  For fixed index_b the row is a bijection of index_c.
+//     Under LSB6 with the identity context map and a stride byte that is the previous byte (mixing values 4-15 with stride 1),
+//     index_c = prev & 63 = index_b & 63: all 256 high priors of a stream are row 0, one contiguous 8 KiB run;
+//   low nibble: row index_c (the high nibble, plus the context's low bits for mixing value 1), column index_b: for text the
+//     hot rows (high nibble 2, 6, 7) hold runs of adjacent previous bytes.
+// The round-1 engines and the encoder keep [which][index_c][index_b] (dv_core.cuh, enter_lit_nibble<..., false>).
+__host__ __device__ __forceinline__ uint32_t lit_index_hi(uint32_t which, uint32_t index_c, uint32_t index_b) {
+    (void)which;
+    return (((index_c - (index_b & 63u)) & 255u) << 8) + index_b;
+}
 __host__ __device__ __forceinline__ uint32_t lit_index_lo(uint32_t which, uint32_t index_c, uint32_t index_b) {
-    return (which << 16) | ((index_c >> 4) << 12) | (index_b << 4) | (index_c & 15u);
+    (void)which;
+    return (index_c << 8) + index_b;
 }
 
 // CTYPE slab entries (indexed by the current command block type)

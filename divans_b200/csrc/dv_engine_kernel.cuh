@@ -62,9 +62,9 @@ __device__ __forceinline__ void enter_lit_nibble(St &s, Next &nx) {
     if (HIGH) { index_b = ssb & mm & (~o1 & 0xffu); index_c = ctx; }
     else { index_b = (mm & ssb) | ((~mm & 0xffu) & ctx); index_c = (s.lit_h & fc) | ((ctx & o1) << 4); }
     const uint32_t which = (uint32_t)cfg & 3u;
-    // v2 engine: the low-nibble table is laid out [index_c >> 4][index_b][index_c & 15] so that the 16 candidates of the
-    // next low nibble (one per value of the high nibble) are 512 contiguous bytes (lit_index_lo, dv_common.cuh)
-    const uint32_t flat = (V2 && !HIGH) ? lit_index_lo(which, index_c, index_b) : (which * 256 + index_c) * 256 + index_b;
+    // v2 engine: the order of lit_index_hi / lit_index_lo (dv_common.cuh), shared with the fast loops
+    const uint32_t flat = V2 ? (which << 16) + (HIGH ? lit_index_hi(which, index_c, index_b) : lit_index_lo(which, index_c, index_b))
+                             : (which * 256 + index_c) * 256 + index_b;
     int16_t *np = A_lit(s, HIGH) + (size_t)flat * 16;
     const bool ro = (cfg & 0x800) != 0;
     nx.mix_hi = HIGH;

@@ -18,7 +18,7 @@ void launch_decode32(const DecodeParams &p, uint32_t n_blocks, cudaStream_t st);
 void launch_decode16(const DecodeParams &p, uint32_t n_blocks, cudaStream_t st);
 int decode_max_blocks_per_sm32();
 // v2 engine (dv2_kernels.cu), lanes_per_stream = 16 (two streams per warp) or 8 (four)
-void launch_decode_v2(int lanes_per_stream, bool prefetch, const DecodeParams &p, uint32_t n_blocks, cudaStream_t st);
+void launch_decode_v2(int lanes_per_stream, const DecodeParams &p, uint32_t n_blocks, cudaStream_t st);
 int decode_max_blocks_per_sm_v2(int lanes_per_stream);
 int decode_groups_per_block_v2(int lanes_per_stream);
 int decode_max_blocks_per_sm16();
