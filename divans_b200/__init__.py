@@ -42,6 +42,7 @@ BATCH_SYMBOLS = [
     "divans_b200_synchronize", "divans_b200_encode_options_default", "divans_b200_encode_batch_host",
     "divans_b200_encode_cmds_batch_host", "divans_b200_encode_batch_device", "divans_b200_ir_to_cmds",
     "divans_b200_decode_batch_host_async", "divans_b200_decode_batch_host_wait", "divans_b200_lz77_cmds_batch", "divans_b200_kernel_version", "divans_b200_last_lanes",
+    "divans_b200_debug_slot_header",
 ]
 
 
@@ -91,6 +92,8 @@ def load_library():
     L.divans_b200_last_main_kernel_ms.restype = ctypes.c_float
     L.divans_b200_synchronize.argtypes = [vp]
     L.divans_b200_synchronize.restype = ctypes.c_uint8
+    L.divans_b200_debug_slot_header.argtypes = [vp, ctypes.c_uint32, ctypes.POINTER(ctypes.c_uint32 * 4)]
+    L.divans_b200_debug_slot_header.restype = ctypes.c_uint8
     batch = [vp, sz, vp, vp, vp, vp, vp, vp, vp, vp]
     L.divans_b200_decode_batch_host.argtypes = batch + [ctypes.c_uint32]
     L.divans_b200_decode_batch_host.restype = ctypes.c_uint8
@@ -240,6 +243,15 @@ class Engine:
 
     def _err(self):
         return self._L.divans_b200_last_error(self._h).decode()
+
+    def slot_header(self, i):
+        """Tests and diagnostics: the four persistent header words of arena slot ``i`` (include/divans_b200.h,
+        divans_b200_debug_slot_header) after the context's last call: [generation counter, untagged-tables flag,
+        literal-context-map high-water mark, stale-mixing-mask flag]."""
+        out = (ctypes.c_uint32 * 4)()
+        if self._L.divans_b200_debug_slot_header(self._h, int(i), ctypes.byref(out)) != DIVANS_SUCCESS:
+            raise DivansError("slot_header(%d): %s" % (i, self._err()))
+        return [int(v) for v in out]
 
     # -- host-buffer paths (numpy arrays; `in_blob`/`out` may be pinned)
     def decode_batch_host(self, in_blob, in_off, in_len, out, out_off, out_cap, flags=0):

@@ -250,8 +250,11 @@ __device__ __forceinline__ uint64_t rans_advance_v2(const uint64_t st, const uin
     }
     if (sym == 0) lo = 0;
     const uint32_t freq = hi - lo - 1;                                       // "major hax": start = lo + 1 (probability/interface.rs:103-104)
-    const uint32_t t = ((uint32_t)st & 0x7fffu) - lo - 1;                    // 0 <= t < freq: the search put the offset in this bin
-    return (uint64_t)freq * (st >> 15) + (uint64_t)t;
+    // 0 <= t < freq in every stream an encoder wrote.  A corrupted payload can put the offset below the bin: offset 0 decodes
+    // symbol 0, whose bin starts at 1 ("major hax"), so t = -1.  The reference computes the state in 64-bit wrapping arithmetic
+    // (ans.rs:230-244, coder_advance): t is sign-extended, not taken modulo 2^32.
+    const uint32_t t = ((uint32_t)st & 0x7fffu) - lo - 1;
+    return (uint64_t)freq * (st >> 15) + (uint64_t)(int64_t)(int32_t)t;
 }
 // The two rANS steps of a byte (state a: high nibble, b: low nibble), then the eager refills in payload order (a before b).  A
 // state needs a word once per ~16 nibbles of text: with 16 lanes per stream the refill code sits behind ONE warp-uniform branch
@@ -311,7 +314,7 @@ __device__ __forceinline__ void mixv_finish(uint64_t &st, const MixV v, const Mi
     const int f_cm = (int)(short)((hi_pn & 0xffffu) - (lo_pn & 0xffffu) - 1);
     const int f_nb = (int)(short)((hi_pn >> 16) - (lo_pn >> 16) - 1);
     const uint32_t t = ((uint32_t)st & 0x7fffu) - lo_a - 1;
-    uint64_t x = (uint64_t)(freq & 0xffffu) * (st >> 15) + (uint64_t)t;   // ans.rs:230-244
+    uint64_t x = (uint64_t)(int64_t)(int16_t)freq * (st >> 15) + (uint64_t)(int64_t)(int32_t)t;   // ans.rs:230-244 (t < 0: see rans_advance_v2)
     const bool refill = x < (1ull << 31);
     if (__any_sync(FULL, refill)) {   // (one warp-uniform branch instead of predicated-off refill code in every nibble, see rans_pair_v2)
         if (refill) { x = (x << 32) | (uint64_t)f.wnext; f.wi = min(f.wi + 1, f.wmax); f.wnext = ld_stream_u32(f.wbase + f.wi); }

@@ -183,7 +183,7 @@ extern "C" void divans_b200_destroy(divans_b200_ctx *ctx) {
     delete ctx;
 }
 // bumped whenever a decode kernel changes: bench.py quotes a stored DRAM-traffic capture (profiles/traffic.json) only for the version it measured
-#define DV_KERNEL_VERSION "r2.13-v2-dense-priors"
+#define DV_KERNEL_VERSION "r2.14-v2-signed-rans-offset"
 extern "C" const char *divans_b200_kernel_version(void) { return DV_KERNEL_VERSION; }
 extern "C" const char *divans_b200_last_error(divans_b200_ctx *ctx) { return ctx ? ctx->err.c_str() : "null context"; }
 extern "C" int divans_b200_last_lanes(divans_b200_ctx *ctx) { return ctx ? ctx->last_lanes : 0; }
@@ -203,6 +203,15 @@ extern "C" float divans_b200_last_main_kernel_ms(divans_b200_ctx *ctx) {
 extern "C" DivansResult divans_b200_synchronize(divans_b200_ctx *ctx) {
     if (!ctx) return DIVANS_FAILURE;
     CK(cudaStreamSynchronize(ctx->stream));
+    return DIVANS_SUCCESS;
+}
+extern "C" DivansResult divans_b200_debug_slot_header(divans_b200_ctx *ctx, uint32_t slot, uint32_t out[4]) {
+    if (!ctx || !out) return DIVANS_FAILURE;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    if (slot >= ctx->arena_slots) { ctx->err = "slot index beyond the arena"; return DIVANS_FAILURE; }
+    CK(cudaSetDevice(ctx->device));
+    if (ctx->busy_recorded) CK(cudaEventSynchronize(ctx->ev_busy));   // the last launch set of this context, on whatever stream
+    CK(cudaMemcpy(out, ctx->d_arena + (size_t)slot * SLOT_STRIDE + OFF_HDR, 16, cudaMemcpyDeviceToHost));
     return DIVANS_SUCCESS;
 }
 

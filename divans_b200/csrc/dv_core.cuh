@@ -173,7 +173,7 @@ __device__ __forceinline__ void mix_finish(Coder &k, uint64_t &st, const uint32_
     const int f_nb = (int)(short)(((unsigned)hi_pn >> 16) - ((unsigned)lo_pn >> 16) - 1);
     if (!ENC) {   // eager refill, see literal_fast
         const uint32_t t = ((uint32_t)st & 0x7fffu) - (uint32_t)start;
-        uint64_t x = (uint64_t)((uint32_t)freq & 0xffffu) * (st >> 15) + (uint64_t)t;   // ans.rs:230-244
+        uint64_t x = (uint64_t)(int64_t)freq * (st >> 15) + (uint64_t)(int64_t)(int32_t)t;   // ans.rs:230-244 (t < 0: see rans_advance_v2)
         if (x < (1ull << 31)) { x = (x << 32) | (uint64_t)wbase[wi]; wi = min(wi + 1, wmax); }
         st = x;
     } else { if (g.store0) const_cast<uint32_t *>(k.p)[k.left] = ((uint32_t)start & 0xffffu) | ((uint32_t)freq << 16); k.left++; }
@@ -273,7 +273,7 @@ __device__ __forceinline__ void literal_fast(St &s, Next &nx, const G2 g, const 
                     const uint32_t start = (uint32_t)(lo + 1), freq = (uint32_t)(hi - lo - 1);   // "major hax", probability/interface.rs:103-104
                     if (!ENC) {
                         const uint32_t t = ((uint32_t)k.a & 0x7fffu) - start;                      // 0 <= t < freq (the search put the offset in this bin)
-                        uint64_t x = (uint64_t)freq * (k.a >> 15) + (uint64_t)t;                    // ans.rs:230-244
+                        uint64_t x = (uint64_t)freq * (k.a >> 15) + (uint64_t)(int64_t)(int32_t)t;  // ans.rs:230-244 (t < 0: see rans_advance_v2)
                         if (x < (1ull << 31)) { x = (x << 32) | (uint64_t)wbase[wi]; wi = min(wi + 1, wmax); }
                         k.a = x;
                     } else { if (g.store0) const_cast<uint32_t *>(k.p)[k.left] = (start & 0xffffu) | (freq << 16); k.left++; }
@@ -305,7 +305,7 @@ __device__ __forceinline__ void literal_fast(St &s, Next &nx, const G2 g, const 
                     const uint32_t start = (uint32_t)(lo + 1), freq = (uint32_t)(hi - lo - 1);
                     if (!ENC) {
                         const uint32_t t = ((uint32_t)k.b & 0x7fffu) - start;
-                        uint64_t x = (uint64_t)freq * (k.b >> 15) + (uint64_t)t;
+                        uint64_t x = (uint64_t)freq * (k.b >> 15) + (uint64_t)(int64_t)(int32_t)t;
                         if (x < (1ull << 31)) { x = (x << 32) | (uint64_t)wbase[wi]; wi = min(wi + 1, wmax); }
                         k.b = x;
                     } else { if (g.store0) const_cast<uint32_t *>(k.p)[k.left] = (start & 0xffffu) | (freq << 16); k.left++; }

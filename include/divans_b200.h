@@ -176,6 +176,16 @@ DivansResult divans_b200_decode_batch_device(divans_b200_ctx *ctx, size_t n, con
                                              const uint64_t *d_out_cap, uint64_t *d_out_len, int32_t *d_status,
                                              uint64_t in_total_bytes, uint32_t flags, void *cuda_stream);
 DivansResult divans_b200_synchronize(divans_b200_ctx *ctx);
+/* For tests and diagnostics only: waits for the context's last call to finish, then copies the 16-byte header of arena
+ * slot `slot` to out[4] -- the state a v2 decoder slot carries from stream to stream and from launch to launch:
+ *   [0] generation counter (its low 16 bits tag the literal priors; 0 is skipped, the tables are wiped at the wrap),
+ *   [1] nonzero: the literal tables may hold untagged 16-bit values (the next v2 stream wipes them),
+ *   [2] literal-context-map bytes written since the map was last zeroed (high-water mark),
+ *   [3] nonzero: the mixing mask holds an earlier stream's values.
+ * Slot i of a decode launch is the i-th lane group (stream) of the grid.  Returns DIVANS_FAILURE when slot is not below the
+ * number of slots the context has allocated (none before its first decode or encode call).  The layout is not a stable
+ * interface. */
+DivansResult divans_b200_debug_slot_header(divans_b200_ctx *ctx, uint32_t slot, uint32_t out[4]);
 
 /* Encoder options (subset of the reference's DivansCompressorOptions, src/interface.rs:444-484, that affects the
  * entropy-coding half; command selection by the brotli crate is out of scope). */
