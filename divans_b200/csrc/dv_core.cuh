@@ -13,6 +13,15 @@ __device__ __forceinline__ uint32_t crc_step(const uint32_t *tab, uint32_t crc, 
 
 constexpr int SMEM_BYTES_PER_GROUP = (int)((sizeof(Cold) + 15) / 16 * 16);
 
+// Encoder: log one coded nibble.  A frequency <= 0 (a stream-supplied speed wrapped an i16 counter) cannot be coded: the
+// reference encoder panics on it and the oracle refuses the stream (ans_enc_put), so the stream fails, as in the blend core.
+// An idle group codes the dummy prior and is never failed.
+__device__ __forceinline__ void enc_log(St &s, const G2 g, int start, int freq) {
+    if (freq <= 0 && s.state != S_IDLE) s.status = ST_FAIL;
+    if (g.store0) const_cast<uint32_t *>(s.cur.p)[s.cur.left] = ((uint32_t)start & 0xffffu) | ((uint32_t)freq << 16);
+    s.cur.left++;
+}
+
 // The converged nibble core.  Every lane of the warp executes it every iteration, unpredicated: a group without work
 // codes against its slot's dummy CDF with a parked coder (no memory side effects that matter).
 template <bool ENC, int LPS>
@@ -36,7 +45,7 @@ __device__ __forceinline__ int nibble_core(St &s, const Next &nx, const G2 g, co
         if (sym == 0) lo = 0;
         start = (int)(short)(lo + 1); freq = (int)(short)(hi - lo - 1);   // "major hax", probability/interface.rs:103-104
         if (!ENC) coder_advance(s.cur, start, freq);
-        else { if (g.store0) const_cast<uint32_t *>(s.cur.p)[s.cur.left] = ((uint32_t)start & 0xffffu) | ((uint32_t)freq << 16); s.cur.left++; }
+        else enc_log(s, g, start, freq);
         int c2 = cdf_blend(gg, c, maxv, sym, inc, lim);
         if (writer) nx.cdf[g.l16] = (int16_t)c2;
         return sym;
@@ -70,7 +79,7 @@ __device__ __forceinline__ int nibble_core(St &s, const Next &nx, const G2 g, co
     int f_cm = cdf_freq(gg, cc, mc, sym);
     int f_nb = cdf_freq(gg, c, maxv, sym);
     if (!ENC) coder_advance(s.cur, start, freq);
-    else { if (g.store0) const_cast<uint32_t *>(s.cur.p)[s.cur.left] = ((uint32_t)start & 0xffffu) | ((uint32_t)freq << 16); s.cur.left++; }
+    else enc_log(s, g, start, freq);
     if (mixg) {
         weights_update(w, f_cm, f_nb, freq);
         if (nx.mix_hi) s.c->w_hi = w; else s.c->w_lo = w;
@@ -159,7 +168,7 @@ __device__ __forceinline__ MixSym mix_search(const uint64_t st, const G2 g, cons
 template <bool ENC>
 __device__ __forceinline__ void mix_finish(Coder &k, uint64_t &st, const uint32_t *const wbase, uint32_t &wi, const uint32_t wmax,
                                            const G2 g, const bool writer, char *nb, char *cm, const MixVals v, const MixSym ms, Weights &w,
-                                           const int nb_inc, const int nb_lim, const int cm_inc, const int cm_lim) {
+                                           const int nb_inc, const int nb_lim, const int cm_inc, const int cm_lim, bool &refused) {
     const int sym = ms.sym;
     // cumulative values of the three CDFs at sym and sym-1: two registers, four shuffles
     const int cum_a = cdf_div(ms.ca, ms.ma);
@@ -176,7 +185,11 @@ __device__ __forceinline__ void mix_finish(Coder &k, uint64_t &st, const uint32_
         uint64_t x = (uint64_t)(int64_t)freq * (st >> 15) + (uint64_t)(int64_t)(int32_t)t;   // ans.rs:230-244 (t < 0: see rans_advance_v2)
         if (x < (1ull << 31)) { x = (x << 32) | (uint64_t)wbase[wi]; wi = min(wi + 1, wmax); }
         st = x;
-    } else { if (g.store0) const_cast<uint32_t *>(k.p)[k.left] = ((uint32_t)start & 0xffffu) | ((uint32_t)freq << 16); k.left++; }
+    } else {   // small speeds keep both priors' steps >= 3, but their average can still round to a step of 1: freq 0 (see enc_log)
+        refused |= freq <= 0;
+        if (g.store0) const_cast<uint32_t *>(k.p)[k.left] = ((uint32_t)start & 0xffffu) | ((uint32_t)freq << 16);
+        k.left++;
+    }
     weights_update32(w, f_cm, f_nb, freq);
     const Grp gg = {FULL, g.shift, g.l16, writer, false, g.store0};
     const int c2 = cdf_blend(gg, v.cc, v.mc, sym, cm_inc, cm_lim);
@@ -348,6 +361,7 @@ __device__ __forceinline__ void literal_fast(St &s, Next &nx, const G2 g, const 
         uint8_t *dst = s.out + s.out_pos;
         Coder k = s.cur;
         Weights wh = s.c->w_hi, wl = s.c->w_lo;
+        bool refused = false;
         const uint32_t *const wbase = k.p;
         const uint32_t wmax = k.left + 1;
         uint32_t wi = 0;
@@ -384,7 +398,7 @@ __device__ __forceinline__ void literal_fast(St &s, Next &nx, const G2 g, const 
                 char *const nbl = lo_tab + (ic * 256u + ib) * 32u, *const cml = cmb + (256u + h + 16u * ctx) * 32u;
                 __syncwarp();
                 const MixVals vl = mix_load(g, nbl, cml);
-                mix_finish<ENC>(k, k.a, wbase, wi, wmax, g, writer, nbh, cmh, vh, sh_, wh, inc, lim, ch_inc, ch_lim);
+                mix_finish<ENC>(k, k.a, wbase, wi, wmax, g, writer, nbh, cmh, vh, sh_, wh, inc, lim, ch_inc, ch_lim, refused);
                 const MixSym sl_ = mix_search<ENC>(k.b, g, vl, wl, (int)(byte_in & 0xf));
                 const uint32_t cur = ((uint32_t)sl_.sym | (h << 4)) & 0xff;
                 l8 = (l8 >> 8) | ((unsigned long long)cur << 56);
@@ -395,7 +409,7 @@ __device__ __forceinline__ void literal_fast(St &s, Next &nx, const G2 g, const 
                 nbh = hi_tab + (ctx * 256u + ((uint32_t)(l8 >> sh) & mm & (~o1 & 0xffu))) * 32u; cmh = cmb + ctx * 32u;
                 __syncwarp();
                 vh = mix_load(g, nbh, cmh);   // speculative on the last byte: initialised slabs
-                mix_finish<ENC>(k, k.b, wbase, wi, wmax, g, writer, nbl, cml, vl, sl_, wl, inc, lim, cl_inc, cl_lim);
+                mix_finish<ENC>(k, k.b, wbase, wi, wmax, g, writer, nbl, cml, vl, sl_, wl, inc, lim, cl_inc, cl_lim, refused);
             }
             done += m;
             if (!ENC) k.sym_count += 2 * m;
@@ -407,6 +421,7 @@ __device__ __forceinline__ void literal_fast(St &s, Next &nx, const G2 g, const 
         }
         s.cur = k; s.l8 = l8; s.lit_ctx = ctx; s.out_pos += done; s.lit_left -= done;
         s.c->w_hi = wh; s.c->w_lo = wl;
+        if (ENC && refused) s.status = ST_FAIL;
         enter_lit_nibble<ENC, true>(s, nx);
         return;
     }

@@ -106,29 +106,34 @@ __global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) encode_model_kernel(E
             if (__all_sync(FULL, exhausted && s.state == S_IDLE)) break;
             __syncwarp();
         }
+        // end of a stream: report it, park the group on the dummy prior
+        auto finish = [&]() {
+            const uint32_t v = s.c->sidx;
+            if (g.store0) {
+                p.status[v] = s.status;
+                const uint32_t nc = s.c->cur_is_lit ? s.c->oth.left : s.cur.left, nl = s.c->cur_is_lit ? s.cur.left : s.c->oth.left;
+                p.sf_counts[2 * v] = s.status == ST_OK ? nc : 0; p.sf_counts[2 * v + 1] = s.status == ST_OK ? nl : 0;
+            }
+            s.state = S_IDLE; s.status = ST_OK;
+            nx.cdf = A_misc(s, MI_DUMMY); nx.cdf2 = nullptr; nx.speed = SPK_NONE; nx.tagged = false; nx.sym = 0;
+            coder_init_enc(s.cur, dummy_log);
+        };
         if (!BLEND && __all_sync(FULL, s.state == S_LIT_HI)) {
             literal_fast<true, LPS>(s, nx, g, writer);
             if (s.lit_left == 0 && s.status == ST_OK) { swap_coders(s, g); s.c->in.pos++; enter_cmd_type<true>(s, nx); }
+            if (s.status != ST_OK) finish();   // a symbol the loop could not code (enc_log): the stream ends here
             continue;
         }
         const bool busy = s.state != S_IDLE;
         int sym = core_dispatch<true, LPS, BLEND>(s, nx, g, writer);
         if (!busy) s.cur.left = 0;
         else {
-            // log overflow cannot happen for command lists whose sizes match the header; guard hostile blobs anyway
-            if (s.cur.left + 1 >= (s.c->cur_is_lit ? p.lit_cap : p.cmd_cap)) s.status = ST_FAIL;
-            else transition<true>(s, nx, g, sym);
-            if (s.status != ST_OK || s.state == S_IDLE) {
-                const uint32_t v = s.c->sidx;
-                if (g.store0) {
-                    p.status[v] = s.status;
-                    const uint32_t nc = s.c->cur_is_lit ? s.c->oth.left : s.cur.left, nl = s.c->cur_is_lit ? s.cur.left : s.c->oth.left;
-                    p.sf_counts[2 * v] = s.status == ST_OK ? nc : 0; p.sf_counts[2 * v + 1] = s.status == ST_OK ? nl : 0;
-                }
-                s.state = S_IDLE; s.status = ST_OK;
-                nx.cdf = A_misc(s, MI_DUMMY); nx.cdf2 = nullptr; nx.speed = SPK_NONE; nx.tagged = false; nx.sym = 0;
-                coder_init_enc(s.cur, dummy_log);
+            if (s.status == ST_OK) {   // (else the core could not code the symbol: enc_log)
+                // log overflow cannot happen for command lists whose sizes match the header; guard hostile blobs anyway
+                if (s.cur.left + 1 >= (s.c->cur_is_lit ? p.lit_cap : p.cmd_cap)) s.status = ST_FAIL;
+                else transition<true>(s, nx, g, sym);
             }
+            if (s.status != ST_OK || s.state == S_IDLE) finish();
         }
     }
 }
@@ -335,7 +340,7 @@ __global__ void __launch_bounds__(128) encode_mux_kernel(EncodeParams p) {
             bool any = false, have = false; uint64_t lf = 0;
             for (int i = 0; i < 2; i++) if (r[i]) { if (!have || last_flush[i] < lf) { lf = last_flush[i]; have = true; } }
             for (int i = 0; i < 2; i++) {
-                if ((!have || last_flush[i] <= lf + 131073) && r[i]) {
+                if ((!have || last_flush[i] <= lf + 131073) && r[i]) {   // (the lag test never fails when all is flushed at close: DESIGN §2)
                     const uint32_t n = r[i];
                     uint32_t take, hdr;
                     if (n == 4096 || n == 16384 || n >= 65536) {   // get_code(.., is_lagging = true), mux.rs:55-78

@@ -8,6 +8,7 @@ its name says; tests/test_gpu_slot_state.py sends them through one warp in every
 import collections
 import ctypes
 import functools
+import itertools
 
 import numpy as np
 
@@ -167,6 +168,169 @@ def build(name, oracle, variant=0):
 
 
 WIDE = (8192, 8192)    # 4 * (inc + 16) > 0x7fff: not speed_is_small (dv_engine.cuh), yet no i16 counter wraps
+
+
+# ---- the command list and encoder options behind every GOOD regime (tests/test_gpu_encode.py sends them to the GPU encoder) ----
+_RAW_DEFAULT = ("lsb6", "msb6", "utf8", "sign", "mix2_flat", "chunk_restart")   # raw mode, window 22
+
+
+def encode_options(name):
+    """oracle.options(**kw) / divans_b200.encode_options(**kw) arguments that encode command_list(name) to build(name).stream"""
+    if name in _RAW_DEFAULT:
+        return dict(window_size=22)
+    if name == "dcm2":
+        return dict(window_size=22, dynamic_context_mixing=2)
+    return dict(window_size=10 if name == "lit_quirk_w10" else 16)
+
+
+def command_list(name, oracle, variant=0):
+    """the command list of regime `name` as the oracle decodes it from build(name).stream (a raw-mode regime's list is the
+    PredictionMode and literal commands the raw encoder made).  Re-encoded under encode_options(name), it gives the stream
+    back byte for byte (tests/test_regimes.py)."""
+    case = build(name, oracle, variant)
+    rc, out, cl = oracle.decode_cmds(case.stream, out_cap=case.cap)
+    assert rc == 0
+    return cl
+
+
+# ---- framing and chunk edges: streams whose mux records or rANS chunks sit exactly on a boundary ----
+# (the parameters were found with the oracle; tests/test_regimes.py checks that each stream still has its property)
+#   name: (source, offset, length, property)   source "rnd" = random bytes under default options (raw mode),
+#   "lz16" = the oracle's LZ77 of the text corpus, window 16
+EDGES = {
+    "lit4096": ("rnd", 0, 3824, ("lit_payload", 4096)),
+    "lit16384": ("rnd", 1, 15178, ("lit_payload", 16384)),
+    "lit65536": ("rnd", 3, 60786, ("lit_payload", 65536)),
+    "lit69632": ("rnd", 0, 64594, ("lit_payload", 65536 + 4096)),
+    "lit81920": ("rnd", 0, 76036, ("lit_payload", 65536 + 16384)),
+    "lit131072": ("rnd", 0, 122248, ("lit_payload", 131072)),
+    "cmd4096": ("lz16", 0, 16784, ("cmd_payload", 4096)),
+    "cmd16384": ("lz16", 0, 59558, ("cmd_payload", 16384)),
+    "nib65535": ("lz16", 3, 63352, ("cmd_nibbles", 65535)),
+    "nib65536": ("lz16", 2, 63353, ("cmd_nibbles", 65536)),
+    "nib65537": ("lz16", 11, 63347, ("cmd_nibbles", 65537)),   # the command coder's last chunk holds 1 symbol
+    "both_over": ("both", 0, 125, ("both_over", 131073)),        # both payloads over 131073 bytes: 65536-byte records alternate
+}
+EDGE_NAMES = list(EDGES)
+
+
+@functools.lru_cache(maxsize=1)
+def _rnd():
+    return np.random.default_rng(1).integers(0, 256, 400000).astype(np.uint8).tobytes()
+
+
+@functools.lru_cache(maxsize=1)
+def _corpus():
+    from divans_b200 import synth
+    return synth.text_corpus(1 << 20)
+
+
+def edge_options(name):
+    return dict(window_size=22) if EDGES[name][0] == "rnd" else dict(window_size=16)
+
+
+@functools.lru_cache(maxsize=None)
+def edge(name, oracle):
+    """(Commands, raw, stream) of framing edge `name`"""
+    src, off, n, _prop = EDGES[name]
+    if src == "rnd":
+        raw = _rnd()[off:off + n]
+        stream = oracle.encode_raw(raw, oracle.options(**edge_options(name)))
+        cl = oracle.decode_cmds(stream, out_cap=n + 64)[2]
+        return cl, raw, stream
+    if src == "lz16":
+        raw = _corpus()[off:off + n]
+    else:                       # "both": n pieces of 5000 text bytes (copy-heavy) and 1000 random bytes (literal-heavy)
+        raw = b"".join(_corpus()[k * 5000:(k + 1) * 5000] + _rnd()[k * 1000:(k + 1) * 1000] for k in range(n))
+    cl = oracle.Commands.lz77(raw, window=16)
+    return cl, raw, cl.encode(oracle.options(**edge_options(name)))
+
+
+# ---- re-muxing: the same two coder payloads under another record chain ----
+def mux_records(oracle, stream, plan):
+    """`stream` with its record chain replaced by `plan`, a list of (coder, n, k): n bytes of coder 0 (commands) or 1
+    (literals), in a three-byte record (k None) or a one-byte record of code k (n = 1024 << 2k).  Header, EOF marker and
+    trailer as the mux writes them (mux.rs:29, codec/mod.rs:541-556); the CRC32C is recomputed by the oracle library."""
+    pay = oracle.demux(stream)
+    pos = [0, 0]
+    out = bytearray(stream[:16])
+    for coder, n, k in plan:
+        if k is None:
+            assert 1 <= n <= 65536
+            out += bytes([coder, (n - 1) & 0xFF, (n - 1) >> 8])
+        else:
+            assert n == 1024 << (2 * k)
+            out += bytes([coder | (k << 4)])
+        out += pay[coder][pos[coder]:pos[coder] + n]
+        pos[coder] += n
+    assert pos == [len(pay[0]), len(pay[1])], (pos, len(pay[0]), len(pay[1]))
+    return close(oracle, bytes(out))
+
+
+def close(oracle, body):
+    """header + records -> a complete stream: EOF marker, then the trailer with the CRC32C of everything before it"""
+    body += b"\xff\xfe\xff"
+    return body + oracle.crc32c(body).to_bytes(4, "little") + b"ans~"
+
+
+def record_starts(plan):
+    """offset in the stream of every record's first payload byte"""
+    o, res = 16, []
+    for _coder, n, k in plan:
+        o += 3 if k is None else 1
+        res.append(o)
+        o += n
+    return res
+
+
+def _split(n, sizes):
+    """cut n bytes into pieces of the given sizes (cycled), the last piece what is left"""
+    out, i = [], 0
+    while n:
+        t = min(n, sizes[i % len(sizes)])
+        out.append(t); n -= t; i += 1
+    return out
+
+
+def layout(name, lens, seed=0):
+    """a record plan over payload lengths lens = (commands, literals)"""
+    rng = np.random.default_rng(seed)
+    if name == "one_byte":                      # every record carries one byte, coders alternating while both last
+        q = [[(c, 1, None)] * lens[c] for c in (0, 1)]
+        return [r for pair in itertools.zip_longest(*q) for r in pair if r is not None]
+    if name == "random":                        # three-byte records of random sizes, coders in random order
+        q = [[(c, n, None) for n in _split(lens[c], [int(x) for x in rng.integers(1, 9000, 64)])] for c in (0, 1)]
+        return _interleave(q, rng)
+    if name == "codes":                         # one-byte codes k = 3, 2, 1 while the payload allows, then a tail
+        # (code 0 would be the byte 0x00 / 0x01, which is the first byte of a three-byte record: no stream can carry it)
+        q = []
+        for c in (0, 1):
+            left, recs = lens[c], []
+            for k in (3, 2, 1):
+                while left >= 1024 << (2 * k) and (k == 1 or rng.random() < 0.7 or left < 2 * (1024 << (2 * k))):
+                    recs.append((c, 1024 << (2 * k), k)); left -= 1024 << (2 * k)
+            recs += [(c, n, None) for n in _split(left, [777])]
+            q.append(recs)
+        return _interleave(q, rng)
+    if name == "lit_first":                     # every literal record before every command record
+        return [(1, n, None) for n in _split(lens[1], [5000])] + [(0, n, None) for n in _split(lens[0], [3000])]
+    if name == "align16":                       # sizes 1, 2, ..., 16, 1, ...: record starts at every offset mod 16
+        q = [[(c, n, None) for n in _split(lens[c], list(range(1, 17)))] for c in (0, 1)]
+        return [r for pair in itertools.zip_longest(*q) for r in pair if r is not None]
+    raise KeyError(name)
+
+
+LAYOUTS = ["one_byte", "random", "codes", "lit_first", "align16"]
+
+
+def _interleave(q, rng):
+    out, i = [], [0, 0]
+    while i[0] < len(q[0]) or i[1] < len(q[1]):
+        c = int(rng.integers(0, 2))
+        if i[c] >= len(q[c]):
+            c ^= 1
+        out.append(q[c][i[c]]); i[c] += 1
+    return out
 
 
 def speed_is_small(inc, lim):

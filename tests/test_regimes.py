@@ -108,3 +108,69 @@ def test_failing_regimes(oracle):
         assert rc == c.status == want
         if want != 2:                                   # the failure comes after the decoder went through literal bytes
             assert c.flags == R.SKIP_CRC and st["lit_nibbles"] > 1000
+
+
+# ---- the command lists behind the regimes, the framing edges and the re-muxer ----
+@pytest.mark.parametrize("name", R.GOOD)
+def test_regime_command_list_reencodes_to_its_stream(oracle, name):
+    """The GPU encoder tests send command_list(name) under encode_options(name); the oracle must turn that pair back into
+    exactly build(name).stream, so the encoder and decoder tests cannot drift apart."""
+    cl = R.command_list(name, oracle)
+    assert cl.encode(oracle.options(**R.encode_options(name))) == R.build(name, oracle).stream
+
+
+def _edge_property(oracle, name):
+    _cl, raw, stream = R.edge(name, oracle)
+    rc, out, st = oracle.decode(stream, out_cap=len(raw) + 64, stats=True)
+    assert rc == 0 and out == raw
+    cmd, lit = oracle.demux(stream)
+    return dict(cmd_payload=len(cmd), lit_payload=len(lit), cmd_nibbles=st["cmd_nibbles"], lit_nibbles=st["lit_nibbles"])
+
+
+@pytest.mark.parametrize("name", R.EDGE_NAMES)
+def test_framing_edge_has_its_property(oracle, name):
+    prop, want = R.EDGES[name][3]
+    got = _edge_property(oracle, name)
+    if prop == "both_over":
+        assert got["cmd_payload"] > want and got["lit_payload"] > want, got
+    else:
+        assert got[prop] == want, got
+    cl, raw, stream = R.edge(name, oracle)
+    assert cl.encode(oracle.options(**R.edge_options(name))) == stream
+
+
+def test_framing_edges_cover_the_mux_codes(oracle):
+    """the mux writes a one-byte record code for a 4096- or 16384-byte payload, and 65536-byte records before a tail; the
+    edges put each payload exactly on these sizes (and the command coder's final chunk at 1 symbol)"""
+    lit = sorted(R.EDGES[n][3][1] for n in R.EDGE_NAMES if R.EDGES[n][3][0] == "lit_payload")
+    cmd = sorted(R.EDGES[n][3][1] for n in R.EDGE_NAMES if R.EDGES[n][3][0] == "cmd_payload")
+    nib = sorted(R.EDGES[n][3][1] for n in R.EDGE_NAMES if R.EDGES[n][3][0] == "cmd_nibbles")
+    assert lit == [4096, 16384, 65536, 65536 + 4096, 65536 + 16384, 131072]
+    assert cmd == [4096, 16384] and nib == [65535, 65536, 65537]
+    stream = R.edge("lit16384", oracle)[2]
+    at = stream.find(oracle.demux(stream)[1][:64])
+    assert stream[at - 1] == 0x21   # literal coder, code k = 2: one header byte
+
+
+@pytest.mark.parametrize("lay", R.LAYOUTS)
+def test_remuxed_stream_decodes_on_the_oracle(oracle, lay):
+    """a new record chain over the same payloads decodes to the same bytes; each layout has the shape it is named for"""
+    for name in ("lit16384", "cmd4096", "both_over"):
+        _cl, raw, stream = R.edge(name, oracle)
+        lens = tuple(len(p) for p in oracle.demux(stream))
+        plan = R.layout(lay, lens, seed=3)
+        s2 = R.mux_records(oracle, stream, plan)
+        assert s2 != stream or lay == "codes"      # (codes on a 16384-byte payload: the mux's own layout)
+        rc, out = oracle.decode(s2, out_cap=len(raw) + 64)
+        assert rc == 0 and out == raw, (name, lay)
+        assert oracle.demux(s2) == oracle.demux(stream)
+        if lay == "one_byte":
+            assert all(n == 1 for _c, n, _k in plan)
+        if lay == "lit_first":
+            assert [c for c, _n, _k in plan] == sorted((c for c, _n, _k in plan), reverse=True)
+        if lay == "align16":
+            assert {o % 16 for o in R.record_starts(plan)} == set(range(16))
+        if lay == "codes" and name == "both_over":
+            assert {k for _c, _n, k in plan} == {1, 2, 3, None}
+        if lay == "random" and name == "both_over":
+            assert len({n for _c, n, _k in plan}) > 10 and len({c for c, _n, _k in plan[:20]}) == 2
