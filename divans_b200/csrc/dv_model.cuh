@@ -68,12 +68,13 @@ __device__ __forceinline__ void coder_advance(Coder &k, int start, int freq) {
 }
 
 // exact floor((c<<15)/max): the reference divides through a reciprocal LUT that is asserted equal to integer
-// division (probability/numeric.rs:26-31, make_div_lut.rs:37-39).  fp32 estimate + integer fix-up: c<<15 has <=16
-// significant bits, so the estimate is within 1 of the true quotient (<= 2^16).
+// division (probability/numeric.rs:26-31, make_div_lut.rs:37-39).  fp32 estimate + integer fix-up, for 0 <= c <= max <=
+// 0x7fff only: c<<15 has <= 15 significant bits and the quotient is <= 2^15, so the estimate is within 1 of it.
 // The reference's divide, literally (probability/numeric.rs:14-31 with RECIPROCAL[d as u16] = compute_divisor(d),
-// make_div_lut.rs:29-41).  Only reached with operands outside the adaptive range 0 <= c <= max <= 0x7fff, i.e. after a
-// stream-supplied speed made an i16 counter wrap (frequentist_cdf.rs:74-85): there the LUT divide is NOT integer division
-// and the decoder has to reproduce its exact value to stay in step with the reference.
+// make_div_lut.rs:29-41).  Reached with every other operand pair, i.e. after a stream-supplied speed made an i16 counter
+// wrap (frequentist_cdf.rs:74-85): with a negative element or max the LUT divide is NOT integer division and the coders have
+// to reproduce its exact value to stay in step with the reference; with an element above the max (a counter below it
+// wrapped, the element did not) the quotient reaches 2^30, far beyond what one fp32 estimate gets within 1 of (r2.16).
 static __device__ __noinline__ int cdf_div_ref(int c, int maxv) {
     const uint32_t d = (uint32_t)maxv & 0xffffu;
     const int32_t num = (int32_t)((uint32_t)c << 15);
@@ -88,7 +89,7 @@ static __device__ __noinline__ int cdf_div_ref(int c, int maxv) {
     return (t + (((int32_t)((long long)num - (m >> 31))) >> 1)) >> shift;
 }
 __device__ __forceinline__ int cdf_div(int c, int maxv) {
-    if (((unsigned)c | (unsigned)(maxv - 1)) > 0x7fffu) return cdf_div_ref(c, maxv);   // wrapped counters (never with the named speeds)
+    if ((unsigned)c > (unsigned)maxv || (unsigned)(maxv - 1) > 0x7ffeu) return cdf_div_ref(c, maxv);   // wrapped counters (never with the named speeds)
     uint32_t d = (uint32_t)maxv & 0xffffu;
     uint32_t n = (uint32_t)(c << 15);
     float rc;

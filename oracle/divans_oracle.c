@@ -303,6 +303,66 @@ void dvo_weights_update(dvo_weights *w, int16_t p0, int16_t p1, int16_t weighted
     w->norm = compute_normalized_weight(w->w);
 }
 
+/* batch helpers for the arithmetic tests (tests/test_gpu_arith.py, tests/test_arith_domains.py): many cases per call */
+void dvo_weights_update_batch(size_t n, const int32_t *w0, const int32_t *w1, const int16_t *p0, const int16_t *p1,
+                              const int16_t *weighted, int32_t *out_w0, int32_t *out_w1, int16_t *out_norm) {
+    for (size_t i = 0; i < n; i++) {
+        dvo_weights w; dvo_weights_init(&w);
+        w.w[0] = w0[i]; w.w[1] = w1[i];
+        dvo_weights_update(&w, p0[i], p1[i], weighted[i]);
+        out_w0[i] = w.w[0]; out_w1[i] = w.w[1]; out_norm[i] = w.norm;
+    }
+}
+void dvo_cdf_step_batch(size_t n, int mix, int enc, const int16_t *cdf, const int16_t *cdf2, const int32_t *wts,
+                        const dvo_speed *speeds, const uint64_t *state, const uint8_t *sym_in, uint8_t *sym_out, int16_t *start_out,
+                        int16_t *freq_out, uint64_t *state_out, int16_t *cdf_out, int16_t *cdf2_out, int32_t *wts_out) {
+    /* one literal nibble as code_lit_nibble codes it (codec/literal.rs:154-259): cdf = the stride prior, cdf2 = the
+     * context-map prior and wts = (w0, w1, norm) when mixing, speeds[2i] / [2i+1] = stride / context-map speed; decode
+     * takes the symbol from the rANS state (ans.rs:230-244, before renormalisation), encode from sym_in */
+    for (size_t i = 0; i < n; i++) {
+        dvo_cdf16 nb, cm, prob;
+        memcpy(nb.c, cdf + 16 * i, 32);
+        const dvo_cdf16 *coded = &nb;
+        dvo_weights w; dvo_weights_init(&w);
+        if (mix) {
+            memcpy(cm.c, cdf2 + 16 * i, 32);
+            w.w[0] = wts[3 * i]; w.w[1] = wts[3 * i + 1]; w.norm = (int16_t)wts[3 * i + 2];
+            dvo_cdf_average(&cm, &nb, (int32_t)(uint16_t)w.norm, &prob);
+            coded = &prob;
+        }
+        const uint64_t a = enc ? 0 : state[i];
+        int16_t start, freq;
+        uint8_t sym;
+        if (enc) { sym = sym_in[i] & 15; dvo_cdf_sym_start_freq(coded, sym, &start, &freq); }
+        else sym = dvo_cdf_lookup(coded, (int16_t)(a & 0x7fff), &start, &freq);
+        if (!enc) state_out[i] = (uint64_t)(int64_t)freq * (a >> 15) + (a & 0x7fff) - (uint64_t)(int64_t)start;
+        if (mix) {
+            int16_t st, f_cm, f_nb;
+            dvo_cdf_sym_start_freq(&cm, sym, &st, &f_cm);
+            dvo_cdf_sym_start_freq(&nb, sym, &st, &f_nb);
+            dvo_weights_update(&w, f_cm, f_nb, freq);
+            dvo_cdf_blend(&cm, sym, speeds[2 * i + 1]);
+            memcpy(cdf2_out + 16 * i, cm.c, 32);
+            wts_out[3 * i] = w.w[0]; wts_out[3 * i + 1] = w.w[1]; wts_out[3 * i + 2] = (uint16_t)w.norm;
+        }
+        dvo_cdf_blend(&nb, sym, speeds[2 * i]);
+        memcpy(cdf_out + 16 * i, nb.c, 32);
+        sym_out[i] = sym; start_out[i] = start; freq_out[i] = freq;
+    }
+}
+void dvo_cdf_walk_batch(size_t n_walks, size_t n_steps, const dvo_speed *speeds, const uint8_t *syms, dvo_cdf16 *trace) {
+    /* walk w starts at the default CDF and blends syms[w * n_steps + j] under speeds[w]; trace[w * (n_steps + 1) + j] is
+     * the CDF before step j (the last entry: after the walk) */
+    for (size_t w = 0; w < n_walks; w++) {
+        dvo_cdf16 c; dvo_cdf_default(&c);
+        for (size_t j = 0; j < n_steps; j++) {
+            trace[w * (n_steps + 1) + j] = c;
+            dvo_cdf_blend(&c, syms[w * n_steps + j], speeds[w]);
+        }
+        trace[w * (n_steps + 1) + n_steps] = c;
+    }
+}
+
 /* ------------------------------------------------------------------------------------------
  * prior tables: flat arrays, index rule of src/priors.rs:211-237 incl. the fall-through quirk
  * (a type that is not listed resolves to the LAST listed entry's offset)

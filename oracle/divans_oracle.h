@@ -76,6 +76,15 @@ uint32_t dvo_crc32c(uint32_t crc, const uint8_t *buf, size_t n); /* codec/crc32.
 typedef struct { int32_t w[2]; uint8_t mixing_param; int16_t norm; } dvo_weights;
 void dvo_weights_init(dvo_weights *w);
 void dvo_weights_update(dvo_weights *w, int16_t p0, int16_t p1, int16_t weighted);
+/* batch forms for the arithmetic tests: one update per case from (w0, w1) (mixing_param 1: not read by the update), and
+ * symbol walks from the default CDF (trace: n_steps + 1 CDFs per walk, the state before each step, then the final one) */
+void dvo_weights_update_batch(size_t n, const int32_t *w0, const int32_t *w1, const int16_t *p0, const int16_t *p1,
+                              const int16_t *weighted, int32_t *out_w0, int32_t *out_w1, int16_t *out_norm);
+/* one coded literal nibble per case at CDF level (plain, or mixing a context-map prior cdf2 with weights (w0, w1, norm)) */
+void dvo_cdf_step_batch(size_t n, int mix, int enc, const int16_t *cdf, const int16_t *cdf2, const int32_t *wts,
+                        const dvo_speed *speeds, const uint64_t *state, const uint8_t *sym_in, uint8_t *sym_out, int16_t *start_out,
+                        int16_t *freq_out, uint64_t *state_out, int16_t *cdf_out, int16_t *cdf2_out, int32_t *wts_out);
+void dvo_cdf_walk_batch(size_t n_walks, size_t n_steps, const dvo_speed *speeds, const uint8_t *syms, dvo_cdf16 *trace);
 
 /* ---- commands (the IR): reference src/interface.rs (re-exported brotli::enc::interface types) ---- */
 enum {

@@ -99,6 +99,9 @@ def lib():
         L.dvo_cdf_blend.argtypes = [ctypes.POINTER(Cdf16), ctypes.c_uint8, Speed]
         L.dvo_cdf_average.argtypes = [ctypes.POINTER(Cdf16), ctypes.POINTER(Cdf16), ctypes.c_int32, ctypes.POINTER(Cdf16)]
         L.dvo_weights_update.argtypes = [ctypes.POINTER(Weights), ctypes.c_int16, ctypes.c_int16, ctypes.c_int16]
+        L.dvo_weights_update_batch.argtypes = [ctypes.c_size_t] + [ctypes.c_void_p] * 8
+        L.dvo_cdf_step_batch.argtypes = [ctypes.c_size_t, ctypes.c_int, ctypes.c_int] + [ctypes.c_void_p] * 13
+        L.dvo_cdf_walk_batch.argtypes = [ctypes.c_size_t, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
         assert L.dvo_feature_blend() == (1 if _VARIANT == "blend" else 0)
         if _VARIANT == "blend":
             L.dvo_cdf_value.argtypes = [ctypes.POINTER(Cdf16), ctypes.c_uint8]
@@ -254,6 +257,43 @@ def demux(stream):
     rc = lib().dvo_demux(_ptr(body), body.size, _ptr(cmd), ctypes.byref(cl), _ptr(lit), ctypes.byref(ll), ctypes.byref(cons))
     assert rc == SUCCESS, rc
     return cmd[: cl.value].tobytes(), lit[: ll.value].tobytes()
+
+
+def weights_update_batch(w0, w1, f_cm, f_nb, weighted):
+    """codec/weights.rs update of every case (w0[i], w1[i]) with (f_cm, f_nb, weighted)[i]; returns (w0, w1, norm) arrays"""
+    w0, w1 = np.ascontiguousarray(w0, np.int32), np.ascontiguousarray(w1, np.int32)
+    p0, p1, wt = (np.ascontiguousarray(a, np.int16) for a in (f_cm, f_nb, weighted))
+    o0, o1, on = np.empty_like(w0), np.empty_like(w1), np.empty(w0.size, np.int16)
+    lib().dvo_weights_update_batch(w0.size, _ptr(w0), _ptr(w1), _ptr(p0), _ptr(p1), _ptr(wt), _ptr(o0), _ptr(o1), _ptr(on))
+    return o0, o1, on
+
+
+def cdf_steps(cdf, speeds, state=None, sym=None, cdf2=None, wts=None):
+    """one coded literal nibble per case (dvo_cdf_step_batch): cdf (n, 16) i16, speeds (n, 2, 2) i16 [(stride inc, lim),
+    (context-map inc, lim)], state (n,) u64 to decode or sym (n,) to encode, cdf2 (n, 16) and wts (n, 3) = (w0, w1, norm) to
+    mix.  Returns a dict of sym, start, freq, state (decode), cdf, and cdf2, wts (mixing)"""
+    cdf = np.ascontiguousarray(cdf, np.int16).reshape(-1, 16)
+    n, mix, enc = cdf.shape[0], cdf2 is not None, sym is not None
+    sp = np.ascontiguousarray(speeds, np.int16).reshape(n, 4)
+    c2 = np.ascontiguousarray(cdf2 if mix else np.zeros((n, 16)), np.int16)
+    w = np.ascontiguousarray(wts if mix else np.zeros((n, 3)), np.int32)
+    st = np.ascontiguousarray(state if not enc else np.zeros(n), np.uint64)
+    si = np.ascontiguousarray(sym if enc else np.zeros(n), np.uint8)
+    out = dict(sym=np.empty(n, np.uint8), start=np.empty(n, np.int16), freq=np.empty(n, np.int16), state=np.zeros(n, np.uint64),
+               cdf=np.empty((n, 16), np.int16), cdf2=np.zeros((n, 16), np.int16), wts=np.zeros((n, 3), np.int32))
+    lib().dvo_cdf_step_batch(n, int(mix), int(enc), _ptr(cdf), _ptr(c2), _ptr(w), _ptr(sp), _ptr(st), _ptr(si), _ptr(out["sym"]),
+                             _ptr(out["start"]), _ptr(out["freq"]), _ptr(out["state"]), _ptr(out["cdf"]), _ptr(out["cdf2"]), _ptr(out["wts"]))
+    return out
+
+
+def cdf_walks(speeds, syms):
+    """symbol walks from the default CDF: speeds (n, 2) i16 (inc, lim), syms (n, steps) u8.  Returns (n, steps + 1, 16) i16:
+    the CDF before each step, then the final one (frequentist_cdf.rs:74-85 through dvo_cdf_blend)"""
+    sp = np.ascontiguousarray(speeds, np.int16).reshape(-1, 2)
+    sy = np.ascontiguousarray(syms, np.uint8).reshape(sp.shape[0], -1)
+    tr = np.empty((sp.shape[0], sy.shape[1] + 1, ctypes.sizeof(Cdf16) // 2), np.int16)
+    lib().dvo_cdf_walk_batch(sp.shape[0], sy.shape[1], _ptr(sp), _ptr(sy), _ptr(tr))
+    return tr[:, :, :16]
 
 
 def decode_batch(blob, in_off, in_len, out_off, out_cap, n_threads=1, skip_crc=False):

@@ -333,6 +333,77 @@ def _interleave(q, rng):
     return out
 
 
+# ---- one literal prior driven into a state whose CDF element exceeds its max, then coded at that element ----
+# Literal speed (8192, 1920) (f8-representable, far outside speed_is_small) wraps the i16 counters of the high-nibble prior.
+# The all-zero literal context map with mixing value 0 sends every high nibble to one prior (index_b = index_c = 0,
+# codec/literal.rs:154-200).  The bytes were found by a seeded search over random high-nibble walks: the last byte's high
+# nibble is coded at element c = 9377 of a CDF whose max is 6, a quotient (c << 15) / max of 51,210,922 (> 2^24, where fp32
+# cannot even hold every integer), and every frequency the oracle encoder codes is > 0.
+# Dynamic context mixing 2 keeps the same stride prior and walk (the context-map priors take small speeds, or the averaged
+# CDF codes a frequency <= 0): a second path through the same prior state, whose frequency for the weights divides by that max.
+C_OVER_MAX_BYTES = bytes.fromhex("f50a0918421d1eb063b121b1b416a2a5f4d9884b48d1d58ff66b")
+C_OVER_MAX_SPEED = (8192, 1920)
+C_OVER_MAX_OPTIONS = {
+    "plain": dict(window_size=16, literal_adaptation=[C_OVER_MAX_SPEED] * 4),
+    "dcm2": dict(window_size=16, dynamic_context_mixing=2,
+                 literal_adaptation=[C_OVER_MAX_SPEED, C_OVER_MAX_SPEED, (16, 8192), (16, 8192)]),
+}
+
+
+def c_over_max(oracle, variant="plain"):
+    """(Commands, stream) of the c > max regime: one PredictionMode command, then the literal bytes"""
+    ir = "window 16 0 0 0\n%s\n%s\n" % (pm_line("lsb6", lmap=[0] * 64, mix=0), insert(C_OVER_MAX_BYTES))
+    cl = oracle.Commands.from_ir(ir)
+    return cl, cl.encode(oracle.options(**C_OVER_MAX_OPTIONS[variant]))
+
+
+def fp32_cdf_div(c, d):
+    """the fp32 path cdf_div took for every 0 <= c <= 0x7fff before kernel r2.16, emulated with a correctly rounded reciprocal in
+    place of rcp.approx (which cannot be emulated bit for bit)"""
+    n = np.uint32((c << 15) & 0xFFFFFFFF)
+    q = int(np.uint32(np.float32(n) * (np.float32(1) / np.float32(d))))
+    r = (int(n) - q * d) & 0xFFFFFFFF
+    r = r - (1 << 32) if r >= 1 << 31 else r
+    if r < 0:
+        q, r = q - 1, r + d
+    return q + 1 if r >= d else q
+
+
+def search_c_over_max(oracle, seed=3, speed=C_OVER_MAX_SPEED, misdivides=None, trials=20000):
+    """the seeded search that found C_OVER_MAX_BYTES (seed 3, trial 19585; about two minutes; not run by the tests).  Random
+    64-nibble high-nibble walks under `speed`; at the first nibble coded at an element c above the max with a quotient >= 2^24
+    that `misdivides(c, max)` (default: the fp32 emulation above differs from exact division; pass a set of measured
+    mismatch pairs to aim at those), up to 20 random low-nibble choices are tried until the oracle encoder accepts the bytes
+    under both C_OVER_MAX_OPTIONS.  Returns the bytes, or None."""
+    misdivides = misdivides or (lambda c, m: fp32_cdf_div(c, m) != (c << 15) // m)
+    rng = np.random.default_rng(seed)
+    pm = pm_line("lsb6", lmap=[0] * 64, mix=0)
+    for _trial in range(trials):
+        hs = rng.integers(0, 16, 64).astype(np.uint8)
+        tr = oracle.cdf_walks(np.array([speed], np.int16), hs[None, :])[0].astype(np.int64)
+        for k in range(64):
+            cdf, h = tr[k], int(hs[k])
+            c, m = int(cdf[h]), int(cdf[15])
+            if not (0 < m < c <= 0x7FFF and (c << 15) // m >= 1 << 24 and misdivides(c, m)):
+                continue
+            for _ in range(20):
+                data = bytes(int(x) << 4 | int(l) for x, l in zip(hs[:k + 1], rng.integers(0, 16, k + 1)))
+                try:
+                    for opts in C_OVER_MAX_OPTIONS.values():
+                        from_ir(oracle, [pm, insert(data)], **{k: v for k, v in opts.items() if k != "window_size"})
+                    return data
+                except ValueError:               # the oracle encoder refuses a frequency <= 0
+                    continue
+            break
+    return None
+
+
+def c_over_max_walk(oracle):
+    """the high-nibble prior before each byte (the oracle's dvo_cdf_blend walk), as (n, 16) ints"""
+    hs = np.frombuffer(C_OVER_MAX_BYTES, np.uint8) >> 4
+    return oracle.cdf_walks(np.array([C_OVER_MAX_SPEED], np.int16), hs[None, :])[0, :-1].astype(np.int64)
+
+
 def speed_is_small(inc, lim):
     """dv_engine.cuh speed_is_small: adaptive values of a prior with this speed stay inside [0, 0x7fff]"""
     return inc >= 0 and lim >= 0 and lim + inc + 16 <= 0x7FFF and 4 * (inc + 16) <= 0x7FFF

@@ -1,6 +1,7 @@
 """CPU checks of the regime builders (tests/regimes.py): each stream decodes on the oracle to its input or to its stated
 status, and really is the regime its name says -- command kinds, PredictionMode commands, speeds, mixing values, literal
 lengths and nibble counts -- so that the GPU tests built on them cannot quietly lose the case they were written to hit."""
+import numpy as np
 import pytest
 
 import regimes as R
@@ -174,3 +175,22 @@ def test_remuxed_stream_decodes_on_the_oracle(oracle, lay):
             assert {k for _c, _n, k in plan} == {1, 2, 3, None}
         if lay == "random" and name == "both_over":
             assert len({n for _c, n, _k in plan}) > 10 and len({c for c, _n, _k in plan[:20]}) == 2
+
+
+@pytest.mark.parametrize("variant", sorted(R.C_OVER_MAX_OPTIONS))
+def test_c_over_max_regime_codes_an_element_above_the_max(oracle, variant):
+    """the oracle encoder accepts the list (every coded frequency > 0), the stream decodes on the oracle, every high nibble
+    takes one prior, and the last one is coded at an element above that prior's max with a quotient >= 2^24"""
+    cl, stream = R.c_over_max(oracle, variant)
+    cmds, pms = R.commands(cl)
+    assert [c[0] for c in cmds] == [R.PREDMODE, R.LITERAL] and pms[0]["lit_map"] == bytes(64)
+    assert set(pms[0]["mixing"]) == {0}
+    rc, out = oracle.decode(stream, out_cap=len(R.C_OVER_MAX_BYTES) + 64)
+    assert rc == 0 and len(out) == len(R.C_OVER_MAX_BYTES)
+    walk = R.c_over_max_walk(oracle)
+    over = [(k, int(h)) for k, h in enumerate(np.frombuffer(R.C_OVER_MAX_BYTES, np.uint8) >> 4)
+            if 0 < walk[k, 15] < walk[k, h] <= 0x7FFF]
+    assert over, "no high nibble is coded at an element above the max"
+    k, h = over[-1]
+    assert k == len(R.C_OVER_MAX_BYTES) - 1
+    assert (int(walk[k, h]) << 15) // int(walk[k, 15]) >= 1 << 24
