@@ -418,6 +418,125 @@ __device__ __forceinline__ void literal_mix_loop16(St &s, const G2 g, const bool
     s.c->w_hi = wh; s.c->w_lo = wl;
 }
 
+// The plain loop of literal_fast_v2 (below).  SMALL: every group reads its context from T2S (16 lanes, LSB6 / MSB6); the loop is
+// compiled once for each case so that the one taken does not issue the other's predicated-off context load.
+template <int LPG, bool SMALL>
+__device__ __forceinline__ bool literal_plain_loop_v2(St &s, Next &nx, const G2 g, const bool active, const uint32_t t2s, const uint32_t n) {
+    constexpr bool small = SMALL;
+    const int li = g.l16;
+    const int cfg = active ? s.lit_cfg : mm_cfg(4);
+    const uint32_t mm = (cfg & 0x100) ? 0xffu : 0u, o1 = (cfg & 0x200) ? 0xfu : 0u, fc = (cfg & 0x400) ? 0xfu : 0u;
+    const uint32_t sh = (uint32_t)(cfg >> 2) & 63u, which = (uint32_t)cfg & 3u, mhi = mm & (~o1 & 0xffu);
+    FastK f;
+    f.inc = active ? (int)(short)(s.ad_stride & 0xffff) : 0x10; f.lim = active ? (s.ad_stride >> 16) : 0x2000;
+    f.incp = (uint32_t)f.inc * 0x10001u;
+    f.kp = LPG == 16 ? (uint32_t)(li + 1) : ((uint32_t)(2 * li + 1) | ((uint32_t)(2 * li + 2) << 16));
+    f.mytag = lane_tag<LPG>(s.gen, li);
+    const uint32_t tbits = LPG == 16 ? TAG_BITS16 : TAG_BITS8;
+    const uint32_t defe = default_elems<LPG>(li);
+    const uint32_t bsel = LPG == 16 ? (0xffffu << g.shift) : ((uint32_t)(g.shift >> 3) * 0x1111u + 0x4040u);
+    const unsigned gm = g.gmask;
+    // every address inside the slot is (slot_hi : slot_lo + offset): slots are 16 MiB aligned
+    const uint32_t slot_lo = (uint32_t)(uintptr_t)s.slot, slot_hi = (uint32_t)((uintptr_t)s.slot >> 32);
+    const uint32_t hi_tab = slot_lo + (uint32_t)OFF_LIT_HI + which * (65536u * 32u), lo_tab = slot_lo + (uint32_t)OFF_LIT_LO + which * (65536u * 32u);
+    const uint32_t t2 = slot_lo + (uint32_t)OFF_T2;
+    unsigned long long l8 = active ? s.l8 : 0ull;
+    uint32_t ctx = active ? s.lit_ctx : 0u;
+    uint32_t pcp = ld_u16g(mk_ptr(t2 + (uint32_t)(l8 >> 56) * 16u, slot_hi)) >> 8;   // class of the byte before the next one to decode
+    // output: an aligned 8-byte store of l8 whenever the cursor completes an 8-byte word (l8 mirrors the 8 bytes in front of
+    // the cursor here: the caller keeps the first 7 bytes of a literal that began within 8 bytes of the ring start away)
+    uint8_t *const dbase = s.out + s.out_pos;
+    uint32_t ap = (uint32_t)(uintptr_t)dbase & 7u;                        // alignment of the ADDRESS of the byte being decoded
+    const bool st_lane = g.store0 && active;
+    Coder k = s.cur;
+    if (!active) { k.p = reinterpret_cast<const uint32_t *>(s.slot + OFF_T2); k.left = 0; k.need_a = 0; k.need_b = 0; k.sym_count = 0; k.a = k.b = 1ull << 40; }
+    // ---- eager-refill coder (dv_core.cuh literal_fast): state a codes every high nibble, b every low nibble ----
+    f.wbase = k.p; f.wmax = k.left + 1; f.wi = 0;
+    coder_fill(k);                                                        // pending refill / 16-byte (re)initialisation of `a`
+    f.wi = (uint32_t)(k.p - f.wbase);
+    if (k.need_b) { k.b = (k.b << 32) | (uint64_t)f.wbase[f.wi]; f.wi = min(f.wi + 1, f.wmax); k.need_b = 0; }
+    f.wnext = f.wbase[f.wi];
+    uint32_t done = 0;
+    while (done < n) {
+        uint32_t m = n - done;
+        if (k.sym_count >= NUM_SYMBOLS_BEFORE_FLUSH) {   // chunk restart, ans.rs:173-189
+            if (f.wi + 5 <= f.wmax) { k.a = (uint64_t)f.wbase[f.wi] | ((uint64_t)f.wbase[f.wi + 1] << 32); k.b = (uint64_t)f.wbase[f.wi + 2] | ((uint64_t)f.wbase[f.wi + 3] << 32); f.wi += 4; }
+            else { k.a = k.b = 0; f.wi = f.wmax; }
+            f.wnext = f.wbase[f.wi];
+            k.sym_count = 0;
+        }
+        m = min(m, (NUM_SYMBOLS_BEFORE_FLUSH - k.sym_count) >> 1);
+        if (LPG == 8) m = min(m, __shfl_xor_sync(FULL, m, 8));
+        m = min(m, __shfl_xor_sync(FULL, m, 16));
+        if (m == 0) break;   // unreachable: the literal coder codes nibbles in pairs, sym_count stays even
+        // ---- priors of the first byte ----
+        // (low nibble: index_c = (high nibble & fc) + ((ctx & o1) << 4), index_b = ib -- all but the high nibble known a byte ahead)
+        uint32_t ssb = (uint32_t)(l8 >> sh) & 0xffu;
+        uint32_t cl = (ctx & o1) << 4, ib = (mm & ssb) | ((~mm & 0xffu) & ctx);
+        const char *ph = mk_ptr(hi_tab + lit_index_hi(which, ctx, ssb & mhi) * 32u, slot_hi);
+        __syncwarp();
+        uint32_t eh = load_elems<LPG>(ph, li), mh = ld_u16g(ph + 30);
+// (16 lanes per stream: not unrolled -- the literal loop itself times the same with 1, 2 or 4 bytes per trip, but the
+        // command path, which is instruction-fetch bound, is faster with the smaller kernel.  8 lanes per stream: two bytes
+        // per trip)
+#pragma unroll (LPG == 16 ? 1 : 2)
+        for (uint32_t i = 0; i < m; i++) {
+            // -- high nibble: search (speculative: the prior is almost always one this stream has written)
+            uint32_t eh_v = eh & ~tbits, mh_v = mh & 0x7fffu;
+            int h = search_v2<LPG>(k.a, eh_v, mh_v, bsel);
+            const unsigned okh = __ballot_sync(FULL, !active || (eh & tbits) == f.mytag);
+            if (__builtin_expect(okh != FULL, 0)) {                       // some group met a prior of an older stream: default CDF
+                if ((okh & gm) != gm) { eh_v = defe; mh_v = 64u; }
+                h = search_v2<LPG>(k.a, eh_v, mh_v, bsel);
+            }
+            // -- low nibble: prior
+            const char *const pl = mk_ptr(lo_tab + lit_index_lo(which, ((uint32_t)h & fc) + cl, ib) * 32u, slot_hi);
+            __syncwarp();
+            const uint32_t el = load_elems<LPG>(pl, li), ml = ld_u16g(pl + 30);
+            // -- high nibble: blend (this prior may be the next one to be loaded)
+            blend_store_v2<LPG>(eh_v, mh_v, h, ph, g, f);
+            // -- low nibble: search
+            uint32_t el_v = el & ~tbits, ml_v = ml & 0x7fffu;
+            int l = search_v2<LPG>(k.b, el_v, ml_v, bsel);
+            const unsigned okl = __ballot_sync(FULL, !active || (el & tbits) == f.mytag);
+            if (__builtin_expect(okl != FULL, 0)) {
+                if ((okl & gm) != gm) { el_v = defe; ml_v = 64u; }
+                l = search_v2<LPG>(k.b, el_v, ml_v, bsel);
+            }
+            const uint32_t cur = ((uint32_t)l | ((uint32_t)h << 4)) & 0xffu;
+            l8 = (l8 >> 8) | ((unsigned long long)cur << 56);              // push_literal_byte, codec/interface.rs:280-284
+            if (st_lane && (ap & 7u) == 7u) st_stream_u64(dbase + (done + i) - 7, l8);
+            ap++;
+            // -- context and priors of the next byte (get_prev_word_context, codec/literal.rs:87-117, through T2)
+            const uint32_t cv = small ? ld_shared_u8(t2s + cur) : ld_u16g(mk_ptr(t2 + (cur * 8u + pcp) * 2u, slot_hi));
+            ctx = cv & 0xffu; pcp = cv >> 8;
+            ssb = (uint32_t)(l8 >> sh) & 0xffu;
+            ph = mk_ptr(hi_tab + lit_index_hi(which, ctx, ssb & mhi) * 32u, slot_hi);
+            __syncwarp();
+            eh = load_elems<LPG>(ph, li); mh = ld_u16g(ph + 30);   // speculative on the last byte: inside the slot
+            cl = (ctx & o1) << 4; ib = (mm & ssb) | ((~mm & 0xffu) & ctx);
+            // -- low nibble: blend; then the rANS steps of both nibbles (state a before b: the order of the payload words)
+            blend_store_v2<LPG>(el_v, ml_v, l, pl, g, f);
+            rans_pair_v2<LPG>(k.a, k.b, eh_v, mh_v, h, el_v, ml_v, l, f);
+        }
+        done += m;
+        if (active) k.sym_count += 2 * m;
+    }
+    if (!active) return true;
+    // the bytes after the last aligned 8-byte store are still only in l8
+    if (g.store0) {
+        const uint32_t tail = min(ap & 7u, done);
+        for (uint32_t t = 0; t < tail; t++) dbase[done - tail + t] = (uint8_t)(l8 >> (8 * (8 - tail + t)));
+    }
+    // back to the lazy representation the state machine uses
+    if (f.wi >= f.wmax) { k.underflow = 1; f.wi = f.wmax - 1; }
+    k.p = f.wbase + f.wi; k.left = f.wmax - 1 - f.wi;
+    k.need_a = (k.sym_count >= NUM_SYMBOLS_BEFORE_FLUSH) ? 8u : 0u; k.need_b = 0;
+    s.cur = k; s.l8 = l8; s.lit_ctx = ctx; s.out_pos += done; s.lit_left -= done;
+    enter_lit_nibble<false, true, true>(s, nx);
+    return true;
+}
+
 // Converged literal fast path: code_nibble_array (codec/literal.rs:261-394) for whole bytes of every stream of the warp.
 // `active`: this group really is at the start of a literal byte.  A group that has run out of streams rides along as a dummy
 // (it codes garbage against its own slot and stores no output) so that its warp-mates keep the fast loop.
@@ -451,118 +570,8 @@ __device__ __forceinline__ bool literal_fast_v2(St &s, Next &nx, const G2 g, con
         // every group in LSB6 / MSB6 (16 lanes): the context comes from T2S in shared memory (a dummy group reads garbage
         // contexts, which still address inside its own slot)
         const bool small = LPG == 16 && __all_sync(FULL, !active || t2s_mode(s.pred_mode));
-        const int li = g.l16;
-        const int cfg = active ? s.lit_cfg : mm_cfg(4);
-        const uint32_t mm = (cfg & 0x100) ? 0xffu : 0u, o1 = (cfg & 0x200) ? 0xfu : 0u, fc = (cfg & 0x400) ? 0xfu : 0u;
-        const uint32_t sh = (uint32_t)(cfg >> 2) & 63u, which = (uint32_t)cfg & 3u, mhi = mm & (~o1 & 0xffu);
-        FastK f;
-        f.inc = active ? (int)(short)(s.ad_stride & 0xffff) : 0x10; f.lim = active ? (s.ad_stride >> 16) : 0x2000;
-        f.incp = (uint32_t)f.inc * 0x10001u;
-        f.kp = LPG == 16 ? (uint32_t)(li + 1) : ((uint32_t)(2 * li + 1) | ((uint32_t)(2 * li + 2) << 16));
-        f.mytag = lane_tag<LPG>(s.gen, li);
-        const uint32_t tbits = LPG == 16 ? TAG_BITS16 : TAG_BITS8;
-        const uint32_t defe = default_elems<LPG>(li);
-        const uint32_t bsel = LPG == 16 ? (0xffffu << g.shift) : ((uint32_t)(g.shift >> 3) * 0x1111u + 0x4040u);
-        const unsigned gm = g.gmask;
-        // every address inside the slot is (slot_hi : slot_lo + offset): slots are 16 MiB aligned
-        const uint32_t slot_lo = (uint32_t)(uintptr_t)s.slot, slot_hi = (uint32_t)((uintptr_t)s.slot >> 32);
-        const uint32_t hi_tab = slot_lo + (uint32_t)OFF_LIT_HI + which * (65536u * 32u), lo_tab = slot_lo + (uint32_t)OFF_LIT_LO + which * (65536u * 32u);
-        const uint32_t t2 = slot_lo + (uint32_t)OFF_T2;
-        unsigned long long l8 = active ? s.l8 : 0ull;
-        uint32_t ctx = active ? s.lit_ctx : 0u;
-        uint32_t pcp = ld_u16g(mk_ptr(t2 + (uint32_t)(l8 >> 56) * 16u, slot_hi)) >> 8;   // class of the byte before the next one to decode
-        // output: an aligned 8-byte store of l8 whenever the cursor completes an 8-byte word (l8 mirrors the 8 bytes in front of
-        // the cursor here: the caller keeps the first 7 bytes of a literal that began within 8 bytes of the ring start away)
-        uint8_t *const dbase = s.out + s.out_pos;
-        uint32_t ap = (uint32_t)(uintptr_t)dbase & 7u;                        // alignment of the ADDRESS of the byte being decoded
-        const bool st_lane = g.store0 && active;
-        Coder k = s.cur;
-        if (!active) { k.p = reinterpret_cast<const uint32_t *>(s.slot + OFF_T2); k.left = 0; k.need_a = 0; k.need_b = 0; k.sym_count = 0; k.a = k.b = 1ull << 40; }
-        // ---- eager-refill coder (dv_core.cuh literal_fast): state a codes every high nibble, b every low nibble ----
-        f.wbase = k.p; f.wmax = k.left + 1; f.wi = 0;
-        coder_fill(k);                                                        // pending refill / 16-byte (re)initialisation of `a`
-        f.wi = (uint32_t)(k.p - f.wbase);
-        if (k.need_b) { k.b = (k.b << 32) | (uint64_t)f.wbase[f.wi]; f.wi = min(f.wi + 1, f.wmax); k.need_b = 0; }
-        f.wnext = f.wbase[f.wi];
-        uint32_t done = 0;
-        while (done < n) {
-            uint32_t m = n - done;
-            if (k.sym_count >= NUM_SYMBOLS_BEFORE_FLUSH) {   // chunk restart, ans.rs:173-189
-                if (f.wi + 5 <= f.wmax) { k.a = (uint64_t)f.wbase[f.wi] | ((uint64_t)f.wbase[f.wi + 1] << 32); k.b = (uint64_t)f.wbase[f.wi + 2] | ((uint64_t)f.wbase[f.wi + 3] << 32); f.wi += 4; }
-                else { k.a = k.b = 0; f.wi = f.wmax; }
-                f.wnext = f.wbase[f.wi];
-                k.sym_count = 0;
-            }
-            m = min(m, (NUM_SYMBOLS_BEFORE_FLUSH - k.sym_count) >> 1);
-            if (LPG == 8) m = min(m, __shfl_xor_sync(FULL, m, 8));
-            m = min(m, __shfl_xor_sync(FULL, m, 16));
-            if (m == 0) break;   // unreachable: the literal coder codes nibbles in pairs, sym_count stays even
-            // ---- priors of the first byte ----
-            // (low nibble: index_c = (high nibble & fc) + ((ctx & o1) << 4), index_b = ib -- all but the high nibble known a byte ahead)
-            uint32_t ssb = (uint32_t)(l8 >> sh) & 0xffu;
-            uint32_t cl = (ctx & o1) << 4, ib = (mm & ssb) | ((~mm & 0xffu) & ctx);
-            const char *ph = mk_ptr(hi_tab + lit_index_hi(which, ctx, ssb & mhi) * 32u, slot_hi);
-            __syncwarp();
-            uint32_t eh = load_elems<LPG>(ph, li), mh = ld_u16g(ph + 30);
-// (16 lanes per stream: not unrolled -- the literal loop itself times the same with 1, 2 or 4 bytes per trip, but the
-            // command path, which is instruction-fetch bound, is faster with the smaller kernel.  8 lanes per stream: two bytes
-            // per trip)
-#pragma unroll (LPG == 16 ? 1 : 2)
-            for (uint32_t i = 0; i < m; i++) {
-                // -- high nibble: search (speculative: the prior is almost always one this stream has written)
-                uint32_t eh_v = eh & ~tbits, mh_v = mh & 0x7fffu;
-                int h = search_v2<LPG>(k.a, eh_v, mh_v, bsel);
-                const unsigned okh = __ballot_sync(FULL, !active || (eh & tbits) == f.mytag);
-                if (__builtin_expect(okh != FULL, 0)) {                       // some group met a prior of an older stream: default CDF
-                    if ((okh & gm) != gm) { eh_v = defe; mh_v = 64u; }
-                    h = search_v2<LPG>(k.a, eh_v, mh_v, bsel);
-                }
-                // -- low nibble: prior
-                const char *const pl = mk_ptr(lo_tab + lit_index_lo(which, ((uint32_t)h & fc) + cl, ib) * 32u, slot_hi);
-                __syncwarp();
-                const uint32_t el = load_elems<LPG>(pl, li), ml = ld_u16g(pl + 30);
-                // -- high nibble: blend (this prior may be the next one to be loaded)
-                blend_store_v2<LPG>(eh_v, mh_v, h, ph, g, f);
-                // -- low nibble: search
-                uint32_t el_v = el & ~tbits, ml_v = ml & 0x7fffu;
-                int l = search_v2<LPG>(k.b, el_v, ml_v, bsel);
-                const unsigned okl = __ballot_sync(FULL, !active || (el & tbits) == f.mytag);
-                if (__builtin_expect(okl != FULL, 0)) {
-                    if ((okl & gm) != gm) { el_v = defe; ml_v = 64u; }
-                    l = search_v2<LPG>(k.b, el_v, ml_v, bsel);
-                }
-                const uint32_t cur = ((uint32_t)l | ((uint32_t)h << 4)) & 0xffu;
-                l8 = (l8 >> 8) | ((unsigned long long)cur << 56);              // push_literal_byte, codec/interface.rs:280-284
-                if (st_lane && (ap & 7u) == 7u) st_stream_u64(dbase + (done + i) - 7, l8);
-                ap++;
-                // -- context and priors of the next byte (get_prev_word_context, codec/literal.rs:87-117, through T2)
-                const uint32_t cv = small ? ld_shared_u8(t2s + cur) : ld_u16g(mk_ptr(t2 + (cur * 8u + pcp) * 2u, slot_hi));
-                ctx = cv & 0xffu; pcp = cv >> 8;
-                ssb = (uint32_t)(l8 >> sh) & 0xffu;
-                ph = mk_ptr(hi_tab + lit_index_hi(which, ctx, ssb & mhi) * 32u, slot_hi);
-                __syncwarp();
-                eh = load_elems<LPG>(ph, li); mh = ld_u16g(ph + 30);   // speculative on the last byte: inside the slot
-                cl = (ctx & o1) << 4; ib = (mm & ssb) | ((~mm & 0xffu) & ctx);
-                // -- low nibble: blend; then the rANS steps of both nibbles (state a before b: the order of the payload words)
-                blend_store_v2<LPG>(el_v, ml_v, l, pl, g, f);
-                rans_pair_v2<LPG>(k.a, k.b, eh_v, mh_v, h, el_v, ml_v, l, f);
-            }
-            done += m;
-            if (active) k.sym_count += 2 * m;
-        }
-        if (!active) return true;
-        // the bytes after the last aligned 8-byte store are still only in l8
-        if (g.store0) {
-            const uint32_t tail = min(ap & 7u, done);
-            for (uint32_t t = 0; t < tail; t++) dbase[done - tail + t] = (uint8_t)(l8 >> (8 * (8 - tail + t)));
-        }
-        // back to the lazy representation the state machine uses
-        if (f.wi >= f.wmax) { k.underflow = 1; f.wi = f.wmax - 1; }
-        k.p = f.wbase + f.wi; k.left = f.wmax - 1 - f.wi;
-        k.need_a = (k.sym_count >= NUM_SYMBOLS_BEFORE_FLUSH) ? 8u : 0u; k.need_b = 0;
-        s.cur = k; s.l8 = l8; s.lit_ctx = ctx; s.out_pos += done; s.lit_left -= done;
-        enter_lit_nibble<false, true, true>(s, nx);
-        return true;
+        if (small) return literal_plain_loop_v2<LPG, LPG == 16>(s, nx, g, active, t2s, n);
+        return literal_plain_loop_v2<LPG, false>(s, nx, g, active, t2s, n);
     }
 }
 
