@@ -200,8 +200,8 @@ def encode_options(**kw):
 
 
 class Engine:
-    """Batch engine bound to one GPU.  ``lanes_per_stream``: 0 = by batch size (16, or 8 where their residency holds the batch in fewer passes; never on an 80 GB H100, whose slot memory caps both), 16 / 8 = the round-2
-    engine with two / four streams per warp, 32 / 116 = the round-1 kernels (include/divans_b200.h)."""
+    """Batch engine bound to one GPU.  ``lanes_per_stream``: 0 = by batch size (16, or 8 where their residency holds the batch in fewer passes; never on an 80 GB H100, whose slot memory caps both), 16 / 8 = the v2
+    engine with two / four streams per warp; any other value means 16 (include/divans_b200.h)."""
 
     def __init__(self, device=0, max_resident=0, lanes_per_stream=0):
         self._L = load_library()

@@ -450,7 +450,13 @@ __device__ __forceinline__ bool literal_plain_loop_v2(St &s, Next &nx, const G2 
     const bool st_lane = g.store0 && active;
     Coder k = s.cur;
     if (!active) { k.p = reinterpret_cast<const uint32_t *>(s.slot + OFF_T2); k.left = 0; k.need_a = 0; k.need_b = 0; k.sym_count = 0; k.a = k.b = 1ull << 40; }
-    // ---- eager-refill coder (dv_core.cuh literal_fast): state a codes every high nibble, b every low nibble ----
+    // ---- EAGER-refill coder for the duration of the loop ----
+    // The reference refills a state right before it is used (ans.rs:428-442); the word order in the stream is the order in
+    // which states were produced, so refilling a state as soon as it drops below 2^31 consumes the same words.  The literal
+    // coder codes nibbles in pairs: state `a` serves every high nibble, `b` every low nibble (two rotations of
+    // ans.rs:240-243 are the identity), so the loop never swaps them.  Payload words are addressed by a saturating index:
+    // the demux kernel leaves >= 16 readable bytes after every coder's payload, so index n_words may be read once; an index
+    // that ends above n_words means underflow.
     f.wbase = k.p; f.wmax = k.left + 1; f.wi = 0;
     coder_fill(k);                                                        // pending refill / 16-byte (re)initialisation of `a`
     f.wi = (uint32_t)(k.p - f.wbase);

@@ -1,6 +1,6 @@
 // dv2_kernels.cu -- stream decoder of the v2 engine (dv2_core.cuh): persistent warps, every warp runs 32 / LPG streams in
 // lock step (LPG = 16: two, LPG = 8: four), work pulled from a global counter.  Same framing pre-pass (dv_kernels.cu) and
-// the same command state machine (dv_engine_kernel.cuh, transition<false, true>) as the round-1 decoders.
+// the same command state machine (dv_engine_kernel.cuh, transition<false, true>) as the blend decoder and the encoder.
 #include "dv2_core.cuh"
 
 namespace dv {

@@ -73,9 +73,9 @@ __device__ __forceinline__ int blend_update(const int c, const int k, const int 
     return (e & 0x7fff) | ((l16 < 9 && ((k2 >> l16) & 1)) ? 0x8000 : 0);
 }
 
-template <bool ENC, int LPS>
-__device__ __forceinline__ int nibble_core_blend(St &s, const Next &nx, const G2 g, const bool writer) {
-    static_assert(LPS == 16, "the blend model is instantiated for 16 lanes per stream");
+// one nibble of a 16-lane group, decoded (ENC = false) or encoded (ENC = true)
+template <bool ENC>
+__device__ __forceinline__ int nibble_core_blend(St &s, const Next &nx, const G2 g) {
     const int raw = nx.cdf[g.l16];
     const int c = raw & 0x7fff;
     const int k = (int)((__ballot_sync(FULL, raw < 0) >> g.shift) & 0x1ffu);
@@ -122,11 +122,11 @@ __device__ __forceinline__ int nibble_core_blend(St &s, const Next &nx, const G2
         if (mixg) {
             weights_update(w, (int)(short)(h_cm - l_cm - 1), (int)(short)(h_nb - l_nb - 1), freq);
             if (nx.mix_hi) s.c->w_hi = w; else s.c->w_lo = w;
-            if (writer) nx.cdf2[g.l16] = (int16_t)cm_new;
+            nx.cdf2[g.l16] = (int16_t)cm_new;
         }
     }
     const int nb_new = blend_update(c, k, sym, g.l16);
-    if (writer && nx.speed != SPK_NONE) nx.cdf[g.l16] = (int16_t)nb_new;   // SPK_NONE: the never-adapted default prior / a read-only stride prior
+    if (nx.speed != SPK_NONE) nx.cdf[g.l16] = (int16_t)nb_new;   // SPK_NONE: the never-adapted default prior / a read-only stride prior
     return sym;
 }
 

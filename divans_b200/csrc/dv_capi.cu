@@ -1,7 +1,7 @@
 // dv_capi.cu -- the C ABI of libdivans_b200.so: batch engine context + the reference's FFI surface as a drop-in.
 //
 // Host side only marshals: offsets/lengths tables, H2D/D2H copies, kernel launches.  All model/entropy work runs in
-// the sm_90a kernels (dv_kernels.cu); there is no CPU decode path in this library.
+// the sm_90a kernels (dv2_kernels.cu, dv_kernels.cu, dv_encode.cu); there is no CPU decode path in this library.
 #include <cuda_runtime.h>
 #include <stdarg.h>
 #include <stdio.h>
@@ -33,7 +33,6 @@ using namespace dv;
 struct divans_b200_ctx {
     int device = 0;
     int lanes_per_stream = 8;
-    uint32_t groups_per_block = 4;   // decode: lane-groups (streams) per block of the selected layout
     int sm_count = 0;
     uint32_t max_resident = 0;       // slots in the arena
     cudaStream_t stream = nullptr;
@@ -42,7 +41,6 @@ struct divans_b200_ctx {
     bool auto_lanes = false;         // lanes_per_stream 0: 16 lanes, or 8 where their residency holds the batch in fewer passes
     int last_lanes = 0;              // layout the most recent decode call used
     uint32_t cap16 = 0, cap8 = 0;    // resident streams of the two v2 layouts
-    int engine = 0;                  // 0: v2 (dv2_kernels.cu, lanes 16 or 8), 1: round-1 kernels (dv_kernels.cu, lanes 16 or 32)
     uint8_t *d_tables = nullptr;
     uint32_t *d_counter = nullptr;
     uint64_t *d_nibbles = nullptr;
@@ -105,11 +103,9 @@ extern "C" divans_b200_ctx *divans_b200_create(int device, uint32_t max_resident
     divans_b200_ctx *ctx = new (std::nothrow) divans_b200_ctx();
     if (!ctx) return nullptr;
     ctx->device = device;
-    // 16 (default, also 0): v2 engine, two streams per warp; 8: v2 engine, four streams per warp; 32: the round-1 kernel with one
-    // warp per stream; 116: the round-1 16-lane kernel (kept for A/B measurements)
-    ctx->engine = (lanes_per_stream == 32 || lanes_per_stream == 116) ? 1 : 0;
+    // 8: v2 engine, four streams per warp; anything else: v2 engine, two streams per warp (0: chosen per batch, see decode)
     ctx->auto_lanes = lanes_per_stream == 0;
-    ctx->lanes_per_stream = lanes_per_stream == 8 ? 8 : (lanes_per_stream == 32 ? 32 : 16);
+    ctx->lanes_per_stream = lanes_per_stream == 8 ? 8 : 16;
     cudaDeviceProp prop;
     if (!ck(ctx, cudaSetDevice(device), "cudaSetDevice") || !ck(ctx, cudaGetDeviceProperties(&prop, device), "cudaGetDeviceProperties")) {
         fprintf(stderr, "divans_b200: no usable CUDA device %d -- this library has no CPU path\n", device);
@@ -130,10 +126,9 @@ extern "C" divans_b200_ctx *divans_b200_create(int device, uint32_t max_resident
               ck(ctx, cudaMalloc((void **)&ctx->d_nibbles, 64), "cudaMalloc(nibbles)") &&
               ck(ctx, cudaMemset(ctx->d_nibbles, 0, 64), "cudaMemset");
     if (!ok) { delete ctx; return nullptr; }
-    int per_sm = ctx->engine == 0 ? decode_max_blocks_per_sm_v2(ctx->lanes_per_stream) : ctx->lanes_per_stream == 16 ? decode_max_blocks_per_sm16() : decode_max_blocks_per_sm32();
+    int per_sm = decode_max_blocks_per_sm_v2(ctx->lanes_per_stream);
     if (per_sm < 1) per_sm = 1;
-    uint32_t groups_per_block = ctx->engine == 0 ? (uint32_t)decode_groups_per_block_v2(ctx->lanes_per_stream) : DECODE_BLOCK_THREADS / ctx->lanes_per_stream;
-    ctx->groups_per_block = groups_per_block;
+    const uint32_t groups_per_block = (uint32_t)decode_groups_per_block_v2(ctx->lanes_per_stream);
     uint32_t auto_res = (uint32_t)ctx->sm_count * (uint32_t)per_sm * groups_per_block;
     size_t free_b = 0, total_b = 0;
     cudaMemGetInfo(&free_b, &total_b);
@@ -143,15 +138,13 @@ extern "C" divans_b200_ctx *divans_b200_create(int device, uint32_t max_resident
     if (auto_res > mem_cap) auto_res = mem_cap;
     ctx->max_resident = max_resident ? (max_resident < auto_res ? max_resident : auto_res) : auto_res;
     if (ctx->max_resident < groups_per_block) ctx->max_resident = groups_per_block;
-    if (ctx->engine == 0) {
-        auto cap = [&](int lanes) {
-            uint32_t c = (uint32_t)ctx->sm_count * (uint32_t)std::max(1, decode_max_blocks_per_sm_v2(lanes)) * (uint32_t)decode_groups_per_block_v2(lanes);
-            if (c > mem_cap) c = mem_cap;
-            if (max_resident && c > max_resident) c = max_resident;
-            return std::max(c, (uint32_t)decode_groups_per_block_v2(lanes));
-        };
-        ctx->cap16 = cap(16); ctx->cap8 = cap(8);
-    }
+    auto cap = [&](int lanes) {
+        uint32_t c = (uint32_t)ctx->sm_count * (uint32_t)std::max(1, decode_max_blocks_per_sm_v2(lanes)) * (uint32_t)decode_groups_per_block_v2(lanes);
+        if (c > mem_cap) c = mem_cap;
+        if (max_resident && c > max_resident) c = max_resident;
+        return std::max(c, (uint32_t)decode_groups_per_block_v2(lanes));
+    };
+    ctx->cap16 = cap(16); ctx->cap8 = cap(8);
     return ctx;
 }
 
@@ -239,13 +232,13 @@ static DivansResult decode_device_nolock(divans_b200_ctx *ctx, size_t n, const u
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream;
     if (ctx->busy_recorded) CK(cudaStreamWaitEvent(st, ctx->ev_busy, 0));
     int lanes = ctx->lanes_per_stream;
-    uint32_t gpb = ctx->groups_per_block, cap = ctx->max_resident;
-    const bool blend = (flags & DIVANS_B200_FLAG_CDF_BLEND) != 0;   // BlendCDF16 streams: the round-1 engine's generic path, 16 lanes
+    uint32_t gpb, cap;
+    const bool blend = (flags & DIVANS_B200_FLAG_CDF_BLEND) != 0;   // BlendCDF16 streams: the blend decoder (dv_kernels.cu), 16 lanes
     if (blend) {
         lanes = 16; gpb = (uint32_t)(DECODE_BLOCK_THREADS / 16);
         cap = (uint32_t)ctx->sm_count * (uint32_t)std::max(1, decode_max_blocks_per_sm16_blend()) * gpb;
         if (cap > ctx->max_resident) cap = std::max(ctx->max_resident / gpb * gpb, gpb);   // (memory / caller limits of the context)
-    } else if (ctx->engine == 0) {
+    } else {
         // 16 lanes per stream unless 8 hold the batch in fewer passes.  At equal residency 8 lanes is the slower layout (half the
         // warps per scheduler); it only pays where registers, not slot memory, cap residency: there it keeps twice the streams in
         // flight.  On an 80 GB H100 both layouts are capped by slot memory (cap8 ~ cap16), so 16 lanes run every batch size.
@@ -276,7 +269,7 @@ static DivansResult decode_device_nolock(divans_b200_ctx *ctx, size_t n, const u
     launch_frame(fp, ctx->d_payload, (uint64_t)ctx->payload_cap, st);
     if (dbg) { CK(cudaStreamSynchronize(st)); fprintf(stderr, "divans_b200[debug]: frame kernel ok (n=%zu)\n", n); }
     CK(cudaEventRecord(ctx->evm, st));
-    if (!skip_decode) { if (blend) launch_decode16_blend(dp, blocks, st); else if (ctx->engine == 0) launch_decode_v2(lanes, dp, blocks, st); else if (ctx->lanes_per_stream == 16) launch_decode16(dp, blocks, st); else launch_decode32(dp, blocks, st); }
+    if (!skip_decode) { if (blend) launch_decode16_blend(dp, blocks, st); else launch_decode_v2(lanes, dp, blocks, st); }
     if (dbg) { CK(cudaStreamSynchronize(st)); fprintf(stderr, "divans_b200[debug]: decode kernel ok (blocks=%u, lps=%d)\n", blocks, ctx->lanes_per_stream); }
     CK(cudaEventRecord(ctx->ev1, st));
     CK(cudaEventRecord(ctx->ev_busy, st)); ctx->busy_recorded = true;

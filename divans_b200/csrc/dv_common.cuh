@@ -8,7 +8,7 @@
 //
 // A CDF is 16 x int16 = 32 B = one DRAM sector; lane i of a 16-lane group owns element i.
 // The in-memory order of priors is NOT on the wire (reference: src/priors.rs:211-237 only fixes the index rule),
-// so the round-1 engines lay the literal tables out [which][index_c][index_b]: one (which, index_c) "slab" is 256
+// so the encoder and the blend decoder lay the literal tables out [which][index_c][index_b]: one (which, index_c) "slab" is 256
 // consecutive CDFs (8 KiB) and is default-initialised lazily by the kernel the first time the stream's context map /
 // mixing mask makes it reachable -- no 12.6 MB memset per stream (the reference default-initialises all of it,
 // codec/interface.rs:728-729).  The v2 engine orders each which-block by lit_index_hi / lit_index_lo (below).
@@ -56,7 +56,7 @@ static_assert(OFF_SLOT_END <= SLOT_STRIDE, "slot layout exceeds the slot stride"
 //     index_c = prev & 63 = index_b & 63: all 256 high priors of a stream are row 0, one contiguous 8 KiB run;
 //   low nibble: row index_c (the high nibble, plus the context's low bits for mixing value 1), column index_b: for text the
 //     hot rows (high nibble 2, 6, 7) hold runs of adjacent previous bytes.
-// The round-1 engines and the encoder keep [which][index_c][index_b] (dv_core.cuh, enter_lit_nibble<..., false>).
+// The encoder and the blend decoder keep [which][index_c][index_b] (dv_engine_kernel.cuh, enter_lit_nibble<..., false>).
 __host__ __device__ __forceinline__ uint32_t lit_index_hi(uint32_t which, uint32_t index_c, uint32_t index_b) {
     (void)which;
     return (((index_c - (index_b & 63u)) & 255u) << 8) + index_b;

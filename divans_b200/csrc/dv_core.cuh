@@ -1,5 +1,5 @@
-// dv_core.cuh -- the converged per-nibble core and the literal fast path shared by the stream decoder (dv_kernels.cu)
-// and the encoder's model pass (dv_encode.cu).
+// dv_core.cuh -- the encoder's converged per-nibble core and literal fast path (dv_encode.cu), and the warp CRC32C of the
+// framing and mux passes.  Included by the blend decoder (dv_kernels.cu) for the engine and the blend core.
 #pragma once
 #include "dv_engine_kernel.cuh"
 #include "dv_blend.cuh"
@@ -22,32 +22,23 @@ __device__ __forceinline__ void enc_log(St &s, const G2 g, int start, int freq) 
     s.cur.left++;
 }
 
-// The converged nibble core.  Every lane of the warp executes it every iteration, unpredicated: a group without work
-// codes against its slot's dummy CDF with a parked coder (no memory side effects that matter).
-template <bool ENC, int LPS>
-__device__ __forceinline__ int nibble_core(St &s, const Next &nx, const G2 g, const bool writer) {
-    const Grp gg = {FULL, g.shift, g.l16, writer, false, g.store0};
+// The encoder's converged nibble core.  Every lane of the warp executes it every iteration, unpredicated: a group without
+// work codes against its slot's dummy CDF with a parked coder (no memory side effects that matter).
+__device__ __forceinline__ int nibble_core_enc(St &s, const Next &nx, const G2 g) {
+    const Grp gg = {FULL, g.l16};
     const int c = nx.cdf[g.l16], maxv = nx.cdf[15];
     const int inc = (int)(short)(nx.speed & 0xffff), lim = nx.speed >> 16;
-    int sym, start, freq;
+    const int sym = nx.sym;
+    int start, freq;
     if (!__any_sync(FULL, nx.cdf2 != nullptr)) {
-        if (!ENC) {
-            coder_fill(s.cur);
-            int off = (int)(s.cur.a & 0x7fff);
-            int r = (int)(short)((off * maxv) >> 15);                       // probability/interface.rs:140
-            bool pred = (g.l16 == 15) || (r < c);
-            unsigned bal = __ballot_sync(FULL, pred);
-            sym = __ffs((bal >> g.shift) & 0xffffu) - 1;
-        } else sym = nx.sym;
         int cum = cdf_div(c, maxv);
         int hi = __shfl_sync(FULL, cum, sym, 16);
         int lo = __shfl_sync(FULL, cum, (sym - 1) & 15, 16);
         if (sym == 0) lo = 0;
         start = (int)(short)(lo + 1); freq = (int)(short)(hi - lo - 1);   // "major hax", probability/interface.rs:103-104
-        if (!ENC) coder_advance(s.cur, start, freq);
-        else enc_log(s, g, start, freq);
+        enc_log(s, g, start, freq);
         int c2 = cdf_blend(gg, c, maxv, sym, inc, lim);
-        if (writer) nx.cdf[g.l16] = (int16_t)c2;
+        nx.cdf[g.l16] = (int16_t)c2;
         return sym;
     }
     // ---- at least one group mixes two priors (dynamic context mixing >= 2, codec/literal.rs:219-243) ----
@@ -63,14 +54,6 @@ __device__ __forceinline__ int nibble_core(St &s, const Next &nx, const G2 g, co
     int ca = (int)(short)((int)((unsigned)rs * (unsigned)mixr + (unsigned)ro * (unsigned)inv + 1u) >> 15);   // frequentist_cdf.rs:58-72
     int ma = __shfl_sync(FULL, ca, 15, 16);
     int cu = mixg ? ca : c, mu = mixg ? ma : maxv;
-    if (!ENC) {
-        coder_fill(s.cur);
-        int off = (int)(s.cur.a & 0x7fff);
-        int r = (int)(short)((off * mu) >> 15);
-        bool pred = (g.l16 == 15) || (r < cu);
-        unsigned bal = __ballot_sync(FULL, pred);
-        sym = __ffs((bal >> g.shift) & 0xffffu) - 1;
-    } else sym = nx.sym;
     int cum = cdf_div(cu, mu);
     int hi = __shfl_sync(FULL, cum, sym, 16);
     int lo = __shfl_sync(FULL, cum, (sym - 1) & 15, 16);
@@ -78,17 +61,16 @@ __device__ __forceinline__ int nibble_core(St &s, const Next &nx, const G2 g, co
     start = (int)(short)(lo + 1); freq = (int)(short)(hi - lo - 1);
     int f_cm = cdf_freq(gg, cc, mc, sym);
     int f_nb = cdf_freq(gg, c, maxv, sym);
-    if (!ENC) coder_advance(s.cur, start, freq);
-    else enc_log(s, g, start, freq);
+    enc_log(s, g, start, freq);
     if (mixg) {
         weights_update(w, f_cm, f_nb, freq);
         if (nx.mix_hi) s.c->w_hi = w; else s.c->w_lo = w;
         const int sp = nx.mix_hi ? s.c->ad_cm_hi : s.c->ad_cm_lo;
         int c2 = cdf_blend(gg, cc, mc, sym, (int)(short)(sp & 0xffff), sp >> 16);
-        if (writer) nx.cdf2[g.l16] = (int16_t)c2;
+        nx.cdf2[g.l16] = (int16_t)c2;
     }
     int s2 = cdf_blend(gg, c, maxv, sym, inc, lim);
-    if (writer) nx.cdf[g.l16] = (int16_t)s2;
+    nx.cdf[g.l16] = (int16_t)s2;
     return sym;
 }
 
@@ -148,8 +130,7 @@ __device__ __forceinline__ MixVals mix_load(const G2 g, const char *nb, const ch
     MixVals v; v.c = ld_s16(nb + 2 * g.l16); v.maxv = ld_s16(nb + 30); v.cc = ld_s16(cm + 2 * g.l16); v.mc = ld_s16(cm + 30); return v;
 }
 struct MixSym { int sym, ca, ma; };
-template <bool ENC>
-__device__ __forceinline__ MixSym mix_search(const uint64_t st, const G2 g, const MixVals v, const Weights &w, const int sym_in) {
+__device__ __forceinline__ MixSym mix_search(const MixVals v, const Weights &w, const int sym) {
     const int prod = v.mc * v.maxv;
     int lz = prod == 0 ? 32 : __clz(prod); if (lz > 17) lz = 17;
     const int shift = 17 - lz;
@@ -158,16 +139,10 @@ __device__ __forceinline__ MixSym mix_search(const uint64_t st, const G2 g, cons
     MixSym r;
     r.ca = (int)(short)((int)((unsigned)rs * (unsigned)mixr + (unsigned)ro * (unsigned)inv + 1u) >> 15);   // frequentist_cdf.rs:58-72
     r.ma = __shfl_sync(FULL, r.ca, 15, 16);
-    if (!ENC) {
-        const int q = (int)(short)(((int)((uint32_t)st & 0x7fffu) * r.ma) >> 15);
-        const bool pred = (g.l16 == 15) || (q < r.ca);
-        r.sym = __ffs(__ballot_sync(FULL, pred) >> g.shift) - 1;
-    } else r.sym = sym_in;
+    r.sym = sym;
     return r;
 }
-template <bool ENC>
-__device__ __forceinline__ void mix_finish(Coder &k, uint64_t &st, const uint32_t *const wbase, uint32_t &wi, const uint32_t wmax,
-                                           const G2 g, const bool writer, char *nb, char *cm, const MixVals v, const MixSym ms, Weights &w,
+__device__ __forceinline__ void mix_finish(Coder &k, const G2 g, char *nb, char *cm, const MixVals v, const MixSym ms, Weights &w,
                                            const int nb_inc, const int nb_lim, const int cm_inc, const int cm_lim, bool &refused) {
     const int sym = ms.sym;
     // cumulative values of the three CDFs at sym and sym-1: two registers, four shuffles
@@ -180,31 +155,23 @@ __device__ __forceinline__ void mix_finish(Coder &k, uint64_t &st, const uint32_
     const int start = (int)(short)(lo_a + 1), freq = (int)(short)(hi_a - lo_a - 1);
     const int f_cm = (int)(short)((hi_pn & 0xffff) - (lo_pn & 0xffff) - 1);
     const int f_nb = (int)(short)(((unsigned)hi_pn >> 16) - ((unsigned)lo_pn >> 16) - 1);
-    if (!ENC) {   // eager refill, see literal_fast
-        const uint32_t t = ((uint32_t)st & 0x7fffu) - (uint32_t)start;
-        uint64_t x = (uint64_t)(int64_t)freq * (st >> 15) + (uint64_t)(int64_t)(int32_t)t;   // ans.rs:230-244 (t < 0: see rans_advance_v2)
-        if (x < (1ull << 31)) { x = (x << 32) | (uint64_t)wbase[wi]; wi = min(wi + 1, wmax); }
-        st = x;
-    } else {   // small speeds keep both priors' steps >= 3, but their average can still round to a step of 1: freq 0 (see enc_log)
-        refused |= freq <= 0;
-        if (g.store0) const_cast<uint32_t *>(k.p)[k.left] = ((uint32_t)start & 0xffffu) | ((uint32_t)freq << 16);
-        k.left++;
-    }
+    // small speeds keep both priors' steps >= 3, but their average can still round to a step of 1: freq 0 (see enc_log)
+    refused |= freq <= 0;
+    if (g.store0) const_cast<uint32_t *>(k.p)[k.left] = ((uint32_t)start & 0xffffu) | ((uint32_t)freq << 16);
+    k.left++;
     weights_update32(w, f_cm, f_nb, freq);
-    const Grp gg = {FULL, g.shift, g.l16, writer, false, g.store0};
+    const Grp gg = {FULL, g.l16};
     const int c2 = cdf_blend(gg, v.cc, v.mc, sym, cm_inc, cm_lim);
     const int s2 = cdf_blend(gg, v.c, v.maxv, sym, nb_inc, nb_lim);
-    if (writer) { *reinterpret_cast<int16_t *>(cm + 2 * g.l16) = (int16_t)c2; *reinterpret_cast<int16_t *>(nb + 2 * g.l16) = (int16_t)s2; }
+    *reinterpret_cast<int16_t *>(cm + 2 * g.l16) = (int16_t)c2; *reinterpret_cast<int16_t *>(nb + 2 * g.l16) = (int16_t)s2;
 }
 
-// Converged literal fast path: when both groups of the warp sit at the start of a literal byte, run whole bytes
-// (high nibble, low nibble, context of the next byte) back to back without going through the state-machine dispatch.
+// The encoder's converged literal fast path: when both groups of the warp sit at the start of a literal byte, code whole
+// bytes (high nibble, low nibble, context of the next byte) back to back without going through the state-machine dispatch.
 // This is code_nibble_array (codec/literal.rs:261-394) for two streams at once.  The common case -- no dynamic context
 // mixing and one mixing-mask value for the whole map -- gets a loop with every selector hoisted out.
-template <bool ENC, int LPS>
-__device__ __forceinline__ void literal_fast(St &s, Next &nx, const G2 g, const bool writer) {
-    uint32_t n = s.lit_left;
-    if (LPS == 16) n = min(n, __shfl_xor_sync(FULL, n, 16));
+__device__ __forceinline__ void literal_fast_enc(St &s, Next &nx, const G2 g) {
+    const uint32_t n = min(s.lit_left, __shfl_xor_sync(FULL, s.lit_left, 16));
     const bool simple = __all_sync(FULL, !s.mixing_trait && s.lit_cfg >= 0 && s.speeds_small);
     if (simple) {
         const int cfg = s.lit_cfg;
@@ -218,41 +185,16 @@ __device__ __forceinline__ void literal_fast(St &s, Next &nx, const G2 g, const 
         const uint8_t *const lcm = A_lcm(s) + (s.btype_last << 6);
         const uint8_t *const lut = s.tables + TB_CTX + 512 * s.pred_mode;
         const uint32_t pm = s.pred_mode;
-        const uint8_t *src = ENC ? s.c->in.lits + s.c->e0 + (s.c->e1 - s.lit_left) : nullptr;
+        const uint8_t *src = s.c->in.lits + s.c->e0 + (s.c->e1 - s.lit_left);
         unsigned long long l8 = s.l8;
         uint32_t ctx = s.lit_ctx;
         uint8_t *dst = s.out + s.out_pos;
         Coder k = s.cur;
         const uint32_t src_last = s.lit_left - 1;                   // (lit_left >= 1 here)
         const uint32_t pm_shift = pm == 1 ? 2u : 0u;
-        // ---- decoder: switch the coder to EAGER refill for the duration of the loop ----
-        // The reference refills a state right before it is used (ans.rs:428-442); the word order in the stream is the
-        // order in which states were produced, so refilling a state as soon as it drops below 2^31 consumes the same
-        // words.  The literal coder codes nibbles in pairs: state `a` serves every high nibble, `b` every low nibble
-        // (two rotations of ans.rs:240-243 are the identity), so the loop never swaps them.
-        // Payload words are addressed by a saturating index: the demux kernel leaves >= 16 readable bytes after every
-        // coder's payload, so index n_words may be read once; an index that ends above n_words means underflow.
-        const uint32_t *const wbase = k.p;
-        const uint32_t wmax = k.left + 1;
-        uint32_t wi = 0;
-        if (!ENC) {
-            coder_fill(k);                                        // pending refill / 16-byte (re)initialisation of `a`
-            wi = (uint32_t)(k.p - wbase);
-            if (k.need_b) { k.b = (k.b << 32) | (uint64_t)wbase[wi]; wi = min(wi + 1, wmax); k.need_b = 0; }
-        }
         uint32_t done = 0;
         while (done < n) {
             uint32_t m = n - done;
-            if (!ENC) {
-                if (k.sym_count >= NUM_SYMBOLS_BEFORE_FLUSH) {   // chunk restart, ans.rs:173-189
-                    if (wi + 5 <= wmax) { k.a = (uint64_t)wbase[wi] | ((uint64_t)wbase[wi + 1] << 32); k.b = (uint64_t)wbase[wi + 2] | ((uint64_t)wbase[wi + 3] << 32); wi += 4; }
-                    else { k.a = k.b = 0; wi = wmax; }
-                    k.sym_count = 0;
-                }
-                m = min(m, (NUM_SYMBOLS_BEFORE_FLUSH - k.sym_count) >> 1);
-                if (LPS == 16) m = min(m, __shfl_xor_sync(FULL, m, 16));
-                if (m == 0) break;   // unreachable: the literal coder codes nibbles in pairs, sym_count stays even
-            }
             // Software pipeline (the loads of the NEXT prior are issued before the bookkeeping of the CURRENT nibble):
             //   search(hi) -> load(lo) -> finish(hi) -> search(lo) -> context -> load(next hi) -> finish(lo)
             // The high and low tables never alias, so the early loads cannot overtake a store to the same CDF; the
@@ -262,17 +204,13 @@ __device__ __forceinline__ void literal_fast(St &s, Next &nx, const G2 g, const 
             char *ph = hi_tab + (ctx * 256u + ((uint32_t)(l8 >> sh) & mm & (~o1 & 0xffu))) * scale;
             __syncwarp();
             int ch = ld_s16(ph + 2 * g.l16), mh = ld_s16(ph + 30);
-            uint32_t nxt_in = ENC ? src[done] : 0u;                   // encoder: the input byte is fetched one iteration ahead
+            uint32_t nxt_in = src[done];                              // the input byte is fetched one iteration ahead
             for (uint32_t i = 0; i < m; i++) {
                 const uint32_t ssb = (uint32_t)(l8 >> sh) & 0xffu;
                 const uint32_t byte_in = nxt_in;
-                if (ENC) nxt_in = src[min(done + i + 1, src_last)];
-                // -- high nibble: search
-                int h;
-                if (!ENC) {
-                    const int rr = ((int)((uint32_t)k.a & 0x7fffu) * mh) >> 15;                    // probability/interface.rs:140
-                    h = __ffs(__ballot_sync(FULL, (g.l16 == 15) || (rr < ch)) >> g.shift) - 1;   // bit 15 of the group is always set
-                } else h = (int)(byte_in >> 4);
+                nxt_in = src[min(done + i + 1, src_last)];
+                // -- high nibble
+                const int h = (int)(byte_in >> 4);
                 const uint32_t ib = (mm & ssb) | ((~mm & 0xffu) & ctx), ic = ((uint32_t)h & fc) | ((ctx & o1) << 4);
                 char *const pl = lo_tab + (ic * 256u + ib) * scale;
                 __syncwarp();
@@ -284,22 +222,14 @@ __device__ __forceinline__ void literal_fast(St &s, Next &nx, const G2 g, const 
                     int lo = __shfl_sync(FULL, cum, (h - 1) & 15, 16);
                     if (h == 0) lo = 0;
                     const uint32_t start = (uint32_t)(lo + 1), freq = (uint32_t)(hi - lo - 1);   // "major hax", probability/interface.rs:103-104
-                    if (!ENC) {
-                        const uint32_t t = ((uint32_t)k.a & 0x7fffu) - start;                      // 0 <= t < freq (the search put the offset in this bin)
-                        uint64_t x = (uint64_t)freq * (k.a >> 15) + (uint64_t)(int64_t)(int32_t)t;  // ans.rs:230-244 (t < 0: see rans_advance_v2)
-                        if (x < (1ull << 31)) { x = (x << 32) | (uint64_t)wbase[wi]; wi = min(wi + 1, wmax); }
-                        k.a = x;
-                    } else { if (g.store0) const_cast<uint32_t *>(k.p)[k.left] = (start & 0xffffu) | (freq << 16); k.left++; }
+                    if (g.store0) const_cast<uint32_t *>(k.p)[k.left] = (start & 0xffffu) | (freq << 16);
+                    k.left++;
                     int c2 = ch + ((g.l16 >= h) ? inc : 0);
                     if (mh + inc >= lim) { const int t = c2 + g.l16 + 1; c2 = t - (t >> 2); }
-                    if (writer) *reinterpret_cast<int16_t *>(ph + 2 * g.l16) = (int16_t)c2;
+                    *reinterpret_cast<int16_t *>(ph + 2 * g.l16) = (int16_t)c2;
                 }
-                // -- low nibble: search
-                int l;
-                if (!ENC) {
-                    const int rr = ((int)((uint32_t)k.b & 0x7fffu) * ml) >> 15;
-                    l = __ffs(__ballot_sync(FULL, (g.l16 == 15) || (rr < cl)) >> g.shift) - 1;
-                } else l = (int)(byte_in & 0xf);
+                // -- low nibble
+                const int l = (int)(byte_in & 0xf);
                 const uint32_t cur = ((uint32_t)l | ((uint32_t)h << 4)) & 0xff;
                 l8 = (l8 >> 8) | ((unsigned long long)cur << 56);   // push_literal_byte, codec/interface.rs:280-284
                 if (g.store0) dst[done + i] = (uint8_t)cur;
@@ -316,27 +246,17 @@ __device__ __forceinline__ void literal_fast(St &s, Next &nx, const G2 g, const 
                     int lo = __shfl_sync(FULL, cum, (l - 1) & 15, 16);
                     if (l == 0) lo = 0;
                     const uint32_t start = (uint32_t)(lo + 1), freq = (uint32_t)(hi - lo - 1);
-                    if (!ENC) {
-                        const uint32_t t = ((uint32_t)k.b & 0x7fffu) - start;
-                        uint64_t x = (uint64_t)freq * (k.b >> 15) + (uint64_t)(int64_t)(int32_t)t;
-                        if (x < (1ull << 31)) { x = (x << 32) | (uint64_t)wbase[wi]; wi = min(wi + 1, wmax); }
-                        k.b = x;
-                    } else { if (g.store0) const_cast<uint32_t *>(k.p)[k.left] = (start & 0xffffu) | (freq << 16); k.left++; }
+                    if (g.store0) const_cast<uint32_t *>(k.p)[k.left] = (start & 0xffffu) | (freq << 16);
+                    k.left++;
                     int c2 = cl + ((g.l16 >= l) ? inc : 0);
                     if (ml + inc >= lim) { const int t = c2 + g.l16 + 1; c2 = t - (t >> 2); }
-                    if (writer) *reinterpret_cast<int16_t *>(pl + 2 * g.l16) = (int16_t)c2;
+                    *reinterpret_cast<int16_t *>(pl + 2 * g.l16) = (int16_t)c2;
                 }
             }
             done += m;
-            if (!ENC) k.sym_count += 2 * m;
-        }
-        if (!ENC) {   // back to the lazy representation the state machine uses
-            if (wi >= wmax) { k.underflow = 1; wi = wmax - 1; }
-            k.p = wbase + wi; k.left = wmax - 1 - wi;
-            k.need_a = (k.sym_count >= NUM_SYMBOLS_BEFORE_FLUSH) ? 8u : 0u; k.need_b = 0;
         }
         s.cur = k; s.l8 = l8; s.lit_ctx = ctx; s.out_pos += done; s.lit_left -= done;
-        enter_lit_nibble<ENC, true>(s, nx);
+        enter_lit_nibble<true, true>(s, nx);
         return;
     }
     if (__all_sync(FULL, s.mixing_trait && s.lit_cfg >= 0 && s.speeds_small)) {
@@ -355,34 +275,16 @@ __device__ __forceinline__ void literal_fast(St &s, Next &nx, const G2 g, const 
         const uint8_t *const lcm = A_lcm(s) + (s.btype_last << 6);
         const uint8_t *const lut = s.tables + TB_CTX + 512 * s.pred_mode;
         const uint32_t pm = s.pred_mode;
-        const uint8_t *src = ENC ? s.c->in.lits + s.c->e0 + (s.c->e1 - s.lit_left) : nullptr;
+        const uint8_t *src = s.c->in.lits + s.c->e0 + (s.c->e1 - s.lit_left);
         unsigned long long l8 = s.l8;
         uint32_t ctx = s.lit_ctx;
         uint8_t *dst = s.out + s.out_pos;
         Coder k = s.cur;
         Weights wh = s.c->w_hi, wl = s.c->w_lo;
         bool refused = false;
-        const uint32_t *const wbase = k.p;
-        const uint32_t wmax = k.left + 1;
-        uint32_t wi = 0;
-        if (!ENC) {   // eager refill for the duration of the loop (see the plain loop above)
-            coder_fill(k);
-            wi = (uint32_t)(k.p - wbase);
-            if (k.need_b) { k.b = (k.b << 32) | (uint64_t)wbase[wi]; wi = min(wi + 1, wmax); k.need_b = 0; }
-        }
         uint32_t done = 0;
         while (done < n) {
             uint32_t m = n - done;
-            if (!ENC) {
-                if (k.sym_count >= NUM_SYMBOLS_BEFORE_FLUSH) {   // chunk restart, ans.rs:173-189
-                    if (wi + 5 <= wmax) { k.a = (uint64_t)wbase[wi] | ((uint64_t)wbase[wi + 1] << 32); k.b = (uint64_t)wbase[wi + 2] | ((uint64_t)wbase[wi + 3] << 32); wi += 4; }
-                    else { k.a = k.b = 0; wi = wmax; }
-                    k.sym_count = 0;
-                }
-                m = min(m, (NUM_SYMBOLS_BEFORE_FLUSH - k.sym_count) >> 1);
-                if (LPS == 16) m = min(m, __shfl_xor_sync(FULL, m, 16));
-                if (m == 0) break;
-            }
             // search(hi) -> load(lo) -> finish(hi) -> search(lo) -> context -> load(next hi) -> finish(lo); the stride tables
             // of the two nibbles are distinct and so are their context-map regions (FirstNibble / SecondNibble), so an
             // early load never overtakes a store to the same CDF
@@ -391,15 +293,15 @@ __device__ __forceinline__ void literal_fast(St &s, Next &nx, const G2 g, const 
             MixVals vh = mix_load(g, nbh, cmh);
             for (uint32_t i = 0; i < m; i++) {
                 const uint32_t ssb = (uint32_t)(l8 >> sh) & 0xffu;
-                const uint32_t byte_in = ENC ? src[done + i] : 0u;
-                const MixSym sh_ = mix_search<ENC>(k.a, g, vh, wh, (int)(byte_in >> 4));
+                const uint32_t byte_in = src[done + i];
+                const MixSym sh_ = mix_search(vh, wh, (int)(byte_in >> 4));
                 const uint32_t h = (uint32_t)sh_.sym;
                 const uint32_t ib = (mm & ssb) | ((~mm & 0xffu) & ctx), ic = (h & fc) | ((ctx & o1) << 4);
                 char *const nbl = lo_tab + (ic * 256u + ib) * 32u, *const cml = cmb + (256u + h + 16u * ctx) * 32u;
                 __syncwarp();
                 const MixVals vl = mix_load(g, nbl, cml);
-                mix_finish<ENC>(k, k.a, wbase, wi, wmax, g, writer, nbh, cmh, vh, sh_, wh, inc, lim, ch_inc, ch_lim, refused);
-                const MixSym sl_ = mix_search<ENC>(k.b, g, vl, wl, (int)(byte_in & 0xf));
+                mix_finish(k, g, nbh, cmh, vh, sh_, wh, inc, lim, ch_inc, ch_lim, refused);
+                const MixSym sl_ = mix_search(vl, wl, (int)(byte_in & 0xf));
                 const uint32_t cur = ((uint32_t)sl_.sym | (h << 4)) & 0xff;
                 l8 = (l8 >> 8) | ((unsigned long long)cur << 56);
                 if (g.store0) dst[done + i] = (uint8_t)cur;
@@ -409,44 +311,38 @@ __device__ __forceinline__ void literal_fast(St &s, Next &nx, const G2 g, const 
                 nbh = hi_tab + (ctx * 256u + ((uint32_t)(l8 >> sh) & mm & (~o1 & 0xffu))) * 32u; cmh = cmb + ctx * 32u;
                 __syncwarp();
                 vh = mix_load(g, nbh, cmh);   // speculative on the last byte: initialised slabs
-                mix_finish<ENC>(k, k.b, wbase, wi, wmax, g, writer, nbl, cml, vl, sl_, wl, inc, lim, cl_inc, cl_lim, refused);
+                mix_finish(k, g, nbl, cml, vl, sl_, wl, inc, lim, cl_inc, cl_lim, refused);
             }
             done += m;
-            if (!ENC) k.sym_count += 2 * m;
-        }
-        if (!ENC) {
-            if (wi >= wmax) { k.underflow = 1; wi = wmax - 1; }
-            k.p = wbase + wi; k.left = wmax - 1 - wi;
-            k.need_a = (k.sym_count >= NUM_SYMBOLS_BEFORE_FLUSH) ? 8u : 0u; k.need_b = 0;
         }
         s.cur = k; s.l8 = l8; s.lit_ctx = ctx; s.out_pos += done; s.lit_left -= done;
         s.c->w_hi = wh; s.c->w_lo = wl;
-        if (ENC && refused) s.status = ST_FAIL;
-        enter_lit_nibble<ENC, true>(s, nx);
+        if (refused) s.status = ST_FAIL;
+        enter_lit_nibble<true, true>(s, nx);
         return;
     }
     for (uint32_t i = 0; i < n; i++) {
         __syncwarp();
-        int h = nibble_core<ENC, LPS>(s, nx, g, writer);
+        int h = nibble_core_enc(s, nx, g);
         s.lit_h = (uint32_t)h;
-        enter_lit_nibble<ENC, false>(s, nx);
+        enter_lit_nibble<true, false>(s, nx);
         __syncwarp();
-        int l = nibble_core<ENC, LPS>(s, nx, g, writer);
+        int l = nibble_core_enc(s, nx, g);
         uint32_t cur = ((uint32_t)l | ((uint32_t)h << 4)) & 0xff;
         s.l8 = (s.l8 >> 8) | ((unsigned long long)cur << 56);   // push_literal_byte, codec/interface.rs:280-284
         if (g.store0) s.out[s.out_pos] = (uint8_t)cur;
         s.out_pos++;
         s.lit_left--;
         lit_context(s);
-        enter_lit_nibble<ENC, true>(s, nx);
+        enter_lit_nibble<true, true>(s, nx);
     }
 }
 
-// the nibble core of the kernel's probability model
-template <bool ENC, int LPS, bool BLEND>
-__device__ __forceinline__ int core_dispatch(St &s, const Next &nx, const G2 g, const bool writer) {
-    if constexpr (BLEND) return nibble_core_blend<ENC, LPS>(s, nx, g, writer);
-    else return nibble_core<ENC, LPS>(s, nx, g, writer);
+// the encoder's nibble core of the kernel's probability model
+template <bool BLEND>
+__device__ __forceinline__ int core_dispatch(St &s, const Next &nx, const G2 g) {
+    if constexpr (BLEND) return nibble_core_blend<true>(s, nx, g);
+    else return nibble_core_enc(s, nx, g);
 }
 
 }  // namespace dv

@@ -14,24 +14,20 @@
 
 namespace dv {
 
-template <int LPS, bool BLEND = false>
+template <bool BLEND>
 __global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) encode_model_kernel(EncodeParams p) {
     extern __shared__ __align__(16) uint8_t smem[];
     const int lane = threadIdx.x & 31;
-    const int warp_in_block = threadIdx.x >> 5;
-    constexpr int GPW = 32 / LPS;
-    const int group_in_warp = (LPS == 16) ? (lane >> 4) : 0;
-    const int group_in_block = warp_in_block * GPW + group_in_warp;
-    const uint32_t slot = blockIdx.x * (DECODE_BLOCK_THREADS / LPS) + group_in_block;
+    const int group_in_block = (threadIdx.x >> 5) * 2 + (lane >> 4);
+    const uint32_t slot = blockIdx.x * (DECODE_BLOCK_THREADS / 16) + group_in_block;
     G2 g;
     g.l16 = lane & 15;
-    g.shift = (LPS == 16) ? (lane & 16) : 0;
-    g.gmask = (LPS == 16) ? (0xffffu << (lane & 16)) : 0xffffffffu;
-    g.store0 = (LPS == 16) ? ((lane & 15) == 0) : (lane == 0);
+    g.shift = lane & 16;
+    g.gmask = 0xffffu << (lane & 16);
+    g.store0 = (lane & 15) == 0;
     g.nl = 16;
     g.grp = group_in_block;
     g.blend = BLEND;
-    const bool writer = (LPS == 16) ? true : (lane < 16);
 
     St s;
     s.slot = p.arena + (uint64_t)slot * SLOT_STRIDE;
@@ -58,7 +54,7 @@ __global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) encode_model_kernel(E
         if (__any_sync(FULL, want)) {
             uint32_t v = 0;
             if (want && g.store0) v = atomicAdd(p.work_counter, 1u);
-            v = __shfl_sync(FULL, v, 0, LPS);
+            v = __shfl_sync(FULL, v, 0, 16);
             if (want) {
                 if (v >= p.n_streams) exhausted = true;
                 else {
@@ -119,13 +115,13 @@ __global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) encode_model_kernel(E
             coder_init_enc(s.cur, dummy_log);
         };
         if (!BLEND && __all_sync(FULL, s.state == S_LIT_HI)) {
-            literal_fast<true, LPS>(s, nx, g, writer);
+            literal_fast_enc(s, nx, g);
             if (s.lit_left == 0 && s.status == ST_OK) { swap_coders(s, g); s.c->in.pos++; enter_cmd_type<true>(s, nx); }
             if (s.status != ST_OK) finish();   // a symbol the loop could not code (enc_log): the stream ends here
             continue;
         }
         const bool busy = s.state != S_IDLE;
-        int sym = core_dispatch<true, LPS, BLEND>(s, nx, g, writer);
+        int sym = core_dispatch<BLEND>(s, nx, g);
         if (!busy) s.cur.left = 0;
         else {
             if (s.status == ST_OK) {   // (else the core could not code the symbol: enc_log)
@@ -379,12 +375,12 @@ __global__ void __launch_bounds__(128) encode_mux_kernel(EncodeParams p) {
 #ifdef DV_BLEND
 void launch_encode_model_blend(const EncodeParams &p, uint32_t n_blocks, cudaStream_t st) {
     size_t smem = (size_t)(DECODE_BLOCK_THREADS / 16) * SMEM_BYTES_PER_GROUP;
-    encode_model_kernel<16, true><<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p);
+    encode_model_kernel<true><<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p);
 }
 #else
 void launch_encode_model(const EncodeParams &p, uint32_t n_blocks, cudaStream_t st) {
     size_t smem = (size_t)(DECODE_BLOCK_THREADS / 16) * SMEM_BYTES_PER_GROUP;
-    encode_model_kernel<16><<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p);
+    encode_model_kernel<false><<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p);
 }
 // M[f] = floor((2^64 - 1) / f), f = 1..32767 (entry 0 unused)
 __global__ void rcp15_init_kernel(uint64_t *tab) {
@@ -399,7 +395,7 @@ void launch_encode_flush_mux(const EncodeParams &p, cudaStream_t st) {
     encode_mux_kernel<<<(p.n_streams + 3) / 4, 128, 0, st>>>(p);
 }
 int encode_max_blocks_per_sm() {
-    const int nb = stream_kernel_blocks_per_sm(encode_model_kernel<16>, DECODE_BLOCK_THREADS, (size_t)(DECODE_BLOCK_THREADS / 16) * SMEM_BYTES_PER_GROUP);
+    const int nb = stream_kernel_blocks_per_sm(encode_model_kernel<false>, DECODE_BLOCK_THREADS, (size_t)(DECODE_BLOCK_THREADS / 16) * SMEM_BYTES_PER_GROUP);
     return nb;
 }
 

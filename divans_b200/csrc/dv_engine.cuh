@@ -141,7 +141,7 @@ __device__ __forceinline__ uint32_t BL(const St &s, int k, int j) { return (uint
 __device__ __forceinline__ uint32_t BMAX(const St &s, int k) { return (s.c->btype_max >> (8 * k)) & 0xffu; }
 
 struct G2 {            // lane geometry of one lane-group (16 lanes: one CDF element per lane; 8 lanes: two per lane)
-    int l16;           // lane index inside the group: lane & 15 (16/32 lanes per stream) or lane & 7 (8 lanes per stream)
+    int l16;           // lane index inside the group: lane & 15 (16 lanes per stream) or lane & 7 (8 lanes per stream)
     int shift;         // position of the group's ballot bits: 0 / 16, or 0 / 8 / 16 / 24
     unsigned gmask;    // this group's lanes
     bool store0;       // lane that performs the group's scalar stores
@@ -281,7 +281,7 @@ static __device__ __noinline__ void v2_clear_literal_tables(const G2 g, uint8_t 
 }
 // v2 engine: a stream whose speeds can wrap i16 counters needs all 16 bits of every element.  Priors of the current generation
 // lose their tag bits, every other prior becomes the default CDF, and every slab is marked initialised (the bitmaps the
-// round-1 engine uses).  From here on the stream's literal priors are plain i16 arrays.
+// [which][index_c][index_b] layout keeps, dv_common.cuh).  From here on the stream's literal priors are plain i16 arrays.
 static __device__ __noinline__ void v2_make_untagged(const G2 g, uint8_t *slot, uint32_t gen) {
     uint32_t *bitmaps = cold_of_group(g)->bitmaps;
     uint32_t *p = reinterpret_cast<uint32_t *>(slot + OFF_LIT_HI);

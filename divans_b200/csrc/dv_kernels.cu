@@ -1,4 +1,6 @@
-// dv_kernels.cu -- sm_90a kernels of the divANS batch engine: framing/CRC pre-pass and the stream decoder.
+// dv_kernels.cu -- sm_90a kernels of the divANS batch engine: the framing/CRC pre-pass every decode runs first, and the
+// stream decoder of the reference's feature="blend" probability model (dv_blend.cuh).  Frequentist streams decode on the
+// v2 engine (dv2_kernels.cu).
 #include "dv_core.cuh"
 
 namespace dv {
@@ -6,7 +8,6 @@ namespace dv {
 // ---------------------------------------------------------------------------------------------------------------
 // framing pre-pass: frame kernel (header, record walk, trailer, CRC32C -- one warp per stream), payload scan, demux.
 // ---------------------------------------------------------------------------------------------------------------
-#if DV_LPS == 32
 // frame kernel: one WARP per stream.  Lane 0 walks the 16-byte header and the mux record chain (mux.rs:384-444) to the
 // EOF marker and checks the trailer magic; the warp checks the CRC32C of header..EOF marker (codec/decoder.rs:186-213).
 __global__ void __launch_bounds__(128) frame_kernel(FrameParams p) {
@@ -141,31 +142,30 @@ __global__ void __launch_bounds__(128) demux_kernel(FrameParams p, uint8_t *payl
     }
 }
 
-
-#endif  // DV_LPS == 32 (frame kernel)
+void launch_frame(const FrameParams &p, uint8_t *payload, uint64_t payload_cap_bytes, cudaStream_t st) {
+    uint32_t blocks = (p.n_streams + 3) / 4;   // one warp per stream
+    frame_kernel<<<blocks, 128, 0, st>>>(p);
+    payload_scan_kernel<<<1, 1024, 0, st>>>(p.frame, p.n_streams, p.status, payload_cap_bytes / 16);
+    demux_kernel<<<(p.n_streams + 3) / 4, 128, 0, st>>>(p, payload);
+}
 
 // ---------------------------------------------------------------------------------------------------------------
-// stream kernel: persistent warps, two streams per warp in lock step (dv_engine.cuh), work pulled from a global counter.
-// LPS == 32 keeps the north-star "one warp owns one stream" layout: the upper half-warp mirrors the lower one.
+// blend stream decoder: persistent warps, two streams per warp in lock step (dv_engine.cuh), work pulled from a global
+// counter.  Every nibble goes through the blend core (nibble_core_blend): the model has no literal fast loop.
 // ---------------------------------------------------------------------------------------------------------------
-template <int LPS, bool BLEND = false>
-__global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) decode_kernel(DecodeParams p) {
+__global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) decode_kernel_blend(DecodeParams p) {
     extern __shared__ __align__(16) uint8_t smem[];
     const int lane = threadIdx.x & 31;
-    const int warp_in_block = threadIdx.x >> 5;
-    constexpr int GPW = 32 / LPS;
-    const int group_in_warp = (LPS == 16) ? (lane >> 4) : 0;
-    const int group_in_block = warp_in_block * GPW + group_in_warp;
-    const uint32_t slot = blockIdx.x * (DECODE_BLOCK_THREADS / LPS) + group_in_block;
+    const int group_in_block = (threadIdx.x >> 5) * 2 + (lane >> 4);
+    const uint32_t slot = blockIdx.x * (DECODE_BLOCK_THREADS / 16) + group_in_block;
     G2 g;
     g.l16 = lane & 15;
-    g.shift = (LPS == 16) ? (lane & 16) : 0;
-    g.gmask = (LPS == 16) ? (0xffffu << (lane & 16)) : 0xffffffffu;
-    g.store0 = (LPS == 16) ? ((lane & 15) == 0) : (lane == 0);
+    g.shift = lane & 16;
+    g.gmask = 0xffffu << (lane & 16);
+    g.store0 = (lane & 15) == 0;
     g.nl = 16;
     g.grp = group_in_block;
-    g.blend = BLEND;
-    const bool writer = (LPS == 16) ? true : (lane < 16);
+    g.blend = true;
 
     St s;
     s.slot = p.arena + (uint64_t)slot * SLOT_STRIDE;
@@ -190,7 +190,7 @@ __global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) decode_kernel(DecodeP
         if (__any_sync(FULL, want)) {
             uint32_t v = 0;
             if (want && g.store0) v = atomicAdd(p.work_counter, 1u);
-            v = __shfl_sync(FULL, v, 0, LPS);
+            v = __shfl_sync(FULL, v, 0, 16);
             if (want) {
                 if (v >= p.n_streams) exhausted = true;
                 else if (p.status[v] != ST_OK) { if (g.store0) p.out_len[v] = 0; }   // framing / CRC failure: stay idle, fetch again
@@ -214,20 +214,8 @@ __global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) decode_kernel(DecodeP
             __syncwarp();
         }
         // ---- one nibble per group ----
-        if (!BLEND && __all_sync(FULL, s.state == S_LIT_HI)) {   // (the fast loops are frequentist arithmetic)
-            literal_fast<false, LPS>(s, nx, g, writer);
-            if (s.cur.underflow) s.status = ST_NEED_INPUT;
-            if (s.lit_left == 0 && s.status == ST_OK) { swap_coders(s, g); enter_cmd_type<false>(s, nx); }
-            if (s.status != ST_OK) {
-                if (g.store0) { p.out_len[s.c->sidx] = s.out_pos; p.status[s.c->sidx] = s.status; }
-                s.state = S_IDLE; s.status = ST_OK;
-                nx.cdf = A_misc(s, MI_DUMMY); nx.cdf2 = nullptr; nx.speed = SPK_NONE; nx.tagged = false;
-                coder_init_dec(s.cur, nullptr, 0); s.cur.need_a = 0;
-            }
-            continue;
-        }
         const bool busy = s.state != S_IDLE;
-        int sym = core_dispatch<false, LPS, BLEND>(s, nx, g, writer);
+        int sym = nibble_core_blend<false>(s, nx, g);
         // ---- per-group scalar state machines (divergent) ----
         if (busy) {
             if (s.cur.underflow) s.status = ST_NEED_INPUT;
@@ -243,44 +231,12 @@ __global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) decode_kernel(DecodeP
     }
 }
 
-#if DV_LPS == 32
-void launch_frame(const FrameParams &p, uint8_t *payload, uint64_t payload_cap_bytes, cudaStream_t st) {
-    uint32_t blocks = (p.n_streams + 3) / 4;   // one warp per stream
-    frame_kernel<<<blocks, 128, 0, st>>>(p);
-    payload_scan_kernel<<<1, 1024, 0, st>>>(p.frame, p.n_streams, p.status, payload_cap_bytes / 16);
-    demux_kernel<<<(p.n_streams + 3) / 4, 128, 0, st>>>(p, payload);
-}
-#endif
-#ifndef DV_LPS
-#error "compile with -DDV_LPS=16 or 32 (one translation unit per instantiation keeps ptxas time in check)"
-#endif
-#if DV_LPS == 32
-void launch_decode32(const DecodeParams &p, uint32_t n_blocks, cudaStream_t st) {
-    size_t smem = (size_t)(DECODE_BLOCK_THREADS / 32) * SMEM_BYTES_PER_GROUP;
-    decode_kernel<32><<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p);
-}
-int decode_max_blocks_per_sm32() {
-    const int nb = stream_kernel_blocks_per_sm(decode_kernel<32>, DECODE_BLOCK_THREADS, (size_t)(DECODE_BLOCK_THREADS / 32) * SMEM_BYTES_PER_GROUP);
-    return nb;
-}
-#elif defined(DV_BLEND)
-// the reference's feature="blend" probability model (dv_blend.cuh): its own translation unit, 16 lanes per stream
 void launch_decode16_blend(const DecodeParams &p, uint32_t n_blocks, cudaStream_t st) {
     size_t smem = (size_t)(DECODE_BLOCK_THREADS / 16) * SMEM_BYTES_PER_GROUP;
-    decode_kernel<16, true><<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p);
+    decode_kernel_blend<<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p);
 }
 int decode_max_blocks_per_sm16_blend() {
-    return stream_kernel_blocks_per_sm(decode_kernel<16, true>, DECODE_BLOCK_THREADS, (size_t)(DECODE_BLOCK_THREADS / 16) * SMEM_BYTES_PER_GROUP);
+    return stream_kernel_blocks_per_sm(decode_kernel_blend, DECODE_BLOCK_THREADS, (size_t)(DECODE_BLOCK_THREADS / 16) * SMEM_BYTES_PER_GROUP);
 }
-#else
-void launch_decode16(const DecodeParams &p, uint32_t n_blocks, cudaStream_t st) {
-    size_t smem = (size_t)(DECODE_BLOCK_THREADS / 16) * SMEM_BYTES_PER_GROUP;
-    decode_kernel<16><<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p);
-}
-int decode_max_blocks_per_sm16() {
-    const int nb = stream_kernel_blocks_per_sm(decode_kernel<16>, DECODE_BLOCK_THREADS, (size_t)(DECODE_BLOCK_THREADS / 16) * SMEM_BYTES_PER_GROUP);
-    return nb;
-}
-#endif
 
 }  // namespace dv

@@ -14,18 +14,14 @@ template <typename K> static inline int stream_kernel_blocks_per_sm(K kernel, in
 }
 
 void launch_frame(const FrameParams &p, uint8_t *payload, uint64_t payload_cap_bytes, cudaStream_t st);   // frame + payload scan + demux (3 launches)
-void launch_decode32(const DecodeParams &p, uint32_t n_blocks, cudaStream_t st);
-void launch_decode16(const DecodeParams &p, uint32_t n_blocks, cudaStream_t st);
-int decode_max_blocks_per_sm32();
 // v2 engine (dv2_kernels.cu), lanes_per_stream = 16 (two streams per warp) or 8 (four)
 void launch_decode_v2(int lanes_per_stream, const DecodeParams &p, uint32_t n_blocks, cudaStream_t st);
 int decode_max_blocks_per_sm_v2(int lanes_per_stream);
 int decode_groups_per_block_v2(int lanes_per_stream);
-int decode_max_blocks_per_sm16();
 void launch_encode_model(const EncodeParams &p, uint32_t n_blocks, cudaStream_t st);   // groups of 16 lanes
 void launch_encode_flush_mux(const EncodeParams &p, cudaStream_t st);                  // reverse rANS + mux/CRC (2 launches)
 int encode_max_blocks_per_sm();
-// the reference's feature="blend" probability model (dv_blend.cuh): 16 lanes per stream, generic nibble path only
+// the reference's feature="blend" probability model (dv_blend.cuh, dv_kernels.cu): 16 lanes per stream, no literal fast loop
 void launch_decode16_blend(const DecodeParams &p, uint32_t n_blocks, cudaStream_t st);
 int decode_max_blocks_per_sm16_blend();
 void launch_encode_model_blend(const EncodeParams &p, uint32_t n_blocks, cudaStream_t st);

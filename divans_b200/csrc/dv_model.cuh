@@ -7,10 +7,10 @@
 //   blend       (probability/frequentist_cdf.rs:74-85) -> per-lane predicated add + uniform rescale branch
 //   average     (probability/frequentist_cdf.rs:58-72) -> per-lane integer mad
 // Everything that is scalar in the reference (rANS states, book-keeping) is replicated across the lanes of the
-// group (uniform registers).  With LANES_PER_STREAM==32 the upper half-warp mirrors the lower one (same stream);
-// with 16 the two half-warps run two different streams.
+// group (uniform registers).  The two half-warps run two different streams (the v2 decoder also runs 8-lane groups,
+// dv2_core.cuh).
 //
-// The same code runs as decoder (ENC=false: symbols come out of the rANS state) and as encoder (ENC=true: symbols
+// The same model code runs as decoder (ENC=false: symbols come out of the rANS state) and as encoder (ENC=true: symbols
 // are given, (start,freq) pairs are recorded for the reverse rANS pass) -- exactly how the reference shares
 // DivansCodec between ANSDecoder and ANSEncoder (codec/mod.rs:160-186).
 #pragma once
@@ -116,14 +116,10 @@ __device__ __forceinline__ int cdf_div_pos(int c, int maxv) {
     return (int)qi;
 }
 
-// group-wide context handed around (all uniform except l16)
+// what the CDF helpers below need of a 16-lane group
 struct Grp {
-    unsigned mask;     // participating lanes of this group
-    int shift;         // 0 or 16: position of the group's 16 ballot bits
+    unsigned mask;     // participating lanes of the shuffles
     int l16;           // lane & 15
-    bool writer;       // lane that performs CDF stores for element l16 (false on the mirrored upper half)
-    bool lane0;        // l16 == 0 (scalar work; true on lane 16 too when the upper half mirrors)
-    bool store0;       // the single lane that performs scalar stores for the group
 };
 
 // freq only (for the mixing weights: codec/literal.rs:236-239)

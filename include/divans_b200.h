@@ -126,9 +126,8 @@ typedef struct divans_b200_ctx divans_b200_ctx;
 /* device = CUDA ordinal; max_resident = cap on concurrently resident streams (0 = auto: sized to the GPU);
  * lanes_per_stream: 0 = by batch size (16 lanes per stream, 8 when their residency holds the batch in fewer passes); 16 = two
  * streams per warp, one CDF element per lane; 8 = four streams per warp, two elements per lane (up to twice the resident
- * streams where registers, not slot memory, limit residency) --
- * all three the round-2 engine; 32 = round-1 kernel, one warp owns one stream (the upper half-warp mirrors the lower);
- * 116 = the round-1 16-lane kernel (A/B measurements). */
+ * streams where registers, not slot memory, limit residency).  Any other value means 16 (divans_b200_last_lanes reports
+ * the layout a decode ran on). */
 divans_b200_ctx *divans_b200_create(int device, uint32_t max_resident, uint32_t lanes_per_stream);
 void divans_b200_destroy(divans_b200_ctx *ctx);
 const char *divans_b200_last_error(divans_b200_ctx *ctx);

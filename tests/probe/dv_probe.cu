@@ -80,7 +80,7 @@ __global__ void gate_kernel(int32_t *out) {
 }
 
 // ---- one coding step at CDF level, one lane group per case ----
-enum StepVariant { V2_16 = 0, V2_8 = 1, R1_DEC = 2, R1_ENC = 3, FAST_16 = 4, FAST_8 = 5, FAST_MIX_16 = 6 };
+enum StepVariant { V2_16 = 0, V2_8 = 1, R1_ENC = 3, FAST_16 = 4, FAST_8 = 5, FAST_MIX_16 = 6 };   // (2 is unused: the values seed the tests' cases)
 struct StepIo {
     const int16_t *cdf, *cdf2; const int32_t *wts, *speeds; const uint64_t *state; const int32_t *sym_in;
     int16_t *s_cdf, *s_cdf2; dv::Cold *cold; uint32_t *log; const uint32_t *zero_word;   // per padded case scratch
@@ -107,7 +107,7 @@ __global__ void step_kernel(StepIo io) {
     int sym = 0, start = 0, freq = 0, status = 0;
     uint64_t st = 0;
     dv::Weights w = w0;
-    if (V == V2_16 || V == V2_8 || V == R1_DEC || V == R1_ENC) {
+    if (V == V2_16 || V == V2_8 || V == R1_ENC) {
         dv::St s;
         memset(&s, 0, sizeof s);
         s.c = c; s.state = 1; s.status = dv::ST_OK; s.gen = io.gen; s.tagged = false;
@@ -117,8 +117,7 @@ __global__ void step_kernel(StepIo io) {
         nx.cdf = cdf; nx.cdf2 = io.mix ? cdf2 : nullptr; nx.speed = io.speeds[2 * i]; nx.sym = io.sym_in[i]; nx.mix_hi = true; nx.tagged = false;
         if (V == V2_16) sym = dv::nibble_core_v2<16>(s, nx, g);
         else if (V == V2_8) sym = dv::nibble_core_v2<8>(s, nx, g);
-        else if (V == R1_DEC) sym = dv::nibble_core<false, 16>(s, nx, g, true);
-        else sym = dv::nibble_core<true, 16>(s, nx, g, true);
+        else sym = dv::nibble_core_enc(s, nx, g);
         __syncwarp();
         st = s.cur.b;
         status = s.status;
@@ -177,7 +176,7 @@ int dvp_step(int variant, size_t n, int mix, uint32_t gen, const int16_t *cdf, c
     const size_t per_block = 256 / nl, np = (n + per_block - 1) / per_block * per_block;
     void *bufs[17] = {};
     if (n == 0) return 0;
-    if (variant < 0 || variant > 6) return (int)cudaErrorInvalidValue;
+    if (variant < 0 || variant > 6 || variant == 2) return (int)cudaErrorInvalidValue;
     PK(cudaSetDevice(0));
 #define ALLOC(k, ptr, bytes) do { PK(cudaMalloc(&bufs[k], (bytes))); PK(cudaMemset(bufs[k], 0, (bytes))); ptr = decltype(ptr)(bufs[k]); } while (0)
     ALLOC(0, io.cdf, n * 32); ALLOC(1, io.cdf2, n * 32); ALLOC(2, io.wts, n * 12); ALLOC(3, io.speeds, n * 8);
@@ -199,7 +198,6 @@ int dvp_step(int variant, size_t n, int mix, uint32_t gen, const int16_t *cdf, c
         switch (variant) {
             case V2_16: step_kernel<V2_16><<<blocks, 256>>>(io); break;
             case V2_8: step_kernel<V2_8><<<blocks, 256>>>(io); break;
-            case R1_DEC: step_kernel<R1_DEC><<<blocks, 256>>>(io); break;
             case R1_ENC: step_kernel<R1_ENC><<<blocks, 256>>>(io); break;
             case FAST_16: step_kernel<FAST_16><<<blocks, 256>>>(io); break;
             case FAST_8: step_kernel<FAST_8><<<blocks, 256>>>(io); break;

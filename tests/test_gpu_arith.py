@@ -64,7 +64,7 @@ def test_cdf_div_equals_the_reference_division_on_the_whole_i16_domain(probe):
 
 
 def test_cdf_div_pos_is_exact_for_every_c_up_to_max(probe):
-    """the round-1 fast loops' and the encoder's division: 0 <= c <= max < 2^15"""
+    """the division of the encoder's literal fast loop: 0 <= c <= max < 2^15"""
     r = sweep(probe, MODE_CDF_DIV_POS, 1, 32768)
     _report("cdf_div_pos", r)
     assert r["cases"] == sum(d + 1 for d in range(1, 32768))
@@ -182,7 +182,7 @@ def test_speed_is_small_on_every_i16_pair(probe):
 
 
 @pytest.mark.parametrize("variant", sorted(R.C_OVER_MAX_OPTIONS))
-def test_c_over_max_regime_matches_the_oracle(engine, engine16, engine32, oracle, variant):
+def test_c_over_max_regime_matches_the_oracle(engine, engine16, oracle, variant):
     """one literal prior driven into a state with an element far above its max, then coded at that element: the GPU
     encoder's bytes equal the oracle's, and every decode layout returns the oracle's status and bytes"""
     import divans_b200
@@ -191,7 +191,7 @@ def test_c_over_max_regime_matches_the_oracle(engine, engine16, engine32, oracle
     assert got[0] == stream, "GPU encoder output differs from the oracle's"
     cap = len(R.C_OVER_MAX_BYTES) + 64
     rc, ref = oracle.decode(stream, out_cap=cap)
-    for layout, eng in (("16 lanes", engine), ("8 lanes", engine16), ("32 lanes", engine32)):
+    for layout, eng in (("16 lanes", engine), ("8 lanes", engine16)):
         st, out = eng.decode([stream], [cap])[0]
         assert (st, out) == (rc, ref), "%s: status %d, oracle %d" % (layout, st, rc)
 
@@ -200,7 +200,7 @@ def test_c_over_max_regime_matches_the_oracle(engine, engine16, engine32, oracle
 # One coding step at CDF level: the cores as the engine calls them (the probe's dvp_step), against the oracle's
 # dvo_cdf_step_batch (code_lit_nibble, codec/literal.rs:154-259, with the rANS step of ans.rs:230-244)
 # ---------------------------------------------------------------------------------------------------------------------
-V2_16, V2_8, R1_DEC, R1_ENC, FAST_16, FAST_8, FAST_MIX_16 = range(7)
+V2_16, V2_8, R1_ENC, FAST_16, FAST_8, FAST_MIX_16 = 0, 1, 3, 4, 5, 6   # dv_probe.cu StepVariant
 GEN = 0xA5C3                                             # a nonzero generation: the fast pieces store its bits as tags
 HIGH_WORDS = [1, 1 << 16, (1 << 31) - 1, 1 << 47]
 
@@ -336,9 +336,9 @@ def test_walk_states_reach_c_over_max_with_quotients_above_2_24(step_states):
 
 
 @pytest.mark.parametrize("mix", [False, True], ids=["plain", "mixing"])
-@pytest.mark.parametrize("variant", [V2_16, V2_8, R1_DEC, R1_ENC], ids=["v2_16", "v2_8", "r1_decode", "r1_encode"])
+@pytest.mark.parametrize("variant", [V2_16, V2_8, R1_ENC], ids=["v2_16", "v2_8", "r1_encode"])
 def test_generic_core_step_equals_the_oracle(probe, oracle, step_states, weight_states, variant, mix):
-    """nibble_core_v2<16> / <8> (untagged) and the round-1 nibble_core (decode, and encode with the enc_log refusal) on walk
+    """nibble_core_v2<16> / <8> (untagged) and the round-1 core's encoder step (nibble_core_enc, with the enc_log refusal) on walk
     states under every f8 speed pair, the c > max states those walks reach, and edge vectors"""
     rng = np.random.default_rng(40 + variant + 8 * mix)
     cdf, spd, _ = step_states["wide"]

@@ -372,7 +372,7 @@ def test_encoder_slot_succession(oracle):
 # ---------------------------------------------------------------------------------------------------------------------
 # framing and chunk edges
 # ---------------------------------------------------------------------------------------------------------------------
-def test_framing_edges_encode_like_the_oracle_and_decode(engine, engine16, engine32, oracle):
+def test_framing_edges_encode_like_the_oracle_and_decode(engine, engine16, oracle):
     """Literal payloads of exactly 4096, 16384, 65536, 65536 + 4096, 65536 + 16384 and 131072 bytes, command payloads of
     4096 and 16384 bytes, 65535 / 65536 / 65537 command nibbles, both payloads over 131073 bytes: the GPU encoder equals
     the oracle (raw mode for the random-byte edges, command lists for the LZ77 ones), and every decode layout returns the
@@ -389,13 +389,13 @@ def test_framing_edges_encode_like_the_oracle_and_decode(engine, engine16, engin
             got = engine.encode([cl.serialize()], divans_b200.encode_options(**kw), cmds=True)[0]
         _check(got, ref, name)
         streams.append(ref); raws.append(raw)
-    for eng in (engine, engine16, engine32):
+    for eng in (engine, engine16):
         res = eng.decode(streams, [len(r) + 64 for r in raws])
         for name, (st, out), r in zip(R.EDGE_NAMES, res, raws):
             assert st == 0 and out == r, (name, eng.last_lanes())
 
 
-def test_remuxed_streams_decode_on_every_layout(engine, engine16, engine32, oracle):
+def test_remuxed_streams_decode_on_every_layout(engine, engine16, oracle):
     """The same payloads under other record chains (1-byte records, random sizes and coder order, one-byte codes, all
     literal records first, record starts at every offset mod 16), mixed into one batch with the streams as the mux
     wrote them: the oracle and every GPU decode layout return the original bytes."""
@@ -412,13 +412,13 @@ def test_remuxed_streams_decode_on_every_layout(engine, engine16, engine32, orac
             rc, out = oracle.decode(s2, out_cap=len(raw) + 64)
             assert rc == 0 and out == raw, (name, lay)
             streams.append(s2); raws.append(raw)
-    for eng in (engine, engine16, engine32):
+    for eng in (engine, engine16):
         res = eng.decode(streams, [len(r) + 64 for r in raws])
         for i, ((st, out), r) in enumerate(zip(res, raws)):
             assert st == 0 and out == r, (i, eng.last_lanes())
 
 
-def test_hostile_record_chains_match_the_oracle(engine, engine16, engine32, oracle):
+def test_hostile_record_chains_match_the_oracle(engine, engine16, oracle):
     """Record-chain damage: truncation inside a three-byte record header, truncation inside a one-byte-code record, a code
     k > 3, and a header byte 2..15 (the low bit picks the coder, mux.rs; valid once the CRC is recomputed).  Every status
     equals the oracle's, and so does every output the oracle accepts."""
@@ -448,7 +448,7 @@ def test_hostile_record_chains_match_the_oracle(engine, engine16, engine32, orac
     cap = len(raw) + 64
     ref = [oracle.decode(s, out_cap=cap) for s in streams]
     assert [r[0] for r in ref].count(0) >= 6 and {r[0] for r in ref} >= {0, 1, 3}, [r[0] for r in ref]
-    for eng in (engine, engine16, engine32):
+    for eng in (engine, engine16):
         res = eng.decode(streams, [cap] * len(streams))
         for i, ((st, out), (rc, rb)) in enumerate(zip(res, ref)):
             assert st == rc, "stream %d: status %d, oracle %d (lanes %d)" % (i, st, rc, eng.last_lanes())

@@ -24,10 +24,9 @@ def _decode_and_compare(engine, oracle, streams, raws=None, flags=0, layout=""):
 
 
 @pytest.fixture
-def decode_engines(engine, engine16, engine32):
-    """every decode layout, as (name, engine): the v2 engine with two (16 lanes) and four (8 lanes) streams per warp, and the
-    round-1 kernel with one warp per stream (32 lanes)"""
-    return [("16 lanes", engine), ("8 lanes", engine16), ("32 lanes", engine32)]
+def decode_engines(engine, engine16):
+    """every decode layout, as (name, engine): the v2 engine with two (16 lanes) and four (8 lanes) streams per warp"""
+    return [("16 lanes", engine), ("8 lanes", engine16)]
 
 
 @pytest.fixture(scope="module")
@@ -44,16 +43,21 @@ def test_golden_fixtures(engine, oracle, golden):
         assert hashlib.sha256(out).hexdigest() == e["raw_sha256"], e["name"]   # == the reference's raw testdata file
 
 
-def test_golden_fixtures_other_lane_layouts(engine16, engine32, oracle, golden):
-    # 16 lanes per stream (two streams per warp) and 32 (one warp owns one stream: the upper half-warp mirrors the lower)
+def test_golden_fixtures_other_lane_layouts(engine16, oracle, golden):
+    # 8 lanes per stream (four streams per warp)
     streams = [open(e["path"], "rb").read() for e in golden]
-    for eng in (engine16, engine32):
-        res = eng.decode(streams, [e["raw_len"] + 64 for e in golden])
-        for e, (st, out) in zip(golden, res):
-            assert st == 0 and hashlib.sha256(out).hexdigest() == e["raw_sha256"], e["name"]
+    res = engine16.decode(streams, [e["raw_len"] + 64 for e in golden])
+    for e, (st, out) in zip(golden, res):
+        assert st == 0 and hashlib.sha256(out).hexdigest() == e["raw_sha256"], e["name"]
 
 
-def test_reference_held_stream(engine, engine16, engine32, oracle):
+def test_other_lane_counts_run_16_lanes(engine32, oracle, golden):
+    """lanes_per_stream values other than 0 (auto) and 8 select 16 lanes per stream; 32 is one of them"""
+    _decode_and_compare(engine32, oracle, [open(e["path"], "rb").read() for e in golden])
+    assert engine32.last_lanes() == 16
+
+
+def test_reference_held_stream(engine, engine16, oracle):
     """The one compressed stream the reference tree holds (wasm/wasm.html:98-107, written by the reference's Rust encoder):
     both lane layouts decode it bit-exactly under its model revision (include/divans_b200.h), CRC checked on the GPU; under
     today's model revision it is rejected exactly like the oracle rejects it."""
@@ -64,7 +68,7 @@ def test_reference_held_stream(engine, engine16, engine32, oracle):
     meta = json.load(open(os.path.join(d, "ref_wasm_example.json")))
     want = meta["plain_text"].encode("ascii")
     assert want == b"It snowed, rained, and hailed the same morning.\n" * 7
-    for eng in (engine, engine16, engine32):
+    for eng in (engine, engine16):
         # a batch that mixes the 2018 stream with copies of itself exercises both groups of a warp
         res = eng.decode([vec] * 5, [len(want) + 64] * 5, divans_b200.FLAG_MODEL_WASM_2018)
         for st, out in res:
@@ -134,16 +138,7 @@ def test_random_ir_fuzz(decode_engines, oracle, text):
         _decode_and_compare(eng, oracle, streams, layout=layout)
 
 
-def test_random_ir_fuzz_one_warp_per_stream(engine32, oracle, text):
-    import irfuzz
-    streams = []
-    for seed in range(100, 112):
-        c = oracle.Commands.from_ir(irfuzz.random_ir(oracle, seed, n_cmds=100, window=16, text=text))
-        streams.append(c.encode(oracle.options(window_size=16, dynamic_context_mixing=seed % 3)))
-    _decode_and_compare(engine32, oracle, streams)
-
-
-def test_random_ir_fuzz_full_f8_speed_range(engine, engine16, engine32, oracle, text):
+def test_random_ir_fuzz_full_f8_speed_range(engine, engine16, oracle, text):
     """Speeds are carried by the stream: the literal fast loops (32-bit adaptive arithmetic) must hand over to the generic
     core (i16 wrap + the reference's literal LUT divide) whenever a counter could wrap.  GPU and oracle must agree on
     status and on every output byte, whether or not the stream decodes back to its input."""
@@ -158,7 +153,7 @@ def test_random_ir_fuzz_full_f8_speed_range(engine, engine16, engine32, oracle, 
         except ValueError:
             pass   # a wrapped counter gave a coded symbol frequency <= 0: the reference encoder divides by it and panics
     caps = [1 << 18] * len(streams)
-    for eng in (engine, engine16, engine32):
+    for eng in (engine, engine16):
         res = eng.decode(streams, caps, 1)   # FLAG_SKIP_CRC: payloads are well-formed, only the model misbehaves
         for i, (st, out) in enumerate(res):
             rc, ref = oracle.decode(streams[i], out_cap=caps[i], skip_crc=True)

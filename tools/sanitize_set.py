@@ -24,7 +24,7 @@ streams.append(O.Commands.lz77(raw64, window=16).encode(O.options(window_size=16
 refs = [O.decode(s, out_cap=1 << 20) for s in streams]
 assert all(rc == 0 for rc, _ in refs)
 wasm = open(os.path.join(ROOT, "tests", "golden", "ref_wasm_example.divans"), "rb").read()
-for lps in (8, 16, 32):
+for lps in (8, 16):
     eng = divans_b200.Engine(0, 32, lps)
     res = eng.decode(streams, [len(r) + 64 for _, r in refs])
     assert all(st == 0 and out == r for (st, out), (_, r) in zip(res, refs)), "decode mismatch lps=%d" % lps
