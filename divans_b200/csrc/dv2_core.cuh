@@ -215,12 +215,37 @@ struct FastK {
     uint32_t mytag;                                    // this lane's bit(s) of the stream's generation (lane_tag)
 };
 
+// The eager-refill coder of the fast loops.  The reference refills a state right before it is used (ans.rs:428-442); the word
+// order in the stream is the order in which states were produced, so refilling a state as soon as it drops below 2^31 consumes
+// the same words.  Payload words are addressed by a saturating index: the demux kernel leaves >= 16 readable bytes after every
+// coder's payload, so index n_words may be read once; an index that ends above n_words means underflow.
+// coder_to_eager: the lazy Coder the state machine keeps -> eager form (pending refill or 16-byte (re)initialisation of `a`
+// done, `b` refilled now).  A group that is not `active` rides along as a dummy: states that never refill, payload words read
+// from its own slot.
+__device__ __forceinline__ void coder_to_eager(Coder &k, FastK &f, const uint8_t *slot, const bool active) {
+    if (!active) { k.p = reinterpret_cast<const uint32_t *>(slot + OFF_T2); k.left = 0; k.need_a = 0; k.need_b = 0; k.sym_count = 0; k.a = k.b = 1ull << 40; }
+    f.wbase = k.p; f.wmax = k.left + 1; f.wi = 0;
+    coder_fill(k);
+    f.wi = (uint32_t)(k.p - f.wbase);
+    if (k.need_b) { k.b = (k.b << 32) | (uint64_t)f.wbase[f.wi]; f.wi = min(f.wi + 1, f.wmax); k.need_b = 0; }
+    f.wnext = f.wbase[f.wi];
+}
+// ... and back: `a` is the state the next nibble uses, every produced state is refilled already
+__device__ __forceinline__ void coder_from_eager(Coder &k, FastK &f) {
+    if (f.wi >= f.wmax) { k.underflow = 1; f.wi = f.wmax - 1; }
+    k.p = f.wbase + f.wi; k.left = f.wmax - 1 - f.wi;
+    k.need_a = (k.sym_count >= NUM_SYMBOLS_BEFORE_FLUSH) ? 8u : 0u; k.need_b = 0;
+}
+__device__ __forceinline__ void eager_refill(uint64_t &x, FastK &f) {
+    x = (x << 32) | (uint64_t)f.wnext; f.wi = min(f.wi + 1, f.wmax); f.wnext = ld_stream_u32(f.wbase + f.wi);
+}
+
 // One literal nibble after its symbol is known, in two parts.  (1) blend + store (+ tag) happens at once: the same prior may
 // be the next one to be loaded.  (2) exact start/freq and the rANS step with eager refill only have to be done before the state
 // is used again, one byte later: the loop runs the two steps of a byte back to back so that their (long, serial) dependency
 // chains overlap.  `ev` / `mv`: the validated prior (elements of this lane, max).
 template <int LPG>
-__device__ __forceinline__ void blend_store_v2(const uint32_t ev, const uint32_t mv, const int sym, const char *const p, const G2 g, const FastK &f) {
+__device__ __forceinline__ uint32_t blend_v2(const uint32_t ev, const uint32_t mv, const int sym, const G2 g, const FastK &f) {
     uint32_t c2;
     if (LPG == 16) {
         c2 = ev + ((g.l16 >= sym) ? (uint32_t)f.inc : 0u);
@@ -231,7 +256,11 @@ __device__ __forceinline__ void blend_store_v2(const uint32_t ev, const uint32_t
         c2 = ev + (f.incp & m);
         if ((int)mv + f.inc >= f.lim) { const uint32_t u = c2 + f.kp; c2 = u - ((u >> 2) & 0x3fff3fffu); }
     }
-    store_elems<LPG>(p, g.l16, c2 | f.mytag);
+    return c2;
+}
+template <int LPG>
+__device__ __forceinline__ void blend_store_v2(const uint32_t ev, const uint32_t mv, const int sym, const char *const p, const G2 g, const FastK &f) {
+    store_elems<LPG>(p, g.l16, blend_v2<LPG>(ev, mv, sym, g, f) | f.mytag);
 }
 // state after coding `sym` of the validated prior (ev, mv), before renormalisation (ans.rs:230-244)
 template <int LPG>
@@ -267,8 +296,8 @@ __device__ __forceinline__ void rans_pair_v2(uint64_t &a, uint64_t &b, const uin
     // two streams per warp: no state refills in 78 % of the bytes, the branch pays; four streams per warp: 61 %, the
     // predicated form is the faster one
     if (LPG == 8 || __any_sync(FULL, na || nb)) {
-        if (na) { xa = (xa << 32) | (uint64_t)f.wnext; f.wi = min(f.wi + 1, f.wmax); f.wnext = ld_stream_u32(f.wbase + f.wi); }
-        if (nb) { xb = (xb << 32) | (uint64_t)f.wnext; f.wi = min(f.wi + 1, f.wmax); f.wnext = ld_stream_u32(f.wbase + f.wi); }
+        if (na) eager_refill(xa, f);
+        if (nb) eager_refill(xb, f);
     }
     a = xa; b = xb;
 }
@@ -317,7 +346,7 @@ __device__ __forceinline__ void mixv_finish(uint64_t &st, const MixV v, const Mi
     uint64_t x = (uint64_t)(int64_t)(int16_t)freq * (st >> 15) + (uint64_t)(int64_t)(int32_t)t;   // ans.rs:230-244 (t < 0: see rans_advance_v2)
     const bool refill = x < (1ull << 31);
     if (__any_sync(FULL, refill)) {   // (one warp-uniform branch instead of predicated-off refill code in every nibble, see rans_pair_v2)
-        if (refill) { x = (x << 32) | (uint64_t)f.wnext; f.wi = min(f.wi + 1, f.wmax); f.wnext = ld_stream_u32(f.wbase + f.wi); }
+        if (refill) eager_refill(x, f);
     }
     st = x;
     weights_update32(w, f_cm, f_nb, (int)(short)freq);
@@ -353,13 +382,8 @@ __device__ __forceinline__ void literal_mix_loop16(St &s, const G2 g, const bool
     uint32_t ap = (uint32_t)(uintptr_t)dbase & 7u;
     const bool st_lane = g.store0 && active;
     Coder k = s.cur;
-    if (!active) { k.p = reinterpret_cast<const uint32_t *>(s.slot + OFF_T2); k.left = 0; k.need_a = 0; k.need_b = 0; k.sym_count = 0; k.a = k.b = 1ull << 40; }
     Weights wh = s.c->w_hi, wl = s.c->w_lo;
-    f.wbase = k.p; f.wmax = k.left + 1; f.wi = 0;
-    coder_fill(k);
-    f.wi = (uint32_t)(k.p - f.wbase);
-    if (k.need_b) { k.b = (k.b << 32) | (uint64_t)f.wbase[f.wi]; f.wi = min(f.wi + 1, f.wmax); k.need_b = 0; }
-    f.wnext = f.wbase[f.wi];
+    coder_to_eager(k, f, s.slot, active);
     uint32_t done = 0;
     while (done < n) {
         uint32_t m = n - done;
@@ -411,9 +435,7 @@ __device__ __forceinline__ void literal_mix_loop16(St &s, const G2 g, const bool
         const uint32_t tail = min(ap & 7u, done);
         for (uint32_t t = 0; t < tail; t++) dbase[done - tail + t] = (uint8_t)(l8 >> (8 * (8 - tail + t)));
     }
-    if (f.wi >= f.wmax) { k.underflow = 1; f.wi = f.wmax - 1; }
-    k.p = f.wbase + f.wi; k.left = f.wmax - 1 - f.wi;
-    k.need_a = (k.sym_count >= NUM_SYMBOLS_BEFORE_FLUSH) ? 8u : 0u; k.need_b = 0;
+    coder_from_eager(k, f);
     s.cur = k; s.l8 = l8; s.lit_ctx = ctx; s.out_pos += done; s.lit_left -= done;
     s.c->w_hi = wh; s.c->w_lo = wl;
 }
@@ -448,20 +470,11 @@ __device__ __forceinline__ bool literal_plain_loop_v2(St &s, Next &nx, const G2 
     uint8_t *const dbase = s.out + s.out_pos;
     uint32_t ap = (uint32_t)(uintptr_t)dbase & 7u;                        // alignment of the ADDRESS of the byte being decoded
     const bool st_lane = g.store0 && active;
+    // eager-refill coder for the duration of the loop (coder_to_eager).  The literal coder codes nibbles in pairs: state `a`
+    // serves every high nibble, `b` every low nibble (two rotations of ans.rs:240-243 are the identity), so the loop never
+    // swaps them.
     Coder k = s.cur;
-    if (!active) { k.p = reinterpret_cast<const uint32_t *>(s.slot + OFF_T2); k.left = 0; k.need_a = 0; k.need_b = 0; k.sym_count = 0; k.a = k.b = 1ull << 40; }
-    // ---- EAGER-refill coder for the duration of the loop ----
-    // The reference refills a state right before it is used (ans.rs:428-442); the word order in the stream is the order in
-    // which states were produced, so refilling a state as soon as it drops below 2^31 consumes the same words.  The literal
-    // coder codes nibbles in pairs: state `a` serves every high nibble, `b` every low nibble (two rotations of
-    // ans.rs:240-243 are the identity), so the loop never swaps them.  Payload words are addressed by a saturating index:
-    // the demux kernel leaves >= 16 readable bytes after every coder's payload, so index n_words may be read once; an index
-    // that ends above n_words means underflow.
-    f.wbase = k.p; f.wmax = k.left + 1; f.wi = 0;
-    coder_fill(k);                                                        // pending refill / 16-byte (re)initialisation of `a`
-    f.wi = (uint32_t)(k.p - f.wbase);
-    if (k.need_b) { k.b = (k.b << 32) | (uint64_t)f.wbase[f.wi]; f.wi = min(f.wi + 1, f.wmax); k.need_b = 0; }
-    f.wnext = f.wbase[f.wi];
+    coder_to_eager(k, f, s.slot, active);
     uint32_t done = 0;
     while (done < n) {
         uint32_t m = n - done;
@@ -534,10 +547,7 @@ __device__ __forceinline__ bool literal_plain_loop_v2(St &s, Next &nx, const G2 
         const uint32_t tail = min(ap & 7u, done);
         for (uint32_t t = 0; t < tail; t++) dbase[done - tail + t] = (uint8_t)(l8 >> (8 * (8 - tail + t)));
     }
-    // back to the lazy representation the state machine uses
-    if (f.wi >= f.wmax) { k.underflow = 1; f.wi = f.wmax - 1; }
-    k.p = f.wbase + f.wi; k.left = f.wmax - 1 - f.wi;
-    k.need_a = (k.sym_count >= NUM_SYMBOLS_BEFORE_FLUSH) ? 8u : 0u; k.need_b = 0;
+    coder_from_eager(k, f);                                               // back to the lazy representation the state machine uses
     s.cur = k; s.l8 = l8; s.lit_ctx = ctx; s.out_pos += done; s.lit_left -= done;
     enter_lit_nibble<false, true, true>(s, nx);
     return true;
@@ -579,6 +589,93 @@ __device__ __forceinline__ bool literal_fast_v2(St &s, Next &nx, const G2 g, con
         if (small) return literal_plain_loop_v2<LPG, LPG == 16>(s, nx, g, active, t2s, n);
         return literal_plain_loop_v2<LPG, false>(s, nx, g, active, t2s, n);
     }
+}
+
+// Converged fast path for the 8192 mixing values of a PredictionMode command (context_map.rs:385-425), every group of the warp
+// in S_PM_MIXVAL (`active`) or out of work (a dummy, as in literal_fast_v2).  Each value is one nibble of the command coder
+// against an untagged MISC prior adapted at SPK_PLANE, a speed that keeps every adaptive value inside i16 (speed_is_small): the
+// 32-bit arithmetic of the literal loops is exact.  The prior of value f1 depends on the value coded 256 nibbles earlier, not
+// on the nibble just coded, and consecutive nibbles alternate between the two rANS states (ans.rs:240-243), so a nibble's
+// dependency chain is search -> blend of the same prior -> the next search; the rANS step stays off it.
+// The run stops short of two positions, where the generic path, which keeps the reference's lazy refills, codes the nibbles:
+//   * value 8190: the last value ends the command (mixing_param, pred_mode, the speeds, t2_dirty, the f0 > 3 failure), and an
+//     underflow of the last eager refill must not be reported before the failure of the nibble after it;
+//   * symbol 65534 of the coder's chunk: the 16-byte re-initialisation after symbol 65535 drops the refill of the state of
+//     symbol 65534 and moves that of symbol 65535 behind its own words (ans.rs:230-244).
+// The run proper, out of line: the command path that shares the kernel is instruction-fetch bound (DESIGN section 4), and the
+// loop inlined into the main loop made LZ77 command streams slower.  Everything crosses the call by value, so that the caller's
+// St stays in registers.  Returns the coder (lazy form) and the next mixing value.
+struct MixvalRun { Coder k; uint32_t f1; };
+template <int LPG>
+static __device__ __noinline__ MixvalRun mixval_run_v2(Coder k, const uint32_t f1, const uint32_t n, uint8_t *const slot, const bool rev,
+                                                       const G2 g, const bool active) {
+    const int li = g.l16;
+    FastK f;
+    f.inc = (int)(short)(SPK_PLANE & 0xffff); f.lim = SPK_PLANE >> 16;
+    f.incp = (uint32_t)f.inc * 0x10001u;
+    f.kp = LPG == 16 ? (uint32_t)(li + 1) : ((uint32_t)(2 * li + 1) | ((uint32_t)(2 * li + 2) << 16));
+    f.mytag = 0;
+    const uint32_t bsel = LPG == 16 ? (0xffffu << g.shift) : ((uint32_t)(g.shift >> 3) * 0x1111u + 0x4040u);
+    const uint32_t slot_lo = (uint32_t)(uintptr_t)slot, slot_hi = (uint32_t)((uintptr_t)slot >> 32);
+    // (32-bit addresses inside the slot, as in the literal loops; `pe` below: this lane's element(s) of the prior's CDF)
+    const uint32_t pbase = slot_lo + (uint32_t)OFF_MISC + (uint32_t)(MI_PRED + PM_MIXING_VALUE) * CDF_BYTES, mixb = slot_lo + (uint32_t)OFF_MIX;
+    const auto mix = [slot_hi, mixb](uint32_t i) { return ld_u8g(mk_ptr(mixb + i, slot_hi)); };
+    const bool st_lane = g.store0 && active;
+    coder_to_eager(k, f, slot, active);
+    if (st_lane && f1 == 0) reinterpret_cast<uint32_t *>(slot + OFF_HDR)[3] = 1u;   // the mask is about to hold this stream's values
+    // Runs of values whose prior stays the same for every group: the prior is loaded once and then kept in registers (each blend
+    // is stored as well).  With one mixing value for the whole map, the usual case, the prior changes once, at value 256.
+    // Consecutive values alternate between the states (ans.rs:240-243): the loop codes them in pairs, value 2j on `a` and 2j + 1
+    // on `b`, and swaps the two only when a run ends after an odd number of values.
+    constexpr uint32_t EB = CDF_BYTES / LPG;                              // bytes of a lane's element(s)
+    uint32_t pi = mixval_prior(f1, rev, mix), i = 0;
+    while (i < n) {
+        const uint32_t pa = pbase + pi * CDF_BYTES;
+        __syncwarp();                                                    // (the other lanes' stores: mixing values, the max)
+        const char *const pe = mk_ptr(pa + EB * li, slot_hi);
+        uint32_t ev = load_elems<LPG>(pe, 0), mv = ld_u16g(mk_ptr(pa + 30u, slot_hi));
+        uint32_t pn;
+        // value f1 + i on state `st`; true when the run ends after it
+        const auto value = [&](uint64_t &st) {
+            pn = mixval_prior(f1 + i + 1, rev, mix);                     // its mixing value was coded 255 nibbles ago
+            const int sym = search_v2<LPG>(st, ev, mv, bsel);
+            if (st_lane) st_u8(mk_ptr(mixb + f1 + i, slot_hi), (uint32_t)sym);
+            const uint32_t ne = blend_v2<LPG>(ev, mv, sym, g, f);
+            store_elems<LPG>(pe, 0, ne);
+            uint32_t nm = mv + (uint32_t)f.inc;                          // element 15 of `ne`: the new max
+            if ((int)nm >= f.lim) { const uint32_t u = nm + 16u; nm = u - (u >> 2); }
+            uint64_t x = rans_advance_v2<LPG>(st, ev, mv, sym);
+            const bool rf = x < (1ull << 31);
+            if (LPG == 8 || __any_sync(FULL, rf)) { if (rf) eager_refill(x, f); }   // (as in rans_pair_v2)
+            st = x; ev = ne; mv = nm;
+            __syncwarp();
+            const bool change = __any_sync(FULL, pn != pi);              // (not behind `||`: a branch costs more than the vote)
+            return (++i == n) | change;
+        };
+        for (;;) {
+            if (value(k.a)) { const uint64_t t = k.a; k.a = k.b; k.b = t; break; }
+            if (value(k.b)) break;
+        }
+        pi = pn;
+    }
+    k.sym_count += n;
+    coder_from_eager(k, f);
+    return MixvalRun{k, f1 + n};
+}
+// Returns false (nothing done) when some group has fewer than 8 values to go before one of them.
+template <int LPG>
+__device__ __forceinline__ bool mixval_fast_v2(St &s, Next &nx, const G2 g, const bool active) {
+    const uint32_t sc = s.cur.need_a > 1 ? 0u : s.cur.sym_count;       // (a pending 16-byte initialisation starts a new chunk)
+    uint32_t n = active ? min(8190u - min(s.f1, 8190u), 65534u - min(sc, 65534u)) : 0xffffffffu;
+    if (LPG == 8) n = min(n, __shfl_xor_sync(FULL, n, 8));
+    n = min(n, __shfl_xor_sync(FULL, n, 16));
+    if (n < 8) return false;
+    // a dummy codes against slot 16 of its own slot
+    const MixvalRun r = mixval_run_v2<LPG>(s.cur, active ? s.f1 : 0u, n, s.slot, !active || s.c->model_rev, g, active);
+    if (!active) return true;
+    s.cur = r.k; s.f1 = r.f1;
+    enter_pm_mixval<false>(s, nx);
+    return true;
 }
 
 }  // namespace dv

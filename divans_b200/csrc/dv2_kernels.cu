@@ -94,12 +94,17 @@ __global__ void __launch_bounds__(DEC2_BLOCK_THREADS, DEC2_MIN_BLOCKS) decode_ke
             if (__all_sync(FULL, s.state == S_DONE)) break;
             __syncwarp();
         }
-        // ---- whole literal bytes while every group is at a byte boundary of a literal (or out of work) ----
-        const bool lit = s.state == S_LIT_HI;
-        if (__any_sync(FULL, lit) && __all_sync(FULL, lit || s.state == S_DONE) && literal_fast_v2<LPG>(s, nx, g, lit, t2s)) {   // (the cheaper, usually false test first)
-            if (lit) {
+        // ---- whole literal bytes while every group is at a byte boundary of a literal, or runs of mixing values while every
+        // group is in the mixing values of a PredictionMode command (or out of work) ----
+        // (the cheaper, usually false vote first; then one warp reduction of a class bit per group, out of work: none; 1 = only
+        // literal bytes, 2 = only mixing values)
+        const bool lit = s.state == S_LIT_HI, pmv = s.state == S_PM_MIXVAL;
+        uint32_t seen = 0;
+        if (__any_sync(FULL, lit || pmv)) seen = __reduce_or_sync(FULL, lit ? 1u : pmv ? 2u : s.state == S_DONE ? 0u : 4u);
+        if ((seen == 1u && literal_fast_v2<LPG>(s, nx, g, lit, t2s)) || (seen == 2u && mixval_fast_v2<LPG>(s, nx, g, pmv))) {
+            if (lit || pmv) {
                 if (s.cur.underflow) s.status = ST_NEED_INPUT;
-                if (s.lit_left == 0 && s.status == ST_OK) { swap_coders(s, g); enter_cmd_type<false>(s, nx); }
+                if (lit && s.lit_left == 0 && s.status == ST_OK) { swap_coders(s, g); enter_cmd_type<false>(s, nx); }
                 if (s.status != ST_OK) {
                     if (g.store0) { p.out_len[s.c->sidx] = s.out_pos; p.status[s.c->sidx] = s.status; }
                     s.state = S_IDLE; s.status = ST_OK;

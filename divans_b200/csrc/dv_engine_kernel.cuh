@@ -265,9 +265,15 @@ template <bool ENC> __device__ __forceinline__ void enter_pm_map_mnemonic(St &s,
     // ContextMapSpeedPalette[0] share (model_rev 1, include/divans_b200.h).
     set_next<ENC>(nx, A_misc(s, MI_PRED + (s.c->model_rev ? PM_SPEED_PALETTE : PM_MNEMONIC + (int)s.f2)), SPK_MED, sym);
 }
+// the MISC slot (after MI_PRED + PM_MIXING_VALUE) of mixing value f1: context_map.rs:395-399; model_rev 1: always slot 16.
+// `mix(i)` reads mixing value i (the v2 fast loop addresses it in 32 bits)
+template <class Mix> __device__ __forceinline__ uint32_t mixval_prior(const uint32_t f1, const bool model_rev, const Mix mix) {
+    return (f1 >= 256 && !model_rev) ? (mix(f1 - 256) & 0xfu) : 16u;
+}
 template <bool ENC> __device__ __forceinline__ void enter_pm_mixval(St &s, Next &nx) {
     s.state = S_PM_MIXVAL;
-    uint32_t prior = (s.f1 >= 256 && !s.c->model_rev) ? (uint32_t)(A_mix(s)[s.f1 - 256] & 0xf) : 16u;   // context_map.rs:395-399; model_rev 1: always slot 16
+    const uint8_t *const m = A_mix(s);
+    const uint32_t prior = mixval_prior(s.f1, s.c->model_rev, [m](uint32_t i) { return (uint32_t)m[i]; });
     int sym = 0;
     if (ENC) sym = !s.c->desired_do_context_map ? 4 : (!(s.f3 & 1) ? 0 : (int)pm_rec<ENC>(s)[32 + 16384 + 1024 + s.f1]);
     set_next<ENC>(nx, A_misc(s, MI_PRED + PM_MIXING_VALUE + (int)prior), SPK_PLANE, sym);

@@ -1,7 +1,9 @@
 """Dev probe (not a test, not the bench): device time of decode/encode for several stream populations.
   python tools/perf_probe.py [n_streams] [--l-only] [--lz-all] [--decode-once]     (DIVANS_B200_LPS selects the lane layout)
   python tools/perf_probe.py --sweep [n1,n2,...]     literal-only text decode kernel time per decoded byte per stream, by batch size
-                                                     (default 132,528,1056,2112,4224: 1/8 to 4 warps per scheduler on 132 SMs)"""
+                                                     (default 132,528,1056,2112,4224: 1/8 to 4 warps per scheduler on 132 SMs)
+  python tools/perf_probe.py --prelude [n1,n2,...]   decode kernel time of the bench's text streams cut to 16 bytes (the fixed
+                                                     per-stream cost) next to the full 64 KiB streams, by batch size"""
 import os, subprocess, sys, time, numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -11,17 +13,22 @@ from divans_b200 import synth
 once = "--decode-once" in sys.argv
 
 
-def sweep(sizes):
-    """Is the literal loop bound by its dependency chain (time per byte flat in the warps per scheduler), by issue (time grows
-    with them), or by memory (a step where the batch's literal priors, ~28 KB per stream, outgrow the L2)?"""
+def card_line():
     import torch
     prop = torch.cuda.get_device_properties(0)
     try:
-        card = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+        card = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
                               capture_output=True, text=True, timeout=20).stdout.strip()
     except Exception as e:
         card = "%s (nvidia-smi: %s)" % (prop.name, e)
     print("card: %s | %d SMs | kernel %s" % (card, prop.multi_processor_count, divans_b200.kernel_version()), flush=True)
+    return prop
+
+
+def sweep(sizes):
+    """Is the literal loop bound by its dependency chain (time per byte flat in the warps per scheduler), by issue (time grows
+    with them), or by memory (a step where the batch's literal priors, ~28 KB per stream, outgrow the L2)?"""
+    prop = card_line()
     eng = divans_b200.Engine(0, 0, 16)
     blob, off, ln = synth.text_streams(max(sizes), 65536, seed=3)
     raws_all = [blob[int(o):int(o + l)].tobytes() for o, l in zip(off, ln)]
@@ -41,11 +48,46 @@ def sweep(sizes):
     eng.close()
 
 
-if "--sweep" in sys.argv:
-    i = sys.argv.index("--sweep")
-    spec = sys.argv[i + 1] if i + 1 < len(sys.argv) and not sys.argv[i + 1].startswith("--") else "132,528,1056,2112,4224"
-    sweep([int(x) for x in spec.split(",")])
-    sys.exit(0)
+def prelude(sizes):
+    """The fixed per-stream cost: the bench's text streams cut to their first 16 bytes (per-stream setup, the PredictionMode
+    command with its 8192 mixing values, a 16-byte literal) against the full 64 KiB streams, decode kernel time by batch size.
+    A third column codes the same 16 bytes without the PredictionMode command: setup and literal only."""
+    card_line()
+    eng = divans_b200.Engine(0, 0, int(os.environ.get("DIVANS_B200_LPS", "16")))
+    blob, off, ln = synth.text_streams(max(sizes), 65536)     # bench.py's seed
+    full_all = [blob[int(o):int(o + l)].tobytes() for o, l in zip(off, ln)]
+
+    def kernel_ms(raws, no_pm=False):
+        if no_pm:
+            cl = [divans_b200.ir_to_cmds("window 22 0 0 0\ninsert %d %s\n" % (len(r), r.hex()))[0] for r in raws]
+            streams = eng.encode(cl, divans_b200.encode_options(), cmds=True)
+        else:
+            streams = eng.encode(raws, divans_b200.encode_options())
+        caps = [len(r) + 64 for r in raws]
+        ms = []
+        for _ in range(4):
+            res = eng.decode(streams, caps)
+            ms.append(eng.last_main_kernel_ms())
+        ok = all(st == 0 and out == r for (st, out), r in zip(res, raws))
+        return float(np.median(ms[1:])), min(ms[1:]), max(ms[1:]), ok
+
+    for n in sizes:
+        full = full_all[:n]
+        fm, fmin, fmax, fok = kernel_ms(full)
+        pm, pmin, pmax, pok = kernel_ms([r[:16] for r in full])
+        nm, nmin, nmax, nok = kernel_ms([r[:16] for r in full], no_pm=True)
+        print("streams %5d  lanes %2d  64 KiB decode kernel %8.3f ms (min %8.3f max %8.3f)  16 B decode kernel %7.3f ms "
+              "(min %7.3f max %7.3f)  prelude share %5.1f %%  16 B without PredictionMode %7.3f ms (min %7.3f max %7.3f)  ok=%s/%s/%s"
+              % (n, eng.last_lanes(), fm, fmin, fmax, pm, pmin, pmax, 100.0 * pm / fm, nm, nmin, nmax, fok, pok, nok), flush=True)
+    eng.close()
+
+
+for mode, default, fn in (("--sweep", "132,528,1056,2112,4224", sweep), ("--prelude", "132,1056,4096,4224", prelude)):
+    if mode in sys.argv:
+        i = sys.argv.index(mode)
+        spec = sys.argv[i + 1] if i + 1 < len(sys.argv) and not sys.argv[i + 1].startswith("--") else default
+        fn([int(x) for x in spec.split(",")])
+        sys.exit(0)
 
 def run(name, raws, opts, eng, cmds=None):
     streams = eng.encode(cmds if cmds is not None else raws, opts, cmds=cmds is not None)
