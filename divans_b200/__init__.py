@@ -42,8 +42,9 @@ BATCH_SYMBOLS = [
     "divans_b200_synchronize", "divans_b200_encode_options_default", "divans_b200_encode_batch_host",
     "divans_b200_encode_cmds_batch_host", "divans_b200_encode_batch_device", "divans_b200_ir_to_cmds",
     "divans_b200_decode_batch_host_async", "divans_b200_decode_batch_host_wait", "divans_b200_lz77_cmds_batch", "divans_b200_kernel_version", "divans_b200_last_lanes",
-    "divans_b200_debug_slot_header",
+    "divans_b200_debug_slot_header", "divans_b200_decode_cmds_batch_host", "divans_b200_decode_cmds_batch_device",
 ]
+PM_RECORD_BYTES = 32 + 16384 + 1024 + 8192   # one prediction-mode record of a DVCL blob (include/divans_b200.h)
 
 
 class DivansError(RuntimeError):
@@ -103,6 +104,10 @@ def load_library():
     L.divans_b200_decode_batch_host_wait.restype = ctypes.c_uint8
     L.divans_b200_decode_batch_device.argtypes = batch + [ctypes.c_uint64, ctypes.c_uint32, vp]
     L.divans_b200_decode_batch_device.restype = ctypes.c_uint8
+    L.divans_b200_decode_cmds_batch_host.argtypes = batch[:-2] + [vp, vp, vp, vp, vp, vp, ctypes.c_uint32]
+    L.divans_b200_decode_cmds_batch_host.restype = ctypes.c_uint8
+    L.divans_b200_decode_cmds_batch_device.argtypes = batch[:-2] + [vp, vp, vp, vp, vp, vp, ctypes.c_uint64, ctypes.c_uint32, vp]
+    L.divans_b200_decode_cmds_batch_device.restype = ctypes.c_uint8
     L.divans_b200_encode_options_default.argtypes = [ctypes.POINTER(EncodeOptions)]
     L.divans_b200_encode_batch_host.argtypes = batch + [ctypes.POINTER(EncodeOptions)]
     L.divans_b200_encode_batch_host.restype = ctypes.c_uint8
@@ -321,6 +326,95 @@ class Engine:
         out = np.zeros(int(opad.sum()) + 256, np.uint8)
         out_len, status = self.decode_batch_host(blob, in_off, in_len, out, out_off, out_cap, flags)
         return [(int(st), out[int(o):int(o) + int(n)].tobytes()) for st, o, n in zip(status, out_off, out_len)]
+
+    # -- decoding to command lists (DVCL blobs, include/divans_b200.h)
+    def decode_cmds_batch_host(self, in_blob, in_off, in_len, out, out_off, out_cap, blobs, blob_off, blob_cap, flags=0):
+        """decode_batch_host that also records every stream's command list into blobs[blob_off[i] .. +blob_cap[i]): returns
+        (out_len, blob_len, status).  Status 2 with blob_len > blob_cap: the blob region was too small, blob_len is the size it
+        needs (the stream was still decoded)."""
+        n = len(in_off)
+        in_off, in_len = np.ascontiguousarray(in_off, np.uint64), np.ascontiguousarray(in_len, np.uint64)
+        out_off, out_cap = np.ascontiguousarray(out_off, np.uint64), np.ascontiguousarray(out_cap, np.uint64)
+        blob_off, blob_cap = np.ascontiguousarray(blob_off, np.uint64), np.ascontiguousarray(blob_cap, np.uint64)
+        out_len, blob_len = np.zeros(n, np.uint64), np.zeros(n, np.uint64)
+        status = np.full(n, DIVANS_FAILURE, np.int32)
+        rc = self._L.divans_b200_decode_cmds_batch_host(self._h, n, _ptr(in_blob), _ptr(in_off), _ptr(in_len), _ptr(out), _ptr(out_off),
+                                                        _ptr(out_cap), _ptr(out_len), _ptr(blobs), _ptr(blob_off), _ptr(blob_cap),
+                                                        _ptr(blob_len), _ptr(status), flags)
+        if rc != DIVANS_SUCCESS:
+            raise DivansError("decode_cmds_batch_host: " + self._err())
+        return out_len, blob_len, status
+
+    def decode_cmds_batch_device(self, d_in, d_in_off, d_in_len, d_out, d_out_off, d_out_cap, d_out_len, d_blobs, d_blob_off, d_blob_cap,
+                                 d_blob_len, d_status, n, in_total_bytes, flags=0, stream=None):
+        """decode_cmds_batch_host with raw device pointers (ints).  Asynchronous, like decode_batch_device."""
+        rc = self._L.divans_b200_decode_cmds_batch_device(self._h, n, d_in, d_in_off, d_in_len, d_out, d_out_off, d_out_cap, d_out_len,
+                                                          d_blobs, d_blob_off, d_blob_cap, d_blob_len, d_status, int(in_total_bytes),
+                                                          flags, stream)
+        if rc != DIVANS_SUCCESS:
+            raise DivansError("decode_cmds_batch_device: " + self._err())
+
+    def decode_cmds(self, streams, out_caps, flags=0):
+        """Convenience: list of .divans bytes -> list of (status, decoded bytes, DVCL blob bytes).  A stream whose blob did not fit
+        the first guess is decoded once more with the exact size the first call reported."""
+        bufs = [_u8(s) for s in streams]
+        n = len(bufs)
+        in_len = np.array([b.size for b in bufs], np.uint64)
+        in_off = np.zeros(n, np.uint64)
+        pad = (in_len + np.uint64(15)) & ~np.uint64(15)
+        if n > 1:
+            in_off[1:] = np.cumsum(pad)[:-1]
+        blob = np.zeros(int(pad.sum()) + 16, np.uint8)
+        for b, o in zip(bufs, in_off):
+            blob[int(o):int(o) + b.size] = b
+        out_cap = np.array(out_caps, np.uint64).reshape(n)
+        # first guess: header, one prediction-mode record, every byte a literal byte plus a few commands per 64 bytes
+        blob_cap = np.uint64(32 + PM_RECORD_BYTES + 4096) + out_cap + out_cap // np.uint64(4)
+        res = [None] * n
+        todo = np.arange(n)
+        for attempt in range(2):
+            idx = todo
+            opad = (out_cap[idx] + np.uint64(255)) & ~np.uint64(255)
+            bpad = (blob_cap[idx] + np.uint64(255)) & ~np.uint64(255)
+            out_off, blob_off = np.zeros(len(idx), np.uint64), np.zeros(len(idx), np.uint64)
+            if len(idx) > 1:
+                out_off[1:], blob_off[1:] = np.cumsum(opad)[:-1], np.cumsum(bpad)[:-1]
+            out = np.zeros(int(opad.sum()) + 256, np.uint8)
+            blobs = np.zeros(int(bpad.sum()) + 256, np.uint8)
+            out_len, blob_len, status = self.decode_cmds_batch_host(blob, in_off[idx], in_len[idx], out, out_off, out_cap[idx], blobs,
+                                                                   blob_off, blob_cap[idx], flags)
+            retry = []
+            for k, i in enumerate(idx):
+                if status[k] == DIVANS_NEEDS_MORE_OUTPUT and blob_len[k] > blob_cap[i] and attempt == 0:
+                    blob_cap[i] = blob_len[k]
+                    retry.append(i)
+                    continue
+                raw = out[int(out_off[k]):int(out_off[k]) + int(out_len[k])].tobytes()
+                res[i] = (int(status[k]), raw, blobs[int(blob_off[k]):int(blob_off[k]) + int(blob_len[k])].tobytes() if status[k] == 0 else b"")
+            if not retry:
+                break
+            todo = np.array(retry)
+        return res
+
+    def transcode(self, streams, out_caps, opts=None, flags=0):
+        """Re-encode .divans streams under other entropy options: decode_cmds (``flags`` as for decode: the model and revision the
+        streams were written with), then encode(..., cmds=True) with ``opts`` (encode_options; a window_size of 0, the
+        default when ``opts`` is None, keeps each stream's own window).  Returns the new streams; raises DivansError naming the
+        first stream that does not decode."""
+        dec = self.decode_cmds(streams, out_caps, flags)
+        for i, (st, _, _) in enumerate(dec):
+            if st != DIVANS_SUCCESS:
+                raise DivansError("transcode: stream %d does not decode (status %d)" % (i, st))
+        o = opts if opts is not None else encode_options(window_size=0)
+        wins = [int(np.frombuffer(b[20:24], np.uint32)[0]) if o.window_size == 0 else int(o.window_size) for _, _, b in dec]
+        res = [None] * len(dec)
+        for w in sorted(set(wins)):
+            idx = [i for i, x in enumerate(wins) if x == w]
+            ow = EncodeOptions.from_buffer_copy(o)
+            ow.window_size = w
+            for i, e in zip(idx, self.encode([dec[i][2] for i in idx], ow, cmds=True)):
+                res[i] = e
+        return res
 
     def encode_batch_host(self, in_blob, in_off, in_len, out, out_off, out_cap, opts=None, cmds=False):
         n = len(in_off)

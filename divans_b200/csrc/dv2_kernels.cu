@@ -10,8 +10,10 @@ constexpr int DEC2_MIN_BLOCKS = 16;             // 4 one-warp blocks per schedul
                                                 // 16-lane streams per SM (4224 on an H100's 132 SMs).  (144 registers = 3 per partition = 12 per
                                                 // SM: 3168 resident 16-lane streams, a second wave for 4096)
 
-template <int LPG>
-__global__ void __launch_bounds__(DEC2_BLOCK_THREADS, DEC2_MIN_BLOCKS) decode_kernel_v2(DecodeParams p) {
+// The kernel body; REC = the recording decoder (decode to command lists, dv_engine_kernel.cuh): the same loop, which in
+// addition hands each stream its blob region and reports what it recorded.
+template <int LPG, bool REC>
+__device__ __forceinline__ void decode_v2(const DecodeParams p, const RecParams r) {
     extern __shared__ __align__(16) uint8_t smem[];
     const int lane = threadIdx.x & 31;
     const int warp_in_block = threadIdx.x >> 5;
@@ -88,6 +90,11 @@ __global__ void __launch_bounds__(DEC2_BLOCK_THREADS, DEC2_MIN_BLOCKS) decode_ke
                     s.c->gen_ctr = ctr; s.gen = ctr & 0xffffu;
                     coder_init_dec(s.cur, reinterpret_cast<const uint32_t *>(pl), pay0 >> 2);   // command stream (CMD_CODER, codec/interface.rs:49)
                     coder_init_dec(s.c->oth, reinterpret_cast<const uint32_t *>(pl + (((uint64_t)pay0 + 15) & ~15ull)), pay1 >> 2);   // literal stream (LIT_CODER, :50)
+                    if (REC) {
+                        s.c->rec.blob = r.blobs + r.blob_off[v];
+                        s.c->rec.cap = r.blob_cap[v] > 0xffffffffull ? 0xffffffffu : (uint32_t)r.blob_cap[v];
+                        s.c->rec.n_cmds = 0; s.c->rec.n_pms = 0; s.c->rec.n_lits = 0;
+                    }
                     enter_cmd_type<false>(s, nx);
                 }
             }
@@ -107,6 +114,10 @@ __global__ void __launch_bounds__(DEC2_BLOCK_THREADS, DEC2_MIN_BLOCKS) decode_ke
                 if (lit && s.lit_left == 0 && s.status == ST_OK) { swap_coders(s, g); enter_cmd_type<false>(s, nx); }
                 if (s.status != ST_OK) {
                     if (g.store0) { p.out_len[s.c->sidx] = s.out_pos; p.status[s.c->sidx] = s.status; }
+                    if (REC && g.store0) {
+                        uint32_t *cnt = r.counts + 3 * (size_t)s.c->sidx;
+                        cnt[0] = s.c->rec.n_cmds; cnt[1] = s.c->rec.n_pms; cnt[2] = s.c->rec.n_lits;
+                    }
                     s.state = S_IDLE; s.status = ST_OK;
                     nx.cdf = A_misc(s, MI_DUMMY); nx.cdf2 = nullptr; nx.speed = SPK_NONE; nx.tagged = false;
                     coder_init_dec(s.cur, nullptr, 0); s.cur.need_a = 0;
@@ -120,10 +131,14 @@ __global__ void __launch_bounds__(DEC2_BLOCK_THREADS, DEC2_MIN_BLOCKS) decode_ke
         // ---- per-group scalar state machines (divergent) ----
         if (busy) {
             if (s.cur.underflow) s.status = ST_NEED_INPUT;
-            else transition<false, true>(s, nx, g, sym);
+            else transition<false, true, REC>(s, nx, g, sym);
             if (s.status != ST_OK || s.state == S_IDLE) {
                 if (s.status == ST_OK && s.c->oth.underflow) s.status = ST_NEED_INPUT;
                 if (g.store0) { p.out_len[s.c->sidx] = s.out_pos; p.status[s.c->sidx] = s.status; }
+                if (REC && g.store0) {
+                    uint32_t *cnt = r.counts + 3 * (size_t)s.c->sidx;
+                    cnt[0] = s.c->rec.n_cmds; cnt[1] = s.c->rec.n_pms; cnt[2] = s.c->rec.n_lits;
+                }
                 s.state = S_IDLE; s.status = ST_OK;
                 nx.cdf = A_misc(s, MI_DUMMY); nx.cdf2 = nullptr; nx.speed = SPK_NONE; nx.tagged = false;
                 coder_init_dec(s.cur, nullptr, 0); s.cur.need_a = 0;
@@ -132,6 +147,10 @@ __global__ void __launch_bounds__(DEC2_BLOCK_THREADS, DEC2_MIN_BLOCKS) decode_ke
     }
     if (g.store0) *reinterpret_cast<uint32_t *>(s.slot + OFF_HDR) = s.c->gen_ctr;
 }
+template <int LPG>
+__global__ void __launch_bounds__(DEC2_BLOCK_THREADS, DEC2_MIN_BLOCKS) decode_kernel_v2(DecodeParams p) { decode_v2<LPG, false>(p, RecParams{}); }
+// recording decoder: 16 lanes per stream only
+__global__ void __launch_bounds__(DEC2_BLOCK_THREADS, DEC2_MIN_BLOCKS) decode_kernel_v2_rec(DecodeParams p, RecParams r) { decode_v2<16, true>(p, r); }
 
 // per block: the groups' cold state, 16 lanes per stream their T2S
 template <int LPG> static size_t smem_v2() {
@@ -143,6 +162,9 @@ template <int LPG> static void launch_v2(const DecodeParams &p, uint32_t n_block
 template <int LPG> static int max_blocks_v2() { return stream_kernel_blocks_per_sm(decode_kernel_v2<LPG>, DEC2_BLOCK_THREADS, smem_v2<LPG>()); }
 void launch_decode_v2(int lanes_per_stream, const DecodeParams &p, uint32_t n_blocks, cudaStream_t st) {
     if (lanes_per_stream == 8) launch_v2<8>(p, n_blocks, st); else launch_v2<16>(p, n_blocks, st);
+}
+void launch_decode_v2_rec(const DecodeParams &p, const RecParams &r, uint32_t n_blocks, cudaStream_t st) {
+    decode_kernel_v2_rec<<<n_blocks, DEC2_BLOCK_THREADS, smem_v2<16>(), st>>>(p, r);
 }
 int decode_max_blocks_per_sm_v2(int lanes_per_stream) { return lanes_per_stream == 8 ? max_blocks_v2<8>() : max_blocks_v2<16>(); }
 int decode_groups_per_block_v2(int lanes_per_stream) { return DEC2_BLOCK_THREADS / lanes_per_stream; }

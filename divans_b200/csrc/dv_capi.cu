@@ -49,7 +49,9 @@ struct divans_b200_ctx {
     uint8_t *d_payload = nullptr; size_t payload_cap = 0;
     uint8_t *d_in = nullptr; size_t d_in_cap = 0;
     uint8_t *d_out = nullptr; size_t d_out_cap = 0;
-    uint64_t *d_meta = nullptr; size_t d_meta_cap = 0;   // in_off,in_len,out_off,out_cap,out_len (+status)
+    uint64_t *d_meta = nullptr; size_t d_meta_cap = 0;   // in_off,in_len,out_off,out_cap,out_len (+status; decode_cmds: + blob_off,blob_cap,blob_len)
+    uint8_t *d_blobs = nullptr; size_t d_blobs_cap = 0;   // decode_cmds_batch_host: the DVCL blob regions
+    uint32_t *d_rec_counts = nullptr; size_t rec_counts_cap = 0;   // decode_cmds: per stream [3] what the recording decoder counted
     // pipelined host API (decode_batch_host_async): two batches in flight, copies on their own streams
     struct Lane {
         uint8_t *d_in = nullptr; size_t d_in_cap = 0;
@@ -157,6 +159,7 @@ extern "C" void divans_b200_destroy(divans_b200_ctx *ctx) {
     if (ctx->s_d2h) cudaStreamSynchronize(ctx->s_d2h);
     cudaFree(ctx->d_arena_raw); cudaFree(ctx->d_tables); cudaFree(ctx->d_counter); cudaFree(ctx->d_nibbles);
     cudaFree(ctx->d_frame); cudaFree(ctx->d_payload); cudaFree(ctx->d_in); cudaFree(ctx->d_out); cudaFree(ctx->d_meta);
+    cudaFree(ctx->d_blobs); cudaFree(ctx->d_rec_counts);
     if (ctx->ev0) cudaEventDestroy(ctx->ev0);
     if (ctx->ev1) cudaEventDestroy(ctx->ev1);
     if (ctx->evm) cudaEventDestroy(ctx->evm);
@@ -223,10 +226,11 @@ static DivansResult ensure_arena(divans_b200_ctx *ctx, size_t slots) {
 // One context = one set of scratch buffers (work counter, frame table, compacted payload, arena slots, timing events):
 // launches of different calls must not overlap on the GPU.  Calls are serialised on the host by ctx->mu and on the device
 // by `ev_busy`: a launch set on any stream first waits for the previous call's last kernel.
+// `rec` (decode to command lists): the recording decoder on 16 lanes per stream, then the pack kernel that finishes the blobs.
 static DivansResult decode_device_nolock(divans_b200_ctx *ctx, size_t n, const uint8_t *d_in, const uint64_t *d_in_off,
                                          const uint64_t *d_in_len, uint8_t *d_out, const uint64_t *d_out_off,
                                          const uint64_t *d_out_cap, uint64_t *d_out_len, int32_t *d_status,
-                                         uint64_t in_total_bytes, uint32_t flags, void *cuda_stream) {
+                                         uint64_t in_total_bytes, uint32_t flags, void *cuda_stream, const RecParams *rec = nullptr) {
     if (n > 0xffffffffull) { ctx->err = "too many streams"; return DIVANS_FAILURE; }
     CK(cudaSetDevice(ctx->device));
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream;
@@ -246,6 +250,7 @@ static DivansResult decode_device_nolock(divans_b200_ctx *ctx, size_t n, const u
             const uint64_t passes16 = (n + ctx->cap16 - 1) / ctx->cap16, passes8 = (n + ctx->cap8 - 1) / ctx->cap8;
             lanes = passes8 < passes16 ? 8 : 16;
         }
+        if (rec) lanes = 16;   // the recording decoder has the 16-lane layout only
         gpb = (uint32_t)decode_groups_per_block_v2(lanes); cap = lanes == 16 ? ctx->cap16 : ctx->cap8;
     }
     ctx->last_lanes = lanes;
@@ -255,6 +260,12 @@ static DivansResult decode_device_nolock(divans_b200_ctx *ctx, size_t n, const u
     if (!grow(ctx, &ctx->d_frame, &ctx->frame_cap, 4 * n)) return DIVANS_FAILURE;
     if (!grow(ctx, &ctx->d_payload, &ctx->payload_cap, (size_t)in_total_bytes + 48 * n + 64)) return DIVANS_FAILURE;
     CK(cudaMemsetAsync(ctx->d_counter, 0, 4, st));
+    RecParams rp;
+    if (rec) {
+        if (!grow(ctx, &ctx->d_rec_counts, &ctx->rec_counts_cap, 3 * n)) return DIVANS_FAILURE;
+        rp = *rec; rp.counts = ctx->d_rec_counts;
+        CK(cudaMemsetAsync(rp.counts, 0, 12 * n, st));   // (the pack kernel reads zeros for streams the decoder never started)
+    }
     FrameParams fp;
     fp.in = d_in; fp.in_off = d_in_off; fp.in_len = d_in_len; fp.frame = ctx->d_frame; fp.status = d_status;
     fp.n_streams = (uint32_t)n; fp.flags = flags;
@@ -269,12 +280,16 @@ static DivansResult decode_device_nolock(divans_b200_ctx *ctx, size_t n, const u
     launch_frame(fp, ctx->d_payload, (uint64_t)ctx->payload_cap, st);
     if (dbg) { CK(cudaStreamSynchronize(st)); fprintf(stderr, "divans_b200[debug]: frame kernel ok (n=%zu)\n", n); }
     CK(cudaEventRecord(ctx->evm, st));
-    if (!skip_decode) { if (blend) launch_decode16_blend(dp, blocks, st); else launch_decode_v2(lanes, dp, blocks, st); }
+    if (rec) {
+        if (blend) launch_decode16_blend_rec(dp, rp, blocks, st); else launch_decode_v2_rec(dp, rp, blocks, st);
+        CK(cudaEventRecord(ctx->evm1, st));
+        launch_pack_cmds(dp, rp, st);
+    } else if (!skip_decode) { if (blend) launch_decode16_blend(dp, blocks, st); else launch_decode_v2(lanes, dp, blocks, st); }
     if (dbg) { CK(cudaStreamSynchronize(st)); fprintf(stderr, "divans_b200[debug]: decode kernel ok (blocks=%u, lps=%d)\n", blocks, ctx->lanes_per_stream); }
     CK(cudaEventRecord(ctx->ev1, st));
     CK(cudaEventRecord(ctx->ev_busy, st)); ctx->busy_recorded = true;
-    ctx->main_end_is_evm1 = false;
-    ctx->launches += skip_decode ? 3 : 4;
+    ctx->main_end_is_evm1 = rec != nullptr;
+    ctx->launches += rec ? 5 : skip_decode ? 3 : 4;
     CK(cudaGetLastError());
     return DIVANS_SUCCESS;
 }
@@ -329,6 +344,78 @@ extern "C" DivansResult divans_b200_decode_batch_host(divans_b200_ctx *ctx, size
         if (hi > lo) CK(cudaMemcpyAsync(out + lo, ctx->d_out + lo, hi - lo, cudaMemcpyDeviceToHost, st));
         i = j;
     }
+    CK(cudaStreamSynchronize(st));
+    return DIVANS_SUCCESS;
+}
+
+// ---- decode to command lists ----
+extern "C" DivansResult divans_b200_decode_cmds_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_in, const uint64_t *d_in_off,
+                                                             const uint64_t *d_in_len, uint8_t *d_out, const uint64_t *d_out_off,
+                                                             const uint64_t *d_out_cap, uint64_t *d_out_len, uint8_t *d_blobs,
+                                                             const uint64_t *d_blob_off, const uint64_t *d_blob_cap, uint64_t *d_blob_len,
+                                                             int32_t *d_status, uint64_t in_total_bytes, uint32_t flags, void *cuda_stream) {
+    if (!ctx) return DIVANS_FAILURE;
+    if (n == 0) return DIVANS_SUCCESS;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    RecParams rp;
+    rp.blobs = d_blobs; rp.blob_off = d_blob_off; rp.blob_cap = d_blob_cap; rp.blob_len = d_blob_len; rp.counts = nullptr;
+    return decode_device_nolock(ctx, n, d_in, d_in_off, d_in_len, d_out, d_out_off, d_out_cap, d_out_len, d_status, in_total_bytes, flags,
+                                cuda_stream, &rp);
+}
+// D2H of whole regions base[off[i] .. +cap[i]), one transfer per run of exactly adjacent regions: nothing outside them is written
+static DivansResult copy_regions_back(divans_b200_ctx *ctx, size_t n, uint8_t *dst, const uint8_t *src, const uint64_t *off,
+                                      const uint64_t *cap, cudaStream_t st) {
+    for (size_t i = 0; i < n;) {
+        const uint64_t lo = off[i]; uint64_t hi = lo + cap[i];
+        size_t j = i + 1;
+        while (j < n && off[j] == hi) { hi += cap[j]; j++; }
+        if (hi > lo) CK(cudaMemcpyAsync(dst + lo, src + lo, hi - lo, cudaMemcpyDeviceToHost, st));
+        i = j;
+    }
+    return DIVANS_SUCCESS;
+}
+extern "C" DivansResult divans_b200_decode_cmds_batch_host(divans_b200_ctx *ctx, size_t n, const uint8_t *in, const uint64_t *in_off,
+                                                           const uint64_t *in_len, uint8_t *out, const uint64_t *out_off,
+                                                           const uint64_t *out_cap, uint64_t *out_len, uint8_t *blobs,
+                                                           const uint64_t *blob_off, const uint64_t *blob_cap, uint64_t *blob_len,
+                                                           int32_t *status, uint32_t flags) {
+    if (!ctx) return DIVANS_FAILURE;
+    if (n == 0) return DIVANS_SUCCESS;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    CK(cudaSetDevice(ctx->device));
+    uint64_t in_end = 0, out_end = 0, blob_end = 0, in_sum = 0;
+    for (size_t i = 0; i < n; i++) {
+        in_end = std::max(in_end, in_off[i] + in_len[i]);
+        out_end = std::max(out_end, out_off[i] + out_cap[i]);
+        blob_end = std::max(blob_end, blob_off[i] + blob_cap[i]);
+        in_sum += in_len[i];
+    }
+    if (!grow(ctx, &ctx->d_in, &ctx->d_in_cap, (size_t)in_end + 64)) return DIVANS_FAILURE;
+    if (!grow(ctx, &ctx->d_out, &ctx->d_out_cap, (size_t)out_end + 64)) return DIVANS_FAILURE;
+    if (!grow(ctx, &ctx->d_blobs, &ctx->d_blobs_cap, (size_t)blob_end + 64)) return DIVANS_FAILURE;
+    if (!grow(ctx, &ctx->d_meta, &ctx->d_meta_cap, n * 9)) return DIVANS_FAILURE;
+    uint64_t *m = ctx->d_meta;   // in_off, in_len, out_off, out_cap, out_len, status, blob_off, blob_cap, blob_len
+    cudaStream_t st = ctx->stream;
+    CK(cudaMemcpyAsync(ctx->d_in, in, in_end, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(m, in_off, n * 8, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(m + n, in_len, n * 8, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(m + 2 * n, out_off, n * 8, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(m + 3 * n, out_cap, n * 8, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(m + 6 * n, blob_off, n * 8, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(m + 7 * n, blob_cap, n * 8, cudaMemcpyHostToDevice, st));
+    int32_t *d_status = reinterpret_cast<int32_t *>(m + 5 * n);
+    CK(cudaMemsetAsync(ctx->d_out, 0, out_end, st));      // the regions are copied back whole: zeros past the lengths
+    CK(cudaMemsetAsync(ctx->d_blobs, 0, blob_end, st));
+    RecParams rp;
+    rp.blobs = ctx->d_blobs; rp.blob_off = m + 6 * n; rp.blob_cap = m + 7 * n; rp.blob_len = m + 8 * n; rp.counts = nullptr;
+    DivansResult r = decode_device_nolock(ctx, n, ctx->d_in, m, m + n, ctx->d_out, m + 2 * n, m + 3 * n, m + 4 * n, d_status,
+                                          in_sum > in_end ? in_sum : in_end, flags, st, &rp);
+    if (r != DIVANS_SUCCESS) return r;
+    CK(cudaMemcpyAsync(out_len, m + 4 * n, n * 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(blob_len, m + 8 * n, n * 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(status, d_status, n * 4, cudaMemcpyDeviceToHost, st));
+    if (copy_regions_back(ctx, n, out, ctx->d_out, out_off, out_cap, st) != DIVANS_SUCCESS) return DIVANS_FAILURE;
+    if (copy_regions_back(ctx, n, blobs, ctx->d_blobs, blob_off, blob_cap, st) != DIVANS_SUCCESS) return DIVANS_FAILURE;
     CK(cudaStreamSynchronize(st));
     return DIVANS_SUCCESS;
 }

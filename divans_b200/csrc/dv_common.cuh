@@ -120,6 +120,15 @@ struct DecodeParams {
     uint32_t model_rev;         // 0 = the reference tree as mounted; 1 = DIVANS_B200_MODEL_WASM_2018 (include/divans_b200.h)
 };
 
+// Decoding to command lists: the recording decoder writes each stream's records into its blob region and counts them, the pack
+// kernel turns that into the stream's DVCL blob (include/divans_b200.h).
+struct RecParams {
+    uint8_t *blobs;
+    const uint64_t *blob_off, *blob_cap;
+    uint64_t *blob_len;
+    uint32_t *counts;           // per stream [3]: commands, prediction-mode records, literal bytes
+};
+
 struct FrameParams {
     const uint8_t *in;
     const uint64_t *in_off, *in_len;

@@ -68,6 +68,16 @@ struct CmdIn {
     const uint8_t *pms;      // prediction mode records (32 + 16384 + 1024 + 8192 each)
     const uint8_t *lits;     // literal pool
 };
+// recording decoder output: the DVCL blob region of the stream being decoded.  Command records grow forward from byte 32,
+// prediction-mode records backward from the region's end; a record is written only while both ends stay apart, but every
+// record is counted, so the pack kernel (dv_kernels.cu) knows the exact size the blob needs either way.
+struct RecOut {
+    uint8_t *blob;
+    uint32_t cap;                            // region bytes (capped at 4 GiB - 1)
+    uint32_t n_cmds, n_pms, n_lits;          // records so far; literal bytes so far
+    uint32_t lit_map_len, dist_map_len;      // the index at which each map's mnemonic 14 arrived (PredictionMode in flight)
+};
+static_assert(sizeof(RecOut) <= sizeof(CmdIn) && alignof(RecOut) <= alignof(CmdIn), "RecOut shares CmdIn's storage");
 
 // Per-stream state, split by temperature.
 //  * Cold: everything only the command interpreter touches -- lives in SHARED memory (one struct per lane-group; every
@@ -98,8 +108,8 @@ struct Cold {
     bool lit_quirk;                          // v2 engine: the literal began within 8 bytes of the ring start (last_8_literals is not a plain mirror of the output)
     bool pm_seen;                            // a PredictionMode command of THIS stream has written the mixing mask
     bool t2_dirty;                           // v2 engine: the slot's context table (OFF_T2) does not match lcm / mode / block type
-    // encoder
-    CmdIn in;
+    // encoder input, or the recording decoder's output (a decoder never reads `in`)
+    union { CmdIn in; RecOut rec; };
     uint32_t e0, e1, e2, e3;                 // current input command fields
     uint32_t desired_context_mixing, desired_prior_depth, desired_force_stride;
     bool desired_do_context_map, have_desired_adapt;

@@ -117,9 +117,58 @@ __device__ __forceinline__ void swap_coders(St &s, const G2 g) {
     s.cur = parked;
 }
 
-template <bool ENC, bool V2 = false>
+// ---- recording decoder (REC): one DVCL record per command (include/divans_b200.h), the values the encoder reads back from
+// it (load_cmd, pm_rec), written where the decoder resolves them.  A literal's `a` holds the output position of its bytes
+// until the pack kernel (dv_kernels.cu) gathers them into the literal pool.
+__device__ __forceinline__ void st_le32(uint8_t *p, uint32_t v) {   // blob regions may start at any byte
+    p[0] = (uint8_t)v; p[1] = (uint8_t)(v >> 8); p[2] = (uint8_t)(v >> 16); p[3] = (uint8_t)(v >> 24);
+}
+template <bool REC>
+__device__ __forceinline__ void rec_cmd(St &s, const G2 g, uint32_t type, uint32_t a, uint32_t b, uint32_t c = 0, uint32_t d = 0) {
+    if (!REC) return;
+    RecOut &r = s.c->rec;
+    const uint32_t k = r.n_cmds;
+    if (g.store0 && 32ull + 20ull * (k + 1ull) + (uint64_t)PM_RECORD_BYTES * r.n_pms <= r.cap) {
+        uint8_t *p = r.blob + 32 + 20ull * k;
+        st_le32(p, type); st_le32(p + 4, a); st_le32(p + 8, b); st_le32(p + 12, c); st_le32(p + 16, d);
+    }
+    r.n_cmds = k + 1;
+}
+// The PredictionMode record of a decoded command: mode, has_speeds, the three speed pairs from the coded f8 bytes (`f8`
+// byte 2k + j = pair k, element j; the stride and combined speeds are the same pairs), both maps with zeros past their
+// lengths, the 8192 mixing values.  The group's lanes copy it out of the slot.
+static __device__ __noinline__ void rec_predmode(const G2 g, const uint8_t *slot, uint8_t *dst, uint32_t pred_mode, unsigned long long f8,
+                                                 uint32_t lit_len, uint32_t dist_len) {
+    __syncwarp(g.gmask);   // the last mixing value, written by the group's store lane
+    for (uint32_t i = (uint32_t)g.l16; i < 32; i += (uint32_t)g.nl) {
+        uint32_t v;
+        if (i < 4) v = i == 0 ? pred_mode : i == 2 ? 1u : 0u;
+        else if (i < 28) {
+            const uint32_t w = (i - 4) >> 1, pair = w < 4 ? w + 4 : (w - 4) & 3;   // cm_speed[2][2], stride_speed, combined_speed
+            v = u8_to_speed_u16((uint32_t)(f8 >> (8 * pair)) & 0xffu) >> (8 * (i & 1));
+        } else v = (i < 30 ? lit_len : dist_len) >> (8 * (i & 1));
+        dst[i] = (uint8_t)v;
+    }
+    for (uint32_t i = (uint32_t)g.l16; i < 16384; i += (uint32_t)g.nl) dst[32 + i] = i < lit_len ? slot[OFF_LCM + i] : (uint8_t)0;
+    for (uint32_t i = (uint32_t)g.l16; i < 1024; i += (uint32_t)g.nl) dst[32 + 16384 + i] = i < dist_len ? slot[OFF_DCM + i] : (uint8_t)0;
+    for (uint32_t i = (uint32_t)g.l16; i < 8192; i += (uint32_t)g.nl) dst[32 + 16384 + 1024 + i] = slot[OFF_MIX + i];
+    __syncwarp(g.gmask);
+}
+template <bool REC>
+__device__ __forceinline__ void rec_pm(St &s, const G2 g) {
+    if (!REC) return;
+    RecOut &r = s.c->rec;
+    const uint32_t j = r.n_pms;
+    rec_cmd<REC>(s, g, 7, j, 0);
+    if (32ull + 20ull * r.n_cmds + (uint64_t)PM_RECORD_BYTES * (j + 1ull) <= r.cap)
+        rec_predmode(g, s.slot, r.blob + r.cap - (size_t)PM_RECORD_BYTES * (j + 1), s.f0, s.l8, r.lit_map_len, r.dist_map_len);
+    r.n_pms = j + 1;
+}
+
+template <bool ENC, bool V2 = false, bool REC = false>
 __device__ __forceinline__ void start_literal(St &s, Next &nx, const G2 g, uint32_t len) {
     if ((uint64_t)len > (uint64_t)(s.c->out_cap - s.out_pos)) { s.status = ST_NEED_OUTPUT; return; }
+    if (REC) { rec_cmd<REC>(s, g, 3, s.out_pos, len, s.f3); s.c->rec.n_lits += len; }
     if (!s.c->lit_slabs_ready) {
         if (V2 && !s.c->pm_seen) v2_mix_before_use(g, s.slot);   // no PredictionMode command yet: the mask must read as zeros
         // v2 engine: literal priors carry generation tags and read as the default CDF until first written: nothing to initialise
@@ -226,13 +275,14 @@ template <bool ENC> __device__ __forceinline__ void enter_bt_mnemonic(St &s, Nex
     set_next<ENC>(nx, A_misc(s, MI_BTYPE + BT_MNEMONIC + which), SPK_SLOW, varint);
 }
 // returns true when the block switch is complete (the caller's common tail fetches the next command)
-template <bool ENC> __device__ __forceinline__ bool bt_done(St &s, Next &nx, uint32_t bt) {
+template <bool ENC, bool REC = false> __device__ __forceinline__ bool bt_done(St &s, Next &nx, const G2 g, uint32_t bt) {
     if (s.f0 == 0) {
         s.f1 = bt; s.state = S_BT_STRIDE;
         set_next<ENC>(nx, A_misc(s, MI_BTYPE + BT_STRIDE), SPK_SLOW, (int)(s.c->desired_force_stride == 9 ? (s.c->e1 & 0xf) : s.c->desired_force_stride));
         return false;
     }
     obs_btype(s, (int)s.f0, bt);
+    rec_cmd<REC>(s, g, 4 + s.f0, bt, 0);
     return true;
 }
 template <bool ENC> __device__ __forceinline__ const uint8_t *pm_rec(const St &s) { return s.c->in.pms + (size_t)s.c->e0 * (32 + 16384 + 1024 + 8192); }
@@ -291,7 +341,7 @@ template <bool ENC> __device__ __forceinline__ void pm_map_store(St &s, Next &nx
 }
 
 // The transition: consume the nibble just coded in state s.state, perform its side effects, choose the next prior.
-template <bool ENC, bool V2 = false>
+template <bool ENC, bool V2 = false, bool REC = false>
 __device__ __forceinline__ void transition(St &s, Next &nx, const G2 g, int nib) {
     // Two tails are shared by all states (one copy of their code keeps the kernel inside the instruction cache when the
     // streams of a batch are in different states): 1 = the command is complete, fetch the next one; 2 = a literal of tail_len bytes begins.
@@ -342,6 +392,7 @@ __device__ __forceinline__ void transition(St &s, Next &nx, const G2 g, int nib)
             uint32_t len = s.f0;
             if (dist == 0 || dist >= s.c->ring_len) { s.status = ST_FAIL; return; }   // DistanceGreaterRingBuffer & friends
             if ((uint64_t)len > (uint64_t)(s.c->out_cap - s.out_pos)) { s.status = ST_NEED_OUTPUT; return; }
+            rec_cmd<REC>(s, g, 1, dist, len);
             replay_copy(g, s.out, s.out_pos, dist, len);
             s.out_pos += len;
             tail = 1;
@@ -446,6 +497,7 @@ __device__ __forceinline__ void transition(St &s, Next &nx, const G2 g, int nib)
         if (n < 0) { s.status = ST_FAIL; return; }
         __syncwarp(g.gmask);
         if ((uint64_t)n > (uint64_t)(s.c->out_cap - s.out_pos)) { s.status = ST_NEED_OUTPUT; return; }
+        rec_cmd<REC>(s, g, 2, s.f2, s.f0, tr, (uint32_t)n);
         for (int i = g.l16; i < n; i += g.nl) s.out[s.out_pos + i] = s.c->scratch[i];
         __syncwarp(g.gmask);
         s.out_pos += (uint32_t)n;
@@ -454,14 +506,14 @@ __device__ __forceinline__ void transition(St &s, Next &nx, const G2 g, int nib)
     // ---- block switches ----
     case S_BT_MNEMONIC: {
         int which = (int)s.f0;
-        if (nib == 0) tail = bt_done<ENC>(s, nx, BL(s, which, 1)) ? 1 : 0;
-        else if (nib == 1) tail = bt_done<ENC>(s, nx, (BMAX(s, which) + 1) & 0xff) ? 1 : 0;
-        else if (nib != 15) tail = bt_done<ENC>(s, nx, (uint32_t)nib - 2) ? 1 : 0;
+        if (nib == 0) tail = bt_done<ENC, REC>(s, nx, g, BL(s, which, 1)) ? 1 : 0;
+        else if (nib == 1) tail = bt_done<ENC, REC>(s, nx, g, (BMAX(s, which) + 1) & 0xff) ? 1 : 0;
+        else if (nib != 15) tail = bt_done<ENC, REC>(s, nx, g, (uint32_t)nib - 2) ? 1 : 0;
         else { s.state = S_BT_FIRST; set_next<ENC>(nx, A_misc(s, MI_BTYPE + BT_FIRST + which), SPK_SLOW, (int)(s.c->e0 & 0xf)); }
     } break;
     case S_BT_FIRST: { s.f1 = (uint32_t)nib; s.state = S_BT_SECOND; set_next<ENC>(nx, A_misc(s, MI_BTYPE + BT_SECOND + (int)s.f0), SPK_SLOW, (int)((s.c->e0 >> 4) & 0xf)); } break;
-    case S_BT_SECOND: tail = bt_done<ENC>(s, nx, ((uint32_t)nib << 4) | s.f1) ? 1 : 0; break;
-    case S_BT_STRIDE: { obs_btype(s, 0, s.f1); s.btype_last = s.f1; s.c->t2_dirty = true; tail = 1; } break;
+    case S_BT_SECOND: tail = bt_done<ENC, REC>(s, nx, g, ((uint32_t)nib << 4) | s.f1) ? 1 : 0; break;
+    case S_BT_STRIDE: { obs_btype(s, 0, s.f1); s.btype_last = s.f1; s.c->t2_dirty = true; rec_cmd<REC>(s, g, 4, s.f1, (uint32_t)nib); tail = 1; } break;
     // ---- prediction mode ----
     case S_PM_MODE: {
         s.f0 = (uint32_t)nib; s.state = S_PM_MIX;
@@ -483,8 +535,8 @@ __device__ __forceinline__ void transition(St &s, Next &nx, const G2 g, int nib)
     } break;
     case S_PM_MAP_MNEMONIC: {
         if (nib == 14) {
-            if (s.f2 == 0) { cmap_reset(s); s.f2 = 1; s.f1 = 0; enter_pm_map_mnemonic<ENC>(s, nx); }
-            else { s.f1 = 0; enter_pm_mixval<ENC>(s, nx); }
+            if (s.f2 == 0) { if (REC) s.c->rec.lit_map_len = s.f1; cmap_reset(s); s.f2 = 1; s.f1 = 0; enter_pm_map_mnemonic<ENC>(s, nx); }
+            else { if (REC) s.c->rec.dist_map_len = s.f1; s.f1 = 0; enter_pm_mixval<ENC>(s, nx); }
         } else if (nib == 15) {
             s.state = S_PM_MAP_FIRST;
             int sym = 0;
@@ -514,13 +566,14 @@ __device__ __forceinline__ void transition(St &s, Next &nx, const G2 g, int nib)
             if (V2 && !s.speeds_small && s.tagged) { v2_make_untagged(g, s.slot, s.gen); s.tagged = false; }
             if (!V2 && !s.speeds_small && g.store0) reinterpret_cast<uint32_t *>(s.slot + OFF_HDR)[1] = 1u;   // elements may use their sign bits: the v2 engine must wipe before trusting tags
             s.c->lit_slabs_ready = false; s.c->t2_dirty = true; s.c->pm_seen = true;
+            rec_pm<REC>(s, g);
             tail = 1;
         } else enter_pm_mixval<ENC>(s, nx);
     } break;
     default: s.status = ST_FAIL; break;
     }
     if (tail == 1) { if (ENC) s.c->in.pos++; enter_cmd_type<ENC>(s, nx); }
-    else if (tail == 2) start_literal<ENC, V2>(s, nx, g, tail_len);
+    else if (tail == 2) start_literal<ENC, V2, REC>(s, nx, g, tail_len);
 }
 
 // fresh book-keeping for a new stream (CrossCommandBookKeeping::new codec/interface.rs:348-402, LiteralBookKeeping::new :246-264)

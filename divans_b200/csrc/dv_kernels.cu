@@ -142,6 +142,86 @@ __global__ void __launch_bounds__(128) demux_kernel(FrameParams p, uint8_t *payl
     }
 }
 
+// pack kernel of the recording decoders (decode to command lists): one warp per stream turns what the decoder recorded into the
+// stream's DVCL blob (include/divans_b200.h).  The decoder left the command records at byte 32 (a literal's `a` = the output
+// position of its bytes) and prediction-mode record j at the region's end minus j + 1 records; counts[] says how many of each
+// and how many literal bytes.  The warp puts the prediction-mode records in order behind the commands, gathers the literal
+// bytes from the decoded output into the pool, rewrites each literal's `a` to its pool offset and writes the header.
+__device__ __forceinline__ uint32_t ld_le32(const uint8_t *p) {
+    return (uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24);
+}
+__global__ void __launch_bounds__(128) pack_cmds_kernel(DecodeParams p, RecParams r) {
+    const uint32_t sidx = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const uint32_t lane = threadIdx.x & 31;
+    if (sidx >= p.n_streams) return;
+    uint8_t *blob = r.blobs + r.blob_off[sidx];
+    const uint64_t cap = r.blob_cap[sidx];
+    const uint32_t *cnt = r.counts + 3 * (size_t)sidx;   // (zeros for a stream the decoder never started)
+    const uint32_t nc = cnt[0], np = cnt[1], nl = cnt[2];
+    const uint64_t cmd_end = 32ull + 20ull * nc, pm_bytes = (uint64_t)PM_RECORD_BYTES * np;
+    const uint64_t need = cmd_end + pm_bytes + nl;
+    const bool ok = p.status[sidx] == ST_OK;
+    if (!ok || need > cap) {
+        // a failed stream (blob_len 0) or a region too small for the blob (status 2, blob_len = the size it needs): the region
+        // keeps no partial records
+        const uint64_t lo_end = min(cap, cmd_end), hi_beg = cap - min(cap, pm_bytes);
+        for (uint64_t i = 32 + lane; i < lo_end; i += 32) blob[i] = 0;
+        for (uint64_t i = hi_beg + lane; i < cap; i += 32) blob[i] = 0;
+        if (lane == 0) { r.blob_len[sidx] = ok ? need : 0; if (ok) p.status[sidx] = ST_NEED_OUTPUT; }
+        return;
+    }
+    // prediction-mode records: reverse their order in place, then move them down behind the commands (by at least the literal
+    // pool's size: every chunk is read before it is written)
+    for (uint32_t j = 0; j < np / 2; j++) {
+        uint8_t *x = blob + cap - (uint64_t)PM_RECORD_BYTES * (j + 1), *y = blob + cap - (uint64_t)PM_RECORD_BYTES * (np - j);
+        for (uint32_t i = lane; i < PM_RECORD_BYTES; i += 32) { const uint8_t t = x[i]; x[i] = y[i]; y[i] = t; }
+    }
+    __syncwarp();
+    const uint64_t src = cap - pm_bytes;
+    if (src != cmd_end) {
+        for (uint64_t i = 0; i < pm_bytes; i += 128) {
+            uint8_t v[4];
+#pragma unroll
+            for (int k = 0; k < 4; k++) { const uint64_t x = i + lane + 32 * k; v[k] = x < pm_bytes ? blob[src + x] : (uint8_t)0; }
+            __syncwarp();
+#pragma unroll
+            for (int k = 0; k < 4; k++) { const uint64_t x = i + lane + 32 * k; if (x < pm_bytes) blob[cmd_end + x] = v[k]; }
+            __syncwarp();
+        }
+        for (uint64_t i = max(src, need) + lane; i < cap; i += 32) blob[i] = 0;   // where they were, past the blob
+    }
+    // literal pool: 32 command records at a time, pool offsets by a warp scan of the literal lengths
+    uint8_t *pool = blob + cmd_end + pm_bytes;
+    const uint8_t *out = p.out + p.out_off[sidx];
+    uint32_t base = 0;
+    for (uint32_t c0 = 0; c0 < nc; c0 += 32) {
+        const uint32_t c = c0 + lane;
+        uint8_t *rec = blob + 32 + 20ull * c;
+        const bool lit = c < nc && ld_le32(rec) == 3u;
+        const uint32_t pos = lit ? ld_le32(rec + 4) : 0u, len = lit ? ld_le32(rec + 8) : 0u;
+        uint32_t incl = len;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) { const uint32_t t = __shfl_up_sync(FULL, incl, o); if ((int)lane >= o) incl += t; }
+        const uint32_t off = base + incl - len;
+        if (lit) st_le32(rec + 4, off);
+        for (uint32_t m = __ballot_sync(FULL, len != 0); m; m &= m - 1) {
+            const int l = __ffs((int)m) - 1;
+            const uint32_t lp = __shfl_sync(FULL, pos, l), ll = __shfl_sync(FULL, len, l), lo = __shfl_sync(FULL, off, l);
+            for (uint32_t i = lane; i < ll; i += 32) pool[lo + i] = out[lp + i];
+        }
+        base += __shfl_sync(FULL, incl, 31);
+    }
+    if (lane < 8) {
+        const uint32_t window = p.in[p.in_off[sidx] + 5];
+        const uint32_t w = lane == 0 ? 0x4c435644u : lane == 1 ? 1u : lane == 2 ? nc : lane == 3 ? np : lane == 4 ? nl : lane == 5 ? window : 0u;
+        st_le32(blob + 4 * lane, w);
+    }
+    if (lane == 0) r.blob_len[sidx] = need;
+}
+void launch_pack_cmds(const DecodeParams &p, const RecParams &r, cudaStream_t st) {
+    pack_cmds_kernel<<<(p.n_streams + 3) / 4, 128, 0, st>>>(p, r);   // one warp per stream
+}
+
 void launch_frame(const FrameParams &p, uint8_t *payload, uint64_t payload_cap_bytes, cudaStream_t st) {
     uint32_t blocks = (p.n_streams + 3) / 4;   // one warp per stream
     frame_kernel<<<blocks, 128, 0, st>>>(p);
@@ -153,7 +233,9 @@ void launch_frame(const FrameParams &p, uint8_t *payload, uint64_t payload_cap_b
 // blend stream decoder: persistent warps, two streams per warp in lock step (dv_engine.cuh), work pulled from a global
 // counter.  Every nibble goes through the blend core (nibble_core_blend): the model has no literal fast loop.
 // ---------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) decode_kernel_blend(DecodeParams p) {
+// (REC: the recording decoder, as in dv2_kernels.cu)
+template <bool REC>
+__device__ __forceinline__ void decode_blend(const DecodeParams p, const RecParams r) {
     extern __shared__ __align__(16) uint8_t smem[];
     const int lane = threadIdx.x & 31;
     const int group_in_block = (threadIdx.x >> 5) * 2 + (lane >> 4);
@@ -207,6 +289,11 @@ __global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) decode_kernel_blend(D
                     st_reset(s);
                     coder_init_dec(s.cur, reinterpret_cast<const uint32_t *>(pl), pay0 >> 2);   // command stream (CMD_CODER, codec/interface.rs:49)
                     coder_init_dec(s.c->oth, reinterpret_cast<const uint32_t *>(pl + (((uint64_t)pay0 + 15) & ~15ull)), pay1 >> 2);   // literal stream (LIT_CODER, :50)
+                    if (REC) {
+                        s.c->rec.blob = r.blobs + r.blob_off[v];
+                        s.c->rec.cap = r.blob_cap[v] > 0xffffffffull ? 0xffffffffu : (uint32_t)r.blob_cap[v];
+                        s.c->rec.n_cmds = 0; s.c->rec.n_pms = 0; s.c->rec.n_lits = 0;
+                    }
                     enter_cmd_type<false>(s, nx);
                 }
             }
@@ -219,10 +306,14 @@ __global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) decode_kernel_blend(D
         // ---- per-group scalar state machines (divergent) ----
         if (busy) {
             if (s.cur.underflow) s.status = ST_NEED_INPUT;
-            else transition<false>(s, nx, g, sym);
+            else transition<false, false, REC>(s, nx, g, sym);
             if (s.status != ST_OK || s.state == S_IDLE) {
                 if (s.status == ST_OK && s.c->oth.underflow) s.status = ST_NEED_INPUT;
                 if (g.store0) { p.out_len[s.c->sidx] = s.out_pos; p.status[s.c->sidx] = s.status; }
+                if (REC && g.store0) {
+                    uint32_t *cnt = r.counts + 3 * (size_t)s.c->sidx;
+                    cnt[0] = s.c->rec.n_cmds; cnt[1] = s.c->rec.n_pms; cnt[2] = s.c->rec.n_lits;
+                }
                 s.state = S_IDLE; s.status = ST_OK;
                 nx.cdf = A_misc(s, MI_DUMMY); nx.cdf2 = nullptr; nx.speed = SPK_NONE; nx.tagged = false;
                 coder_init_dec(s.cur, nullptr, 0); s.cur.need_a = 0;
@@ -231,9 +322,16 @@ __global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) decode_kernel_blend(D
     }
 }
 
+__global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) decode_kernel_blend(DecodeParams p) { decode_blend<false>(p, RecParams{}); }
+__global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) decode_kernel_blend_rec(DecodeParams p, RecParams r) { decode_blend<true>(p, r); }
+
 void launch_decode16_blend(const DecodeParams &p, uint32_t n_blocks, cudaStream_t st) {
     size_t smem = (size_t)(DECODE_BLOCK_THREADS / 16) * SMEM_BYTES_PER_GROUP;
     decode_kernel_blend<<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p);
+}
+void launch_decode16_blend_rec(const DecodeParams &p, const RecParams &r, uint32_t n_blocks, cudaStream_t st) {
+    size_t smem = (size_t)(DECODE_BLOCK_THREADS / 16) * SMEM_BYTES_PER_GROUP;
+    decode_kernel_blend_rec<<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p, r);
 }
 int decode_max_blocks_per_sm16_blend() {
     return stream_kernel_blocks_per_sm(decode_kernel_blend, DECODE_BLOCK_THREADS, (size_t)(DECODE_BLOCK_THREADS / 16) * SMEM_BYTES_PER_GROUP);

@@ -26,4 +26,8 @@ void launch_decode16_blend(const DecodeParams &p, uint32_t n_blocks, cudaStream_
 int decode_max_blocks_per_sm16_blend();
 void launch_encode_model_blend(const EncodeParams &p, uint32_t n_blocks, cudaStream_t st);
 void launch_rcp15_init(uint64_t *tab, cudaStream_t st);
+// decoding to command lists: the recording decoders (16 lanes per stream) and the pack kernel that finishes the blobs
+void launch_decode_v2_rec(const DecodeParams &p, const RecParams &r, uint32_t n_blocks, cudaStream_t st);
+void launch_decode16_blend_rec(const DecodeParams &p, const RecParams &r, uint32_t n_blocks, cudaStream_t st);
+void launch_pack_cmds(const DecodeParams &p, const RecParams &r, cudaStream_t st);
 }  // namespace dv

@@ -175,6 +175,30 @@ DivansResult divans_b200_decode_batch_device(divans_b200_ctx *ctx, size_t n, con
                                              const uint64_t *d_out_cap, uint64_t *d_out_len, int32_t *d_status,
                                              uint64_t in_total_bytes, uint32_t flags, void *cuda_stream);
 DivansResult divans_b200_synchronize(divans_b200_ctx *ctx);
+/* Decode n .divans streams held in HOST memory to their command lists: each stream is decoded as divans_b200_decode_batch_host
+ * decodes it, and every command it carries is recorded as one DVCL record (the "command list blob" below), so a stored stream
+ * can be re-encoded with divans_b200_encode_cmds_batch_host under other options.  The blob of stream i goes to
+ * blobs[blob_off[i] .. +blob_cap[i]); its header's window is the stream's own.  Per stream:
+ *   status 0: out_len[i] bytes were decoded and blob_len[i] bytes of DVCL were written;
+ *   status 2 with blob_len[i] > blob_cap[i]: the blob region was too small.  The stream was still decoded to its end, out_len[i]
+ *     is its full length, blob_len[i] the exact size its blob needs (retry with that);
+ *   otherwise (output region too small, truncated or corrupt input): the status and out_len[i] of divans_b200_decode_batch_host,
+ *     blob_len[i] = 0.
+ * Both regions of every stream are written whole (zeros past the lengths; a failed stream's blob region is all zeros), nothing
+ * outside them is touched.  Input regions may alias.  Frequentist streams run on the 16-lane layout whatever the context's
+ * lanes_per_stream (divans_b200_last_lanes reports 16); flags as for decode (SKIP_CRC, NO_CRC_KERNEL, MODEL_WASM_2018, CDF_BLEND). */
+DivansResult divans_b200_decode_cmds_batch_host(divans_b200_ctx *ctx, size_t n, const uint8_t *in, const uint64_t *in_off,
+                                                const uint64_t *in_len, uint8_t *out, const uint64_t *out_off,
+                                                const uint64_t *out_cap, uint64_t *out_len, uint8_t *blobs, const uint64_t *blob_off,
+                                                const uint64_t *blob_cap, uint64_t *blob_len, int32_t *status, uint32_t flags);
+/* Same, all pointers are DEVICE pointers.  `in_total_bytes` and `cuda_stream` as for divans_b200_decode_batch_device; asynchronous
+ * and serialised on the context exactly as that call.  Regions are not cleared first: past the lengths they hold what they held,
+ * except that the records of a failed stream or of a region too small for its blob are zeroed. */
+DivansResult divans_b200_decode_cmds_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_in, const uint64_t *d_in_off,
+                                                  const uint64_t *d_in_len, uint8_t *d_out, const uint64_t *d_out_off,
+                                                  const uint64_t *d_out_cap, uint64_t *d_out_len, uint8_t *d_blobs,
+                                                  const uint64_t *d_blob_off, const uint64_t *d_blob_cap, uint64_t *d_blob_len,
+                                                  int32_t *d_status, uint64_t in_total_bytes, uint32_t flags, void *cuda_stream);
 /* For tests and diagnostics only: waits for the context's last call to finish, then copies the 16-byte header of arena
  * slot `slot` to out[4] -- the state a v2 decoder slot carries from stream to stream and from launch to launch:
  *   [0] generation counter (its low 16 bits tag the literal priors; 0 is skipped, the tables are wiped at the wrap),

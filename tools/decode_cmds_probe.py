@@ -1,0 +1,89 @@
+"""Cost of decoding to command lists against a plain decode, and of whole transcodes, on the bench's two populations:
+4096 x 64 KiB synthetic text encoded by the literal-only generator (the flagship) and its LZ77 command streams (window 16).
+
+    python tools/decode_cmds_probe.py [n_streams] [reps]
+
+Per population it prints, as JSON lines: the device time of the plain decode and of the recording decode + pack kernel
+(divans_b200_last_kernel_ms: framing through the last kernel, host copies excluded), the wall time of a transcode to
+dynamic_context_mixing = 2, and the same for the blend-coded streams transcoded to the frequentist model.  Medians over `reps`
+after one warm-up call.  The GPU's name, power limit and SM clock are printed with them."""
+import json
+import os
+import statistics
+import subprocess
+import sys
+import time
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+import divans_b200  # noqa: E402
+from divans_b200 import synth  # noqa: E402
+
+
+def gpu_info():
+    try:
+        q = "name,power.limit,clocks.sm,clocks.max.sm"
+        return subprocess.run(["nvidia-smi", "--query-gpu=" + q, "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    except OSError:
+        return "unknown"
+
+
+def median(f, reps):
+    f()
+    return statistics.median(f() for _ in range(reps))
+
+
+def main():
+    n = int(sys.argv[1]) if len(sys.argv) > 1 else 4096
+    reps = int(sys.argv[2]) if len(sys.argv) > 2 else 5
+    eng = divans_b200.Engine(0, 0, 16)
+    blob, off, ln = synth.text_streams(n, 65536, seed=0xD1FA15)
+    raws = [blob[int(o):int(o + l)].tobytes() for o, l in zip(off, ln)]
+    caps = [len(r) + 64 for r in raws]
+    cb, co, cl = divans_b200.lz77_cmds_batch(blob, off, ln, 16, 2, 4)
+    lz = [cb[int(o):int(o + l)].tobytes() for o, l in zip(co, cl)]
+    pops = {
+        "flagship_literal_only": (raws, divans_b200.encode_options(), False),
+        "Z_lz77_window16": (lz, divans_b200.encode_options(window_size=16), True),
+    }
+    print(json.dumps({"gpu": gpu_info(), "streams": n, "reps": reps}))
+    for name, (inp, opts, cmds) in pops.items():
+        streams = eng.encode(inp, opts, cmds=cmds)
+
+        def plain():
+            res = eng.decode(streams, caps)
+            assert all(st == 0 for st, _ in res)
+            return eng.last_kernel_ms()
+
+        def rec():
+            res = eng.decode_cmds(streams, caps)
+            assert all(st == 0 for st, _, _ in res)
+            return eng.last_kernel_ms()
+
+        def transcode(src, flags, o):
+            def f():
+                t = time.perf_counter()
+                eng.transcode(src, caps, o, flags)
+                return (time.perf_counter() - t) * 1e3
+            return f
+
+        bopts = divans_b200.encode_options(window_size=opts.window_size, cdf_model=divans_b200.CDF_BLEND)
+        blend = eng.encode(inp, bopts, cmds=cmds)
+        plain_ms, rec_ms = median(plain, reps), median(rec, reps)
+        # correctness at the measured size: the recovered lists re-encode to the streams
+        back = eng.encode([b for _, _, b in eng.decode_cmds(streams[:64], caps[:64])], opts, cmds=True)
+        assert back == streams[:64]
+        row = {
+            "population": name,
+            "decode_kernel_ms": round(plain_ms, 3),
+            "decode_cmds_kernel_ms": round(rec_ms, 3),
+            "overhead": round(rec_ms / plain_ms - 1, 4),
+            "transcode_to_mix2_ms": round(median(transcode(streams, 0, divans_b200.encode_options(window_size=0, dynamic_context_mixing=2)), reps), 1),
+            "transcode_blend_to_frequentist_ms": round(median(transcode(blend, divans_b200.FLAG_CDF_BLEND, None), reps), 1),
+        }
+        print(json.dumps(row), flush=True)
+    eng.close()
+
+
+if __name__ == "__main__":
+    main()
