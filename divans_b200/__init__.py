@@ -43,6 +43,7 @@ BATCH_SYMBOLS = [
     "divans_b200_encode_cmds_batch_host", "divans_b200_encode_batch_device", "divans_b200_ir_to_cmds",
     "divans_b200_decode_batch_host_async", "divans_b200_decode_batch_host_wait", "divans_b200_lz77_cmds_batch", "divans_b200_kernel_version", "divans_b200_last_lanes",
     "divans_b200_debug_slot_header", "divans_b200_decode_cmds_batch_host", "divans_b200_decode_cmds_batch_device",
+    "divans_b200_encode_cmds_batch_device",
 ]
 PM_RECORD_BYTES = 32 + 16384 + 1024 + 8192   # one prediction-mode record of a DVCL blob (include/divans_b200.h)
 
@@ -115,6 +116,9 @@ def load_library():
     L.divans_b200_encode_cmds_batch_host.restype = ctypes.c_uint8
     L.divans_b200_encode_batch_device.argtypes = [vp, sz, vp, vp, vp, ctypes.c_uint64, vp, vp, vp, vp, vp, ctypes.POINTER(EncodeOptions), vp]
     L.divans_b200_encode_batch_device.restype = ctypes.c_uint8
+    L.divans_b200_encode_cmds_batch_device.argtypes = [vp, sz, vp, vp, vp, ctypes.c_uint64, ctypes.c_uint64, vp, vp, vp, vp, vp,
+                                                       ctypes.POINTER(EncodeOptions), vp]
+    L.divans_b200_encode_cmds_batch_device.restype = ctypes.c_uint8
     L.divans_b200_ir_to_cmds.argtypes = [ctypes.c_char_p, sz, vp, sz, szp, ctypes.POINTER(ctypes.c_int32)]
     L.divans_b200_ir_to_cmds.restype = ctypes.c_uint8
     L.divans_b200_lz77_cmds_batch.argtypes = [sz, vp, vp, vp, ctypes.c_int32, ctypes.c_int32, ctypes.c_int32, vp, sz, vp, vp, szp, ctypes.c_int32]
@@ -189,6 +193,14 @@ def lz77_cmds_batch(blob, in_off, in_len, window=16, pred_mode=2, mixing_value=4
     if rc != DIVANS_SUCCESS:
         raise ValueError("lz77_cmds_batch failed")
     return out, boff, blen
+
+
+def first_blob_cap(out_cap):
+    """The blob region decoding to a command list tries first, for streams of up to ``out_cap`` decoded bytes: header, one
+    prediction-mode record, every byte a literal byte plus a few commands per 64 bytes.  Lists with more commands than that
+    report the exact size they need and are decoded once more."""
+    out_cap = np.asarray(out_cap, np.uint64)
+    return np.uint64(32 + PM_RECORD_BYTES + 4096) + out_cap + out_cap // np.uint64(4)
 
 
 def encode_options(**kw):
@@ -368,8 +380,7 @@ class Engine:
         for b, o in zip(bufs, in_off):
             blob[int(o):int(o) + b.size] = b
         out_cap = np.array(out_caps, np.uint64).reshape(n)
-        # first guess: header, one prediction-mode record, every byte a literal byte plus a few commands per 64 bytes
-        blob_cap = np.uint64(32 + PM_RECORD_BYTES + 4096) + out_cap + out_cap // np.uint64(4)
+        blob_cap = first_blob_cap(out_cap)
         res = [None] * n
         todo = np.arange(n)
         for attempt in range(2):
@@ -438,6 +449,97 @@ class Engine:
                                                      d_out_len, d_status, ctypes.byref(o), stream)
         if rc != DIVANS_SUCCESS:
             raise DivansError("encode_batch_device: " + self._err())
+
+    def encode_cmds_batch_device(self, n, d_blobs, d_blob_off, d_blob_len, max_blob_len, max_raw_len, d_out, d_out_off, d_out_cap, d_out_len,
+                                 d_status, opts=None, stream=None):
+        """encode_batch_host(..., cmds=True) with raw device pointers (ints): command lists resident in HBM, blob offsets 4-byte
+        aligned.  ``max_blob_len`` >= every blob length sizes the symbol logs, ``max_raw_len`` >= every list's decoded length the
+        replay window; a ``window_size`` of 0 takes each list's own window.  Asynchronous on ``stream``."""
+        o = opts or encode_options()
+        rc = self._L.divans_b200_encode_cmds_batch_device(self._h, n, d_blobs, d_blob_off, d_blob_len, int(max_blob_len), int(max_raw_len), d_out,
+                                                          d_out_off, d_out_cap, d_out_len, d_status, ctypes.byref(o), stream)
+        if rc != DIVANS_SUCCESS:
+            raise DivansError("encode_cmds_batch_device: " + self._err())
+
+    def transcode_device(self, d_in, in_off, in_len, out_caps, opts=None, flags=0, stream=None):
+        """transcode without leaving the GPU: ``d_in`` is a CUDA uint8 tensor of concatenated .divans streams, stream i at
+        in_off[i] .. +in_len[i] (host arrays), decoding to at most out_caps[i] bytes.  decode_cmds_batch_device then
+        encode_cmds_batch_device on one CUDA stream, ordered after the work queued on ``stream`` (a torch.cuda.Stream, default
+        the current one), the command
+        lists staying in a device tensor.  Streams whose list did not fit the first guess (first_blob_cap) run once more with
+        the exact size.  Returns (d_new, new_off, new_len, status): a CUDA uint8 tensor holding the re-encoded streams and host
+        arrays; status[i] is the decode status where that failed, else the encode status.  ``opts`` as for transcode."""
+        import torch
+        n = len(in_off)
+        in_off, in_len = np.ascontiguousarray(in_off, np.uint64).reshape(n), np.ascontiguousarray(in_len, np.uint64).reshape(n)
+        out_cap = np.array(out_caps, np.uint64).reshape(n)
+        o = opts if opts is not None else encode_options(window_size=0)
+        dev = d_in.device
+        # the calls run on a stream of their own, ordered after the work already queued on `stream` (a default stream has no
+        # handle the library could take: NULL would mean the context's stream)
+        caller = stream if stream is not None else torch.cuda.current_stream(dev)
+        s = torch.cuda.Stream(dev)
+        s.wait_stream(caller)
+        u64 = lambda a: torch.from_numpy(np.ascontiguousarray(a, np.uint64).view(np.int64)).to(dev, non_blocking=False)
+        self.last_transcode_retried = 0
+        if n == 0:
+            return torch.zeros(0, dtype=torch.uint8, device=dev), np.zeros(0, np.uint64), np.zeros(0, np.uint64), np.zeros(0, np.int32)
+
+        pad = lambda c: (c + np.uint64(255)) & ~np.uint64(255)
+        new_caps = lambda bcap: pad(bcap + bcap // np.uint64(2) + np.uint64(70000))   # (Engine.encode's output rule)
+
+        def run(idx, blob_cap, d_new=None):
+            """decode + encode of streams idx on the device, one synchronisation: (d_new, new_off, new_len, status, blob_len).
+            The new streams go to `d_new` when given (at least new_caps(blob_cap).sum() bytes)."""
+            m = len(idx)
+            ocap, bcap = out_cap[idx], blob_cap
+            offs = lambda c: np.concatenate([[0], np.cumsum(pad(c))[:-1]]).astype(np.uint64)
+            new_cap = new_caps(bcap)
+            out_off, blob_off, new_off = offs(ocap), offs(bcap), offs(new_cap)
+            with torch.cuda.stream(s):
+                d_meta = u64(np.concatenate([in_off[idx], in_len[idx], out_off, ocap, blob_off, bcap, new_off, new_cap]))
+                M = [d_meta[k * m:(k + 1) * m] for k in range(8)]
+                d_out = torch.empty(int(pad(ocap).sum()), dtype=torch.uint8, device=dev)
+                d_blobs = torch.empty(int(pad(bcap).sum()), dtype=torch.uint8, device=dev)
+                if d_new is None:
+                    d_new = torch.empty(int(new_cap.sum()), dtype=torch.uint8, device=dev)
+                d_res = torch.zeros(4 * m, dtype=torch.int64, device=dev)   # out_len | blob_len | new_len | both statuses
+                d_st = d_res[3 * m:].view(torch.int32)
+                d_dec_st, d_enc_st = d_st[:m], d_st[m:]
+                self.decode_cmds_batch_device(d_in.data_ptr(), M[0].data_ptr(), M[1].data_ptr(), d_out.data_ptr(), M[2].data_ptr(), M[3].data_ptr(),
+                                              d_res.data_ptr(), d_blobs.data_ptr(), M[4].data_ptr(), M[5].data_ptr(), d_res[m:].data_ptr(),
+                                              d_dec_st.data_ptr(), m, int(in_len[idx].sum()), flags, s.cuda_stream)
+                # a stream that did not decode reaches the encoder with no blob (status 2's blob_len is larger than its region)
+                d_enc_len = torch.where(d_dec_st == 0, d_res[m:2 * m], torch.zeros_like(d_res[m:2 * m]))
+                self.encode_cmds_batch_device(m, d_blobs.data_ptr(), M[4].data_ptr(), d_enc_len.data_ptr(), int(bcap.max()), int(ocap.max()),
+                                              d_new.data_ptr(), M[6].data_ptr(), M[7].data_ptr(), d_res[2 * m:].data_ptr(), d_enc_st.data_ptr(),
+                                              o, s.cuda_stream)
+                res = d_res.cpu()   # (the one synchronisation of the pass)
+            r = res.numpy()
+            st = r[3 * m:].view(np.int32)
+            dec_st, enc_st = st[:m], st[m:]
+            return d_new, new_off, r[2 * m:3 * m].view(np.uint64).copy(), np.where(dec_st != 0, dec_st, enc_st).astype(np.int32), \
+                r[m:2 * m].view(np.uint64).copy(), dec_st.copy()
+
+        cap1 = first_blob_cap(out_cap)
+        d_new, new_off, new_len, status, blob_len, dec_st = run(np.arange(n), cap1)
+        retry = np.nonzero((dec_st == DIVANS_NEEDS_MORE_OUTPUT) & (blob_len > cap1))[0]
+        self.last_transcode_retried = int(retry.size)   # (streams of the most recent call that ran twice)
+        if retry.size:
+            # one output tensor: the first pass's streams move into it before the second pass allocates its buffers, and the
+            # second pass encodes straight into its tail
+            base = d_new.numel()
+            with torch.cuda.stream(s):
+                out = torch.empty(base + int(new_caps(blob_len[retry]).sum()), dtype=torch.uint8, device=dev)
+                out[:base].copy_(d_new)
+            del d_new
+            _, off2, len2, st2, _, _ = run(retry, blob_len[retry], out[base:])
+            d_new = out
+            new_off[retry] = off2 + np.uint64(base)
+            new_len[retry], status[retry] = len2, st2
+        caller.wait_stream(s)
+        d_new.record_stream(caller)   # (allocated on the private stream, used on the caller's from here on)
+        return d_new, new_off, new_len, status
 
     def encode(self, raws, opts=None, cmds=False):
         """Convenience: list of raw byte strings (or DVCL command-list blobs with cmds=True) -> list of .divans bytes."""

@@ -523,12 +523,16 @@ static size_t encode_slots(const divans_b200_ctx *ctx, size_t n) {
     return (size_t)((resident + ENCODE_GROUPS_PER_BLOCK - 1) / ENCODE_GROUPS_PER_BLOCK) * ENCODE_GROUPS_PER_BLOCK;
 }
 
+static int clamp_window(int w) { return w < 10 ? 10 : (w > 24 ? 24 : w); }
+
 // One launch set over n streams whose inputs/outputs already sit in HBM.  `cmd_cap`/`lit_cap`: log entries per stream,
-// `replay_stride`: bytes of replay window per resident slot.
+// `replay_stride`: bytes of replay window per resident slot, `max_in_len`: the longest command list the caps were sized for,
+// `window`: 10..24, or 0 for each command list's own window.
 static DivansResult encode_device_internal(divans_b200_ctx *ctx, size_t n, int raw_mode, const uint8_t *d_in, const uint64_t *d_in_off,
-                                           const uint64_t *d_in_len, uint32_t cmd_cap, uint32_t lit_cap, uint64_t replay_stride,
-                                           uint8_t *d_out, const uint64_t *d_out_off, const uint64_t *d_out_cap, uint64_t *d_out_len,
-                                           int32_t *d_status, const divans_b200_encode_options *o, cudaStream_t st) {
+                                           const uint64_t *d_in_len, uint64_t max_in_len, uint32_t cmd_cap, uint32_t lit_cap,
+                                           uint64_t replay_stride, uint8_t *d_out, const uint64_t *d_out_off, const uint64_t *d_out_cap,
+                                           uint64_t *d_out_len, int32_t *d_status, const divans_b200_encode_options *o, int window,
+                                           cudaStream_t st) {
     const size_t slots = encode_slots(ctx, n);
     const uint32_t blocks = (uint32_t)(slots / ENCODE_GROUPS_PER_BLOCK);
     if (ensure_arena(ctx, slots) != DIVANS_SUCCESS) return DIVANS_FAILURE;
@@ -537,8 +541,8 @@ static DivansResult encode_device_internal(divans_b200_ctx *ctx, size_t n, int r
     const uint32_t max_chunks = cmd_chunks + lit_chunks;
     if (!grow(ctx, &ctx->d_sf, &ctx->sf_cap, n * ((size_t)cmd_cap + lit_cap))) return DIVANS_FAILURE;
     if (!grow(ctx, &ctx->d_replay, &ctx->replay_cap, slots * (size_t)replay_stride)) return DIVANS_FAILURE;
-    // small per-stream scratch: counts [2n] | dummy [slots] | chunk_w [n*max_chunks] | chunk_state [16*n*max_chunks]
-    size_t words = 2 * n + slots + n * (size_t)max_chunks + 4 * n * (size_t)max_chunks + 16 + 2 * n * (size_t)max_chunks * (NUM_SYMBOLS_BEFORE_FLUSH / 64);
+    // small per-stream scratch: counts [2n] | window [n] | dummy [slots] | chunk_w [n*max_chunks] | chunk_state [16*n*max_chunks]
+    size_t words = 3 * n + slots + n * (size_t)max_chunks + 4 * n * (size_t)max_chunks + 16 + 2 * n * (size_t)max_chunks * (NUM_SYMBOLS_BEFORE_FLUSH / 64);
     if (!grow(ctx, &ctx->d_enc_scratch, &ctx->enc_scratch_cap, words)) return DIVANS_FAILURE;
     if (!ctx->d_pm_internal) CK(cudaMalloc((void **)&ctx->d_pm_internal, PM_RECORD_BYTES));
     if (!ctx->d_rcp15) { CK(cudaMalloc((void **)&ctx->d_rcp15, 32768 * sizeof(uint64_t))); launch_rcp15_init(ctx->d_rcp15, st); ctx->launches += 1; }
@@ -559,6 +563,7 @@ static DivansResult encode_device_internal(divans_b200_ctx *ctx, size_t n, int r
     ep.sf = ctx->d_sf; ep.cmd_cap = cmd_cap; ep.lit_cap = lit_cap;
     uint32_t *w = ctx->d_enc_scratch;
     ep.sf_counts = w; w += 2 * n;
+    ep.stream_window = w; w += n;
     ep.sf_dummy = w; w += slots;
     ep.chunk_w = w; w += n * (size_t)max_chunks;
     w = reinterpret_cast<uint32_t *>(((uintptr_t)w + 15) & ~(uintptr_t)15);
@@ -568,8 +573,7 @@ static DivansResult encode_device_internal(divans_b200_ctx *ctx, size_t n, int r
     ep.replay = ctx->d_replay; ep.replay_stride = replay_stride;
     ep.max_chunks = max_chunks; ep.cmd_chunks = cmd_chunks;
     ep.out = d_out; ep.out_off = d_out_off; ep.out_cap = d_out_cap; ep.out_len = d_out_len; ep.status = d_status;
-    int window = o->window_size < 10 ? 10 : (o->window_size > 24 ? 24 : o->window_size);
-    ep.window_size = window; ep.dynamic_context_mixing = o->dynamic_context_mixing & 0xff; ep.prior_depth = o->prior_depth & 0xff;
+    ep.window_size = window; ep.max_in_len = max_in_len; ep.dynamic_context_mixing = o->dynamic_context_mixing & 0xff; ep.prior_depth = o->prior_depth & 0xff;
     ep.use_context_map = o->use_context_map; ep.force_stride = o->force_stride; ep.have_literal_adaptation = o->have_literal_adaptation;
     for (int k = 0; k < 4; k++) ep.literal_adaptation[k] = pack_speed(o->literal_adaptation[k]);
     ep.model_rev = o->model_rev == DIVANS_B200_MODEL_WASM_2018 ? 1 : 0;
@@ -599,10 +603,63 @@ extern "C" DivansResult divans_b200_encode_batch_device(divans_b200_ctx *ctx, si
     if (n > 0xffffffffull || max_in_len > 0x7fff0000ull) { ctx->err = "batch too large"; return DIVANS_FAILURE; }
     std::lock_guard<std::mutex> lk(ctx->mu);
     CK(cudaSetDevice(ctx->device));
-    int window = opts->window_size < 10 ? 10 : (opts->window_size > 24 ? 24 : opts->window_size);
+    const int window = clamp_window(opts->window_size);
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream;
-    return encode_device_internal(ctx, n, 1, d_in, d_in_off, d_in_len, raw_cmd_cap(max_in_len, window), (uint32_t)(2 * max_in_len + 16),
-                                  (max_in_len + 31) & ~15ull, d_out, d_out_off, d_out_cap, d_out_len, d_status, opts, st);
+    return encode_device_internal(ctx, n, 1, d_in, d_in_off, d_in_len, max_in_len, raw_cmd_cap(max_in_len, window),
+                                  (uint32_t)(2 * max_in_len + 16), (max_in_len + 31) & ~15ull, d_out, d_out_off, d_out_cap, d_out_len,
+                                  d_status, opts, window, st);
+}
+
+// Log entries of the command lists of one launch: at most L bytes each, replaying at most `replay` bytes each.
+//  * Command entries.  The host call sizes a list with header (n_cmds c, n_predmodes p) at 32c + 62000p + 64, and a list the
+//    model pass accepts has 20c + 25632p <= R = L - 32.  For a fixed p the most commands are c = floor((R - 25632p) / 20).  One
+//    more record (p + 1) costs 25632 bytes, at most ceil(25632 / 20) = 1282 commands, and gains 62000 - 32 * 1282 = 20976 > 0
+//    entries: the maximum is at the most records, p = floor(R / 25632), with the rest of the bytes in commands.
+//  * Literal entries.  The host call sizes a list at 2s + 16, s = the sum of its literal records' lengths; records may re-read
+//    pool bytes, so s is not bounded by L.  But every literal byte coded is also replayed, and the model pass refuses a literal
+//    that would not fit the replay window (status 2) before it checks the log: s <= replay, and 2 * replay + 16 always suffices.
+static void cmds_log_caps(uint64_t L, uint64_t replay, uint64_t &cmd, uint64_t &lit) {
+    const uint64_t R = L > 32 ? L - 32 : 0, p = R / PM_RECORD_BYTES;
+    cmd = 32 * ((R - (uint64_t)PM_RECORD_BYTES * p) / 20) + 62000 * p + 64;
+    lit = 2 * replay + 16;
+}
+
+extern "C" DivansResult divans_b200_encode_cmds_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_blobs, const uint64_t *d_blob_off,
+                                                             const uint64_t *d_blob_len, uint64_t max_blob_len, uint64_t max_raw_len,
+                                                             uint8_t *d_out, const uint64_t *d_out_off, const uint64_t *d_out_cap,
+                                                             uint64_t *d_out_len, int32_t *d_status, const divans_b200_encode_options *opts,
+                                                             void *cuda_stream) {
+    if (!ctx || !opts) return DIVANS_FAILURE;
+    if (n == 0) return DIVANS_SUCCESS;
+    if (n > 0xffffffffull || max_blob_len > 0x7fff0000ull || max_raw_len > 0x7fff0000ull) { ctx->err = "batch too large"; return DIVANS_FAILURE; }
+    const uint64_t replay_stride = (max_raw_len + 31) & ~15ull;
+    uint64_t cmd_cap, lit_cap;
+    cmds_log_caps(max_blob_len, replay_stride, cmd_cap, lit_cap);
+    // the kernels address a stream's logs at v * (cmd_cap + lit_cap) with a 32-bit stride
+    if (cmd_cap + lit_cap > 0xffffffffull) { ctx->err = "batch too large"; return DIVANS_FAILURE; }
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream;
+    // the slots first, as in the host call: the logs are sized from what is left, and a failure names them
+    if (ensure_arena(ctx, encode_slots(ctx, n)) != DIVANS_SUCCESS) return DIVANS_FAILURE;
+    // No sub-batching: the logs of all n streams are one allocation, of exactly their size (they are most of what the call
+    // needs next to the arena).  When it fails, the call fails and says how much it asked for.
+    const size_t words = n * (size_t)(cmd_cap + lit_cap);
+    if (words > ctx->sf_cap) {
+        cudaFree(ctx->d_sf); ctx->d_sf = nullptr; ctx->sf_cap = 0;
+        if (cudaMalloc((void **)&ctx->d_sf, words * 4) != cudaSuccess) {
+            cudaGetLastError();
+            char buf[200];
+            snprintf(buf, sizeof buf, "divans_b200: cannot allocate the symbol logs of %zu command lists of up to %llu bytes: %llu bytes", n,
+                     (unsigned long long)max_blob_len, (unsigned long long)words * 4);
+            ctx->err = buf;
+            return DIVANS_FAILURE;
+        }
+        ctx->sf_cap = words;
+    }
+    return encode_device_internal(ctx, n, 0, d_blobs, d_blob_off, d_blob_len, max_blob_len, (uint32_t)cmd_cap, (uint32_t)lit_cap,
+                                  replay_stride, d_out, d_out_off, d_out_cap, d_out_len, d_status, opts,
+                                  opts->window_size == 0 ? 0 : clamp_window(opts->window_size), st);
 }
 
 // host batch: marshal, split into sub-batches whose symbol logs fit in HBM, run, copy back
@@ -613,7 +670,7 @@ static DivansResult encode_host_common(divans_b200_ctx *ctx, size_t n, int raw_m
     if (n == 0) return DIVANS_SUCCESS;
     std::lock_guard<std::mutex> lk(ctx->mu);
     CK(cudaSetDevice(ctx->device));
-    const int window = opts->window_size < 10 ? 10 : (opts->window_size > 24 ? 24 : opts->window_size);
+    const int window = clamp_window(opts->window_size);
     // per-stream requirements
     std::vector<uint64_t> s_off(n), need_cmd(n), need_lit(n), need_replay(n);
     std::vector<uint8_t> staged;   // command lists are re-based to 4-byte aligned offsets
@@ -659,14 +716,15 @@ static DivansResult encode_host_common(divans_b200_ctx *ctx, size_t n, int raw_m
     size_t i0 = 0;
     while (i0 < n) {
         // grow the sub-batch while its uniform-capacity logs fit
-        uint64_t mc = 0, ml = 0, mr = 0; size_t i1 = i0;
+        uint64_t mc = 0, ml = 0, mr = 0, mx = 0; size_t i1 = i0;
         while (i1 < n) {
             uint64_t c = need_cmd[i1] > mc ? need_cmd[i1] : mc, l = need_lit[i1] > ml ? need_lit[i1] : ml;
             if (i1 > i0 && (c + l) * 4 * (uint64_t)(i1 - i0 + 1) > budget) break;
             mc = c; ml = l; if (need_replay[i1] > mr) mr = need_replay[i1];
+            if (in_len[i1] > mx) mx = in_len[i1];
             i1++;
         }
-        if (mc > 0xffffffffull || ml > 0xffffffffull) { ctx->err = "stream too large"; return DIVANS_FAILURE; }
+        if (mc + ml > 0xffffffffull) { ctx->err = "stream too large"; return DIVANS_FAILURE; }   // (the kernels' 32-bit log stride)
         const size_t m = i1 - i0;
         uint64_t out_lo = ~0ull, out_hi = 0;
         for (size_t i = i0; i < i1; i++) { if (out_off[i] < out_lo) out_lo = out_off[i]; if (out_off[i] + out_cap[i] > out_hi) out_hi = out_off[i] + out_cap[i]; }
@@ -680,8 +738,8 @@ static DivansResult encode_host_common(divans_b200_ctx *ctx, size_t n, int raw_m
         CK(cudaMemcpyAsync(mm + 2 * m, rel.data(), m * 8, cudaMemcpyHostToDevice, st));
         CK(cudaMemcpyAsync(mm + 3 * m, out_cap + i0, m * 8, cudaMemcpyHostToDevice, st));
         int32_t *d_status = reinterpret_cast<int32_t *>(mm + 5 * m);
-        DivansResult r = encode_device_internal(ctx, m, raw_mode, ctx->d_in, mm, mm + m, (uint32_t)mc, (uint32_t)ml, mr, ctx->d_out, mm + 2 * m,
-                                                mm + 3 * m, mm + 4 * m, d_status, opts, st);
+        DivansResult r = encode_device_internal(ctx, m, raw_mode, ctx->d_in, mm, mm + m, mx, (uint32_t)mc, (uint32_t)ml, mr, ctx->d_out,
+                                                mm + 2 * m, mm + 3 * m, mm + 4 * m, d_status, opts, window, st);
         if (r != DIVANS_SUCCESS) return r;
         CK(cudaMemcpyAsync(out_len + i0, mm + 4 * m, m * 8, cudaMemcpyDeviceToHost, st));
         CK(cudaMemcpyAsync(status + i0, d_status, m * 4, cudaMemcpyDeviceToHost, st));

@@ -165,6 +165,10 @@ struct EncodeParams {
     int window_size, dynamic_context_mixing, prior_depth, use_context_map, force_stride, have_literal_adaptation;
     int literal_adaptation[4];    // packed inc | lim << 16
     int model_rev;                // see DecodeParams::model_rev
+    // command lists: window_size 0 = each stream takes the window of its blob header (clamped to 10..24); a blob longer than
+    // max_in_len (the bound cmd_cap / lit_cap were derived from) is refused unread
+    uint64_t max_in_len;
+    uint32_t *stream_window;      // per stream: the window the model pass coded it with (the mux writes it into the header)
 };
 constexpr uint32_t PM_RECORD_BYTES = 32 + 16384 + 1024 + 8192;
 

@@ -39,7 +39,6 @@ __global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) encode_model_kernel(E
     s.c->sidx = 0; s.c->raw_len = 0; s.c->lit_log_cap = p.lit_cap;
     s.out = p.replay + (uint64_t)slot * p.replay_stride; s.out_pos = 0;
     s.c->out_cap = p.replay_stride > 0xffffffffull ? 0xffffffffu : (uint32_t)p.replay_stride;
-    s.c->ring_len = 1u << p.window_size;
     st_reset(s);
     uint32_t *const dummy_log = p.sf_dummy + slot;
     coder_init_enc(s.cur, dummy_log); coder_init_enc(s.c->oth, dummy_log);
@@ -74,15 +73,20 @@ __global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) encode_model_kernel(E
                     s.c->desired_adapt0 = p.literal_adaptation[0]; s.c->desired_adapt1 = p.literal_adaptation[1];
                     s.c->desired_adapt2 = p.literal_adaptation[2]; s.c->desired_adapt3 = p.literal_adaptation[3];
                     s.c->in.pos = 0;
+                    uint32_t win = (uint32_t)p.window_size;   // 0 (command lists only): the window of the blob's header
                     if (p.raw_mode) {
                         if (blen > 0xffffffffull - 16) ok = false;
                         s.c->in.cmds = nullptr; s.c->in.pms = p.pm_internal; s.c->in.n_pms = 1; s.c->in.lits = blob;
                         s.c->raw_len = (uint32_t)blen;
-                        s.c->in.n_cmds = 1u + (uint32_t)((blen + s.c->ring_len - 1) >> p.window_size);
+                        s.c->in.n_cmds = 1u + (uint32_t)((blen + (1ull << win) - 1) >> win);
                     } else {
                         const uint32_t *h = reinterpret_cast<const uint32_t *>(blob);
-                        if (blen < 32 || h[0] != 0x4c435644u || h[1] != 1u) ok = false;
+                        // the records are read as u32; the logs were sized for blobs of at most max_in_len bytes: a misaligned or
+                        // longer blob is refused before any of its bytes is read
+                        if (((uintptr_t)blob & 3u) != 0 || blen > p.max_in_len) ok = false;
+                        else if (blen < 32 || h[0] != 0x4c435644u || h[1] != 1u) ok = false;
                         else {
+                            if (win == 0) win = min(max(h[5], 10u), 24u);
                             const uint64_t need = 32ull + 20ull * h[2] + (uint64_t)PM_RECORD_BYTES * h[3] + h[4];
                             if (need > blen) ok = false;
                             s.c->in.cmds = h + 8; s.c->in.n_cmds = h[2]; s.c->in.n_pms = h[3];
@@ -93,6 +97,8 @@ __global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) encode_model_kernel(E
                     }
                     if (!ok) { if (g.store0) { p.status[v] = ST_FAIL; p.sf_counts[2 * v] = 0; p.sf_counts[2 * v + 1] = 0; } }
                     else {
+                        s.c->ring_len = 1u << win;
+                        if (g.store0) p.stream_window[v] = win;
                         coder_init_enc(s.cur, p.sf + (uint64_t)v * per_stream);                   // CMD_CODER
                         coder_init_enc(s.c->oth, p.sf + (uint64_t)v * per_stream + p.cmd_cap);   // LIT_CODER
                         enter_cmd_type<true>(s, nx);
@@ -313,6 +319,7 @@ __global__ void __launch_bounds__(128) encode_mux_kernel(EncodeParams p) {
     const int lane = threadIdx.x & 31;
     if (v >= p.n_streams) return;
     if (p.status[v] != ST_OK) { if (lane == 0) p.out_len[v] = 0; return; }
+    const uint8_t window = (uint8_t)p.stream_window[v];
     VStream vs[2];
     const uint32_t lit_chunks = p.max_chunks - p.cmd_chunks;
     for (int c = 0; c < 2; c++) {
@@ -331,7 +338,7 @@ __global__ void __launch_bounds__(128) encode_mux_kernel(EncodeParams p) {
     for (int pass = 0; pass < 2; pass++) {
         uint32_t r[2] = {rem[0], rem[1]}, d[2] = {0, 0};
         uint64_t last_flush[2] = {0, 0}, bytes_flushed = 0, o = 16;
-        if (pass == 1 && lane < 16) out[lane] = lane == 0 ? 0xff : lane == 1 ? 0xe5 : lane == 2 ? 0x8c : lane == 3 ? 0x9f : lane == 5 ? (uint8_t)p.window_size : 0;   // make_header, divans_compressor.rs:126-131
+        if (pass == 1 && lane < 16) out[lane] = lane == 0 ? 0xff : lane == 1 ? 0xe5 : lane == 2 ? 0x8c : lane == 3 ? 0x9f : lane == 5 ? window : 0;   // make_header, divans_compressor.rs:126-131
         for (;;) {   // flush_internal, mux.rs:500-548: alternate the streams, 65536-byte fixed records while they last
             bool any = false, have = false; uint64_t lf = 0;
             for (int i = 0; i < 2; i++) if (r[i]) { if (!have || last_flush[i] < lf) { lf = last_flush[i]; have = true; } }

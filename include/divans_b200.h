@@ -245,6 +245,31 @@ DivansResult divans_b200_encode_cmds_batch_host(divans_b200_ctx *ctx, size_t n, 
                                                 const uint64_t *blob_len, uint8_t *out, const uint64_t *out_off,
                                                 const uint64_t *out_cap, uint64_t *out_len, int32_t *status,
                                                 const divans_b200_encode_options *opts);
+/* Same as divans_b200_encode_cmds_batch_host with every pointer a DEVICE pointer: command lists resident in HBM (for example
+ * the blobs divans_b200_decode_cmds_batch_device wrote), framed streams left in HBM.
+ *  - Every blob the host call accepts gives the same bytes, out_len and status as the host call with the same options: status 3
+ *    for refused and hostile lists, status 2 with out_len the size the stream needs when out_cap is too small.  The logs here are
+ *    at least as large as the host call's for the same batch, so the one refusal that can differ is the host call's own log
+ *    overflow: a list whose PredictionMode commands share records can code more command symbols than its header's sizes
+ *    provide for, and the host call refuses it when its sub-batch's logs are too small.
+ *  - Asynchronous on `cuda_stream` (NULL = the context's own stream) and serialised on the context like the other device calls;
+ *    divans_b200_last_kernel_ms / _last_main_kernel_ms are valid for it.
+ *  - `max_blob_len` >= every blob_len[i] sizes the command logs, `max_raw_len` the literal logs, one capacity for the whole
+ *    launch: a blob of up to max_blob_len bytes whose replay fits max_raw_len never fails for lack of log space.  A longer blob
+ *    fails with status 3 and none of its bytes is read.
+ *  - `max_raw_len` sizes the replay window of each slot: the decoded length of every list (one copy record can write megabytes).
+ *    A list whose replay outgrows it fails with status 2 and out_len 0 (an output region too small gives out_len > out_cap).
+ *  - blob_off[i] must be 4-byte aligned (records are read as u32): a blob at a misaligned address fails with status 3 unread.
+ *  - opts->window_size == 0: each stream takes the window of its blob header (word 5), clamped to 10..24.  Any other value is
+ *    clamped to 10..24 and applies to every stream, as in the host call.
+ *  - The symbol logs of all n streams are one allocation, per stream about 10 bytes per byte of max_blob_len plus 8 per byte of
+ *    max_raw_len; when it cannot be made the call returns DIVANS_FAILURE and divans_b200_last_error names the size.  There is no splitting into sub-batches.
+ *  - Only d_out[out_off[i] .. +out_cap[i]) is written for stream i.  n == 0 returns DIVANS_SUCCESS. */
+DivansResult divans_b200_encode_cmds_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_blobs, const uint64_t *d_blob_off,
+                                                  const uint64_t *d_blob_len, uint64_t max_blob_len, uint64_t max_raw_len,
+                                                  uint8_t *d_out, const uint64_t *d_out_off, const uint64_t *d_out_cap,
+                                                  uint64_t *d_out_len, int32_t *d_status, const divans_b200_encode_options *opts,
+                                                  void *cuda_stream);
 /* IR text front-end (reference: src/bin/divans.rs:191-483, the textual IR that `divans -i` consumes): parse `ir_text` into a
  * DVCL blob.  *blob_len receives the size of the blob; with out == NULL or out_cap too small the call returns
  * DIVANS_NEEDS_MORE_OUTPUT.  *window_size (optional) receives the `window` line's value (0 if absent).  Host only. */
