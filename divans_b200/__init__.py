@@ -43,7 +43,7 @@ BATCH_SYMBOLS = [
     "divans_b200_encode_cmds_batch_host", "divans_b200_encode_batch_device", "divans_b200_ir_to_cmds",
     "divans_b200_decode_batch_host_async", "divans_b200_decode_batch_host_wait", "divans_b200_lz77_cmds_batch", "divans_b200_kernel_version", "divans_b200_last_lanes",
     "divans_b200_debug_slot_header", "divans_b200_decode_cmds_batch_host", "divans_b200_decode_cmds_batch_device",
-    "divans_b200_encode_cmds_batch_device",
+    "divans_b200_encode_cmds_batch_device", "divans_b200_encode_auto_batch_host", "divans_b200_encode_auto_batch_device",
 ]
 PM_RECORD_BYTES = 32 + 16384 + 1024 + 8192   # one prediction-mode record of a DVCL blob (include/divans_b200.h)
 
@@ -59,6 +59,17 @@ class EncodeOptions(ctypes.Structure):
         ("literal_adaptation", (ctypes.c_int16 * 2) * 4), ("literal_pred_mode", ctypes.c_int32),
         ("literal_mixing_value", ctypes.c_int32), ("model_rev", ctypes.c_int32), ("cdf_model", ctypes.c_int32),
     ]
+
+
+class LiteralModel(ctypes.Structure):
+    """divans_b200_literal_model: a candidate of encode_auto (literal context mode LSB6=0 MSB6=1 UTF8=2 SIGN=3, mixing value)"""
+    _fields_ = [("literal_pred_mode", ctypes.c_int32), ("literal_mixing_value", ctypes.c_int32)]
+
+
+# encode_auto's default candidates, (pred_mode, mixing_value).  Entry 0 is the encoder's default model, so no stream's cost
+# under encode_auto exceeds its cost under the default.  The others are the models that code the survey corpora in the
+# fewest bits (tools/auto_probe.py --survey, DESIGN.md section 4); mixing value 2 is left out (it decodes on the generic path).
+DEFAULT_LITERAL_MODELS = [(0, 4), (2, 8), (2, 5), (2, 1), (2, 7), (3, 5), (0, 5), (2, 4)]
 
 
 class CAllocator(ctypes.Structure):
@@ -119,6 +130,11 @@ def load_library():
     L.divans_b200_encode_cmds_batch_device.argtypes = [vp, sz, vp, vp, vp, ctypes.c_uint64, ctypes.c_uint64, vp, vp, vp, vp, vp,
                                                        ctypes.POINTER(EncodeOptions), vp]
     L.divans_b200_encode_cmds_batch_device.restype = ctypes.c_uint8
+    L.divans_b200_encode_auto_batch_host.argtypes = batch + [ctypes.POINTER(EncodeOptions), vp, ctypes.c_uint32, vp, vp]
+    L.divans_b200_encode_auto_batch_host.restype = ctypes.c_uint8
+    L.divans_b200_encode_auto_batch_device.argtypes = [vp, sz, vp, vp, vp, ctypes.c_uint64, vp, vp, vp, vp, vp, ctypes.POINTER(EncodeOptions),
+                                                       vp, ctypes.c_uint32, vp, vp, vp]
+    L.divans_b200_encode_auto_batch_device.restype = ctypes.c_uint8
     L.divans_b200_ir_to_cmds.argtypes = [ctypes.c_char_p, sz, vp, sz, szp, ctypes.POINTER(ctypes.c_int32)]
     L.divans_b200_ir_to_cmds.restype = ctypes.c_uint8
     L.divans_b200_lz77_cmds_batch.argtypes = [sz, vp, vp, vp, ctypes.c_int32, ctypes.c_int32, ctypes.c_int32, vp, sz, vp, vp, szp, ctypes.c_int32]
@@ -449,6 +465,62 @@ class Engine:
                                                      d_out_len, d_status, ctypes.byref(o), stream)
         if rc != DIVANS_SUCCESS:
             raise DivansError("encode_batch_device: " + self._err())
+
+    @staticmethod
+    def _cands(candidates):
+        cs = DEFAULT_LITERAL_MODELS if candidates is None else candidates
+        arr = (LiteralModel * max(1, len(cs)))()
+        for i, (pm, mv) in enumerate(cs):
+            arr[i].literal_pred_mode, arr[i].literal_mixing_value = int(pm), int(mv)
+        return arr, len(cs)
+
+    def encode_auto_batch_host(self, in_blob, in_off, in_len, out, out_off, out_cap, opts=None, candidates=None):
+        """encode_batch_host with each stream's literal model chosen among ``candidates`` ((pred_mode, mixing_value) pairs,
+        default DEFAULT_LITERAL_MODELS) by its coding cost.  Returns (out_len, status, chosen, cost): cost[i, c] is stream i's
+        cost under candidate c in 1/65536 bit (2**64 - 1 where that pass failed)."""
+        n = len(in_off)
+        in_off, in_len = np.ascontiguousarray(in_off, np.uint64), np.ascontiguousarray(in_len, np.uint64)
+        out_off, out_cap = np.ascontiguousarray(out_off, np.uint64), np.ascontiguousarray(out_cap, np.uint64)
+        cands, nc = self._cands(candidates)
+        out_len = np.zeros(n, np.uint64)
+        status = np.full(n, DIVANS_FAILURE, np.int32)
+        chosen = np.zeros(n, np.uint32)
+        cost = np.zeros((n, nc), np.uint64)
+        o = opts or encode_options()
+        rc = self._L.divans_b200_encode_auto_batch_host(self._h, n, _ptr(in_blob), _ptr(in_off), _ptr(in_len), _ptr(out), _ptr(out_off),
+                                                        _ptr(out_cap), _ptr(out_len), _ptr(status), ctypes.byref(o), ctypes.addressof(cands),
+                                                        nc, _ptr(chosen), _ptr(cost))
+        if rc != DIVANS_SUCCESS:
+            raise DivansError("encode_auto_batch_host: " + self._err())
+        return out_len, status, chosen, cost
+
+    def encode_auto_batch_device(self, n, d_in, d_in_off, d_in_len, max_in_len, d_out, d_out_off, d_out_cap, d_out_len, d_status, d_chosen,
+                                 d_cost=None, opts=None, candidates=None, stream=None):
+        """encode_auto_batch_host with raw device pointers (ints; d_chosen u32 [n], d_cost u64 [n * C] or None).  Asynchronous
+        on ``stream``."""
+        cands, nc = self._cands(candidates)
+        o = opts or encode_options()
+        rc = self._L.divans_b200_encode_auto_batch_device(self._h, n, d_in, d_in_off, d_in_len, int(max_in_len), d_out, d_out_off, d_out_cap,
+                                                          d_out_len, d_status, ctypes.byref(o), ctypes.addressof(cands), nc, d_chosen,
+                                                          d_cost, stream)
+        if rc != DIVANS_SUCCESS:
+            raise DivansError("encode_auto_batch_device: " + self._err())
+
+    def encode_auto(self, raws, opts=None, candidates=None):
+        """Convenience: list of raw byte strings -> list of (status, .divans bytes or None, chosen candidate index)."""
+        bufs = [_u8(s) for s in raws]
+        in_len = np.array([b.size for b in bufs], np.uint64)
+        pad = (in_len + np.uint64(15)) & ~np.uint64(15)
+        in_off = np.concatenate([[0], np.cumsum(pad)[:-1]]).astype(np.uint64) if bufs else np.zeros(0, np.uint64)
+        blob = np.zeros(int(pad.sum()) + 16, np.uint8)
+        for b, o in zip(bufs, in_off):
+            blob[int(o):int(o) + b.size] = b
+        out_cap = (in_len + in_len // np.uint64(2) + np.uint64(70000 + 255)) & ~np.uint64(255)
+        out_off = np.concatenate([[0], np.cumsum(out_cap)[:-1]]).astype(np.uint64) if bufs else np.zeros(0, np.uint64)
+        out = np.zeros(int(out_cap.sum()) + 16, np.uint8)
+        out_len, status, chosen, _ = self.encode_auto_batch_host(blob, in_off, in_len, out, out_off, out_cap, opts, candidates)
+        return [(int(s), out[int(o):int(o) + int(n)].tobytes() if s == DIVANS_SUCCESS else None, int(c))
+                for s, o, n, c in zip(status, out_off, out_len, chosen)]
 
     def encode_cmds_batch_device(self, n, d_blobs, d_blob_off, d_blob_len, max_blob_len, max_raw_len, d_out, d_out_off, d_out_cap, d_out_len,
                                  d_status, opts=None, stream=None):

@@ -73,8 +73,8 @@ __device__ __forceinline__ int blend_update(const int c, const int k, const int 
     return (e & 0x7fff) | ((l16 < 9 && ((k2 >> l16) & 1)) ? 0x8000 : 0);
 }
 
-// one nibble of a 16-lane group, decoded (ENC = false) or encoded (ENC = true)
-template <bool ENC>
+// one nibble of a 16-lane group, decoded (ENC = false) or encoded (ENC = true; TALLY: costed, see enc_log in dv_core.cuh)
+template <bool ENC, bool TALLY = false>
 __device__ __forceinline__ int nibble_core_blend(St &s, const Next &nx, const G2 g) {
     const int raw = nx.cdf[g.l16];
     const int c = raw & 0x7fff;
@@ -111,7 +111,8 @@ __device__ __forceinline__ int nibble_core_blend(St &s, const Next &nx, const G2
     if (!ENC) coder_advance(s.cur, start, freq);
     else {
         if (freq <= 0 && s.state != S_IDLE) s.status = ST_FAIL;   // a symbol whose probability has decayed to the bias floor cannot be coded
-        if (g.store0) const_cast<uint32_t *>(s.cur.p)[s.cur.left] = ((uint32_t)start & 0xffffu) | ((uint32_t)freq << 16);
+        if constexpr (TALLY) s.cur.a += __ldg(s.cur.p + ((uint32_t)freq & 0x7fffu));
+        else if (g.store0) const_cast<uint32_t *>(s.cur.p)[s.cur.left] = ((uint32_t)start & 0xffffu) | ((uint32_t)freq << 16);
         s.cur.left++;
     }
     if (anymix) {

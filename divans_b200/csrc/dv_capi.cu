@@ -69,6 +69,10 @@ struct divans_b200_ctx {
     uint32_t *d_enc_scratch = nullptr; size_t enc_scratch_cap = 0;
     uint8_t *d_pm_internal = nullptr; std::vector<uint8_t> h_pm;
     uint64_t *d_rcp15 = nullptr;
+    // literal model selection (encode_auto_*): the candidates' PredictionMode records, the cost table, per (stream, candidate)
+    // scratch: offsets, lengths, record index, status and cost
+    uint8_t *d_pm_records = nullptr; uint32_t *d_cost_tab = nullptr;
+    uint64_t *d_auto = nullptr; size_t auto_cap = 0;
     bool main_end_is_evm1 = false;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr, evm = nullptr, evm1 = nullptr;   // ev0 | frame kernel | evm | decode kernel | ev1
     cudaEvent_t ev_busy = nullptr; bool busy_recorded = false;                 // end of the most recent launch set on any stream
@@ -166,6 +170,7 @@ extern "C" void divans_b200_destroy(divans_b200_ctx *ctx) {
     if (ctx->evm1) cudaEventDestroy(ctx->evm1);
     if (ctx->ev_busy) cudaEventDestroy(ctx->ev_busy);
     cudaFree(ctx->d_sf); cudaFree(ctx->d_replay); cudaFree(ctx->d_enc_scratch); cudaFree(ctx->d_pm_internal); cudaFree(ctx->d_rcp15);
+    cudaFree(ctx->d_pm_records); cudaFree(ctx->d_cost_tab); cudaFree(ctx->d_auto);
     for (auto &ln : ctx->lane) {
         cudaFree(ln.d_in); cudaFree(ln.d_out); cudaFree(ln.d_meta);
         if (ln.h_res) cudaFreeHost(ln.h_res);
@@ -525,6 +530,16 @@ static size_t encode_slots(const divans_b200_ctx *ctx, size_t n) {
 
 static int clamp_window(int w) { return w < 10 ? 10 : (w > 24 ? 24 : w); }
 
+// The PredictionMode record every raw stream starts with (zeroed by the caller), raw_to_cmd/mod.rs:116-143: 64-entry identity
+// literal map, 4 distance entries, one mixing value for all 8192 entries, speeds unset.
+static void raw_record(uint8_t *pm, int pred_mode, int mixing_value) {
+    pm[0] = (uint8_t)pred_mode; pm[2] = 1;
+    pm[28] = 64; pm[30] = 4;
+    for (int i = 0; i < 64; i++) pm[32 + i] = (uint8_t)i;
+    for (int i = 0; i < 4; i++) pm[32 + 16384 + i] = (uint8_t)i;
+    memset(pm + 32 + 16384 + 1024, mixing_value, 8192);
+}
+
 // One launch set over n streams whose inputs/outputs already sit in HBM.  `cmd_cap`/`lit_cap`: log entries per stream,
 // `replay_stride`: bytes of replay window per resident slot, `max_in_len`: the longest command list the caps were sized for,
 // `window`: 10..24, or 0 for each command list's own window.
@@ -532,7 +547,7 @@ static DivansResult encode_device_internal(divans_b200_ctx *ctx, size_t n, int r
                                            const uint64_t *d_in_len, uint64_t max_in_len, uint32_t cmd_cap, uint32_t lit_cap,
                                            uint64_t replay_stride, uint8_t *d_out, const uint64_t *d_out_off, const uint64_t *d_out_cap,
                                            uint64_t *d_out_len, int32_t *d_status, const divans_b200_encode_options *o, int window,
-                                           cudaStream_t st) {
+                                           cudaStream_t st, const uint8_t *d_pm_records = nullptr, const uint32_t *d_pm_index = nullptr) {
     const size_t slots = encode_slots(ctx, n);
     const uint32_t blocks = (uint32_t)(slots / ENCODE_GROUPS_PER_BLOCK);
     if (ensure_arena(ctx, slots) != DIVANS_SUCCESS) return DIVANS_FAILURE;
@@ -546,20 +561,17 @@ static DivansResult encode_device_internal(divans_b200_ctx *ctx, size_t n, int r
     if (!grow(ctx, &ctx->d_enc_scratch, &ctx->enc_scratch_cap, words)) return DIVANS_FAILURE;
     if (!ctx->d_pm_internal) CK(cudaMalloc((void **)&ctx->d_pm_internal, PM_RECORD_BYTES));
     if (!ctx->d_rcp15) { CK(cudaMalloc((void **)&ctx->d_rcp15, 32768 * sizeof(uint64_t))); launch_rcp15_init(ctx->d_rcp15, st); ctx->launches += 1; }
-    if (raw_mode) {
-        // raw_to_cmd/mod.rs:116-143: 64-entry identity literal map, 4 distance entries, one mixing value, speeds unset
+    if (raw_mode && !d_pm_records) {
         std::vector<uint8_t> &pm = ctx->h_pm;
         pm.assign(PM_RECORD_BYTES, 0);
-        pm[0] = (uint8_t)o->literal_pred_mode; pm[2] = 1;
-        pm[28] = 64; pm[30] = 4;
-        for (int i = 0; i < 64; i++) pm[32 + i] = (uint8_t)i;
-        for (int i = 0; i < 4; i++) pm[32 + 16384 + i] = (uint8_t)i;
-        memset(pm.data() + 32 + 16384 + 1024, o->literal_mixing_value, 8192);
+        raw_record(pm.data(), o->literal_pred_mode, o->literal_mixing_value);
         CK(cudaMemcpyAsync(ctx->d_pm_internal, pm.data(), PM_RECORD_BYTES, cudaMemcpyHostToDevice, st));
     }
     EncodeParams ep;
     ep.in = d_in; ep.in_off = d_in_off; ep.in_len = d_in_len; ep.raw_mode = raw_mode; ep.n_streams = (uint32_t)n;
-    ep.work_counter = ctx->d_counter; ep.arena = ctx->d_arena; ep.tables = ctx->d_tables; ep.pm_internal = ctx->d_pm_internal;
+    ep.work_counter = ctx->d_counter; ep.arena = ctx->d_arena; ep.tables = ctx->d_tables;
+    ep.pm_internal = d_pm_records ? d_pm_records : ctx->d_pm_internal; ep.pm_index = d_pm_index;   // (raw mode: the caller's records)
+    ep.cost_tab = nullptr; ep.tally = nullptr;
     ep.sf = ctx->d_sf; ep.cmd_cap = cmd_cap; ep.lit_cap = lit_cap;
     uint32_t *w = ctx->d_enc_scratch;
     ep.sf_counts = w; w += 2 * n;
@@ -662,12 +674,131 @@ extern "C" DivansResult divans_b200_encode_cmds_batch_device(divans_b200_ctx *ct
                                   opts->window_size == 0 ? 0 : clamp_window(opts->window_size), st);
 }
 
+// ---- literal model selection ----
+// Cost of coding a nibble of frequency f (1..32767 of 32768) in 1/65536 bit: 65536 * (15 - log2 f), the 16 fraction bits of
+// log2 f by repeated squaring of the mantissa (each round: square, and one more bit when the square reaches 2).  Integer-only,
+// so the CPU oracle's tally (oracle_tally/tally_api.c, dvo_cost_table) computes the same table.  T[0] (freq 0: the stream fails) = T[1].
+static uint32_t freq_cost(uint32_t f) {
+    if (f == 0) f = 1;
+    uint32_t e = 0;
+    while ((f >> (e + 1)) != 0) e++;
+    uint64_t x = (uint64_t)f << (31 - e);   // f / 2^e in [1, 2), Q31
+    uint32_t frac = 0;
+    for (int i = 0; i < 16; i++) {
+        x = (x * x) >> 31;
+        frac <<= 1;
+        if (x >= (1ull << 32)) { x >>= 1; frac |= 1; }
+    }
+    return (15u << 16) - ((e << 16) | frac);
+}
+
+static bool check_cands(divans_b200_ctx *ctx, const divans_b200_literal_model *cands, uint32_t n_cands) {
+    if (!cands || n_cands < 1 || n_cands > 16) { ctx->err = "encode_auto: 1..16 candidate literal models are required"; return false; }
+    for (uint32_t c = 0; c < n_cands; c++)
+        if (cands[c].literal_pred_mode < 0 || cands[c].literal_pred_mode > 3 || cands[c].literal_mixing_value < 0 ||
+            cands[c].literal_mixing_value > 15) {
+            char buf[160];
+            snprintf(buf, sizeof buf, "encode_auto: candidate %u (pred_mode %d, mixing value %d) is outside pred_mode 0..3, mixing value 0..15",
+                     c, (int)cands[c].literal_pred_mode, (int)cands[c].literal_mixing_value);
+            ctx->err = buf;
+            return false;
+        }
+    return true;
+}
+
+// One launch sequence over n raw streams in HBM: fan out to n * C virtual streams (dv_encode.cu: candidate-major), the cost-only
+// model pass over all of them, the per-stream argmin into d_chosen, then the encoder pipeline with stream i starting from
+// record d_chosen[i].  The cost pass pulls virtual streams from the work counter like the model pass, so however many there
+// are, the context's encoder slots code them as many at a time as they hold.
+static DivansResult encode_auto_device_nolock(divans_b200_ctx *ctx, size_t n, const uint8_t *d_in, const uint64_t *d_in_off,
+                                              const uint64_t *d_in_len, uint64_t max_in_len, uint8_t *d_out, const uint64_t *d_out_off,
+                                              const uint64_t *d_out_cap, uint64_t *d_out_len, int32_t *d_status,
+                                              const divans_b200_encode_options *o, const divans_b200_literal_model *cands,
+                                              uint32_t n_cands, uint32_t *d_chosen, uint64_t *d_cost, cudaStream_t st) {
+    const int window = clamp_window(o->window_size);
+    const uint64_t nv = (uint64_t)n * n_cands;
+    const uint64_t replay_stride = (max_in_len + 31) & ~15ull;
+    const size_t vslots = encode_slots(ctx, nv);
+    if (ensure_arena(ctx, vslots) != DIVANS_SUCCESS) return DIVANS_FAILURE;
+    if (!grow(ctx, &ctx->d_replay, &ctx->replay_cap, vslots * (size_t)replay_stride)) return DIVANS_FAILURE;
+    // v_off [nv] | v_len [nv] | tally [nv] | v_pm u32 [nv] | v_status i32 [nv]
+    if (!grow(ctx, &ctx->d_auto, &ctx->auto_cap, 4 * nv + 2)) return DIVANS_FAILURE;
+    uint64_t *v_off = ctx->d_auto, *v_len = v_off + nv, *tally = v_len + nv;
+    uint32_t *v_pm = reinterpret_cast<uint32_t *>(tally + nv);
+    int32_t *v_status = reinterpret_cast<int32_t *>(v_pm + nv);
+    if (!ctx->d_pm_records) CK(cudaMalloc((void **)&ctx->d_pm_records, 16 * (size_t)PM_RECORD_BYTES));
+    if (ctx->busy_recorded) CK(cudaStreamWaitEvent(st, ctx->ev_busy, 0));   // (the records and scratch may still be read by the previous call)
+    if (!ctx->d_cost_tab) {
+        static uint32_t tab[32768];
+        static std::once_flag once;
+        std::call_once(once, [] { for (uint32_t f = 0; f < 32768; f++) tab[f] = freq_cost(f); });
+        CK(cudaMalloc((void **)&ctx->d_cost_tab, sizeof tab));
+        CK(cudaMemcpyAsync(ctx->d_cost_tab, tab, sizeof tab, cudaMemcpyHostToDevice, st));
+    }
+    std::vector<uint8_t> &pm = ctx->h_pm;
+    pm.assign((size_t)n_cands * PM_RECORD_BYTES, 0);
+    for (uint32_t c = 0; c < n_cands; c++) raw_record(pm.data() + (size_t)c * PM_RECORD_BYTES, cands[c].literal_pred_mode, cands[c].literal_mixing_value);
+    CK(cudaMemcpyAsync(ctx->d_pm_records, pm.data(), pm.size(), cudaMemcpyHostToDevice, st));
+    launch_auto_fanout(d_in_off, d_in_len, n, n_cands, v_off, v_len, v_pm, st);
+
+    EncodeParams tp;
+    memset(&tp, 0, sizeof tp);
+    tp.in = d_in; tp.in_off = v_off; tp.in_len = v_len; tp.raw_mode = 1; tp.n_streams = (uint32_t)nv;
+    tp.work_counter = ctx->d_counter; tp.arena = ctx->d_arena; tp.tables = ctx->d_tables;
+    tp.pm_internal = ctx->d_pm_records; tp.pm_index = v_pm;
+    tp.replay = ctx->d_replay; tp.replay_stride = replay_stride;
+    tp.status = v_status; tp.cost_tab = ctx->d_cost_tab; tp.tally = tally;
+    tp.window_size = window; tp.max_in_len = max_in_len; tp.dynamic_context_mixing = o->dynamic_context_mixing & 0xff; tp.prior_depth = o->prior_depth & 0xff;
+    tp.use_context_map = o->use_context_map; tp.force_stride = o->force_stride; tp.have_literal_adaptation = o->have_literal_adaptation;
+    for (int k = 0; k < 4; k++) tp.literal_adaptation[k] = pack_speed(o->literal_adaptation[k]);
+    tp.model_rev = o->model_rev == DIVANS_B200_MODEL_WASM_2018 ? 1 : 0;
+    CK(cudaMemsetAsync(ctx->d_counter, 0, 4, st));
+    const uint32_t blocks = (uint32_t)(vslots / ENCODE_GROUPS_PER_BLOCK);
+    if (o->cdf_model == DIVANS_B200_CDF_BLEND) launch_encode_tally_blend(tp, blocks, st); else launch_encode_tally(tp, blocks, st);
+    launch_auto_select(tally, v_status, n, n_cands, d_chosen, d_cost, st);
+    ctx->launches += 3;
+    CK(cudaGetLastError());
+    return encode_device_internal(ctx, n, 1, d_in, d_in_off, d_in_len, max_in_len, raw_cmd_cap(max_in_len, window),
+                                  (uint32_t)(2 * max_in_len + 16), replay_stride, d_out, d_out_off, d_out_cap, d_out_len, d_status, o,
+                                  window, st, ctx->d_pm_records, d_chosen);
+}
+
+extern "C" DivansResult divans_b200_encode_auto_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_in, const uint64_t *d_in_off,
+                                                             const uint64_t *d_in_len, uint64_t max_in_len, uint8_t *d_out,
+                                                             const uint64_t *d_out_off, const uint64_t *d_out_cap, uint64_t *d_out_len,
+                                                             int32_t *d_status, const divans_b200_encode_options *opts,
+                                                             const divans_b200_literal_model *cands, uint32_t n_cands, uint32_t *d_chosen,
+                                                             uint64_t *d_cost, void *cuda_stream) {
+    if (!ctx || !opts) return DIVANS_FAILURE;
+    if (!check_cands(ctx, cands, n_cands)) return DIVANS_FAILURE;
+    if (n == 0) return DIVANS_SUCCESS;
+    if (!d_chosen) { ctx->err = "encode_auto: d_chosen is required"; return DIVANS_FAILURE; }
+    if ((uint64_t)n * n_cands > 0xffffffffull || max_in_len > 0x7fff0000ull) { ctx->err = "batch too large"; return DIVANS_FAILURE; }
+    try {
+        std::lock_guard<std::mutex> lk(ctx->mu);
+        CK(cudaSetDevice(ctx->device));
+        cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream;
+        return encode_auto_device_nolock(ctx, n, d_in, d_in_off, d_in_len, max_in_len, d_out, d_out_off, d_out_cap, d_out_len, d_status,
+                                         opts, cands, n_cands, d_chosen, d_cost, st);
+    } catch (...) { ctx->err = "divans_b200: out of host memory"; return DIVANS_FAILURE; }
+}
+
+// literal model selection of a host batch (encode_host_common): the candidates, and where chosen / cost go
+struct AutoSel {
+    const divans_b200_literal_model *cands; uint32_t n_cands;
+    uint32_t *chosen; uint64_t *cost;
+};
+
 // host batch: marshal, split into sub-batches whose symbol logs fit in HBM, run, copy back
 static DivansResult encode_host_common(divans_b200_ctx *ctx, size_t n, int raw_mode, const uint8_t *in, const uint64_t *in_off,
                                        const uint64_t *in_len, uint8_t *out, const uint64_t *out_off, const uint64_t *out_cap,
-                                       uint64_t *out_len, int32_t *status, const divans_b200_encode_options *opts) {
+                                       uint64_t *out_len, int32_t *status, const divans_b200_encode_options *opts,
+                                       const AutoSel *sel = nullptr) {
     if (!ctx || !opts) return DIVANS_FAILURE;
+    if (sel && !check_cands(ctx, sel->cands, sel->n_cands)) return DIVANS_FAILURE;
     if (n == 0) return DIVANS_SUCCESS;
+    if (sel && !sel->chosen) { ctx->err = "encode_auto: chosen is required"; return DIVANS_FAILURE; }
+    if (sel && (uint64_t)n * sel->n_cands > 0xffffffffull) { ctx->err = "batch too large"; return DIVANS_FAILURE; }
     std::lock_guard<std::mutex> lk(ctx->mu);
     CK(cudaSetDevice(ctx->device));
     const int window = clamp_window(opts->window_size);
@@ -729,7 +860,8 @@ static DivansResult encode_host_common(divans_b200_ctx *ctx, size_t n, int raw_m
         uint64_t out_lo = ~0ull, out_hi = 0;
         for (size_t i = i0; i < i1; i++) { if (out_off[i] < out_lo) out_lo = out_off[i]; if (out_off[i] + out_cap[i] > out_hi) out_hi = out_off[i] + out_cap[i]; }
         if (!grow(ctx, &ctx->d_out, &ctx->d_out_cap, (size_t)(out_hi - out_lo) + 64)) return DIVANS_FAILURE;
-        if (!grow(ctx, &ctx->d_meta, &ctx->d_meta_cap, m * 6)) return DIVANS_FAILURE;
+        // in_off | in_len | out_off | out_cap | out_len | status (+ encode_auto: chosen | cost [m * C])
+        if (!grow(ctx, &ctx->d_meta, &ctx->d_meta_cap, m * 6 + (sel ? m + m * (size_t)sel->n_cands : 0))) return DIVANS_FAILURE;
         std::vector<uint64_t> rel(m);
         for (size_t i = 0; i < m; i++) rel[i] = out_off[i0 + i] - out_lo;
         uint64_t *mm = ctx->d_meta;
@@ -738,9 +870,17 @@ static DivansResult encode_host_common(divans_b200_ctx *ctx, size_t n, int raw_m
         CK(cudaMemcpyAsync(mm + 2 * m, rel.data(), m * 8, cudaMemcpyHostToDevice, st));
         CK(cudaMemcpyAsync(mm + 3 * m, out_cap + i0, m * 8, cudaMemcpyHostToDevice, st));
         int32_t *d_status = reinterpret_cast<int32_t *>(mm + 5 * m);
-        DivansResult r = encode_device_internal(ctx, m, raw_mode, ctx->d_in, mm, mm + m, mx, (uint32_t)mc, (uint32_t)ml, mr, ctx->d_out,
-                                                mm + 2 * m, mm + 3 * m, mm + 4 * m, d_status, opts, window, st);
+        uint32_t *d_chosen = reinterpret_cast<uint32_t *>(mm + 6 * m);
+        uint64_t *d_cost = mm + 7 * m;
+        DivansResult r = sel ? encode_auto_device_nolock(ctx, m, ctx->d_in, mm, mm + m, mx, ctx->d_out, mm + 2 * m, mm + 3 * m, mm + 4 * m,
+                                                         d_status, opts, sel->cands, sel->n_cands, d_chosen, d_cost, st)
+                             : encode_device_internal(ctx, m, raw_mode, ctx->d_in, mm, mm + m, mx, (uint32_t)mc, (uint32_t)ml, mr, ctx->d_out,
+                                                      mm + 2 * m, mm + 3 * m, mm + 4 * m, d_status, opts, window, st);
         if (r != DIVANS_SUCCESS) return r;
+        if (sel) {
+            CK(cudaMemcpyAsync(sel->chosen + i0, d_chosen, m * 4, cudaMemcpyDeviceToHost, st));
+            if (sel->cost) CK(cudaMemcpyAsync(sel->cost + i0 * sel->n_cands, d_cost, m * (size_t)sel->n_cands * 8, cudaMemcpyDeviceToHost, st));
+        }
         CK(cudaMemcpyAsync(out_len + i0, mm + 4 * m, m * 8, cudaMemcpyDeviceToHost, st));
         CK(cudaMemcpyAsync(status + i0, d_status, m * 4, cudaMemcpyDeviceToHost, st));
         CK(cudaStreamSynchronize(st));
@@ -758,6 +898,15 @@ extern "C" DivansResult divans_b200_encode_batch_host(divans_b200_ctx *ctx, size
                                                       const divans_b200_encode_options *opts) {
     // (host marshalling uses std::vector sized by the caller's arguments: no C++ exception may cross the C boundary)
     try { return encode_host_common(ctx, n, 1, in, in_off, in_len, out, out_off, out_cap, out_len, status, opts); }
+    catch (...) { if (ctx) ctx->err = "divans_b200: out of host memory while marshalling the batch"; return DIVANS_FAILURE; }
+}
+extern "C" DivansResult divans_b200_encode_auto_batch_host(divans_b200_ctx *ctx, size_t n, const uint8_t *in, const uint64_t *in_off,
+                                                           const uint64_t *in_len, uint8_t *out, const uint64_t *out_off, const uint64_t *out_cap,
+                                                           uint64_t *out_len, int32_t *status, const divans_b200_encode_options *opts,
+                                                           const divans_b200_literal_model *cands, uint32_t n_cands, uint32_t *chosen,
+                                                           uint64_t *cost) {
+    const AutoSel sel = {cands, n_cands, chosen, cost};
+    try { return encode_host_common(ctx, n, 1, in, in_off, in_len, out, out_off, out_cap, out_len, status, opts, &sel); }
     catch (...) { if (ctx) ctx->err = "divans_b200: out of host memory while marshalling the batch"; return DIVANS_FAILURE; }
 }
 extern "C" DivansResult divans_b200_encode_cmds_batch_host(divans_b200_ctx *ctx, size_t n, const uint8_t *blobs, const uint64_t *blob_off,

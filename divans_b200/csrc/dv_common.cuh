@@ -169,6 +169,12 @@ struct EncodeParams {
     // max_in_len (the bound cmd_cap / lit_cap were derived from) is refused unread
     uint64_t max_in_len;
     uint32_t *stream_window;      // per stream: the window the model pass coded it with (the mux writes it into the header)
+    // raw mode: stream v starts with record pm_internal + pm_index[v] * PM_RECORD_BYTES (nullptr: record 0 for every stream)
+    const uint32_t *pm_index;
+    // cost-only model pass (encode_model_kernel<BLEND, true>): no logs; per stream the sum of cost_tab[freq] over every coded
+    // nibble of both coders, in 1/65536 bit (cost_tab[f] = -log2(f / 32768), include/divans_b200.h)
+    const uint32_t *cost_tab;
+    uint64_t *tally;
 };
 constexpr uint32_t PM_RECORD_BYTES = 32 + 16384 + 1024 + 8192;
 

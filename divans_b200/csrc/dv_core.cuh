@@ -16,14 +16,19 @@ constexpr int SMEM_BYTES_PER_GROUP = (int)((sizeof(Cold) + 15) / 16 * 16);
 // Encoder: log one coded nibble.  A frequency <= 0 (a stream-supplied speed wrapped an i16 counter) cannot be coded: the
 // reference encoder panics on it and the oracle refuses the stream (ans_enc_put), so the stream fails, as in the blend core.
 // An idle group codes the dummy prior and is never failed.
+// TALLY (the cost-only pass, encode_model_kernel<BLEND, true>): nothing is logged.  The coder's `p` is the cost table and its
+// `a` (unused by the encoder otherwise) the running cost; every lane of the group adds the same value.
+template <bool TALLY = false>
 __device__ __forceinline__ void enc_log(St &s, const G2 g, int start, int freq) {
     if (freq <= 0 && s.state != S_IDLE) s.status = ST_FAIL;
-    if (g.store0) const_cast<uint32_t *>(s.cur.p)[s.cur.left] = ((uint32_t)start & 0xffffu) | ((uint32_t)freq << 16);
+    if constexpr (TALLY) s.cur.a += __ldg(s.cur.p + ((uint32_t)freq & 0x7fffu));
+    else if (g.store0) const_cast<uint32_t *>(s.cur.p)[s.cur.left] = ((uint32_t)start & 0xffffu) | ((uint32_t)freq << 16);
     s.cur.left++;
 }
 
 // The encoder's converged nibble core.  Every lane of the warp executes it every iteration, unpredicated: a group without
 // work codes against its slot's dummy CDF with a parked coder (no memory side effects that matter).
+template <bool TALLY = false>
 __device__ __forceinline__ int nibble_core_enc(St &s, const Next &nx, const G2 g) {
     const Grp gg = {FULL, g.l16};
     const int c = nx.cdf[g.l16], maxv = nx.cdf[15];
@@ -36,7 +41,7 @@ __device__ __forceinline__ int nibble_core_enc(St &s, const Next &nx, const G2 g
         int lo = __shfl_sync(FULL, cum, (sym - 1) & 15, 16);
         if (sym == 0) lo = 0;
         start = (int)(short)(lo + 1); freq = (int)(short)(hi - lo - 1);   // "major hax", probability/interface.rs:103-104
-        enc_log(s, g, start, freq);
+        enc_log<TALLY>(s, g, start, freq);
         int c2 = cdf_blend(gg, c, maxv, sym, inc, lim);
         nx.cdf[g.l16] = (int16_t)c2;
         return sym;
@@ -61,7 +66,7 @@ __device__ __forceinline__ int nibble_core_enc(St &s, const Next &nx, const G2 g
     start = (int)(short)(lo + 1); freq = (int)(short)(hi - lo - 1);
     int f_cm = cdf_freq(gg, cc, mc, sym);
     int f_nb = cdf_freq(gg, c, maxv, sym);
-    enc_log(s, g, start, freq);
+    enc_log<TALLY>(s, g, start, freq);
     if (mixg) {
         weights_update(w, f_cm, f_nb, freq);
         if (nx.mix_hi) s.c->w_hi = w; else s.c->w_lo = w;
@@ -142,6 +147,7 @@ __device__ __forceinline__ MixSym mix_search(const MixVals v, const Weights &w, 
     r.sym = sym;
     return r;
 }
+template <bool TALLY>
 __device__ __forceinline__ void mix_finish(Coder &k, const G2 g, char *nb, char *cm, const MixVals v, const MixSym ms, Weights &w,
                                            const int nb_inc, const int nb_lim, const int cm_inc, const int cm_lim, bool &refused) {
     const int sym = ms.sym;
@@ -157,7 +163,8 @@ __device__ __forceinline__ void mix_finish(Coder &k, const G2 g, char *nb, char 
     const int f_nb = (int)(short)(((unsigned)hi_pn >> 16) - ((unsigned)lo_pn >> 16) - 1);
     // small speeds keep both priors' steps >= 3, but their average can still round to a step of 1: freq 0 (see enc_log)
     refused |= freq <= 0;
-    if (g.store0) const_cast<uint32_t *>(k.p)[k.left] = ((uint32_t)start & 0xffffu) | ((uint32_t)freq << 16);
+    if constexpr (TALLY) k.a += __ldg(k.p + ((uint32_t)freq & 0x7fffu));
+    else if (g.store0) const_cast<uint32_t *>(k.p)[k.left] = ((uint32_t)start & 0xffffu) | ((uint32_t)freq << 16);
     k.left++;
     weights_update32(w, f_cm, f_nb, freq);
     const Grp gg = {FULL, g.l16};
@@ -170,6 +177,7 @@ __device__ __forceinline__ void mix_finish(Coder &k, const G2 g, char *nb, char 
 // bytes (high nibble, low nibble, context of the next byte) back to back without going through the state-machine dispatch.
 // This is code_nibble_array (codec/literal.rs:261-394) for two streams at once.  The common case -- no dynamic context
 // mixing and one mixing-mask value for the whole map -- gets a loop with every selector hoisted out.
+template <bool TALLY>
 __device__ __forceinline__ void literal_fast_enc(St &s, Next &nx, const G2 g) {
     const uint32_t n = min(s.lit_left, __shfl_xor_sync(FULL, s.lit_left, 16));
     const bool simple = __all_sync(FULL, !s.mixing_trait && s.lit_cfg >= 0 && s.speeds_small);
@@ -222,7 +230,8 @@ __device__ __forceinline__ void literal_fast_enc(St &s, Next &nx, const G2 g) {
                     int lo = __shfl_sync(FULL, cum, (h - 1) & 15, 16);
                     if (h == 0) lo = 0;
                     const uint32_t start = (uint32_t)(lo + 1), freq = (uint32_t)(hi - lo - 1);   // "major hax", probability/interface.rs:103-104
-                    if (g.store0) const_cast<uint32_t *>(k.p)[k.left] = (start & 0xffffu) | (freq << 16);
+                    if constexpr (TALLY) k.a += __ldg(k.p + (freq & 0x7fffu));
+                    else if (g.store0) const_cast<uint32_t *>(k.p)[k.left] = (start & 0xffffu) | (freq << 16);
                     k.left++;
                     int c2 = ch + ((g.l16 >= h) ? inc : 0);
                     if (mh + inc >= lim) { const int t = c2 + g.l16 + 1; c2 = t - (t >> 2); }
@@ -246,7 +255,8 @@ __device__ __forceinline__ void literal_fast_enc(St &s, Next &nx, const G2 g) {
                     int lo = __shfl_sync(FULL, cum, (l - 1) & 15, 16);
                     if (l == 0) lo = 0;
                     const uint32_t start = (uint32_t)(lo + 1), freq = (uint32_t)(hi - lo - 1);
-                    if (g.store0) const_cast<uint32_t *>(k.p)[k.left] = (start & 0xffffu) | (freq << 16);
+                    if constexpr (TALLY) k.a += __ldg(k.p + (freq & 0x7fffu));
+                    else if (g.store0) const_cast<uint32_t *>(k.p)[k.left] = (start & 0xffffu) | (freq << 16);
                     k.left++;
                     int c2 = cl + ((g.l16 >= l) ? inc : 0);
                     if (ml + inc >= lim) { const int t = c2 + g.l16 + 1; c2 = t - (t >> 2); }
@@ -300,7 +310,7 @@ __device__ __forceinline__ void literal_fast_enc(St &s, Next &nx, const G2 g) {
                 char *const nbl = lo_tab + (ic * 256u + ib) * 32u, *const cml = cmb + (256u + h + 16u * ctx) * 32u;
                 __syncwarp();
                 const MixVals vl = mix_load(g, nbl, cml);
-                mix_finish(k, g, nbh, cmh, vh, sh_, wh, inc, lim, ch_inc, ch_lim, refused);
+                mix_finish<TALLY>(k, g, nbh, cmh, vh, sh_, wh, inc, lim, ch_inc, ch_lim, refused);
                 const MixSym sl_ = mix_search(vl, wl, (int)(byte_in & 0xf));
                 const uint32_t cur = ((uint32_t)sl_.sym | (h << 4)) & 0xff;
                 l8 = (l8 >> 8) | ((unsigned long long)cur << 56);
@@ -311,7 +321,7 @@ __device__ __forceinline__ void literal_fast_enc(St &s, Next &nx, const G2 g) {
                 nbh = hi_tab + (ctx * 256u + ((uint32_t)(l8 >> sh) & mm & (~o1 & 0xffu))) * 32u; cmh = cmb + ctx * 32u;
                 __syncwarp();
                 vh = mix_load(g, nbh, cmh);   // speculative on the last byte: initialised slabs
-                mix_finish(k, g, nbl, cml, vl, sl_, wl, inc, lim, cl_inc, cl_lim, refused);
+                mix_finish<TALLY>(k, g, nbl, cml, vl, sl_, wl, inc, lim, cl_inc, cl_lim, refused);
             }
             done += m;
         }
@@ -323,11 +333,11 @@ __device__ __forceinline__ void literal_fast_enc(St &s, Next &nx, const G2 g) {
     }
     for (uint32_t i = 0; i < n; i++) {
         __syncwarp();
-        int h = nibble_core_enc(s, nx, g);
+        int h = nibble_core_enc<TALLY>(s, nx, g);
         s.lit_h = (uint32_t)h;
         enter_lit_nibble<true, false>(s, nx);
         __syncwarp();
-        int l = nibble_core_enc(s, nx, g);
+        int l = nibble_core_enc<TALLY>(s, nx, g);
         uint32_t cur = ((uint32_t)l | ((uint32_t)h << 4)) & 0xff;
         s.l8 = (s.l8 >> 8) | ((unsigned long long)cur << 56);   // push_literal_byte, codec/interface.rs:280-284
         if (g.store0) s.out[s.out_pos] = (uint8_t)cur;
@@ -339,10 +349,10 @@ __device__ __forceinline__ void literal_fast_enc(St &s, Next &nx, const G2 g) {
 }
 
 // the encoder's nibble core of the kernel's probability model
-template <bool BLEND>
+template <bool BLEND, bool TALLY>
 __device__ __forceinline__ int core_dispatch(St &s, const Next &nx, const G2 g) {
-    if constexpr (BLEND) return nibble_core_blend<true>(s, nx, g);
-    else return nibble_core_enc(s, nx, g);
+    if constexpr (BLEND) return nibble_core_blend<true, TALLY>(s, nx, g);
+    else return nibble_core_enc<TALLY>(s, nx, g);
 }
 
 }  // namespace dv

@@ -5,6 +5,9 @@
 //   1. encode_model_kernel  the lock-step engine (dv_engine.cuh) run with ENC=true: walks the command list, adapts
 //                           the priors exactly as the decoder will, and logs one (start | freq << 16) word per nibble
 //                           into the stream's command / literal log.
+//                           TALLY = true is the cost-only variant (encode_model_kernel<BLEND, true>, divans_b200_encode_auto_*):
+//                           the same walk, but each coded nibble adds cost_tab[freq] to the stream's total instead of
+//                           writing a log entry.  It has no logs, so no log capacity, and no passes 2 and 3.
 //   2. encode_flush_kernel  one thread per (65536-symbol chunk, rANS state) runs the recurrence last symbol -> first
 //                           symbol (ans.rs:302-378); encode_pack_kernel then stacks the renormalisation words in
 //                           symbol order IN PLACE at the top of the chunk's own log region (<= one word per symbol).
@@ -14,7 +17,7 @@
 
 namespace dv {
 
-template <bool BLEND>
+template <bool BLEND, bool TALLY>
 __global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) encode_model_kernel(EncodeParams p) {
     extern __shared__ __align__(16) uint8_t smem[];
     const int lane = threadIdx.x & 31;
@@ -36,11 +39,12 @@ __global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) encode_model_kernel(E
     s.state = S_IDLE;
     s.c->in.cmds = nullptr; s.c->in.n_cmds = 0; s.c->in.pos = 0; s.c->in.n_pms = 0; s.c->in.pms = nullptr; s.c->in.lits = nullptr;
     s.c->model_rev = (uint32_t)p.model_rev;
-    s.c->sidx = 0; s.c->raw_len = 0; s.c->lit_log_cap = p.lit_cap;
+    s.c->sidx = 0; s.c->raw_len = 0; s.c->lit_log_cap = TALLY ? 0xffffffffu : p.lit_cap;   // (TALLY: no log to outgrow)
     s.out = p.replay + (uint64_t)slot * p.replay_stride; s.out_pos = 0;
     s.c->out_cap = p.replay_stride > 0xffffffffull ? 0xffffffffu : (uint32_t)p.replay_stride;
     st_reset(s);
-    uint32_t *const dummy_log = p.sf_dummy + slot;
+    // TALLY: every coder, parked ones included, reads the cost table through `p` and never writes (enc_log)
+    uint32_t *const dummy_log = TALLY ? const_cast<uint32_t *>(p.cost_tab) : p.sf_dummy + slot;
     coder_init_enc(s.cur, dummy_log); coder_init_enc(s.c->oth, dummy_log);
     Next nx; nx.cdf = A_misc(s, MI_DUMMY); nx.cdf2 = nullptr; nx.speed = SPK_NONE; nx.tagged = false; nx.sym = 0; nx.mix_hi = false;
     store_default_cdfs(g, reinterpret_cast<int16_t *>(s.slot + OFF_MISC), (uint32_t)MISC_CDFS);
@@ -76,7 +80,8 @@ __global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) encode_model_kernel(E
                     uint32_t win = (uint32_t)p.window_size;   // 0 (command lists only): the window of the blob's header
                     if (p.raw_mode) {
                         if (blen > 0xffffffffull - 16) ok = false;
-                        s.c->in.cmds = nullptr; s.c->in.pms = p.pm_internal; s.c->in.n_pms = 1; s.c->in.lits = blob;
+                        s.c->in.cmds = nullptr; s.c->in.n_pms = 1; s.c->in.lits = blob;
+                        s.c->in.pms = p.pm_internal + (p.pm_index ? (uint64_t)p.pm_index[v] * PM_RECORD_BYTES : 0ull);
                         s.c->raw_len = (uint32_t)blen;
                         s.c->in.n_cmds = 1u + (uint32_t)((blen + (1ull << win) - 1) >> win);
                     } else {
@@ -95,8 +100,16 @@ __global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) encode_model_kernel(E
                             s.c->raw_len = h[4];
                         }
                     }
-                    if (!ok) { if (g.store0) { p.status[v] = ST_FAIL; p.sf_counts[2 * v] = 0; p.sf_counts[2 * v + 1] = 0; } }
-                    else {
+                    if (!ok) {
+                        if (g.store0) {
+                            p.status[v] = ST_FAIL;
+                            if constexpr (TALLY) p.tally[v] = 0; else { p.sf_counts[2 * v] = 0; p.sf_counts[2 * v + 1] = 0; }
+                        }
+                    } else if constexpr (TALLY) {
+                        s.c->ring_len = 1u << win;
+                        coder_init_enc(s.cur, dummy_log); coder_init_enc(s.c->oth, dummy_log);   // (a = 0: the stream's cost so far)
+                        enter_cmd_type<true>(s, nx);
+                    } else {
                         s.c->ring_len = 1u << win;
                         if (g.store0) p.stream_window[v] = win;
                         coder_init_enc(s.cur, p.sf + (uint64_t)v * per_stream);                   // CMD_CODER
@@ -111,7 +124,8 @@ __global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) encode_model_kernel(E
         // end of a stream: report it, park the group on the dummy prior
         auto finish = [&]() {
             const uint32_t v = s.c->sidx;
-            if (g.store0) {
+            if (g.store0 && TALLY) { p.status[v] = s.status; p.tally[v] = s.cur.a + s.c->oth.a; }
+            if (g.store0 && !TALLY) {
                 p.status[v] = s.status;
                 const uint32_t nc = s.c->cur_is_lit ? s.c->oth.left : s.cur.left, nl = s.c->cur_is_lit ? s.cur.left : s.c->oth.left;
                 p.sf_counts[2 * v] = s.status == ST_OK ? nc : 0; p.sf_counts[2 * v + 1] = s.status == ST_OK ? nl : 0;
@@ -121,18 +135,18 @@ __global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) encode_model_kernel(E
             coder_init_enc(s.cur, dummy_log);
         };
         if (!BLEND && __all_sync(FULL, s.state == S_LIT_HI)) {
-            literal_fast_enc(s, nx, g);
+            literal_fast_enc<TALLY>(s, nx, g);
             if (s.lit_left == 0 && s.status == ST_OK) { swap_coders(s, g); s.c->in.pos++; enter_cmd_type<true>(s, nx); }
             if (s.status != ST_OK) finish();   // a symbol the loop could not code (enc_log): the stream ends here
             continue;
         }
         const bool busy = s.state != S_IDLE;
-        int sym = core_dispatch<BLEND>(s, nx, g);
+        int sym = core_dispatch<BLEND, TALLY>(s, nx, g);
         if (!busy) s.cur.left = 0;
         else {
             if (s.status == ST_OK) {   // (else the core could not code the symbol: enc_log)
                 // log overflow cannot happen for command lists whose sizes match the header; guard hostile blobs anyway
-                if (s.cur.left + 1 >= (s.c->cur_is_lit ? p.lit_cap : p.cmd_cap)) s.status = ST_FAIL;
+                if (!TALLY && s.cur.left + 1 >= (s.c->cur_is_lit ? p.lit_cap : p.cmd_cap)) s.status = ST_FAIL;
                 else transition<true>(s, nx, g, sym);
             }
             if (s.status != ST_OK || s.state == S_IDLE) finish();
@@ -382,12 +396,58 @@ __global__ void __launch_bounds__(128) encode_mux_kernel(EncodeParams p) {
 #ifdef DV_BLEND
 void launch_encode_model_blend(const EncodeParams &p, uint32_t n_blocks, cudaStream_t st) {
     size_t smem = (size_t)(DECODE_BLOCK_THREADS / 16) * SMEM_BYTES_PER_GROUP;
-    encode_model_kernel<true><<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p);
+    encode_model_kernel<true, false><<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p);
+}
+void launch_encode_tally_blend(const EncodeParams &p, uint32_t n_blocks, cudaStream_t st) {
+    size_t smem = (size_t)(DECODE_BLOCK_THREADS / 16) * SMEM_BYTES_PER_GROUP;
+    encode_model_kernel<true, true><<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p);
 }
 #else
 void launch_encode_model(const EncodeParams &p, uint32_t n_blocks, cudaStream_t st) {
     size_t smem = (size_t)(DECODE_BLOCK_THREADS / 16) * SMEM_BYTES_PER_GROUP;
-    encode_model_kernel<false><<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p);
+    encode_model_kernel<false, false><<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p);
+}
+void launch_encode_tally(const EncodeParams &p, uint32_t n_blocks, cudaStream_t st) {
+    size_t smem = (size_t)(DECODE_BLOCK_THREADS / 16) * SMEM_BYTES_PER_GROUP;
+    encode_model_kernel<false, true><<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// model selection (divans_b200_encode_auto_*): n streams x C candidate PredictionMode records
+// ---------------------------------------------------------------------------------------------------------------
+// Virtual stream v = c * n + i codes stream i under candidate c.  Candidate-major: the work counter hands consecutive virtual
+// streams to the two groups of a warp, so warp mates code the same literal context mode and mixing value (the fast loop's
+// per-mode context lookup stays converged) on neighbouring streams.
+__global__ void auto_fanout_kernel(const uint64_t *in_off, const uint64_t *in_len, uint64_t n, uint32_t n_cands, uint64_t *v_off,
+                                   uint64_t *v_len, uint32_t *v_pm) {
+    const uint64_t v = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (v >= n * n_cands) return;
+    const uint64_t i = v % n;
+    v_off[v] = in_off[i]; v_len[v] = in_len[i]; v_pm[v] = (uint32_t)(v / n);
+}
+// chosen[i] = argmin_c cost of (i, c), ties to the lowest c; a candidate the tally pass failed costs UINT64_MAX.  cost (optional)
+// is the matrix row per stream: cost[i * C + c].
+__global__ void auto_select_kernel(const uint64_t *tally, const int32_t *v_status, uint64_t n, uint32_t n_cands, uint32_t *chosen,
+                                   uint64_t *cost) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    uint64_t best = ~0ull; uint32_t arg = 0;
+    for (uint32_t c = 0; c < n_cands; c++) {
+        const uint64_t v = (uint64_t)c * n + i;
+        const uint64_t t = v_status[v] == ST_OK ? tally[v] : ~0ull;
+        if (cost) cost[i * n_cands + c] = t;
+        if (t < best) { best = t; arg = c; }
+    }
+    chosen[i] = arg;
+}
+void launch_auto_fanout(const uint64_t *in_off, const uint64_t *in_len, uint64_t n, uint32_t n_cands, uint64_t *v_off, uint64_t *v_len,
+                        uint32_t *v_pm, cudaStream_t st) {
+    const uint64_t nv = n * n_cands;
+    auto_fanout_kernel<<<(unsigned)((nv + 255) / 256), 256, 0, st>>>(in_off, in_len, n, n_cands, v_off, v_len, v_pm);
+}
+void launch_auto_select(const uint64_t *tally, const int32_t *v_status, uint64_t n, uint32_t n_cands, uint32_t *chosen, uint64_t *cost,
+                        cudaStream_t st) {
+    auto_select_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(tally, v_status, n, n_cands, chosen, cost);
 }
 // M[f] = floor((2^64 - 1) / f), f = 1..32767 (entry 0 unused)
 __global__ void rcp15_init_kernel(uint64_t *tab) {
@@ -402,7 +462,7 @@ void launch_encode_flush_mux(const EncodeParams &p, cudaStream_t st) {
     encode_mux_kernel<<<(p.n_streams + 3) / 4, 128, 0, st>>>(p);
 }
 int encode_max_blocks_per_sm() {
-    const int nb = stream_kernel_blocks_per_sm(encode_model_kernel<false>, DECODE_BLOCK_THREADS, (size_t)(DECODE_BLOCK_THREADS / 16) * SMEM_BYTES_PER_GROUP);
+    const int nb = stream_kernel_blocks_per_sm(encode_model_kernel<false, false>, DECODE_BLOCK_THREADS, (size_t)(DECODE_BLOCK_THREADS / 16) * SMEM_BYTES_PER_GROUP);
     return nb;
 }
 

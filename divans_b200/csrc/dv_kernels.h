@@ -26,6 +26,14 @@ void launch_decode16_blend(const DecodeParams &p, uint32_t n_blocks, cudaStream_
 int decode_max_blocks_per_sm16_blend();
 void launch_encode_model_blend(const EncodeParams &p, uint32_t n_blocks, cudaStream_t st);
 void launch_rcp15_init(uint64_t *tab, cudaStream_t st);
+// model selection: the cost-only model passes (no logs: EncodeParams::cost_tab / tally), the fan-out of n streams to n x C
+// virtual streams (candidate-major) and the per-stream argmin
+void launch_encode_tally(const EncodeParams &p, uint32_t n_blocks, cudaStream_t st);
+void launch_encode_tally_blend(const EncodeParams &p, uint32_t n_blocks, cudaStream_t st);
+void launch_auto_fanout(const uint64_t *in_off, const uint64_t *in_len, uint64_t n, uint32_t n_cands, uint64_t *v_off, uint64_t *v_len,
+                        uint32_t *v_pm, cudaStream_t st);
+void launch_auto_select(const uint64_t *tally, const int32_t *v_status, uint64_t n, uint32_t n_cands, uint32_t *chosen, uint64_t *cost,
+                        cudaStream_t st);
 // decoding to command lists: the recording decoders (16 lanes per stream) and the pack kernel that finishes the blobs
 void launch_decode_v2_rec(const DecodeParams &p, const RecParams &r, uint32_t n_blocks, cudaStream_t st);
 void launch_decode16_blend_rec(const DecodeParams &p, const RecParams &r, uint32_t n_blocks, cudaStream_t st);

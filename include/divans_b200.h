@@ -270,6 +270,45 @@ DivansResult divans_b200_encode_cmds_batch_device(divans_b200_ctx *ctx, size_t n
                                                   uint8_t *d_out, const uint64_t *d_out_off, const uint64_t *d_out_cap,
                                                   uint64_t *d_out_len, int32_t *d_status, const divans_b200_encode_options *opts,
                                                   void *cuda_stream);
+
+/* ---- literal model selection ----
+ * A candidate literal model of the raw-buffer encoder: the PredictionMode record divans_b200_encode_batch_host builds from
+ * opts->literal_pred_mode / literal_mixing_value (LSB6=0 MSB6=1 UTF8=2 SIGN=3; mixing value 0..15). */
+typedef struct {
+    int32_t literal_pred_mode;
+    int32_t literal_mixing_value;
+} divans_b200_literal_model;
+/* Encode n raw HOST buffers, each with the cheapest of n_cands candidate literal models.
+ *  - A cost-only pass runs the encoder's model walk for every (stream, candidate) pair and sums, over every coded nibble of
+ *    both coders, T[freq] = 65536 * -log2(freq / 32768) (1/65536 bit; the exact integer rule is freq_cost in dv_capi.cu).
+ *    chosen[i] = the candidate with the lowest sum, ties to the lowest index.  Then stream i is encoded once with candidate
+ *    chosen[i]: its bytes, out_len and status equal divans_b200_encode_batch_host's with opts->literal_pred_mode /
+ *    literal_mixing_value set to that candidate (status 2: out_len is the size the chosen stream needs).
+ *  - opts supplies every other option; its literal_pred_mode / literal_mixing_value are ignored.
+ *  - cands: 1..16 entries, pred_mode 0..3, mixing value 0..15; anything else returns DIVANS_FAILURE (divans_b200_last_error
+ *    says why) before any work.  Mixing value 2 (the flat prior that never adapts) is accepted but decodes on the generic path.
+ *  - cost (may be NULL): n * n_cands sums, row per stream (cost[i * n_cands + c]).  A candidate whose pass failed (status 3, e.g.
+ *    a literal_adaptation speed that wraps) costs UINT64_MAX; when every candidate failed, chosen[i] = 0 and the stream fails.
+ *  - A stream's two coder payloads hold between cost / 8 bytes and 16 bytes per 65536-symbol rANS chunk more (DESIGN.md
+ *    section 4, "Literal model selection").
+ *  - The cost pass runs the model walk C times, so the call takes about C plain encodes.
+ *  - n == 0 returns DIVANS_SUCCESS. */
+DivansResult divans_b200_encode_auto_batch_host(divans_b200_ctx *ctx, size_t n, const uint8_t *in, const uint64_t *in_off,
+                                                const uint64_t *in_len, uint8_t *out, const uint64_t *out_off, const uint64_t *out_cap,
+                                                uint64_t *out_len, int32_t *status, const divans_b200_encode_options *opts,
+                                                const divans_b200_literal_model *cands, uint32_t n_cands, uint32_t *chosen,
+                                                uint64_t *cost);
+/* Same as divans_b200_encode_auto_batch_host with the buffers, d_chosen and d_cost DEVICE pointers (cands is a host array,
+ * copied before the call returns).  Conventions of divans_b200_encode_batch_device: `max_in_len` >= every in_len[i];
+ * asynchronous on `cuda_stream` (NULL = the context's own stream), serialised on the context.  One launch sequence, no host
+ * synchronisation: the cost pass runs the n * n_cands (stream, candidate) pairs through the context's encoder slots, as many at
+ * a time as the slots hold. */
+DivansResult divans_b200_encode_auto_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_in, const uint64_t *d_in_off,
+                                                  const uint64_t *d_in_len, uint64_t max_in_len, uint8_t *d_out,
+                                                  const uint64_t *d_out_off, const uint64_t *d_out_cap, uint64_t *d_out_len,
+                                                  int32_t *d_status, const divans_b200_encode_options *opts,
+                                                  const divans_b200_literal_model *cands, uint32_t n_cands, uint32_t *d_chosen,
+                                                  uint64_t *d_cost, void *cuda_stream);
 /* IR text front-end (reference: src/bin/divans.rs:191-483, the textual IR that `divans -i` consumes): parse `ir_text` into a
  * DVCL blob.  *blob_len receives the size of the blob; with out == NULL or out_cap too small the call returns
  * DIVANS_NEEDS_MORE_OUTPUT.  *window_size (optional) receives the `window` line's value (0 if absent).  Host only. */

@@ -1,0 +1,90 @@
+/*
+ * tally_api.c -- literal model selection on top of the CPU oracle.  TEST INFRASTRUCTURE, NOT PRODUCT CODE.
+ *
+ * oracle_tally/tally_py.py compiles this file appended to a copy of oracle/divans_oracle.c whose ans_enc_put has one hook
+ * inserted (dvt_tally, below): while dvt_tally is set, every symbol the encoder would code adds the cost of its frequency to
+ * *dvt_tally instead of being recorded.  So the walk is the oracle's encoder walk itself -- the same commands, priors and
+ * end-of-stream nibble -- and only what happens to each (start, freq) differs.  This is the cost rule of the reference's
+ * TallyingArithmeticEncoder (ir_optimize/statistics_tracking_codec.rs:20-42) in fixed point.
+ *
+ * The functions here see the oracle's static helpers (cl_add, internal_predmode, ...) because they share its translation unit.
+ */
+
+/* cost of a symbol of frequency f (1..32767 of 32768) in 1/65536 bit: 65536 * (15 - log2 f), the 16 fraction bits of log2 f by
+ * repeated squaring of the mantissa.  Integer-only: the GPU library's table (divans_b200/csrc/dv_capi.cu, freq_cost) is the
+ * same rule, so GPU and oracle costs are equal, not merely close.  f = 0 costs as f = 1. */
+static uint32_t dvt_freq_cost(uint32_t f) {
+    if (f == 0) f = 1;
+    uint32_t e = 0;
+    while ((f >> (e + 1)) != 0) e++;
+    uint64_t x = (uint64_t)f << (31 - e);
+    uint32_t frac = 0;
+    for (int i = 0; i < 16; i++) {
+        x = (x * x) >> 31;
+        frac <<= 1;
+        if (x >= ((uint64_t)1 << 32)) { x >>= 1; frac |= 1; }
+    }
+    return (15u << 16) - ((e << 16) | frac);
+}
+
+void dvo_cost_table(uint32_t *tab) { for (uint32_t f = 0; f < 32768; f++) tab[f] = dvt_freq_cost(f); }
+
+/* the walk of dvo_encode_cmds without output: *cost = the sum of the costs of every coded nibble of both coders, the
+ * end-of-stream nibble included; a list the encoder refuses returns its failure with *cost = UINT64_MAX */
+int dvo_tally_cmds(const dvo_cmdlist *l, const dvo_options *o, uint64_t *cost) {
+    uint8_t frame[4096];   /* the framing of two empty payloads: header, EOF marker, trailer */
+    size_t n = 0;
+    uint64_t t = 0;
+    dvt_tally = &t;
+    int rc = dvo_encode_cmds(l, o, frame, sizeof frame, &n);
+    dvt_tally = NULL;
+    *cost = rc == DVO_SUCCESS ? t : UINT64_MAX;
+    return rc;
+}
+
+/* dvo_encode_raw's command list with the PredictionMode record of (pred_mode, mixing_value): one PredictionMode command, then
+ * Literal commands of at most 2^window bytes (the GPU raw-mode encoder's list for the same options) */
+static void dvt_raw_cmds(const uint8_t *in, size_t n, int window_size, int pred_mode, int mixing_value, dvo_cmdlist *l) {
+    int window = window_size < 10 ? 10 : (window_size > 24 ? 24 : window_size);
+    dvo_cmd *c = cl_add(l); c->type = DVO_CMD_PREDMODE; c->a = 0;
+    internal_predmode(cl_add_pm(l), pred_mode, mixing_value);
+    size_t ring = (size_t)1 << window;
+    for (size_t pos = 0; pos < n;) {
+        size_t chunk = n - pos < ring ? n - pos : ring;
+        size_t off = cl_add_lit(l, in + pos, chunk);
+        c = cl_add(l); c->type = DVO_CMD_LITERAL; c->a = (uint32_t)off; c->b = (uint32_t)chunk; c->c = 0;
+        pos += chunk;
+    }
+}
+
+int dvo_encode_raw_model(const uint8_t *in, size_t n, const dvo_options *o, int pred_mode, int mixing_value, uint8_t *out, size_t cap,
+                         size_t *out_len) {
+    dvo_cmdlist l; dvo_cmdlist_init(&l);
+    dvt_raw_cmds(in, n, o->window_size, pred_mode, mixing_value, &l);
+    int rc = dvo_encode_cmds(&l, o, out, cap, out_len);
+    dvo_cmdlist_free(&l);
+    return rc;
+}
+
+int dvo_tally_raw(const uint8_t *in, size_t n, const dvo_options *o, int pred_mode, int mixing_value, uint64_t *cost) {
+    dvo_cmdlist l; dvo_cmdlist_init(&l);
+    dvt_raw_cmds(in, n, o->window_size, pred_mode, mixing_value, &l);
+    int rc = dvo_tally_cmds(&l, o, cost);
+    dvo_cmdlist_free(&l);
+    return rc;
+}
+
+/* cands = n_cands (pred_mode, mixing_value) pairs: *chosen = the argmin of their costs (ties to the lowest index; costs[c]
+ * optional), and the stream encoded with it */
+int dvo_encode_auto(const uint8_t *in, size_t n, const dvo_options *o, const int32_t *cands, uint32_t n_cands, uint8_t *out, size_t cap,
+                    size_t *out_len, uint32_t *chosen, uint64_t *costs) {
+    uint64_t best = UINT64_MAX; uint32_t arg = 0;
+    for (uint32_t c = 0; c < n_cands; c++) {
+        uint64_t t;
+        dvo_tally_raw(in, n, o, cands[2 * c], cands[2 * c + 1], &t);
+        if (costs) costs[c] = t;
+        if (t < best) { best = t; arg = c; }
+    }
+    *chosen = arg;
+    return dvo_encode_raw_model(in, n, o, cands[2 * arg], cands[2 * arg + 1], out, cap, out_len);
+}
