@@ -44,6 +44,7 @@ BATCH_SYMBOLS = [
     "divans_b200_decode_batch_host_async", "divans_b200_decode_batch_host_wait", "divans_b200_lz77_cmds_batch", "divans_b200_kernel_version", "divans_b200_last_lanes",
     "divans_b200_debug_slot_header", "divans_b200_decode_cmds_batch_host", "divans_b200_decode_cmds_batch_device",
     "divans_b200_encode_cmds_batch_device", "divans_b200_encode_auto_batch_host", "divans_b200_encode_auto_batch_device",
+    "divans_b200_encode_cmds_auto_batch_host", "divans_b200_encode_cmds_auto_batch_device",
 ]
 PM_RECORD_BYTES = 32 + 16384 + 1024 + 8192   # one prediction-mode record of a DVCL blob (include/divans_b200.h)
 
@@ -70,6 +71,12 @@ class LiteralModel(ctypes.Structure):
 # under encode_auto exceeds its cost under the default.  The others are the models that code the survey corpora in the
 # fewest bits (tools/auto_probe.py --survey, DESIGN.md section 4); mixing value 2 is left out (it decodes on the generic path).
 DEFAULT_LITERAL_MODELS = [(0, 4), (2, 8), (2, 5), (2, 1), (2, 7), (3, 5), (0, 5), (2, 4)]
+
+# DIVANS_B200_LITERAL_MODEL_KEEP: the candidate of the command-list calls (encode_cmds_auto_*, transcode*) that keeps a list's own
+# PredictionMode records.  Their default candidates are [LITERAL_MODEL_KEEP] + DEFAULT_LITERAL_MODELS: ties go to the lowest
+# index, and a pair whose list would outgrow the encoder's logs costs the maximum, so a list the plain call encodes is encoded,
+# and by the tally at no higher cost than under its own records.
+LITERAL_MODEL_KEEP = (-1, -1)
 
 
 class CAllocator(ctypes.Structure):
@@ -135,6 +142,11 @@ def load_library():
     L.divans_b200_encode_auto_batch_device.argtypes = [vp, sz, vp, vp, vp, ctypes.c_uint64, vp, vp, vp, vp, vp, ctypes.POINTER(EncodeOptions),
                                                        vp, ctypes.c_uint32, vp, vp, vp]
     L.divans_b200_encode_auto_batch_device.restype = ctypes.c_uint8
+    L.divans_b200_encode_cmds_auto_batch_host.argtypes = batch + [ctypes.POINTER(EncodeOptions), vp, ctypes.c_uint32, vp, vp]
+    L.divans_b200_encode_cmds_auto_batch_host.restype = ctypes.c_uint8
+    L.divans_b200_encode_cmds_auto_batch_device.argtypes = [vp, sz, vp, vp, vp, ctypes.c_uint64, ctypes.c_uint64, vp, vp, vp, vp, vp,
+                                                            ctypes.POINTER(EncodeOptions), vp, ctypes.c_uint32, vp, vp, vp]
+    L.divans_b200_encode_cmds_auto_batch_device.restype = ctypes.c_uint8
     L.divans_b200_ir_to_cmds.argtypes = [ctypes.c_char_p, sz, vp, sz, szp, ctypes.POINTER(ctypes.c_int32)]
     L.divans_b200_ir_to_cmds.restype = ctypes.c_uint8
     L.divans_b200_lz77_cmds_batch.argtypes = [sz, vp, vp, vp, ctypes.c_int32, ctypes.c_int32, ctypes.c_int32, vp, sz, vp, vp, szp, ctypes.c_int32]
@@ -423,11 +435,12 @@ class Engine:
             todo = np.array(retry)
         return res
 
-    def transcode(self, streams, out_caps, opts=None, flags=0):
+    def transcode(self, streams, out_caps, opts=None, flags=0, candidates=None):
         """Re-encode .divans streams under other entropy options: decode_cmds (``flags`` as for decode: the model and revision the
         streams were written with), then encode(..., cmds=True) with ``opts`` (encode_options; a window_size of 0, the
         default when ``opts`` is None, keeps each stream's own window).  Returns the new streams; raises DivansError naming the
-        first stream that does not decode."""
+        first stream that does not decode.  With ``candidates`` (a list, see encode_cmds_auto_batch_host) each list is coded
+        under the cheapest of them instead, and the call returns (streams, chosen, cost)."""
         dec = self.decode_cmds(streams, out_caps, flags)
         for i, (st, _, _) in enumerate(dec):
             if st != DIVANS_SUCCESS:
@@ -435,13 +448,23 @@ class Engine:
         o = opts if opts is not None else encode_options(window_size=0)
         wins = [int(np.frombuffer(b[20:24], np.uint32)[0]) if o.window_size == 0 else int(o.window_size) for _, _, b in dec]
         res = [None] * len(dec)
+        chosen = np.zeros(len(dec), np.uint32)
+        cost = np.zeros((len(dec), len(candidates) if candidates is not None else 0), np.uint64)
         for w in sorted(set(wins)):
             idx = [i for i, x in enumerate(wins) if x == w]
             ow = EncodeOptions.from_buffer_copy(o)
             ow.window_size = w
-            for i, e in zip(idx, self.encode([dec[i][2] for i in idx], ow, cmds=True)):
-                res[i] = e
-        return res
+            if candidates is None:
+                for i, e in zip(idx, self.encode([dec[i][2] for i in idx], ow, cmds=True)):
+                    res[i] = e
+                continue
+            st, outs, ch, co = self._auto_lists(True, [dec[i][2] for i in idx], ow, candidates)
+            if (st != 0).any():
+                raise DivansError("encode failed for streams %s" % np.array(idx)[np.nonzero(st)[0][:8]])
+            for k, i in enumerate(idx):
+                res[i] = outs[k]
+            chosen[idx], cost[idx] = ch, co
+        return res if candidates is None else (res, chosen, cost)
 
     def encode_batch_host(self, in_blob, in_off, in_len, out, out_off, out_cap, opts=None, cmds=False):
         n = len(in_off)
@@ -467,32 +490,42 @@ class Engine:
             raise DivansError("encode_batch_device: " + self._err())
 
     @staticmethod
-    def _cands(candidates):
-        cs = DEFAULT_LITERAL_MODELS if candidates is None else candidates
+    def _cands(candidates, cmds=False):
+        cs = candidates if candidates is not None else [LITERAL_MODEL_KEEP] + DEFAULT_LITERAL_MODELS if cmds else DEFAULT_LITERAL_MODELS
         arr = (LiteralModel * max(1, len(cs)))()
         for i, (pm, mv) in enumerate(cs):
             arr[i].literal_pred_mode, arr[i].literal_mixing_value = int(pm), int(mv)
         return arr, len(cs)
 
-    def encode_auto_batch_host(self, in_blob, in_off, in_len, out, out_off, out_cap, opts=None, candidates=None):
-        """encode_batch_host with each stream's literal model chosen among ``candidates`` ((pred_mode, mixing_value) pairs,
-        default DEFAULT_LITERAL_MODELS) by its coding cost.  Returns (out_len, status, chosen, cost): cost[i, c] is stream i's
-        cost under candidate c in 1/65536 bit (2**64 - 1 where that pass failed)."""
+    def _auto_host(self, cmds, in_blob, in_off, in_len, out, out_off, out_cap, opts, candidates):
         n = len(in_off)
         in_off, in_len = np.ascontiguousarray(in_off, np.uint64), np.ascontiguousarray(in_len, np.uint64)
         out_off, out_cap = np.ascontiguousarray(out_off, np.uint64), np.ascontiguousarray(out_cap, np.uint64)
-        cands, nc = self._cands(candidates)
+        cands, nc = self._cands(candidates, cmds)
         out_len = np.zeros(n, np.uint64)
         status = np.full(n, DIVANS_FAILURE, np.int32)
         chosen = np.zeros(n, np.uint32)
         cost = np.zeros((n, nc), np.uint64)
         o = opts or encode_options()
-        rc = self._L.divans_b200_encode_auto_batch_host(self._h, n, _ptr(in_blob), _ptr(in_off), _ptr(in_len), _ptr(out), _ptr(out_off),
-                                                        _ptr(out_cap), _ptr(out_len), _ptr(status), ctypes.byref(o), ctypes.addressof(cands),
-                                                        nc, _ptr(chosen), _ptr(cost))
+        fn = self._L.divans_b200_encode_cmds_auto_batch_host if cmds else self._L.divans_b200_encode_auto_batch_host
+        rc = fn(self._h, n, _ptr(in_blob), _ptr(in_off), _ptr(in_len), _ptr(out), _ptr(out_off), _ptr(out_cap), _ptr(out_len), _ptr(status),
+                ctypes.byref(o), ctypes.addressof(cands), nc, _ptr(chosen), _ptr(cost))
         if rc != DIVANS_SUCCESS:
-            raise DivansError("encode_auto_batch_host: " + self._err())
+            raise DivansError("%s_batch_host: %s" % ("encode_cmds_auto" if cmds else "encode_auto", self._err()))
         return out_len, status, chosen, cost
+
+    def encode_auto_batch_host(self, in_blob, in_off, in_len, out, out_off, out_cap, opts=None, candidates=None):
+        """encode_batch_host with each stream's literal model chosen among ``candidates`` ((pred_mode, mixing_value) pairs,
+        default DEFAULT_LITERAL_MODELS) by its coding cost.  Returns (out_len, status, chosen, cost): cost[i, c] is stream i's
+        cost under candidate c in 1/65536 bit (2**64 - 1 where that pass failed)."""
+        return self._auto_host(False, in_blob, in_off, in_len, out, out_off, out_cap, opts, candidates)
+
+    def encode_cmds_auto_batch_host(self, blobs, blob_off, blob_len, out, out_off, out_cap, opts=None, candidates=None):
+        """encode_batch_host(..., cmds=True) with each command list coded under the cheapest of ``candidates``: (pred_mode,
+        mixing_value) pairs whose PredictionMode record replaces every record of the list, or LITERAL_MODEL_KEEP for the list's
+        own (default [LITERAL_MODEL_KEEP] + DEFAULT_LITERAL_MODELS).  Returns (out_len, status, chosen, cost) as
+        encode_auto_batch_host; stream i equals encode_batch_host(..., cmds=True) on the list under candidate chosen[i]."""
+        return self._auto_host(True, blobs, blob_off, blob_len, out, out_off, out_cap, opts, candidates)
 
     def encode_auto_batch_device(self, n, d_in, d_in_off, d_in_len, max_in_len, d_out, d_out_off, d_out_cap, d_out_len, d_status, d_chosen,
                                  d_cost=None, opts=None, candidates=None, stream=None):
@@ -506,9 +539,21 @@ class Engine:
         if rc != DIVANS_SUCCESS:
             raise DivansError("encode_auto_batch_device: " + self._err())
 
-    def encode_auto(self, raws, opts=None, candidates=None):
-        """Convenience: list of raw byte strings -> list of (status, .divans bytes or None, chosen candidate index)."""
-        bufs = [_u8(s) for s in raws]
+    def encode_cmds_auto_batch_device(self, n, d_blobs, d_blob_off, d_blob_len, max_blob_len, max_raw_len, d_out, d_out_off, d_out_cap,
+                                      d_out_len, d_status, d_chosen, d_cost=None, opts=None, candidates=None, stream=None):
+        """encode_cmds_batch_device with each list coded under the cheapest of ``candidates`` (as encode_cmds_auto_batch_host;
+        d_chosen u32 [n], d_cost u64 [n * C] or None).  Asynchronous on ``stream``."""
+        cands, nc = self._cands(candidates, cmds=True)
+        o = opts or encode_options()
+        rc = self._L.divans_b200_encode_cmds_auto_batch_device(self._h, n, d_blobs, d_blob_off, d_blob_len, int(max_blob_len), int(max_raw_len),
+                                                               d_out, d_out_off, d_out_cap, d_out_len, d_status, ctypes.byref(o),
+                                                               ctypes.addressof(cands), nc, d_chosen, d_cost, stream)
+        if rc != DIVANS_SUCCESS:
+            raise DivansError("encode_cmds_auto_batch_device: " + self._err())
+
+    def _auto_lists(self, cmds, bufs, opts, candidates):
+        """encode_auto / encode_cmds_auto of byte strings: (status, list of bytes or None, chosen, cost)"""
+        bufs = [_u8(s) for s in bufs]
         in_len = np.array([b.size for b in bufs], np.uint64)
         pad = (in_len + np.uint64(15)) & ~np.uint64(15)
         in_off = np.concatenate([[0], np.cumsum(pad)[:-1]]).astype(np.uint64) if bufs else np.zeros(0, np.uint64)
@@ -518,9 +563,20 @@ class Engine:
         out_cap = (in_len + in_len // np.uint64(2) + np.uint64(70000 + 255)) & ~np.uint64(255)
         out_off = np.concatenate([[0], np.cumsum(out_cap)[:-1]]).astype(np.uint64) if bufs else np.zeros(0, np.uint64)
         out = np.zeros(int(out_cap.sum()) + 16, np.uint8)
-        out_len, status, chosen, _ = self.encode_auto_batch_host(blob, in_off, in_len, out, out_off, out_cap, opts, candidates)
-        return [(int(s), out[int(o):int(o) + int(n)].tobytes() if s == DIVANS_SUCCESS else None, int(c))
-                for s, o, n, c in zip(status, out_off, out_len, chosen)]
+        out_len, status, chosen, cost = self._auto_host(cmds, blob, in_off, in_len, out, out_off, out_cap, opts, candidates)
+        return status, [out[int(o):int(o) + int(n)].tobytes() if s == DIVANS_SUCCESS else None for s, o, n in zip(status, out_off, out_len)], \
+            chosen, cost
+
+    def encode_auto(self, raws, opts=None, candidates=None):
+        """Convenience: list of raw byte strings -> list of (status, .divans bytes or None, chosen candidate index)."""
+        status, outs, chosen, _ = self._auto_lists(False, raws, opts, candidates)
+        return [(int(s), b, int(c)) for s, b, c in zip(status, outs, chosen)]
+
+    def encode_cmds_auto(self, blobs, opts=None, candidates=None):
+        """Convenience: list of DVCL command-list blobs -> list of (status, .divans bytes or None, chosen candidate index), each
+        list coded under the cheapest of ``candidates`` (encode_cmds_auto_batch_host)."""
+        status, outs, chosen, _ = self._auto_lists(True, blobs, opts, candidates)
+        return [(int(s), b, int(c)) for s, b, c in zip(status, outs, chosen)]
 
     def encode_cmds_batch_device(self, n, d_blobs, d_blob_off, d_blob_len, max_blob_len, max_raw_len, d_out, d_out_off, d_out_cap, d_out_len,
                                  d_status, opts=None, stream=None):
@@ -533,14 +589,17 @@ class Engine:
         if rc != DIVANS_SUCCESS:
             raise DivansError("encode_cmds_batch_device: " + self._err())
 
-    def transcode_device(self, d_in, in_off, in_len, out_caps, opts=None, flags=0, stream=None):
+    def transcode_device(self, d_in, in_off, in_len, out_caps, opts=None, flags=0, stream=None, candidates=None):
         """transcode without leaving the GPU: ``d_in`` is a CUDA uint8 tensor of concatenated .divans streams, stream i at
         in_off[i] .. +in_len[i] (host arrays), decoding to at most out_caps[i] bytes.  decode_cmds_batch_device then
         encode_cmds_batch_device on one CUDA stream, ordered after the work queued on ``stream`` (a torch.cuda.Stream, default
         the current one), the command
         lists staying in a device tensor.  Streams whose list did not fit the first guess (first_blob_cap) run once more with
         the exact size.  Returns (d_new, new_off, new_len, status): a CUDA uint8 tensor holding the re-encoded streams and host
-        arrays; status[i] is the decode status where that failed, else the encode status.  ``opts`` as for transcode."""
+        arrays; status[i] is the decode status where that failed, else the encode status.  ``opts`` as for transcode.
+        With ``candidates`` (a list) the encode step is encode_cmds_auto_batch_device, and the call returns (d_new, new_off,
+        new_len, status, chosen, cost) with chosen [n] and cost [n, C] host arrays (a stream that did not decode: every pass
+        failed, chosen 0)."""
         import torch
         n = len(in_off)
         in_off, in_len = np.ascontiguousarray(in_off, np.uint64).reshape(n), np.ascontiguousarray(in_len, np.uint64).reshape(n)
@@ -554,15 +613,18 @@ class Engine:
         s.wait_stream(caller)
         u64 = lambda a: torch.from_numpy(np.ascontiguousarray(a, np.uint64).view(np.int64)).to(dev, non_blocking=False)
         self.last_transcode_retried = 0
+        auto = candidates is not None
+        nc = len(candidates) if auto else 0
         if n == 0:
-            return torch.zeros(0, dtype=torch.uint8, device=dev), np.zeros(0, np.uint64), np.zeros(0, np.uint64), np.zeros(0, np.int32)
+            empty = torch.zeros(0, dtype=torch.uint8, device=dev), np.zeros(0, np.uint64), np.zeros(0, np.uint64), np.zeros(0, np.int32)
+            return empty + (np.zeros(0, np.uint32), np.zeros((0, nc), np.uint64)) if auto else empty
 
         pad = lambda c: (c + np.uint64(255)) & ~np.uint64(255)
         new_caps = lambda bcap: pad(bcap + bcap // np.uint64(2) + np.uint64(70000))   # (Engine.encode's output rule)
 
         def run(idx, blob_cap, d_new=None):
-            """decode + encode of streams idx on the device, one synchronisation: (d_new, new_off, new_len, status, blob_len).
-            The new streams go to `d_new` when given (at least new_caps(blob_cap).sum() bytes)."""
+            """decode + encode of streams idx on the device, one synchronisation: (d_new, new_off, new_len, status, blob_len,
+            decode status, chosen, cost).  The new streams go to `d_new` when given (at least new_caps(blob_cap).sum() bytes)."""
             m = len(idx)
             ocap, bcap = out_cap[idx], blob_cap
             offs = lambda c: np.concatenate([[0], np.cumsum(pad(c))[:-1]]).astype(np.uint64)
@@ -575,26 +637,33 @@ class Engine:
                 d_blobs = torch.empty(int(pad(bcap).sum()), dtype=torch.uint8, device=dev)
                 if d_new is None:
                     d_new = torch.empty(int(new_cap.sum()), dtype=torch.uint8, device=dev)
-                d_res = torch.zeros(4 * m, dtype=torch.int64, device=dev)   # out_len | blob_len | new_len | both statuses
-                d_st = d_res[3 * m:].view(torch.int32)
+                # out_len | blob_len | new_len | both statuses (| candidates: cost [m * C] | chosen)
+                d_res = torch.zeros((4 + (nc + 1 if auto else 0)) * m, dtype=torch.int64, device=dev)
+                d_st = d_res[3 * m:4 * m].view(torch.int32)
                 d_dec_st, d_enc_st = d_st[:m], d_st[m:]
                 self.decode_cmds_batch_device(d_in.data_ptr(), M[0].data_ptr(), M[1].data_ptr(), d_out.data_ptr(), M[2].data_ptr(), M[3].data_ptr(),
                                               d_res.data_ptr(), d_blobs.data_ptr(), M[4].data_ptr(), M[5].data_ptr(), d_res[m:].data_ptr(),
                                               d_dec_st.data_ptr(), m, int(in_len[idx].sum()), flags, s.cuda_stream)
                 # a stream that did not decode reaches the encoder with no blob (status 2's blob_len is larger than its region)
                 d_enc_len = torch.where(d_dec_st == 0, d_res[m:2 * m], torch.zeros_like(d_res[m:2 * m]))
-                self.encode_cmds_batch_device(m, d_blobs.data_ptr(), M[4].data_ptr(), d_enc_len.data_ptr(), int(bcap.max()), int(ocap.max()),
-                                              d_new.data_ptr(), M[6].data_ptr(), M[7].data_ptr(), d_res[2 * m:].data_ptr(), d_enc_st.data_ptr(),
-                                              o, s.cuda_stream)
+                enc = (m, d_blobs.data_ptr(), M[4].data_ptr(), d_enc_len.data_ptr(), int(bcap.max()), int(ocap.max()), d_new.data_ptr(),
+                       M[6].data_ptr(), M[7].data_ptr(), d_res[2 * m:].data_ptr(), d_enc_st.data_ptr())
+                if auto:
+                    self.encode_cmds_auto_batch_device(*enc, d_res[(4 + nc) * m:].data_ptr(), d_res[4 * m:(4 + nc) * m].data_ptr(), o,
+                                                       candidates, s.cuda_stream)
+                else:
+                    self.encode_cmds_batch_device(*enc, o, s.cuda_stream)
                 res = d_res.cpu()   # (the one synchronisation of the pass)
             r = res.numpy()
-            st = r[3 * m:].view(np.int32)
+            st = r[3 * m:4 * m].view(np.int32)
             dec_st, enc_st = st[:m], st[m:]
+            chosen = r[(4 + nc) * m:].view(np.uint32)[:m].copy() if auto else None
+            cost = r[4 * m:(4 + nc) * m].view(np.uint64).reshape(m, nc).copy() if auto else None
             return d_new, new_off, r[2 * m:3 * m].view(np.uint64).copy(), np.where(dec_st != 0, dec_st, enc_st).astype(np.int32), \
-                r[m:2 * m].view(np.uint64).copy(), dec_st.copy()
+                r[m:2 * m].view(np.uint64).copy(), dec_st.copy(), chosen, cost
 
         cap1 = first_blob_cap(out_cap)
-        d_new, new_off, new_len, status, blob_len, dec_st = run(np.arange(n), cap1)
+        d_new, new_off, new_len, status, blob_len, dec_st, chosen, cost = run(np.arange(n), cap1)
         retry = np.nonzero((dec_st == DIVANS_NEEDS_MORE_OUTPUT) & (blob_len > cap1))[0]
         self.last_transcode_retried = int(retry.size)   # (streams of the most recent call that ran twice)
         if retry.size:
@@ -605,13 +674,15 @@ class Engine:
                 out = torch.empty(base + int(new_caps(blob_len[retry]).sum()), dtype=torch.uint8, device=dev)
                 out[:base].copy_(d_new)
             del d_new
-            _, off2, len2, st2, _, _ = run(retry, blob_len[retry], out[base:])
+            _, off2, len2, st2, _, _, ch2, co2 = run(retry, blob_len[retry], out[base:])
             d_new = out
             new_off[retry] = off2 + np.uint64(base)
             new_len[retry], status[retry] = len2, st2
+            if auto:
+                chosen[retry], cost[retry] = ch2, co2
         caller.wait_stream(s)
         d_new.record_stream(caller)   # (allocated on the private stream, used on the caller's from here on)
-        return d_new, new_off, new_len, status
+        return (d_new, new_off, new_len, status, chosen, cost) if auto else (d_new, new_off, new_len, status)
 
     def encode(self, raws, opts=None, cmds=False):
         """Convenience: list of raw byte strings (or DVCL command-list blobs with cmds=True) -> list of .divans bytes."""

@@ -547,7 +547,8 @@ static DivansResult encode_device_internal(divans_b200_ctx *ctx, size_t n, int r
                                            const uint64_t *d_in_len, uint64_t max_in_len, uint32_t cmd_cap, uint32_t lit_cap,
                                            uint64_t replay_stride, uint8_t *d_out, const uint64_t *d_out_off, const uint64_t *d_out_cap,
                                            uint64_t *d_out_len, int32_t *d_status, const divans_b200_encode_options *o, int window,
-                                           cudaStream_t st, const uint8_t *d_pm_records = nullptr, const uint32_t *d_pm_index = nullptr) {
+                                           cudaStream_t st, const uint8_t *d_pm_records = nullptr, const uint32_t *d_pm_index = nullptr,
+                                           uint32_t pm_keep = 0) {
     const size_t slots = encode_slots(ctx, n);
     const uint32_t blocks = (uint32_t)(slots / ENCODE_GROUPS_PER_BLOCK);
     if (ensure_arena(ctx, slots) != DIVANS_SUCCESS) return DIVANS_FAILURE;
@@ -570,7 +571,7 @@ static DivansResult encode_device_internal(divans_b200_ctx *ctx, size_t n, int r
     EncodeParams ep;
     ep.in = d_in; ep.in_off = d_in_off; ep.in_len = d_in_len; ep.raw_mode = raw_mode; ep.n_streams = (uint32_t)n;
     ep.work_counter = ctx->d_counter; ep.arena = ctx->d_arena; ep.tables = ctx->d_tables;
-    ep.pm_internal = d_pm_records ? d_pm_records : ctx->d_pm_internal; ep.pm_index = d_pm_index;   // (raw mode: the caller's records)
+    ep.pm_internal = d_pm_records ? d_pm_records : ctx->d_pm_internal; ep.pm_index = d_pm_index; ep.pm_keep = pm_keep;   // (the caller's records)
     ep.cost_tab = nullptr; ep.tally = nullptr;
     ep.sf = ctx->d_sf; ep.cmd_cap = cmd_cap; ep.lit_cap = lit_cap;
     uint32_t *w = ctx->d_enc_scratch;
@@ -635,25 +636,50 @@ static void cmds_log_caps(uint64_t L, uint64_t replay, uint64_t &cmd, uint64_t &
     cmd = 32 * ((R - (uint64_t)PM_RECORD_BYTES * p) / 20) + 62000 * p + 64;
     lit = 2 * replay + 16;
 }
+//  * A candidate literal model (encode_cmds_auto) replaces records, not commands, so (c, p) and the bound stay those of the blob.
+//    But the bound holds per record, not per PredictionMode command: any number of commands may re-read one record, and each
+//    codes the whole record.  A raw record codes 64 literal-map and 4 distance-map entries more than a minimal one (empty maps),
+//    so a list whose commands re-read minimal records can fit the logs as given and outgrow them under every replacing record.
+//    The cost pass therefore counts each pair's entries against these same capacities: a pair that would outgrow them fails
+//    there (cost UINT64_MAX), and KEEP or another candidate that fits is chosen (test_many_commands_re_reading_small_records).
 
-extern "C" DivansResult divans_b200_encode_cmds_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_blobs, const uint64_t *d_blob_off,
-                                                             const uint64_t *d_blob_len, uint64_t max_blob_len, uint64_t max_raw_len,
-                                                             uint8_t *d_out, const uint64_t *d_out_off, const uint64_t *d_out_cap,
-                                                             uint64_t *d_out_len, int32_t *d_status, const divans_b200_encode_options *opts,
-                                                             void *cuda_stream) {
+// literal model selection of a batch (encode_host_common, encode_cmds_device_common): the candidates, and where chosen / cost go
+struct AutoSel {
+    const divans_b200_literal_model *cands; uint32_t n_cands;
+    uint32_t *chosen; uint64_t *cost;
+};
+
+static DivansResult encode_auto_device_nolock(divans_b200_ctx *ctx, size_t n, int raw_mode, const uint8_t *d_in, const uint64_t *d_in_off,
+                                              const uint64_t *d_in_len, uint64_t max_in_len, uint32_t cmd_cap, uint32_t lit_cap,
+                                              uint64_t replay_stride, uint8_t *d_out, const uint64_t *d_out_off,
+                                              const uint64_t *d_out_cap, uint64_t *d_out_len, int32_t *d_status,
+                                              const divans_b200_encode_options *o, int window, const divans_b200_literal_model *cands,
+                                              uint32_t n_cands, uint32_t *d_chosen, uint64_t *d_cost, cudaStream_t st);
+static bool check_cands(divans_b200_ctx *ctx, const divans_b200_literal_model *cands, uint32_t n_cands, bool cmds);
+
+// divans_b200_encode_cmds_batch_device, and with `sel` (device chosen / cost) divans_b200_encode_cmds_auto_batch_device
+static DivansResult encode_cmds_device_common(divans_b200_ctx *ctx, size_t n, const uint8_t *d_blobs, const uint64_t *d_blob_off,
+                                              const uint64_t *d_blob_len, uint64_t max_blob_len, uint64_t max_raw_len, uint8_t *d_out,
+                                              const uint64_t *d_out_off, const uint64_t *d_out_cap, uint64_t *d_out_len, int32_t *d_status,
+                                              const divans_b200_encode_options *opts, void *cuda_stream, const AutoSel *sel) {
     if (!ctx || !opts) return DIVANS_FAILURE;
+    if (sel && !check_cands(ctx, sel->cands, sel->n_cands, true)) return DIVANS_FAILURE;
     if (n == 0) return DIVANS_SUCCESS;
-    if (n > 0xffffffffull || max_blob_len > 0x7fff0000ull || max_raw_len > 0x7fff0000ull) { ctx->err = "batch too large"; return DIVANS_FAILURE; }
+    if (sel && !sel->chosen) { ctx->err = "encode_cmds_auto: d_chosen is required"; return DIVANS_FAILURE; }
+    const uint64_t nv = (uint64_t)n * (sel ? sel->n_cands : 1);
+    if (nv > 0xffffffffull || max_blob_len > 0x7fff0000ull || max_raw_len > 0x7fff0000ull) { ctx->err = "batch too large"; return DIVANS_FAILURE; }
     const uint64_t replay_stride = (max_raw_len + 31) & ~15ull;
     uint64_t cmd_cap, lit_cap;
     cmds_log_caps(max_blob_len, replay_stride, cmd_cap, lit_cap);
     // the kernels address a stream's logs at v * (cmd_cap + lit_cap) with a 32-bit stride
     if (cmd_cap + lit_cap > 0xffffffffull) { ctx->err = "batch too large"; return DIVANS_FAILURE; }
+    const int window = opts->window_size == 0 ? 0 : clamp_window(opts->window_size);
     std::lock_guard<std::mutex> lk(ctx->mu);
     CK(cudaSetDevice(ctx->device));
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream;
-    // the slots first, as in the host call: the logs are sized from what is left, and a failure names them
-    if (ensure_arena(ctx, encode_slots(ctx, n)) != DIVANS_SUCCESS) return DIVANS_FAILURE;
+    // the slots first, as in the host call: the logs are sized from what is left, and a failure names them.  (The cost pass of
+    // the n * C pairs has no logs; it runs in as many slots as the pairs fill.)
+    if (ensure_arena(ctx, encode_slots(ctx, nv)) != DIVANS_SUCCESS) return DIVANS_FAILURE;
     // No sub-batching: the logs of all n streams are one allocation, of exactly their size (they are most of what the call
     // needs next to the arena).  When it fails, the call fails and says how much it asked for.
     const size_t words = n * (size_t)(cmd_cap + lit_cap);
@@ -669,9 +695,34 @@ extern "C" DivansResult divans_b200_encode_cmds_batch_device(divans_b200_ctx *ct
         }
         ctx->sf_cap = words;
     }
+    if (sel)
+        try {
+            return encode_auto_device_nolock(ctx, n, 0, d_blobs, d_blob_off, d_blob_len, max_blob_len, (uint32_t)cmd_cap, (uint32_t)lit_cap,
+                                             replay_stride, d_out, d_out_off, d_out_cap, d_out_len, d_status, opts, window, sel->cands,
+                                             sel->n_cands, sel->chosen, sel->cost, st);
+        } catch (...) { ctx->err = "divans_b200: out of host memory"; return DIVANS_FAILURE; }
     return encode_device_internal(ctx, n, 0, d_blobs, d_blob_off, d_blob_len, max_blob_len, (uint32_t)cmd_cap, (uint32_t)lit_cap,
-                                  replay_stride, d_out, d_out_off, d_out_cap, d_out_len, d_status, opts,
-                                  opts->window_size == 0 ? 0 : clamp_window(opts->window_size), st);
+                                  replay_stride, d_out, d_out_off, d_out_cap, d_out_len, d_status, opts, window, st);
+}
+
+extern "C" DivansResult divans_b200_encode_cmds_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_blobs, const uint64_t *d_blob_off,
+                                                             const uint64_t *d_blob_len, uint64_t max_blob_len, uint64_t max_raw_len,
+                                                             uint8_t *d_out, const uint64_t *d_out_off, const uint64_t *d_out_cap,
+                                                             uint64_t *d_out_len, int32_t *d_status, const divans_b200_encode_options *opts,
+                                                             void *cuda_stream) {
+    return encode_cmds_device_common(ctx, n, d_blobs, d_blob_off, d_blob_len, max_blob_len, max_raw_len, d_out, d_out_off, d_out_cap,
+                                     d_out_len, d_status, opts, cuda_stream, nullptr);
+}
+extern "C" DivansResult divans_b200_encode_cmds_auto_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_blobs,
+                                                                  const uint64_t *d_blob_off, const uint64_t *d_blob_len,
+                                                                  uint64_t max_blob_len, uint64_t max_raw_len, uint8_t *d_out,
+                                                                  const uint64_t *d_out_off, const uint64_t *d_out_cap, uint64_t *d_out_len,
+                                                                  int32_t *d_status, const divans_b200_encode_options *opts,
+                                                                  const divans_b200_literal_model *cands, uint32_t n_cands,
+                                                                  uint32_t *d_chosen, uint64_t *d_cost, void *cuda_stream) {
+    const AutoSel sel = {cands, n_cands, d_chosen, d_cost};
+    return encode_cmds_device_common(ctx, n, d_blobs, d_blob_off, d_blob_len, max_blob_len, max_raw_len, d_out, d_out_off, d_out_cap,
+                                     d_out_len, d_status, opts, cuda_stream, &sel);
 }
 
 // ---- literal model selection ----
@@ -692,32 +743,42 @@ static uint32_t freq_cost(uint32_t f) {
     return (15u << 16) - ((e << 16) | frac);
 }
 
-static bool check_cands(divans_b200_ctx *ctx, const divans_b200_literal_model *cands, uint32_t n_cands) {
-    if (!cands || n_cands < 1 || n_cands > 16) { ctx->err = "encode_auto: 1..16 candidate literal models are required"; return false; }
+// DIVANS_B200_LITERAL_MODEL_KEEP: a command list's own PredictionMode records (command-list calls only)
+static bool is_keep(const divans_b200_literal_model &c) { return c.literal_pred_mode == -1 && c.literal_mixing_value == -1; }
+
+// `cmds`: the candidates of a command-list call, which may also be KEEP
+static bool check_cands(divans_b200_ctx *ctx, const divans_b200_literal_model *cands, uint32_t n_cands, bool cmds = false) {
+    const char *who = cmds ? "encode_cmds_auto" : "encode_auto";
+    char buf[200];
+    if (!cands || n_cands < 1 || n_cands > 16) {
+        snprintf(buf, sizeof buf, "%s: 1..16 candidate literal models are required", who);
+        ctx->err = buf;
+        return false;
+    }
     for (uint32_t c = 0; c < n_cands; c++)
-        if (cands[c].literal_pred_mode < 0 || cands[c].literal_pred_mode > 3 || cands[c].literal_mixing_value < 0 ||
-            cands[c].literal_mixing_value > 15) {
-            char buf[160];
-            snprintf(buf, sizeof buf, "encode_auto: candidate %u (pred_mode %d, mixing value %d) is outside pred_mode 0..3, mixing value 0..15",
-                     c, (int)cands[c].literal_pred_mode, (int)cands[c].literal_mixing_value);
+        if ((cands[c].literal_pred_mode < 0 || cands[c].literal_pred_mode > 3 || cands[c].literal_mixing_value < 0 ||
+             cands[c].literal_mixing_value > 15) && !(cmds && is_keep(cands[c]))) {
+            snprintf(buf, sizeof buf, "%s: candidate %u (pred_mode %d, mixing value %d) is outside pred_mode 0..3, mixing value 0..15%s",
+                     who, c, (int)cands[c].literal_pred_mode, (int)cands[c].literal_mixing_value, cmds ? ", and is not KEEP (-1, -1)" : "");
             ctx->err = buf;
             return false;
         }
     return true;
 }
 
-// One launch sequence over n raw streams in HBM: fan out to n * C virtual streams (dv_encode.cu: candidate-major), the cost-only
-// model pass over all of them, the per-stream argmin into d_chosen, then the encoder pipeline with stream i starting from
-// record d_chosen[i].  The cost pass pulls virtual streams from the work counter like the model pass, so however many there
-// are, the context's encoder slots code them as many at a time as they hold.
-static DivansResult encode_auto_device_nolock(divans_b200_ctx *ctx, size_t n, const uint8_t *d_in, const uint64_t *d_in_off,
-                                              const uint64_t *d_in_len, uint64_t max_in_len, uint8_t *d_out, const uint64_t *d_out_off,
+// One launch sequence over n streams in HBM (raw buffers, or command lists with raw_mode 0): fan out to n * C virtual streams
+// (dv_encode.cu: candidate-major), the cost-only model pass over all of them, the per-stream argmin into d_chosen, then the
+// encoder pipeline with stream i coded under candidate d_chosen[i] (raw: its starting record; command lists: the record that
+// replaces each of the list's own, unless the candidate is KEEP).  The cost pass pulls virtual streams from the work counter
+// like the model pass, so however many there are, the context's encoder slots code them as many at a time as they hold.
+// cmd_cap / lit_cap / replay_stride / window: those of the plain call over the same n streams.
+static DivansResult encode_auto_device_nolock(divans_b200_ctx *ctx, size_t n, int raw_mode, const uint8_t *d_in, const uint64_t *d_in_off,
+                                              const uint64_t *d_in_len, uint64_t max_in_len, uint32_t cmd_cap, uint32_t lit_cap,
+                                              uint64_t replay_stride, uint8_t *d_out, const uint64_t *d_out_off,
                                               const uint64_t *d_out_cap, uint64_t *d_out_len, int32_t *d_status,
-                                              const divans_b200_encode_options *o, const divans_b200_literal_model *cands,
+                                              const divans_b200_encode_options *o, int window, const divans_b200_literal_model *cands,
                                               uint32_t n_cands, uint32_t *d_chosen, uint64_t *d_cost, cudaStream_t st) {
-    const int window = clamp_window(o->window_size);
     const uint64_t nv = (uint64_t)n * n_cands;
-    const uint64_t replay_stride = (max_in_len + 31) & ~15ull;
     const size_t vslots = encode_slots(ctx, nv);
     if (ensure_arena(ctx, vslots) != DIVANS_SUCCESS) return DIVANS_FAILURE;
     if (!grow(ctx, &ctx->d_replay, &ctx->replay_cap, vslots * (size_t)replay_stride)) return DIVANS_FAILURE;
@@ -737,16 +798,21 @@ static DivansResult encode_auto_device_nolock(divans_b200_ctx *ctx, size_t n, co
     }
     std::vector<uint8_t> &pm = ctx->h_pm;
     pm.assign((size_t)n_cands * PM_RECORD_BYTES, 0);
-    for (uint32_t c = 0; c < n_cands; c++) raw_record(pm.data() + (size_t)c * PM_RECORD_BYTES, cands[c].literal_pred_mode, cands[c].literal_mixing_value);
+    uint32_t keep = 0;   // bit c: candidate c is KEEP (its record stays zero and is never read)
+    for (uint32_t c = 0; c < n_cands; c++) {
+        if (is_keep(cands[c])) keep |= 1u << c;
+        else raw_record(pm.data() + (size_t)c * PM_RECORD_BYTES, cands[c].literal_pred_mode, cands[c].literal_mixing_value);
+    }
     CK(cudaMemcpyAsync(ctx->d_pm_records, pm.data(), pm.size(), cudaMemcpyHostToDevice, st));
     launch_auto_fanout(d_in_off, d_in_len, n, n_cands, v_off, v_len, v_pm, st);
 
     EncodeParams tp;
     memset(&tp, 0, sizeof tp);
-    tp.in = d_in; tp.in_off = v_off; tp.in_len = v_len; tp.raw_mode = 1; tp.n_streams = (uint32_t)nv;
+    tp.in = d_in; tp.in_off = v_off; tp.in_len = v_len; tp.raw_mode = raw_mode; tp.n_streams = (uint32_t)nv;
     tp.work_counter = ctx->d_counter; tp.arena = ctx->d_arena; tp.tables = ctx->d_tables;
-    tp.pm_internal = ctx->d_pm_records; tp.pm_index = v_pm;
+    tp.pm_internal = ctx->d_pm_records; tp.pm_index = v_pm; tp.pm_keep = keep;
     tp.replay = ctx->d_replay; tp.replay_stride = replay_stride;
+    tp.cmd_cap = cmd_cap; tp.lit_cap = lit_cap;   // (no logs: the final encode's capacity, which a pair must fit to be chosen)
     tp.status = v_status; tp.cost_tab = ctx->d_cost_tab; tp.tally = tally;
     tp.window_size = window; tp.max_in_len = max_in_len; tp.dynamic_context_mixing = o->dynamic_context_mixing & 0xff; tp.prior_depth = o->prior_depth & 0xff;
     tp.use_context_map = o->use_context_map; tp.force_stride = o->force_stride; tp.have_literal_adaptation = o->have_literal_adaptation;
@@ -758,9 +824,8 @@ static DivansResult encode_auto_device_nolock(divans_b200_ctx *ctx, size_t n, co
     launch_auto_select(tally, v_status, n, n_cands, d_chosen, d_cost, st);
     ctx->launches += 3;
     CK(cudaGetLastError());
-    return encode_device_internal(ctx, n, 1, d_in, d_in_off, d_in_len, max_in_len, raw_cmd_cap(max_in_len, window),
-                                  (uint32_t)(2 * max_in_len + 16), replay_stride, d_out, d_out_off, d_out_cap, d_out_len, d_status, o,
-                                  window, st, ctx->d_pm_records, d_chosen);
+    return encode_device_internal(ctx, n, raw_mode, d_in, d_in_off, d_in_len, max_in_len, cmd_cap, lit_cap, replay_stride, d_out, d_out_off,
+                                  d_out_cap, d_out_len, d_status, o, window, st, ctx->d_pm_records, d_chosen, keep);
 }
 
 extern "C" DivansResult divans_b200_encode_auto_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_in, const uint64_t *d_in_off,
@@ -778,16 +843,12 @@ extern "C" DivansResult divans_b200_encode_auto_batch_device(divans_b200_ctx *ct
         std::lock_guard<std::mutex> lk(ctx->mu);
         CK(cudaSetDevice(ctx->device));
         cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream;
-        return encode_auto_device_nolock(ctx, n, d_in, d_in_off, d_in_len, max_in_len, d_out, d_out_off, d_out_cap, d_out_len, d_status,
-                                         opts, cands, n_cands, d_chosen, d_cost, st);
+        const int window = clamp_window(opts->window_size);
+        return encode_auto_device_nolock(ctx, n, 1, d_in, d_in_off, d_in_len, max_in_len, raw_cmd_cap(max_in_len, window),
+                                         (uint32_t)(2 * max_in_len + 16), (max_in_len + 31) & ~15ull, d_out, d_out_off, d_out_cap, d_out_len,
+                                         d_status, opts, window, cands, n_cands, d_chosen, d_cost, st);
     } catch (...) { ctx->err = "divans_b200: out of host memory"; return DIVANS_FAILURE; }
 }
-
-// literal model selection of a host batch (encode_host_common): the candidates, and where chosen / cost go
-struct AutoSel {
-    const divans_b200_literal_model *cands; uint32_t n_cands;
-    uint32_t *chosen; uint64_t *cost;
-};
 
 // host batch: marshal, split into sub-batches whose symbol logs fit in HBM, run, copy back
 static DivansResult encode_host_common(divans_b200_ctx *ctx, size_t n, int raw_mode, const uint8_t *in, const uint64_t *in_off,
@@ -795,9 +856,9 @@ static DivansResult encode_host_common(divans_b200_ctx *ctx, size_t n, int raw_m
                                        uint64_t *out_len, int32_t *status, const divans_b200_encode_options *opts,
                                        const AutoSel *sel = nullptr) {
     if (!ctx || !opts) return DIVANS_FAILURE;
-    if (sel && !check_cands(ctx, sel->cands, sel->n_cands)) return DIVANS_FAILURE;
+    if (sel && !check_cands(ctx, sel->cands, sel->n_cands, !raw_mode)) return DIVANS_FAILURE;
     if (n == 0) return DIVANS_SUCCESS;
-    if (sel && !sel->chosen) { ctx->err = "encode_auto: chosen is required"; return DIVANS_FAILURE; }
+    if (sel && !sel->chosen) { ctx->err = raw_mode ? "encode_auto: chosen is required" : "encode_cmds_auto: chosen is required"; return DIVANS_FAILURE; }
     if (sel && (uint64_t)n * sel->n_cands > 0xffffffffull) { ctx->err = "batch too large"; return DIVANS_FAILURE; }
     std::lock_guard<std::mutex> lk(ctx->mu);
     CK(cudaSetDevice(ctx->device));
@@ -850,8 +911,11 @@ static DivansResult encode_host_common(divans_b200_ctx *ctx, size_t n, int raw_m
         uint64_t mc = 0, ml = 0, mr = 0, mx = 0; size_t i1 = i0;
         while (i1 < n) {
             uint64_t c = need_cmd[i1] > mc ? need_cmd[i1] : mc, l = need_lit[i1] > ml ? need_lit[i1] : ml;
-            if (i1 > i0 && (c + l) * 4 * (uint64_t)(i1 - i0 + 1) > budget) break;
-            mc = c; ml = l; if (need_replay[i1] > mr) mr = need_replay[i1];
+            // encode_auto: the cost pass also holds a replay window per slot for up to m * C pairs
+            const uint64_t r = need_replay[i1] > mr ? need_replay[i1] : mr;
+            const uint64_t rep = sel ? (uint64_t)encode_slots(ctx, (i1 - i0 + 1) * (size_t)sel->n_cands) * r : 0;
+            if (i1 > i0 && (c + l) * 4 * (uint64_t)(i1 - i0 + 1) + rep > budget) break;
+            mc = c; ml = l; mr = r;
             if (in_len[i1] > mx) mx = in_len[i1];
             i1++;
         }
@@ -872,8 +936,9 @@ static DivansResult encode_host_common(divans_b200_ctx *ctx, size_t n, int raw_m
         int32_t *d_status = reinterpret_cast<int32_t *>(mm + 5 * m);
         uint32_t *d_chosen = reinterpret_cast<uint32_t *>(mm + 6 * m);
         uint64_t *d_cost = mm + 7 * m;
-        DivansResult r = sel ? encode_auto_device_nolock(ctx, m, ctx->d_in, mm, mm + m, mx, ctx->d_out, mm + 2 * m, mm + 3 * m, mm + 4 * m,
-                                                         d_status, opts, sel->cands, sel->n_cands, d_chosen, d_cost, st)
+        DivansResult r = sel ? encode_auto_device_nolock(ctx, m, raw_mode, ctx->d_in, mm, mm + m, mx, (uint32_t)mc, (uint32_t)ml, mr, ctx->d_out,
+                                                         mm + 2 * m, mm + 3 * m, mm + 4 * m, d_status, opts, window, sel->cands,
+                                                         sel->n_cands, d_chosen, d_cost, st)
                              : encode_device_internal(ctx, m, raw_mode, ctx->d_in, mm, mm + m, mx, (uint32_t)mc, (uint32_t)ml, mr, ctx->d_out,
                                                       mm + 2 * m, mm + 3 * m, mm + 4 * m, d_status, opts, window, st);
         if (r != DIVANS_SUCCESS) return r;
@@ -914,6 +979,15 @@ extern "C" DivansResult divans_b200_encode_cmds_batch_host(divans_b200_ctx *ctx,
                                                            const uint64_t *out_cap, uint64_t *out_len, int32_t *status,
                                                            const divans_b200_encode_options *opts) {
     try { return encode_host_common(ctx, n, 0, blobs, blob_off, blob_len, out, out_off, out_cap, out_len, status, opts); }
+    catch (...) { if (ctx) ctx->err = "divans_b200: out of host memory while marshalling the batch"; return DIVANS_FAILURE; }
+}
+extern "C" DivansResult divans_b200_encode_cmds_auto_batch_host(divans_b200_ctx *ctx, size_t n, const uint8_t *blobs, const uint64_t *blob_off,
+                                                                const uint64_t *blob_len, uint8_t *out, const uint64_t *out_off,
+                                                                const uint64_t *out_cap, uint64_t *out_len, int32_t *status,
+                                                                const divans_b200_encode_options *opts, const divans_b200_literal_model *cands,
+                                                                uint32_t n_cands, uint32_t *chosen, uint64_t *cost) {
+    const AutoSel sel = {cands, n_cands, chosen, cost};
+    try { return encode_host_common(ctx, n, 0, blobs, blob_off, blob_len, out, out_off, out_cap, out_len, status, opts, &sel); }
     catch (...) { if (ctx) ctx->err = "divans_b200: out of host memory while marshalling the batch"; return DIVANS_FAILURE; }
 }
 

@@ -169,8 +169,11 @@ struct EncodeParams {
     // max_in_len (the bound cmd_cap / lit_cap were derived from) is refused unread
     uint64_t max_in_len;
     uint32_t *stream_window;      // per stream: the window the model pass coded it with (the mux writes it into the header)
-    // raw mode: stream v starts with record pm_internal + pm_index[v] * PM_RECORD_BYTES (nullptr: record 0 for every stream)
+    // raw mode: stream v starts with record pm_internal + pm_index[v] * PM_RECORD_BYTES (nullptr: record 0 for every stream).
+    // command lists: stream v codes every PredictionMode command with that one record instead of the list's own, unless bit
+    // pm_index[v] of pm_keep is set (nullptr: every stream keeps its records)
     const uint32_t *pm_index;
+    uint32_t pm_keep;
     // cost-only model pass (encode_model_kernel<BLEND, true>): no logs; per stream the sum of cost_tab[freq] over every coded
     // nibble of both coders, in 1/65536 bit (cost_tab[f] = -log2(f / 32768), include/divans_b200.h)
     const uint32_t *cost_tab;

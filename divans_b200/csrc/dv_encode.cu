@@ -7,7 +7,8 @@
 //                           into the stream's command / literal log.
 //                           TALLY = true is the cost-only variant (encode_model_kernel<BLEND, true>, divans_b200_encode_auto_*):
 //                           the same walk, but each coded nibble adds cost_tab[freq] to the stream's total instead of
-//                           writing a log entry.  It has no logs, so no log capacity, and no passes 2 and 3.
+//                           writing a log entry.  It has no logs and no passes 2 and 3, but counts the entries it would
+//                           log against cmd_cap / lit_cap, the capacity of the final encode's logs.
 //   2. encode_flush_kernel  one thread per (65536-symbol chunk, rANS state) runs the recurrence last symbol -> first
 //                           symbol (ans.rs:302-378); encode_pack_kernel then stacks the renormalisation words in
 //                           symbol order IN PLACE at the top of the chunk's own log region (<= one word per symbol).
@@ -39,7 +40,7 @@ __global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) encode_model_kernel(E
     s.state = S_IDLE;
     s.c->in.cmds = nullptr; s.c->in.n_cmds = 0; s.c->in.pos = 0; s.c->in.n_pms = 0; s.c->in.pms = nullptr; s.c->in.lits = nullptr;
     s.c->model_rev = (uint32_t)p.model_rev;
-    s.c->sidx = 0; s.c->raw_len = 0; s.c->lit_log_cap = TALLY ? 0xffffffffu : p.lit_cap;   // (TALLY: no log to outgrow)
+    s.c->sidx = 0; s.c->raw_len = 0; s.c->lit_log_cap = p.lit_cap;   // (TALLY: the capacity of the final encode's log)
     s.out = p.replay + (uint64_t)slot * p.replay_stride; s.out_pos = 0;
     s.c->out_cap = p.replay_stride > 0xffffffffull ? 0xffffffffu : (uint32_t)p.replay_stride;
     st_reset(s);
@@ -80,7 +81,7 @@ __global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) encode_model_kernel(E
                     uint32_t win = (uint32_t)p.window_size;   // 0 (command lists only): the window of the blob's header
                     if (p.raw_mode) {
                         if (blen > 0xffffffffull - 16) ok = false;
-                        s.c->in.cmds = nullptr; s.c->in.n_pms = 1; s.c->in.lits = blob;
+                        s.c->in.cmds = nullptr; s.c->in.n_pms = 1; s.c->in.lits = blob; s.c->in.pm_mask = 0;
                         s.c->in.pms = p.pm_internal + (p.pm_index ? (uint64_t)p.pm_index[v] * PM_RECORD_BYTES : 0ull);
                         s.c->raw_len = (uint32_t)blen;
                         s.c->in.n_cmds = 1u + (uint32_t)((blen + (1ull << win) - 1) >> win);
@@ -97,6 +98,11 @@ __global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) encode_model_kernel(E
                             s.c->in.cmds = h + 8; s.c->in.n_cmds = h[2]; s.c->in.n_pms = h[3];
                             s.c->in.pms = blob + 32 + 20ull * h[2];
                             s.c->in.lits = s.c->in.pms + (uint64_t)PM_RECORD_BYTES * h[3];
+                            s.c->in.pm_mask = ~0u;
+                            if (p.pm_index) {   // a candidate literal model: its one record stands in for each of the list's
+                                const uint32_t c = p.pm_index[v];
+                                if (!((p.pm_keep >> c) & 1u)) { s.c->in.pms = p.pm_internal + (uint64_t)c * PM_RECORD_BYTES; s.c->in.pm_mask = 0; }
+                            }
                             s.c->raw_len = h[4];
                         }
                     }
@@ -145,8 +151,10 @@ __global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) encode_model_kernel(E
         if (!busy) s.cur.left = 0;
         else {
             if (s.status == ST_OK) {   // (else the core could not code the symbol: enc_log)
-                // log overflow cannot happen for command lists whose sizes match the header; guard hostile blobs anyway
-                if (!TALLY && s.cur.left + 1 >= (s.c->cur_is_lit ? p.lit_cap : p.cmd_cap)) s.status = ST_FAIL;
+                // log overflow cannot happen for command lists whose sizes match the header; guard hostile blobs anyway.  The
+                // cost pass keeps no log but counts the same entries against the final encode's capacity, so a (stream,
+                // candidate) pair that encode would refuse fails here (cost UINT64_MAX) and is never chosen over one that fits.
+                if (s.cur.left + 1 >= (s.c->cur_is_lit ? p.lit_cap : p.cmd_cap)) s.status = ST_FAIL;
                 else transition<true>(s, nx, g, sym);
             }
             if (s.status != ST_OK || s.state == S_IDLE) finish();

@@ -65,6 +65,8 @@ constexpr int MI_DUMMY = 127;   // MISC slot idle groups "code" against while th
 struct CmdIn {
     const uint32_t *cmds;    // 5 x u32 per command
     uint32_t n_cmds, pos, n_pms;
+    uint32_t pm_mask;        // ~0: PredictionMode command k reads record k of `pms`; 0: every one reads record 0 (raw mode, or a
+                             // list whose records a candidate literal model replaces; k is still checked against n_pms)
     const uint8_t *pms;      // prediction mode records (32 + 16384 + 1024 + 8192 each)
     const uint8_t *lits;     // literal pool
 };

@@ -285,7 +285,7 @@ template <bool ENC, bool REC = false> __device__ __forceinline__ bool bt_done(St
     rec_cmd<REC>(s, g, 4 + s.f0, bt, 0);
     return true;
 }
-template <bool ENC> __device__ __forceinline__ const uint8_t *pm_rec(const St &s) { return s.c->in.pms + (size_t)s.c->e0 * (32 + 16384 + 1024 + 8192); }
+template <bool ENC> __device__ __forceinline__ const uint8_t *pm_rec(const St &s) { return s.c->in.pms + (size_t)(s.c->e0 & s.c->in.pm_mask) * (32 + 16384 + 1024 + 8192); }
 template <bool ENC> __device__ __forceinline__ void enter_pm_speed(St &s, Next &nx) {
     s.state = S_PM_SPEED;
     uint32_t si = s.f1 >> 2, pt = s.f1 & 3;

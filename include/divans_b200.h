@@ -309,6 +309,41 @@ DivansResult divans_b200_encode_auto_batch_device(divans_b200_ctx *ctx, size_t n
                                                   int32_t *d_status, const divans_b200_encode_options *opts,
                                                   const divans_b200_literal_model *cands, uint32_t n_cands, uint32_t *d_chosen,
                                                   uint64_t *d_cost, void *cuda_stream);
+/* The candidate of the command-list calls below that keeps a list's own PredictionMode records (pred_mode -1, mixing value
+ * -1; an initialiser of divans_b200_literal_model).  The raw calls above refuse it. */
+#define DIVANS_B200_LITERAL_MODEL_KEEP { -1, -1 }
+/* Encode n command lists (DVCL blobs) held in HOST memory, each coded under the cheapest of n_cands candidate literal models.
+ *  - Coding a list under candidate c replaces EVERY PredictionMode record of the list by c's record: the one
+ *    divans_b200_encode_batch_host builds from (pred_mode, mixing value), whole (mode, speeds, both context maps and the 8192
+ *    mixing values; a context map only means something for the mode it was built for).  Commands, literal pool and window are
+ *    unchanged.  KEEP ({-1, -1}) codes the list as given.
+ *  - Contract: stream i's bytes, out_len and status equal divans_b200_encode_cmds_batch_host's for the same blob with every
+ *    PredictionMode record replaced by candidate chosen[i]'s record (when chosen[i] is KEEP: the blob as given).
+ *  - chosen[i] and cost as in divans_b200_encode_auto_batch_host: the sum of T[freq] over every coded nibble of both coders,
+ *    ties to the lowest index, a failed pass costs UINT64_MAX.  A pass also fails when the list under that candidate would
+ *    outgrow the symbol logs the final encode has for it: the log capacity holds per PredictionMode record, and commands that
+ *    re-read small records code more entries under a replacing record than under their own.  So no chosen candidate is
+ *    refused for lack of log space, and with KEEP among the candidates a list that the plain call encodes is encoded, at no
+ *    higher cost than as given.
+ *  - cands: 1..16 entries, each KEEP or pred_mode 0..3 with mixing value 0..15; anything else returns DIVANS_FAILURE before any
+ *    work.  Sub-batched like divans_b200_encode_cmds_batch_host; n == 0 returns DIVANS_SUCCESS. */
+DivansResult divans_b200_encode_cmds_auto_batch_host(divans_b200_ctx *ctx, size_t n, const uint8_t *blobs, const uint64_t *blob_off,
+                                                     const uint64_t *blob_len, uint8_t *out, const uint64_t *out_off,
+                                                     const uint64_t *out_cap, uint64_t *out_len, int32_t *status,
+                                                     const divans_b200_encode_options *opts, const divans_b200_literal_model *cands,
+                                                     uint32_t n_cands, uint32_t *chosen, uint64_t *cost);
+/* Same as divans_b200_encode_cmds_auto_batch_host with the buffers, d_chosen and d_cost DEVICE pointers (cands is a host array,
+ * copied before the call returns).  Every convention of divans_b200_encode_cmds_batch_device holds: max_blob_len / max_raw_len,
+ * window_size 0 = each blob's header window, status 2 and 3, guard rules, no sub-batching.  Its contract is with that call:
+ * stream i equals divans_b200_encode_cmds_batch_device on the blob with its records replaced by chosen[i]'s.  One launch
+ * sequence, no host synchronisation; the n * n_cands (stream, candidate) pairs run through the context's encoder slots in waves.
+ * The cost pass holds a replay window of max_raw_len bytes per slot for up to n * n_cands pairs (the plain call: up to n). */
+DivansResult divans_b200_encode_cmds_auto_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_blobs, const uint64_t *d_blob_off,
+                                                       const uint64_t *d_blob_len, uint64_t max_blob_len, uint64_t max_raw_len,
+                                                       uint8_t *d_out, const uint64_t *d_out_off, const uint64_t *d_out_cap,
+                                                       uint64_t *d_out_len, int32_t *d_status, const divans_b200_encode_options *opts,
+                                                       const divans_b200_literal_model *cands, uint32_t n_cands, uint32_t *d_chosen,
+                                                       uint64_t *d_cost, void *cuda_stream);
 /* IR text front-end (reference: src/bin/divans.rs:191-483, the textual IR that `divans -i` consumes): parse `ir_text` into a
  * DVCL blob.  *blob_len receives the size of the blob; with out == NULL or out_cap too small the call returns
  * DIVANS_NEEDS_MORE_OUTPUT.  *window_size (optional) receives the `window` line's value (0 if absent).  Host only. */

@@ -88,3 +88,50 @@ int dvo_encode_auto(const uint8_t *in, size_t n, const dvo_options *o, const int
     *chosen = arg;
     return dvo_encode_raw_model(in, n, o, cands[2 * arg], cands[2 * arg + 1], out, cap, out_len);
 }
+
+/* ---- command lists ----
+ * A candidate (pred_mode, mixing_value) replaces every PredictionMode record of a list by the raw-mode record of that model
+ * (internal_predmode); commands, literal pool and window are kept.  (-1, -1) is KEEP: the list's own records. */
+static int dvt_is_keep(int pred_mode, int mixing_value) { return pred_mode == -1 && mixing_value == -1; }
+
+int dvo_cmdlist_set_model(dvo_cmdlist *l, int pred_mode, int mixing_value) {
+    if (dvt_is_keep(pred_mode, mixing_value)) return DVO_SUCCESS;
+    if (pred_mode < 0 || pred_mode > 3 || mixing_value < 0 || mixing_value > 15) return DVO_FAILURE;
+    for (size_t k = 0; k < l->n_pms; k++) internal_predmode(&l->pms[k], pred_mode, mixing_value);
+    return DVO_SUCCESS;
+}
+
+/* calls fn on the list as coded under candidate (pred_mode, mixing_value): a shallow copy whose records are replaced */
+static int dvt_with_model(const dvo_cmdlist *l, int pred_mode, int mixing_value, int (*fn)(const dvo_cmdlist *, void *), void *arg) {
+    if (dvt_is_keep(pred_mode, mixing_value) || l->n_pms == 0) return fn(l, arg);
+    dvo_cmdlist m = *l;
+    m.pms = (dvo_predmode *)malloc(l->n_pms * sizeof(dvo_predmode));
+    if (!m.pms) return DVO_FAILURE;
+    m.cap_pms = l->n_pms;
+    int rc = dvo_cmdlist_set_model(&m, pred_mode, mixing_value);
+    if (rc == DVO_SUCCESS) rc = fn(&m, arg);
+    free(m.pms);
+    return rc;
+}
+
+typedef struct { const dvo_options *o; uint64_t *cost; uint8_t *out; size_t cap; size_t *out_len; } dvt_call;
+static int dvt_tally_fn(const dvo_cmdlist *l, void *p) { dvt_call *c = (dvt_call *)p; return dvo_tally_cmds(l, c->o, c->cost); }
+static int dvt_encode_fn(const dvo_cmdlist *l, void *p) { dvt_call *c = (dvt_call *)p; return dvo_encode_cmds(l, c->o, c->out, c->cap, c->out_len); }
+
+/* dvo_encode_auto for a command list: *chosen = the argmin of the candidates' costs (ties to the lowest index; a candidate the
+ * encoder refuses costs UINT64_MAX; costs[c] optional), and the list encoded under it */
+int dvo_encode_cmds_auto(const dvo_cmdlist *l, const dvo_options *o, const int32_t *cands, uint32_t n_cands, uint8_t *out, size_t cap,
+                         size_t *out_len, uint32_t *chosen, uint64_t *costs) {
+    uint64_t best = UINT64_MAX; uint32_t arg = 0;
+    for (uint32_t c = 0; c < n_cands; c++) {
+        uint64_t t = UINT64_MAX;
+        dvt_call call = {o, &t, NULL, 0, NULL};
+        if (dvt_with_model(l, cands[2 * c], cands[2 * c + 1], dvt_tally_fn, &call) != DVO_SUCCESS) t = UINT64_MAX;
+        if (costs) costs[c] = t;
+        if (t < best) { best = t; arg = c; }
+    }
+    *chosen = arg;
+    *out_len = 0;
+    dvt_call call = {o, NULL, out, cap, out_len};
+    return dvt_with_model(l, cands[2 * arg], cands[2 * arg + 1], dvt_encode_fn, &call);
+}

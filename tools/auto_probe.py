@@ -2,6 +2,7 @@
 
     python tools/auto_probe.py --survey [--streams 8]        # CPU (oracle): the cost of every literal model on each corpus
     python tools/auto_probe.py [--n 4096] [--len 65536] [--reps 3]   # H100: ratio, pick accuracy, encode and decode times
+    python tools/auto_probe.py --transcode [--n 4096] [--lz-n 512]   # H100: transcode_device with and without candidates
 
 --survey tallies every (pred_mode, mixing value) pair, mixing value 2 included, with the CPU oracle on a few streams of each
 corpus and prints the table DESIGN.md section 4 quotes; it is how divans_b200.DEFAULT_LITERAL_MODELS was chosen.
@@ -12,6 +13,11 @@ The GPU mode, for the bench's text streams and for a mixed corpus (text, UTF-8 t
   * wall time of encode_auto_batch_device against C x encode_batch_device (inputs already in HBM);
   * decode time of the auto-encoded corpus against the default-encoded one.
 Times alternate the two sides run by run and report medians (CUDA events around each call).
+
+--transcode stores the same two corpora with the default model (literal-only streams, n of them) and as LZ77 lists from
+divans_b200.lz77_cmds_batch (window 16, the generator's model (UTF8, 4); --lz-n of them: an LZ77 transcode needs a blob
+region per stream on top of the encoder's logs), then reports the bytes and wall time of Engine.transcode_device without
+candidates and with [LITERAL_MODEL_KEEP] + DEFAULT_LITERAL_MODELS, and the decode time of both outputs.
 """
 import argparse
 import json
@@ -200,6 +206,91 @@ def gpu(args):
     print(json.dumps(dict(device=props.name, n=args.n, len=L, reps=args.reps, candidates=cands, results=out)))
 
 
+def gpu_info():
+    """the card, its power limit and its SM clock, read in the same process as the timings"""
+    import subprocess
+    import torch
+    q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
+                       capture_output=True, text=True).stdout.strip()
+    return dict(device=torch.cuda.get_device_properties(0).name, power_limit_clock_sm_max_sm=q)
+
+
+def transcode(args):
+    import time
+    import torch
+    import divans_b200
+    cands = [divans_b200.LITERAL_MODEL_KEEP] + divans_b200.DEFAULT_LITERAL_MODELS
+    L = args.len
+    cs = corpora(args.n, L)
+    mixed = [cs[("text", "utf8", "stride2", "stride4", "stride8")[k % 5]][k] for k in range(args.n)]
+    out = {}
+    for name, raws in (("text", cs["text"]), ("mixed", mixed)):
+        for kind in ("literal", "lz77"):
+            rs = raws if kind == "literal" else raws[:args.lz_n]
+            n = len(rs)
+            eng = divans_b200.Engine(0)   # (one per corpus: the transcode's logs are freed before the decodes allocate theirs)
+            if kind == "literal":
+                stored = eng.encode(rs)
+            else:
+                blob = np.frombuffer(b"".join(rs), np.uint8)
+                bl, boff, blen = divans_b200.lz77_cmds_batch(blob, np.arange(n, dtype=np.uint64) * np.uint64(L),
+                                                            np.array([len(r) for r in rs], np.uint64), window=16)
+                stored = eng.encode([bl[int(o):int(o + l)] for o, l in zip(boff, blen)], divans_b200.encode_options(window_size=16),
+                                    cmds=True)
+            lens = np.array([len(s) for s in stored], np.uint64)
+            offs = np.concatenate([[0], np.cumsum((lens + np.uint64(15)) & ~np.uint64(15))[:-1]]).astype(np.uint64)
+            buf = np.zeros(int(offs[-1] + lens[-1]) + 16, np.uint8)
+            for s, o in zip(stored, offs):
+                buf[int(o):int(o) + len(s)] = np.frombuffer(s, np.uint8)
+            d_in = torch.from_numpy(buf).cuda()
+            caps = [L + 64] * n
+
+            def run(c):
+                torch.cuda.synchronize()
+                t0 = time.perf_counter()
+                res = eng.transcode_device(d_in, offs, lens, caps, candidates=c)
+                torch.cuda.synchronize()
+                return time.perf_counter() - t0, res
+
+            tp, ta = [], []
+            for _ in range(args.reps):
+                t, rp = run(None)
+                tp.append(t)
+                t, ra = run(cands)
+                ta.append(t)
+            r = dict(n=n, raw=int(sum(len(x) for x in rs)), stored=int(lens.sum()), plain=int(rp[2].sum()), auto=int(ra[2].sum()),
+                     transcode_plain_ms=1e3 * float(np.median(tp)), transcode_auto_ms=1e3 * float(np.median(ta)),
+                     chosen_hist=np.bincount(ra[4], minlength=len(cands)).tolist())
+            assert (rp[3] == 0).all() and (ra[3] == 0).all()
+            eng.close()
+            torch.cuda.empty_cache()
+            eng = divans_b200.Engine(0)
+            # decode both outputs, alternating
+            td = {"plain": [], "auto": []}
+            d_doff = torch.from_numpy((np.arange(n, dtype=np.uint64) * np.uint64(L)).view(np.int64)).cuda()
+            d_dcap = torch.from_numpy(np.full(n, L, np.uint64).view(np.int64)).cuda()
+            d_dec = torch.empty(n * L, dtype=torch.uint8, device="cuda")
+            d_ol = torch.zeros(n, dtype=torch.int64, device="cuda")
+            d_st = torch.zeros(n, dtype=torch.int32, device="cuda")
+            for _ in range(args.reps):
+                for tag, res in (("plain", rp), ("auto", ra)):
+                    d_new, new_off, new_len = res[0], res[1], res[2]
+                    d_o = torch.from_numpy(new_off.view(np.int64)).cuda()
+                    d_l = torch.from_numpy(new_len.view(np.int64)).cuda()
+                    torch.cuda.synchronize()
+                    t0 = time.perf_counter()
+                    eng.decode_batch_device(d_new.data_ptr(), d_o.data_ptr(), d_l.data_ptr(), d_dec.data_ptr(), d_doff.data_ptr(),
+                                            d_dcap.data_ptr(), d_ol.data_ptr(), d_st.data_ptr(), n, int(d_new.numel()), 0)
+                    eng.synchronize()
+                    td[tag].append(time.perf_counter() - t0)
+                    assert (d_st.cpu().numpy() == 0).all() and bytes(d_dec.cpu().numpy()) == b"".join(rs)   # (every stream is L bytes)
+            r["decode_plain_ms"], r["decode_auto_ms"] = 1e3 * float(np.median(td["plain"])), 1e3 * float(np.median(td["auto"]))
+            eng.close()
+            out[name + " " + kind] = r
+            print(name, kind, json.dumps(r), flush=True)
+    print(json.dumps(dict(gpu_info(), n=args.n, lz_n=args.lz_n, len=L, reps=args.reps, results=out)))
+
+
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--survey", action="store_true")
@@ -207,8 +298,12 @@ if __name__ == "__main__":
     ap.add_argument("--n", type=int, default=4096)
     ap.add_argument("--len", type=int, default=65536)
     ap.add_argument("--reps", type=int, default=3)
+    ap.add_argument("--transcode", action="store_true")
+    ap.add_argument("--lz-n", type=int, default=512)
     a = ap.parse_args()
     if a.survey:
         survey(a.streams, a.len)
+    elif a.transcode:
+        transcode(a)
     else:
         gpu(a)
