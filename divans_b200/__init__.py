@@ -181,6 +181,40 @@ def _u8(b):
     return np.frombuffer(bytes(b), dtype=np.uint8) if len(b) else np.zeros(0, np.uint8)
 
 
+def _pack(bufs):
+    """Byte strings -> (blob, off, len) of one input blob: each at a 16-byte aligned offset, and 16 bytes of zeros at the end."""
+    bufs = [_u8(b) for b in bufs]
+    ln = np.array([b.size for b in bufs], np.uint64)
+    pad = (ln + np.uint64(15)) & ~np.uint64(15)
+    off = np.zeros(len(bufs), np.uint64)
+    off[1:] = np.cumsum(pad)[:-1]
+    blob = np.zeros(int(pad.sum()) + 16, np.uint8)
+    for b, o in zip(bufs, off):
+        blob[int(o):int(o) + b.size] = b
+    return blob, off, ln
+
+
+def _regions(caps):
+    """Output regions of caps[i] bytes, back to back at 256-byte aligned offsets -> (off, total bytes)."""
+    pad = (np.asarray(caps, np.uint64) + np.uint64(255)) & ~np.uint64(255)
+    off = np.zeros(pad.size, np.uint64)
+    off[1:] = np.cumsum(pad)[:-1]
+    return off, int(pad.sum())
+
+
+def _encoded_cap(in_len):
+    """The output region an encode of in_len bytes (raw bytes or a command list) gets: half as much again plus a fixed
+    headroom, rounded up to 256 bytes."""
+    L = np.asarray(in_len, np.uint64)
+    return (L + L // np.uint64(2) + np.uint64(70000 + 255)) & ~np.uint64(255)
+
+
+def _host_batch(*desc):
+    """The descriptor arrays of a host call as contiguous uint64 arrays, then its out_len and status arrays."""
+    n = len(desc[0])
+    return [np.ascontiguousarray(a, np.uint64) for a in desc] + [np.zeros(n, np.uint64), np.full(n, DIVANS_FAILURE, np.int32)]
+
+
 def ir_to_cmds(text):
     """Reference IR text (src/bin/divans.rs:191-483) -> (DVCL command-list blob, window size).  Host-side parser of the
     C ABI (divans_b200_ir_to_cmds); feed the blob to ``Engine.encode(..., cmds=True)``."""
@@ -301,10 +335,7 @@ class Engine:
     # -- host-buffer paths (numpy arrays; `in_blob`/`out` may be pinned)
     def decode_batch_host(self, in_blob, in_off, in_len, out, out_off, out_cap, flags=0):
         n = len(in_off)
-        in_off, in_len = np.ascontiguousarray(in_off, np.uint64), np.ascontiguousarray(in_len, np.uint64)
-        out_off, out_cap = np.ascontiguousarray(out_off, np.uint64), np.ascontiguousarray(out_cap, np.uint64)
-        out_len = np.zeros(n, np.uint64)
-        status = np.full(n, DIVANS_FAILURE, np.int32)
+        in_off, in_len, out_off, out_cap, out_len, status = _host_batch(in_off, in_len, out_off, out_cap)
         rc = self._L.divans_b200_decode_batch_host(self._h, n, _ptr(in_blob), _ptr(in_off), _ptr(in_len), _ptr(out), _ptr(out_off),
                                                    _ptr(out_cap), _ptr(out_len), _ptr(status), flags)
         if rc != DIVANS_SUCCESS:
@@ -316,10 +347,7 @@ class Engine:
         batches in flight; pass pinned ``in_blob`` / ``out`` (e.g. torch pinned tensors' numpy views) for the copies to
         overlap the kernels of the neighbouring batches."""
         n = len(in_off)
-        keep = [np.ascontiguousarray(in_off, np.uint64), np.ascontiguousarray(in_len, np.uint64),
-                np.ascontiguousarray(out_off, np.uint64), np.ascontiguousarray(out_cap, np.uint64)]
-        out_len = np.zeros(n, np.uint64)
-        status = np.full(n, DIVANS_FAILURE, np.int32)
+        *keep, out_len, status = _host_batch(in_off, in_len, out_off, out_cap)
         ticket = ctypes.c_int32(-1)
         rc = self._L.divans_b200_decode_batch_host_async(self._h, n, _ptr(in_blob), _ptr(keep[0]), _ptr(keep[1]), _ptr(out), _ptr(keep[2]),
                                                          _ptr(keep[3]), _ptr(out_len), _ptr(status), flags, ctypes.byref(ticket))
@@ -349,21 +377,10 @@ class Engine:
 
     def decode(self, streams, out_caps, flags=0):
         """Convenience: list of bytes -> list of (status, bytes)."""
-        bufs = [_u8(s) for s in streams]
-        in_len = np.array([b.size for b in bufs], np.uint64)
-        in_off = np.zeros(len(bufs), np.uint64)
-        pad = (in_len + np.uint64(15)) & ~np.uint64(15)
-        if len(bufs) > 1:
-            in_off[1:] = np.cumsum(pad)[:-1]
-        blob = np.zeros(int(pad.sum()) + 16, np.uint8)
-        for b, o in zip(bufs, in_off):
-            blob[int(o):int(o) + b.size] = b
+        blob, in_off, in_len = _pack(streams)
         out_cap = np.array(out_caps, np.uint64)
-        opad = (out_cap + np.uint64(255)) & ~np.uint64(255)
-        out_off = np.zeros(len(bufs), np.uint64)
-        if len(bufs) > 1:
-            out_off[1:] = np.cumsum(opad)[:-1]
-        out = np.zeros(int(opad.sum()) + 256, np.uint8)
+        out_off, out_total = _regions(out_cap)
+        out = np.zeros(out_total, np.uint8)
         out_len, status = self.decode_batch_host(blob, in_off, in_len, out, out_off, out_cap, flags)
         return [(int(st), out[int(o):int(o) + int(n)].tobytes()) for st, o, n in zip(status, out_off, out_len)]
 
@@ -373,11 +390,9 @@ class Engine:
         (out_len, blob_len, status).  Status 2 with blob_len > blob_cap: the blob region was too small, blob_len is the size it
         needs (the stream was still decoded)."""
         n = len(in_off)
-        in_off, in_len = np.ascontiguousarray(in_off, np.uint64), np.ascontiguousarray(in_len, np.uint64)
-        out_off, out_cap = np.ascontiguousarray(out_off, np.uint64), np.ascontiguousarray(out_cap, np.uint64)
-        blob_off, blob_cap = np.ascontiguousarray(blob_off, np.uint64), np.ascontiguousarray(blob_cap, np.uint64)
-        out_len, blob_len = np.zeros(n, np.uint64), np.zeros(n, np.uint64)
-        status = np.full(n, DIVANS_FAILURE, np.int32)
+        in_off, in_len, out_off, out_cap, blob_off, blob_cap, out_len, status = _host_batch(in_off, in_len, out_off, out_cap, blob_off,
+                                                                                            blob_cap)
+        blob_len = np.zeros(n, np.uint64)
         rc = self._L.divans_b200_decode_cmds_batch_host(self._h, n, _ptr(in_blob), _ptr(in_off), _ptr(in_len), _ptr(out), _ptr(out_off),
                                                         _ptr(out_cap), _ptr(out_len), _ptr(blobs), _ptr(blob_off), _ptr(blob_cap),
                                                         _ptr(blob_len), _ptr(status), flags)
@@ -397,29 +412,16 @@ class Engine:
     def decode_cmds(self, streams, out_caps, flags=0):
         """Convenience: list of .divans bytes -> list of (status, decoded bytes, DVCL blob bytes).  A stream whose blob did not fit
         the first guess is decoded once more with the exact size the first call reported."""
-        bufs = [_u8(s) for s in streams]
-        n = len(bufs)
-        in_len = np.array([b.size for b in bufs], np.uint64)
-        in_off = np.zeros(n, np.uint64)
-        pad = (in_len + np.uint64(15)) & ~np.uint64(15)
-        if n > 1:
-            in_off[1:] = np.cumsum(pad)[:-1]
-        blob = np.zeros(int(pad.sum()) + 16, np.uint8)
-        for b, o in zip(bufs, in_off):
-            blob[int(o):int(o) + b.size] = b
+        blob, in_off, in_len = _pack(streams)
+        n = in_len.size
         out_cap = np.array(out_caps, np.uint64).reshape(n)
         blob_cap = first_blob_cap(out_cap)
         res = [None] * n
         todo = np.arange(n)
         for attempt in range(2):
             idx = todo
-            opad = (out_cap[idx] + np.uint64(255)) & ~np.uint64(255)
-            bpad = (blob_cap[idx] + np.uint64(255)) & ~np.uint64(255)
-            out_off, blob_off = np.zeros(len(idx), np.uint64), np.zeros(len(idx), np.uint64)
-            if len(idx) > 1:
-                out_off[1:], blob_off[1:] = np.cumsum(opad)[:-1], np.cumsum(bpad)[:-1]
-            out = np.zeros(int(opad.sum()) + 256, np.uint8)
-            blobs = np.zeros(int(bpad.sum()) + 256, np.uint8)
+            (out_off, out_total), (blob_off, blobs_total) = _regions(out_cap[idx]), _regions(blob_cap[idx])
+            out, blobs = np.zeros(out_total, np.uint8), np.zeros(blobs_total, np.uint8)
             out_len, blob_len, status = self.decode_cmds_batch_host(blob, in_off[idx], in_len[idx], out, out_off, out_cap[idx], blobs,
                                                                    blob_off, blob_cap[idx], flags)
             retry = []
@@ -447,31 +449,26 @@ class Engine:
                 raise DivansError("transcode: stream %d does not decode (status %d)" % (i, st))
         o = opts if opts is not None else encode_options(window_size=0)
         wins = [int(np.frombuffer(b[20:24], np.uint32)[0]) if o.window_size == 0 else int(o.window_size) for _, _, b in dec]
+        auto = candidates is not None
         res = [None] * len(dec)
         chosen = np.zeros(len(dec), np.uint32)
-        cost = np.zeros((len(dec), len(candidates) if candidates is not None else 0), np.uint64)
+        cost = np.zeros((len(dec), len(candidates) if auto else 0), np.uint64)
         for w in sorted(set(wins)):
             idx = [i for i, x in enumerate(wins) if x == w]
             ow = EncodeOptions.from_buffer_copy(o)
             ow.window_size = w
-            if candidates is None:
-                for i, e in zip(idx, self.encode([dec[i][2] for i in idx], ow, cmds=True)):
-                    res[i] = e
-                continue
-            st, outs, ch, co = self._auto_lists(True, [dec[i][2] for i in idx], ow, candidates)
+            st, outs, ch, co = self._encode_lists([dec[i][2] for i in idx], ow, True, auto, candidates)
             if (st != 0).any():
                 raise DivansError("encode failed for streams %s" % np.array(idx)[np.nonzero(st)[0][:8]])
             for k, i in enumerate(idx):
                 res[i] = outs[k]
-            chosen[idx], cost[idx] = ch, co
-        return res if candidates is None else (res, chosen, cost)
+            if auto:
+                chosen[idx], cost[idx] = ch, co
+        return (res, chosen, cost) if auto else res
 
     def encode_batch_host(self, in_blob, in_off, in_len, out, out_off, out_cap, opts=None, cmds=False):
         n = len(in_off)
-        in_off, in_len = np.ascontiguousarray(in_off, np.uint64), np.ascontiguousarray(in_len, np.uint64)
-        out_off, out_cap = np.ascontiguousarray(out_off, np.uint64), np.ascontiguousarray(out_cap, np.uint64)
-        out_len = np.zeros(n, np.uint64)
-        status = np.full(n, DIVANS_FAILURE, np.int32)
+        in_off, in_len, out_off, out_cap, out_len, status = _host_batch(in_off, in_len, out_off, out_cap)
         o = opts or encode_options()
         fn = self._L.divans_b200_encode_cmds_batch_host if cmds else self._L.divans_b200_encode_batch_host
         rc = fn(self._h, n, _ptr(in_blob), _ptr(in_off), _ptr(in_len), _ptr(out), _ptr(out_off), _ptr(out_cap), _ptr(out_len),
@@ -499,11 +496,8 @@ class Engine:
 
     def _auto_host(self, cmds, in_blob, in_off, in_len, out, out_off, out_cap, opts, candidates):
         n = len(in_off)
-        in_off, in_len = np.ascontiguousarray(in_off, np.uint64), np.ascontiguousarray(in_len, np.uint64)
-        out_off, out_cap = np.ascontiguousarray(out_off, np.uint64), np.ascontiguousarray(out_cap, np.uint64)
+        in_off, in_len, out_off, out_cap, out_len, status = _host_batch(in_off, in_len, out_off, out_cap)
         cands, nc = self._cands(candidates, cmds)
-        out_len = np.zeros(n, np.uint64)
-        status = np.full(n, DIVANS_FAILURE, np.int32)
         chosen = np.zeros(n, np.uint32)
         cost = np.zeros((n, nc), np.uint64)
         o = opts or encode_options()
@@ -551,31 +545,29 @@ class Engine:
         if rc != DIVANS_SUCCESS:
             raise DivansError("encode_cmds_auto_batch_device: " + self._err())
 
-    def _auto_lists(self, cmds, bufs, opts, candidates):
-        """encode_auto / encode_cmds_auto of byte strings: (status, list of bytes or None, chosen, cost)"""
-        bufs = [_u8(s) for s in bufs]
-        in_len = np.array([b.size for b in bufs], np.uint64)
-        pad = (in_len + np.uint64(15)) & ~np.uint64(15)
-        in_off = np.concatenate([[0], np.cumsum(pad)[:-1]]).astype(np.uint64) if bufs else np.zeros(0, np.uint64)
-        blob = np.zeros(int(pad.sum()) + 16, np.uint8)
-        for b, o in zip(bufs, in_off):
-            blob[int(o):int(o) + b.size] = b
-        out_cap = (in_len + in_len // np.uint64(2) + np.uint64(70000 + 255)) & ~np.uint64(255)
-        out_off = np.concatenate([[0], np.cumsum(out_cap)[:-1]]).astype(np.uint64) if bufs else np.zeros(0, np.uint64)
-        out = np.zeros(int(out_cap.sum()) + 16, np.uint8)
-        out_len, status, chosen, cost = self._auto_host(cmds, blob, in_off, in_len, out, out_off, out_cap, opts, candidates)
+    def _encode_lists(self, bufs, opts, cmds, auto, candidates=None):
+        """Byte strings (raw, or command lists with ``cmds``) through encode_batch_host, or with ``auto`` through
+        encode_auto / encode_cmds_auto: (status, list of bytes or None, chosen, cost), chosen and cost None without ``auto``."""
+        blob, in_off, in_len = _pack(bufs)
+        out_cap = _encoded_cap(in_len)
+        out_off, out_total = _regions(out_cap)
+        out = np.zeros(out_total, np.uint8)
+        if auto:
+            out_len, status, chosen, cost = self._auto_host(cmds, blob, in_off, in_len, out, out_off, out_cap, opts, candidates)
+        else:
+            (out_len, status), chosen, cost = self.encode_batch_host(blob, in_off, in_len, out, out_off, out_cap, opts, cmds), None, None
         return status, [out[int(o):int(o) + int(n)].tobytes() if s == DIVANS_SUCCESS else None for s, o, n in zip(status, out_off, out_len)], \
             chosen, cost
 
     def encode_auto(self, raws, opts=None, candidates=None):
         """Convenience: list of raw byte strings -> list of (status, .divans bytes or None, chosen candidate index)."""
-        status, outs, chosen, _ = self._auto_lists(False, raws, opts, candidates)
+        status, outs, chosen, _ = self._encode_lists(raws, opts, False, True, candidates)
         return [(int(s), b, int(c)) for s, b, c in zip(status, outs, chosen)]
 
     def encode_cmds_auto(self, blobs, opts=None, candidates=None):
         """Convenience: list of DVCL command-list blobs -> list of (status, .divans bytes or None, chosen candidate index), each
         list coded under the cheapest of ``candidates`` (encode_cmds_auto_batch_host)."""
-        status, outs, chosen, _ = self._auto_lists(True, blobs, opts, candidates)
+        status, outs, chosen, _ = self._encode_lists(blobs, opts, True, True, candidates)
         return [(int(s), b, int(c)) for s, b, c in zip(status, outs, chosen)]
 
     def encode_cmds_batch_device(self, n, d_blobs, d_blob_off, d_blob_len, max_blob_len, max_raw_len, d_out, d_out_off, d_out_cap, d_out_len,
@@ -619,24 +611,21 @@ class Engine:
             empty = torch.zeros(0, dtype=torch.uint8, device=dev), np.zeros(0, np.uint64), np.zeros(0, np.uint64), np.zeros(0, np.int32)
             return empty + (np.zeros(0, np.uint32), np.zeros((0, nc), np.uint64)) if auto else empty
 
-        pad = lambda c: (c + np.uint64(255)) & ~np.uint64(255)
-        new_caps = lambda bcap: pad(bcap + bcap // np.uint64(2) + np.uint64(70000))   # (Engine.encode's output rule)
-
         def run(idx, blob_cap, d_new=None):
             """decode + encode of streams idx on the device, one synchronisation: (d_new, new_off, new_len, status, blob_len,
-            decode status, chosen, cost).  The new streams go to `d_new` when given (at least new_caps(blob_cap).sum() bytes)."""
+            decode status, chosen, cost).  The new streams go to `d_new` when given (at least the total of
+            _regions(_encoded_cap(blob_cap)) bytes)."""
             m = len(idx)
             ocap, bcap = out_cap[idx], blob_cap
-            offs = lambda c: np.concatenate([[0], np.cumsum(pad(c))[:-1]]).astype(np.uint64)
-            new_cap = new_caps(bcap)
-            out_off, blob_off, new_off = offs(ocap), offs(bcap), offs(new_cap)
+            new_cap = _encoded_cap(bcap)
+            (out_off, out_total), (blob_off, blobs_total), (new_off, new_total) = _regions(ocap), _regions(bcap), _regions(new_cap)
             with torch.cuda.stream(s):
                 d_meta = u64(np.concatenate([in_off[idx], in_len[idx], out_off, ocap, blob_off, bcap, new_off, new_cap]))
                 M = [d_meta[k * m:(k + 1) * m] for k in range(8)]
-                d_out = torch.empty(int(pad(ocap).sum()), dtype=torch.uint8, device=dev)
-                d_blobs = torch.empty(int(pad(bcap).sum()), dtype=torch.uint8, device=dev)
+                d_out = torch.empty(out_total, dtype=torch.uint8, device=dev)
+                d_blobs = torch.empty(blobs_total, dtype=torch.uint8, device=dev)
                 if d_new is None:
-                    d_new = torch.empty(int(new_cap.sum()), dtype=torch.uint8, device=dev)
+                    d_new = torch.empty(new_total, dtype=torch.uint8, device=dev)
                 # out_len | blob_len | new_len | both statuses (| candidates: cost [m * C] | chosen)
                 d_res = torch.zeros((4 + (nc + 1 if auto else 0)) * m, dtype=torch.int64, device=dev)
                 d_st = d_res[3 * m:4 * m].view(torch.int32)
@@ -671,7 +660,7 @@ class Engine:
             # second pass encodes straight into its tail
             base = d_new.numel()
             with torch.cuda.stream(s):
-                out = torch.empty(base + int(new_caps(blob_len[retry]).sum()), dtype=torch.uint8, device=dev)
+                out = torch.empty(base + _regions(_encoded_cap(blob_len[retry]))[1], dtype=torch.uint8, device=dev)
                 out[:base].copy_(d_new)
             del d_new
             _, off2, len2, st2, _, _, ch2, co2 = run(retry, blob_len[retry], out[base:])
@@ -686,24 +675,10 @@ class Engine:
 
     def encode(self, raws, opts=None, cmds=False):
         """Convenience: list of raw byte strings (or DVCL command-list blobs with cmds=True) -> list of .divans bytes."""
-        bufs = [_u8(s) for s in raws]
-        in_len = np.array([b.size for b in bufs], np.uint64)
-        in_off = np.zeros(len(bufs), np.uint64)
-        pad = (in_len + np.uint64(15)) & ~np.uint64(15)
-        if len(bufs) > 1:
-            in_off[1:] = np.cumsum(pad)[:-1]
-        blob = np.zeros(int(pad.sum()) + 16, np.uint8)
-        for b, o in zip(bufs, in_off):
-            blob[int(o):int(o) + b.size] = b
-        out_cap = (in_len + in_len // np.uint64(2) + np.uint64(70000 + 255)) & ~np.uint64(255)
-        out_off = np.zeros(len(bufs), np.uint64)
-        if len(bufs) > 1:
-            out_off[1:] = np.cumsum(out_cap)[:-1]
-        out = np.zeros(int(out_cap.sum()), np.uint8)
-        out_len, status = self.encode_batch_host(blob, in_off, in_len, out, out_off, out_cap, opts, cmds)
+        status, outs, _, _ = self._encode_lists(raws, opts, cmds, False)
         if (status != 0).any():
             raise DivansError("encode failed for streams %s" % np.nonzero(status)[0][:8])
-        return [out[int(o):int(o) + int(n)].tobytes() for o, n in zip(out_off, out_len)]
+        return outs
 
 
 class DivansDecompressorReader(io.RawIOBase):

@@ -30,6 +30,15 @@ extern "C" const uint8_t dv_tables_blob[];
 
 using namespace dv;
 
+// HBM copies of a host batch (grow-only): the input blob, the output regions, and the descriptor arrays
+// in_off,in_len,out_off,out_cap,out_len (+status; decode_cmds: + blob_off,blob_cap,blob_len; encode_auto: + chosen,cost)
+struct HostBufs {
+    uint8_t *d_in = nullptr; size_t d_in_cap = 0;
+    uint8_t *d_out = nullptr; size_t d_out_cap = 0;
+    uint64_t *d_meta = nullptr; size_t d_meta_cap = 0;
+};
+static void free_host_bufs(HostBufs &b) { cudaFree(b.d_in); cudaFree(b.d_out); cudaFree(b.d_meta); }
+
 struct divans_b200_ctx {
     int device = 0;
     int lanes_per_stream = 8;
@@ -47,16 +56,12 @@ struct divans_b200_ctx {
     // grow-only scratch
     uint32_t *d_frame = nullptr; size_t frame_cap = 0;
     uint8_t *d_payload = nullptr; size_t payload_cap = 0;
-    uint8_t *d_in = nullptr; size_t d_in_cap = 0;
-    uint8_t *d_out = nullptr; size_t d_out_cap = 0;
-    uint64_t *d_meta = nullptr; size_t d_meta_cap = 0;   // in_off,in_len,out_off,out_cap,out_len (+status; decode_cmds: + blob_off,blob_cap,blob_len)
+    HostBufs host;                                         // the blocking host calls (decode and encode)
     uint8_t *d_blobs = nullptr; size_t d_blobs_cap = 0;   // decode_cmds_batch_host: the DVCL blob regions
     uint32_t *d_rec_counts = nullptr; size_t rec_counts_cap = 0;   // decode_cmds: per stream [3] what the recording decoder counted
     // pipelined host API (decode_batch_host_async): two batches in flight, copies on their own streams
     struct Lane {
-        uint8_t *d_in = nullptr; size_t d_in_cap = 0;
-        uint8_t *d_out = nullptr; size_t d_out_cap = 0;
-        uint64_t *d_meta = nullptr; size_t d_meta_cap = 0;
+        HostBufs bufs;
         cudaEvent_t e_in = nullptr, e_k = nullptr, e_out = nullptr;
         uint8_t *h_res = nullptr; size_t h_res_cap = 0;      // pinned staging of out_len[] + status[] (the caller's arrays may be pageable)
         uint64_t *u_out_len = nullptr; int32_t *u_status = nullptr; size_t n = 0;
@@ -162,7 +167,7 @@ extern "C" void divans_b200_destroy(divans_b200_ctx *ctx) {
     if (ctx->s_h2d) cudaStreamSynchronize(ctx->s_h2d);
     if (ctx->s_d2h) cudaStreamSynchronize(ctx->s_d2h);
     cudaFree(ctx->d_arena_raw); cudaFree(ctx->d_tables); cudaFree(ctx->d_counter); cudaFree(ctx->d_nibbles);
-    cudaFree(ctx->d_frame); cudaFree(ctx->d_payload); cudaFree(ctx->d_in); cudaFree(ctx->d_out); cudaFree(ctx->d_meta);
+    cudaFree(ctx->d_frame); cudaFree(ctx->d_payload); free_host_bufs(ctx->host);
     cudaFree(ctx->d_blobs); cudaFree(ctx->d_rec_counts);
     if (ctx->ev0) cudaEventDestroy(ctx->ev0);
     if (ctx->ev1) cudaEventDestroy(ctx->ev1);
@@ -172,7 +177,7 @@ extern "C" void divans_b200_destroy(divans_b200_ctx *ctx) {
     cudaFree(ctx->d_sf); cudaFree(ctx->d_replay); cudaFree(ctx->d_enc_scratch); cudaFree(ctx->d_pm_internal); cudaFree(ctx->d_rcp15);
     cudaFree(ctx->d_pm_records); cudaFree(ctx->d_cost_tab); cudaFree(ctx->d_auto);
     for (auto &ln : ctx->lane) {
-        cudaFree(ln.d_in); cudaFree(ln.d_out); cudaFree(ln.d_meta);
+        free_host_bufs(ln.bufs);
         if (ln.h_res) cudaFreeHost(ln.h_res);
         if (ln.e_in) cudaEventDestroy(ln.e_in);
         if (ln.e_k) cudaEventDestroy(ln.e_k);
@@ -308,49 +313,99 @@ extern "C" DivansResult divans_b200_decode_batch_device(divans_b200_ctx *ctx, si
     return decode_device_nolock(ctx, n, d_in, d_in_off, d_in_len, d_out, d_out_off, d_out_cap, d_out_len, d_status, in_total_bytes, flags, cuda_stream);
 }
 
-extern "C" DivansResult divans_b200_decode_batch_host(divans_b200_ctx *ctx, size_t n, const uint8_t *in, const uint64_t *in_off,
-                                                      const uint64_t *in_len, uint8_t *out, const uint64_t *out_off,
-                                                      const uint64_t *out_cap, uint64_t *out_len, int32_t *status, uint32_t flags) {
+// ---- host-buffer decode ----
+// the blob regions of divans_b200_decode_cmds_batch_host
+struct HostBlobs {
+    uint8_t *blobs; const uint64_t *off, *cap; uint64_t *len;
+};
+
+// [lo, hi): the span of the regions off[i] .. +cap[i] (n > 0)
+static void regions_span(size_t n, const uint64_t *off, const uint64_t *cap, uint64_t &lo, uint64_t &hi) {
+    lo = ~0ull; hi = 0;
+    for (size_t i = 0; i < n; i++) { lo = std::min(lo, off[i]); hi = std::max(hi, off[i] + cap[i]); }
+}
+
+// Stage a host batch into `b`: the input and the descriptor arrays in_off | in_len | out_off | out_cap (| blob_off | blob_cap
+// at 6n, 7n) are copied on `h2d`; then, on `st` (ordered after them by `e_in` when the two streams differ), the output (and
+// blob) regions are zeroed.  The regions are copied back whole, so what they hold past the lengths is zeros, not an earlier
+// batch.  Input regions may alias (the same stream decoded n times): `in_total` bounds the decoder's payload by the larger
+// of their sum and their extent.
+static DivansResult stage_decode(divans_b200_ctx *ctx, HostBufs &b, size_t n, const uint8_t *in, const uint64_t *in_off,
+                                 const uint64_t *in_len, const uint64_t *out_off, const uint64_t *out_cap, const HostBlobs *bl,
+                                 cudaStream_t h2d, cudaEvent_t e_in, cudaStream_t st, uint64_t &in_total) {
+    uint64_t in_end = 0, in_sum = 0, out_lo, out_hi, blob_lo = 0, blob_hi = 0;
+    for (size_t i = 0; i < n; i++) { in_end = std::max(in_end, in_off[i] + in_len[i]); in_sum += in_len[i]; }
+    regions_span(n, out_off, out_cap, out_lo, out_hi);
+    if (bl) regions_span(n, bl->off, bl->cap, blob_lo, blob_hi);
+    // (re)allocation synchronises the device: with the pipelined call, only while it warms up
+    if (!grow(ctx, &b.d_in, &b.d_in_cap, (size_t)in_end + 64)) return DIVANS_FAILURE;
+    if (!grow(ctx, &b.d_out, &b.d_out_cap, (size_t)out_hi + 64)) return DIVANS_FAILURE;
+    if (!grow(ctx, &b.d_meta, &b.d_meta_cap, n * (bl ? 9 : 6))) return DIVANS_FAILURE;
+    if (bl && !grow(ctx, &ctx->d_blobs, &ctx->d_blobs_cap, (size_t)blob_hi + 64)) return DIVANS_FAILURE;
+    uint64_t *m = b.d_meta;
+    CK(cudaMemcpyAsync(b.d_in, in, in_end, cudaMemcpyHostToDevice, h2d));
+    CK(cudaMemcpyAsync(m, in_off, n * 8, cudaMemcpyHostToDevice, h2d));
+    CK(cudaMemcpyAsync(m + n, in_len, n * 8, cudaMemcpyHostToDevice, h2d));
+    CK(cudaMemcpyAsync(m + 2 * n, out_off, n * 8, cudaMemcpyHostToDevice, h2d));
+    CK(cudaMemcpyAsync(m + 3 * n, out_cap, n * 8, cudaMemcpyHostToDevice, h2d));
+    if (bl) {
+        CK(cudaMemcpyAsync(m + 6 * n, bl->off, n * 8, cudaMemcpyHostToDevice, h2d));
+        CK(cudaMemcpyAsync(m + 7 * n, bl->cap, n * 8, cudaMemcpyHostToDevice, h2d));
+    }
+    if (h2d != st) {
+        CK(cudaEventRecord(e_in, h2d));
+        CK(cudaStreamWaitEvent(st, e_in, 0));
+    }
+    if (out_hi > out_lo) CK(cudaMemsetAsync(b.d_out + out_lo, 0, out_hi - out_lo, st));
+    if (blob_hi > blob_lo) CK(cudaMemsetAsync(ctx->d_blobs + blob_lo, 0, blob_hi - blob_lo, st));
+    in_total = std::max(in_sum, in_end);
+    return DIVANS_SUCCESS;
+}
+
+// D2H of whole regions src[off[i] .. +cap[i]) to dst, one transfer per run of exactly adjacent regions: nothing outside them is written
+static DivansResult copy_regions_back(divans_b200_ctx *ctx, size_t n, uint8_t *dst, const uint8_t *src, const uint64_t *off,
+                                      const uint64_t *cap, cudaStream_t st) {
+    for (size_t i = 0; i < n;) {
+        const uint64_t lo = off[i]; uint64_t hi = lo + cap[i];
+        size_t j = i + 1;
+        while (j < n && off[j] == hi) { hi += cap[j]; j++; }
+        if (hi > lo) CK(cudaMemcpyAsync(dst + lo, src + lo, hi - lo, cudaMemcpyDeviceToHost, st));
+        i = j;
+    }
+    return DIVANS_SUCCESS;
+}
+
+// divans_b200_decode_batch_host, and with `bl` divans_b200_decode_cmds_batch_host: one synchronisation, at the end
+static DivansResult decode_host(divans_b200_ctx *ctx, size_t n, const uint8_t *in, const uint64_t *in_off, const uint64_t *in_len,
+                                uint8_t *out, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_len, int32_t *status,
+                                uint32_t flags, const HostBlobs *bl) {
     if (!ctx) return DIVANS_FAILURE;
     if (n == 0) return DIVANS_SUCCESS;
     std::lock_guard<std::mutex> lk(ctx->mu);
     CK(cudaSetDevice(ctx->device));
-    // extent of the input / output blobs
-    uint64_t in_end = 0, out_end = 0, in_sum = 0;
-    for (size_t i = 0; i < n; i++) {
-        if (in_off[i] + in_len[i] > in_end) in_end = in_off[i] + in_len[i];
-        if (out_off[i] + out_cap[i] > out_end) out_end = out_off[i] + out_cap[i];
-        in_sum += in_len[i];                       // input regions may alias (the same stream decoded n times)
-    }
-    if (!grow(ctx, &ctx->d_in, &ctx->d_in_cap, (size_t)in_end + 64)) return DIVANS_FAILURE;
-    if (!grow(ctx, &ctx->d_out, &ctx->d_out_cap, (size_t)out_end + 64)) return DIVANS_FAILURE;
-    if (!grow(ctx, &ctx->d_meta, &ctx->d_meta_cap, n * 6)) return DIVANS_FAILURE;
-    uint64_t *m = ctx->d_meta;
+    HostBufs &b = ctx->host;
     cudaStream_t st = ctx->stream;
-    CK(cudaMemcpyAsync(ctx->d_in, in, in_end, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(m, in_off, n * 8, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(m + n, in_len, n * 8, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(m + 2 * n, out_off, n * 8, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(m + 3 * n, out_cap, n * 8, cudaMemcpyHostToDevice, st));
+    uint64_t in_total;
+    if (stage_decode(ctx, b, n, in, in_off, in_len, out_off, out_cap, bl, st, nullptr, st, in_total) != DIVANS_SUCCESS) return DIVANS_FAILURE;
+    uint64_t *m = b.d_meta;
     int32_t *d_status = reinterpret_cast<int32_t *>(m + 5 * n);
-    CK(cudaMemsetAsync(ctx->d_out, 0, out_end, st));   // what the regions hold past out_len[i] is zeros, not an earlier batch
-    DivansResult r = decode_device_nolock(ctx, n, ctx->d_in, m, m + n, ctx->d_out, m + 2 * n, m + 3 * n, m + 4 * n, d_status,
-                                          in_sum > in_end ? in_sum : in_end, flags, st);
+    RecParams rp;
+    if (bl) { rp.blobs = ctx->d_blobs; rp.blob_off = m + 6 * n; rp.blob_cap = m + 7 * n; rp.blob_len = m + 8 * n; rp.counts = nullptr; }
+    DivansResult r = decode_device_nolock(ctx, n, b.d_in, m, m + n, b.d_out, m + 2 * n, m + 3 * n, m + 4 * n, d_status, in_total, flags,
+                                          st, bl ? &rp : nullptr);
     if (r != DIVANS_SUCCESS) return r;
     CK(cudaMemcpyAsync(out_len, m + 4 * n, n * 8, cudaMemcpyDeviceToHost, st));
+    if (bl) CK(cudaMemcpyAsync(bl->len, m + 8 * n, n * 8, cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(status, d_status, n * 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    // Copy back whole regions (zeros past out_len[i]: d_out was cleared before the kernels) and never a byte outside a declared
-    // region out[out_off[i] .. +out_cap[i]): consecutive streams whose regions are exactly adjacent share one transfer.
-    for (size_t i = 0; i < n;) {
-        const uint64_t lo = out_off[i]; uint64_t hi = lo + out_cap[i];
-        size_t j = i + 1;
-        while (j < n && out_off[j] == hi) { hi += out_cap[j]; j++; }
-        if (hi > lo) CK(cudaMemcpyAsync(out + lo, ctx->d_out + lo, hi - lo, cudaMemcpyDeviceToHost, st));
-        i = j;
-    }
+    if (copy_regions_back(ctx, n, out, b.d_out, out_off, out_cap, st) != DIVANS_SUCCESS) return DIVANS_FAILURE;
+    if (bl && copy_regions_back(ctx, n, bl->blobs, ctx->d_blobs, bl->off, bl->cap, st) != DIVANS_SUCCESS) return DIVANS_FAILURE;
     CK(cudaStreamSynchronize(st));
     return DIVANS_SUCCESS;
+}
+extern "C" DivansResult divans_b200_decode_batch_host(divans_b200_ctx *ctx, size_t n, const uint8_t *in, const uint64_t *in_off,
+                                                      const uint64_t *in_len, uint8_t *out, const uint64_t *out_off,
+                                                      const uint64_t *out_cap, uint64_t *out_len, int32_t *status, uint32_t flags) {
+    return decode_host(ctx, n, in, in_off, in_len, out, out_off, out_cap, out_len, status, flags, nullptr);
 }
 
 // ---- decode to command lists ----
@@ -367,62 +422,13 @@ extern "C" DivansResult divans_b200_decode_cmds_batch_device(divans_b200_ctx *ct
     return decode_device_nolock(ctx, n, d_in, d_in_off, d_in_len, d_out, d_out_off, d_out_cap, d_out_len, d_status, in_total_bytes, flags,
                                 cuda_stream, &rp);
 }
-// D2H of whole regions base[off[i] .. +cap[i]), one transfer per run of exactly adjacent regions: nothing outside them is written
-static DivansResult copy_regions_back(divans_b200_ctx *ctx, size_t n, uint8_t *dst, const uint8_t *src, const uint64_t *off,
-                                      const uint64_t *cap, cudaStream_t st) {
-    for (size_t i = 0; i < n;) {
-        const uint64_t lo = off[i]; uint64_t hi = lo + cap[i];
-        size_t j = i + 1;
-        while (j < n && off[j] == hi) { hi += cap[j]; j++; }
-        if (hi > lo) CK(cudaMemcpyAsync(dst + lo, src + lo, hi - lo, cudaMemcpyDeviceToHost, st));
-        i = j;
-    }
-    return DIVANS_SUCCESS;
-}
 extern "C" DivansResult divans_b200_decode_cmds_batch_host(divans_b200_ctx *ctx, size_t n, const uint8_t *in, const uint64_t *in_off,
                                                            const uint64_t *in_len, uint8_t *out, const uint64_t *out_off,
                                                            const uint64_t *out_cap, uint64_t *out_len, uint8_t *blobs,
                                                            const uint64_t *blob_off, const uint64_t *blob_cap, uint64_t *blob_len,
                                                            int32_t *status, uint32_t flags) {
-    if (!ctx) return DIVANS_FAILURE;
-    if (n == 0) return DIVANS_SUCCESS;
-    std::lock_guard<std::mutex> lk(ctx->mu);
-    CK(cudaSetDevice(ctx->device));
-    uint64_t in_end = 0, out_end = 0, blob_end = 0, in_sum = 0;
-    for (size_t i = 0; i < n; i++) {
-        in_end = std::max(in_end, in_off[i] + in_len[i]);
-        out_end = std::max(out_end, out_off[i] + out_cap[i]);
-        blob_end = std::max(blob_end, blob_off[i] + blob_cap[i]);
-        in_sum += in_len[i];
-    }
-    if (!grow(ctx, &ctx->d_in, &ctx->d_in_cap, (size_t)in_end + 64)) return DIVANS_FAILURE;
-    if (!grow(ctx, &ctx->d_out, &ctx->d_out_cap, (size_t)out_end + 64)) return DIVANS_FAILURE;
-    if (!grow(ctx, &ctx->d_blobs, &ctx->d_blobs_cap, (size_t)blob_end + 64)) return DIVANS_FAILURE;
-    if (!grow(ctx, &ctx->d_meta, &ctx->d_meta_cap, n * 9)) return DIVANS_FAILURE;
-    uint64_t *m = ctx->d_meta;   // in_off, in_len, out_off, out_cap, out_len, status, blob_off, blob_cap, blob_len
-    cudaStream_t st = ctx->stream;
-    CK(cudaMemcpyAsync(ctx->d_in, in, in_end, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(m, in_off, n * 8, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(m + n, in_len, n * 8, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(m + 2 * n, out_off, n * 8, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(m + 3 * n, out_cap, n * 8, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(m + 6 * n, blob_off, n * 8, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(m + 7 * n, blob_cap, n * 8, cudaMemcpyHostToDevice, st));
-    int32_t *d_status = reinterpret_cast<int32_t *>(m + 5 * n);
-    CK(cudaMemsetAsync(ctx->d_out, 0, out_end, st));      // the regions are copied back whole: zeros past the lengths
-    CK(cudaMemsetAsync(ctx->d_blobs, 0, blob_end, st));
-    RecParams rp;
-    rp.blobs = ctx->d_blobs; rp.blob_off = m + 6 * n; rp.blob_cap = m + 7 * n; rp.blob_len = m + 8 * n; rp.counts = nullptr;
-    DivansResult r = decode_device_nolock(ctx, n, ctx->d_in, m, m + n, ctx->d_out, m + 2 * n, m + 3 * n, m + 4 * n, d_status,
-                                          in_sum > in_end ? in_sum : in_end, flags, st, &rp);
-    if (r != DIVANS_SUCCESS) return r;
-    CK(cudaMemcpyAsync(out_len, m + 4 * n, n * 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(blob_len, m + 8 * n, n * 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(status, d_status, n * 4, cudaMemcpyDeviceToHost, st));
-    if (copy_regions_back(ctx, n, out, ctx->d_out, out_off, out_cap, st) != DIVANS_SUCCESS) return DIVANS_FAILURE;
-    if (copy_regions_back(ctx, n, blobs, ctx->d_blobs, blob_off, blob_cap, st) != DIVANS_SUCCESS) return DIVANS_FAILURE;
-    CK(cudaStreamSynchronize(st));
-    return DIVANS_SUCCESS;
+    const HostBlobs bl = {blobs, blob_off, blob_cap, blob_len};
+    return decode_host(ctx, n, in, in_off, in_len, out, out_off, out_cap, out_len, status, flags, &bl);
 }
 
 extern "C" void divans_b200_encode_options_default(divans_b200_encode_options *o) {
@@ -464,51 +470,27 @@ extern "C" DivansResult divans_b200_decode_batch_host_async(divans_b200_ctx *ctx
         CK(cudaEventCreateWithFlags(&ln.e_in, cudaEventDisableTiming)); CK(cudaEventCreateWithFlags(&ln.e_k, cudaEventDisableTiming));
         CK(cudaEventCreateWithFlags(&ln.e_out, cudaEventDisableTiming));
     }
-    uint64_t in_end = 0, in_sum = 0, out_lo = ~0ull, out_hi = 0;
-    for (size_t i = 0; i < n; i++) {
-        if (in_off[i] + in_len[i] > in_end) in_end = in_off[i] + in_len[i];
-        if (out_off[i] < out_lo) out_lo = out_off[i];
-        if (out_off[i] + out_cap[i] > out_hi) out_hi = out_off[i] + out_cap[i];
-        in_sum += in_len[i];
-    }
-    // (re)allocation of a lane's buffers synchronises the device: only while the pipeline warms up
-    if (!grow(ctx, &ln.d_in, &ln.d_in_cap, (size_t)in_end + 64)) return DIVANS_FAILURE;
-    if (!grow(ctx, &ln.d_out, &ln.d_out_cap, (size_t)out_hi + 64)) return DIVANS_FAILURE;
-    if (!grow(ctx, &ln.d_meta, &ln.d_meta_cap, n * 6)) return DIVANS_FAILURE;
     if (ln.h_res_cap < n * 12) {
         if (ln.h_res) cudaFreeHost(ln.h_res);
         ln.h_res = nullptr; ln.h_res_cap = 0;
         CK(cudaMallocHost((void **)&ln.h_res, n * 12 + 64));
         ln.h_res_cap = n * 12 + 64;
     }
+    uint64_t in_total;
+    if (stage_decode(ctx, ln.bufs, n, in, in_off, in_len, out_off, out_cap, nullptr, ctx->s_h2d, ln.e_in, ctx->stream, in_total) !=
+        DIVANS_SUCCESS)
+        return DIVANS_FAILURE;
     ln.u_out_len = out_len; ln.u_status = status; ln.n = n;
-    uint64_t *m = ln.d_meta;
-    CK(cudaMemcpyAsync(ln.d_in, in, in_end, cudaMemcpyHostToDevice, ctx->s_h2d));
-    CK(cudaMemcpyAsync(m, in_off, n * 8, cudaMemcpyHostToDevice, ctx->s_h2d));
-    CK(cudaMemcpyAsync(m + n, in_len, n * 8, cudaMemcpyHostToDevice, ctx->s_h2d));
-    CK(cudaMemcpyAsync(m + 2 * n, out_off, n * 8, cudaMemcpyHostToDevice, ctx->s_h2d));
-    CK(cudaMemcpyAsync(m + 3 * n, out_cap, n * 8, cudaMemcpyHostToDevice, ctx->s_h2d));
-    CK(cudaEventRecord(ln.e_in, ctx->s_h2d));
-    CK(cudaStreamWaitEvent(ctx->stream, ln.e_in, 0));
+    uint64_t *m = ln.bufs.d_meta;
     int32_t *d_status = reinterpret_cast<int32_t *>(m + 5 * n);
-    // the regions are copied back whole (out_len is not known yet): zero them first so that the bytes past out_len are
-    // zeros, not plaintext of an earlier batch
-    if (out_hi > out_lo) CK(cudaMemsetAsync(ln.d_out + out_lo, 0, out_hi - out_lo, ctx->stream));
-    DivansResult r = decode_device_nolock(ctx, n, ln.d_in, m, m + n, ln.d_out, m + 2 * n, m + 3 * n, m + 4 * n, d_status,
-                                          in_sum > in_end ? in_sum : in_end, flags, ctx->stream);
+    DivansResult r = decode_device_nolock(ctx, n, ln.bufs.d_in, m, m + n, ln.bufs.d_out, m + 2 * n, m + 3 * n, m + 4 * n, d_status,
+                                          in_total, flags, ctx->stream);
     if (r != DIVANS_SUCCESS) return r;
     CK(cudaEventRecord(ln.e_k, ctx->stream));
     CK(cudaStreamWaitEvent(ctx->s_d2h, ln.e_k, 0));
     CK(cudaMemcpyAsync(ln.h_res, m + 4 * n, n * 8, cudaMemcpyDeviceToHost, ctx->s_d2h));
     CK(cudaMemcpyAsync(ln.h_res + n * 8, d_status, n * 4, cudaMemcpyDeviceToHost, ctx->s_d2h));
-    // one transfer per run of exactly adjacent regions: nothing outside out[out_off[i] .. +out_cap[i]) is written
-    for (size_t i = 0; i < n;) {
-        const uint64_t lo = out_off[i]; uint64_t hi = lo + out_cap[i];
-        size_t j = i + 1;
-        while (j < n && out_off[j] == hi) { hi += out_cap[j]; j++; }
-        if (hi > lo) CK(cudaMemcpyAsync(out + lo, ln.d_out + lo, hi - lo, cudaMemcpyDeviceToHost, ctx->s_d2h));
-        i = j;
-    }
+    if (copy_regions_back(ctx, n, out, ln.bufs.d_out, out_off, out_cap, ctx->s_d2h) != DIVANS_SUCCESS) return DIVANS_FAILURE;
     CK(cudaEventRecord(ln.e_out, ctx->s_d2h));
     ln.pending = true;
     *ticket = t;
@@ -540,27 +522,101 @@ static void raw_record(uint8_t *pm, int pred_mode, int mixing_value) {
     memset(pm + 32 + 16384 + 1024, mixing_value, 8192);
 }
 
-// One launch set over n streams whose inputs/outputs already sit in HBM.  `cmd_cap`/`lit_cap`: log entries per stream,
-// `replay_stride`: bytes of replay window per resident slot, `max_in_len`: the longest command list the caps were sized for,
-// `window`: 10..24, or 0 for each command list's own window.
+// ---- encoder log sizing ----
+// Every stream of a launch owns `cmd` + `lit` u32 symbol-log entries, and every resident slot `replay` bytes of replay window.
+struct LogCaps {
+    uint64_t cmd, lit, replay;
+};
+
+// the replay window of a stream whose commands replay at most `len` bytes
+static uint64_t replay_bytes(uint64_t len) { return (len + 31) & ~15ull; }
+
+static uint32_t raw_cmd_cap(uint64_t max_len, int window) { return (uint32_t)(32 * (2 + (max_len >> window)) + 62000 + 64); }
+// raw buffers of at most max_len bytes, coded with `window` (10..24)
+static LogCaps raw_log_caps(uint64_t max_len, int window) { return {raw_cmd_cap(max_len, window), 2 * max_len + 16, replay_bytes(max_len)}; }
+
+// Log entries of the command lists of one device call: at most L bytes each, replaying at most max_raw_len bytes each.
+//  * Command entries.  The host call sizes a list with header (n_cmds c, n_predmodes p) at 32c + 62000p + 64, and a list the
+//    model pass accepts has 20c + 25632p <= R = L - 32.  For a fixed p the most commands are c = floor((R - 25632p) / 20).  One
+//    more record (p + 1) costs 25632 bytes, at most ceil(25632 / 20) = 1282 commands, and gains 62000 - 32 * 1282 = 20976 > 0
+//    entries: the maximum is at the most records, p = floor(R / 25632), with the rest of the bytes in commands.
+//  * Literal entries.  The host call sizes a list at 2s + 16, s = the sum of its literal records' lengths; records may re-read
+//    pool bytes, so s is not bounded by L.  But every literal byte coded is also replayed, and the model pass refuses a literal
+//    that would not fit the replay window (status 2) before it checks the log: s <= replay, and 2 * replay + 16 always suffices.
+static LogCaps cmds_log_caps(uint64_t L, uint64_t max_raw_len) {
+    const uint64_t R = L > 32 ? L - 32 : 0, p = R / PM_RECORD_BYTES, replay = replay_bytes(max_raw_len);
+    return {32 * ((R - (uint64_t)PM_RECORD_BYTES * p) / 20) + 62000 * p + 64, 2 * replay + 16, replay};
+}
+//  * A candidate literal model (encode_cmds_auto) replaces records, not commands, so (c, p) and the bound stay those of the blob.
+//    But the bound holds per record, not per PredictionMode command: any number of commands may re-read one record, and each
+//    codes the whole record.  A raw record codes 64 literal-map and 4 distance-map entries more than a minimal one (empty maps),
+//    so a list whose commands re-read minimal records can fit the logs as given and outgrow them under every replacing record.
+//    The cost pass therefore counts each pair's entries against these same capacities: a pair that would outgrow them fails
+//    there (cost UINT64_MAX), and KEEP or another candidate that fits is chosen (test_many_commands_re_reading_small_records).
+
+// The host call sizes each command list exactly, from its header and commands: 32c + 62000p + 64 command entries, 2s + 16
+// literal entries (s: the bytes its literal records code), and the window of the bytes its commands replay.  A list that does
+// not parse gets the capacities of its header, and the model pass refuses it.  False: a list too large to encode.
+static bool list_log_caps(const uint8_t *b, uint64_t len, LogCaps &caps) {
+    uint32_t h[8] = {0};
+    if (len >= 32) memcpy(h, b, 32);
+    const uint64_t need = 32ull + 20ull * h[2] + (uint64_t)PM_RECORD_BYTES * h[3] + h[4];
+    uint64_t lit = 0, rep = 0;
+    if (len >= 32 && h[0] == 0x4c435644u && h[1] == 1 && need <= len) {
+        for (uint32_t c = 0; c < h[2]; c++) {
+            uint32_t r[5]; memcpy(r, b + 32 + 20ull * c, 20);
+            if (r[0] == 1) rep += r[2];
+            else if (r[0] == 2) rep += 64;            // dictionary word + transform prefix/suffix
+            else if (r[0] == 3) { lit += r[2]; rep += r[2]; }
+        }
+    }
+    if (lit > 0x7fff0000ull || rep > 0xfffffff0ull) return false;
+    caps = {32ull * h[2] + 62000ull * h[3] + 64, 2 * lit + 16, replay_bytes(rep)};
+    return true;
+}
+
+// The EncodeParams fields the model pass and the cost pass share: the n streams at d_in[d_in_off[v] .. +d_in_len[v]), the
+// context's arena, tables and replay windows, the log capacities `caps` (sized for streams of up to max_in_len bytes), the
+// window (10..24, or 0 for each command list's own) and the options.  Every other field is zero.
+static EncodeParams encode_params(const divans_b200_ctx *ctx, size_t n, int raw_mode, const uint8_t *d_in, const uint64_t *d_in_off,
+                                  const uint64_t *d_in_len, uint64_t max_in_len, const LogCaps &caps, const divans_b200_encode_options *o,
+                                  int window) {
+    EncodeParams ep;
+    memset(&ep, 0, sizeof ep);
+    ep.in = d_in; ep.in_off = d_in_off; ep.in_len = d_in_len; ep.raw_mode = raw_mode; ep.n_streams = (uint32_t)n;
+    ep.work_counter = ctx->d_counter; ep.arena = ctx->d_arena; ep.tables = ctx->d_tables;
+    ep.replay = ctx->d_replay; ep.replay_stride = caps.replay;
+    ep.cmd_cap = (uint32_t)caps.cmd; ep.lit_cap = (uint32_t)caps.lit;
+    ep.window_size = window; ep.max_in_len = max_in_len; ep.dynamic_context_mixing = o->dynamic_context_mixing & 0xff; ep.prior_depth = o->prior_depth & 0xff;
+    ep.use_context_map = o->use_context_map; ep.force_stride = o->force_stride; ep.have_literal_adaptation = o->have_literal_adaptation;
+    for (int k = 0; k < 4; k++) ep.literal_adaptation[k] = pack_speed(o->literal_adaptation[k]);
+    ep.model_rev = o->model_rev == DIVANS_B200_MODEL_WASM_2018 ? 1 : 0;
+    return ep;
+}
+
+// One launch set over n streams whose inputs/outputs already sit in HBM, with the log capacities `caps`.  Like every launch
+// sequence of a context, it waits for the previous call's last kernel (`ev_busy`, on whatever stream) before its first write to
+// the context's scratch.  `d_pm_records`: the caller's records (encode_auto_device_nolock), else raw streams start with the
+// record of the options.
 static DivansResult encode_device_internal(divans_b200_ctx *ctx, size_t n, int raw_mode, const uint8_t *d_in, const uint64_t *d_in_off,
-                                           const uint64_t *d_in_len, uint64_t max_in_len, uint32_t cmd_cap, uint32_t lit_cap,
-                                           uint64_t replay_stride, uint8_t *d_out, const uint64_t *d_out_off, const uint64_t *d_out_cap,
-                                           uint64_t *d_out_len, int32_t *d_status, const divans_b200_encode_options *o, int window,
-                                           cudaStream_t st, const uint8_t *d_pm_records = nullptr, const uint32_t *d_pm_index = nullptr,
-                                           uint32_t pm_keep = 0) {
+                                           const uint64_t *d_in_len, uint64_t max_in_len, const LogCaps &caps, uint8_t *d_out,
+                                           const uint64_t *d_out_off, const uint64_t *d_out_cap, uint64_t *d_out_len, int32_t *d_status,
+                                           const divans_b200_encode_options *o, int window, cudaStream_t st,
+                                           const uint8_t *d_pm_records = nullptr, const uint32_t *d_pm_index = nullptr, uint32_t pm_keep = 0) {
     const size_t slots = encode_slots(ctx, n);
     const uint32_t blocks = (uint32_t)(slots / ENCODE_GROUPS_PER_BLOCK);
     if (ensure_arena(ctx, slots) != DIVANS_SUCCESS) return DIVANS_FAILURE;
+    const uint32_t cmd_cap = (uint32_t)caps.cmd, lit_cap = (uint32_t)caps.lit;
     const uint32_t cmd_chunks = (cmd_cap + NUM_SYMBOLS_BEFORE_FLUSH - 1) / NUM_SYMBOLS_BEFORE_FLUSH;
     const uint32_t lit_chunks = (lit_cap + NUM_SYMBOLS_BEFORE_FLUSH - 1) / NUM_SYMBOLS_BEFORE_FLUSH;
     const uint32_t max_chunks = cmd_chunks + lit_chunks;
     if (!grow(ctx, &ctx->d_sf, &ctx->sf_cap, n * ((size_t)cmd_cap + lit_cap))) return DIVANS_FAILURE;
-    if (!grow(ctx, &ctx->d_replay, &ctx->replay_cap, slots * (size_t)replay_stride)) return DIVANS_FAILURE;
+    if (!grow(ctx, &ctx->d_replay, &ctx->replay_cap, slots * (size_t)caps.replay)) return DIVANS_FAILURE;
     // small per-stream scratch: counts [2n] | window [n] | dummy [slots] | chunk_w [n*max_chunks] | chunk_state [16*n*max_chunks]
     size_t words = 3 * n + slots + n * (size_t)max_chunks + 4 * n * (size_t)max_chunks + 16 + 2 * n * (size_t)max_chunks * (NUM_SYMBOLS_BEFORE_FLUSH / 64);
     if (!grow(ctx, &ctx->d_enc_scratch, &ctx->enc_scratch_cap, words)) return DIVANS_FAILURE;
     if (!ctx->d_pm_internal) CK(cudaMalloc((void **)&ctx->d_pm_internal, PM_RECORD_BYTES));
+    if (ctx->busy_recorded) CK(cudaStreamWaitEvent(st, ctx->ev_busy, 0));
     if (!ctx->d_rcp15) { CK(cudaMalloc((void **)&ctx->d_rcp15, 32768 * sizeof(uint64_t))); launch_rcp15_init(ctx->d_rcp15, st); ctx->launches += 1; }
     if (raw_mode && !d_pm_records) {
         std::vector<uint8_t> &pm = ctx->h_pm;
@@ -568,12 +624,9 @@ static DivansResult encode_device_internal(divans_b200_ctx *ctx, size_t n, int r
         raw_record(pm.data(), o->literal_pred_mode, o->literal_mixing_value);
         CK(cudaMemcpyAsync(ctx->d_pm_internal, pm.data(), PM_RECORD_BYTES, cudaMemcpyHostToDevice, st));
     }
-    EncodeParams ep;
-    ep.in = d_in; ep.in_off = d_in_off; ep.in_len = d_in_len; ep.raw_mode = raw_mode; ep.n_streams = (uint32_t)n;
-    ep.work_counter = ctx->d_counter; ep.arena = ctx->d_arena; ep.tables = ctx->d_tables;
-    ep.pm_internal = d_pm_records ? d_pm_records : ctx->d_pm_internal; ep.pm_index = d_pm_index; ep.pm_keep = pm_keep;   // (the caller's records)
-    ep.cost_tab = nullptr; ep.tally = nullptr;
-    ep.sf = ctx->d_sf; ep.cmd_cap = cmd_cap; ep.lit_cap = lit_cap;
+    EncodeParams ep = encode_params(ctx, n, raw_mode, d_in, d_in_off, d_in_len, max_in_len, caps, o, window);
+    ep.pm_internal = d_pm_records ? d_pm_records : ctx->d_pm_internal; ep.pm_index = d_pm_index; ep.pm_keep = pm_keep;
+    ep.sf = ctx->d_sf;
     uint32_t *w = ctx->d_enc_scratch;
     ep.sf_counts = w; w += 2 * n;
     ep.stream_window = w; w += n;
@@ -583,14 +636,8 @@ static DivansResult encode_device_internal(divans_b200_ctx *ctx, size_t n, int r
     ep.chunk_state = reinterpret_cast<uint8_t *>(w);
     ep.emit_bits = w + 4 * n * (size_t)max_chunks;
     ep.rcp15 = ctx->d_rcp15;
-    ep.replay = ctx->d_replay; ep.replay_stride = replay_stride;
     ep.max_chunks = max_chunks; ep.cmd_chunks = cmd_chunks;
     ep.out = d_out; ep.out_off = d_out_off; ep.out_cap = d_out_cap; ep.out_len = d_out_len; ep.status = d_status;
-    ep.window_size = window; ep.max_in_len = max_in_len; ep.dynamic_context_mixing = o->dynamic_context_mixing & 0xff; ep.prior_depth = o->prior_depth & 0xff;
-    ep.use_context_map = o->use_context_map; ep.force_stride = o->force_stride; ep.have_literal_adaptation = o->have_literal_adaptation;
-    for (int k = 0; k < 4; k++) ep.literal_adaptation[k] = pack_speed(o->literal_adaptation[k]);
-    ep.model_rev = o->model_rev == DIVANS_B200_MODEL_WASM_2018 ? 1 : 0;
-    if (ctx->busy_recorded) CK(cudaStreamWaitEvent(st, ctx->ev_busy, 0));
     CK(cudaMemsetAsync(ctx->d_counter, 0, 4, st));
     CK(cudaEventRecord(ctx->ev0, st));
     CK(cudaEventRecord(ctx->evm, st));
@@ -605,125 +652,11 @@ static DivansResult encode_device_internal(divans_b200_ctx *ctx, size_t n, int r
     return DIVANS_SUCCESS;
 }
 
-static uint32_t raw_cmd_cap(uint64_t max_len, int window) { return (uint32_t)(32 * (2 + (max_len >> window)) + 62000 + 64); }
-
-extern "C" DivansResult divans_b200_encode_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_in, const uint64_t *d_in_off,
-                                                        const uint64_t *d_in_len, uint64_t max_in_len, uint8_t *d_out,
-                                                        const uint64_t *d_out_off, const uint64_t *d_out_cap, uint64_t *d_out_len,
-                                                        int32_t *d_status, const divans_b200_encode_options *opts, void *cuda_stream) {
-    if (!ctx || !opts) return DIVANS_FAILURE;
-    if (n == 0) return DIVANS_SUCCESS;
-    if (n > 0xffffffffull || max_in_len > 0x7fff0000ull) { ctx->err = "batch too large"; return DIVANS_FAILURE; }
-    std::lock_guard<std::mutex> lk(ctx->mu);
-    CK(cudaSetDevice(ctx->device));
-    const int window = clamp_window(opts->window_size);
-    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream;
-    return encode_device_internal(ctx, n, 1, d_in, d_in_off, d_in_len, max_in_len, raw_cmd_cap(max_in_len, window),
-                                  (uint32_t)(2 * max_in_len + 16), (max_in_len + 31) & ~15ull, d_out, d_out_off, d_out_cap, d_out_len,
-                                  d_status, opts, window, st);
-}
-
-// Log entries of the command lists of one launch: at most L bytes each, replaying at most `replay` bytes each.
-//  * Command entries.  The host call sizes a list with header (n_cmds c, n_predmodes p) at 32c + 62000p + 64, and a list the
-//    model pass accepts has 20c + 25632p <= R = L - 32.  For a fixed p the most commands are c = floor((R - 25632p) / 20).  One
-//    more record (p + 1) costs 25632 bytes, at most ceil(25632 / 20) = 1282 commands, and gains 62000 - 32 * 1282 = 20976 > 0
-//    entries: the maximum is at the most records, p = floor(R / 25632), with the rest of the bytes in commands.
-//  * Literal entries.  The host call sizes a list at 2s + 16, s = the sum of its literal records' lengths; records may re-read
-//    pool bytes, so s is not bounded by L.  But every literal byte coded is also replayed, and the model pass refuses a literal
-//    that would not fit the replay window (status 2) before it checks the log: s <= replay, and 2 * replay + 16 always suffices.
-static void cmds_log_caps(uint64_t L, uint64_t replay, uint64_t &cmd, uint64_t &lit) {
-    const uint64_t R = L > 32 ? L - 32 : 0, p = R / PM_RECORD_BYTES;
-    cmd = 32 * ((R - (uint64_t)PM_RECORD_BYTES * p) / 20) + 62000 * p + 64;
-    lit = 2 * replay + 16;
-}
-//  * A candidate literal model (encode_cmds_auto) replaces records, not commands, so (c, p) and the bound stay those of the blob.
-//    But the bound holds per record, not per PredictionMode command: any number of commands may re-read one record, and each
-//    codes the whole record.  A raw record codes 64 literal-map and 4 distance-map entries more than a minimal one (empty maps),
-//    so a list whose commands re-read minimal records can fit the logs as given and outgrow them under every replacing record.
-//    The cost pass therefore counts each pair's entries against these same capacities: a pair that would outgrow them fails
-//    there (cost UINT64_MAX), and KEEP or another candidate that fits is chosen (test_many_commands_re_reading_small_records).
-
-// literal model selection of a batch (encode_host_common, encode_cmds_device_common): the candidates, and where chosen / cost go
+// literal model selection of a batch (encode_host_common, encode_device_common): the candidates, and where chosen / cost go
 struct AutoSel {
     const divans_b200_literal_model *cands; uint32_t n_cands;
     uint32_t *chosen; uint64_t *cost;
 };
-
-static DivansResult encode_auto_device_nolock(divans_b200_ctx *ctx, size_t n, int raw_mode, const uint8_t *d_in, const uint64_t *d_in_off,
-                                              const uint64_t *d_in_len, uint64_t max_in_len, uint32_t cmd_cap, uint32_t lit_cap,
-                                              uint64_t replay_stride, uint8_t *d_out, const uint64_t *d_out_off,
-                                              const uint64_t *d_out_cap, uint64_t *d_out_len, int32_t *d_status,
-                                              const divans_b200_encode_options *o, int window, const divans_b200_literal_model *cands,
-                                              uint32_t n_cands, uint32_t *d_chosen, uint64_t *d_cost, cudaStream_t st);
-static bool check_cands(divans_b200_ctx *ctx, const divans_b200_literal_model *cands, uint32_t n_cands, bool cmds);
-
-// divans_b200_encode_cmds_batch_device, and with `sel` (device chosen / cost) divans_b200_encode_cmds_auto_batch_device
-static DivansResult encode_cmds_device_common(divans_b200_ctx *ctx, size_t n, const uint8_t *d_blobs, const uint64_t *d_blob_off,
-                                              const uint64_t *d_blob_len, uint64_t max_blob_len, uint64_t max_raw_len, uint8_t *d_out,
-                                              const uint64_t *d_out_off, const uint64_t *d_out_cap, uint64_t *d_out_len, int32_t *d_status,
-                                              const divans_b200_encode_options *opts, void *cuda_stream, const AutoSel *sel) {
-    if (!ctx || !opts) return DIVANS_FAILURE;
-    if (sel && !check_cands(ctx, sel->cands, sel->n_cands, true)) return DIVANS_FAILURE;
-    if (n == 0) return DIVANS_SUCCESS;
-    if (sel && !sel->chosen) { ctx->err = "encode_cmds_auto: d_chosen is required"; return DIVANS_FAILURE; }
-    const uint64_t nv = (uint64_t)n * (sel ? sel->n_cands : 1);
-    if (nv > 0xffffffffull || max_blob_len > 0x7fff0000ull || max_raw_len > 0x7fff0000ull) { ctx->err = "batch too large"; return DIVANS_FAILURE; }
-    const uint64_t replay_stride = (max_raw_len + 31) & ~15ull;
-    uint64_t cmd_cap, lit_cap;
-    cmds_log_caps(max_blob_len, replay_stride, cmd_cap, lit_cap);
-    // the kernels address a stream's logs at v * (cmd_cap + lit_cap) with a 32-bit stride
-    if (cmd_cap + lit_cap > 0xffffffffull) { ctx->err = "batch too large"; return DIVANS_FAILURE; }
-    const int window = opts->window_size == 0 ? 0 : clamp_window(opts->window_size);
-    std::lock_guard<std::mutex> lk(ctx->mu);
-    CK(cudaSetDevice(ctx->device));
-    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream;
-    // the slots first, as in the host call: the logs are sized from what is left, and a failure names them.  (The cost pass of
-    // the n * C pairs has no logs; it runs in as many slots as the pairs fill.)
-    if (ensure_arena(ctx, encode_slots(ctx, nv)) != DIVANS_SUCCESS) return DIVANS_FAILURE;
-    // No sub-batching: the logs of all n streams are one allocation, of exactly their size (they are most of what the call
-    // needs next to the arena).  When it fails, the call fails and says how much it asked for.
-    const size_t words = n * (size_t)(cmd_cap + lit_cap);
-    if (words > ctx->sf_cap) {
-        cudaFree(ctx->d_sf); ctx->d_sf = nullptr; ctx->sf_cap = 0;
-        if (cudaMalloc((void **)&ctx->d_sf, words * 4) != cudaSuccess) {
-            cudaGetLastError();
-            char buf[200];
-            snprintf(buf, sizeof buf, "divans_b200: cannot allocate the symbol logs of %zu command lists of up to %llu bytes: %llu bytes", n,
-                     (unsigned long long)max_blob_len, (unsigned long long)words * 4);
-            ctx->err = buf;
-            return DIVANS_FAILURE;
-        }
-        ctx->sf_cap = words;
-    }
-    if (sel)
-        try {
-            return encode_auto_device_nolock(ctx, n, 0, d_blobs, d_blob_off, d_blob_len, max_blob_len, (uint32_t)cmd_cap, (uint32_t)lit_cap,
-                                             replay_stride, d_out, d_out_off, d_out_cap, d_out_len, d_status, opts, window, sel->cands,
-                                             sel->n_cands, sel->chosen, sel->cost, st);
-        } catch (...) { ctx->err = "divans_b200: out of host memory"; return DIVANS_FAILURE; }
-    return encode_device_internal(ctx, n, 0, d_blobs, d_blob_off, d_blob_len, max_blob_len, (uint32_t)cmd_cap, (uint32_t)lit_cap,
-                                  replay_stride, d_out, d_out_off, d_out_cap, d_out_len, d_status, opts, window, st);
-}
-
-extern "C" DivansResult divans_b200_encode_cmds_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_blobs, const uint64_t *d_blob_off,
-                                                             const uint64_t *d_blob_len, uint64_t max_blob_len, uint64_t max_raw_len,
-                                                             uint8_t *d_out, const uint64_t *d_out_off, const uint64_t *d_out_cap,
-                                                             uint64_t *d_out_len, int32_t *d_status, const divans_b200_encode_options *opts,
-                                                             void *cuda_stream) {
-    return encode_cmds_device_common(ctx, n, d_blobs, d_blob_off, d_blob_len, max_blob_len, max_raw_len, d_out, d_out_off, d_out_cap,
-                                     d_out_len, d_status, opts, cuda_stream, nullptr);
-}
-extern "C" DivansResult divans_b200_encode_cmds_auto_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_blobs,
-                                                                  const uint64_t *d_blob_off, const uint64_t *d_blob_len,
-                                                                  uint64_t max_blob_len, uint64_t max_raw_len, uint8_t *d_out,
-                                                                  const uint64_t *d_out_off, const uint64_t *d_out_cap, uint64_t *d_out_len,
-                                                                  int32_t *d_status, const divans_b200_encode_options *opts,
-                                                                  const divans_b200_literal_model *cands, uint32_t n_cands,
-                                                                  uint32_t *d_chosen, uint64_t *d_cost, void *cuda_stream) {
-    const AutoSel sel = {cands, n_cands, d_chosen, d_cost};
-    return encode_cmds_device_common(ctx, n, d_blobs, d_blob_off, d_blob_len, max_blob_len, max_raw_len, d_out, d_out_off, d_out_cap,
-                                     d_out_len, d_status, opts, cuda_stream, &sel);
-}
 
 // ---- literal model selection ----
 // Cost of coding a nibble of frequency f (1..32767 of 32768) in 1/65536 bit: 65536 * (15 - log2 f), the 16 fraction bits of
@@ -747,7 +680,7 @@ static uint32_t freq_cost(uint32_t f) {
 static bool is_keep(const divans_b200_literal_model &c) { return c.literal_pred_mode == -1 && c.literal_mixing_value == -1; }
 
 // `cmds`: the candidates of a command-list call, which may also be KEEP
-static bool check_cands(divans_b200_ctx *ctx, const divans_b200_literal_model *cands, uint32_t n_cands, bool cmds = false) {
+static bool check_cands(divans_b200_ctx *ctx, const divans_b200_literal_model *cands, uint32_t n_cands, bool cmds) {
     const char *who = cmds ? "encode_cmds_auto" : "encode_auto";
     char buf[200];
     if (!cands || n_cands < 1 || n_cands > 16) {
@@ -771,24 +704,23 @@ static bool check_cands(divans_b200_ctx *ctx, const divans_b200_literal_model *c
 // encoder pipeline with stream i coded under candidate d_chosen[i] (raw: its starting record; command lists: the record that
 // replaces each of the list's own, unless the candidate is KEEP).  The cost pass pulls virtual streams from the work counter
 // like the model pass, so however many there are, the context's encoder slots code them as many at a time as they hold.
-// cmd_cap / lit_cap / replay_stride / window: those of the plain call over the same n streams.
+// caps / window: those of the plain call over the same n streams.
 static DivansResult encode_auto_device_nolock(divans_b200_ctx *ctx, size_t n, int raw_mode, const uint8_t *d_in, const uint64_t *d_in_off,
-                                              const uint64_t *d_in_len, uint64_t max_in_len, uint32_t cmd_cap, uint32_t lit_cap,
-                                              uint64_t replay_stride, uint8_t *d_out, const uint64_t *d_out_off,
-                                              const uint64_t *d_out_cap, uint64_t *d_out_len, int32_t *d_status,
+                                              const uint64_t *d_in_len, uint64_t max_in_len, const LogCaps &caps, uint8_t *d_out,
+                                              const uint64_t *d_out_off, const uint64_t *d_out_cap, uint64_t *d_out_len, int32_t *d_status,
                                               const divans_b200_encode_options *o, int window, const divans_b200_literal_model *cands,
                                               uint32_t n_cands, uint32_t *d_chosen, uint64_t *d_cost, cudaStream_t st) {
     const uint64_t nv = (uint64_t)n * n_cands;
     const size_t vslots = encode_slots(ctx, nv);
     if (ensure_arena(ctx, vslots) != DIVANS_SUCCESS) return DIVANS_FAILURE;
-    if (!grow(ctx, &ctx->d_replay, &ctx->replay_cap, vslots * (size_t)replay_stride)) return DIVANS_FAILURE;
+    if (!grow(ctx, &ctx->d_replay, &ctx->replay_cap, vslots * (size_t)caps.replay)) return DIVANS_FAILURE;
     // v_off [nv] | v_len [nv] | tally [nv] | v_pm u32 [nv] | v_status i32 [nv]
     if (!grow(ctx, &ctx->d_auto, &ctx->auto_cap, 4 * nv + 2)) return DIVANS_FAILURE;
     uint64_t *v_off = ctx->d_auto, *v_len = v_off + nv, *tally = v_len + nv;
     uint32_t *v_pm = reinterpret_cast<uint32_t *>(tally + nv);
     int32_t *v_status = reinterpret_cast<int32_t *>(v_pm + nv);
     if (!ctx->d_pm_records) CK(cudaMalloc((void **)&ctx->d_pm_records, 16 * (size_t)PM_RECORD_BYTES));
-    if (ctx->busy_recorded) CK(cudaStreamWaitEvent(st, ctx->ev_busy, 0));   // (the records and scratch may still be read by the previous call)
+    if (ctx->busy_recorded) CK(cudaStreamWaitEvent(st, ctx->ev_busy, 0));
     if (!ctx->d_cost_tab) {
         static uint32_t tab[32768];
         static std::once_flag once;
@@ -806,55 +738,113 @@ static DivansResult encode_auto_device_nolock(divans_b200_ctx *ctx, size_t n, in
     CK(cudaMemcpyAsync(ctx->d_pm_records, pm.data(), pm.size(), cudaMemcpyHostToDevice, st));
     launch_auto_fanout(d_in_off, d_in_len, n, n_cands, v_off, v_len, v_pm, st);
 
-    EncodeParams tp;
-    memset(&tp, 0, sizeof tp);
-    tp.in = d_in; tp.in_off = v_off; tp.in_len = v_len; tp.raw_mode = raw_mode; tp.n_streams = (uint32_t)nv;
-    tp.work_counter = ctx->d_counter; tp.arena = ctx->d_arena; tp.tables = ctx->d_tables;
+    // no logs: cmd_cap / lit_cap are the final encode's capacities, which a pair must fit to be chosen
+    EncodeParams tp = encode_params(ctx, nv, raw_mode, d_in, v_off, v_len, max_in_len, caps, o, window);
     tp.pm_internal = ctx->d_pm_records; tp.pm_index = v_pm; tp.pm_keep = keep;
-    tp.replay = ctx->d_replay; tp.replay_stride = replay_stride;
-    tp.cmd_cap = cmd_cap; tp.lit_cap = lit_cap;   // (no logs: the final encode's capacity, which a pair must fit to be chosen)
     tp.status = v_status; tp.cost_tab = ctx->d_cost_tab; tp.tally = tally;
-    tp.window_size = window; tp.max_in_len = max_in_len; tp.dynamic_context_mixing = o->dynamic_context_mixing & 0xff; tp.prior_depth = o->prior_depth & 0xff;
-    tp.use_context_map = o->use_context_map; tp.force_stride = o->force_stride; tp.have_literal_adaptation = o->have_literal_adaptation;
-    for (int k = 0; k < 4; k++) tp.literal_adaptation[k] = pack_speed(o->literal_adaptation[k]);
-    tp.model_rev = o->model_rev == DIVANS_B200_MODEL_WASM_2018 ? 1 : 0;
     CK(cudaMemsetAsync(ctx->d_counter, 0, 4, st));
     const uint32_t blocks = (uint32_t)(vslots / ENCODE_GROUPS_PER_BLOCK);
     if (o->cdf_model == DIVANS_B200_CDF_BLEND) launch_encode_tally_blend(tp, blocks, st); else launch_encode_tally(tp, blocks, st);
     launch_auto_select(tally, v_status, n, n_cands, d_chosen, d_cost, st);
     ctx->launches += 3;
     CK(cudaGetLastError());
-    return encode_device_internal(ctx, n, raw_mode, d_in, d_in_off, d_in_len, max_in_len, cmd_cap, lit_cap, replay_stride, d_out, d_out_off,
-                                  d_out_cap, d_out_len, d_status, o, window, st, ctx->d_pm_records, d_chosen, keep);
+    return encode_device_internal(ctx, n, raw_mode, d_in, d_in_off, d_in_len, max_in_len, caps, d_out, d_out_off, d_out_cap, d_out_len,
+                                  d_status, o, window, st, ctx->d_pm_records, d_chosen, keep);
 }
 
+// The four device encode calls: raw buffers (max_raw_len = max_in_len) or command lists (raw_mode 0), each plain or, with
+// `sel` (device chosen / cost), coded under the cheapest candidate literal model.  Host marshalling (the candidates' records,
+// the error strings) may throw, and no C++ exception may cross the C boundary.
+static DivansResult encode_device_common(divans_b200_ctx *ctx, size_t n, int raw_mode, const uint8_t *d_in, const uint64_t *d_in_off,
+                                         const uint64_t *d_in_len, uint64_t max_in_len, uint64_t max_raw_len, uint8_t *d_out,
+                                         const uint64_t *d_out_off, const uint64_t *d_out_cap, uint64_t *d_out_len, int32_t *d_status,
+                                         const divans_b200_encode_options *opts, void *cuda_stream, const AutoSel *sel) try {
+    if (!ctx || !opts) return DIVANS_FAILURE;
+    if (sel && !check_cands(ctx, sel->cands, sel->n_cands, !raw_mode)) return DIVANS_FAILURE;
+    if (n == 0) return DIVANS_SUCCESS;
+    if (sel && !sel->chosen) { ctx->err = raw_mode ? "encode_auto: d_chosen is required" : "encode_cmds_auto: d_chosen is required"; return DIVANS_FAILURE; }
+    const uint64_t nv = (uint64_t)n * (sel ? sel->n_cands : 1);
+    if (nv > 0xffffffffull || max_in_len > 0x7fff0000ull || max_raw_len > 0x7fff0000ull) { ctx->err = "batch too large"; return DIVANS_FAILURE; }
+    const int window = !raw_mode && opts->window_size == 0 ? 0 : clamp_window(opts->window_size);
+    const LogCaps caps = raw_mode ? raw_log_caps(max_in_len, window) : cmds_log_caps(max_in_len, max_raw_len);
+    // the kernels address a stream's logs at v * (cmd_cap + lit_cap) with a 32-bit stride
+    if (caps.cmd + caps.lit > 0xffffffffull) { ctx->err = "batch too large"; return DIVANS_FAILURE; }
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream;
+    if (!raw_mode) {
+        // the slots first, as in the host call: the logs are sized from what is left, and a failure names them.  (The cost pass of
+        // the n * C pairs has no logs; it runs in as many slots as the pairs fill.)
+        if (ensure_arena(ctx, encode_slots(ctx, nv)) != DIVANS_SUCCESS) return DIVANS_FAILURE;
+        // No sub-batching: the logs of all n streams are one allocation, of exactly their size (they are most of what the call
+        // needs next to the arena).  When it fails, the call fails and says how much it asked for.
+        const size_t words = n * (size_t)(caps.cmd + caps.lit);
+        if (words > ctx->sf_cap) {
+            cudaFree(ctx->d_sf); ctx->d_sf = nullptr; ctx->sf_cap = 0;
+            if (cudaMalloc((void **)&ctx->d_sf, words * 4) != cudaSuccess) {
+                cudaGetLastError();
+                char buf[200];
+                snprintf(buf, sizeof buf, "divans_b200: cannot allocate the symbol logs of %zu command lists of up to %llu bytes: %llu bytes", n,
+                         (unsigned long long)max_in_len, (unsigned long long)words * 4);
+                ctx->err = buf;
+                return DIVANS_FAILURE;
+            }
+            ctx->sf_cap = words;
+        }
+    }
+    if (sel)
+        return encode_auto_device_nolock(ctx, n, raw_mode, d_in, d_in_off, d_in_len, max_in_len, caps, d_out, d_out_off, d_out_cap, d_out_len,
+                                         d_status, opts, window, sel->cands, sel->n_cands, sel->chosen, sel->cost, st);
+    return encode_device_internal(ctx, n, raw_mode, d_in, d_in_off, d_in_len, max_in_len, caps, d_out, d_out_off, d_out_cap, d_out_len,
+                                  d_status, opts, window, st);
+} catch (...) {
+    if (ctx) ctx->err = "divans_b200: out of host memory";
+    return DIVANS_FAILURE;
+}
+
+extern "C" DivansResult divans_b200_encode_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_in, const uint64_t *d_in_off,
+                                                        const uint64_t *d_in_len, uint64_t max_in_len, uint8_t *d_out,
+                                                        const uint64_t *d_out_off, const uint64_t *d_out_cap, uint64_t *d_out_len,
+                                                        int32_t *d_status, const divans_b200_encode_options *opts, void *cuda_stream) {
+    return encode_device_common(ctx, n, 1, d_in, d_in_off, d_in_len, max_in_len, max_in_len, d_out, d_out_off, d_out_cap, d_out_len,
+                                d_status, opts, cuda_stream, nullptr);
+}
 extern "C" DivansResult divans_b200_encode_auto_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_in, const uint64_t *d_in_off,
                                                              const uint64_t *d_in_len, uint64_t max_in_len, uint8_t *d_out,
                                                              const uint64_t *d_out_off, const uint64_t *d_out_cap, uint64_t *d_out_len,
                                                              int32_t *d_status, const divans_b200_encode_options *opts,
                                                              const divans_b200_literal_model *cands, uint32_t n_cands, uint32_t *d_chosen,
                                                              uint64_t *d_cost, void *cuda_stream) {
-    if (!ctx || !opts) return DIVANS_FAILURE;
-    if (!check_cands(ctx, cands, n_cands)) return DIVANS_FAILURE;
-    if (n == 0) return DIVANS_SUCCESS;
-    if (!d_chosen) { ctx->err = "encode_auto: d_chosen is required"; return DIVANS_FAILURE; }
-    if ((uint64_t)n * n_cands > 0xffffffffull || max_in_len > 0x7fff0000ull) { ctx->err = "batch too large"; return DIVANS_FAILURE; }
-    try {
-        std::lock_guard<std::mutex> lk(ctx->mu);
-        CK(cudaSetDevice(ctx->device));
-        cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream;
-        const int window = clamp_window(opts->window_size);
-        return encode_auto_device_nolock(ctx, n, 1, d_in, d_in_off, d_in_len, max_in_len, raw_cmd_cap(max_in_len, window),
-                                         (uint32_t)(2 * max_in_len + 16), (max_in_len + 31) & ~15ull, d_out, d_out_off, d_out_cap, d_out_len,
-                                         d_status, opts, window, cands, n_cands, d_chosen, d_cost, st);
-    } catch (...) { ctx->err = "divans_b200: out of host memory"; return DIVANS_FAILURE; }
+    const AutoSel sel = {cands, n_cands, d_chosen, d_cost};
+    return encode_device_common(ctx, n, 1, d_in, d_in_off, d_in_len, max_in_len, max_in_len, d_out, d_out_off, d_out_cap, d_out_len,
+                                d_status, opts, cuda_stream, &sel);
+}
+extern "C" DivansResult divans_b200_encode_cmds_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_blobs, const uint64_t *d_blob_off,
+                                                             const uint64_t *d_blob_len, uint64_t max_blob_len, uint64_t max_raw_len,
+                                                             uint8_t *d_out, const uint64_t *d_out_off, const uint64_t *d_out_cap,
+                                                             uint64_t *d_out_len, int32_t *d_status, const divans_b200_encode_options *opts,
+                                                             void *cuda_stream) {
+    return encode_device_common(ctx, n, 0, d_blobs, d_blob_off, d_blob_len, max_blob_len, max_raw_len, d_out, d_out_off, d_out_cap,
+                                d_out_len, d_status, opts, cuda_stream, nullptr);
+}
+extern "C" DivansResult divans_b200_encode_cmds_auto_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_blobs,
+                                                                  const uint64_t *d_blob_off, const uint64_t *d_blob_len,
+                                                                  uint64_t max_blob_len, uint64_t max_raw_len, uint8_t *d_out,
+                                                                  const uint64_t *d_out_off, const uint64_t *d_out_cap, uint64_t *d_out_len,
+                                                                  int32_t *d_status, const divans_b200_encode_options *opts,
+                                                                  const divans_b200_literal_model *cands, uint32_t n_cands,
+                                                                  uint32_t *d_chosen, uint64_t *d_cost, void *cuda_stream) {
+    const AutoSel sel = {cands, n_cands, d_chosen, d_cost};
+    return encode_device_common(ctx, n, 0, d_blobs, d_blob_off, d_blob_len, max_blob_len, max_raw_len, d_out, d_out_off, d_out_cap,
+                                d_out_len, d_status, opts, cuda_stream, &sel);
 }
 
-// host batch: marshal, split into sub-batches whose symbol logs fit in HBM, run, copy back
+// The four host encode calls: marshal, split into sub-batches whose symbol logs fit in HBM, run, copy back.  Host marshalling
+// uses std::vector sized by the caller's arguments, and no C++ exception may cross the C boundary.
 static DivansResult encode_host_common(divans_b200_ctx *ctx, size_t n, int raw_mode, const uint8_t *in, const uint64_t *in_off,
                                        const uint64_t *in_len, uint8_t *out, const uint64_t *out_off, const uint64_t *out_cap,
                                        uint64_t *out_len, int32_t *status, const divans_b200_encode_options *opts,
-                                       const AutoSel *sel = nullptr) {
+                                       const AutoSel *sel) try {
     if (!ctx || !opts) return DIVANS_FAILURE;
     if (sel && !check_cands(ctx, sel->cands, sel->n_cands, !raw_mode)) return DIVANS_FAILURE;
     if (n == 0) return DIVANS_SUCCESS;
@@ -864,7 +854,8 @@ static DivansResult encode_host_common(divans_b200_ctx *ctx, size_t n, int raw_m
     CK(cudaSetDevice(ctx->device));
     const int window = clamp_window(opts->window_size);
     // per-stream requirements
-    std::vector<uint64_t> s_off(n), need_cmd(n), need_lit(n), need_replay(n);
+    std::vector<uint64_t> s_off(n);
+    std::vector<LogCaps> need(n);
     std::vector<uint8_t> staged;   // command lists are re-based to 4-byte aligned offsets
     uint64_t in_end = 0;
     for (size_t i = 0; i < n; i++) {
@@ -872,27 +863,13 @@ static DivansResult encode_host_common(divans_b200_ctx *ctx, size_t n, int raw_m
         if (raw_mode) {
             if (in_len[i] > 0x7fff0000ull) { ctx->err = "stream too large"; return DIVANS_FAILURE; }
             s_off[i] = in_off[i];
-            need_cmd[i] = raw_cmd_cap(in_len[i], window); need_lit[i] = 2 * in_len[i] + 16; need_replay[i] = (in_len[i] + 31) & ~15ull;
+            need[i] = raw_log_caps(in_len[i], window);
             if (in_off[i] + in_len[i] > in_end) in_end = in_off[i] + in_len[i];
         } else {
-            const uint8_t *b = in + in_off[i];
-            uint32_t h[8] = {0};
-            if (in_len[i] >= 32) memcpy(h, b, 32);
-            uint64_t need = 32ull + 20ull * h[2] + (uint64_t)PM_RECORD_BYTES * h[3] + h[4];
-            uint64_t lit = 0, rep = 0;
-            if (in_len[i] >= 32 && h[0] == 0x4c435644u && h[1] == 1 && need <= in_len[i]) {
-                for (uint32_t c = 0; c < h[2]; c++) {
-                    uint32_t r[5]; memcpy(r, b + 32 + 20ull * c, 20);
-                    if (r[0] == 1) rep += r[2];
-                    else if (r[0] == 2) rep += 64;            // dictionary word + transform prefix/suffix
-                    else if (r[0] == 3) { lit += r[2]; rep += r[2]; }
-                }
-            }
-            if (lit > 0x7fff0000ull || rep > 0xfffffff0ull) { ctx->err = "stream too large"; return DIVANS_FAILURE; }
-            need_cmd[i] = 32ull * h[2] + 62000ull * h[3] + 64; need_lit[i] = 2 * lit + 16; need_replay[i] = (rep + 31) & ~15ull;
+            if (!list_log_caps(in + in_off[i], in_len[i], need[i])) { ctx->err = "stream too large"; return DIVANS_FAILURE; }
             s_off[i] = (staged.size() + 3) & ~(size_t)3;
             staged.resize(s_off[i] + in_len[i]);
-            if (in_len[i]) memcpy(staged.data() + s_off[i], b, in_len[i]);
+            if (in_len[i]) memcpy(staged.data() + s_off[i], in + in_off[i], in_len[i]);
             in_end = staged.size();
         }
     }
@@ -902,33 +879,34 @@ static DivansResult encode_host_common(divans_b200_ctx *ctx, size_t n, int raw_m
     size_t free_b = 0, total_b = 0;
     cudaMemGetInfo(&free_b, &total_b);
     const uint64_t budget = (uint64_t)(free_b + ctx->sf_cap * 4) * 6 / 10;
-    if (!grow(ctx, &ctx->d_in, &ctx->d_in_cap, (size_t)in_end + 64)) return DIVANS_FAILURE;
+    HostBufs &b = ctx->host;
+    if (!grow(ctx, &b.d_in, &b.d_in_cap, (size_t)in_end + 64)) return DIVANS_FAILURE;
     cudaStream_t st = ctx->stream;
-    CK(cudaMemcpyAsync(ctx->d_in, src, in_end, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(b.d_in, src, in_end, cudaMemcpyHostToDevice, st));
     size_t i0 = 0;
     while (i0 < n) {
         // grow the sub-batch while its uniform-capacity logs fit
-        uint64_t mc = 0, ml = 0, mr = 0, mx = 0; size_t i1 = i0;
+        LogCaps mc = {0, 0, 0};
+        uint64_t mx = 0; size_t i1 = i0;
         while (i1 < n) {
-            uint64_t c = need_cmd[i1] > mc ? need_cmd[i1] : mc, l = need_lit[i1] > ml ? need_lit[i1] : ml;
+            const LogCaps c = {std::max(need[i1].cmd, mc.cmd), std::max(need[i1].lit, mc.lit), std::max(need[i1].replay, mc.replay)};
             // encode_auto: the cost pass also holds a replay window per slot for up to m * C pairs
-            const uint64_t r = need_replay[i1] > mr ? need_replay[i1] : mr;
-            const uint64_t rep = sel ? (uint64_t)encode_slots(ctx, (i1 - i0 + 1) * (size_t)sel->n_cands) * r : 0;
-            if (i1 > i0 && (c + l) * 4 * (uint64_t)(i1 - i0 + 1) + rep > budget) break;
-            mc = c; ml = l; mr = r;
+            const uint64_t rep = sel ? (uint64_t)encode_slots(ctx, (i1 - i0 + 1) * (size_t)sel->n_cands) * c.replay : 0;
+            if (i1 > i0 && (c.cmd + c.lit) * 4 * (uint64_t)(i1 - i0 + 1) + rep > budget) break;
+            mc = c;
             if (in_len[i1] > mx) mx = in_len[i1];
             i1++;
         }
-        if (mc + ml > 0xffffffffull) { ctx->err = "stream too large"; return DIVANS_FAILURE; }   // (the kernels' 32-bit log stride)
+        if (mc.cmd + mc.lit > 0xffffffffull) { ctx->err = "stream too large"; return DIVANS_FAILURE; }   // (the kernels' 32-bit log stride)
         const size_t m = i1 - i0;
-        uint64_t out_lo = ~0ull, out_hi = 0;
-        for (size_t i = i0; i < i1; i++) { if (out_off[i] < out_lo) out_lo = out_off[i]; if (out_off[i] + out_cap[i] > out_hi) out_hi = out_off[i] + out_cap[i]; }
-        if (!grow(ctx, &ctx->d_out, &ctx->d_out_cap, (size_t)(out_hi - out_lo) + 64)) return DIVANS_FAILURE;
+        uint64_t out_lo, out_hi;
+        regions_span(m, out_off + i0, out_cap + i0, out_lo, out_hi);
+        if (!grow(ctx, &b.d_out, &b.d_out_cap, (size_t)(out_hi - out_lo) + 64)) return DIVANS_FAILURE;
         // in_off | in_len | out_off | out_cap | out_len | status (+ encode_auto: chosen | cost [m * C])
-        if (!grow(ctx, &ctx->d_meta, &ctx->d_meta_cap, m * 6 + (sel ? m + m * (size_t)sel->n_cands : 0))) return DIVANS_FAILURE;
+        if (!grow(ctx, &b.d_meta, &b.d_meta_cap, m * 6 + (sel ? m + m * (size_t)sel->n_cands : 0))) return DIVANS_FAILURE;
         std::vector<uint64_t> rel(m);
         for (size_t i = 0; i < m; i++) rel[i] = out_off[i0 + i] - out_lo;
-        uint64_t *mm = ctx->d_meta;
+        uint64_t *mm = b.d_meta;
         CK(cudaMemcpyAsync(mm, s_off.data() + i0, m * 8, cudaMemcpyHostToDevice, st));
         CK(cudaMemcpyAsync(mm + m, in_len + i0, m * 8, cudaMemcpyHostToDevice, st));
         CK(cudaMemcpyAsync(mm + 2 * m, rel.data(), m * 8, cudaMemcpyHostToDevice, st));
@@ -936,11 +914,10 @@ static DivansResult encode_host_common(divans_b200_ctx *ctx, size_t n, int raw_m
         int32_t *d_status = reinterpret_cast<int32_t *>(mm + 5 * m);
         uint32_t *d_chosen = reinterpret_cast<uint32_t *>(mm + 6 * m);
         uint64_t *d_cost = mm + 7 * m;
-        DivansResult r = sel ? encode_auto_device_nolock(ctx, m, raw_mode, ctx->d_in, mm, mm + m, mx, (uint32_t)mc, (uint32_t)ml, mr, ctx->d_out,
-                                                         mm + 2 * m, mm + 3 * m, mm + 4 * m, d_status, opts, window, sel->cands,
-                                                         sel->n_cands, d_chosen, d_cost, st)
-                             : encode_device_internal(ctx, m, raw_mode, ctx->d_in, mm, mm + m, mx, (uint32_t)mc, (uint32_t)ml, mr, ctx->d_out,
-                                                      mm + 2 * m, mm + 3 * m, mm + 4 * m, d_status, opts, window, st);
+        DivansResult r = sel ? encode_auto_device_nolock(ctx, m, raw_mode, b.d_in, mm, mm + m, mx, mc, b.d_out, mm + 2 * m, mm + 3 * m,
+                                                         mm + 4 * m, d_status, opts, window, sel->cands, sel->n_cands, d_chosen, d_cost, st)
+                             : encode_device_internal(ctx, m, raw_mode, b.d_in, mm, mm + m, mx, mc, b.d_out, mm + 2 * m, mm + 3 * m,
+                                                      mm + 4 * m, d_status, opts, window, st);
         if (r != DIVANS_SUCCESS) return r;
         if (sel) {
             CK(cudaMemcpyAsync(sel->chosen + i0, d_chosen, m * 4, cudaMemcpyDeviceToHost, st));
@@ -950,20 +927,21 @@ static DivansResult encode_host_common(divans_b200_ctx *ctx, size_t n, int raw_m
         CK(cudaMemcpyAsync(status + i0, d_status, m * 4, cudaMemcpyDeviceToHost, st));
         CK(cudaStreamSynchronize(st));
         for (size_t i = i0; i < i1; i++) {
-            if (status[i] == DIVANS_SUCCESS && out_len[i]) CK(cudaMemcpyAsync(out + out_off[i], ctx->d_out + (out_off[i] - out_lo), out_len[i], cudaMemcpyDeviceToHost, st));
+            if (status[i] == DIVANS_SUCCESS && out_len[i]) CK(cudaMemcpyAsync(out + out_off[i], b.d_out + (out_off[i] - out_lo), out_len[i], cudaMemcpyDeviceToHost, st));
         }
         CK(cudaStreamSynchronize(st));
         i0 = i1;
     }
     return DIVANS_SUCCESS;
+} catch (...) {
+    if (ctx) ctx->err = "divans_b200: out of host memory while marshalling the batch";
+    return DIVANS_FAILURE;
 }
 extern "C" DivansResult divans_b200_encode_batch_host(divans_b200_ctx *ctx, size_t n, const uint8_t *in, const uint64_t *in_off,
                                                       const uint64_t *in_len, uint8_t *out, const uint64_t *out_off,
                                                       const uint64_t *out_cap, uint64_t *out_len, int32_t *status,
                                                       const divans_b200_encode_options *opts) {
-    // (host marshalling uses std::vector sized by the caller's arguments: no C++ exception may cross the C boundary)
-    try { return encode_host_common(ctx, n, 1, in, in_off, in_len, out, out_off, out_cap, out_len, status, opts); }
-    catch (...) { if (ctx) ctx->err = "divans_b200: out of host memory while marshalling the batch"; return DIVANS_FAILURE; }
+    return encode_host_common(ctx, n, 1, in, in_off, in_len, out, out_off, out_cap, out_len, status, opts, nullptr);
 }
 extern "C" DivansResult divans_b200_encode_auto_batch_host(divans_b200_ctx *ctx, size_t n, const uint8_t *in, const uint64_t *in_off,
                                                            const uint64_t *in_len, uint8_t *out, const uint64_t *out_off, const uint64_t *out_cap,
@@ -971,15 +949,13 @@ extern "C" DivansResult divans_b200_encode_auto_batch_host(divans_b200_ctx *ctx,
                                                            const divans_b200_literal_model *cands, uint32_t n_cands, uint32_t *chosen,
                                                            uint64_t *cost) {
     const AutoSel sel = {cands, n_cands, chosen, cost};
-    try { return encode_host_common(ctx, n, 1, in, in_off, in_len, out, out_off, out_cap, out_len, status, opts, &sel); }
-    catch (...) { if (ctx) ctx->err = "divans_b200: out of host memory while marshalling the batch"; return DIVANS_FAILURE; }
+    return encode_host_common(ctx, n, 1, in, in_off, in_len, out, out_off, out_cap, out_len, status, opts, &sel);
 }
 extern "C" DivansResult divans_b200_encode_cmds_batch_host(divans_b200_ctx *ctx, size_t n, const uint8_t *blobs, const uint64_t *blob_off,
                                                            const uint64_t *blob_len, uint8_t *out, const uint64_t *out_off,
                                                            const uint64_t *out_cap, uint64_t *out_len, int32_t *status,
                                                            const divans_b200_encode_options *opts) {
-    try { return encode_host_common(ctx, n, 0, blobs, blob_off, blob_len, out, out_off, out_cap, out_len, status, opts); }
-    catch (...) { if (ctx) ctx->err = "divans_b200: out of host memory while marshalling the batch"; return DIVANS_FAILURE; }
+    return encode_host_common(ctx, n, 0, blobs, blob_off, blob_len, out, out_off, out_cap, out_len, status, opts, nullptr);
 }
 extern "C" DivansResult divans_b200_encode_cmds_auto_batch_host(divans_b200_ctx *ctx, size_t n, const uint8_t *blobs, const uint64_t *blob_off,
                                                                 const uint64_t *blob_len, uint8_t *out, const uint64_t *out_off,
@@ -987,8 +963,7 @@ extern "C" DivansResult divans_b200_encode_cmds_auto_batch_host(divans_b200_ctx 
                                                                 const divans_b200_encode_options *opts, const divans_b200_literal_model *cands,
                                                                 uint32_t n_cands, uint32_t *chosen, uint64_t *cost) {
     const AutoSel sel = {cands, n_cands, chosen, cost};
-    try { return encode_host_common(ctx, n, 0, blobs, blob_off, blob_len, out, out_off, out_cap, out_len, status, opts, &sel); }
-    catch (...) { if (ctx) ctx->err = "divans_b200: out of host memory while marshalling the batch"; return DIVANS_FAILURE; }
+    return encode_host_common(ctx, n, 0, blobs, blob_off, blob_len, out, out_off, out_cap, out_len, status, opts, &sel);
 }
 
 // =================================================================================================================
