@@ -45,6 +45,7 @@ BATCH_SYMBOLS = [
     "divans_b200_debug_slot_header", "divans_b200_decode_cmds_batch_host", "divans_b200_decode_cmds_batch_device",
     "divans_b200_encode_cmds_batch_device", "divans_b200_encode_auto_batch_host", "divans_b200_encode_auto_batch_device",
     "divans_b200_encode_cmds_auto_batch_host", "divans_b200_encode_cmds_auto_batch_device",
+    "divans_b200_replay_cmds_batch_host", "divans_b200_replay_cmds_batch_device",
 ]
 PM_RECORD_BYTES = 32 + 16384 + 1024 + 8192   # one prediction-mode record of a DVCL blob (include/divans_b200.h)
 
@@ -147,6 +148,10 @@ def load_library():
     L.divans_b200_encode_cmds_auto_batch_device.argtypes = [vp, sz, vp, vp, vp, ctypes.c_uint64, ctypes.c_uint64, vp, vp, vp, vp, vp,
                                                             ctypes.POINTER(EncodeOptions), vp, ctypes.c_uint32, vp, vp, vp]
     L.divans_b200_encode_cmds_auto_batch_device.restype = ctypes.c_uint8
+    L.divans_b200_replay_cmds_batch_host.argtypes = batch + [ctypes.c_int32]
+    L.divans_b200_replay_cmds_batch_host.restype = ctypes.c_uint8
+    L.divans_b200_replay_cmds_batch_device.argtypes = batch + [ctypes.c_int32, vp]
+    L.divans_b200_replay_cmds_batch_device.restype = ctypes.c_uint8
     L.divans_b200_ir_to_cmds.argtypes = [ctypes.c_char_p, sz, vp, sz, szp, ctypes.POINTER(ctypes.c_int32)]
     L.divans_b200_ir_to_cmds.restype = ctypes.c_uint8
     L.divans_b200_lz77_cmds_batch.argtypes = [sz, vp, vp, vp, ctypes.c_int32, ctypes.c_int32, ctypes.c_int32, vp, sz, vp, vp, szp, ctypes.c_int32]
@@ -672,6 +677,53 @@ class Engine:
         caller.wait_stream(s)
         d_new.record_stream(caller)   # (allocated on the private stream, used on the caller's from here on)
         return (d_new, new_off, new_len, status, chosen, cost) if auto else (d_new, new_off, new_len, status)
+
+    # -- replaying command lists to raw bytes (include/divans_b200.h, divans_b200_replay_cmds_batch_*)
+    def replay_cmds_batch_host(self, blobs, blob_off, blob_len, out, out_off, out_cap, window_size=0):
+        """Realise the DVCL command lists blobs[blob_off[i] .. +blob_len[i]) as raw bytes in out[out_off[i] .. +out_cap[i]):
+        returns (out_len, status).  ``window_size`` 0 takes each list's header window; status 2: out_len is the exact length
+        and the region holds its first out_cap bytes (out_cap 0 measures lengths only); status 3: the list is refused."""
+        n = len(blob_off)
+        blob_off, blob_len, out_off, out_cap, out_len, status = _host_batch(blob_off, blob_len, out_off, out_cap)
+        rc = self._L.divans_b200_replay_cmds_batch_host(self._h, n, _ptr(blobs), _ptr(blob_off), _ptr(blob_len), _ptr(out), _ptr(out_off),
+                                                        _ptr(out_cap), _ptr(out_len), _ptr(status), int(window_size))
+        if rc != DIVANS_SUCCESS:
+            raise DivansError("replay_cmds_batch_host: " + self._err())
+        return out_len, status
+
+    def replay_cmds_batch_device(self, n, d_blobs, d_blob_off, d_blob_len, d_out, d_out_off, d_out_cap, d_out_len, d_status, window_size=0,
+                                 stream=None):
+        """replay_cmds_batch_host with raw device pointers (ints); blobs 4-byte aligned.  Asynchronous on ``stream``; regions
+        are not cleared first."""
+        rc = self._L.divans_b200_replay_cmds_batch_device(self._h, n, d_blobs, d_blob_off, d_blob_len, d_out, d_out_off, d_out_cap,
+                                                          d_out_len, d_status, int(window_size), stream)
+        if rc != DIVANS_SUCCESS:
+            raise DivansError("replay_cmds_batch_device: " + self._err())
+
+    def replay(self, blobs, window_size=0, max_bytes=1 << 32):
+        """Convenience: list of DVCL command-list blobs -> list of (status, raw bytes).  A length pass (out_cap 0), then one
+        exact pass over the lists it measured; a refused list gives (3, b"").  The exact pass holds the whole output in host
+        memory and in HBM, and a short list can describe gigabytes (one copy record: up to 4 GiB), so when the measured lengths
+        add up to more than ``max_bytes`` the call raises DivansError instead of allocating them; pass a larger bound knowingly,
+        or replay such lists with replay_cmds_batch_host / _device into regions of your own."""
+        n = len(blobs)
+        if n == 0:
+            return []
+        blob, off, ln = _pack(blobs)
+        out_len, status = self.replay_cmds_batch_host(blob, off, ln, np.zeros(1, np.uint8), np.zeros(n, np.uint64), np.zeros(n, np.uint64),
+                                                      window_size)
+        res = [(DIVANS_FAILURE, b"")] * n
+        idx = np.nonzero(status != DIVANS_FAILURE)[0]
+        if idx.size:
+            cap = out_len[idx]
+            if sum(int(c) for c in cap) > max_bytes:
+                raise DivansError("replay: the lists measure %d bytes in all, more than max_bytes = %d" % (sum(int(c) for c in cap), max_bytes))
+            out_off, total = _regions(cap)
+            out = np.zeros(max(total, 1), np.uint8)
+            ln2, st2 = self.replay_cmds_batch_host(blob, off[idx], ln[idx], out, out_off, cap, window_size)
+            for k, i in enumerate(idx):
+                res[i] = (int(st2[k]), out[int(out_off[k]):int(out_off[k]) + int(ln2[k])].tobytes())
+        return res
 
     def encode(self, raws, opts=None, cmds=False):
         """Convenience: list of raw byte strings (or DVCL command-list blobs with cmds=True) -> list of .divans bytes."""

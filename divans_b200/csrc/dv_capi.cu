@@ -575,6 +575,16 @@ static bool list_log_caps(const uint8_t *b, uint64_t len, LogCaps &caps) {
     return true;
 }
 
+// Command-list records are read as u32, so the host calls (encode_host_common, divans_b200_replay_cmds_batch_host) re-base
+// blobs that a caller may place at any offset: src[0 .. len) is appended to `staged` at its next 4-byte aligned offset, which is
+// returned.
+static uint64_t stage_aligned(std::vector<uint8_t> &staged, const uint8_t *src, uint64_t len) {
+    const uint64_t o = (staged.size() + 3) & ~(uint64_t)3;
+    staged.resize(o + len);
+    if (len) memcpy(staged.data() + o, src, len);
+    return o;
+}
+
 // The EncodeParams fields the model pass and the cost pass share: the n streams at d_in[d_in_off[v] .. +d_in_len[v]), the
 // context's arena, tables and replay windows, the log capacities `caps` (sized for streams of up to max_in_len bytes), the
 // window (10..24, or 0 for each command list's own) and the options.  Every other field is zero.
@@ -867,9 +877,7 @@ static DivansResult encode_host_common(divans_b200_ctx *ctx, size_t n, int raw_m
             if (in_off[i] + in_len[i] > in_end) in_end = in_off[i] + in_len[i];
         } else {
             if (!list_log_caps(in + in_off[i], in_len[i], need[i])) { ctx->err = "stream too large"; return DIVANS_FAILURE; }
-            s_off[i] = (staged.size() + 3) & ~(size_t)3;
-            staged.resize(s_off[i] + in_len[i]);
-            if (in_len[i]) memcpy(staged.data() + s_off[i], in + in_off[i], in_len[i]);
+            s_off[i] = stage_aligned(staged, in + in_off[i], in_len[i]);
             in_end = staged.size();
         }
     }
@@ -964,6 +972,79 @@ extern "C" DivansResult divans_b200_encode_cmds_auto_batch_host(divans_b200_ctx 
                                                                 uint32_t n_cands, uint32_t *chosen, uint64_t *cost) {
     const AutoSel sel = {cands, n_cands, chosen, cost};
     return encode_host_common(ctx, n, 0, blobs, blob_off, blob_len, out, out_off, out_cap, out_len, status, opts, &sel);
+}
+
+// ---- replaying command lists to raw bytes ----
+// One launch (dv_replay.cu) over n lists in HBM.  It uses the context's work counter, tables and timing events only: no slot,
+// arena or encoder log, so it runs on a context that has never decoded or encoded.
+static DivansResult replay_device_nolock(divans_b200_ctx *ctx, size_t n, const uint8_t *d_blobs, const uint64_t *d_blob_off,
+                                         const uint64_t *d_blob_len, uint8_t *d_out, const uint64_t *d_out_off, const uint64_t *d_out_cap,
+                                         uint64_t *d_out_len, int32_t *d_status, int32_t window_size, cudaStream_t st) {
+    if (n > 0xffffffffull) { ctx->err = "too many command lists"; return DIVANS_FAILURE; }
+    if (ctx->busy_recorded) CK(cudaStreamWaitEvent(st, ctx->ev_busy, 0));
+    ReplayParams rp;
+    rp.blobs = d_blobs; rp.blob_off = d_blob_off; rp.blob_len = d_blob_len;
+    rp.out = d_out; rp.out_off = d_out_off; rp.out_cap = d_out_cap; rp.out_len = d_out_len; rp.status = d_status;
+    rp.n_lists = (uint32_t)n; rp.window = window_size == 0 ? 0 : clamp_window(window_size);   // the encoder's window rule
+    rp.work_counter = ctx->d_counter; rp.tables = ctx->d_tables;
+    CK(cudaMemsetAsync(ctx->d_counter, 0, 4, st));
+    CK(cudaEventRecord(ctx->ev0, st));
+    CK(cudaEventRecord(ctx->evm, st));
+    launch_replay_cmds(rp, ctx->sm_count, st);
+    CK(cudaEventRecord(ctx->ev1, st));
+    CK(cudaEventRecord(ctx->ev_busy, st)); ctx->busy_recorded = true;
+    ctx->main_end_is_evm1 = false;
+    ctx->launches += 1;
+    CK(cudaGetLastError());
+    return DIVANS_SUCCESS;
+}
+extern "C" DivansResult divans_b200_replay_cmds_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_blobs, const uint64_t *d_blob_off,
+                                                             const uint64_t *d_blob_len, uint8_t *d_out, const uint64_t *d_out_off,
+                                                             const uint64_t *d_out_cap, uint64_t *d_out_len, int32_t *d_status,
+                                                             int32_t window_size, void *cuda_stream) {
+    if (!ctx) return DIVANS_FAILURE;
+    if (n == 0) return DIVANS_SUCCESS;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    CK(cudaSetDevice(ctx->device));
+    return replay_device_nolock(ctx, n, d_blobs, d_blob_off, d_blob_len, d_out, d_out_off, d_out_cap, d_out_len, d_status, window_size,
+                                cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream);
+}
+// Staged like a host decode (stage_decode, copy_regions_back); the records are read as u32, so blobs at offsets that are not
+// 4-byte aligned are first re-based on the host, as divans_b200_encode_cmds_batch_host does.
+extern "C" DivansResult divans_b200_replay_cmds_batch_host(divans_b200_ctx *ctx, size_t n, const uint8_t *blobs, const uint64_t *blob_off,
+                                                           const uint64_t *blob_len, uint8_t *out, const uint64_t *out_off,
+                                                           const uint64_t *out_cap, uint64_t *out_len, int32_t *status,
+                                                           int32_t window_size) try {
+    if (!ctx) return DIVANS_FAILURE;
+    if (n == 0) return DIVANS_SUCCESS;
+    const uint8_t *src = blobs;
+    const uint64_t *src_off = blob_off;
+    std::vector<uint64_t> s_off;
+    std::vector<uint8_t> staged;
+    if (std::any_of(blob_off, blob_off + n, [](uint64_t o) { return (o & 3u) != 0; })) {
+        s_off.resize(n);
+        for (size_t i = 0; i < n; i++) s_off[i] = stage_aligned(staged, blobs + blob_off[i], blob_len[i]);
+        src = staged.data(); src_off = s_off.data();
+    }
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    CK(cudaSetDevice(ctx->device));
+    HostBufs &b = ctx->host;
+    cudaStream_t st = ctx->stream;
+    uint64_t in_total;
+    if (stage_decode(ctx, b, n, src, src_off, blob_len, out_off, out_cap, nullptr, st, nullptr, st, in_total) != DIVANS_SUCCESS)
+        return DIVANS_FAILURE;
+    uint64_t *m = b.d_meta;
+    int32_t *d_status = reinterpret_cast<int32_t *>(m + 5 * n);
+    DivansResult r = replay_device_nolock(ctx, n, b.d_in, m, m + n, b.d_out, m + 2 * n, m + 3 * n, m + 4 * n, d_status, window_size, st);
+    if (r != DIVANS_SUCCESS) return r;
+    CK(cudaMemcpyAsync(out_len, m + 4 * n, n * 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(status, d_status, n * 4, cudaMemcpyDeviceToHost, st));
+    if (copy_regions_back(ctx, n, out, b.d_out, out_off, out_cap, st) != DIVANS_SUCCESS) return DIVANS_FAILURE;
+    CK(cudaStreamSynchronize(st));
+    return DIVANS_SUCCESS;
+} catch (...) {
+    if (ctx) ctx->err = "divans_b200: out of host memory while staging the command lists";
+    return DIVANS_FAILURE;
 }
 
 // =================================================================================================================

@@ -38,4 +38,14 @@ void launch_auto_select(const uint64_t *tally, const int32_t *v_status, uint64_t
 void launch_decode_v2_rec(const DecodeParams &p, const RecParams &r, uint32_t n_blocks, cudaStream_t st);
 void launch_decode16_blend_rec(const DecodeParams &p, const RecParams &r, uint32_t n_blocks, cudaStream_t st);
 void launch_pack_cmds(const DecodeParams &p, const RecParams &r, cudaStream_t st);
+
+// replaying command lists to raw bytes (dv_replay.cu): list i is blobs[blob_off[i] .. +blob_len[i]), its bytes go to
+// out[out_off[i] .. +out_cap[i]); window 10..24 for every list, or 0 for each list's header window (clamped to 10..24)
+struct ReplayParams {
+    const uint8_t *blobs; const uint64_t *blob_off, *blob_len;
+    uint8_t *out; const uint64_t *out_off, *out_cap; uint64_t *out_len; int32_t *status;
+    uint32_t n_lists; int32_t window;
+    uint32_t *work_counter; const uint8_t *tables;
+};
+void launch_replay_cmds(const ReplayParams &p, int sm_count, cudaStream_t st);   // one launch, persistent warps
 }  // namespace dv

@@ -344,6 +344,41 @@ DivansResult divans_b200_encode_cmds_auto_batch_device(divans_b200_ctx *ctx, siz
                                                        uint64_t *d_out_len, int32_t *d_status, const divans_b200_encode_options *opts,
                                                        const divans_b200_literal_model *cands, uint32_t n_cands, uint32_t *d_chosen,
                                                        uint64_t *d_cost, void *cuda_stream);
+
+/* ---- replaying command lists to raw bytes ----
+ * Realise n command lists (DVCL blobs, below) as the bytes they describe: the reference's `recode` (src/bin/divans.rs:1108,
+ * cmd_to_raw/mod.rs) on the GPU.  List i is blobs[blob_off[i] .. +blob_len[i]); its bytes go to out[out_off[i] .. +out_cap[i]).
+ *  - Window: the ring is 1 << w.  window_size == 0: w is the blob header's window (word 5) clamped to 10..24; any other value is
+ *    clamped to 10..24 and applies to every list.  This is the opts->window_size rule of divans_b200_encode_cmds_batch_device,
+ *    so a list the encoder codes with window w replays with the same w.
+ *  - Commands: literal (type 3) appends pool bytes [a, a + b); copy (1) appends b bytes at distance a, bytes before output
+ *    position 0 reading as 0 (a fresh ring); dictionary (2) appends word a of size b under transform c, whose length must equal
+ *    d when d != 0; block switches and PredictionMode commands (4..7) append nothing.
+ *  - status 0: out_len[i] bytes were written at out + out_off[i].
+ *  - status 2: the output needs more than out_cap[i] bytes.  out_len[i] is its exact length and the region holds its first
+ *    out_cap[i] bytes: the walk goes on to the end of the list without moving bytes, applying every check below.  out_cap = 0
+ *    measures lengths only (a length pass).
+ *  - status 3 (refused): the blob is not 4-byte aligned (device call) or shorter than 32 bytes; the header's magic or version is
+ *    wrong, or 32 + 20 * n_cmds + PM_RECORD_BYTES * n_predmodes + n_literal_bytes > blob_len (64-bit); a record's type is outside
+ *    1..7; a literal has a + b > n_literal_bytes (64-bit); a copy has a == 0 or a >= 1 << w; a dictionary word or transform
+ *    does not exist, or d != 0 differs from the transformed length.  Status 3 takes precedence over status 2.  out_len[i] counts
+ *    the bytes of the commands before the refused one (0 for a refusal at blob or header level), and nothing past them is
+ *    written.
+ *  - No list reads outside its blob or writes outside its region.  Output positions and lengths are 64-bit.
+ *  - One kernel launch per call; no arena slot or encoder log is used, so it works on a fresh context.
+ * Host call: every region is written whole, with zeros past out_len[i]; nothing outside the regions is touched; input regions
+ * may alias; blob offsets need no alignment (as for divans_b200_encode_cmds_batch_host).  n == 0 returns DIVANS_SUCCESS. */
+DivansResult divans_b200_replay_cmds_batch_host(divans_b200_ctx *ctx, size_t n, const uint8_t *blobs, const uint64_t *blob_off,
+                                                const uint64_t *blob_len, uint8_t *out, const uint64_t *out_off,
+                                                const uint64_t *out_cap, uint64_t *out_len, int32_t *status, int32_t window_size);
+/* Same, all pointers DEVICE pointers.  Asynchronous on `cuda_stream` (NULL = the context's own stream) and serialised on the
+ * context like every device call; divans_b200_last_kernel_ms is valid after it.  Regions are not cleared first.  With out_cap = 0
+ * it sizes `max_raw_len` of divans_b200_encode_cmds_batch_device / _cmds_auto_batch_device for lists held in HBM: the largest
+ * out_len of a length pass is the decoded length of every list. */
+DivansResult divans_b200_replay_cmds_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_blobs, const uint64_t *d_blob_off,
+                                                  const uint64_t *d_blob_len, uint8_t *d_out, const uint64_t *d_out_off,
+                                                  const uint64_t *d_out_cap, uint64_t *d_out_len, int32_t *d_status,
+                                                  int32_t window_size, void *cuda_stream);
 /* IR text front-end (reference: src/bin/divans.rs:191-483, the textual IR that `divans -i` consumes): parse `ir_text` into a
  * DVCL blob.  *blob_len receives the size of the blob; with out == NULL or out_cap too small the call returns
  * DIVANS_NEEDS_MORE_OUTPUT.  *window_size (optional) receives the `window` line's value (0 if absent).  Host only. */

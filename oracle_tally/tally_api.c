@@ -1,5 +1,6 @@
 /*
- * tally_api.c -- literal model selection on top of the CPU oracle.  TEST INFRASTRUCTURE, NOT PRODUCT CODE.
+ * tally_api.c -- literal model selection, and the replay of serialised command lists, on top of the CPU oracle.
+ * TEST INFRASTRUCTURE, NOT PRODUCT CODE.
  *
  * oracle_tally/tally_py.py compiles this file appended to a copy of oracle/divans_oracle.c whose ans_enc_put has one hook
  * inserted (dvt_tally, below): while dvt_tally is set, every symbol the encoder would code adds the cost of its frequency to
@@ -134,4 +135,50 @@ int dvo_encode_cmds_auto(const dvo_cmdlist *l, const dvo_options *o, const int32
     *out_len = 0;
     dvt_call call = {o, NULL, out, cap, out_len};
     return dvt_with_model(l, cands[2 * arg], cands[2 * arg + 1], dvt_encode_fn, &call);
+}
+
+/* ---- replaying a DVCL blob (include/divans_b200.h) ----
+ * The CPU reference of divans_b200_replay_cmds_batch_*: dvo_recode's semantics (the oracle's ring, rc_copy, rc_dict and
+ * dvo_dict_word) on the serialised form, with the blob's refusal rules applied where the library applies them -- the blob and
+ * header first, then each record as the walk reaches it.  window 0: the header's window; either way clamped to 10..24.
+ * Returns DVO_SUCCESS, DVO_NEEDS_MORE_OUTPUT (*out_len is still the exact length, out holds its first `cap` bytes) or
+ * DVO_FAILURE (*out_len: the bytes of the commands before the refused one, 0 for a refused blob or header).  Past `cap` the
+ * walk only counts bytes: nothing is written any more, so the ring's contents no longer matter. */
+#define DVT_PM_RECORD_BYTES (32u + 16384u + 1024u + 8192u)
+int dvo_recode_blob(const uint8_t *blob, size_t len, int window, uint8_t *out, size_t cap, size_t *out_len) {
+    uint32_t h[8];
+    *out_len = 0;
+    if (len < 32) return DVO_FAILURE;
+    memcpy(h, blob, 32);
+    const uint64_t lit_base = 32ull + 20ull * h[2] + (uint64_t)DVT_PM_RECORD_BYTES * h[3];
+    if (h[0] != 0x4c435644u || h[1] != 1u || lit_base + h[4] > len) return DVO_FAILURE;
+    const uint32_t w = window != 0 ? (uint32_t)(window < 10 ? 10 : (window > 24 ? 24 : window)) : (h[5] < 10 ? 10 : (h[5] > 24 ? 24 : h[5]));
+    recoder r; memset(&r, 0, sizeof r);
+    r.ring_len = 1u << w; r.ring = (uint8_t *)calloc(1, r.ring_len); r.out = out; r.out_cap = cap;
+    if (!r.ring) return DVO_FAILURE;
+    const uint8_t *lits = blob + lit_base;
+    int rc = DVO_SUCCESS;
+    for (uint32_t i = 0; i < h[2] && rc == DVO_SUCCESS; i++) {
+        uint32_t c[5];
+        memcpy(c, blob + 32 + 20ull * i, 20);
+        const size_t room = r.out_len < cap ? cap - r.out_len : 0;
+        if (c[0] == DVO_CMD_LITERAL) {
+            if ((uint64_t)c[1] + c[2] > h[4]) { rc = DVO_FAILURE; break; }
+            const size_t take = c[2] < room ? c[2] : room;
+            for (size_t k = 0; k < take; k++) rc_put(&r, lits[c[1] + k]);
+            if (take < c[2]) { r.out_len += c[2] - take; r.overflow = 1; }
+        } else if (c[0] == DVO_CMD_COPY) {
+            const size_t take = c[2] < room ? c[2] : room;
+            rc = rc_copy(&r, c[1], (uint32_t)take);   /* refuses a == 0 and a >= the ring before it writes anything */
+            if (rc == DVO_SUCCESS && take < c[2]) { r.out_len += c[2] - take; r.overflow = 1; }
+        } else if (c[0] == DVO_CMD_DICT) {
+            rc = rc_dict(&r, c[2], c[1], c[3], c[4]);
+        } else if (c[0] < DVO_CMD_COPY || c[0] > DVO_CMD_PREDMODE) {
+            rc = DVO_FAILURE;
+        }
+    }
+    *out_len = r.out_len;
+    if (r.overflow && rc == DVO_SUCCESS) rc = DVO_NEEDS_MORE_OUTPUT;
+    free(r.ring);
+    return rc;
 }
