@@ -30,8 +30,6 @@
 
 namespace dv {
 
-constexpr int SMEM_BYTES_PER_GROUP_V2 = (int)((sizeof(Cold) + 15) / 16 * 16);
-
 __device__ __forceinline__ const char *mk_ptr(const uint32_t lo, const uint32_t hi) {
     unsigned long long p; asm("mov.b64 %0, {%1, %2};" : "=l"(p) : "r"(lo), "r"(hi)); return reinterpret_cast<const char *>(p);
 }

@@ -189,7 +189,7 @@ extern "C" void divans_b200_destroy(divans_b200_ctx *ctx) {
     delete ctx;
 }
 // bumped whenever a decode kernel changes: bench.py quotes a stored DRAM-traffic capture (profiles/traffic.json) only for the version it measured
-#define DV_KERNEL_VERSION "r2.18-v2-mixval-loop"
+#define DV_KERNEL_VERSION "r2.19-one-decoder-body"
 extern "C" const char *divans_b200_kernel_version(void) { return DV_KERNEL_VERSION; }
 extern "C" const char *divans_b200_last_error(divans_b200_ctx *ctx) { return ctx ? ctx->err.c_str() : "null context"; }
 extern "C" int divans_b200_last_lanes(divans_b200_ctx *ctx) { return ctx ? ctx->last_lanes : 0; }
@@ -246,23 +246,17 @@ static DivansResult decode_device_nolock(divans_b200_ctx *ctx, size_t n, const u
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream;
     if (ctx->busy_recorded) CK(cudaStreamWaitEvent(st, ctx->ev_busy, 0));
     int lanes = ctx->lanes_per_stream;
-    uint32_t gpb, cap;
-    const bool blend = (flags & DIVANS_B200_FLAG_CDF_BLEND) != 0;   // BlendCDF16 streams: the blend decoder (dv_kernels.cu), 16 lanes
-    if (blend) {
-        lanes = 16; gpb = (uint32_t)(DECODE_BLOCK_THREADS / 16);
-        cap = (uint32_t)ctx->sm_count * (uint32_t)std::max(1, decode_max_blocks_per_sm16_blend()) * gpb;
-        if (cap > ctx->max_resident) cap = std::max(ctx->max_resident / gpb * gpb, gpb);   // (memory / caller limits of the context)
-    } else {
-        // 16 lanes per stream unless 8 hold the batch in fewer passes.  At equal residency 8 lanes is the slower layout (half the
-        // warps per scheduler); it only pays where registers, not slot memory, cap residency: there it keeps twice the streams in
-        // flight.  On an 80 GB H100 both layouts are capped by slot memory (cap8 ~ cap16), so 16 lanes run every batch size.
-        if (ctx->auto_lanes) {
-            const uint64_t passes16 = (n + ctx->cap16 - 1) / ctx->cap16, passes8 = (n + ctx->cap8 - 1) / ctx->cap8;
-            lanes = passes8 < passes16 ? 8 : 16;
-        }
-        if (rec) lanes = 16;   // the recording decoder has the 16-lane layout only
-        gpb = (uint32_t)decode_groups_per_block_v2(lanes); cap = lanes == 16 ? ctx->cap16 : ctx->cap8;
+    const bool blend = (flags & DIVANS_B200_FLAG_CDF_BLEND) != 0;   // BlendCDF16 streams: the decoder's blend model
+    // 16 lanes per stream unless 8 hold the batch in fewer passes.  At equal residency 8 lanes is the slower layout (half the
+    // warps per scheduler); it only pays where registers, not slot memory, cap residency: there it keeps twice the streams in
+    // flight.  On an 80 GB H100 both layouts are capped by slot memory (cap8 ~ cap16), so 16 lanes run every batch size.
+    if (ctx->auto_lanes) {
+        const uint64_t passes16 = (n + ctx->cap16 - 1) / ctx->cap16, passes8 = (n + ctx->cap8 - 1) / ctx->cap8;
+        lanes = passes8 < passes16 ? 8 : 16;
     }
+    if (rec || blend) lanes = 16;   // the recording decoder and the blend model have the 16-lane layout only
+    uint32_t gpb = (uint32_t)decode_groups_per_block_v2(lanes), cap = lanes == 16 ? ctx->cap16 : ctx->cap8;
+    if (blend) { gpb = DECODE_BLOCK_THREADS / 16; cap = std::max(cap / gpb * gpb, gpb); }   // whole blocks of the blend kernels
     ctx->last_lanes = lanes;
     uint32_t resident = (uint32_t)(n < cap ? n : cap);
     uint32_t blocks = (resident + gpb - 1) / gpb;
@@ -291,10 +285,10 @@ static DivansResult decode_device_nolock(divans_b200_ctx *ctx, size_t n, const u
     if (dbg) { CK(cudaStreamSynchronize(st)); fprintf(stderr, "divans_b200[debug]: frame kernel ok (n=%zu)\n", n); }
     CK(cudaEventRecord(ctx->evm, st));
     if (rec) {
-        if (blend) launch_decode16_blend_rec(dp, rp, blocks, st); else launch_decode_v2_rec(dp, rp, blocks, st);
+        launch_decode_v2_rec(blend, dp, rp, blocks, st);
         CK(cudaEventRecord(ctx->evm1, st));
         launch_pack_cmds(dp, rp, st);
-    } else if (!skip_decode) { if (blend) launch_decode16_blend(dp, blocks, st); else launch_decode_v2(lanes, dp, blocks, st); }
+    } else if (!skip_decode) launch_decode_v2(lanes, blend, dp, blocks, st);
     if (dbg) { CK(cudaStreamSynchronize(st)); fprintf(stderr, "divans_b200[debug]: decode kernel ok (blocks=%u, lps=%d)\n", blocks, ctx->lanes_per_stream); }
     CK(cudaEventRecord(ctx->ev1, st));
     CK(cudaEventRecord(ctx->ev_busy, st)); ctx->busy_recorded = true;

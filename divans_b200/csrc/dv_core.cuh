@@ -1,5 +1,5 @@
 // dv_core.cuh -- the encoder's converged per-nibble core and literal fast path (dv_encode.cu), and the warp CRC32C of the
-// framing and mux passes.  Included by the blend decoder (dv_kernels.cu) for the engine and the blend core.
+// framing and mux passes (dv_kernels.cu, dv_encode.cu).
 #pragma once
 #include "dv_engine_kernel.cuh"
 #include "dv_blend.cuh"
@@ -10,8 +10,6 @@ namespace dv {
 __device__ __forceinline__ uint32_t crc_step(const uint32_t *tab, uint32_t crc, uint32_t byte) {
     return tab[(crc ^ byte) & 0xff] ^ (crc >> 8);
 }
-
-constexpr int SMEM_BYTES_PER_GROUP = (int)((sizeof(Cold) + 15) / 16 * 16);
 
 // Encoder: log one coded nibble.  A frequency <= 0 (a stream-supplied speed wrapped an i16 counter) cannot be coded: the
 // reference encoder panics on it and the oracle refuses the stream (ans_enc_put), so the stream fails, as in the blend core.

@@ -162,12 +162,15 @@ struct G2 {            // lane geometry of one lane-group (16 lanes: one CDF ele
     bool blend;        // probability model: false = FrequentistCDF16, true = BlendCDF16 (dv_blend.cuh); a kernel template constant
 };
 
+// Dynamic shared memory of every kernel that runs groups (decoders, encoder, replay) starts with one Cold per group, at this
+// stride.
+constexpr int SMEM_BYTES_PER_GROUP = (int)((sizeof(Cold) + 15) / 16 * 16);
 // The group's cold state, found from scratch.  The out-of-line helpers below use this instead of taking pointers into it: a
 // generic pointer to shared memory costs two special-register reads to build, and the compiler builds the arguments of those
 // (rare) calls at the head of every iteration of the main loop (~25 instructions per iteration).
 __device__ __forceinline__ Cold *cold_of_group(const G2 g) {
     extern __shared__ __align__(16) uint8_t dv_dynamic_smem[];
-    return reinterpret_cast<Cold *>(dv_dynamic_smem + (unsigned)g.grp * ((sizeof(Cold) + 15) / 16 * 16));
+    return reinterpret_cast<Cold *>(dv_dynamic_smem + (unsigned)g.grp * (size_t)SMEM_BYTES_PER_GROUP);
 }
 
 // ---------------------------------------------------------------------------------------------------------------

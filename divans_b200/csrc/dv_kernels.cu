@@ -1,6 +1,5 @@
-// dv_kernels.cu -- sm_90a kernels of the divANS batch engine: the framing/CRC pre-pass every decode runs first, and the
-// stream decoder of the reference's feature="blend" probability model (dv_blend.cuh).  Frequentist streams decode on the
-// v2 engine (dv2_kernels.cu).
+// dv_kernels.cu -- sm_90a kernels of the divANS batch engine around the stream decoder (dv2_kernels.cu): the framing/CRC
+// pre-pass every decode runs first (frame, payload scan, demux), and the pack kernel of the recording decoders.
 #include "dv_core.cuh"
 
 namespace dv {
@@ -227,114 +226,6 @@ void launch_frame(const FrameParams &p, uint8_t *payload, uint64_t payload_cap_b
     frame_kernel<<<blocks, 128, 0, st>>>(p);
     payload_scan_kernel<<<1, 1024, 0, st>>>(p.frame, p.n_streams, p.status, payload_cap_bytes / 16);
     demux_kernel<<<(p.n_streams + 3) / 4, 128, 0, st>>>(p, payload);
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// blend stream decoder: persistent warps, two streams per warp in lock step (dv_engine.cuh), work pulled from a global
-// counter.  Every nibble goes through the blend core (nibble_core_blend): the model has no literal fast loop.
-// ---------------------------------------------------------------------------------------------------------------
-// (REC: the recording decoder, as in dv2_kernels.cu)
-template <bool REC>
-__device__ __forceinline__ void decode_blend(const DecodeParams p, const RecParams r) {
-    extern __shared__ __align__(16) uint8_t smem[];
-    const int lane = threadIdx.x & 31;
-    const int group_in_block = (threadIdx.x >> 5) * 2 + (lane >> 4);
-    const uint32_t slot = blockIdx.x * (DECODE_BLOCK_THREADS / 16) + group_in_block;
-    G2 g;
-    g.l16 = lane & 15;
-    g.shift = lane & 16;
-    g.gmask = 0xffffu << (lane & 16);
-    g.store0 = (lane & 15) == 0;
-    g.nl = 16;
-    g.grp = group_in_block;
-    g.blend = true;
-
-    St s;
-    s.slot = p.arena + (uint64_t)slot * SLOT_STRIDE;
-    s.c = reinterpret_cast<Cold *>(smem + group_in_block * SMEM_BYTES_PER_GROUP);
-    s.tables = p.tables;
-    s.state = S_IDLE;
-    s.c->desired_context_mixing = 0; s.c->desired_prior_depth = 0; s.c->desired_force_stride = 9; s.c->desired_do_context_map = true;
-    s.c->have_desired_adapt = false; s.c->desired_adapt0 = s.c->desired_adapt1 = s.c->desired_adapt2 = s.c->desired_adapt3 = 0;
-    s.c->in.cmds = nullptr; s.c->in.n_cmds = 0; s.c->in.pos = 0; s.c->in.n_pms = 0; s.c->in.pms = nullptr; s.c->in.lits = nullptr;
-    s.c->model_rev = p.model_rev;
-    s.c->sidx = 0; s.out = nullptr; s.out_pos = 0; s.c->out_cap = 0; s.c->ring_len = 1024;
-    st_reset(s);
-    coder_init_dec(s.cur, nullptr, 0); s.cur.need_a = 0; coder_init_dec(s.c->oth, nullptr, 0);
-    Next nx; nx.cdf = A_misc(s, MI_DUMMY); nx.cdf2 = nullptr; nx.speed = SPK_NONE; nx.tagged = false; nx.sym = 0; nx.mix_hi = false;
-    store_default_cdfs(g, reinterpret_cast<int16_t *>(s.slot + OFF_MISC), (uint32_t)MISC_CDFS);   // incl. the dummy CDF
-    bool exhausted = false;
-
-    for (;;) {
-        __syncwarp();
-        // ---- fetch work for idle groups (converged; the broadcast shuffle is executed by every lane) ----
-        const bool want = (s.state == S_IDLE) && !exhausted;
-        if (__any_sync(FULL, want)) {
-            uint32_t v = 0;
-            if (want && g.store0) v = atomicAdd(p.work_counter, 1u);
-            v = __shfl_sync(FULL, v, 0, 16);
-            if (want) {
-                if (v >= p.n_streams) exhausted = true;
-                else if (p.status[v] != ST_OK) { if (g.store0) p.out_len[v] = 0; }   // framing / CRC failure: stay idle, fetch again
-                else {
-                    const uint8_t *in = p.in + p.in_off[v];
-                    const uint32_t pay0 = p.frame[4 * v + 1], pay1 = p.frame[4 * v + 2];
-                    const uint8_t *pl = p.payload + 16ull * p.frame[4 * v + 3];
-                    s.c->sidx = v;
-                    s.out = p.out + p.out_off[v];
-                    uint64_t cap = p.out_cap[v];
-                    s.c->out_cap = cap > 0xffffffffull ? 0xffffffffu : (uint32_t)cap; s.out_pos = 0;
-                    s.c->ring_len = 1u << in[5];
-                    reset_slot(g, s.slot);
-                    st_reset(s);
-                    coder_init_dec(s.cur, reinterpret_cast<const uint32_t *>(pl), pay0 >> 2);   // command stream (CMD_CODER, codec/interface.rs:49)
-                    coder_init_dec(s.c->oth, reinterpret_cast<const uint32_t *>(pl + (((uint64_t)pay0 + 15) & ~15ull)), pay1 >> 2);   // literal stream (LIT_CODER, :50)
-                    if (REC) {
-                        s.c->rec.blob = r.blobs + r.blob_off[v];
-                        s.c->rec.cap = r.blob_cap[v] > 0xffffffffull ? 0xffffffffu : (uint32_t)r.blob_cap[v];
-                        s.c->rec.n_cmds = 0; s.c->rec.n_pms = 0; s.c->rec.n_lits = 0;
-                    }
-                    enter_cmd_type<false>(s, nx);
-                }
-            }
-            if (__all_sync(FULL, exhausted && s.state == S_IDLE)) break;
-            __syncwarp();
-        }
-        // ---- one nibble per group ----
-        const bool busy = s.state != S_IDLE;
-        int sym = nibble_core_blend<false>(s, nx, g);
-        // ---- per-group scalar state machines (divergent) ----
-        if (busy) {
-            if (s.cur.underflow) s.status = ST_NEED_INPUT;
-            else transition<false, false, REC>(s, nx, g, sym);
-            if (s.status != ST_OK || s.state == S_IDLE) {
-                if (s.status == ST_OK && s.c->oth.underflow) s.status = ST_NEED_INPUT;
-                if (g.store0) { p.out_len[s.c->sidx] = s.out_pos; p.status[s.c->sidx] = s.status; }
-                if (REC && g.store0) {
-                    uint32_t *cnt = r.counts + 3 * (size_t)s.c->sidx;
-                    cnt[0] = s.c->rec.n_cmds; cnt[1] = s.c->rec.n_pms; cnt[2] = s.c->rec.n_lits;
-                }
-                s.state = S_IDLE; s.status = ST_OK;
-                nx.cdf = A_misc(s, MI_DUMMY); nx.cdf2 = nullptr; nx.speed = SPK_NONE; nx.tagged = false;
-                coder_init_dec(s.cur, nullptr, 0); s.cur.need_a = 0;
-            }
-        }
-    }
-}
-
-__global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) decode_kernel_blend(DecodeParams p) { decode_blend<false>(p, RecParams{}); }
-__global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) decode_kernel_blend_rec(DecodeParams p, RecParams r) { decode_blend<true>(p, r); }
-
-void launch_decode16_blend(const DecodeParams &p, uint32_t n_blocks, cudaStream_t st) {
-    size_t smem = (size_t)(DECODE_BLOCK_THREADS / 16) * SMEM_BYTES_PER_GROUP;
-    decode_kernel_blend<<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p);
-}
-void launch_decode16_blend_rec(const DecodeParams &p, const RecParams &r, uint32_t n_blocks, cudaStream_t st) {
-    size_t smem = (size_t)(DECODE_BLOCK_THREADS / 16) * SMEM_BYTES_PER_GROUP;
-    decode_kernel_blend_rec<<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p, r);
-}
-int decode_max_blocks_per_sm16_blend() {
-    return stream_kernel_blocks_per_sm(decode_kernel_blend, DECODE_BLOCK_THREADS, (size_t)(DECODE_BLOCK_THREADS / 16) * SMEM_BYTES_PER_GROUP);
 }
 
 }  // namespace dv

@@ -3,7 +3,7 @@
 #include "dv_common.cuh"
 
 namespace dv {
-constexpr int DECODE_BLOCK_THREADS = 64;
+constexpr int DECODE_BLOCK_THREADS = 64;   // the encoder's model pass and the blend decoder: two warps of two 16-lane groups per block
 
 // Resident blocks per SM of a stream kernel (register-limited; the kernels use ~2.3 KB of shared memory per block, so no
 // shared-memory carve-out preference is set).
@@ -14,16 +14,18 @@ template <typename K> static inline int stream_kernel_blocks_per_sm(K kernel, in
 }
 
 void launch_frame(const FrameParams &p, uint8_t *payload, uint64_t payload_cap_bytes, cudaStream_t st);   // frame + payload scan + demux (3 launches)
-// v2 engine (dv2_kernels.cu), lanes_per_stream = 16 (two streams per warp) or 8 (four)
-void launch_decode_v2(int lanes_per_stream, const DecodeParams &p, uint32_t n_blocks, cudaStream_t st);
+// the stream decoder (dv2_kernels.cu), lanes_per_stream = 16 (two streams per warp) or 8 (four).  blend = the reference's
+// feature="blend" probability model (dv_blend.cuh): 16 lanes per stream whatever lanes_per_stream says, no literal fast loop,
+// DECODE_BLOCK_THREADS per block.  Both models keep 32 groups per SM resident, so decode_max_blocks_per_sm_v2(16) x
+// decode_groups_per_block_v2(16) is the blend model's residency too.
+void launch_decode_v2(int lanes_per_stream, bool blend, const DecodeParams &p, uint32_t n_blocks, cudaStream_t st);
+void launch_decode_blend(const DecodeParams &p, const RecParams *r, uint32_t n_blocks, cudaStream_t st);   // its blend kernels (r: recording)
 int decode_max_blocks_per_sm_v2(int lanes_per_stream);
 int decode_groups_per_block_v2(int lanes_per_stream);
 void launch_encode_model(const EncodeParams &p, uint32_t n_blocks, cudaStream_t st);   // groups of 16 lanes
 void launch_encode_flush_mux(const EncodeParams &p, cudaStream_t st);                  // reverse rANS + mux/CRC (2 launches)
 int encode_max_blocks_per_sm();
-// the reference's feature="blend" probability model (dv_blend.cuh, dv_kernels.cu): 16 lanes per stream, no literal fast loop
-void launch_decode16_blend(const DecodeParams &p, uint32_t n_blocks, cudaStream_t st);
-int decode_max_blocks_per_sm16_blend();
+// the encoder's model pass under the blend model (dv_encode.cu built with DV_BLEND)
 void launch_encode_model_blend(const EncodeParams &p, uint32_t n_blocks, cudaStream_t st);
 void launch_rcp15_init(uint64_t *tab, cudaStream_t st);
 // model selection: the cost-only model passes (no logs: EncodeParams::cost_tab / tally), the fan-out of n streams to n x C
@@ -34,9 +36,9 @@ void launch_auto_fanout(const uint64_t *in_off, const uint64_t *in_len, uint64_t
                         uint32_t *v_pm, cudaStream_t st);
 void launch_auto_select(const uint64_t *tally, const int32_t *v_status, uint64_t n, uint32_t n_cands, uint32_t *chosen, uint64_t *cost,
                         cudaStream_t st);
-// decoding to command lists: the recording decoders (16 lanes per stream) and the pack kernel that finishes the blobs
-void launch_decode_v2_rec(const DecodeParams &p, const RecParams &r, uint32_t n_blocks, cudaStream_t st);
-void launch_decode16_blend_rec(const DecodeParams &p, const RecParams &r, uint32_t n_blocks, cudaStream_t st);
+// decoding to command lists: the recording decoder (16 lanes per stream, either model) and the pack kernel that finishes the
+// blobs (dv_kernels.cu)
+void launch_decode_v2_rec(bool blend, const DecodeParams &p, const RecParams &r, uint32_t n_blocks, cudaStream_t st);
 void launch_pack_cmds(const DecodeParams &p, const RecParams &r, cudaStream_t st);
 
 // replaying command lists to raw bytes (dv_replay.cu): list i is blobs[blob_off[i] .. +blob_len[i]), its bytes go to

@@ -17,7 +17,7 @@ namespace dv {
 
 constexpr int REPLAY_BLOCK_THREADS = 256;
 constexpr int REPLAY_WARPS = REPLAY_BLOCK_THREADS / 32;   // (launch bounds: 4 blocks per SM, 64 registers, no spills)
-constexpr size_t REPLAY_SMEM = (size_t)REPLAY_WARPS * ((sizeof(Cold) + 15) / 16 * 16);   // one Cold per warp (cold_of_group)
+constexpr size_t REPLAY_SMEM = (size_t)REPLAY_WARPS * SMEM_BYTES_PER_GROUP;   // one Cold per warp (cold_of_group)
 constexpr uint64_t REPLAY_COPY_CHUNK = 1ull << 31;   // the longest copy one replay_copy call takes
 
 __device__ __forceinline__ uint64_t replay_room(uint64_t pos, uint64_t cap, uint64_t len) { return pos >= cap ? 0 : min(len, cap - pos); }

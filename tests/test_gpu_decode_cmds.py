@@ -1,5 +1,5 @@
-"""Decoding to command lists on the GPU (-m gpu): the recording decoders (16-lane v2 decoder and blend decoder, dv2_kernels.cu /
-dv_kernels.cu) and the pack kernel, called through divans_b200_decode_cmds_batch_host / _device.  Every expected blob is the
+"""Decoding to command lists on the GPU (-m gpu): the recording decoders (the 16-lane decoder under either probability
+model, dv2_kernels.cu) and the pack kernel (dv_kernels.cu), called through divans_b200_decode_cmds_batch_host / _device.  Every expected blob is the
 oracle's: the command list dvo_decode_cmds recovers, serialised (oracle.decode_cmds(stream)[2].serialize())."""
 import ctypes
 import json
