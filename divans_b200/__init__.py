@@ -45,7 +45,7 @@ BATCH_SYMBOLS = [
     "divans_b200_debug_slot_header", "divans_b200_decode_cmds_batch_host", "divans_b200_decode_cmds_batch_device",
     "divans_b200_encode_cmds_batch_device", "divans_b200_encode_auto_batch_host", "divans_b200_encode_auto_batch_device",
     "divans_b200_encode_cmds_auto_batch_host", "divans_b200_encode_cmds_auto_batch_device",
-    "divans_b200_replay_cmds_batch_host", "divans_b200_replay_cmds_batch_device",
+    "divans_b200_replay_cmds_batch_host", "divans_b200_replay_cmds_batch_device", "divans_b200_lz77_cmds_batch_device",
 ]
 PM_RECORD_BYTES = 32 + 16384 + 1024 + 8192   # one prediction-mode record of a DVCL blob (include/divans_b200.h)
 
@@ -156,6 +156,9 @@ def load_library():
     L.divans_b200_ir_to_cmds.restype = ctypes.c_uint8
     L.divans_b200_lz77_cmds_batch.argtypes = [sz, vp, vp, vp, ctypes.c_int32, ctypes.c_int32, ctypes.c_int32, vp, sz, vp, vp, szp, ctypes.c_int32]
     L.divans_b200_lz77_cmds_batch.restype = ctypes.c_uint8
+    L.divans_b200_lz77_cmds_batch_device.argtypes = [vp, sz, vp, vp, vp, ctypes.c_uint64, ctypes.c_int32, ctypes.c_int32, ctypes.c_int32, vp, vp,
+                                                     vp, vp, vp, vp]
+    L.divans_b200_lz77_cmds_batch_device.restype = ctypes.c_uint8
     # reference FFI
     L.divans_new_decompressor.restype = vp
     L.divans_new_serial_decompressor.restype = vp
@@ -260,6 +263,16 @@ def lz77_cmds_batch(blob, in_off, in_len, window=16, pred_mode=2, mixing_value=4
     if rc != DIVANS_SUCCESS:
         raise ValueError("lz77_cmds_batch failed")
     return out, boff, blen
+
+
+def lz77_blob_cap(in_len):
+    """The blob region that always holds the LZ77 command list of in_len raw bytes (lz77_cmds_batch, and
+    Engine.lz77_cmds_batch_device): header, one PredictionMode command and at most 2 + 2 * floor(in_len / 5) Literal / Copy
+    commands, the record, and the literal pool, which is the raw bytes.  The count: with a Copies that have a Literal just
+    before them and b that do not, there are at most a + 1 Literal runs (never two in a row), and 5a + 4b <= in_len (a Copy
+    covers at least 4 bytes, a Literal at least 1), so 2a + b + 1 <= floor(2 in_len / 5) + 1 <= 2 floor(in_len / 5) + 2."""
+    L = np.asarray(in_len, np.uint64)
+    return np.uint64(32 + PM_RECORD_BYTES) + np.uint64(20) * (np.uint64(3) + np.uint64(2) * (L // np.uint64(5))) + L
 
 
 def first_blob_cap(out_cap):
@@ -677,6 +690,100 @@ class Engine:
         caller.wait_stream(s)
         d_new.record_stream(caller)   # (allocated on the private stream, used on the caller's from here on)
         return (d_new, new_off, new_len, status, chosen, cost) if auto else (d_new, new_off, new_len, status)
+
+    # -- generating LZ77 command lists on the GPU (include/divans_b200.h, divans_b200_lz77_cmds_batch_device)
+    def lz77_cmds_batch_device(self, n, d_in, d_in_off, d_in_len, max_in_len, window, pred_mode, mixing_value, d_blobs, d_blob_off,
+                               d_blob_cap, d_blob_len, d_status, stream=None):
+        """lz77_cmds_batch on the GPU, with raw device pointers (ints): the blob of stream i goes to d_blobs[d_blob_off[i] ..
+        +d_blob_cap[i]) (4-byte aligned; lz77_blob_cap always suffices).  Status 0: d_blob_len[i] bytes equal to lz77_cmds_batch's
+        blob; 2: the region is too small and d_blob_len[i] is the size needed; 3: refused (misaligned region, in_len > max_in_len
+        or >= 2**31).  Asynchronous on ``stream``; regions are not cleared first."""
+        rc = self._L.divans_b200_lz77_cmds_batch_device(self._h, n, d_in, d_in_off, d_in_len, int(max_in_len), int(window), int(pred_mode),
+                                                        int(mixing_value), d_blobs, d_blob_off, d_blob_cap, d_blob_len, d_status, stream)
+        if rc != DIVANS_SUCCESS:
+            raise DivansError("lz77_cmds_batch_device: " + self._err())
+
+    def compress_device(self, d_in, in_off, in_len, window=16, pred_mode=2, mixing_value=4, opts=None, candidates=None, stream=None,
+                        sub_batch=None):
+        """Compress raw buffers held in HBM with copy commands, without leaving the GPU: ``d_in`` is a CUDA uint8 tensor, buffer
+        i at in_off[i] .. +in_len[i] (host arrays).  lz77_cmds_batch_device (``window``, ``pred_mode``, ``mixing_value`` as for
+        lz77_cmds_batch) into regions of lz77_blob_cap, one synchronisation to read the blob lengths, then
+        encode_cmds_batch_device with ``opts`` (default: window_size 0, each list coded with its header window) -- the streams
+        Engine.encode(lz77 blobs, opts, cmds=True) returns.  With ``candidates`` the encode step is
+        encode_cmds_auto_batch_device and the call also returns chosen [n] and cost [n, C], as transcode_device.
+        The calls run on a private CUDA stream ordered after ``stream`` (default the current one).  The encoder's symbol logs
+        of a launch are one allocation, so the lists are encoded in as many sub-batches as memory needs: at most ``sub_batch``
+        streams each (default all), halved while the encoder cannot allocate them.  Returns (d_new, new_off, new_len, status):
+        status[i] is the generator's status where that failed (the list then reaches the encoder with length 0), else the
+        encoder's."""
+        import torch
+        n = len(in_off)
+        in_off, in_len = np.ascontiguousarray(in_off, np.uint64).reshape(n), np.ascontiguousarray(in_len, np.uint64).reshape(n)
+        o = opts if opts is not None else encode_options(window_size=0)
+        auto = candidates is not None
+        nc = len(candidates) if auto else 0
+        dev = d_in.device
+        if n == 0:
+            empty = torch.zeros(0, dtype=torch.uint8, device=dev), np.zeros(0, np.uint64), np.zeros(0, np.uint64), np.zeros(0, np.int32)
+            return empty + (np.zeros(0, np.uint32), np.zeros((0, nc), np.uint64)) if auto else empty
+        caller = stream if stream is not None else torch.cuda.current_stream(dev)
+        s = torch.cuda.Stream(dev)
+        s.wait_stream(caller)
+        u64 = lambda a: torch.from_numpy(np.ascontiguousarray(a, np.uint64).view(np.int64)).to(dev, non_blocking=False)
+        max_in = int(in_len.max())
+        bcap = lz77_blob_cap(in_len)
+        blob_off, blob_total = _regions(bcap)
+        with torch.cuda.stream(s):
+            d_meta = u64(np.concatenate([in_off, in_len, blob_off, bcap]))
+            M = [d_meta[k * n:(k + 1) * n] for k in range(4)]
+            d_blobs = torch.empty(blob_total, dtype=torch.uint8, device=dev)
+            d_gen = torch.zeros(2 * n, dtype=torch.int64, device=dev)   # blob_len | status (int32 pairs)
+            self.lz77_cmds_batch_device(n, d_in.data_ptr(), M[0].data_ptr(), M[1].data_ptr(), max_in, window, pred_mode, mixing_value,
+                                        d_blobs.data_ptr(), M[2].data_ptr(), M[3].data_ptr(), d_gen.data_ptr(), d_gen[n:].data_ptr(),
+                                        s.cuda_stream)
+            g = d_gen.cpu().numpy()   # (the synchronisation that reads the blob lengths)
+        gen_st = g[n:].view(np.int32)[:n].copy()
+        blob_len = np.where(gen_st == 0, g[:n].view(np.uint64), np.uint64(0))
+        new_cap = _encoded_cap(blob_len)
+        new_off, new_total = _regions(new_cap)
+        max_blob = int(blob_len.max())
+        with torch.cuda.stream(s):
+            d_enc = u64(np.concatenate([blob_len, new_off, new_cap]))
+            d_new = torch.empty(new_total, dtype=torch.uint8, device=dev)
+            # new_len | status (| candidates: cost [n * C] | chosen)
+            d_res = torch.zeros((2 + (nc + 1 if auto else 0)) * n, dtype=torch.int64, device=dev)
+            m = n if sub_batch is None else max(1, int(sub_batch))
+            i0 = 0
+            self.last_compress_sub_batches = 0   # (encode launches of the most recent call)
+            while i0 < n:
+                k = min(m, n - i0)
+                at = lambda t, esz=8: t.data_ptr() + i0 * esz
+                enc = (k, d_blobs.data_ptr(), at(M[2]), at(d_enc[:n]), max_blob, max_in, d_new.data_ptr(), at(d_enc[n:2 * n]),
+                       at(d_enc[2 * n:]), at(d_res), at(d_res[n:], 4))
+                try:
+                    if auto:
+                        self.encode_cmds_auto_batch_device(*enc, at(d_res[(2 + nc) * n:], 4), at(d_res[2 * n:], 8 * nc), o, candidates,
+                                                           s.cuda_stream)
+                    else:
+                        self.encode_cmds_batch_device(*enc, o, s.cuda_stream)
+                except DivansError as e:
+                    if k == 1 or not ("cannot allocate" in str(e) or "out of memory" in str(e)):
+                        raise
+                    m = k // 2   # the logs of k streams did not fit next to what the GPU holds
+                    continue
+                i0 += k
+                self.last_compress_sub_batches += 1
+            r = d_res.cpu().numpy()
+        enc_st = r[n:2 * n].view(np.int32)[:n]
+        status = np.where(gen_st != 0, gen_st, enc_st).astype(np.int32)
+        new_len = r[:n].view(np.uint64).copy()
+        caller.wait_stream(s)
+        d_new.record_stream(caller)   # (allocated on the private stream, used on the caller's from here on)
+        if auto:
+            chosen = r[(2 + nc) * n:].view(np.uint32)[:n].copy()
+            cost = r[2 * n:(2 + nc) * n].view(np.uint64).reshape(n, nc).copy()
+            return d_new, new_off, new_len, status, chosen, cost
+        return d_new, new_off, new_len, status
 
     # -- replaying command lists to raw bytes (include/divans_b200.h, divans_b200_replay_cmds_batch_*)
     def replay_cmds_batch_host(self, blobs, blob_off, blob_len, out, out_off, out_cap, window_size=0):

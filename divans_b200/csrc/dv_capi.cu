@@ -16,6 +16,7 @@
 
 #include "../../include/divans_b200.h"
 #include "dv_kernels.h"
+#include "dv_lz77.h"
 
 #ifndef DV_TABLES_PATH
 #error "DV_TABLES_PATH must point at brotli_tables.bin"
@@ -78,6 +79,10 @@ struct divans_b200_ctx {
     // scratch: offsets, lengths, record index, status and cost
     uint8_t *d_pm_records = nullptr; uint32_t *d_cost_tab = nullptr;
     uint64_t *d_auto = nullptr; size_t auto_cap = 0;
+    // LZ77 command generator (lz77_cmds_batch_device): per-warp head table + prev array, and the PredictionMode record it copies
+    // (lz_scratch_asked: the request the allocation was made for, which free memory may have cut down to lz_scratch_words)
+    int32_t *d_lz_scratch = nullptr; size_t lz_scratch_words = 0, lz_scratch_asked = 0;
+    uint8_t *d_lz_pm = nullptr;
     bool main_end_is_evm1 = false;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr, evm = nullptr, evm1 = nullptr;   // ev0 | frame kernel | evm | decode kernel | ev1
     cudaEvent_t ev_busy = nullptr; bool busy_recorded = false;                 // end of the most recent launch set on any stream
@@ -176,6 +181,7 @@ extern "C" void divans_b200_destroy(divans_b200_ctx *ctx) {
     if (ctx->ev_busy) cudaEventDestroy(ctx->ev_busy);
     cudaFree(ctx->d_sf); cudaFree(ctx->d_replay); cudaFree(ctx->d_enc_scratch); cudaFree(ctx->d_pm_internal); cudaFree(ctx->d_rcp15);
     cudaFree(ctx->d_pm_records); cudaFree(ctx->d_cost_tab); cudaFree(ctx->d_auto);
+    cudaFree(ctx->d_lz_scratch); cudaFree(ctx->d_lz_pm);
     for (auto &ln : ctx->lane) {
         free_host_bufs(ln.bufs);
         if (ln.h_res) cudaFreeHost(ln.h_res);
@@ -1038,6 +1044,77 @@ extern "C" DivansResult divans_b200_replay_cmds_batch_host(divans_b200_ctx *ctx,
     return DIVANS_SUCCESS;
 } catch (...) {
     if (ctx) ctx->err = "divans_b200: out of host memory while staging the command lists";
+    return DIVANS_FAILURE;
+}
+
+// ---- generating LZ77 command lists on the GPU ----
+// One launch (dv_lz77.cu) over n raw buffers in HBM: the blobs of divans_b200_lz77_cmds_batch.  Like the replay call it uses the
+// context's work counter and timing events only, and its own scratch: 2^15 + max_in_len int32 per warp, kept and grown on demand.
+// The warps are the fewest of n, the context's max_resident and what the scratch allocation holds.
+extern "C" DivansResult divans_b200_lz77_cmds_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_in, const uint64_t *d_in_off,
+                                                           const uint64_t *d_in_len, uint64_t max_in_len, int32_t window, int32_t pred_mode,
+                                                           int32_t mixing_value, uint8_t *d_blobs, const uint64_t *d_blob_off,
+                                                           const uint64_t *d_blob_cap, uint64_t *d_blob_len, int32_t *d_status,
+                                                           void *cuda_stream) try {
+    if (!ctx) return DIVANS_FAILURE;
+    if (window < 10 || window > 24) { ctx->err = "lz77_cmds_batch_device: window must be 10..24"; return DIVANS_FAILURE; }
+    if (n > 0xffffffffull) { ctx->err = "lz77_cmds_batch_device: too many streams"; return DIVANS_FAILURE; }
+    if (n == 0) return DIVANS_SUCCESS;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream;
+    // streams of 2^31 bytes or more are refused by the kernel, so prev never needs more entries than that
+    const uint64_t stride = lz77_scratch_words(std::min<uint64_t>(max_in_len, 0x7fffffffull));
+    uint64_t warps = std::min<uint64_t>(n, std::max<uint32_t>(ctx->max_resident, 1u));
+    // Grown when it holds fewer warps than asked for, unless free memory already cut an equal or larger request down: that
+    // allocation is as large as it gets, and asking again would only free it and wait for the device.
+    const uint64_t want = warps * stride;
+    if (ctx->lz_scratch_words < stride || (ctx->lz_scratch_words < want && want > ctx->lz_scratch_asked)) {
+        // the old scratch may still be in use by the previous launch: cudaFree waits for the device
+        cudaFree(ctx->d_lz_scratch); ctx->d_lz_scratch = nullptr; ctx->lz_scratch_words = ctx->lz_scratch_asked = 0;
+        size_t free_b = 0, total_b = 0;
+        cudaMemGetInfo(&free_b, &total_b);
+        warps = std::min<uint64_t>(warps, (uint64_t)free_b * 9 / 10 / (stride * 4));
+        while (warps > 0 && cudaMalloc((void **)&ctx->d_lz_scratch, warps * stride * 4) != cudaSuccess) {
+            cudaGetLastError();
+            ctx->d_lz_scratch = nullptr;
+            warps /= 2;
+        }
+        if (warps == 0) {
+            char buf[200];
+            snprintf(buf, sizeof buf, "divans_b200: cannot allocate the LZ77 scratch of one warp for streams of up to %llu bytes: %llu bytes",
+                     (unsigned long long)max_in_len, (unsigned long long)stride * 4);
+            ctx->err = buf;
+            return DIVANS_FAILURE;
+        }
+        ctx->lz_scratch_words = warps * stride;
+        ctx->lz_scratch_asked = want;
+    }
+    warps = std::min<uint64_t>(warps, ctx->lz_scratch_words / stride);
+    if (!ctx->d_lz_pm) CK(cudaMalloc((void **)&ctx->d_lz_pm, PM_RECORD_BYTES));
+    if (ctx->busy_recorded) CK(cudaStreamWaitEvent(st, ctx->ev_busy, 0));
+    // the record of lz77_blob: pred_mode and mixing_value stored as bytes
+    std::vector<uint8_t> &pm = ctx->h_pm;
+    pm.assign(PM_RECORD_BYTES, 0);
+    raw_record(pm.data(), pred_mode, mixing_value);
+    CK(cudaMemcpyAsync(ctx->d_lz_pm, pm.data(), PM_RECORD_BYTES, cudaMemcpyHostToDevice, st));
+    Lz77Params lp;
+    lp.in = d_in; lp.in_off = d_in_off; lp.in_len = d_in_len; lp.max_in_len = max_in_len;
+    lp.blobs = d_blobs; lp.blob_off = d_blob_off; lp.blob_cap = d_blob_cap; lp.blob_len = d_blob_len; lp.status = d_status;
+    lp.pm = ctx->d_lz_pm; lp.n_streams = (uint32_t)n; lp.window = window;
+    lp.work_counter = ctx->d_counter; lp.scratch = ctx->d_lz_scratch; lp.stride = stride; lp.n_warps = (uint32_t)warps;
+    CK(cudaMemsetAsync(ctx->d_counter, 0, 4, st));
+    CK(cudaEventRecord(ctx->ev0, st));
+    CK(cudaEventRecord(ctx->evm, st));
+    launch_lz77_cmds(lp, st);
+    CK(cudaEventRecord(ctx->ev1, st));
+    CK(cudaEventRecord(ctx->ev_busy, st)); ctx->busy_recorded = true;
+    ctx->main_end_is_evm1 = false;
+    ctx->launches += 1;
+    CK(cudaGetLastError());
+    return DIVANS_SUCCESS;
+} catch (...) {
+    if (ctx) ctx->err = "divans_b200: out of host memory";
     return DIVANS_FAILURE;
 }
 

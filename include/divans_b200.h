@@ -392,6 +392,29 @@ DivansResult divans_b200_ir_to_cmds(const char *ir_text, size_t ir_len, uint8_t 
 DivansResult divans_b200_lz77_cmds_batch(size_t n, const uint8_t *in, const uint64_t *in_off, const uint64_t *in_len, int32_t window,
                                          int32_t pred_mode, int32_t mixing_value, uint8_t *out, size_t out_cap, uint64_t *blob_off,
                                          uint64_t *blob_len, size_t *total, int32_t n_threads);
+/* The same generator on the GPU, next to raw buffers already in HBM; all pointers are DEVICE pointers.  Stream i is
+ * in[in_off[i] .. +in_len[i]); its blob goes to blobs[blob_off[i] .. +blob_cap[i]).  Per stream:
+ *  - status 0: blob_len[i] bytes were written at blobs + blob_off[i], byte for byte the blob divans_b200_lz77_cmds_batch writes
+ *    for the same input, window, pred_mode and mixing_value (the last two stored as bytes, as there).
+ *  - status 2: the region is too small; blob_len[i] is the exact size the blob needs.  The region's contents are unspecified.
+ *  - status 3 (refused, the input is not read, blob_len[i] = 0): blob_off[i] is not 4-byte aligned (the encoders read records
+ *    as u32), in_len[i] > max_in_len, or in_len[i] >= 2^31.
+ *  - A region of 32 + 20 * (3 + 2 * floor(in_len / 5)) + PM_RECORD_BYTES + in_len bytes always holds the blob (Python:
+ *    divans_b200.lz77_blob_cap): one PredictionMode command, and at most 2 + 2 * floor(in_len / 5) Literal and Copy commands.
+ *    Proof: say a Copies have a Literal just before them and b do not.  Literal runs are maximal (never two in a row), so there
+ *    are at most a + 1 of them.  A Copy covers at least 4 bytes and a Literal at least 1, so 5a + 4b <= in_len, and the Literal
+ *    and Copy commands number at most 2a + b + 1 <= floor(2 in_len / 5) + 1 <= 2 floor(in_len / 5) + 2.
+ *  - Nothing outside the regions is written, and regions are not cleared.
+ * Call level: DIVANS_FAILURE for a window outside 10..24, n > 2^32 - 1, or when not even one warp's scratch (128 KiB +
+ * 4 * max_in_len bytes, kept on the context and grown on demand) can be allocated; divans_b200_last_error names the size.  One
+ * launch on min(n, max_resident, what the scratch holds) warps, asynchronous on `cuda_stream` (NULL = the context's stream) and
+ * serialised on the context like every device call; divans_b200_last_kernel_ms is valid after it.  No arena slot or encoder
+ * log is used, so it works on a fresh context.  Feed the blobs to divans_b200_encode_cmds_batch_device with max_blob_len from
+ * the blob_len of this call and max_raw_len = max_in_len. */
+DivansResult divans_b200_lz77_cmds_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_in, const uint64_t *d_in_off,
+                                                const uint64_t *d_in_len, uint64_t max_in_len, int32_t window, int32_t pred_mode,
+                                                int32_t mixing_value, uint8_t *d_blobs, const uint64_t *d_blob_off,
+                                                const uint64_t *d_blob_cap, uint64_t *d_blob_len, int32_t *d_status, void *cuda_stream);
 /*
  * command list blob ("DVCL", little endian) -- the binary form of the reference's IR (src/bin/divans.rs:191-483):
  *   u32 magic 0x4c435644, u32 version 1, u32 n_cmds, u32 n_predmodes, u32 n_literal_bytes, u32 window, u32[2] 0
