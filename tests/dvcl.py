@@ -1,5 +1,5 @@
 """Hand-built DVCL command-list blobs (include/divans_b200.h) for the replay tests: a builder, and one blob per refusal rule of
-divans_b200_replay_cmds_batch_* together with the status and out_len the rule gives."""
+divans_b200_replay_cmds_batch_* together with the status and out_len the rule gives; and two blobs the encoder refuses."""
 import numpy as np
 
 MAGIC = 0x4C435644
@@ -51,3 +51,25 @@ def refusal_cases():
         ("dictionary length differs from d", blob(pre + [(DICT, 0, 4, 0, 5)], lits), 0, 3),
     ]
     return cases
+
+
+def literal_outside_pool(b):
+    """the first literal command of DVCL blob `b` made to end past the literal pool"""
+    w = np.frombuffer(b, np.uint8).copy()
+    h = w[:32].view(np.uint32)
+    for c in range(int(h[2])):
+        r = w[32 + 20 * c: 52 + 20 * c].view(np.uint32)
+        if r[0] == LIT:
+            r[1] = h[4] - min(int(r[2]), int(h[4])) + 1
+            return w.tobytes()
+    raise AssertionError("no literal")
+
+
+def pm_flood(pm_blob, k):
+    """k PredictionMode commands that all point at the one record of `pm_blob` (a list holding a single PredictionMode):
+    more command nibbles than the header's sizes allow for, i.e. a command-log overflow"""
+    h = np.frombuffer(pm_blob[:32], np.uint32)
+    assert int(h[2]) == 1 and int(h[3]) == 1
+    rec = pm_blob[52:]
+    hdr = np.array([h[0], 1, k, 1, 0, h[5], 0, 0], np.uint32).tobytes()
+    return hdr + np.tile(np.array([PREDMODE, 0, 0, 0, 0], np.uint32), k).tobytes() + rec[:len(rec) - int(h[4])]

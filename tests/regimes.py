@@ -212,6 +212,32 @@ EDGES = {
     "both_over": ("both", 0, 125, ("both_over", 131073)),        # both payloads over 131073 bytes: 65536-byte records alternate
 }
 EDGE_NAMES = list(EDGES)
+# The same properties under the blend model (oracle/oracle_blend.py), whose payloads differ in length for the same input: found
+# by search_blend_edges below.  The command-nibble edges and both_over keep the parameters of EDGES (nibble counts depend on
+# the command list alone).
+BLEND_EDGES = {
+    "lit4096": ("rnd", 0, 3703, ("lit_payload", 4096)),
+    "lit16384": ("rnd", 1, 14855, ("lit_payload", 16384)),
+    "lit65536": ("rnd", 3, 57870, ("lit_payload", 65536)),
+    "lit69632": ("rnd", 0, 61486, ("lit_payload", 65536 + 4096)),
+    "lit81920": ("rnd", 0, 72426, ("lit_payload", 65536 + 16384)),
+    "lit131072": ("rnd", 0, 117133, ("lit_payload", 131072)),
+    "cmd4096": ("lz16", 0, 16692, ("cmd_payload", 4096)),
+    "cmd16384": ("lz16", 0, 59415, ("cmd_payload", 16384)),
+    "nib65535": EDGES["nib65535"],
+    "nib65536": EDGES["nib65536"],
+    "nib65537": EDGES["nib65537"],
+    "both_over": EDGES["both_over"],
+}
+
+
+def is_blend(oracle):
+    return getattr(oracle, "_VARIANT", "") == "blend"
+
+
+def edges(oracle):
+    """the edge table of `oracle`'s probability model"""
+    return BLEND_EDGES if is_blend(oracle) else EDGES
 
 
 @functools.lru_cache(maxsize=1)
@@ -225,25 +251,81 @@ def _corpus():
     return synth.text_corpus(1 << 20)
 
 
-def edge_options(name):
-    return dict(window_size=22) if EDGES[name][0] == "rnd" else dict(window_size=16)
+def edge_options(name, oracle=None):
+    src = (EDGES if oracle is None else edges(oracle))[name][0]
+    return dict(window_size=22) if src == "rnd" else dict(window_size=16)
+
+
+def _edge_raw(src, off, n):
+    if src == "rnd":
+        return _rnd()[off:off + n]
+    if src == "lz16":
+        return _corpus()[off:off + n]
+    # "both": n pieces of 5000 text bytes (copy-heavy) and 1000 random bytes (literal-heavy)
+    return b"".join(_corpus()[k * 5000:(k + 1) * 5000] + _rnd()[k * 1000:(k + 1) * 1000] for k in range(n))
+
+
+def edge_measure(oracle, src, off, n):
+    """payload lengths and nibble counts of the stream an edge with these parameters makes under `oracle`"""
+    raw = _edge_raw(src, off, n)
+    if src == "rnd":
+        stream = oracle.encode_raw(raw, oracle.options(window_size=22))
+    else:
+        stream = oracle.Commands.lz77(raw, window=16).encode(oracle.options(window_size=16))
+    cmd, lit = oracle.demux(stream)
+    rc, out, st = oracle.decode(stream, out_cap=len(raw) + 64, stats=True)
+    assert rc == 0 and out == raw
+    return dict(cmd_payload=len(cmd), lit_payload=len(lit), cmd_nibbles=st["cmd_nibbles"], lit_nibbles=st["lit_nibbles"])
+
+
+def edge_has_property(got, prop):
+    kind, want = prop
+    if kind == "both_over":
+        return got["cmd_payload"] > want and got["lit_payload"] > want
+    return got[kind] == want
+
+
+def search_blend_edges(oracle_blend, seed=5, tries=64):
+    """the seeded search that found BLEND_EDGES (seconds; not run by the tests).  An edge whose EDGES parameters keep their
+    property under the blend model keeps them.  Otherwise, for the EDGES offset and then seeded random offsets below 64, a
+    bisection over the length finds the shortest input whose measured payload reaches the target, and the lengths around it
+    are tried for an exact hit (payload lengths grow in steps of 4 bytes, and not quite monotonically).  Returns the table."""
+    rng = np.random.default_rng(seed)
+    table = {}
+    for name, (src, off0, n0, prop) in EDGES.items():
+        if edge_has_property(edge_measure(oracle_blend, src, off0, n0), prop):
+            table[name] = (src, off0, n0, prop)
+            continue
+        kind, want = prop
+        for t in range(tries):
+            off = off0 if t == 0 else int(rng.integers(0, 64))
+            lo, hi = n0 // 2, n0 * 2
+            while lo < hi:
+                mid = (lo + hi) // 2
+                if edge_measure(oracle_blend, src, off, mid)[kind] >= want:
+                    hi = mid
+                else:
+                    lo = mid + 1
+            hit = next((n for n in range(lo - 16, lo + 17) if edge_measure(oracle_blend, src, off, n)[kind] == want), None)
+            if hit is not None:
+                table[name] = (src, off, hit, prop)
+                break
+        else:
+            raise AssertionError("no blend parameters for edge %s" % name)
+    return table
 
 
 @functools.lru_cache(maxsize=None)
 def edge(name, oracle):
-    """(Commands, raw, stream) of framing edge `name`"""
-    src, off, n, _prop = EDGES[name]
+    """(Commands, raw, stream) of framing edge `name` under `oracle`'s probability model"""
+    src, off, n, _prop = edges(oracle)[name]
+    raw = _edge_raw(src, off, n)
     if src == "rnd":
-        raw = _rnd()[off:off + n]
-        stream = oracle.encode_raw(raw, oracle.options(**edge_options(name)))
+        stream = oracle.encode_raw(raw, oracle.options(**edge_options(name, oracle)))
         cl = oracle.decode_cmds(stream, out_cap=n + 64)[2]
         return cl, raw, stream
-    if src == "lz16":
-        raw = _corpus()[off:off + n]
-    else:                       # "both": n pieces of 5000 text bytes (copy-heavy) and 1000 random bytes (literal-heavy)
-        raw = b"".join(_corpus()[k * 5000:(k + 1) * 5000] + _rnd()[k * 1000:(k + 1) * 1000] for k in range(n))
     cl = oracle.Commands.lz77(raw, window=16)
-    return cl, raw, cl.encode(oracle.options(**edge_options(name)))
+    return cl, raw, cl.encode(oracle.options(**edge_options(name, oracle)))
 
 
 # ---- re-muxing: the same two coder payloads under another record chain ----
@@ -271,6 +353,20 @@ def close(oracle, body):
     """header + records -> a complete stream: EOF marker, then the trailer with the CRC32C of everything before it"""
     body += b"\xff\xfe\xff"
     return body + oracle.crc32c(body).to_bytes(4, "little") + b"ans~"
+
+
+def record_chain(stream):
+    """the record chain of a well-formed stream as a plan (the inverse of mux_records): [(coder, n, k)]"""
+    o, plan = 16, []
+    while stream[o] != 0xFF:
+        b = stream[o]
+        if b < 2:
+            n = (stream[o + 1] | stream[o + 2] << 8) + 1
+            plan.append((b, n, None)); o += 3 + n
+        else:
+            k = b >> 4
+            plan.append((b & 1, 1024 << (2 * k), k)); o += 1 + (1024 << (2 * k))
+    return plan
 
 
 def record_starts(plan):

@@ -5,6 +5,7 @@ import io
 import numpy as np
 import pytest
 
+import dvcl
 from irfuzz import random_ir
 
 pytestmark = pytest.mark.gpu
@@ -304,28 +305,6 @@ def test_wide_speed_raw_encodes_refused_like_the_oracle(engine, oracle, text):
 # ---------------------------------------------------------------------------------------------------------------------
 # slot succession: one block of 4 encoder slots, good regimes between refused and hostile lists
 # ---------------------------------------------------------------------------------------------------------------------
-def _dvcl_literal_outside_pool(blob):
-    """the first literal command of a DVCL blob made to end past the literal pool"""
-    w = np.frombuffer(blob, np.uint8).copy()
-    h = w[:32].view(np.uint32)
-    for c in range(int(h[2])):
-        r = w[32 + 20 * c: 52 + 20 * c].view(np.uint32)
-        if r[0] == 3:
-            r[1] = h[4] - min(int(r[2]), int(h[4])) + 1
-            return w.tobytes()
-    raise AssertionError("no literal")
-
-
-def _dvcl_pm_flood(pm_blob, k):
-    """k PredictionMode commands that all point at the one record of `pm_blob` (a list holding a single PredictionMode):
-    more command nibbles than the header's sizes allow for, i.e. a command-log overflow"""
-    h = np.frombuffer(pm_blob[:32], np.uint32)
-    assert int(h[2]) == 1 and int(h[3]) == 1
-    rec = pm_blob[52:]
-    hdr = np.array([h[0], 1, k, 1, 0, h[5], 0, 0], np.uint32).tobytes()
-    return hdr + np.tile(np.array([7, 0, 0, 0, 0], np.uint32), k).tobytes() + rec[:len(rec) - int(h[4])]
-
-
 def test_encoder_slot_succession(oracle):
     """Engine(0, 2, 16): the encoder runs one 64-thread block, 4 slots.  `[A] * 4 + [X] * 4 + [B] * 4 ...` gives every slot
     A, then X, then B.  The GOOD regimes, grouped by option set (one launch per group, consecutive launches on the same
@@ -354,8 +333,8 @@ def test_encoder_slot_succession(oracle):
             assert refused is not None, kw
             good = [R.command_list(n, oracle).serialize() for n in names]
             cap = max(32 * int(np.frombuffer(b[:32], np.uint32)[2]) + 62000 * int(np.frombuffer(b[:32], np.uint32)[3]) + 64 for b in good + [refused])
-            flood = _dvcl_pm_flood(pm_only.serialize(), cap // per_pm + 2)
-            bad = [refused, _dvcl_literal_outside_pool(good[[i for i, n in enumerate(names) if n != "empty"][0]]), flood]
+            flood = dvcl.pm_flood(pm_only.serialize(), cap // per_pm + 2)
+            bad = [refused, dvcl.literal_outside_pool(good[[i for i, n in enumerate(names) if n != "empty"][0]]), flood]
             seq, want = [], []
             for i, (n, b) in enumerate(zip(names, good)):
                 seq += [b] * 4; want += [(0, R.build(n, oracle).stream)] * 4

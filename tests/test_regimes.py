@@ -153,6 +153,47 @@ def test_framing_edges_cover_the_mux_codes(oracle):
     assert stream[at - 1] == 0x21   # literal coder, code k = 2: one header byte
 
 
+def test_regimes_under_the_blend_model(oracle_blend):
+    """tests/test_gpu_blend_regimes.py builds every regime with the blend oracle: each decodes to its input or its stated
+    status there too, and each good regime's command list re-encodes to its stream"""
+    for name in R.ALL:
+        c = R.build(name, oracle_blend)
+        rc, out = oracle_blend.decode(c.stream, out_cap=c.cap, skip_crc=bool(c.flags))
+        assert rc == c.status and (c.status != 0 or out == c.raw), name
+    for name in R.GOOD:
+        cl = R.command_list(name, oracle_blend)
+        assert cl.encode(oracle_blend.options(**R.encode_options(name))) == R.build(name, oracle_blend).stream, name
+    assert [R.build(n, oracle_blend).status for n in R.FAILING] == [1, 3, 2]
+
+
+@pytest.mark.parametrize("name", R.EDGE_NAMES)
+def test_blend_framing_edge_has_its_property(oracle_blend, name):
+    """BLEND_EDGES: the properties of EDGES under the blend model, whose payloads are longer for the same input"""
+    assert list(R.edges(oracle_blend)) == R.EDGE_NAMES and R.edges(oracle_blend)[name][3] == R.EDGES[name][3]
+    src, off, n, prop = R.BLEND_EDGES[name]
+    cl, raw, stream = R.edge(name, oracle_blend)
+    got = R.edge_measure(oracle_blend, src, off, n)
+    assert R.edge_has_property(got, prop), got
+    assert cl.encode(oracle_blend.options(**R.edge_options(name, oracle_blend))) == stream
+    rc, out = oracle_blend.decode(stream, out_cap=len(raw) + 64)
+    assert rc == 0 and out == raw
+
+
+def test_blend_edges_reach_the_mux_codes_of_the_default_edges(oracle, oracle_blend):
+    """each blend edge has the record chain of its default twin: the same one-byte codes of the same coders, the same
+    three-byte records, in the same order (the sizes of the three-byte records differ)"""
+    shape = lambda stream: [(c, k) if k is not None else (c, None) for c, _n, k in R.record_chain(stream)]
+    for name in R.EDGE_NAMES:
+        d, b = R.edge(name, oracle)[2], R.edge(name, oracle_blend)[2]
+        assert R.mux_records(oracle, d, R.record_chain(d)) == d and R.mux_records(oracle_blend, b, R.record_chain(b)) == b
+        assert shape(b) == shape(d), name
+        assert {k for _c, _n, k in R.record_chain(b)} - {None} == {k for _c, _n, k in R.record_chain(d)} - {None}
+    # the blend model moves the payload edges: the default parameters miss the property under it
+    for name in ("lit4096", "cmd4096"):
+        src, off, n, prop = R.EDGES[name]
+        assert not R.edge_has_property(R.edge_measure(oracle_blend, src, off, n), prop)
+
+
 @pytest.mark.parametrize("lay", R.LAYOUTS)
 def test_remuxed_stream_decodes_on_the_oracle(oracle, lay):
     """a new record chain over the same payloads decodes to the same bytes; each layout has the shape it is named for"""
