@@ -265,17 +265,21 @@ template <int LPG>
 __device__ __forceinline__ uint64_t rans_advance_v2(const uint64_t st, const uint32_t ev, const uint32_t mv, const int sym) {
     const uint32_t inv = recip32(mv);
     uint32_t hi, lo;
-    const int prev = (sym - 1) & 15;
+    // lo: the cumulative value of element sym - 1, 0 for sym = 0, taken as element (sym - 1) mod 16 masked to 15 bits.  For
+    // sym >= 1 on a monotone CDF the search found c[sym - 1] <= r < max, so divq gives less than 0x8000 and the mask keeps
+    // it.  For sym = 0 the source is element 15, the max itself, whose cumulative value is exactly 0x8000: it masks to 0.
+    // (At 16 lanes the shuffle takes its source lane mod 16.)
+    const int prev = sym - 1;
     if (LPG == 16) {
         const uint32_t cum = divq(ev, inv, mv);
         hi = __shfl_sync(FULL, cum, sym, 16); lo = __shfl_sync(FULL, cum, prev, 16);
     } else {
         const uint32_t cum = divq(ev & 0xffffu, inv, mv) | (divq(ev >> 16, inv, mv) << 16);   // element 15: 0x8000
-        const uint32_t whi = __shfl_sync(FULL, cum, sym >> 1, 8), wlo = __shfl_sync(FULL, cum, prev >> 1, 8);
+        const uint32_t whi = __shfl_sync(FULL, cum, sym >> 1, 8), wlo = __shfl_sync(FULL, cum, (prev & 15) >> 1, 8);
         hi = (sym & 1) ? (whi >> 16) : (whi & 0xffffu);
-        lo = (prev & 1) ? (wlo >> 16) : (wlo & 0xffffu);
+        lo = (prev & 1) ? (wlo >> 16) : wlo;
     }
-    if (sym == 0) lo = 0;
+    lo &= 0x7fffu;
     const uint32_t freq = hi - lo - 1;                                       // "major hax": start = lo + 1 (probability/interface.rs:103-104)
     // 0 <= t < freq in every stream an encoder wrote.  A corrupted payload can put the offset below the bin: offset 0 decodes
     // symbol 0, whose bin starts at 1 ("major hax"), so t = -1.  The reference computes the state in 64-bit wrapping arithmetic
@@ -300,13 +304,14 @@ __device__ __forceinline__ void rans_pair_v2(uint64_t &a, uint64_t &b, const uin
     a = xa; b = xb;
 }
 
-// bin search: for a monotone CDF whose last element is max (> r) the number of elements with r < c[i] is 16 - sym
+// bin search: for a monotone CDF whose last element is max (> r) the number of elements with c[i] <= r is sym (the vote
+// counts it directly: no 16 - popc of the complement)
 template <int LPG>
 __device__ __forceinline__ int search_v2(const uint64_t st, const uint32_t ev, const uint32_t mv, const uint32_t bsel) {
     const uint32_t rr = (((uint32_t)st & 0x7fffu) * mv) >> 15;              // probability/interface.rs:140
-    if (LPG == 16) return 16 - __popc(__ballot_sync(FULL, rr < ev) & bsel);  // bsel: the group's 16 ballot bits
-    const unsigned b0 = __ballot_sync(FULL, rr < (ev & 0xffffu)), b1 = __ballot_sync(FULL, rr < (ev >> 16));
-    return 16 - (__popc(__byte_perm(b0, b1, bsel)) >> 1);                    // bsel: PRMT selector [g, 4+g, g, 4+g]
+    if (LPG == 16) return __popc(__ballot_sync(FULL, rr >= ev) & bsel);     // bsel: the group's 16 ballot bits
+    const unsigned b0 = __ballot_sync(FULL, rr >= (ev & 0xffffu)), b1 = __ballot_sync(FULL, rr >= (ev >> 16));
+    return __popc(__byte_perm(b0, b1, bsel)) >> 1;                          // bsel: PRMT selector [g, 4+g, g, 4+g]
 }
 
 // ---- dynamic context mixing >= 2 (codec/literal.rs:219-259), 16 lanes per stream: the stride prior `nb` (tagged literal table) is
@@ -453,6 +458,8 @@ __device__ __forceinline__ bool literal_plain_loop_v2(St &s, Next &nx, const G2 
     f.kp = LPG == 16 ? (uint32_t)(li + 1) : ((uint32_t)(2 * li + 1) | ((uint32_t)(2 * li + 2) << 16));
     f.mytag = lane_tag<LPG>(s.gen, li);
     const uint32_t tbits = LPG == 16 ? TAG_BITS16 : TAG_BITS8;
+    // the tag check is ((element ^ mytag) & tchk) == 0: a dummy group's priors always pass, so its own test stays out of the vote
+    const uint32_t tchk = active ? tbits : 0u;
     const uint32_t defe = default_elems<LPG>(li);
     const uint32_t bsel = LPG == 16 ? (0xffffu << g.shift) : ((uint32_t)(g.shift >> 3) * 0x1111u + 0x4040u);
     const unsigned gm = g.gmask;
@@ -501,8 +508,8 @@ __device__ __forceinline__ bool literal_plain_loop_v2(St &s, Next &nx, const G2 
             // -- high nibble: search (speculative: the prior is almost always one this stream has written)
             uint32_t eh_v = eh & ~tbits, mh_v = mh & 0x7fffu;
             int h = search_v2<LPG>(k.a, eh_v, mh_v, bsel);
-            const unsigned okh = __ballot_sync(FULL, !active || (eh & tbits) == f.mytag);
-            if (__builtin_expect(okh != FULL, 0)) {                       // some group met a prior of an older stream: default CDF
+            if (__builtin_expect(!__all_sync(FULL, ((eh ^ f.mytag) & tchk) == 0), 0)) {   // some group met a prior of an older
+                const unsigned okh = __ballot_sync(FULL, ((eh ^ f.mytag) & tchk) == 0);      // stream: default CDF
                 if ((okh & gm) != gm) { eh_v = defe; mh_v = 64u; }
                 h = search_v2<LPG>(k.a, eh_v, mh_v, bsel);
             }
@@ -515,8 +522,8 @@ __device__ __forceinline__ bool literal_plain_loop_v2(St &s, Next &nx, const G2 
             // -- low nibble: search
             uint32_t el_v = el & ~tbits, ml_v = ml & 0x7fffu;
             int l = search_v2<LPG>(k.b, el_v, ml_v, bsel);
-            const unsigned okl = __ballot_sync(FULL, !active || (el & tbits) == f.mytag);
-            if (__builtin_expect(okl != FULL, 0)) {
+            if (__builtin_expect(!__all_sync(FULL, ((el ^ f.mytag) & tchk) == 0), 0)) {
+                const unsigned okl = __ballot_sync(FULL, ((el ^ f.mytag) & tchk) == 0);
                 if ((okl & gm) != gm) { el_v = defe; ml_v = 64u; }
                 l = search_v2<LPG>(k.b, el_v, ml_v, bsel);
             }
