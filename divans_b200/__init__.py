@@ -46,6 +46,8 @@ BATCH_SYMBOLS = [
     "divans_b200_encode_cmds_batch_device", "divans_b200_encode_auto_batch_host", "divans_b200_encode_auto_batch_device",
     "divans_b200_encode_cmds_auto_batch_host", "divans_b200_encode_cmds_auto_batch_device",
     "divans_b200_replay_cmds_batch_host", "divans_b200_replay_cmds_batch_device", "divans_b200_lz77_cmds_batch_device",
+    "divans_b200_encode_mixmap_batch_host", "divans_b200_encode_mixmap_batch_device", "divans_b200_encode_cmds_mixmap_batch_host",
+    "divans_b200_encode_cmds_mixmap_batch_device",
 ]
 PM_RECORD_BYTES = 32 + 16384 + 1024 + 8192   # one prediction-mode record of a DVCL blob (include/divans_b200.h)
 
@@ -78,6 +80,12 @@ DEFAULT_LITERAL_MODELS = [(0, 4), (2, 8), (2, 5), (2, 1), (2, 7), (3, 5), (0, 5)
 # index, and a pair whose list would outgrow the encoder's logs costs the maximum, so a list the plain call encodes is encoded,
 # and by the tally at no higher cost than under its own records.
 LITERAL_MODEL_KEEP = (-1, -1)
+
+# encode_mixmap's default mixing values, chosen per literal context (mixing-mask entry) under the options' context mode.  The
+# values the survey corpora pick most per entry (tools/mixmap_probe.py --survey, DESIGN.md section 4, "Per-context mixing
+# values"); 4 first, the encoder's default value, so unvisited entries keep it.
+DEFAULT_MIXING_VALUES = [4, 5, 8, 1, 7, 0]
+MIX_ENTRIES = 8192
 
 
 class CAllocator(ctypes.Structure):
@@ -148,6 +156,16 @@ def load_library():
     L.divans_b200_encode_cmds_auto_batch_device.argtypes = [vp, sz, vp, vp, vp, ctypes.c_uint64, ctypes.c_uint64, vp, vp, vp, vp, vp,
                                                             ctypes.POINTER(EncodeOptions), vp, ctypes.c_uint32, vp, vp, vp]
     L.divans_b200_encode_cmds_auto_batch_device.restype = ctypes.c_uint8
+    L.divans_b200_encode_mixmap_batch_host.argtypes = batch + [ctypes.POINTER(EncodeOptions), vp, ctypes.c_uint32, vp, vp, vp, vp]
+    L.divans_b200_encode_mixmap_batch_host.restype = ctypes.c_uint8
+    L.divans_b200_encode_cmds_mixmap_batch_host.argtypes = batch + [ctypes.POINTER(EncodeOptions), vp, ctypes.c_uint32, vp, vp, vp, vp]
+    L.divans_b200_encode_cmds_mixmap_batch_host.restype = ctypes.c_uint8
+    L.divans_b200_encode_mixmap_batch_device.argtypes = [vp, sz, vp, vp, vp, ctypes.c_uint64, vp, vp, vp, vp, vp, ctypes.POINTER(EncodeOptions),
+                                                         vp, ctypes.c_uint32, vp, vp, vp, vp, vp]
+    L.divans_b200_encode_mixmap_batch_device.restype = ctypes.c_uint8
+    L.divans_b200_encode_cmds_mixmap_batch_device.argtypes = [vp, sz, vp, vp, vp, ctypes.c_uint64, ctypes.c_uint64, vp, vp, vp, vp, vp,
+                                                              ctypes.POINTER(EncodeOptions), vp, ctypes.c_uint32, vp, vp, vp, vp, vp]
+    L.divans_b200_encode_cmds_mixmap_batch_device.restype = ctypes.c_uint8
     L.divans_b200_replay_cmds_batch_host.argtypes = batch + [ctypes.c_int32]
     L.divans_b200_replay_cmds_batch_host.restype = ctypes.c_uint8
     L.divans_b200_replay_cmds_batch_device.argtypes = batch + [ctypes.c_int32, vp]
@@ -587,6 +605,79 @@ class Engine:
         list coded under the cheapest of ``candidates`` (encode_cmds_auto_batch_host)."""
         status, outs, chosen, _ = self._encode_lists(blobs, opts, True, True, candidates)
         return [(int(s), b, int(c)) for s, b, c in zip(status, outs, chosen)]
+
+    # ---- per-context mixing values (include/divans_b200.h) ----
+    @staticmethod
+    def _values(values):
+        v = np.ascontiguousarray(DEFAULT_MIXING_VALUES if values is None else values, np.int32)
+        return (v if v.size else np.zeros(1, np.int32)), int(v.size)
+
+    def _mixmap_host(self, cmds, in_blob, in_off, in_len, out, out_off, out_cap, opts, values, want_bins):
+        n = len(in_off)
+        in_off, in_len, out_off, out_cap, out_len, status = _host_batch(in_off, in_len, out_off, out_cap)
+        v, k = self._values(values)
+        chosen = np.zeros(n, np.uint32)
+        mixing = np.zeros((n, MIX_ENTRIES), np.uint8)
+        cost = np.zeros((n, k + 1), np.uint64)
+        bins = np.zeros((n, k, MIX_ENTRIES), np.uint64) if want_bins else None
+        o = opts or encode_options()
+        fn = self._L.divans_b200_encode_cmds_mixmap_batch_host if cmds else self._L.divans_b200_encode_mixmap_batch_host
+        rc = fn(self._h, n, _ptr(in_blob), _ptr(in_off), _ptr(in_len), _ptr(out), _ptr(out_off), _ptr(out_cap), _ptr(out_len), _ptr(status),
+                ctypes.byref(o), _ptr(v), k, _ptr(chosen), _ptr(mixing), _ptr(cost), _ptr(bins) if want_bins else None)
+        if rc != DIVANS_SUCCESS:
+            raise DivansError("%s_batch_host: %s" % ("encode_cmds_mixmap" if cmds else "encode_mixmap", self._err()))
+        return out_len, status, chosen, mixing, cost, bins
+
+    def encode_mixmap_batch_host(self, in_blob, in_off, in_len, out, out_off, out_cap, opts=None, values=None, bins=False):
+        """encode_batch_host with each stream's mixing values chosen per literal context among ``values`` (default
+        DEFAULT_MIXING_VALUES) under opts.literal_pred_mode.  Returns (out_len, status, chosen, mixing [n, 8192], cost [n, k + 1],
+        bins [n, k, 8192] or None): chosen[i] == k is the mixed record, cost[i] = the k uniform costs then the mixed one."""
+        return self._mixmap_host(False, in_blob, in_off, in_len, out, out_off, out_cap, opts, values, bins)
+
+    def encode_cmds_mixmap_batch_host(self, blobs, blob_off, blob_len, out, out_off, out_cap, opts=None, values=None, bins=False):
+        """encode_mixmap_batch_host for command lists: every PredictionMode record of a list is replaced."""
+        return self._mixmap_host(True, blobs, blob_off, blob_len, out, out_off, out_cap, opts, values, bins)
+
+    def encode_mixmap_batch_device(self, n, d_in, d_in_off, d_in_len, max_in_len, d_out, d_out_off, d_out_cap, d_out_len, d_status,
+                                   d_chosen=None, d_mixing=None, d_cost=None, d_bins=None, opts=None, values=None, stream=None):
+        """encode_mixmap_batch_host with raw device pointers (ints, or None for an output not wanted).  Asynchronous."""
+        v, k = self._values(values)
+        o = opts or encode_options()
+        rc = self._L.divans_b200_encode_mixmap_batch_device(self._h, n, d_in, d_in_off, d_in_len, int(max_in_len), d_out, d_out_off, d_out_cap,
+                                                            d_out_len, d_status, ctypes.byref(o), _ptr(v), k, d_chosen, d_mixing, d_cost,
+                                                            d_bins, stream)
+        if rc != DIVANS_SUCCESS:
+            raise DivansError("encode_mixmap_batch_device: " + self._err())
+
+    def encode_cmds_mixmap_batch_device(self, n, d_blobs, d_blob_off, d_blob_len, max_blob_len, max_raw_len, d_out, d_out_off, d_out_cap,
+                                        d_out_len, d_status, d_chosen=None, d_mixing=None, d_cost=None, d_bins=None, opts=None, values=None,
+                                        stream=None):
+        """encode_cmds_mixmap_batch_host with raw device pointers (ints, or None for an output not wanted).  Asynchronous."""
+        v, k = self._values(values)
+        o = opts or encode_options()
+        rc = self._L.divans_b200_encode_cmds_mixmap_batch_device(self._h, n, d_blobs, d_blob_off, d_blob_len, int(max_blob_len),
+                                                                 int(max_raw_len), d_out, d_out_off, d_out_cap, d_out_len, d_status,
+                                                                 ctypes.byref(o), _ptr(v), k, d_chosen, d_mixing, d_cost, d_bins, stream)
+        if rc != DIVANS_SUCCESS:
+            raise DivansError("encode_cmds_mixmap_batch_device: " + self._err())
+
+    def _mixmap_lists(self, bufs, opts, cmds, values):
+        blob, in_off, in_len = _pack(bufs)
+        out_cap = _encoded_cap(in_len)
+        out_off, out_total = _regions(out_cap)
+        out = np.zeros(out_total, np.uint8)
+        out_len, status, chosen, _, _, _ = self._mixmap_host(cmds, blob, in_off, in_len, out, out_off, out_cap, opts, values, False)
+        return [(int(s), out[int(o):int(o) + int(n)].tobytes() if s == DIVANS_SUCCESS else None, int(c))
+                for s, o, n, c in zip(status, out_off, out_len, chosen)]
+
+    def encode_mixmap(self, raws, opts=None, values=None):
+        """Convenience: list of raw byte strings -> list of (status, .divans bytes or None, chosen): chosen < k is the uniform
+        value values[chosen], k the per-context record (encode_mixmap_batch_host)."""
+        return self._mixmap_lists(raws, opts, False, values)
+
+    def encode_cmds_mixmap(self, blobs, opts=None, values=None):
+        """Convenience: encode_mixmap for DVCL command-list blobs (encode_cmds_mixmap_batch_host)."""
+        return self._mixmap_lists(blobs, opts, True, values)
 
     def encode_cmds_batch_device(self, n, d_blobs, d_blob_off, d_blob_len, max_blob_len, max_raw_len, d_out, d_out_off, d_out_cap, d_out_len,
                                  d_status, opts=None, stream=None):

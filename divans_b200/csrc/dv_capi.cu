@@ -79,6 +79,12 @@ struct divans_b200_ctx {
     // scratch: offsets, lengths, record index, status and cost
     uint8_t *d_pm_records = nullptr; uint32_t *d_cost_tab = nullptr;
     uint64_t *d_auto = nullptr; size_t auto_cap = 0;
+    // per-context mixing values (encode_mixmap_*): per-stream scratch (per-entry winners, mixed pass, record index), the k uniform
+    // and n mixed records, the binned cost pass's per-slot bins, and the host calls' staging of the mixing / bins outputs
+    uint64_t *d_mix = nullptr; size_t mix_cap = 0;
+    uint8_t *d_mix_records = nullptr; size_t mix_records_cap = 0;
+    uint64_t *d_slot_bins = nullptr; size_t slot_bins_cap = 0;
+    uint64_t *d_mix_out = nullptr; size_t mix_out_cap = 0;
     // LZ77 command generator (lz77_cmds_batch_device): per-warp head table + prev array, and the PredictionMode record it copies
     // (lz_scratch_asked: the request the allocation was made for, which free memory may have cut down to lz_scratch_words)
     int32_t *d_lz_scratch = nullptr; size_t lz_scratch_words = 0, lz_scratch_asked = 0;
@@ -181,6 +187,7 @@ extern "C" void divans_b200_destroy(divans_b200_ctx *ctx) {
     if (ctx->ev_busy) cudaEventDestroy(ctx->ev_busy);
     cudaFree(ctx->d_sf); cudaFree(ctx->d_replay); cudaFree(ctx->d_enc_scratch); cudaFree(ctx->d_pm_internal); cudaFree(ctx->d_rcp15);
     cudaFree(ctx->d_pm_records); cudaFree(ctx->d_cost_tab); cudaFree(ctx->d_auto);
+    cudaFree(ctx->d_mix); cudaFree(ctx->d_mix_records); cudaFree(ctx->d_slot_bins); cudaFree(ctx->d_mix_out);
     cudaFree(ctx->d_lz_scratch); cudaFree(ctx->d_lz_pm);
     for (auto &ln : ctx->lane) {
         free_host_bufs(ln.bufs);
@@ -662,10 +669,13 @@ static DivansResult encode_device_internal(divans_b200_ctx *ctx, size_t n, int r
     return DIVANS_SUCCESS;
 }
 
-// literal model selection of a batch (encode_host_common, encode_device_common): the candidates, and where chosen / cost go
+// literal model selection of a batch (encode_host_common, encode_device_common): the candidates, and where chosen / cost go.
+// mixmap (divans_b200_encode_mixmap_*): the candidates are (opts->literal_pred_mode, v[c]); chosen may be NULL, cost has k + 1
+// columns, and mixing / bins are the optional per-context outputs.
 struct AutoSel {
     const divans_b200_literal_model *cands; uint32_t n_cands;
     uint32_t *chosen; uint64_t *cost;
+    bool mixmap = false; uint8_t *mixing = nullptr; uint64_t *bins = nullptr;
 };
 
 // ---- literal model selection ----
@@ -709,6 +719,16 @@ static bool check_cands(divans_b200_ctx *ctx, const divans_b200_literal_model *c
     return true;
 }
 
+// the cost table of the cost passes, on the context (uploaded on `st` by the first call that needs it)
+static bool ensure_cost_tab(divans_b200_ctx *ctx, cudaStream_t st) {
+    if (ctx->d_cost_tab) return true;
+    static uint32_t tab[32768];
+    static std::once_flag once;
+    std::call_once(once, [] { for (uint32_t f = 0; f < 32768; f++) tab[f] = freq_cost(f); });
+    if (!ck(ctx, cudaMalloc((void **)&ctx->d_cost_tab, sizeof tab), "cudaMalloc(cost table)")) return false;
+    return ck(ctx, cudaMemcpyAsync(ctx->d_cost_tab, tab, sizeof tab, cudaMemcpyHostToDevice, st), "cudaMemcpyAsync(cost table)");
+}
+
 // One launch sequence over n streams in HBM (raw buffers, or command lists with raw_mode 0): fan out to n * C virtual streams
 // (dv_encode.cu: candidate-major), the cost-only model pass over all of them, the per-stream argmin into d_chosen, then the
 // encoder pipeline with stream i coded under candidate d_chosen[i] (raw: its starting record; command lists: the record that
@@ -731,13 +751,7 @@ static DivansResult encode_auto_device_nolock(divans_b200_ctx *ctx, size_t n, in
     int32_t *v_status = reinterpret_cast<int32_t *>(v_pm + nv);
     if (!ctx->d_pm_records) CK(cudaMalloc((void **)&ctx->d_pm_records, 16 * (size_t)PM_RECORD_BYTES));
     if (ctx->busy_recorded) CK(cudaStreamWaitEvent(st, ctx->ev_busy, 0));
-    if (!ctx->d_cost_tab) {
-        static uint32_t tab[32768];
-        static std::once_flag once;
-        std::call_once(once, [] { for (uint32_t f = 0; f < 32768; f++) tab[f] = freq_cost(f); });
-        CK(cudaMalloc((void **)&ctx->d_cost_tab, sizeof tab));
-        CK(cudaMemcpyAsync(ctx->d_cost_tab, tab, sizeof tab, cudaMemcpyHostToDevice, st));
-    }
+    if (!ensure_cost_tab(ctx, st)) return DIVANS_FAILURE;
     std::vector<uint8_t> &pm = ctx->h_pm;
     pm.assign((size_t)n_cands * PM_RECORD_BYTES, 0);
     uint32_t keep = 0;   // bit c: candidate c is KEEP (its record stays zero and is never read)
@@ -762,6 +776,94 @@ static DivansResult encode_auto_device_nolock(divans_b200_ctx *ctx, size_t n, in
                                   d_status, o, window, st, ctx->d_pm_records, d_chosen, keep);
 }
 
+// Per-context mixing values: one launch sequence over n streams in HBM.  Records [0, k) are R(p, v[c]), records [k, k + n) the
+// streams' mixed records M_i.
+//  1. the binned cost pass over the n * k pairs (fan-out as encode_auto): totals u[i][c], per-entry winners best[i][e]
+//  2. mixmap_map_kernel builds M_i;  3. the cost pass of every stream under M_i: x[i]
+//  4. mixmap_select_kernel: record c* or k + i per stream;  5. the plain pipeline from that record.
+// Command lists: every record of a list is replaced (pm_keep 0).  The record index of a mixed stream, k + i, can exceed 31; the
+// model pass tests it against pm_keep with a 32-bit shift (shr.u32 yields 0 for counts of 32 or more), so it still reads as "replace".
+static DivansResult encode_mixmap_device_nolock(divans_b200_ctx *ctx, size_t n, int raw_mode, const uint8_t *d_in, const uint64_t *d_in_off,
+                                                const uint64_t *d_in_len, uint64_t max_in_len, const LogCaps &caps, uint8_t *d_out,
+                                                const uint64_t *d_out_off, const uint64_t *d_out_cap, uint64_t *d_out_len, int32_t *d_status,
+                                                const divans_b200_encode_options *o, int window, const divans_b200_literal_model *cands,
+                                                uint32_t k, uint32_t *d_chosen, uint64_t *d_cost, uint8_t *d_mixing, uint64_t *d_bins,
+                                                cudaStream_t st) {
+    const uint64_t nv = (uint64_t)n * k;
+    const size_t vslots = encode_slots(ctx, nv);
+    if (ensure_arena(ctx, vslots) != DIVANS_SUCCESS) return DIVANS_FAILURE;
+    if (!grow(ctx, &ctx->d_replay, &ctx->replay_cap, vslots * (size_t)caps.replay)) return DIVANS_FAILURE;
+    // v_off [nv] | v_len [nv] | tally [nv] | v_pm u32 [nv] | v_status i32 [nv]
+    if (!grow(ctx, &ctx->d_auto, &ctx->auto_cap, 4 * nv + 2)) return DIVANS_FAILURE;
+    uint64_t *v_off = ctx->d_auto, *v_len = v_off + nv, *tally = v_len + nv;
+    uint32_t *v_pm = reinterpret_cast<uint32_t *>(tally + nv);
+    int32_t *v_status = reinterpret_cast<int32_t *>(v_pm + nv);
+    // best [n * 8192] | x_tally [n] | x_status i32 [n] | mix_idx u32 [n] | rec_idx u32 [n]
+    if (!grow(ctx, &ctx->d_mix, &ctx->mix_cap, (size_t)n * MIX_ENTRIES + 3 * n)) return DIVANS_FAILURE;
+    uint64_t *best = ctx->d_mix, *x_tally = best + (size_t)n * MIX_ENTRIES;
+    int32_t *x_status = reinterpret_cast<int32_t *>(x_tally + n);
+    uint32_t *mix_idx = reinterpret_cast<uint32_t *>(x_status + n), *rec_idx = mix_idx + n;
+    if (!grow(ctx, &ctx->d_mix_records, &ctx->mix_records_cap, (k + n) * (size_t)PM_RECORD_BYTES)) return DIVANS_FAILURE;
+    if (!grow(ctx, &ctx->d_slot_bins, &ctx->slot_bins_cap, vslots * (size_t)MIX_ENTRIES)) return DIVANS_FAILURE;
+    if (ctx->busy_recorded) CK(cudaStreamWaitEvent(st, ctx->ev_busy, 0));
+    if (!ensure_cost_tab(ctx, st)) return DIVANS_FAILURE;
+    std::vector<uint8_t> &pm = ctx->h_pm;
+    pm.assign((size_t)k * PM_RECORD_BYTES, 0);
+    MixValues vals; memset(&vals, 0, sizeof vals); vals.k = k;
+    for (uint32_t c = 0; c < k; c++) {
+        raw_record(pm.data() + (size_t)c * PM_RECORD_BYTES, cands[c].literal_pred_mode, cands[c].literal_mixing_value);
+        vals.v[c] = (uint8_t)cands[c].literal_mixing_value;
+    }
+    CK(cudaMemcpyAsync(ctx->d_mix_records, pm.data(), pm.size(), cudaMemcpyHostToDevice, st));
+    CK(cudaMemsetAsync(best, 0xff, (size_t)n * MIX_ENTRIES * 8, st));
+    launch_auto_fanout(d_in_off, d_in_len, n, k, v_off, v_len, v_pm, st);
+
+    // 1. uniform passes, binned
+    EncodeParams tp = encode_params(ctx, nv, raw_mode, d_in, v_off, v_len, max_in_len, caps, o, window);
+    tp.pm_internal = ctx->d_mix_records; tp.pm_index = v_pm; tp.pm_keep = 0;
+    tp.status = v_status; tp.cost_tab = ctx->d_cost_tab; tp.tally = tally;
+    BinParams bp;
+    bp.slot_bins = ctx->d_slot_bins; bp.best = best; bp.bins_out = d_bins; bp.n = (uint32_t)n; bp.k = k;
+    CK(cudaMemsetAsync(ctx->d_counter, 0, 4, st));
+    if (o->cdf_model == DIVANS_B200_CDF_BLEND) launch_encode_bins_blend(tp, bp, (uint32_t)(vslots / ENCODE_GROUPS_PER_BLOCK), st);
+    else launch_encode_bins(tp, bp, (uint32_t)(vslots / ENCODE_GROUPS_PER_BLOCK), st);
+    // 2. mixed records;  3. the mixed pass, the plain cost pass (a mixed record is not uniform, so its literals take the per-nibble loop)
+    launch_mixmap_map(best, n, vals, ctx->d_mix_records, mix_idx, st);
+    EncodeParams xp = encode_params(ctx, n, raw_mode, d_in, d_in_off, d_in_len, max_in_len, caps, o, window);
+    xp.pm_internal = ctx->d_mix_records; xp.pm_index = mix_idx; xp.pm_keep = 0;
+    xp.status = x_status; xp.cost_tab = ctx->d_cost_tab; xp.tally = x_tally;
+    CK(cudaMemsetAsync(ctx->d_counter, 0, 4, st));
+    const uint32_t xblocks = (uint32_t)(encode_slots(ctx, n) / ENCODE_GROUPS_PER_BLOCK);
+    if (o->cdf_model == DIVANS_B200_CDF_BLEND) launch_encode_tally_blend(xp, xblocks, st); else launch_encode_tally(xp, xblocks, st);
+    // 4. choice
+    launch_mixmap_select(tally, v_status, x_tally, x_status, n, vals, ctx->d_mix_records, rec_idx, d_chosen, d_cost, d_mixing, st);
+    ctx->launches += 5;
+    CK(cudaGetLastError());
+    return encode_device_internal(ctx, n, raw_mode, d_in, d_in_off, d_in_len, max_in_len, caps, d_out, d_out_off, d_out_cap, d_out_len,
+                                  d_status, o, window, st, ctx->d_mix_records, rec_idx, 0);
+}
+
+// `values` (1..16 mixing values 0..15) and the mode of opts as candidate literal models; false (and the error) for anything else
+static bool mixmap_cands(divans_b200_ctx *ctx, const int32_t *values, uint32_t k, const divans_b200_encode_options *o,
+                         divans_b200_literal_model *cands) {
+    char buf[200];
+    if (!values || k < 1 || k > 16) { ctx->err = "encode_mixmap: 1..16 mixing values are required"; return false; }
+    if (o->literal_pred_mode < 0 || o->literal_pred_mode > 3) {
+        snprintf(buf, sizeof buf, "encode_mixmap: opts->literal_pred_mode %d is outside 0..3", (int)o->literal_pred_mode);
+        ctx->err = buf;
+        return false;
+    }
+    for (uint32_t c = 0; c < k; c++) {
+        if (values[c] < 0 || values[c] > 15) {
+            snprintf(buf, sizeof buf, "encode_mixmap: mixing value %u (%d) is outside 0..15", c, (int)values[c]);
+            ctx->err = buf;
+            return false;
+        }
+        cands[c].literal_pred_mode = o->literal_pred_mode; cands[c].literal_mixing_value = values[c];
+    }
+    return true;
+}
+
 // The four device encode calls: raw buffers (max_raw_len = max_in_len) or command lists (raw_mode 0), each plain or, with
 // `sel` (device chosen / cost), coded under the cheapest candidate literal model.  Host marshalling (the candidates' records,
 // the error strings) may throw, and no C++ exception may cross the C boundary.
@@ -772,7 +874,8 @@ static DivansResult encode_device_common(divans_b200_ctx *ctx, size_t n, int raw
     if (!ctx || !opts) return DIVANS_FAILURE;
     if (sel && !check_cands(ctx, sel->cands, sel->n_cands, !raw_mode)) return DIVANS_FAILURE;
     if (n == 0) return DIVANS_SUCCESS;
-    if (sel && !sel->chosen) { ctx->err = raw_mode ? "encode_auto: d_chosen is required" : "encode_cmds_auto: d_chosen is required"; return DIVANS_FAILURE; }
+    if (sel && !sel->mixmap && !sel->chosen) { ctx->err = raw_mode ? "encode_auto: d_chosen is required" : "encode_cmds_auto: d_chosen is required"; return DIVANS_FAILURE; }
+    if (sel && sel->mixmap && n > 0x7fffffffull) { ctx->err = "batch too large"; return DIVANS_FAILURE; }   // (one block per stream)
     const uint64_t nv = (uint64_t)n * (sel ? sel->n_cands : 1);
     if (nv > 0xffffffffull || max_in_len > 0x7fff0000ull || max_raw_len > 0x7fff0000ull) { ctx->err = "batch too large"; return DIVANS_FAILURE; }
     const int window = !raw_mode && opts->window_size == 0 ? 0 : clamp_window(opts->window_size);
@@ -802,6 +905,9 @@ static DivansResult encode_device_common(divans_b200_ctx *ctx, size_t n, int raw
             ctx->sf_cap = words;
         }
     }
+    if (sel && sel->mixmap)
+        return encode_mixmap_device_nolock(ctx, n, raw_mode, d_in, d_in_off, d_in_len, max_in_len, caps, d_out, d_out_off, d_out_cap, d_out_len,
+                                           d_status, opts, window, sel->cands, sel->n_cands, sel->chosen, sel->cost, sel->mixing, sel->bins, st);
     if (sel)
         return encode_auto_device_nolock(ctx, n, raw_mode, d_in, d_in_off, d_in_len, max_in_len, caps, d_out, d_out_off, d_out_cap, d_out_len,
                                          d_status, opts, window, sel->cands, sel->n_cands, sel->chosen, sel->cost, st);
@@ -858,7 +964,7 @@ static DivansResult encode_host_common(divans_b200_ctx *ctx, size_t n, int raw_m
     if (!ctx || !opts) return DIVANS_FAILURE;
     if (sel && !check_cands(ctx, sel->cands, sel->n_cands, !raw_mode)) return DIVANS_FAILURE;
     if (n == 0) return DIVANS_SUCCESS;
-    if (sel && !sel->chosen) { ctx->err = raw_mode ? "encode_auto: chosen is required" : "encode_cmds_auto: chosen is required"; return DIVANS_FAILURE; }
+    if (sel && !sel->mixmap && !sel->chosen) { ctx->err = raw_mode ? "encode_auto: chosen is required" : "encode_cmds_auto: chosen is required"; return DIVANS_FAILURE; }
     if (sel && (uint64_t)n * sel->n_cands > 0xffffffffull) { ctx->err = "batch too large"; return DIVANS_FAILURE; }
     std::lock_guard<std::mutex> lk(ctx->mu);
     CK(cudaSetDevice(ctx->device));
@@ -898,8 +1004,12 @@ static DivansResult encode_host_common(divans_b200_ctx *ctx, size_t n, int raw_m
         uint64_t mx = 0; size_t i1 = i0;
         while (i1 < n) {
             const LogCaps c = {std::max(need[i1].cmd, mc.cmd), std::max(need[i1].lit, mc.lit), std::max(need[i1].replay, mc.replay)};
-            // encode_auto: the cost pass also holds a replay window per slot for up to m * C pairs
-            const uint64_t rep = sel ? (uint64_t)encode_slots(ctx, (i1 - i0 + 1) * (size_t)sel->n_cands) * c.replay : 0;
+            // encode_auto: the cost pass also holds a replay window per slot for up to m * C pairs.  encode_mixmap: and 64 KiB of
+            // bins per slot, and per stream its winners, mixed record, mixing output and (when asked for) C x 64 KiB of bins
+            const uint64_t vs = sel ? (uint64_t)encode_slots(ctx, (i1 - i0 + 1) * (size_t)sel->n_cands) : 0;
+            uint64_t rep = vs * c.replay;
+            if (sel && sel->mixmap)
+                rep += vs * MIX_ENTRIES * 8 + (uint64_t)(i1 - i0 + 1) * (MIX_ENTRIES * 9 + PM_RECORD_BYTES + (sel->bins ? sel->n_cands * MIX_ENTRIES * 8ull : 0));
             if (i1 > i0 && (c.cmd + c.lit) * 4 * (uint64_t)(i1 - i0 + 1) + rep > budget) break;
             mc = c;
             if (in_len[i1] > mx) mx = in_len[i1];
@@ -910,8 +1020,17 @@ static DivansResult encode_host_common(divans_b200_ctx *ctx, size_t n, int raw_m
         uint64_t out_lo, out_hi;
         regions_span(m, out_off + i0, out_cap + i0, out_lo, out_hi);
         if (!grow(ctx, &b.d_out, &b.d_out_cap, (size_t)(out_hi - out_lo) + 64)) return DIVANS_FAILURE;
-        // in_off | in_len | out_off | out_cap | out_len | status (+ encode_auto: chosen | cost [m * C])
-        if (!grow(ctx, &b.d_meta, &b.d_meta_cap, m * 6 + (sel ? m + m * (size_t)sel->n_cands : 0))) return DIVANS_FAILURE;
+        // in_off | in_len | out_off | out_cap | out_len | status (+ encode_auto: chosen | cost [m * C]; encode_mixmap: cost [m * (C + 1)])
+        const size_t cost_cols = sel ? sel->n_cands + (sel->mixmap ? 1 : 0) : 0;
+        if (!grow(ctx, &b.d_meta, &b.d_meta_cap, m * 6 + (sel ? m + m * cost_cols : 0))) return DIVANS_FAILURE;
+        // encode_mixmap: mixing [m * 8192 bytes] | bins [m * C * 8192]
+        uint8_t *d_mixing = nullptr; uint64_t *d_bins = nullptr;
+        if (sel && sel->mixmap) {
+            const size_t bw = sel->bins ? m * (size_t)sel->n_cands * MIX_ENTRIES : 0;
+            if (!grow(ctx, &ctx->d_mix_out, &ctx->mix_out_cap, m * (size_t)MIX_ENTRIES / 8 + bw)) return DIVANS_FAILURE;
+            if (sel->mixing) d_mixing = reinterpret_cast<uint8_t *>(ctx->d_mix_out);
+            if (sel->bins) d_bins = ctx->d_mix_out + m * (size_t)MIX_ENTRIES / 8;
+        }
         std::vector<uint64_t> rel(m);
         for (size_t i = 0; i < m; i++) rel[i] = out_off[i0 + i] - out_lo;
         uint64_t *mm = b.d_meta;
@@ -922,14 +1041,20 @@ static DivansResult encode_host_common(divans_b200_ctx *ctx, size_t n, int raw_m
         int32_t *d_status = reinterpret_cast<int32_t *>(mm + 5 * m);
         uint32_t *d_chosen = reinterpret_cast<uint32_t *>(mm + 6 * m);
         uint64_t *d_cost = mm + 7 * m;
-        DivansResult r = sel ? encode_auto_device_nolock(ctx, m, raw_mode, b.d_in, mm, mm + m, mx, mc, b.d_out, mm + 2 * m, mm + 3 * m,
-                                                         mm + 4 * m, d_status, opts, window, sel->cands, sel->n_cands, d_chosen, d_cost, st)
-                             : encode_device_internal(ctx, m, raw_mode, b.d_in, mm, mm + m, mx, mc, b.d_out, mm + 2 * m, mm + 3 * m,
-                                                      mm + 4 * m, d_status, opts, window, st);
+        DivansResult r = sel && sel->mixmap
+                             ? encode_mixmap_device_nolock(ctx, m, raw_mode, b.d_in, mm, mm + m, mx, mc, b.d_out, mm + 2 * m, mm + 3 * m, mm + 4 * m,
+                                                           d_status, opts, window, sel->cands, sel->n_cands, d_chosen, d_cost, d_mixing, d_bins, st)
+                         : sel ? encode_auto_device_nolock(ctx, m, raw_mode, b.d_in, mm, mm + m, mx, mc, b.d_out, mm + 2 * m, mm + 3 * m,
+                                                           mm + 4 * m, d_status, opts, window, sel->cands, sel->n_cands, d_chosen, d_cost, st)
+                               : encode_device_internal(ctx, m, raw_mode, b.d_in, mm, mm + m, mx, mc, b.d_out, mm + 2 * m, mm + 3 * m,
+                                                        mm + 4 * m, d_status, opts, window, st);
         if (r != DIVANS_SUCCESS) return r;
         if (sel) {
-            CK(cudaMemcpyAsync(sel->chosen + i0, d_chosen, m * 4, cudaMemcpyDeviceToHost, st));
-            if (sel->cost) CK(cudaMemcpyAsync(sel->cost + i0 * sel->n_cands, d_cost, m * (size_t)sel->n_cands * 8, cudaMemcpyDeviceToHost, st));
+            if (sel->chosen) CK(cudaMemcpyAsync(sel->chosen + i0, d_chosen, m * 4, cudaMemcpyDeviceToHost, st));
+            if (sel->cost) CK(cudaMemcpyAsync(sel->cost + i0 * cost_cols, d_cost, m * cost_cols * 8, cudaMemcpyDeviceToHost, st));
+            if (d_mixing) CK(cudaMemcpyAsync(sel->mixing + i0 * (size_t)MIX_ENTRIES, d_mixing, m * (size_t)MIX_ENTRIES, cudaMemcpyDeviceToHost, st));
+            if (d_bins) CK(cudaMemcpyAsync(sel->bins + i0 * (size_t)sel->n_cands * MIX_ENTRIES, d_bins, m * (size_t)sel->n_cands * MIX_ENTRIES * 8,
+                                           cudaMemcpyDeviceToHost, st));
         }
         CK(cudaMemcpyAsync(out_len + i0, mm + 4 * m, m * 8, cudaMemcpyDeviceToHost, st));
         CK(cudaMemcpyAsync(status + i0, d_status, m * 4, cudaMemcpyDeviceToHost, st));
@@ -972,6 +1097,53 @@ extern "C" DivansResult divans_b200_encode_cmds_auto_batch_host(divans_b200_ctx 
                                                                 uint32_t n_cands, uint32_t *chosen, uint64_t *cost) {
     const AutoSel sel = {cands, n_cands, chosen, cost};
     return encode_host_common(ctx, n, 0, blobs, blob_off, blob_len, out, out_off, out_cap, out_len, status, opts, &sel);
+}
+
+// ---- per-context mixing values ----
+extern "C" DivansResult divans_b200_encode_mixmap_batch_host(divans_b200_ctx *ctx, size_t n, const uint8_t *in, const uint64_t *in_off,
+                                                             const uint64_t *in_len, uint8_t *out, const uint64_t *out_off, const uint64_t *out_cap,
+                                                             uint64_t *out_len, int32_t *status, const divans_b200_encode_options *opts,
+                                                             const int32_t *values, uint32_t n_values, uint32_t *chosen, uint8_t *mixing,
+                                                             uint64_t *cost, uint64_t *bins) {
+    divans_b200_literal_model cands[16];
+    if (!ctx || !opts || !mixmap_cands(ctx, values, n_values, opts, cands)) return DIVANS_FAILURE;
+    const AutoSel sel = {cands, n_values, chosen, cost, true, mixing, bins};
+    return encode_host_common(ctx, n, 1, in, in_off, in_len, out, out_off, out_cap, out_len, status, opts, &sel);
+}
+extern "C" DivansResult divans_b200_encode_mixmap_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_in, const uint64_t *d_in_off,
+                                                               const uint64_t *d_in_len, uint64_t max_in_len, uint8_t *d_out,
+                                                               const uint64_t *d_out_off, const uint64_t *d_out_cap, uint64_t *d_out_len,
+                                                               int32_t *d_status, const divans_b200_encode_options *opts, const int32_t *values,
+                                                               uint32_t n_values, uint32_t *d_chosen, uint8_t *d_mixing, uint64_t *d_cost,
+                                                               uint64_t *d_bins, void *cuda_stream) {
+    divans_b200_literal_model cands[16];
+    if (!ctx || !opts || !mixmap_cands(ctx, values, n_values, opts, cands)) return DIVANS_FAILURE;
+    const AutoSel sel = {cands, n_values, d_chosen, d_cost, true, d_mixing, d_bins};
+    return encode_device_common(ctx, n, 1, d_in, d_in_off, d_in_len, max_in_len, max_in_len, d_out, d_out_off, d_out_cap, d_out_len,
+                                d_status, opts, cuda_stream, &sel);
+}
+extern "C" DivansResult divans_b200_encode_cmds_mixmap_batch_host(divans_b200_ctx *ctx, size_t n, const uint8_t *blobs, const uint64_t *blob_off,
+                                                                  const uint64_t *blob_len, uint8_t *out, const uint64_t *out_off,
+                                                                  const uint64_t *out_cap, uint64_t *out_len, int32_t *status,
+                                                                  const divans_b200_encode_options *opts, const int32_t *values, uint32_t n_values,
+                                                                  uint32_t *chosen, uint8_t *mixing, uint64_t *cost, uint64_t *bins) {
+    divans_b200_literal_model cands[16];
+    if (!ctx || !opts || !mixmap_cands(ctx, values, n_values, opts, cands)) return DIVANS_FAILURE;
+    const AutoSel sel = {cands, n_values, chosen, cost, true, mixing, bins};
+    return encode_host_common(ctx, n, 0, blobs, blob_off, blob_len, out, out_off, out_cap, out_len, status, opts, &sel);
+}
+extern "C" DivansResult divans_b200_encode_cmds_mixmap_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_blobs,
+                                                                    const uint64_t *d_blob_off, const uint64_t *d_blob_len,
+                                                                    uint64_t max_blob_len, uint64_t max_raw_len, uint8_t *d_out,
+                                                                    const uint64_t *d_out_off, const uint64_t *d_out_cap, uint64_t *d_out_len,
+                                                                    int32_t *d_status, const divans_b200_encode_options *opts,
+                                                                    const int32_t *values, uint32_t n_values, uint32_t *d_chosen,
+                                                                    uint8_t *d_mixing, uint64_t *d_cost, uint64_t *d_bins, void *cuda_stream) {
+    divans_b200_literal_model cands[16];
+    if (!ctx || !opts || !mixmap_cands(ctx, values, n_values, opts, cands)) return DIVANS_FAILURE;
+    const AutoSel sel = {cands, n_values, d_chosen, d_cost, true, d_mixing, d_bins};
+    return encode_device_common(ctx, n, 0, d_blobs, d_blob_off, d_blob_len, max_blob_len, max_raw_len, d_out, d_out_off, d_out_cap,
+                                d_out_len, d_status, opts, cuda_stream, &sel);
 }
 
 // ---- replaying command lists to raw bytes ----

@@ -181,4 +181,15 @@ struct EncodeParams {
 };
 constexpr uint32_t PM_RECORD_BYTES = 32 + 16384 + 1024 + 8192;
 
+// Binned cost pass (encode_bins_kernel, divans_b200_encode_mixmap_*): the cost-only pass of n x k (stream, candidate) pairs,
+// candidate-major (pair v = c * n + i), that also sums each literal nibble's cost into the bin of its mixing-mask index.
+constexpr uint32_t MIX_ENTRIES = 8192;
+struct BinParams {
+    uint64_t *slot_bins;   // per slot: MIX_ENTRIES u64, cleared when the slot takes a pair
+    uint64_t *best;        // per stream: MIX_ENTRIES packed (cost << 4) | c, atomicMin of every pair that did not fail
+    uint64_t *bins_out;    // optional, per pair (stream i, candidate c) at (i * k + c) * MIX_ENTRIES: the bins; UINT64_MAX for a failed pair
+    uint32_t n, k;
+};
+struct MixValues { uint8_t v[16]; uint32_t k; };   // the k (1..16) candidate mixing values of a mixmap call
+
 }  // namespace dv

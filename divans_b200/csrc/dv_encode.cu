@@ -18,8 +18,23 @@
 
 namespace dv {
 
-template <bool BLEND, bool TALLY>
-__global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) encode_model_kernel(EncodeParams p) {
+// BINS: the end of pair v (status `ok`): fold the slot's bins into stream i's per-entry minimum (cost << 4) | c; a failed pair
+// takes no part and reports UINT64_MAX bins
+__device__ __forceinline__ void fold_bins(const G2 g, const uint64_t *sbins, const BinParams &bp, uint32_t v, bool ok) {
+    const uint32_t i = v % bp.n, c = v / bp.n;
+    __syncwarp(g.gmask);   // the group's store lane added the last nibble
+    for (uint32_t e = (uint32_t)g.l16; e < MIX_ENTRIES; e += 16) {
+        const uint64_t b = ok ? sbins[e] : ~0ull;
+        if (ok) atomicMin(reinterpret_cast<unsigned long long *>(bp.best + (uint64_t)i * MIX_ENTRIES + e), (unsigned long long)((b << 4) | c));
+        if (bp.bins_out) bp.bins_out[((uint64_t)i * bp.k + c) * MIX_ENTRIES + e] = b;
+    }
+}
+
+// BINS (encode_bins_kernel: TALLY as well) adds each coded literal nibble's cost to bin[mixing-mask index] of the slot's bins and
+// folds them into the stream's per-entry minimum when the pair ends.  It codes every literal on the generic path: the fast
+// loops do not track the mixing-mask index.
+template <bool BLEND, bool TALLY, bool BINS>
+__device__ __forceinline__ void encode_model_walk(const EncodeParams &p, const BinParams &bp) {
     extern __shared__ __align__(16) uint8_t smem[];
     const int lane = threadIdx.x & 31;
     const int group_in_block = (threadIdx.x >> 5) * 2 + (lane >> 4);
@@ -51,7 +66,7 @@ __global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) encode_model_kernel(E
     store_default_cdfs(g, reinterpret_cast<int16_t *>(s.slot + OFF_MISC), (uint32_t)MISC_CDFS);
     bool exhausted = false;
     const uint32_t per_stream = p.cmd_cap + p.lit_cap;
-
+    uint64_t *const sbins = BINS ? bp.slot_bins + (uint64_t)slot * MIX_ENTRIES : nullptr;
     for (;;) {
         __syncwarp();
         const bool want = (s.state == S_IDLE) && !exhausted;
@@ -111,7 +126,12 @@ __global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) encode_model_kernel(E
                             p.status[v] = ST_FAIL;
                             if constexpr (TALLY) p.tally[v] = 0; else { p.sf_counts[2 * v] = 0; p.sf_counts[2 * v + 1] = 0; }
                         }
+                        if constexpr (BINS) fold_bins(g, sbins, bp, v, false);
                     } else if constexpr (TALLY) {
+                        if constexpr (BINS) {
+                            for (uint32_t e = (uint32_t)g.l16; e < MIX_ENTRIES; e += 16) sbins[e] = 0;
+                            __syncwarp(g.gmask);
+                        }
                         s.c->ring_len = 1u << win;
                         coder_init_enc(s.cur, dummy_log); coder_init_enc(s.c->oth, dummy_log);   // (a = 0: the stream's cost so far)
                         enter_cmd_type<true>(s, nx);
@@ -131,6 +151,7 @@ __global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) encode_model_kernel(E
         auto finish = [&]() {
             const uint32_t v = s.c->sidx;
             if (g.store0 && TALLY) { p.status[v] = s.status; p.tally[v] = s.cur.a + s.c->oth.a; }
+            if constexpr (BINS) fold_bins(g, sbins, bp, v, s.status == ST_OK);
             if (g.store0 && !TALLY) {
                 p.status[v] = s.status;
                 const uint32_t nc = s.c->cur_is_lit ? s.c->oth.left : s.cur.left, nl = s.c->cur_is_lit ? s.cur.left : s.c->oth.left;
@@ -140,14 +161,22 @@ __global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) encode_model_kernel(E
             nx.cdf = A_misc(s, MI_DUMMY); nx.cdf2 = nullptr; nx.speed = SPK_NONE; nx.tagged = false; nx.sym = 0;
             coder_init_enc(s.cur, dummy_log);
         };
-        if (!BLEND && __all_sync(FULL, s.state == S_LIT_HI)) {
+        if (!BLEND && !BINS && __all_sync(FULL, s.state == S_LIT_HI)) {
             literal_fast_enc<TALLY>(s, nx, g);
             if (s.lit_left == 0 && s.status == ST_OK) { swap_coders(s, g); s.c->in.pos++; enter_cmd_type<true>(s, nx); }
             if (s.status != ST_OK) finish();   // a symbol the loop could not code (enc_log): the stream ends here
             continue;
         }
         const bool busy = s.state != S_IDLE;
+        // BINS: the mixing-mask index of a literal nibble (codec/literal.rs:176-183), and the coder's cost before it
+        bool lit_nib = false; uint32_t mmi = 0; uint64_t a0 = 0;
+        if constexpr (BINS) {
+            lit_nib = s.state == S_LIT_HI || s.state == S_LIT_LO;
+            mmi = s.lit_ctx | (s.state == S_LIT_HI ? (uint32_t)(s.l8 >> 60) << 8 : ((s.lit_h & 0xfu) << 8) | 4096u);
+            a0 = s.cur.a;
+        }
         int sym = core_dispatch<BLEND, TALLY>(s, nx, g);
+        if constexpr (BINS) if (lit_nib && g.store0) sbins[mmi] += s.cur.a - a0;
         if (!busy) s.cur.left = 0;
         else {
             if (s.status == ST_OK) {   // (else the core could not code the symbol: enc_log)
@@ -160,6 +189,15 @@ __global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) encode_model_kernel(E
             if (s.status != ST_OK || s.state == S_IDLE) finish();
         }
     }
+}
+
+template <bool BLEND, bool TALLY>
+__global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) encode_model_kernel(EncodeParams p) {
+    encode_model_walk<BLEND, TALLY, false>(p, BinParams{});
+}
+template <bool BLEND>
+__global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) encode_bins_kernel(EncodeParams p, BinParams b) {
+    encode_model_walk<BLEND, true, true>(p, b);
 }
 
 #ifndef DV_BLEND   // (the rANS / mux passes do not depend on the probability model: they live in the default translation unit)
@@ -410,6 +448,10 @@ void launch_encode_tally_blend(const EncodeParams &p, uint32_t n_blocks, cudaStr
     size_t smem = (size_t)(DECODE_BLOCK_THREADS / 16) * SMEM_BYTES_PER_GROUP;
     encode_model_kernel<true, true><<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p);
 }
+void launch_encode_bins_blend(const EncodeParams &p, const BinParams &b, uint32_t n_blocks, cudaStream_t st) {
+    size_t smem = (size_t)(DECODE_BLOCK_THREADS / 16) * SMEM_BYTES_PER_GROUP;
+    encode_bins_kernel<true><<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p, b);
+}
 #else
 void launch_encode_model(const EncodeParams &p, uint32_t n_blocks, cudaStream_t st) {
     size_t smem = (size_t)(DECODE_BLOCK_THREADS / 16) * SMEM_BYTES_PER_GROUP;
@@ -418,6 +460,67 @@ void launch_encode_model(const EncodeParams &p, uint32_t n_blocks, cudaStream_t 
 void launch_encode_tally(const EncodeParams &p, uint32_t n_blocks, cudaStream_t st) {
     size_t smem = (size_t)(DECODE_BLOCK_THREADS / 16) * SMEM_BYTES_PER_GROUP;
     encode_model_kernel<false, true><<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p);
+}
+void launch_encode_bins(const EncodeParams &p, const BinParams &b, uint32_t n_blocks, cudaStream_t st) {
+    size_t smem = (size_t)(DECODE_BLOCK_THREADS / 16) * SMEM_BYTES_PER_GROUP;
+    encode_bins_kernel<false><<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p, b);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// per-context mixing values (divans_b200_encode_mixmap_*): n streams x k mixing values v[0..k)
+// ---------------------------------------------------------------------------------------------------------------
+// records: [k uniform records R(p, v[c])][n mixed records].  Block i writes stream i's mixed record M_i: R(p, v[0]) with
+// mixing[e] = v[c] for the c packed in best[i][e] (v[0] where no pair folded anything), and mix_idx[i] = k + i, its index.
+__global__ void __launch_bounds__(256) mixmap_map_kernel(const uint64_t *best, MixValues vals, uint8_t *records, uint32_t *mix_idx) {
+    const uint32_t i = blockIdx.x;
+    const uint32_t k = vals.k;
+    uint8_t *rec = records + (uint64_t)(k + i) * PM_RECORD_BYTES;
+    const uint4 *src = reinterpret_cast<const uint4 *>(records);   // R(p, v[0]): header and both maps
+    uint4 *dst = reinterpret_cast<uint4 *>(rec);
+    for (uint32_t j = threadIdx.x; j < (PM_RECORD_BYTES - MIX_ENTRIES) / 16; j += blockDim.x) dst[j] = src[j];
+    const uint64_t *b = best + (uint64_t)i * MIX_ENTRIES;
+    for (uint32_t e = threadIdx.x; e < MIX_ENTRIES; e += blockDim.x) {
+        const uint64_t w = b[e];
+        rec[PM_RECORD_BYTES - MIX_ENTRIES + e] = vals.v[w == ~0ull ? 0u : (uint32_t)(w & 15u)];
+    }
+    if (threadIdx.x == 0) mix_idx[i] = k + i;
+}
+// Block i: c* = argmin of the uniform costs (ties to the lowest c, a failed pass costs UINT64_MAX), x = the mixed pass's
+// cost; the mixed record when x < u[c*] (chosen k, record k + i), else c* (record c*).  cost (optional): row i is u[0..k), x;
+// mixing (optional): the 8192 values of the chosen record.
+__global__ void __launch_bounds__(256) mixmap_select_kernel(const uint64_t *tally, const int32_t *v_status, const uint64_t *x_tally,
+                                                            const int32_t *x_status, uint64_t n, MixValues vals, const uint8_t *records,
+                                                            uint32_t *rec_idx, uint32_t *chosen, uint64_t *cost, uint8_t *mixing) {
+    const uint64_t i = blockIdx.x;
+    const uint32_t k = vals.k;
+    __shared__ uint32_t ch;
+    if (threadIdx.x == 0) {
+        uint64_t best = ~0ull; uint32_t arg = 0;
+        for (uint32_t c = 0; c < k; c++) {
+            const uint64_t v = (uint64_t)c * n + i;
+            const uint64_t t = v_status[v] == ST_OK ? tally[v] : ~0ull;
+            if (cost) cost[i * (k + 1) + c] = t;
+            if (t < best) { best = t; arg = c; }
+        }
+        const uint64_t x = x_status[i] == ST_OK ? x_tally[i] : ~0ull;
+        if (cost) cost[i * (k + 1) + k] = x;
+        const bool mixed = x < best;   // (a tie keeps the uniform record)
+        ch = mixed ? k : arg;
+        rec_idx[i] = mixed ? k + (uint32_t)i : arg;
+        if (chosen) chosen[i] = ch;
+    }
+    __syncthreads();
+    if (!mixing) return;
+    const uint8_t *mx = records + (uint64_t)(k + i) * PM_RECORD_BYTES + (PM_RECORD_BYTES - MIX_ENTRIES);
+    for (uint32_t e = threadIdx.x; e < MIX_ENTRIES; e += blockDim.x) mixing[i * MIX_ENTRIES + e] = ch == k ? mx[e] : vals.v[ch];
+}
+void launch_mixmap_map(const uint64_t *best, uint64_t n, const MixValues &vals, uint8_t *records, uint32_t *mix_idx, cudaStream_t st) {
+    mixmap_map_kernel<<<(unsigned)n, 256, 0, st>>>(best, vals, records, mix_idx);
+}
+void launch_mixmap_select(const uint64_t *tally, const int32_t *v_status, const uint64_t *x_tally, const int32_t *x_status, uint64_t n,
+                          const MixValues &vals, const uint8_t *records, uint32_t *rec_idx, uint32_t *chosen, uint64_t *cost, uint8_t *mixing,
+                          cudaStream_t st) {
+    mixmap_select_kernel<<<(unsigned)n, 256, 0, st>>>(tally, v_status, x_tally, x_status, n, vals, records, rec_idx, chosen, cost, mixing);
 }
 
 // ---------------------------------------------------------------------------------------------------------------

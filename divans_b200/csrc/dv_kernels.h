@@ -36,6 +36,14 @@ void launch_auto_fanout(const uint64_t *in_off, const uint64_t *in_len, uint64_t
                         uint32_t *v_pm, cudaStream_t st);
 void launch_auto_select(const uint64_t *tally, const int32_t *v_status, uint64_t n, uint32_t n_cands, uint32_t *chosen, uint64_t *cost,
                         cudaStream_t st);
+// per-context mixing values: the binned cost pass over the n x k fan-out (BinParams), the kernel that builds each stream's
+// mixed record from the per-entry winners, and the choice between the best uniform record and the mixed one (dv_encode.cu)
+void launch_encode_bins(const EncodeParams &p, const BinParams &b, uint32_t n_blocks, cudaStream_t st);
+void launch_encode_bins_blend(const EncodeParams &p, const BinParams &b, uint32_t n_blocks, cudaStream_t st);
+void launch_mixmap_map(const uint64_t *best, uint64_t n, const MixValues &vals, uint8_t *records, uint32_t *mix_idx, cudaStream_t st);
+void launch_mixmap_select(const uint64_t *tally, const int32_t *v_status, const uint64_t *x_tally, const int32_t *x_status, uint64_t n,
+                          const MixValues &vals, const uint8_t *records, uint32_t *rec_idx, uint32_t *chosen, uint64_t *cost, uint8_t *mixing,
+                          cudaStream_t st);
 // decoding to command lists: the recording decoder (16 lanes per stream, either model) and the pack kernel that finishes the
 // blobs (dv_kernels.cu)
 void launch_decode_v2_rec(bool blend, const DecodeParams &p, const RecParams &r, uint32_t n_blocks, cudaStream_t st);

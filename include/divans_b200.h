@@ -345,6 +345,63 @@ DivansResult divans_b200_encode_cmds_auto_batch_device(divans_b200_ctx *ctx, siz
                                                        const divans_b200_literal_model *cands, uint32_t n_cands, uint32_t *d_chosen,
                                                        uint64_t *d_cost, void *cuda_stream);
 
+/* ---- per-context mixing values ----
+ * A PredictionMode record holds 8192 mixing values; each literal nibble reads the one at its mixing-mask index (the literal's
+ * context byte, the nibble half, and the high nibble of the current or previous byte; codec/literal.rs:176-183).  These calls
+ * choose each stream's values per entry, by coding cost, from k candidate values v[0..k) under the mode p =
+ * opts->literal_pred_mode.  R(p, x) is the raw-buffer record of (p, x) (divans_b200_literal_model).  For stream i:
+ *  1. Uniform passes: the cost walk under R(p, v[c]) gives the total u[i][c] (as encode_auto) and per-entry sums b[i][c][e]:
+ *     the cost of the literal nibbles, of both coders, whose mixing-mask index is e.  Other nibbles count toward the total only.
+ *  2. m[i][e] = argmin over c of b[i][c][e], ties to the lowest c (an entry no literal visits takes v[0]); a failed pass takes no
+ *     part (when all failed, every entry takes v[0]).
+ *  3. Mixed pass: M_i = R(p, v[0]) with mixing[e] = v[m[i][e]]; its cost walk gives x[i].
+ *  4. c* = argmin of u[i][.], ties to the lowest c.  If x[i] < u[i][c*] stream i is encoded under M_i and chosen[i] = k, else
+ *     under R(p, v[c*]) and chosen[i] = c*.  A tie keeps the uniform record, which decodes on the fast literal loop; a mixed
+ *     record decodes on the generic per-nibble path.
+ *  5. A uniform choice gives exactly the bytes, out_len and status of divans_b200_encode_batch_host with literal_mixing_value =
+ *     v[c*]; a mixed one those of divans_b200_encode_cmds_batch_host on the stream's literal-only list with its record replaced
+ *     by M_i.  So no stream costs more than under its best uniform candidate.
+ *  6. A failed pass costs UINT64_MAX, as in encode_auto; status 2 as in encode_auto.
+ * values: 1..16 entries, each 0..15, and opts->literal_pred_mode 0..3; anything else returns DIVANS_FAILURE before any work
+ * (divans_b200_last_error says why).  Outputs, each may be NULL: chosen [n]; mixing [n * 8192], the values of the chosen record;
+ * cost [n * (k + 1)], row i = u[i][0..k) then x[i]; bins [n * k * 8192], b[i][c][e] at (i * k + c) * 8192 + e (UINT64_MAX for a
+ * failed pass).  Costs are in 1/65536 bit (T[freq], as encode_auto).  The encoder codes a record's mixing values only with
+ * opts->use_context_map set and a nonzero dynamic_context_mixing or force_stride (the defaults); otherwise it codes one value
+ * for every entry whatever the record holds, and every candidate costs the same.
+ * The uniform passes run on the generic per-nibble path (their bins need each literal nibble's index), so the call takes
+ * about k + 1 plain encodes and more.  Host calls are sub-batched like divans_b200_encode_auto_batch_host; n == 0 returns
+ * DIVANS_SUCCESS. */
+DivansResult divans_b200_encode_mixmap_batch_host(divans_b200_ctx *ctx, size_t n, const uint8_t *in, const uint64_t *in_off,
+                                                  const uint64_t *in_len, uint8_t *out, const uint64_t *out_off, const uint64_t *out_cap,
+                                                  uint64_t *out_len, int32_t *status, const divans_b200_encode_options *opts,
+                                                  const int32_t *values, uint32_t n_values, uint32_t *chosen, uint8_t *mixing,
+                                                  uint64_t *cost, uint64_t *bins);
+/* Same with the buffers and outputs DEVICE pointers (values is a host array, copied before the call returns); conventions of
+ * divans_b200_encode_auto_batch_device.  It also holds, per slot of the n * k pairs, 64 KiB of bins, and per stream 64 KiB of
+ * per-entry winners and a record. */
+DivansResult divans_b200_encode_mixmap_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_in, const uint64_t *d_in_off,
+                                                    const uint64_t *d_in_len, uint64_t max_in_len, uint8_t *d_out,
+                                                    const uint64_t *d_out_off, const uint64_t *d_out_cap, uint64_t *d_out_len,
+                                                    int32_t *d_status, const divans_b200_encode_options *opts, const int32_t *values,
+                                                    uint32_t n_values, uint32_t *d_chosen, uint8_t *d_mixing, uint64_t *d_cost,
+                                                    uint64_t *d_bins, void *cuda_stream);
+/* The same choice for command lists (DVCL blobs): every PredictionMode record of a list is replaced, by R(p, v[c]) in the
+ * uniform passes and by M_i in the mixed pass, as encode_cmds_auto replaces them; commands, literal pool and window are kept.
+ * Step 5's literal-only list is the list itself with its records replaced.  The log guard of encode_cmds_auto (a pass fails when
+ * the replaced list would outgrow the final encode's logs) applies to all three kinds of pass.  Conventions of
+ * divans_b200_encode_cmds_auto_batch_host / _device. */
+DivansResult divans_b200_encode_cmds_mixmap_batch_host(divans_b200_ctx *ctx, size_t n, const uint8_t *blobs, const uint64_t *blob_off,
+                                                       const uint64_t *blob_len, uint8_t *out, const uint64_t *out_off,
+                                                       const uint64_t *out_cap, uint64_t *out_len, int32_t *status,
+                                                       const divans_b200_encode_options *opts, const int32_t *values, uint32_t n_values,
+                                                       uint32_t *chosen, uint8_t *mixing, uint64_t *cost, uint64_t *bins);
+DivansResult divans_b200_encode_cmds_mixmap_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_blobs, const uint64_t *d_blob_off,
+                                                         const uint64_t *d_blob_len, uint64_t max_blob_len, uint64_t max_raw_len,
+                                                         uint8_t *d_out, const uint64_t *d_out_off, const uint64_t *d_out_cap,
+                                                         uint64_t *d_out_len, int32_t *d_status, const divans_b200_encode_options *opts,
+                                                         const int32_t *values, uint32_t n_values, uint32_t *d_chosen, uint8_t *d_mixing,
+                                                         uint64_t *d_cost, uint64_t *d_bins, void *cuda_stream);
+
 /* ---- replaying command lists to raw bytes ----
  * Realise n command lists (DVCL blobs, below) as the bytes they describe: the reference's `recode` (src/bin/divans.rs:1108,
  * cmd_to_raw/mod.rs) on the GPU.  List i is blobs[blob_off[i] .. +blob_len[i]); its bytes go to out[out_off[i] .. +out_cap[i]).

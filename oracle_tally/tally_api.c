@@ -182,3 +182,113 @@ int dvo_recode_blob(const uint8_t *blob, size_t len, int window, uint8_t *out, s
     free(r.ring);
     return rc;
 }
+
+/* ---- per-context mixing values ----
+ * The CPU reference of divans_b200_encode_mixmap_* / encode_cmds_mixmap_*.  While dvt_bins is set, ans_enc_put adds each
+ * symbol's cost to the total and to bin dvt_bin -- the mixing-mask index code_lit_nibble read for the literal nibble being
+ * coded -- or, for every other nibble (dvt_bin = -1), to *dvt_nobin.  So the bins and the "no bin" counter sum to the total. */
+#define DVT_MIX 8192
+
+/* dvo_tally_cmds with bins[8192] and *nobin (zeroed first) */
+static int dvt_tally_bins(const dvo_cmdlist *l, const dvo_options *o, uint64_t *cost, uint64_t *bins, uint64_t *nobin) {
+    memset(bins, 0, DVT_MIX * sizeof *bins); *nobin = 0;
+    dvt_bins = bins; dvt_nobin = nobin; dvt_bin = -1;
+    int rc = dvo_tally_cmds(l, o, cost);
+    dvt_bins = NULL; dvt_nobin = NULL; dvt_bin = -1;
+    return rc;
+}
+
+/* calls fn on the list with every PredictionMode record replaced by `rec` (a shallow copy; a list without records as given) */
+static int dvt_with_record(const dvo_cmdlist *l, const dvo_predmode *rec, int (*fn)(const dvo_cmdlist *, void *), void *arg) {
+    if (l->n_pms == 0) return fn(l, arg);
+    dvo_cmdlist m = *l;
+    m.pms = (dvo_predmode *)malloc(l->n_pms * sizeof(dvo_predmode));
+    if (!m.pms) return DVO_FAILURE;
+    m.cap_pms = l->n_pms;
+    for (size_t k = 0; k < l->n_pms; k++) m.pms[k] = *rec;
+    int rc = fn(&m, arg);
+    free(m.pms);
+    return rc;
+}
+
+typedef struct { const dvo_options *o; uint64_t *cost, *bins, *nobin; } dvt_bins_call;
+static int dvt_bins_fn(const dvo_cmdlist *l, void *p) { dvt_bins_call *c = (dvt_bins_call *)p; return dvt_tally_bins(l, c->o, c->cost, c->bins, c->nobin); }
+
+int dvo_tally_raw_bins(const uint8_t *in, size_t n, const dvo_options *o, int pred_mode, int mixing_value, uint64_t *cost, uint64_t *bins,
+                       uint64_t *nobin) {
+    dvo_cmdlist l; dvo_cmdlist_init(&l);
+    dvt_raw_cmds(in, n, o->window_size, pred_mode, mixing_value, &l);
+    int rc = dvt_tally_bins(&l, o, cost, bins, nobin);
+    dvo_cmdlist_free(&l);
+    return rc;
+}
+
+int dvo_tally_cmds_bins(const dvo_cmdlist *l, const dvo_options *o, int pred_mode, int mixing_value, uint64_t *cost, uint64_t *bins,
+                        uint64_t *nobin) {
+    dvo_predmode *rec = (dvo_predmode *)malloc(sizeof *rec);
+    if (!rec) return DVO_FAILURE;
+    internal_predmode(rec, pred_mode, mixing_value);
+    dvt_bins_call call = {o, cost, bins, nobin};
+    *cost = UINT64_MAX;
+    int rc = dvt_with_record(l, rec, dvt_bins_fn, &call);
+    free(rec);
+    return rc;
+}
+
+/* The choice of include/divans_b200.h ("per-context mixing values") for the list `l`, every record replaced: uniform passes under
+ * R(pred_mode, values[c]) with bins, the per-entry argmin (ties to the lowest c; failed passes take no part), the mixed pass, and
+ * the encode under R(pred_mode, values[c*]) or M.  Outputs: *chosen (k = mixed), mixing[8192], cost[k + 1], bins[k * 8192]
+ * (UINT64_MAX for a failed pass); each but chosen may be NULL. */
+static int dvt_mixmap(const dvo_cmdlist *l, const dvo_options *o, int pred_mode, const int32_t *values, uint32_t k, uint8_t *out, size_t cap,
+                      size_t *out_len, uint32_t *chosen, uint8_t *mixing, uint64_t *cost, uint64_t *bins) {
+    dvo_predmode *rec = (dvo_predmode *)malloc(sizeof *rec), *mixed = (dvo_predmode *)malloc(sizeof *mixed);
+    uint64_t *b = (uint64_t *)malloc(DVT_MIX * sizeof(uint64_t)), *best = (uint64_t *)malloc(DVT_MIX * sizeof(uint64_t));
+    uint8_t *arg_e = (uint8_t *)calloc(DVT_MIX, 1);
+    int rc = DVO_FAILURE;
+    *out_len = 0;
+    if (!rec || !mixed || !b || !best || !arg_e) goto done;
+    for (uint32_t e = 0; e < DVT_MIX; e++) best[e] = UINT64_MAX;
+    uint64_t u_best = UINT64_MAX; uint32_t arg = 0;
+    for (uint32_t c = 0; c < k; c++) {
+        uint64_t t = UINT64_MAX, nb = 0;
+        internal_predmode(rec, pred_mode, values[c]);
+        dvt_bins_call call = {o, &t, b, &nb};
+        if (dvt_with_record(l, rec, dvt_bins_fn, &call) != DVO_SUCCESS) t = UINT64_MAX;
+        if (cost) cost[c] = t;
+        if (t < u_best) { u_best = t; arg = c; }
+        for (uint32_t e = 0; e < DVT_MIX; e++) {
+            if (t != UINT64_MAX && b[e] < best[e]) { best[e] = b[e]; arg_e[e] = (uint8_t)c; }
+            if (bins) bins[(size_t)c * DVT_MIX + e] = t != UINT64_MAX ? b[e] : UINT64_MAX;
+        }
+    }
+    internal_predmode(mixed, pred_mode, values[0]);
+    for (uint32_t e = 0; e < DVT_MIX; e++) mixed->mixing[e] = (uint8_t)values[arg_e[e]];
+    uint64_t x = UINT64_MAX;
+    dvt_call xc = {o, &x, NULL, 0, NULL};
+    if (dvt_with_record(l, mixed, dvt_tally_fn, &xc) != DVO_SUCCESS) x = UINT64_MAX;
+    if (cost) cost[k] = x;
+    const int use_mixed = x < u_best;   /* a tie keeps the uniform record */
+    *chosen = use_mixed ? k : arg;
+    if (!use_mixed) internal_predmode(rec, pred_mode, values[arg]);
+    const dvo_predmode *fin = use_mixed ? mixed : rec;
+    if (mixing) memcpy(mixing, fin->mixing, DVT_MIX);
+    dvt_call ec = {o, NULL, out, cap, out_len};
+    rc = dvt_with_record(l, fin, dvt_encode_fn, &ec);
+done:
+    free(rec); free(mixed); free(b); free(best); free(arg_e);
+    return rc;
+}
+
+int dvo_encode_mixmap(const uint8_t *in, size_t n, const dvo_options *o, int pred_mode, const int32_t *values, uint32_t k, uint8_t *out,
+                      size_t cap, size_t *out_len, uint32_t *chosen, uint8_t *mixing, uint64_t *cost, uint64_t *bins) {
+    dvo_cmdlist l; dvo_cmdlist_init(&l);
+    dvt_raw_cmds(in, n, o->window_size, pred_mode, values[0], &l);
+    int rc = dvt_mixmap(&l, o, pred_mode, values, k, out, cap, out_len, chosen, mixing, cost, bins);
+    dvo_cmdlist_free(&l);
+    return rc;
+}
+
+int dvo_encode_cmds_mixmap(const dvo_cmdlist *l, const dvo_options *o, int pred_mode, const int32_t *values, uint32_t k, uint8_t *out,
+                           size_t cap, size_t *out_len, uint32_t *chosen, uint8_t *mixing, uint64_t *cost, uint64_t *bins) {
+    return dvt_mixmap(l, o, pred_mode, values, k, out, cap, out_len, chosen, mixing, cost, bins);
+}
