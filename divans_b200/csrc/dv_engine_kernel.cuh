@@ -325,7 +325,12 @@ template <bool ENC> __device__ __forceinline__ void enter_pm_mixval(St &s, Next 
     const uint8_t *const m = A_mix(s);
     const uint32_t prior = mixval_prior(s.f1, s.c->model_rev, [m](uint32_t i) { return (uint32_t)m[i]; });
     int sym = 0;
-    if (ENC) sym = !s.c->desired_do_context_map ? 4 : (!(s.f3 & 1) ? 0 : (int)pm_rec<ENC>(s)[32 + 16384 + 1024 + s.f1]);
+    if (ENC) {
+        sym = !s.c->desired_do_context_map ? 4 : (!(s.f3 & 1) ? 0 : (int)pm_rec<ENC>(s)[32 + 16384 + 1024 + s.f1]);
+        // a record byte above 15 is no nibble: the core would code the frequency of sym & 15 while this stream's own mask keeps
+        // sym, so the stream would decode to other literals.  Refused (status 3; a cost pass: UINT64_MAX)
+        if (sym > 15) { s.status = ST_FAIL; return; }
+    }
     set_next<ENC>(nx, A_misc(s, MI_PRED + PM_MIXING_VALUE + (int)prior), SPK_PLANE, sym);
 }
 template <bool ENC> __device__ __forceinline__ void pm_map_store(St &s, Next &nx, const G2 g, uint32_t val) {
@@ -517,6 +522,7 @@ __device__ __forceinline__ void transition(St &s, Next &nx, const G2 g, int nib)
     // ---- prediction mode ----
     case S_PM_MODE: {
         s.f0 = (uint32_t)nib; s.state = S_PM_MIX;
+        if (ENC && pm_rec<ENC>(s)[1] > 1) { s.status = ST_FAIL; return; }   // is_adv: bit 3 of the nibble below, so 0 or 1
         set_next<ENC>(nx, A_misc(s, MI_PRED + PM_SPEED_PALETTE), SPK_MED, ENC ? (int)(s.c->desired_context_mixing | ((uint32_t)pm_rec<ENC>(s)[1] << 3)) : 0);   // aliases SpeedPalette[0]
     } break;
     case S_PM_MIX: {

@@ -482,6 +482,10 @@ DivansResult divans_b200_lz77_cmds_batch_device(divans_b200_ctx *ctx, size_t n, 
  *                   u16 combined_speed[2][2], u16 lit_map_len, u16 dist_map_len, u8 lit_map[16384], u8 dist_map[1024],
  *                   u8 mixing[8192] }
  *   u8 literal pool[n_literal_bytes]
+ * A record is coded as command-coder nibbles, so the encoders (encode_cmds_*, and encode_cmds_auto_* / transcode with the
+ * LITERAL_MODEL_KEEP candidate) refuse with status 3 a record they code whose is_adv is above 1, or whose mixing values, when
+ * coded (dynamic context mixing or is_adv set, and the context map in use), include one above 15; a cost pass over such a
+ * record costs UINT64_MAX.  pred_mode above 3 and map lengths above 16384 / 1024 are refused the same way.
  */
 
 #ifdef __cplusplus

@@ -102,6 +102,15 @@ int dvo_cmdlist_set_model(dvo_cmdlist *l, int pred_mode, int mixing_value) {
     return DVO_SUCCESS;
 }
 
+/* record k's 8192 mixing values := mixing.  Values above 15 are refused (a mixing value is one nibble of the command coder);
+ * the IR grammar stops at 8, so this is how a test writes values 9..15, or a mask of its own making, into a list */
+int dvo_cmdlist_set_mixing(dvo_cmdlist *l, size_t k, const uint8_t *mixing) {
+    if (k >= l->n_pms) return DVO_FAILURE;
+    for (size_t e = 0; e < 8192; e++) if (mixing[e] > 15) return DVO_FAILURE;
+    memcpy(l->pms[k].mixing, mixing, 8192);
+    return DVO_SUCCESS;
+}
+
 /* calls fn on the list as coded under candidate (pred_mode, mixing_value): a shallow copy whose records are replaced */
 static int dvt_with_model(const dvo_cmdlist *l, int pred_mode, int mixing_value, int (*fn)(const dvo_cmdlist *, void *), void *arg) {
     if (dvt_is_keep(pred_mode, mixing_value) || l->n_pms == 0) return fn(l, arg);
@@ -225,6 +234,7 @@ int dvo_tally_raw_bins(const uint8_t *in, size_t n, const dvo_options *o, int pr
 
 int dvo_tally_cmds_bins(const dvo_cmdlist *l, const dvo_options *o, int pred_mode, int mixing_value, uint64_t *cost, uint64_t *bins,
                         uint64_t *nobin) {
+    if (dvt_is_keep(pred_mode, mixing_value)) { *cost = UINT64_MAX; return dvt_tally_bins(l, o, cost, bins, nobin); }
     dvo_predmode *rec = (dvo_predmode *)malloc(sizeof *rec);
     if (!rec) return DVO_FAILURE;
     internal_predmode(rec, pred_mode, mixing_value);

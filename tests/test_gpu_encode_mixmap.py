@@ -29,17 +29,17 @@ def _check(got, want, name):
     assert rc == st == 0 and out == wout, "%s: stream differs from the oracle's" % name
 
 
-def _host(eng, blobs, opts, cmds):
+def _host(eng, blobs, opts, cmds, values=VALUES):
     buf, off, ln, out, ooff, ocap = C._host_layout(blobs)
     fn = eng.encode_cmds_mixmap_batch_host if cmds else eng.encode_mixmap_batch_host
-    out_len, st, chosen, mixing, cost, bins = fn(buf, off, ln, out, ooff, ocap, opts, VALUES, bins=True)
+    out_len, st, chosen, mixing, cost, bins = fn(buf, off, ln, out, ooff, ocap, opts, values, bins=True)
     return [(int(st[i]), int(out_len[i]), out[int(ooff[i]):int(ooff[i] + out_len[i])].tobytes(), int(chosen[i]), mixing[i], cost[i],
              bins[i]) for i in range(len(blobs))]
 
 
-def _device(eng, blobs, opts, cmds):
+def _device(eng, blobs, opts, cmds, values=VALUES):
     import torch
-    n = len(blobs)
+    n, k = len(blobs), len(values)
     buf, off, ln, out, ooff, ocap = C._host_layout(blobs)
     dev = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()
     i64 = lambda a: dev(np.asarray(a, np.uint64).view(np.int64))
@@ -47,9 +47,9 @@ def _device(eng, blobs, opts, cmds):
     d_olen, d_st = torch.zeros(n, dtype=torch.int64, device="cuda"), torch.full((n,), -1, dtype=torch.int32, device="cuda")
     d_ch = torch.zeros(n, dtype=torch.int32, device="cuda")
     d_mix = torch.zeros(n * 8192, dtype=torch.uint8, device="cuda")
-    d_cost = torch.zeros(n * (K + 1), dtype=torch.int64, device="cuda")
-    d_bins = torch.zeros(n * K * 8192, dtype=torch.int64, device="cuda")
-    outs = dict(d_chosen=d_ch.data_ptr(), d_mixing=d_mix.data_ptr(), d_cost=d_cost.data_ptr(), d_bins=d_bins.data_ptr(), opts=opts, values=VALUES)
+    d_cost = torch.zeros(n * (k + 1), dtype=torch.int64, device="cuda")
+    d_bins = torch.zeros(n * k * 8192, dtype=torch.int64, device="cuda")
+    outs = dict(d_chosen=d_ch.data_ptr(), d_mixing=d_mix.data_ptr(), d_cost=d_cost.data_ptr(), d_bins=d_bins.data_ptr(), opts=opts, values=values)
     if cmds:
         eng.encode_cmds_mixmap_batch_device(n, d_in.data_ptr(), d_off.data_ptr(), d_len.data_ptr(), int(ln.max()),
                                             max(C._replay_len(b) for b in blobs) + 1, d_out.data_ptr(), d_ooff.data_ptr(), d_ocap.data_ptr(),
@@ -59,8 +59,8 @@ def _device(eng, blobs, opts, cmds):
                                        d_ooff.data_ptr(), d_ocap.data_ptr(), d_olen.data_ptr(), d_st.data_ptr(), **outs)
     eng.synchronize()
     o, olen, st = d_out.cpu().numpy(), d_olen.cpu().numpy(), d_st.cpu().numpy()
-    mix, cost = d_mix.cpu().numpy().reshape(n, 8192), d_cost.cpu().numpy().view(np.uint64).reshape(n, K + 1)
-    bins = d_bins.cpu().numpy().view(np.uint64).reshape(n, K, 8192)
+    mix, cost = d_mix.cpu().numpy().reshape(n, 8192), d_cost.cpu().numpy().view(np.uint64).reshape(n, k + 1)
+    bins = d_bins.cpu().numpy().view(np.uint64).reshape(n, k, 8192)
     ch = d_ch.cpu().numpy()
     return [(int(st[i]), int(olen[i]), o[int(ooff[i]):int(ooff[i] + olen[i])].tobytes(), int(ch[i]), mix[i], cost[i], bins[i])
             for i in range(n)]
