@@ -202,7 +202,7 @@ extern "C" void divans_b200_destroy(divans_b200_ctx *ctx) {
     delete ctx;
 }
 // bumped whenever a decode kernel changes: bench.py quotes a stored DRAM-traffic capture (profiles/traffic.json) only for the version it measured
-#define DV_KERNEL_VERSION "r2.20-lean-literal-loop"
+#define DV_KERNEL_VERSION "r2.21-count-shift-mod-32"
 extern "C" const char *divans_b200_kernel_version(void) { return DV_KERNEL_VERSION; }
 extern "C" const char *divans_b200_last_error(divans_b200_ctx *ctx) { return ctx ? ctx->err.c_str() : "null context"; }
 extern "C" int divans_b200_last_lanes(divans_b200_ctx *ctx) { return ctx ? ctx->last_lanes : 0; }

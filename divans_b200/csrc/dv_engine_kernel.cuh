@@ -31,8 +31,12 @@ __device__ __forceinline__ void enter_cmd_type(St &s, Next &nx) {
     s.state = S_CMD_TYPE;
     nx.cdf = A_misc(s, MI_CC + (int)(s.c->last_4_states >> 4)); nx.cdf2 = nullptr; nx.speed = SPK_ROCKET; nx.tagged = false;
     if (ENC) {
-        if (s.c->in.pos < s.c->in.n_cmds) nx.sym = load_cmd<ENC>(s);
-        else nx.sym = 0xf;   // end of stream nibble (codec/mod.rs:143-148, flush :424-455)
+        if (s.c->in.pos < s.c->in.n_cmds) {
+            nx.sym = load_cmd<ENC>(s);
+            // a record type outside 1..7 is no command: 15 would end the stream here with status 0, 0 and 8..14 would fail it
+            // one nibble later, and 16 and above are no nibble.  Refused before it is coded (status 3; a cost pass: UINT64_MAX)
+            if ((uint32_t)nx.sym - 1u > 6u) s.status = ST_FAIL;
+        } else nx.sym = 0xf;   // end of stream nibble (codec/mod.rs:143-148, flush :424-455)
     }
 }
 
@@ -219,6 +223,8 @@ template <bool ENC> __device__ __forceinline__ void enter_ll_count_small(St &s, 
     uint32_t lm1 = s.c->e1 - 1u;
     int sym = (int)(lm1 < 14 ? lm1 : 14);
     if (ENC && s.c->e2 && !s.f3) sym = 15;   // high_entropy flag nibble (literal.rs:569-571)
+    // lengths 1 .. 2^30 + 14 only: length 0 would code as 2^15 and more, and past 2^30 + 14 SizeLastNib is no nibble
+    if (ENC && lm1 >= (1u << 30) + 14u) { s.status = ST_FAIL; return; }
     set_next<ENC>(nx, ctype_slab(s, g, BL(s, 1, 0)) + CT_LL_COUNT_SMALL * 16, SPK_MED, sym);
 }
 template <bool ENC> __device__ __forceinline__ void enter_ll_mant(St &s, Next &nx, const G2 g) {
@@ -235,7 +241,7 @@ template <bool ENC> __device__ __forceinline__ void enter_cp_count_small(St &s, 
 template <bool ENC> __device__ __forceinline__ void enter_cp_count_mant(St &s, Next &nx, const G2 g) {
     s.state = S_CP_COUNT_MANT;
     uint32_t index2 = s.f2 == 0 ? ((s.c->last_clen % 4) + 1) : 0u;
-    int sym = (int)(((s.c->e1 ^ s.f0) >> (s.f1 - 4)) & 0xf);
+    int sym = (int)(((s.c->e1 ^ s.f0) >> ((s.f1 - 4) & 31)) & 0xf);
     set_next<ENC>(nx, ctype_slab(s, g, BL(s, 1, 0)) + (CT_CP_COUNT_MANT + index2) * 16, SPK_SLOW, sym);
 }
 template <bool ENC> __device__ __forceinline__ void enter_cp_mnemonic(St &s, Next &nx, const G2 g) {
@@ -266,7 +272,9 @@ template <bool ENC> __device__ __forceinline__ void enter_bt_mnemonic(St &s, Nex
     s.state = S_BT_MNEMONIC; s.f0 = (uint32_t)which;
     int varint = 0;
     if (ENC) {
-        uint32_t bt = s.c->e0 & 0xff;
+        // a type above 255, or a literal switch's stride above 15 taken from the record, is no nibble pair: refused
+        if (s.c->e0 > 255u || (which == 0 && s.c->desired_force_stride == 9 && s.c->e1 > 15u)) { s.status = ST_FAIL; return; }
+        uint32_t bt = s.c->e0;
         if (bt == BL(s, which, 1)) varint = 0;
         else if (bt == ((BMAX(s, which) + 1) & 0xff)) varint = 1;
         else if (bt <= 12) varint = (int)bt + 2;
@@ -406,9 +414,14 @@ __device__ __forceinline__ void transition(St &s, Next &nx, const G2 g, int nib)
     switch (s.state) {
     case S_CMD_TYPE: {
         if (nib == 0xf) { s.state = S_IDLE; return; }   // end of stream (trailer/CRC: frame kernel); the main loop parks the group
-        if (nib == 1) { s.c->last_4_states = (s.c->last_4_states >> 2) | 64; if (ENC && s.c->e0 == 0) { s.status = ST_FAIL; return; } enter_cp_count_small<ENC>(s, nx, g); }
-        else if (nib == 2) {
+        if (nib == 1) {
+            s.c->last_4_states = (s.c->last_4_states >> 2) | 64;
+            if (ENC && s.c->e0 - 1u >= (1u << 30) - 1u) { s.status = ST_FAIL; return; }   // distance 1 .. 2^30 - 1: DistanceLastNib is a nibble
+            enter_cp_count_small<ENC>(s, nx, g);
+        } else if (nib == 2) {
             s.c->last_4_states = (s.c->last_4_states >> 2) | 192; s.state = S_DC_SIZE_BEG;
+            // word size 4..24, word id below 2^round_up_mod_4(bits), transform below 256: else a nibble would drop bits
+            if (ENC && (s.c->e1 - 4u > 20u || s.c->e2 > 255u || (s.c->e0 >> round_up_mod_4(s.tables[TB_SIZE_BITS + s.c->e1])) != 0)) { s.status = ST_FAIL; return; }
             set_next<ENC>(nx, ctype_slab(s, g, BL(s, 1, 0)) + CT_DC_SIZE_BEG * 16, SPK_MUD, (int)min(15u, (s.c->e1 - 4u) & 0xffu));
         } else if (nib == 3) { s.c->last_4_states = (s.c->last_4_states >> 2) | 128; s.f3 = 0; if (!ENC) s.c->e1 = 0; enter_ll_count_small<ENC>(s, nx, g); }
         else if (nib == 4) enter_bt_mnemonic<ENC>(s, nx, 0);
@@ -469,12 +482,14 @@ __device__ __forceinline__ void transition(St &s, Next &nx, const G2 g, int nib)
         else { s.c->last_clen = (uint32_t)nib + 4; s.f1 = round_up_mod_4((uint32_t)nib + 3); s.f0 = 1u << (nib + 3); s.f2 = 0; enter_cp_count_mant<ENC>(s, nx, g); }
     } break;
     case S_CP_COUNT_LAST: {
-        s.c->last_clen = (uint32_t)nib + 19; s.f1 = round_up_mod_4((uint32_t)nib + 18); s.f0 = (nib + 18) < 32 ? (1u << (nib + 18)) : 0u; s.f2 = 0;
+        // nibbles 14 and 15 (decoder only: no u32 count needs them) shift by 32 and 33 here and by 32 in the first mantissa
+        // step: every shift count is taken mod 32, as the reference's release build does (copy.rs:136,148; DESIGN.md section 2)
+        s.c->last_clen = (uint32_t)nib + 19; s.f1 = round_up_mod_4((uint32_t)nib + 18); s.f0 = 1u << ((nib + 18) & 31); s.f2 = 0;
         enter_cp_count_mant<ENC>(s, nx, g);
     } break;
     case S_CP_COUNT_MANT: {
         uint32_t next_rem = s.f1 - 4;
-        s.f0 |= (uint32_t)nib << next_rem;
+        s.f0 |= (uint32_t)nib << (next_rem & 31);
         if (next_rem == 0) enter_cp_mnemonic<ENC>(s, nx, g);
         else { s.f1 = next_rem; s.f2 += 4; enter_cp_count_mant<ENC>(s, nx, g); }
     } break;

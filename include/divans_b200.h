@@ -485,7 +485,15 @@ DivansResult divans_b200_lz77_cmds_batch_device(divans_b200_ctx *ctx, size_t n, 
  * A record is coded as command-coder nibbles, so the encoders (encode_cmds_*, and encode_cmds_auto_* / transcode with the
  * LITERAL_MODEL_KEEP candidate) refuse with status 3 a record they code whose is_adv is above 1, or whose mixing values, when
  * coded (dynamic context mixing or is_adv set, and the context map in use), include one above 15; a cost pass over such a
- * record costs UINT64_MAX.  pred_mode above 3 and map lengths above 16384 / 1024 are refused the same way.
+ * record costs UINT64_MAX.  pred_mode above 3 and map lengths above 16384 / 1024 are refused the same way.  So is every other
+ * record whose fields no sequence of nibbles carries (status 3, a cost pass UINT64_MAX, where the first nibble that cannot
+ * carry the value would be built; the stream's bytes are never written): a type outside 1..7 (15 would end
+ * the stream early), a copy distance of 0 or of 2^30 and more, a literal length of 0 or above 2^30 + 14, a dictionary word
+ * size outside 4..24, a word id of 2^round_up_mod_4(bits of the size) or more, or a transform above 255, a block type above
+ * 255, and a literal block switch's stride above 15 when the stride is taken from the record (force_stride 9).  Other values
+ * the stream carries but the decoder rejects (a distance past the window, a transform 121..255, a word id past the
+ * dictionary) fail the encode with status 3 where the decoder would fail.  The fields no nibble codes (a dictionary record's
+ * d, a copy's c and d, a block switch's c and d) are not read.
  */
 
 #ifdef __cplusplus

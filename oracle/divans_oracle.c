@@ -850,7 +850,9 @@ static int code_copy(codec *s, uint32_t *dist_io, uint32_t *num_io) {
                 last = code_and_blend(&s->cmd, last, P(s->copy_priors, T_CP, CP_CountLastNib, ctype, 0, 0), SPEED_FAST);
                 s->last_clen = (uint8_t)(last + 19);
                 len_remaining = round_up_mod_4((uint8_t)(last + 18));
-                decoded = (last + 18) < 32 ? (1u << (last + 18)) : 0;
+                /* last 14 / 15 (decoder only: no u32 count needs them) shift by 32 and 33 here and by 32 in the first mantissa
+                 * step: every shift count is taken mod 32, as the reference's release build does (copy.rs:136,148) */
+                decoded = 1u << ((last + 18) & 31);
             } else {
                 s->last_clen = (uint8_t)(beg + 4);
                 len_remaining = round_up_mod_4((uint8_t)(beg + 4 - 1));
@@ -859,10 +861,10 @@ static int code_copy(codec *s, uint32_t *dist_io, uint32_t *num_io) {
             uint8_t len_decoded = 0;
             for (;;) {
                 uint8_t next_rem = (uint8_t)(len_remaining - 4);
-                uint8_t nb = (uint8_t)((in_num ^ decoded) >> next_rem);
+                uint8_t nb = (uint8_t)((in_num ^ decoded) >> (next_rem & 31));
                 uint32_t index2 = len_decoded == 0 ? (uint32_t)((s->last_clen % 4) + 1) : 0u;
                 nb = code_and_blend(&s->cmd, nb, P(s->copy_priors, T_CP, CP_CountMantissaNib, ctype, index2, 0), SPEED_SLOW);
-                decoded |= (uint32_t)nb << next_rem;
+                decoded |= (uint32_t)nb << (next_rem & 31);
                 if (next_rem == 0) break;
                 len_decoded = (uint8_t)(len_decoded + 4); len_remaining = next_rem;
             }
@@ -1089,6 +1091,7 @@ static int code_predmode(codec *s, const dvo_predmode *in) {
         else if (!s->desired_do_context_map) mv = 4;
         else if (!combine) mv = 0;
         else mv = in ? in->mixing[index] : 0;
+        if (mv > 15) return DVO_FAILURE; /* no nibble: the record is refused (record_representable) */
         /* context_map.rs:395-399; DVO_MODEL_WASM_2018: one prior (slot 16) for every mixing value */
         uint32_t prior = (index >= 256 && s->model_rev != DVO_MODEL_WASM_2018) ? (uint32_t)(s->pm_mixing[index - 256] & 0xf) : 16u;
         mv = code_and_blend(&s->cmd, mv, P(s->pred_priors, T_PM, PM_PriorMixingValue, prior, 0, 0), SPEED_PLANE);
@@ -1309,6 +1312,26 @@ void dvo_options_default(dvo_options *o) {
     memset(o, 0, sizeof *o);
     o->window_size = 22; o->dynamic_context_mixing = 0; o->prior_depth = 0; o->use_context_map = 1; o->force_stride = 9;
 }
+/* Whether a stream can carry record c: every nibble the encoder would build from it is a nibble (0..15) that decodes back to
+ * the record's value.  A record that fails this is refused before its type nibble is coded (include/divans_b200.h, DVCL):
+ *  - type 1..7 (15 would end the stream, 0 and 8..14 fail the decode);
+ *  - copy: distance 1 .. 2^30 - 1 (DistanceLastNib = bit length - 15 must be a nibble);
+ *  - literal: length 1 .. 2^30 + 14 (length 0 codes as 2^15 and more; SizeLastNib = bit length of length - 15, minus 15);
+ *  - dictionary: word size 4..24, word id below 2^round_up_mod_4(bits of the size), transform below 256 (121..255 are
+ *    carried and fail the decode, DictTransformIndexUndefined);
+ *  - block switch: type below 256, and a literal block switch's stride below 16 when the stride comes from the record;
+ *  - PredictionMode: pred_mode below 16 (4..15 are carried and fail the decode), is_adv 0 or 1; mixing values: code_predmode. */
+static int record_representable(const codec *s, const dvo_cmdlist *l, const dvo_cmd *c) {
+    switch (c->type) {
+    case DVO_CMD_COPY: return c->a != 0 && c->a < (1u << 30);
+    case DVO_CMD_LITERAL: return c->b - 1u < (1u << 30) + 14u;
+    case DVO_CMD_DICT: return c->b >= 4 && c->b <= 24 && c->c < 256 && (c->a >> round_up_mod_4(TB_SIZE_BITS[c->b])) == 0;
+    case DVO_CMD_BTYPE_L: return c->a < 256 && (s->desired_force_stride != 9 || c->b < 16);
+    case DVO_CMD_BTYPE_C: case DVO_CMD_BTYPE_D: return c->a < 256;
+    case DVO_CMD_PREDMODE: return c->a < l->n_pms && l->pms[c->a].pred_mode < 16 && l->pms[c->a].is_adv < 2;
+    default: return 0;
+    }
+}
 int dvo_encode_cmds(const dvo_cmdlist *l, const dvo_options *o, uint8_t *out, size_t cap, size_t *out_len) {
     int window = o->window_size < 10 ? 10 : (o->window_size > 24 ? 24 : o->window_size);
     codec *s = (codec *)malloc(sizeof(codec));
@@ -1326,6 +1349,7 @@ int dvo_encode_cmds(const dvo_cmdlist *l, const dvo_options *o, uint8_t *out, si
     uint8_t *scratch = NULL; size_t scratch_cap = 0;
     for (size_t ci = 0; ci < l->n_cmds && rc == DVO_SUCCESS; ci++) {
         const dvo_cmd *c = &l->cmds[ci];
+        if (!record_representable(s, l, c)) { rc = DVO_FAILURE; break; }
         code_and_blend(&s->cmd, (uint8_t)c->type, P(s->cc_priors, T_CC, CC_FullSelection, (uint32_t)s->last_4_states >> 4, 0, 0), SPEED_ROCKET);
         switch (c->type) {
         case DVO_CMD_COPY: {

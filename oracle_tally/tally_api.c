@@ -302,3 +302,98 @@ int dvo_encode_cmds_mixmap(const dvo_cmdlist *l, const dvo_options *o, int pred_
                            size_t cap, size_t *out_len, uint32_t *chosen, uint8_t *mixing, uint64_t *cost, uint64_t *bins) {
     return dvt_mixmap(l, o, pred_mode, values, k, out, cap, out_len, chosen, mixing, cost, bins);
 }
+
+/* ---- command lists from DVCL blobs, and forged command nibbles ----
+ * dvo_cmdlist_from_blob: the list a DVCL blob (include/divans_b200.h) holds, every field as it is, so that a test can hand the
+ * oracle's encoder records the IR grammar cannot write (a word size of 3, a transform of 300, a type of 15).  FAILURE for a
+ * blob whose header, records or pool do not fit, or a literal outside the pool (the encoder reads the pool unchecked).
+ *
+ * dvo_encode_cmds_forged: dvo_encode_cmds with command nibble at[i] (0 = the first command nibble) replaced by val[i]; the
+ * hook in code_and_blend makes the replacement, so the encoder follows the forged nibble exactly as a decoder does, and every
+ * nibble the walk builds after a forged one is taken mod 16.  A walk that fails after a forged nibble ends the stream there:
+ * both coders are flushed, and the mux and the trailer written, so the stream is CRC-valid and fails at that nibble.
+ * *n_nibbles: the command nibbles coded, the end-of-stream nibble included. */
+static __thread size_t dvt_forge_i, dvt_forge_cnt;
+static __thread const uint32_t *dvt_forge_at;
+static __thread const uint8_t *dvt_forge_val;
+
+static uint8_t dvt_forge_nib(uint8_t nib) {
+    size_t i = dvt_forge_i++;
+    for (size_t k = 0; k < dvt_forge_cnt; k++)
+        if (dvt_forge_at[k] == i) { dvt_forge_hit = 1; return dvt_forge_val[k]; }
+    return dvt_forge_hit ? (uint8_t)(nib & 15) : nib;
+}
+
+int dvo_cmdlist_from_blob(const uint8_t *b, size_t len, dvo_cmdlist *l) {
+    uint32_t h[8];
+    if (len < 32) return DVO_FAILURE;
+    memcpy(h, b, 32);
+    const uint64_t lit_base = 32ull + 20ull * h[2] + (uint64_t)DVT_PM_RECORD_BYTES * h[3];
+    if (h[0] != 0x4c435644u || h[1] != 1u || lit_base + h[4] > len) return DVO_FAILURE;
+    for (uint32_t i = 0; i < h[2]; i++) {
+        uint32_t r[5];
+        memcpy(r, b + 32 + 20ull * i, 20);
+        if (r[0] == DVO_CMD_LITERAL && (uint64_t)r[1] + r[2] > h[4]) return DVO_FAILURE;
+        dvo_cmd *c = cl_add(l); c->type = r[0]; c->a = r[1]; c->b = r[2]; c->c = r[3]; c->d = r[4];
+    }
+    for (uint32_t k = 0; k < h[3]; k++) {
+        const uint8_t *p = b + 32 + 20ull * h[2] + (uint64_t)DVT_PM_RECORD_BYTES * k;
+        dvo_predmode *m = cl_add_pm(l);
+        memset(m, 0, sizeof *m);
+        m->pred_mode = p[0]; m->is_adv = p[1]; m->has_speeds = p[2];
+        uint16_t sp[12]; memcpy(sp, p + 4, 24);
+        for (int i = 0; i < 2; i++) for (int j = 0; j < 2; j++) {
+            m->cm_speed[i][j] = sp[i * 2 + j]; m->stride_speed[i][j] = sp[4 + i * 2 + j]; m->combined_speed[i][j] = sp[8 + i * 2 + j];
+        }
+        uint16_t ll, dl; memcpy(&ll, p + 28, 2); memcpy(&dl, p + 30, 2);
+        m->lit_map_len = ll; m->dist_map_len = dl;
+        memcpy(m->lit_map, p + 32, 16384); memcpy(m->dist_map, p + 32 + 16384, 1024); memcpy(m->mixing, p + 32 + 16384 + 1024, 8192);
+    }
+    if (h[4]) cl_add_lit(l, b + lit_base, h[4]);
+    l->window = (int)h[5];
+    return DVO_SUCCESS;
+}
+
+int dvo_encode_cmds_forged(const dvo_cmdlist *l, const dvo_options *o, const uint32_t *at, const uint8_t *val, size_t n, uint8_t *out,
+                           size_t cap, size_t *out_len, uint64_t *n_nibbles) {
+    dvt_forge_i = 0; dvt_forge_cnt = n; dvt_forge_hit = 0; dvt_forge_at = at; dvt_forge_val = val;
+    dvt_forging = 1;
+    *out_len = 0;
+    int rc = dvo_encode_cmds(l, o, out, cap, out_len);
+    dvt_forging = 0;
+    *n_nibbles = dvt_forge_i;
+    return rc;
+}
+
+/* ---- coverage ----
+ * dvo_encode_cmds_cov: dvo_encode_cmds into a scratch buffer with every command nibble counted in cov[flat * 16 + nibble], where
+ * flat is the prior's index in the concatenation of the codec's command prior tables (CC, LL, CP, DC, BT, PM: the layout of
+ * PRIOR_TABLES in tally_py.py, whose total dvo_cov_size returns). */
+size_t dvo_cov_size(void) {
+    return prior_total(T_CC, NEL(T_CC)) + prior_total(T_LL, NEL(T_LL)) + prior_total(T_CP, NEL(T_CP)) + prior_total(T_DC, NEL(T_DC)) +
+           prior_total(T_BT, NEL(T_BT)) + prior_total(T_PM, NEL(T_PM));
+}
+
+static void dvt_cov_add(const void *cdf, uint8_t nib) {
+    const codec *s = (const codec *)dvt_codec;
+    const dvo_cdf16 *p = (const dvo_cdf16 *)cdf;
+    const dvo_cdf16 *base[6] = {s->cc_priors, s->lit_len_priors, s->copy_priors, s->dict_priors, s->btype_priors, s->pred_priors};
+    const size_t n[6] = {prior_total(T_CC, NEL(T_CC)), prior_total(T_LL, NEL(T_LL)), prior_total(T_CP, NEL(T_CP)),
+                         prior_total(T_DC, NEL(T_DC)), prior_total(T_BT, NEL(T_BT)), prior_total(T_PM, NEL(T_PM))};
+    size_t off = 0;
+    for (int t = 0; t < 6; t++) {
+        if (p >= base[t] && p < base[t] + n[t]) { dvt_cov[(off + (size_t)(p - base[t])) * 16 + (nib & 15)]++; return; }
+        off += n[t];
+    }
+}
+
+int dvo_encode_cmds_cov(const dvo_cmdlist *l, const dvo_options *o, uint32_t *cov) {
+    size_t cap = l->n_lits * 2 + l->n_cmds * 16 + ((size_t)1 << 20), n = 0;
+    uint8_t *out = (uint8_t *)malloc(cap);
+    if (!out) return DVO_FAILURE;
+    dvt_cov = cov;
+    int rc = dvo_encode_cmds(l, o, out, cap, &n);
+    dvt_cov = NULL;
+    free(out);
+    return rc;
+}

@@ -5,9 +5,12 @@ TEST INFRASTRUCTURE: imported only by tests/ and tools/.  Nothing under divans_b
 build() writes oracle_tally/_build/divans_oracle_tally.c: oracle/divans_oracle.c (read, never modified) with one hook in
 ans_enc_put -- while a tally is running, each symbol adds the cost of its frequency to the tally instead of being recorded --
 and a second one at the literal nibble's mixing-mask read -- the index becomes the bin of that nibble's cost --
+and three forging hooks -- every command nibble the encoder codes passes through dvt_forge_nib, a command-type nibble other than
+the record's type ends the walk, and a walk that fails after a forged nibble is still flushed and framed --
 followed by tally_api.c, and compiles it twice, with the reference's default probability model and with feature="blend", as
-the oracle's own Makefile does.  Every function of the oracle is in these libraries unchanged; only the tally entry points,
-dvo_cmdlist_set_mixing (a test's own mixing values in a list) and dvo_recode_blob (the CPU reference of the library's command-list replay, on the serialised blob) are new.
+the oracle's own Makefile does.  Every function of the oracle is in these libraries unchanged while no forged encode runs; only
+the tally entry points, dvo_cmdlist_set_mixing (a test's own mixing values in a list), dvo_recode_blob (the CPU reference of
+the library's command-list replay, on the serialised blob), dvo_cmdlist_from_blob and dvo_encode_cmds_forged are new.
 """
 import ctypes
 import os
@@ -38,12 +41,46 @@ _PUT_TALLIED = _PUT + ("    if (dvt_tally) {   /* (oracle_tally) */\n"
 # the second hook: a literal nibble's mixing-mask index becomes the bin of the nibble coded next (ans_enc_put clears it)
 _MM = "    uint8_t mm_opts = s->mixing_mask[mmi];\n"
 _MM_TALLIED = _MM + "    dvt_bin = (int32_t)mmi;   /* (oracle_tally) */\n"
+# the forging hooks (dvo_encode_cmds_forged): every command nibble passes through dvt_forge_nib; the command-type nibble the
+# encoder codes must be the record's type, or the walk fails; and a walk that fails after a forged nibble is flushed and framed
+_CAB = ("static inline uint8_t code_and_blend(coder *k, uint8_t nib, dvo_cdf16 *cdf, dvo_speed sp) {\n"
+        "    nib = code_nibble(k, nib, cdf, NULL);\n")
+_CAB_FORGED = ("static inline uint8_t code_and_blend(coder *k, uint8_t nib, dvo_cdf16 *cdf, dvo_speed sp) {\n"
+               "    if (k->encoding && dvt_forging) nib = dvt_forge_nib(nib);   /* (oracle_tally) */\n"
+               "    nib = code_nibble(k, nib, cdf, NULL);\n"
+               "    if (k->encoding && dvt_cov) dvt_cov_add(cdf, nib);   /* (oracle_tally) coverage */\n")
+# the coverage hook: the encoder's codec, so that a prior pointer maps back to its table and flat index
+_INIT = "    codec_init(s, window, 1);\n"
+_INIT_COV = _INIT + "    dvt_codec = s;   /* (oracle_tally) */\n"
+_TYPE = ("        code_and_blend(&s->cmd, (uint8_t)c->type, P(s->cc_priors, T_CC, CC_FullSelection, (uint32_t)s->last_4_states >> 4, 0, 0), SPEED_ROCKET);\n"
+         "        switch (c->type) {\n")
+_TYPE_FORGED = ("        if (code_and_blend(&s->cmd, (uint8_t)c->type, P(s->cc_priors, T_CC, CC_FullSelection, (uint32_t)s->last_4_states >> 4, 0, 0), SPEED_ROCKET) != c->type) {\n"
+                "            rc = DVO_FAILURE; break;   /* (oracle_tally) a forged command type: the walk ends */\n"
+                "        }\n"
+                "        switch (c->type) {\n")
+_FLUSH = ("    if (rc == DVO_SUCCESS) {\n"
+          "        /* flush: end-of-stream nibble 0xf, close both coders, drain mux, EOF marker, trailer (codec/mod.rs:424-560) */\n"
+          "        code_and_blend(&s->cmd, 0xf, P(s->cc_priors, T_CC, CC_FullSelection, (uint32_t)s->last_4_states >> 4, 0, 0), SPEED_ROCKET);\n")
+_FLUSH_FORGED = ("    const int dvt_cut = rc != DVO_SUCCESS && dvt_forging && dvt_forge_hit;   /* (oracle_tally) failed after a forged nibble */\n"
+                 "    if (rc == DVO_SUCCESS || dvt_cut) {\n"
+                 "        /* flush: end-of-stream nibble 0xf, close both coders, drain mux, EOF marker, trailer (codec/mod.rs:424-560) */\n"
+                 "        if (!dvt_cut) code_and_blend(&s->cmd, 0xf, P(s->cc_priors, T_CC, CC_FullSelection, (uint32_t)s->last_4_states >> 4, 0, 0), SPEED_ROCKET);\n")
+# a forged literal length never reads past the list's pool: the walk fails there instead (and the stream is cut)
+_LIT = "            memcpy(scratch, l->lits + c->a, len);\n"
+_LIT_FORGED = ("            if (dvt_forging && (uint64_t)c->a + len > l->n_lits) { rc = DVO_FAILURE; break; }   /* (oracle_tally) */\n"
+               + _LIT)
 _PREFIX = ("/* generated by oracle_tally/tally_py.py from oracle/divans_oracle.c and oracle_tally/tally_api.c: do not edit */\n"
            "#include <stdint.h>\n"
            "static __thread uint64_t *dvt_tally;   /* set: the encoder's symbols are costed, not coded */\n"
            "static __thread uint64_t *dvt_bins, *dvt_nobin;   /* set: each cost also goes to bin dvt_bin, or to *dvt_nobin */\n"
            "static __thread int32_t dvt_bin = -1;   /* the mixing-mask index of the literal nibble being coded, or -1 */\n"
            "static uint32_t dvt_freq_cost(uint32_t f);\n"
+           "static __thread int dvt_forging;   /* set: dvo_encode_cmds_forged is running */\n"
+           "static __thread int dvt_forge_hit;   /* a forged nibble has been coded */\n"
+           "static uint8_t dvt_forge_nib(uint8_t nib);\n"
+           "static __thread uint32_t *dvt_cov;   /* set: every coded command nibble counts in dvt_cov[flat prior * 16 + nibble] */\n"
+           "static __thread void *dvt_codec;   /* the codec of the running encode */\n"
+           "static void dvt_cov_add(const void *cdf, uint8_t nib);\n"
            "#line 1 \"oracle/divans_oracle.c\"\n")
 
 
@@ -62,9 +99,15 @@ def build(force=False):
         raise RuntimeError("oracle_tally: ans_enc_put of oracle/divans_oracle.c is not the one the tally hook was written for")
     if oracle.count(_MM) != 1:
         raise RuntimeError("oracle_tally: the mixing-mask read of oracle/divans_oracle.c is not the one the bin hook was written for")
+    for pat, what in ((_CAB, "code_and_blend"), (_TYPE, "the command-type nibble of dvo_encode_cmds"), (_FLUSH, "the flush of dvo_encode_cmds"),
+                      (_LIT, "the literal copy of dvo_encode_cmds"), (_INIT, "the codec_init of dvo_encode_cmds")):
+        if oracle.count(pat) != 1:
+            raise RuntimeError("oracle_tally: %s of oracle/divans_oracle.c is not the one the forging hook was written for" % what)
     os.makedirs(_BUILD, exist_ok=True)
+    hooked = oracle.replace(_PUT, _PUT_TALLIED).replace(_MM, _MM_TALLIED)
+    hooked = hooked.replace(_CAB, _CAB_FORGED).replace(_TYPE, _TYPE_FORGED).replace(_FLUSH, _FLUSH_FORGED).replace(_LIT, _LIT_FORGED).replace(_INIT, _INIT_COV)
     with open(_SRC + ".tmp", "w") as f:
-        f.write(_PREFIX + oracle.replace(_PUT, _PUT_TALLIED).replace(_MM, _MM_TALLIED) + '\n#line 1 "oracle_tally/tally_api.c"\n' + open(_API_C).read())
+        f.write(_PREFIX + hooked + '\n#line 1 "oracle_tally/tally_api.c"\n' + open(_API_C).read())
     os.replace(_SRC + ".tmp", _SRC)
     cc = os.environ.get("CC", "gcc")
     flags = ["-O3", "-march=x86-64-v2", "-fwrapv", "-fPIC", "-Wall", "-Wextra", "-Wno-unused-parameter", "-pthread", "-shared",
@@ -111,6 +154,10 @@ def lib(blend=False):
         L.dvo_encode_cmds_mixmap.argtypes = [vp, op, ctypes.c_int, vp, ctypes.c_uint32, vp, ctypes.c_size_t, szp,
                                              ctypes.POINTER(ctypes.c_uint32), vp, vp, vp]
         L.dvo_recode_blob.argtypes = [vp, ctypes.c_size_t, ctypes.c_int, vp, ctypes.c_size_t, szp]
+        L.dvo_cmdlist_from_blob.argtypes = [vp, ctypes.c_size_t, vp]
+        L.dvo_cov_size.restype = ctypes.c_size_t
+        L.dvo_encode_cmds_cov.argtypes = [vp, op, vp]
+        L.dvo_encode_cmds_forged.argtypes = [vp, op, vp, vp, ctypes.c_size_t, vp, ctypes.c_size_t, szp, u64p]
         assert L.dvo_feature_blend() == int(blend)
         _libs[blend] = L
     return _libs[blend]
@@ -277,3 +324,76 @@ def encode_cmds_mixmap(cmds, pred_mode, values, blend=False, **kw):
     rc = lib(blend).dvo_encode_cmds_mixmap(ctypes.addressof(cmds.c), ctypes.byref(options(blend, **kw)), pred_mode, _p(v), v.size, _p(out),
                                            cap, ctypes.byref(n), ctypes.byref(ch), _p(mixing), _p(cost), _p(bins))
     return rc, out[: n.value].tobytes() if rc == SUCCESS else None, ch.value, mixing, cost, bins.reshape(v.size, MIX_ENTRIES)
+
+
+def from_blob(oracle, blob):
+    """the oracle_py / oracle_blend Commands of DVCL blob ``blob``, every field as the blob holds it (dvo_cmdlist_from_blob), or
+    None for a blob whose header, records or literals do not fit"""
+    cl = oracle.Commands()
+    b = _u8(blob)
+    return cl if lib().dvo_cmdlist_from_blob(_p(b), len(blob), ctypes.addressof(cl.c)) == SUCCESS else None
+
+
+def encode_forged(cmds, forge=(), blend=False, cap=None, **kw):
+    """(rc, stream, n_nibbles): the oracle's encoding of ``cmds`` with each (k, v) of ``forge`` making command nibble k (0 = the
+    first) the value v (dvo_encode_cmds_forged).  ``stream`` is the encoded stream, also for rc 3 when the walk failed after a
+    forged nibble (the stream then ends there), else b"".  n_nibbles: the command nibbles coded, the end-of-stream one included."""
+    at = np.ascontiguousarray([k for k, _ in forge] or [0], np.uint32)
+    val = np.ascontiguousarray([v for _, v in forge] or [0], np.uint8)
+    cap = cap or int(cmds.c.n_lits) * 2 + int(cmds.c.n_cmds) * 16 + (1 << 20)
+    out = np.empty(cap, np.uint8)
+    n, nn = ctypes.c_size_t(0), ctypes.c_uint64(0)
+    rc = lib(blend).dvo_encode_cmds_forged(ctypes.addressof(cmds.c), ctypes.byref(options(blend, **kw)), _p(at), _p(val), len(forge),
+                                           _p(out), cap, ctypes.byref(n), ctypes.byref(nn))
+    return rc, out[: n.value].tobytes(), nn.value
+
+
+# ---- coverage of the command coder's priors (dvo_encode_cmds_cov) ----
+# the prior tables of oracle/divans_oracle.c (codec/priors.rs:12-133) in the order dvo_cov_size concatenates them: (table,
+# [(type, dims)]); a flat index is the offset of its table plus the type's offset plus i0 + d0 * (i1 + d1 * i2)
+PRIOR_TABLES = [
+    ("CC", [("FullSelection", (16, 1)), ("EndIndicator", (1, 256))]),
+    ("LL", [("CountSmall", (256, 16)), ("SizeBegNib", (256,)), ("SizeLastNib", (256,)), ("SizeMantissaNib", (256,))]),
+    ("CP", [("DistanceBegNib", (256, 64)), ("DistanceMnemonic", (256, 2)), ("DistanceLastNib", (256, 1)), ("DistanceMantissaNib", (256, 5)),
+            ("CountSmall", (256, 64)), ("CountBegNib", (256, 64)), ("CountLastNib", (256, 64)), ("CountMantissaNib", (256, 64))]),
+    ("DC", [("SizeBegNib", (256,)), ("SizeLastNib", (256,)), ("Index", (256, 5)), ("Transform", (2, 25))]),
+    ("BT", [("Mnemonic", (3,)), ("FirstNibble", (3,)), ("SecondNibble", (3,)), ("StrideNibble", (1,))]),
+    ("PM", [("Only", (1,)), ("LiteralSpeed", (1,)), ("FirstNibble", (2,)), ("SecondNibble", (2,)), ("Mnemonic", (4,)),
+            ("PriorMixingValue", (17,)), ("ContextMapSpeedPalette", (4,))]),
+]
+
+
+def prior_of(flat):
+    """(table, type, (i0, i1)) of flat prior index ``flat`` (the P() indices of the oracle's code_and_blend call)"""
+    for table, ents in PRIOR_TABLES:
+        for typ, dims in ents:
+            n = int(np.prod(dims))
+            if flat < n:
+                return table, typ, (flat % dims[0], flat // dims[0])
+            flat -= n
+    raise IndexError(flat)
+
+
+def cov_size():
+    n = int(lib().dvo_cov_size())
+    assert n == sum(int(np.prod(d)) for _, e in PRIOR_TABLES for _, d in e), "PRIOR_TABLES differs from the oracle's"
+    return n
+
+
+def coverage(cmd_lists, **kw):
+    """counts [n_priors, 16]: how often each command nibble was coded under each prior over the oracle's encodings of the
+    command lists ``cmd_lists`` (oracle_py Commands) with options ``kw``; every encode must succeed"""
+    cov = np.zeros((cov_size(), 16), np.uint32)
+    for cl in cmd_lists:
+        rc = lib().dvo_encode_cmds_cov(ctypes.addressof(cl.c), ctypes.byref(options(**kw)), _p(cov))
+        assert rc == SUCCESS, rc
+    return cov
+
+
+def coverage_pairs(cov):
+    """{(table, type): {(i0, i1): set of nibbles}} of the nonzero entries of ``cov``"""
+    out = {}
+    for flat, nib in zip(*np.nonzero(cov)):
+        t, typ, idx = prior_of(int(flat))
+        out.setdefault((t, typ), {}).setdefault(idx, set()).add(int(nib))
+    return out
