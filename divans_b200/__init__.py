@@ -48,6 +48,10 @@ BATCH_SYMBOLS = [
     "divans_b200_replay_cmds_batch_host", "divans_b200_replay_cmds_batch_device", "divans_b200_lz77_cmds_batch_device",
     "divans_b200_encode_mixmap_batch_host", "divans_b200_encode_mixmap_batch_device", "divans_b200_encode_cmds_mixmap_batch_host",
     "divans_b200_encode_cmds_mixmap_batch_device",
+    "divans_b200_encode_speeds_batch_host",
+    "divans_b200_encode_speeds_batch_device",
+    "divans_b200_encode_cmds_speeds_batch_host",
+    "divans_b200_encode_cmds_speeds_batch_device",
 ]
 PM_RECORD_BYTES = 32 + 16384 + 1024 + 8192   # one prediction-mode record of a DVCL blob (include/divans_b200.h)
 
@@ -86,6 +90,13 @@ LITERAL_MODEL_KEEP = (-1, -1)
 # values"); 4 first, the encoder's default value, so unvisited entries keep it.
 DEFAULT_MIXING_VALUES = [4, 5, 8, 1, 7, 0]
 MIX_ENTRIES = 8192
+
+# The reference encoder's speed palette (Speed::ENCODER_DEFAULT_PALETTE), (inc, lim) pairs.
+LITERAL_SPEED_PALETTE = [(0, 1024), (2, 1024), (1, 128), (1, 16384), (2, 2048), (4, 1024), (8, 8192), (16, 48), (16, 8192), (32, 4096),
+                         (64, 16384), (128, 256), (128, 16384), (512, 16384), (1664, 16384)]
+# encode_speeds' default candidates: MUD (16, 8192), the speed every stream is coded with otherwise, first, then the palette
+# speeds the real-text survey picks (DESIGN.md section 4, "Literal speeds").
+DEFAULT_LITERAL_SPEEDS = [(16, 8192), (32, 4096), (64, 16384), (128, 16384), (512, 16384), (1664, 16384)]
 
 
 class CAllocator(ctypes.Structure):
@@ -166,6 +177,16 @@ def load_library():
     L.divans_b200_encode_cmds_mixmap_batch_device.argtypes = [vp, sz, vp, vp, vp, ctypes.c_uint64, ctypes.c_uint64, vp, vp, vp, vp, vp,
                                                               ctypes.POINTER(EncodeOptions), vp, ctypes.c_uint32, vp, vp, vp, vp, vp]
     L.divans_b200_encode_cmds_mixmap_batch_device.restype = ctypes.c_uint8
+    L.divans_b200_encode_speeds_batch_host.argtypes = batch + [ctypes.POINTER(EncodeOptions), vp, ctypes.c_uint32, vp, vp, vp]
+    L.divans_b200_encode_speeds_batch_host.restype = ctypes.c_uint8
+    L.divans_b200_encode_cmds_speeds_batch_host.argtypes = batch + [ctypes.POINTER(EncodeOptions), vp, ctypes.c_uint32, vp, vp, vp]
+    L.divans_b200_encode_cmds_speeds_batch_host.restype = ctypes.c_uint8
+    L.divans_b200_encode_speeds_batch_device.argtypes = [vp, sz, vp, vp, vp, ctypes.c_uint64, vp, vp, vp, vp, vp, ctypes.POINTER(EncodeOptions),
+                                                         vp, ctypes.c_uint32, vp, vp, vp, vp]
+    L.divans_b200_encode_speeds_batch_device.restype = ctypes.c_uint8
+    L.divans_b200_encode_cmds_speeds_batch_device.argtypes = [vp, sz, vp, vp, vp, ctypes.c_uint64, ctypes.c_uint64, vp, vp, vp, vp, vp,
+                                                              ctypes.POINTER(EncodeOptions), vp, ctypes.c_uint32, vp, vp, vp, vp]
+    L.divans_b200_encode_cmds_speeds_batch_device.restype = ctypes.c_uint8
     L.divans_b200_replay_cmds_batch_host.argtypes = batch + [ctypes.c_int32]
     L.divans_b200_replay_cmds_batch_host.restype = ctypes.c_uint8
     L.divans_b200_replay_cmds_batch_device.argtypes = batch + [ctypes.c_int32, vp]
@@ -678,6 +699,82 @@ class Engine:
     def encode_cmds_mixmap(self, blobs, opts=None, values=None):
         """Convenience: encode_mixmap for DVCL command-list blobs (encode_cmds_mixmap_batch_host)."""
         return self._mixmap_lists(blobs, opts, True, values)
+
+    # ---- literal speeds (include/divans_b200.h) ----
+    @staticmethod
+    def _speeds(values):
+        v = np.ascontiguousarray(DEFAULT_LITERAL_SPEEDS if values is None else values, np.int16).reshape(-1, 2)
+        return (v if v.size else np.zeros((1, 2), np.int16)), int(v.shape[0])
+
+    def _speeds_host(self, cmds, in_blob, in_off, in_len, out, out_off, out_cap, opts, values):
+        n = len(in_off)
+        in_off, in_len, out_off, out_cap, out_len, status = _host_batch(in_off, in_len, out_off, out_cap)
+        v, k = self._speeds(values)
+        chosen = np.zeros((n, 3), np.uint32)
+        cost = np.zeros((n, k + 1), np.uint64)
+        halves = np.zeros((n, k, 2), np.uint64)
+        o = opts or encode_options()
+        fn = self._L.divans_b200_encode_cmds_speeds_batch_host if cmds else self._L.divans_b200_encode_speeds_batch_host
+        rc = fn(self._h, n, _ptr(in_blob), _ptr(in_off), _ptr(in_len), _ptr(out), _ptr(out_off), _ptr(out_cap), _ptr(out_len), _ptr(status),
+                ctypes.byref(o), _ptr(v), k, _ptr(chosen), _ptr(cost), _ptr(halves))
+        if rc != DIVANS_SUCCESS:
+            raise DivansError("%s_batch_host: %s" % ("encode_cmds_speeds" if cmds else "encode_speeds", self._err()))
+        return out_len, status, chosen, cost, halves
+
+    def encode_speeds_batch_host(self, in_blob, in_off, in_len, out, out_off, out_cap, opts=None, values=None):
+        """encode_batch_host with each stream's literal speeds chosen among ``values`` ((inc, lim) pairs, default
+        DEFAULT_LITERAL_SPEEDS).  Returns (out_len, status, chosen [n, 3], cost [n, k + 1], halves [n, k, 2]): stream i is coded
+        with literal_adaptation (v[a], v[a], v[b], v[c]) for (a, b, c) = chosen[i]."""
+        return self._speeds_host(False, in_blob, in_off, in_len, out, out_off, out_cap, opts, values)
+
+    def encode_cmds_speeds_batch_host(self, blobs, blob_off, blob_len, out, out_off, out_cap, opts=None, values=None):
+        """encode_speeds_batch_host for command lists: the speeds override every record's."""
+        return self._speeds_host(True, blobs, blob_off, blob_len, out, out_off, out_cap, opts, values)
+
+    def encode_speeds_batch_device(self, n, d_in, d_in_off, d_in_len, max_in_len, d_out, d_out_off, d_out_cap, d_out_len, d_status,
+                                   d_chosen=None, d_cost=None, d_halves=None, opts=None, values=None, stream=None):
+        """encode_speeds_batch_host with raw device pointers (ints, or None for an output not wanted).  Asynchronous."""
+        v, k = self._speeds(values)
+        o = opts or encode_options()
+        rc = self._L.divans_b200_encode_speeds_batch_device(self._h, n, d_in, d_in_off, d_in_len, int(max_in_len), d_out, d_out_off, d_out_cap,
+                                                            d_out_len, d_status, ctypes.byref(o), _ptr(v), k, d_chosen, d_cost, d_halves, stream)
+        if rc != DIVANS_SUCCESS:
+            raise DivansError("encode_speeds_batch_device: " + self._err())
+
+    def encode_cmds_speeds_batch_device(self, n, d_blobs, d_blob_off, d_blob_len, max_blob_len, max_raw_len, d_out, d_out_off, d_out_cap,
+                                        d_out_len, d_status, d_chosen=None, d_cost=None, d_halves=None, opts=None, values=None, stream=None):
+        """encode_cmds_speeds_batch_host with raw device pointers (ints, or None for an output not wanted).  Asynchronous."""
+        v, k = self._speeds(values)
+        o = opts or encode_options()
+        rc = self._L.divans_b200_encode_cmds_speeds_batch_device(self._h, n, d_blobs, d_blob_off, d_blob_len, int(max_blob_len),
+                                                                 int(max_raw_len), d_out, d_out_off, d_out_cap, d_out_len, d_status,
+                                                                 ctypes.byref(o), _ptr(v), k, d_chosen, d_cost, d_halves, stream)
+        if rc != DIVANS_SUCCESS:
+            raise DivansError("encode_cmds_speeds_batch_device: " + self._err())
+
+    def _speeds_lists(self, bufs, opts, cmds, values):
+        blob, in_off, in_len = _pack(bufs)
+        out_cap = _encoded_cap(in_len)
+        out_off, out_total = _regions(out_cap)
+        out = np.zeros(out_total, np.uint8)
+        out_len, status, chosen, cost, _ = self._speeds_host(cmds, blob, in_off, in_len, out, out_off, out_cap, opts, values)
+        v, _ = self._speeds(values)
+        res = []
+        for i, (s, o, n) in enumerate(zip(status, out_off, out_len)):
+            a, b, c = (int(x) for x in chosen[i])
+            sp = [tuple(int(x) for x in v[j]) for j in (a, a, b, c)]
+            res.append((int(s), out[int(o):int(o) + int(n)].tobytes() if s == DIVANS_SUCCESS else None, sp, [int(x) for x in cost[i]]))
+        return res
+
+    def encode_speeds(self, raws, opts=None, values=None):
+        """Convenience: list of raw byte strings -> list of (status, .divans bytes or None, speeds, cost): speeds = the four
+        (inc, lim) literal speeds the stream was coded with, cost = its k uniform costs then the verify cost
+        (encode_speeds_batch_host)."""
+        return self._speeds_lists(raws, opts, False, values)
+
+    def encode_cmds_speeds(self, blobs, opts=None, values=None):
+        """Convenience: encode_speeds for DVCL command-list blobs (encode_cmds_speeds_batch_host)."""
+        return self._speeds_lists(blobs, opts, True, values)
 
     def encode_cmds_batch_device(self, n, d_blobs, d_blob_off, d_blob_len, max_blob_len, max_raw_len, d_out, d_out_off, d_out_cap, d_out_len,
                                  d_status, opts=None, stream=None):

@@ -85,6 +85,8 @@ struct divans_b200_ctx {
     uint8_t *d_mix_records = nullptr; size_t mix_records_cap = 0;
     uint64_t *d_slot_bins = nullptr; size_t slot_bins_cap = 0;
     uint64_t *d_mix_out = nullptr; size_t mix_out_cap = 0;
+    // literal speeds (encode_speeds_*): the halves and verify passes' costs, statuses and halves, the per-pair and per-stream speeds
+    uint64_t *d_speeds = nullptr; size_t speeds_cap = 0;
     // LZ77 command generator (lz77_cmds_batch_device): per-warp head table + prev array, and the PredictionMode record it copies
     // (lz_scratch_asked: the request the allocation was made for, which free memory may have cut down to lz_scratch_words)
     int32_t *d_lz_scratch = nullptr; size_t lz_scratch_words = 0, lz_scratch_asked = 0;
@@ -187,7 +189,7 @@ extern "C" void divans_b200_destroy(divans_b200_ctx *ctx) {
     if (ctx->ev_busy) cudaEventDestroy(ctx->ev_busy);
     cudaFree(ctx->d_sf); cudaFree(ctx->d_replay); cudaFree(ctx->d_enc_scratch); cudaFree(ctx->d_pm_internal); cudaFree(ctx->d_rcp15);
     cudaFree(ctx->d_pm_records); cudaFree(ctx->d_cost_tab); cudaFree(ctx->d_auto);
-    cudaFree(ctx->d_mix); cudaFree(ctx->d_mix_records); cudaFree(ctx->d_slot_bins); cudaFree(ctx->d_mix_out);
+    cudaFree(ctx->d_mix); cudaFree(ctx->d_mix_records); cudaFree(ctx->d_slot_bins); cudaFree(ctx->d_mix_out); cudaFree(ctx->d_speeds);
     cudaFree(ctx->d_lz_scratch); cudaFree(ctx->d_lz_pm);
     for (auto &ln : ctx->lane) {
         free_host_bufs(ln.bufs);
@@ -619,7 +621,8 @@ static DivansResult encode_device_internal(divans_b200_ctx *ctx, size_t n, int r
                                            const uint64_t *d_in_len, uint64_t max_in_len, const LogCaps &caps, uint8_t *d_out,
                                            const uint64_t *d_out_off, const uint64_t *d_out_cap, uint64_t *d_out_len, int32_t *d_status,
                                            const divans_b200_encode_options *o, int window, cudaStream_t st,
-                                           const uint8_t *d_pm_records = nullptr, const uint32_t *d_pm_index = nullptr, uint32_t pm_keep = 0) {
+                                           const uint8_t *d_pm_records = nullptr, const uint32_t *d_pm_index = nullptr, uint32_t pm_keep = 0,
+                                           const int *d_adapt = nullptr) {
     const size_t slots = encode_slots(ctx, n);
     const uint32_t blocks = (uint32_t)(slots / ENCODE_GROUPS_PER_BLOCK);
     if (ensure_arena(ctx, slots) != DIVANS_SUCCESS) return DIVANS_FAILURE;
@@ -655,10 +658,14 @@ static DivansResult encode_device_internal(divans_b200_ctx *ctx, size_t n, int r
     ep.rcp15 = ctx->d_rcp15;
     ep.max_chunks = max_chunks; ep.cmd_chunks = cmd_chunks;
     ep.out = d_out; ep.out_off = d_out_off; ep.out_cap = d_out_cap; ep.out_len = d_out_len; ep.status = d_status;
+    ep.v_adapt = d_adapt;
     CK(cudaMemsetAsync(ctx->d_counter, 0, 4, st));
     CK(cudaEventRecord(ctx->ev0, st));
     CK(cudaEventRecord(ctx->evm, st));
-    if (o->cdf_model == DIVANS_B200_CDF_BLEND) launch_encode_model_blend(ep, blocks, st); else launch_encode_model(ep, blocks, st);
+    const bool blend = o->cdf_model == DIVANS_B200_CDF_BLEND;
+    if (d_adapt) { if (blend) launch_encode_speeds_blend(ep, false, blocks, st); else launch_encode_speeds(ep, false, blocks, st); }
+    else if (blend) launch_encode_model_blend(ep, blocks, st);
+    else launch_encode_model(ep, blocks, st);
     CK(cudaEventRecord(ctx->evm1, st));
     launch_encode_flush_mux(ep, st);
     CK(cudaEventRecord(ctx->ev1, st));
@@ -676,6 +683,9 @@ struct AutoSel {
     const divans_b200_literal_model *cands; uint32_t n_cands;
     uint32_t *chosen; uint64_t *cost;
     bool mixmap = false; uint8_t *mixing = nullptr; uint64_t *bins = nullptr;
+    // speeds (divans_b200_encode_speeds_*): the k = n_cands candidate speeds (cands unused); chosen has 3 columns, cost k + 1,
+    // halves [n * k * 2] is optional
+    const SpeedValues *speeds = nullptr; uint64_t *halves = nullptr;
 };
 
 // ---- literal model selection ----
@@ -843,6 +853,120 @@ static DivansResult encode_mixmap_device_nolock(divans_b200_ctx *ctx, size_t n, 
                                   d_status, o, window, st, ctx->d_mix_records, rec_idx, 0);
 }
 
+// Literal speeds: one launch sequence over n streams in HBM, k candidate speeds, pairs candidate-major (v = c * n + i), every
+// pass on encode_speeds_kernel (the stream's speeds from v_adapt):
+//  1. uniform passes over the n * k pairs under (v[c], v[c], v[c], v[c]): u[i][c]
+//  2. with dynamic context mixing >= 2 and k > 1: halves passes under (v[c*], v[c*], v[d], v[d]), whose literal low / high
+//     nibble costs give l*, h*; then the verify pass of each stream under (v[c*], v[c*], v[l*], v[h*]): x[i]
+//  3. speeds_select_kernel: the chosen speeds per stream;  4. the plain pipeline under them.
+// Raw streams start with the options' record; command lists keep their records.
+static DivansResult encode_speeds_device_nolock(divans_b200_ctx *ctx, size_t n, int raw_mode, const uint8_t *d_in, const uint64_t *d_in_off,
+                                                const uint64_t *d_in_len, uint64_t max_in_len, const LogCaps &caps, uint8_t *d_out,
+                                                const uint64_t *d_out_off, const uint64_t *d_out_cap, uint64_t *d_out_len, int32_t *d_status,
+                                                const divans_b200_encode_options *o, int window, const SpeedValues &vals,
+                                                uint32_t *d_chosen, uint64_t *d_cost, uint64_t *d_halves, cudaStream_t st) {
+    const uint32_t k = vals.k;
+    const uint64_t nv = (uint64_t)n * k;
+    const size_t vslots = encode_slots(ctx, nv);
+    if (ensure_arena(ctx, vslots) != DIVANS_SUCCESS) return DIVANS_FAILURE;
+    if (!grow(ctx, &ctx->d_replay, &ctx->replay_cap, vslots * (size_t)caps.replay)) return DIVANS_FAILURE;
+    // v_off [nv] | v_len [nv] | tally [nv] | v_pm u32 [nv] | v_status i32 [nv]
+    if (!grow(ctx, &ctx->d_auto, &ctx->auto_cap, 4 * nv + 2)) return DIVANS_FAILURE;
+    uint64_t *v_off = ctx->d_auto, *v_len = v_off + nv, *tally = v_len + nv;
+    uint32_t *v_pm = reinterpret_cast<uint32_t *>(tally + nv);
+    int32_t *v_status = reinterpret_cast<int32_t *>(v_pm + nv);
+    // h_tally [nv] | h_halves [2nv] | x_tally [n] | x_halves [2n] | h_status i32 [nv] | x_status i32 [n] | sel u32 [3n] |
+    // v_adapt i32 [4nv] | x_adapt i32 [4n]
+    if (!grow(ctx, &ctx->d_speeds, &ctx->speeds_cap, 6 * nv + 7 * n + 4)) return DIVANS_FAILURE;
+    uint64_t *h_tally = ctx->d_speeds, *h_halves = h_tally + nv, *x_tally = h_halves + 2 * nv, *x_halves = x_tally + n;
+    int32_t *h_status = reinterpret_cast<int32_t *>(x_halves + 2 * n), *x_status = h_status + nv;
+    uint32_t *sel = reinterpret_cast<uint32_t *>(x_status + n);
+    int *v_adapt = reinterpret_cast<int *>(sel + 3 * n), *x_adapt = v_adapt + 4 * nv;
+    if (!ctx->d_pm_internal) CK(cudaMalloc((void **)&ctx->d_pm_internal, PM_RECORD_BYTES));
+    if (ctx->busy_recorded) CK(cudaStreamWaitEvent(st, ctx->ev_busy, 0));
+    if (!ensure_cost_tab(ctx, st)) return DIVANS_FAILURE;
+    if (raw_mode) {
+        std::vector<uint8_t> &pm = ctx->h_pm;
+        pm.assign(PM_RECORD_BYTES, 0);
+        raw_record(pm.data(), o->literal_pred_mode, o->literal_mixing_value);
+        CK(cudaMemcpyAsync(ctx->d_pm_internal, pm.data(), PM_RECORD_BYTES, cudaMemcpyHostToDevice, st));
+    }
+    const bool blend = o->cdf_model == DIVANS_B200_CDF_BLEND;
+    launch_auto_fanout(d_in_off, d_in_len, n, k, v_off, v_len, v_pm, st);
+    launch_speeds_stage(0, n, vals, tally, v_status, h_halves, sel, v_adapt, x_adapt, st);
+    // 1. uniform passes
+    EncodeParams tp = encode_params(ctx, nv, raw_mode, d_in, v_off, v_len, max_in_len, caps, o, window);
+    tp.pm_internal = ctx->d_pm_internal; tp.cost_tab = ctx->d_cost_tab;
+    tp.status = v_status; tp.tally = tally; tp.v_adapt = v_adapt; tp.halves = h_halves;
+    const uint32_t vblocks = (uint32_t)(vslots / ENCODE_GROUPS_PER_BLOCK);
+    CK(cudaMemsetAsync(ctx->d_counter, 0, 4, st));
+    if (blend) launch_encode_speeds_blend(tp, true, vblocks, st); else launch_encode_speeds(tp, true, vblocks, st);
+    ctx->launches += 3;
+    // 2. halves passes and the verify pass
+    const bool tuned = o->dynamic_context_mixing >= 2 && k > 1;
+    if (tuned) {
+        launch_speeds_stage(1, n, vals, tally, v_status, h_halves, sel, v_adapt, x_adapt, st);
+        EncodeParams hp = tp;
+        hp.status = h_status; hp.tally = h_tally;
+        CK(cudaMemsetAsync(ctx->d_counter, 0, 4, st));
+        if (blend) launch_encode_speeds_blend(hp, true, vblocks, st); else launch_encode_speeds(hp, true, vblocks, st);
+        launch_speeds_stage(2, n, vals, tally, h_status, h_halves, sel, v_adapt, x_adapt, st);
+        EncodeParams xp = encode_params(ctx, n, raw_mode, d_in, d_in_off, d_in_len, max_in_len, caps, o, window);
+        xp.pm_internal = ctx->d_pm_internal; xp.cost_tab = ctx->d_cost_tab;
+        xp.status = x_status; xp.tally = x_tally; xp.v_adapt = x_adapt; xp.halves = x_halves;
+        const uint32_t xblocks = (uint32_t)(encode_slots(ctx, n) / ENCODE_GROUPS_PER_BLOCK);
+        CK(cudaMemsetAsync(ctx->d_counter, 0, 4, st));
+        if (blend) launch_encode_speeds_blend(xp, true, xblocks, st); else launch_encode_speeds(xp, true, xblocks, st);
+        ctx->launches += 4;
+    }
+    // 3. choice
+    launch_speeds_select(n, vals, tuned, tally, v_status, h_halves, h_status, x_tally, x_status, sel, x_adapt, d_chosen, d_cost, d_halves, st);
+    ctx->launches += 1;
+    CK(cudaGetLastError());
+    return encode_device_internal(ctx, n, raw_mode, d_in, d_in_off, d_in_len, max_in_len, caps, d_out, d_out_off, d_out_cap, d_out_len,
+                                  d_status, o, window, st, nullptr, nullptr, 0, x_adapt);
+}
+
+// host twins of the stream's f8 speed codec (dv_engine.cuh: speed_to_u8_i16, u8_to_speed) and of speed_is_small
+static uint32_t host_speed_to_u8(int data) {
+    const uint32_t u = (uint32_t)data & 0xffff;
+    uint32_t length = 0;
+    while (length < 16 && (u >> length) != 0) length++;
+    uint32_t mant = 0;
+    if (data != 0) {
+        const int rem = (int)(short)(data - (short)(1 << (length - 1)));
+        mant = (uint32_t)(((int)(short)(rem << 3)) >> (length - 1)) & 0xff;
+    }
+    return ((length << 3) | mant) & 0xff;
+}
+static int host_u8_to_speed(uint32_t data) {
+    if (data < 8) return 0;
+    const uint32_t log_val = (data >> 3) - 1;
+    const int rem = (int)(short)((data & 7) << log_val);
+    return (int)(short)((short)(1 << log_val) | (rem >> 3));
+}
+
+// `values` (1..16 (inc, lim) pairs, each unchanged by the stream's f8 round trip and small enough for the literal fast loops)
+// packed into `vals`; false (and the error) for anything else
+static bool speed_values(divans_b200_ctx *ctx, const int16_t *values, uint32_t k, SpeedValues &vals) {
+    char buf[200];
+    if (!values || k < 1 || k > 16) { ctx->err = "encode_speeds: 1..16 speeds are required"; return false; }
+    memset(&vals, 0, sizeof vals); vals.k = k;
+    for (uint32_t c = 0; c < k; c++) {
+        const int inc = values[2 * c], lim = values[2 * c + 1];
+        const bool round_trip = host_u8_to_speed(host_speed_to_u8(inc)) == inc && host_u8_to_speed(host_speed_to_u8(lim)) == lim;
+        const bool small = inc >= 0 && lim >= 0 && lim + inc + 16 <= 0x7fff && 4 * (inc + 16) <= 0x7fff;
+        if (!round_trip || !small) {
+            snprintf(buf, sizeof buf, "encode_speeds: speed %u (%d, %d) %s", c, inc, lim,
+                     !round_trip ? "is changed by the stream's f8 speed code" : "could wrap the literal priors' i16 counters");
+            ctx->err = buf;
+            return false;
+        }
+        vals.v[c] = (int)((uint32_t)(uint16_t)inc | ((uint32_t)(uint16_t)lim << 16));
+    }
+    return true;
+}
+
 // `values` (1..16 mixing values 0..15) and the mode of opts as candidate literal models; false (and the error) for anything else
 static bool mixmap_cands(divans_b200_ctx *ctx, const int32_t *values, uint32_t k, const divans_b200_encode_options *o,
                          divans_b200_literal_model *cands) {
@@ -872,9 +996,9 @@ static DivansResult encode_device_common(divans_b200_ctx *ctx, size_t n, int raw
                                          const uint64_t *d_out_off, const uint64_t *d_out_cap, uint64_t *d_out_len, int32_t *d_status,
                                          const divans_b200_encode_options *opts, void *cuda_stream, const AutoSel *sel) try {
     if (!ctx || !opts) return DIVANS_FAILURE;
-    if (sel && !check_cands(ctx, sel->cands, sel->n_cands, !raw_mode)) return DIVANS_FAILURE;
+    if (sel && !sel->speeds && !check_cands(ctx, sel->cands, sel->n_cands, !raw_mode)) return DIVANS_FAILURE;
     if (n == 0) return DIVANS_SUCCESS;
-    if (sel && !sel->mixmap && !sel->chosen) { ctx->err = raw_mode ? "encode_auto: d_chosen is required" : "encode_cmds_auto: d_chosen is required"; return DIVANS_FAILURE; }
+    if (sel && !sel->mixmap && !sel->speeds && !sel->chosen) { ctx->err = raw_mode ? "encode_auto: d_chosen is required" : "encode_cmds_auto: d_chosen is required"; return DIVANS_FAILURE; }
     if (sel && sel->mixmap && n > 0x7fffffffull) { ctx->err = "batch too large"; return DIVANS_FAILURE; }   // (one block per stream)
     const uint64_t nv = (uint64_t)n * (sel ? sel->n_cands : 1);
     if (nv > 0xffffffffull || max_in_len > 0x7fff0000ull || max_raw_len > 0x7fff0000ull) { ctx->err = "batch too large"; return DIVANS_FAILURE; }
@@ -905,6 +1029,9 @@ static DivansResult encode_device_common(divans_b200_ctx *ctx, size_t n, int raw
             ctx->sf_cap = words;
         }
     }
+    if (sel && sel->speeds)
+        return encode_speeds_device_nolock(ctx, n, raw_mode, d_in, d_in_off, d_in_len, max_in_len, caps, d_out, d_out_off, d_out_cap, d_out_len,
+                                           d_status, opts, window, *sel->speeds, sel->chosen, sel->cost, sel->halves, st);
     if (sel && sel->mixmap)
         return encode_mixmap_device_nolock(ctx, n, raw_mode, d_in, d_in_off, d_in_len, max_in_len, caps, d_out, d_out_off, d_out_cap, d_out_len,
                                            d_status, opts, window, sel->cands, sel->n_cands, sel->chosen, sel->cost, sel->mixing, sel->bins, st);
@@ -962,9 +1089,9 @@ static DivansResult encode_host_common(divans_b200_ctx *ctx, size_t n, int raw_m
                                        uint64_t *out_len, int32_t *status, const divans_b200_encode_options *opts,
                                        const AutoSel *sel) try {
     if (!ctx || !opts) return DIVANS_FAILURE;
-    if (sel && !check_cands(ctx, sel->cands, sel->n_cands, !raw_mode)) return DIVANS_FAILURE;
+    if (sel && !sel->speeds && !check_cands(ctx, sel->cands, sel->n_cands, !raw_mode)) return DIVANS_FAILURE;
     if (n == 0) return DIVANS_SUCCESS;
-    if (sel && !sel->mixmap && !sel->chosen) { ctx->err = raw_mode ? "encode_auto: chosen is required" : "encode_cmds_auto: chosen is required"; return DIVANS_FAILURE; }
+    if (sel && !sel->mixmap && !sel->speeds && !sel->chosen) { ctx->err = raw_mode ? "encode_auto: chosen is required" : "encode_cmds_auto: chosen is required"; return DIVANS_FAILURE; }
     if (sel && (uint64_t)n * sel->n_cands > 0xffffffffull) { ctx->err = "batch too large"; return DIVANS_FAILURE; }
     std::lock_guard<std::mutex> lk(ctx->mu);
     CK(cudaSetDevice(ctx->device));
@@ -1010,6 +1137,7 @@ static DivansResult encode_host_common(divans_b200_ctx *ctx, size_t n, int raw_m
             uint64_t rep = vs * c.replay;
             if (sel && sel->mixmap)
                 rep += vs * MIX_ENTRIES * 8 + (uint64_t)(i1 - i0 + 1) * (MIX_ENTRIES * 9 + PM_RECORD_BYTES + (sel->bins ? sel->n_cands * MIX_ENTRIES * 8ull : 0));
+            if (sel && sel->speeds) rep += (uint64_t)(i1 - i0 + 1) * sel->n_cands * 96;   // encode_speeds: scratch and halves, per pair
             if (i1 > i0 && (c.cmd + c.lit) * 4 * (uint64_t)(i1 - i0 + 1) + rep > budget) break;
             mc = c;
             if (in_len[i1] > mx) mx = in_len[i1];
@@ -1020,9 +1148,12 @@ static DivansResult encode_host_common(divans_b200_ctx *ctx, size_t n, int raw_m
         uint64_t out_lo, out_hi;
         regions_span(m, out_off + i0, out_cap + i0, out_lo, out_hi);
         if (!grow(ctx, &b.d_out, &b.d_out_cap, (size_t)(out_hi - out_lo) + 64)) return DIVANS_FAILURE;
-        // in_off | in_len | out_off | out_cap | out_len | status (+ encode_auto: chosen | cost [m * C]; encode_mixmap: cost [m * (C + 1)])
-        const size_t cost_cols = sel ? sel->n_cands + (sel->mixmap ? 1 : 0) : 0;
-        if (!grow(ctx, &b.d_meta, &b.d_meta_cap, m * 6 + (sel ? m + m * cost_cols : 0))) return DIVANS_FAILURE;
+        // in_off | in_len | out_off | out_cap | out_len | status (+ encode_auto: chosen | cost [m * C]; encode_mixmap: cost [m * (C + 1)];
+        // encode_speeds: chosen [3m u32] | cost [m * (C + 1)] | halves [m * C * 2])
+        const bool spd = sel && sel->speeds;
+        const size_t cost_cols = sel ? sel->n_cands + (sel->mixmap || spd ? 1 : 0) : 0;
+        const size_t chosen_words = spd ? 2 * m : m, halves_words = spd ? 2 * m * (size_t)sel->n_cands : 0;
+        if (!grow(ctx, &b.d_meta, &b.d_meta_cap, m * 6 + (sel ? chosen_words + m * cost_cols + halves_words : 0))) return DIVANS_FAILURE;
         // encode_mixmap: mixing [m * 8192 bytes] | bins [m * C * 8192]
         uint8_t *d_mixing = nullptr; uint64_t *d_bins = nullptr;
         if (sel && sel->mixmap) {
@@ -1040,8 +1171,11 @@ static DivansResult encode_host_common(divans_b200_ctx *ctx, size_t n, int raw_m
         CK(cudaMemcpyAsync(mm + 3 * m, out_cap + i0, m * 8, cudaMemcpyHostToDevice, st));
         int32_t *d_status = reinterpret_cast<int32_t *>(mm + 5 * m);
         uint32_t *d_chosen = reinterpret_cast<uint32_t *>(mm + 6 * m);
-        uint64_t *d_cost = mm + 7 * m;
-        DivansResult r = sel && sel->mixmap
+        uint64_t *d_cost = mm + 6 * m + chosen_words, *d_halves = spd && sel->halves ? d_cost + m * cost_cols : nullptr;
+        DivansResult r = spd
+                             ? encode_speeds_device_nolock(ctx, m, raw_mode, b.d_in, mm, mm + m, mx, mc, b.d_out, mm + 2 * m, mm + 3 * m, mm + 4 * m,
+                                                           d_status, opts, window, *sel->speeds, d_chosen, d_cost, d_halves, st)
+                         : sel && sel->mixmap
                              ? encode_mixmap_device_nolock(ctx, m, raw_mode, b.d_in, mm, mm + m, mx, mc, b.d_out, mm + 2 * m, mm + 3 * m, mm + 4 * m,
                                                            d_status, opts, window, sel->cands, sel->n_cands, d_chosen, d_cost, d_mixing, d_bins, st)
                          : sel ? encode_auto_device_nolock(ctx, m, raw_mode, b.d_in, mm, mm + m, mx, mc, b.d_out, mm + 2 * m, mm + 3 * m,
@@ -1050,7 +1184,9 @@ static DivansResult encode_host_common(divans_b200_ctx *ctx, size_t n, int raw_m
                                                         mm + 4 * m, d_status, opts, window, st);
         if (r != DIVANS_SUCCESS) return r;
         if (sel) {
-            if (sel->chosen) CK(cudaMemcpyAsync(sel->chosen + i0, d_chosen, m * 4, cudaMemcpyDeviceToHost, st));
+            const size_t ccols = spd ? 3 : 1;
+            if (sel->chosen) CK(cudaMemcpyAsync(sel->chosen + i0 * ccols, d_chosen, m * ccols * 4, cudaMemcpyDeviceToHost, st));
+            if (d_halves) CK(cudaMemcpyAsync(sel->halves + i0 * 2 * (size_t)sel->n_cands, d_halves, halves_words * 8, cudaMemcpyDeviceToHost, st));
             if (sel->cost) CK(cudaMemcpyAsync(sel->cost + i0 * cost_cols, d_cost, m * cost_cols * 8, cudaMemcpyDeviceToHost, st));
             if (d_mixing) CK(cudaMemcpyAsync(sel->mixing + i0 * (size_t)MIX_ENTRIES, d_mixing, m * (size_t)MIX_ENTRIES, cudaMemcpyDeviceToHost, st));
             if (d_bins) CK(cudaMemcpyAsync(sel->bins + i0 * (size_t)sel->n_cands * MIX_ENTRIES, d_bins, m * (size_t)sel->n_cands * MIX_ENTRIES * 8,
@@ -1142,6 +1278,57 @@ extern "C" DivansResult divans_b200_encode_cmds_mixmap_batch_device(divans_b200_
     divans_b200_literal_model cands[16];
     if (!ctx || !opts || !mixmap_cands(ctx, values, n_values, opts, cands)) return DIVANS_FAILURE;
     const AutoSel sel = {cands, n_values, d_chosen, d_cost, true, d_mixing, d_bins};
+    return encode_device_common(ctx, n, 0, d_blobs, d_blob_off, d_blob_len, max_blob_len, max_raw_len, d_out, d_out_off, d_out_cap,
+                                d_out_len, d_status, opts, cuda_stream, &sel);
+}
+
+// ---- literal speeds ----
+extern "C" DivansResult divans_b200_encode_speeds_batch_host(divans_b200_ctx *ctx, size_t n, const uint8_t *in, const uint64_t *in_off,
+                                                             const uint64_t *in_len, uint8_t *out, const uint64_t *out_off, const uint64_t *out_cap,
+                                                             uint64_t *out_len, int32_t *status, const divans_b200_encode_options *opts,
+                                                             const int16_t *values, uint32_t n_values, uint32_t *chosen, uint64_t *cost,
+                                                             uint64_t *halves) {
+    SpeedValues vals;
+    if (!ctx || !opts || !speed_values(ctx, values, n_values, vals)) return DIVANS_FAILURE;
+    AutoSel sel = {nullptr, n_values, chosen, cost};
+    sel.speeds = &vals; sel.halves = halves;
+    return encode_host_common(ctx, n, 1, in, in_off, in_len, out, out_off, out_cap, out_len, status, opts, &sel);
+}
+extern "C" DivansResult divans_b200_encode_speeds_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_in, const uint64_t *d_in_off,
+                                                               const uint64_t *d_in_len, uint64_t max_in_len, uint8_t *d_out,
+                                                               const uint64_t *d_out_off, const uint64_t *d_out_cap, uint64_t *d_out_len,
+                                                               int32_t *d_status, const divans_b200_encode_options *opts, const int16_t *values,
+                                                               uint32_t n_values, uint32_t *d_chosen, uint64_t *d_cost, uint64_t *d_halves,
+                                                               void *cuda_stream) {
+    SpeedValues vals;
+    if (!ctx || !opts || !speed_values(ctx, values, n_values, vals)) return DIVANS_FAILURE;
+    AutoSel sel = {nullptr, n_values, d_chosen, d_cost};
+    sel.speeds = &vals; sel.halves = d_halves;
+    return encode_device_common(ctx, n, 1, d_in, d_in_off, d_in_len, max_in_len, max_in_len, d_out, d_out_off, d_out_cap, d_out_len,
+                                d_status, opts, cuda_stream, &sel);
+}
+extern "C" DivansResult divans_b200_encode_cmds_speeds_batch_host(divans_b200_ctx *ctx, size_t n, const uint8_t *blobs, const uint64_t *blob_off,
+                                                                  const uint64_t *blob_len, uint8_t *out, const uint64_t *out_off,
+                                                                  const uint64_t *out_cap, uint64_t *out_len, int32_t *status,
+                                                                  const divans_b200_encode_options *opts, const int16_t *values, uint32_t n_values,
+                                                                  uint32_t *chosen, uint64_t *cost, uint64_t *halves) {
+    SpeedValues vals;
+    if (!ctx || !opts || !speed_values(ctx, values, n_values, vals)) return DIVANS_FAILURE;
+    AutoSel sel = {nullptr, n_values, chosen, cost};
+    sel.speeds = &vals; sel.halves = halves;
+    return encode_host_common(ctx, n, 0, blobs, blob_off, blob_len, out, out_off, out_cap, out_len, status, opts, &sel);
+}
+extern "C" DivansResult divans_b200_encode_cmds_speeds_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_blobs,
+                                                                    const uint64_t *d_blob_off, const uint64_t *d_blob_len,
+                                                                    uint64_t max_blob_len, uint64_t max_raw_len, uint8_t *d_out,
+                                                                    const uint64_t *d_out_off, const uint64_t *d_out_cap, uint64_t *d_out_len,
+                                                                    int32_t *d_status, const divans_b200_encode_options *opts,
+                                                                    const int16_t *values, uint32_t n_values, uint32_t *d_chosen,
+                                                                    uint64_t *d_cost, uint64_t *d_halves, void *cuda_stream) {
+    SpeedValues vals;
+    if (!ctx || !opts || !speed_values(ctx, values, n_values, vals)) return DIVANS_FAILURE;
+    AutoSel sel = {nullptr, n_values, d_chosen, d_cost};
+    sel.speeds = &vals; sel.halves = d_halves;
     return encode_device_common(ctx, n, 0, d_blobs, d_blob_off, d_blob_len, max_blob_len, max_raw_len, d_out, d_out_off, d_out_cap,
                                 d_out_len, d_status, opts, cuda_stream, &sel);
 }

@@ -178,8 +178,14 @@ struct EncodeParams {
     // nibble of both coders, in 1/65536 bit (cost_tab[f] = -log2(f / 32768), include/divans_b200.h)
     const uint32_t *cost_tab;
     uint64_t *tally;
+    // per-stream literal speeds (encode_speeds_kernel, divans_b200_encode_speeds_*): stream v codes with the four packed speeds
+    // v_adapt[4v .. 4v + 4) in place of the options' literal_adaptation.  Its cost pass also writes the cost of the stream's
+    // literal low and high nibbles, both coders, to halves[2v] and halves[2v + 1].
+    const int *v_adapt;
+    uint64_t *halves;
 };
 constexpr uint32_t PM_RECORD_BYTES = 32 + 16384 + 1024 + 8192;
+struct SpeedValues { int v[16]; uint32_t k; };   // the k (1..16) candidate speeds of a speeds call, packed inc | lim << 16
 
 // Binned cost pass (encode_bins_kernel, divans_b200_encode_mixmap_*): the cost-only pass of n x k (stream, candidate) pairs,
 // candidate-major (pair v = c * n + i), that also sums each literal nibble's cost into the bin of its mixing-mask index.

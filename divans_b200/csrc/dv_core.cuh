@@ -171,12 +171,18 @@ __device__ __forceinline__ void mix_finish(Coder &k, const G2 g, char *nb, char 
     *reinterpret_cast<int16_t *>(cm + 2 * g.l16) = (int16_t)c2; *reinterpret_cast<int16_t *>(nb + 2 * g.l16) = (int16_t)s2;
 }
 
+// The cost of a stream's literal nibbles (encode_speeds_kernel's cost pass): hi = the high nibbles, lit = all of them.
+struct LitHalves { uint64_t hi, lit; };
+
 // The encoder's converged literal fast path: when both groups of the warp sit at the start of a literal byte, code whole
 // bytes (high nibble, low nibble, context of the next byte) back to back without going through the state-machine dispatch.
 // This is code_nibble_array (codec/literal.rs:261-394) for two streams at once.  The common case -- no dynamic context
 // mixing and one mixing-mask value for the whole map -- gets a loop with every selector hoisted out.
-template <bool TALLY>
-__device__ __forceinline__ void literal_fast_enc(St &s, Next &nx, const G2 g) {
+// HALVES (TALLY as well): the cost of the high nibbles is added to hv->hi; the caller sums the whole delta of the coder's cost.
+// The plain loop's sums are read by no call today (the speeds calls read halves only at dynamic mixing 2, which takes the mixing
+// loop); they are kept so that the cost pass reports the same halves whichever loop codes a literal.
+template <bool TALLY, bool HALVES = false>
+__device__ __forceinline__ void literal_fast_enc(St &s, Next &nx, const G2 g, LitHalves *hv = nullptr) {
     const uint32_t n = min(s.lit_left, __shfl_xor_sync(FULL, s.lit_left, 16));
     const bool simple = __all_sync(FULL, !s.mixing_trait && s.lit_cfg >= 0 && s.speeds_small);
     if (simple) {
@@ -198,6 +204,7 @@ __device__ __forceinline__ void literal_fast_enc(St &s, Next &nx, const G2 g) {
         Coder k = s.cur;
         const uint32_t src_last = s.lit_left - 1;                   // (lit_left >= 1 here)
         const uint32_t pm_shift = pm == 1 ? 2u : 0u;
+        uint64_t hh = 0;
         uint32_t done = 0;
         while (done < n) {
             uint32_t m = n - done;
@@ -228,7 +235,7 @@ __device__ __forceinline__ void literal_fast_enc(St &s, Next &nx, const G2 g) {
                     int lo = __shfl_sync(FULL, cum, (h - 1) & 15, 16);
                     if (h == 0) lo = 0;
                     const uint32_t start = (uint32_t)(lo + 1), freq = (uint32_t)(hi - lo - 1);   // "major hax", probability/interface.rs:103-104
-                    if constexpr (TALLY) k.a += __ldg(k.p + (freq & 0x7fffu));
+                    if constexpr (TALLY) { const uint32_t cst = __ldg(k.p + (freq & 0x7fffu)); k.a += cst; if constexpr (HALVES) hh += cst; }
                     else if (g.store0) const_cast<uint32_t *>(k.p)[k.left] = (start & 0xffffu) | (freq << 16);
                     k.left++;
                     int c2 = ch + ((g.l16 >= h) ? inc : 0);
@@ -264,6 +271,7 @@ __device__ __forceinline__ void literal_fast_enc(St &s, Next &nx, const G2 g) {
             done += m;
         }
         s.cur = k; s.l8 = l8; s.lit_ctx = ctx; s.out_pos += done; s.lit_left -= done;
+        if constexpr (HALVES) hv->hi += hh;
         enter_lit_nibble<true, true>(s, nx);
         return;
     }
@@ -290,6 +298,7 @@ __device__ __forceinline__ void literal_fast_enc(St &s, Next &nx, const G2 g) {
         Coder k = s.cur;
         Weights wh = s.c->w_hi, wl = s.c->w_lo;
         bool refused = false;
+        uint64_t hh = 0;
         uint32_t done = 0;
         while (done < n) {
             uint32_t m = n - done;
@@ -308,7 +317,9 @@ __device__ __forceinline__ void literal_fast_enc(St &s, Next &nx, const G2 g) {
                 char *const nbl = lo_tab + (ic * 256u + ib) * 32u, *const cml = cmb + (256u + h + 16u * ctx) * 32u;
                 __syncwarp();
                 const MixVals vl = mix_load(g, nbl, cml);
+                const uint64_t a_h = k.a;
                 mix_finish<TALLY>(k, g, nbh, cmh, vh, sh_, wh, inc, lim, ch_inc, ch_lim, refused);
+                if constexpr (HALVES) hh += k.a - a_h;
                 const MixSym sl_ = mix_search(vl, wl, (int)(byte_in & 0xf));
                 const uint32_t cur = ((uint32_t)sl_.sym | (h << 4)) & 0xff;
                 l8 = (l8 >> 8) | ((unsigned long long)cur << 56);
@@ -325,13 +336,16 @@ __device__ __forceinline__ void literal_fast_enc(St &s, Next &nx, const G2 g) {
         }
         s.cur = k; s.l8 = l8; s.lit_ctx = ctx; s.out_pos += done; s.lit_left -= done;
         s.c->w_hi = wh; s.c->w_lo = wl;
+        if constexpr (HALVES) hv->hi += hh;
         if (refused) s.status = ST_FAIL;
         enter_lit_nibble<true, true>(s, nx);
         return;
     }
     for (uint32_t i = 0; i < n; i++) {
         __syncwarp();
+        const uint64_t a_h = s.cur.a;
         int h = nibble_core_enc<TALLY>(s, nx, g);
+        if constexpr (HALVES) hv->hi += s.cur.a - a_h;
         s.lit_h = (uint32_t)h;
         enter_lit_nibble<true, false>(s, nx);
         __syncwarp();

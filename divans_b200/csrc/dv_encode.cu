@@ -33,7 +33,9 @@ __device__ __forceinline__ void fold_bins(const G2 g, const uint64_t *sbins, con
 // BINS (encode_bins_kernel: TALLY as well) adds each coded literal nibble's cost to bin[mixing-mask index] of the slot's bins and
 // folds them into the stream's per-entry minimum when the pair ends.  It codes every literal on the generic path: the fast
 // loops do not track the mixing-mask index.
-template <bool BLEND, bool TALLY, bool BINS>
+// SPEEDS (encode_speeds_kernel): each stream codes with its own literal speeds, p.v_adapt; with TALLY the pass also sums the
+// cost of the literal high nibbles and of all literal nibbles (LitHalves), on the fast loops as on the generic path.
+template <bool BLEND, bool TALLY, bool BINS, bool SPEEDS>
 __device__ __forceinline__ void encode_model_walk(const EncodeParams &p, const BinParams &bp) {
     extern __shared__ __align__(16) uint8_t smem[];
     const int lane = threadIdx.x & 31;
@@ -67,6 +69,10 @@ __device__ __forceinline__ void encode_model_walk(const EncodeParams &p, const B
     bool exhausted = false;
     const uint32_t per_stream = p.cmd_cap + p.lit_cap;
     uint64_t *const sbins = BINS ? bp.slot_bins + (uint64_t)slot * MIX_ENTRIES : nullptr;
+    // Every cost pass under SPEEDS tallies the halves; only the halves passes' are read (at dynamic mixing 2, where the records'
+    // literals take the mixing loop).  One kernel for all cost passes keeps the uniform, halves and verify walks identical.
+    constexpr bool HALVES = SPEEDS && TALLY;
+    LitHalves hv = {0, 0};
     for (;;) {
         __syncwarp();
         const bool want = (s.state == S_IDLE) && !exhausted;
@@ -89,9 +95,15 @@ __device__ __forceinline__ void encode_model_walk(const EncodeParams &p, const B
                     if (p.force_stride != 0 && dcm == 0 && p.use_context_map) dcm = 1;
                     s.c->desired_context_mixing = dcm; s.c->desired_prior_depth = (uint32_t)p.prior_depth;
                     s.c->desired_force_stride = (uint32_t)p.force_stride; s.c->desired_do_context_map = p.use_context_map != 0;
-                    s.c->have_desired_adapt = p.have_literal_adaptation != 0;
-                    s.c->desired_adapt0 = p.literal_adaptation[0]; s.c->desired_adapt1 = p.literal_adaptation[1];
-                    s.c->desired_adapt2 = p.literal_adaptation[2]; s.c->desired_adapt3 = p.literal_adaptation[3];
+                    if constexpr (SPEEDS) {
+                        const int *a = p.v_adapt + 4ull * v;
+                        s.c->have_desired_adapt = true;
+                        s.c->desired_adapt0 = a[0]; s.c->desired_adapt1 = a[1]; s.c->desired_adapt2 = a[2]; s.c->desired_adapt3 = a[3];
+                    } else {
+                        s.c->have_desired_adapt = p.have_literal_adaptation != 0;
+                        s.c->desired_adapt0 = p.literal_adaptation[0]; s.c->desired_adapt1 = p.literal_adaptation[1];
+                        s.c->desired_adapt2 = p.literal_adaptation[2]; s.c->desired_adapt3 = p.literal_adaptation[3];
+                    }
                     s.c->in.pos = 0;
                     uint32_t win = (uint32_t)p.window_size;   // 0 (command lists only): the window of the blob's header
                     if (p.raw_mode) {
@@ -132,6 +144,7 @@ __device__ __forceinline__ void encode_model_walk(const EncodeParams &p, const B
                             for (uint32_t e = (uint32_t)g.l16; e < MIX_ENTRIES; e += 16) sbins[e] = 0;
                             __syncwarp(g.gmask);
                         }
+                        if constexpr (HALVES) hv = LitHalves{0, 0};
                         s.c->ring_len = 1u << win;
                         coder_init_enc(s.cur, dummy_log); coder_init_enc(s.c->oth, dummy_log);   // (a = 0: the stream's cost so far)
                         enter_cmd_type<true>(s, nx);
@@ -151,6 +164,7 @@ __device__ __forceinline__ void encode_model_walk(const EncodeParams &p, const B
         auto finish = [&]() {
             const uint32_t v = s.c->sidx;
             if (g.store0 && TALLY) { p.status[v] = s.status; p.tally[v] = s.cur.a + s.c->oth.a; }
+            if constexpr (HALVES) if (g.store0) { p.halves[2ull * v] = hv.lit - hv.hi; p.halves[2ull * v + 1] = hv.hi; }
             if constexpr (BINS) fold_bins(g, sbins, bp, v, s.status == ST_OK);
             if (g.store0 && !TALLY) {
                 p.status[v] = s.status;
@@ -162,21 +176,28 @@ __device__ __forceinline__ void encode_model_walk(const EncodeParams &p, const B
             coder_init_enc(s.cur, dummy_log);
         };
         if (!BLEND && !BINS && __all_sync(FULL, s.state == S_LIT_HI)) {
-            literal_fast_enc<TALLY>(s, nx, g);
+            const uint64_t a_in = s.cur.a;
+            literal_fast_enc<TALLY, HALVES>(s, nx, g, &hv);
+            if constexpr (HALVES) hv.lit += s.cur.a - a_in;
             if (s.lit_left == 0 && s.status == ST_OK) { swap_coders(s, g); s.c->in.pos++; enter_cmd_type<true>(s, nx); }
             if (s.status != ST_OK) finish();   // a symbol the loop could not code (enc_log): the stream ends here
             continue;
         }
         const bool busy = s.state != S_IDLE;
         // BINS: the mixing-mask index of a literal nibble (codec/literal.rs:176-183), and the coder's cost before it
-        bool lit_nib = false; uint32_t mmi = 0; uint64_t a0 = 0;
+        bool lit_nib = false, lit_hi = false; uint32_t mmi = 0; uint64_t a0 = 0;
         if constexpr (BINS) {
             lit_nib = s.state == S_LIT_HI || s.state == S_LIT_LO;
             mmi = s.lit_ctx | (s.state == S_LIT_HI ? (uint32_t)(s.l8 >> 60) << 8 : ((s.lit_h & 0xfu) << 8) | 4096u);
             a0 = s.cur.a;
         }
+        if constexpr (HALVES) {
+            lit_hi = s.state == S_LIT_HI; lit_nib = lit_hi || s.state == S_LIT_LO;
+            a0 = s.cur.a;
+        }
         int sym = core_dispatch<BLEND, TALLY>(s, nx, g);
         if constexpr (BINS) if (lit_nib && g.store0) sbins[mmi] += s.cur.a - a0;
+        if constexpr (HALVES) if (lit_nib) { const uint64_t d = s.cur.a - a0; hv.lit += d; if (lit_hi) hv.hi += d; }
         if (!busy) s.cur.left = 0;
         else {
             if (s.status == ST_OK) {   // (else the core could not code the symbol: enc_log)
@@ -193,11 +214,16 @@ __device__ __forceinline__ void encode_model_walk(const EncodeParams &p, const B
 
 template <bool BLEND, bool TALLY>
 __global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) encode_model_kernel(EncodeParams p) {
-    encode_model_walk<BLEND, TALLY, false>(p, BinParams{});
+    encode_model_walk<BLEND, TALLY, false, false>(p, BinParams{});
 }
 template <bool BLEND>
 __global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) encode_bins_kernel(EncodeParams p, BinParams b) {
-    encode_model_walk<BLEND, true, true>(p, b);
+    encode_model_walk<BLEND, true, true, false>(p, b);
+}
+// the model pass (TALLY: the cost pass with literal halves) with per-stream literal speeds
+template <bool BLEND, bool TALLY>
+__global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) encode_speeds_kernel(EncodeParams p) {
+    encode_model_walk<BLEND, TALLY, false, true>(p, BinParams{});
 }
 
 #ifndef DV_BLEND   // (the rANS / mux passes do not depend on the probability model: they live in the default translation unit)
@@ -452,6 +478,11 @@ void launch_encode_bins_blend(const EncodeParams &p, const BinParams &b, uint32_
     size_t smem = (size_t)(DECODE_BLOCK_THREADS / 16) * SMEM_BYTES_PER_GROUP;
     encode_bins_kernel<true><<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p, b);
 }
+void launch_encode_speeds_blend(const EncodeParams &p, bool tally, uint32_t n_blocks, cudaStream_t st) {
+    size_t smem = (size_t)(DECODE_BLOCK_THREADS / 16) * SMEM_BYTES_PER_GROUP;
+    if (tally) encode_speeds_kernel<true, true><<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p);
+    else encode_speeds_kernel<true, false><<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p);
+}
 #else
 void launch_encode_model(const EncodeParams &p, uint32_t n_blocks, cudaStream_t st) {
     size_t smem = (size_t)(DECODE_BLOCK_THREADS / 16) * SMEM_BYTES_PER_GROUP;
@@ -464,6 +495,114 @@ void launch_encode_tally(const EncodeParams &p, uint32_t n_blocks, cudaStream_t 
 void launch_encode_bins(const EncodeParams &p, const BinParams &b, uint32_t n_blocks, cudaStream_t st) {
     size_t smem = (size_t)(DECODE_BLOCK_THREADS / 16) * SMEM_BYTES_PER_GROUP;
     encode_bins_kernel<false><<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p, b);
+}
+void launch_encode_speeds(const EncodeParams &p, bool tally, uint32_t n_blocks, cudaStream_t st) {
+    size_t smem = (size_t)(DECODE_BLOCK_THREADS / 16) * SMEM_BYTES_PER_GROUP;
+    if (tally) encode_speeds_kernel<false, true><<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p);
+    else encode_speeds_kernel<false, false><<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// literal speeds (divans_b200_encode_speeds_*): n streams x k candidate speeds v[0..k), pairs candidate-major (v = c * n + i)
+// ---------------------------------------------------------------------------------------------------------------
+// The k candidate speeds in shared memory, read with constant indices (a dynamically indexed kernel parameter is copied to the
+// stack first).  Every thread of the block calls it before any returns.
+__device__ __forceinline__ void speeds_to_shared(const SpeedValues &vals, int *sv) {
+    if (threadIdx.x == 0) {
+#pragma unroll
+        for (int j = 0; j < 16; j++) sv[j] = vals.v[j];
+    }
+    __syncthreads();
+}
+// One thread per stream.  stage 0: the uniform passes' speeds, (v[c], v[c], v[c], v[c]) for pair (i, c).  stage 1 (after the
+// uniform passes): c* = argmin u[i][.] (ties low, a failed pass costs UINT64_MAX) and the halves passes' speeds
+// (v[c*], v[c*], v[d], v[d]) for pair (i, d).  stage 2 (after them): l* = argmin lo, h* = argmin hi over the passes that did not
+// fail (all failed: c*) and the verify pass's speeds (v[c*], v[c*], v[l*], v[h*]) into x_adapt.  sel[3i .. 3i + 3) = c*, l*, h*.
+__global__ void __launch_bounds__(256) speeds_stage_kernel(int stage, uint64_t n, SpeedValues vals, const uint64_t *tally,
+                                                           const int32_t *v_status, const uint64_t *halves, uint32_t *sel, int *v_adapt,
+                                                           int *x_adapt) {
+    __shared__ int sv[16];
+    speeds_to_shared(vals, sv);
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint32_t k = vals.k;
+    if (stage == 0) {
+        for (uint32_t c = 0; c < k; c++)
+            for (int j = 0; j < 4; j++) v_adapt[((uint64_t)c * n + i) * 4 + j] = sv[c];
+        return;
+    }
+    if (stage == 1) {
+        uint64_t best = ~0ull; uint32_t arg = 0;
+        for (uint32_t c = 0; c < k; c++) {
+            const uint64_t v = (uint64_t)c * n + i;
+            const uint64_t t = v_status[v] == ST_OK ? tally[v] : ~0ull;
+            if (t < best) { best = t; arg = c; }
+        }
+        sel[3 * i] = arg;
+        for (uint32_t d = 0; d < k; d++) {
+            int *a = v_adapt + ((uint64_t)d * n + i) * 4;
+            a[0] = a[1] = sv[arg]; a[2] = a[3] = sv[d];
+        }
+        return;
+    }
+    const uint32_t cs = sel[3 * i];
+    uint64_t blo = ~0ull, bhi = ~0ull; uint32_t lo = cs, hi = cs;
+    for (uint32_t d = 0; d < k; d++) {
+        const uint64_t v = (uint64_t)d * n + i;
+        if (v_status[v] != ST_OK) continue;
+        if (halves[2 * v] < blo) { blo = halves[2 * v]; lo = d; }
+        if (halves[2 * v + 1] < bhi) { bhi = halves[2 * v + 1]; hi = d; }
+    }
+    sel[3 * i + 1] = lo; sel[3 * i + 2] = hi;
+    int *a = x_adapt + i * 4;
+    a[0] = a[1] = sv[cs]; a[2] = sv[lo]; a[3] = sv[hi];
+}
+// One thread per stream: the final choice.  c* = argmin u; x = the verify pass's cost when `tuned` and u[c*] < UINT64_MAX (t2),
+// else u[c*].  (c*, l*, h*) when x < u[c*], else (c*, c*, c*); x_adapt[i] = the chosen speeds, for the encode.  Optional outputs:
+// chosen [3n], cost [n * (k + 1)] = u then x, halves_out [n * k * 2] = the halves passes' (lo, hi) per d, UINT64_MAX for a failed
+// or skipped pass.
+__global__ void __launch_bounds__(256) speeds_select_kernel(uint64_t n, SpeedValues vals, bool tuned, const uint64_t *tally,
+                                                            const int32_t *v_status, const uint64_t *h_halves, const int32_t *h_status,
+                                                            const uint64_t *x_tally, const int32_t *x_status, const uint32_t *sel,
+                                                            int *x_adapt, uint32_t *chosen, uint64_t *cost, uint64_t *halves_out) {
+    __shared__ int sv[16];
+    speeds_to_shared(vals, sv);
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint32_t k = vals.k;
+    uint64_t best = ~0ull; uint32_t arg = 0;
+    for (uint32_t c = 0; c < k; c++) {
+        const uint64_t v = (uint64_t)c * n + i;
+        const uint64_t t = v_status[v] == ST_OK ? tally[v] : ~0ull;
+        if (cost) cost[i * (k + 1) + c] = t;
+        if (t < best) { best = t; arg = c; }
+    }
+    const bool t2 = tuned && best != ~0ull;
+    uint64_t x = best;
+    if (t2) x = x_status[i] == ST_OK ? x_tally[i] : ~0ull;
+    if (cost) cost[i * (k + 1) + k] = x;
+    const bool take = t2 && x < best;
+    const uint32_t a = arg, b = take ? sel[3 * i + 1] : arg, c = take ? sel[3 * i + 2] : arg;
+    if (chosen) { chosen[3 * i] = a; chosen[3 * i + 1] = b; chosen[3 * i + 2] = c; }
+    int *ad = x_adapt + i * 4;
+    ad[0] = ad[1] = sv[a]; ad[2] = sv[b]; ad[3] = sv[c];
+    if (halves_out)
+        for (uint32_t d = 0; d < k; d++) {
+            const uint64_t v = (uint64_t)d * n + i;
+            const bool ok = t2 && h_status[v] == ST_OK;   // (skipped when every uniform pass failed, as the header says)
+            halves_out[(i * k + d) * 2] = ok ? h_halves[2 * v] : ~0ull;
+            halves_out[(i * k + d) * 2 + 1] = ok ? h_halves[2 * v + 1] : ~0ull;
+        }
+}
+void launch_speeds_stage(int stage, uint64_t n, const SpeedValues &vals, const uint64_t *tally, const int32_t *v_status, const uint64_t *halves,
+                         uint32_t *sel, int *v_adapt, int *x_adapt, cudaStream_t st) {
+    speeds_stage_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(stage, n, vals, tally, v_status, halves, sel, v_adapt, x_adapt);
+}
+void launch_speeds_select(uint64_t n, const SpeedValues &vals, bool tuned, const uint64_t *tally, const int32_t *v_status,
+                          const uint64_t *h_halves, const int32_t *h_status, const uint64_t *x_tally, const int32_t *x_status,
+                          const uint32_t *sel, int *x_adapt, uint32_t *chosen, uint64_t *cost, uint64_t *halves_out, cudaStream_t st) {
+    speeds_select_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(n, vals, tuned, tally, v_status, h_halves, h_status, x_tally, x_status,
+                                                                      sel, x_adapt, chosen, cost, halves_out);
 }
 
 // ---------------------------------------------------------------------------------------------------------------

@@ -44,6 +44,15 @@ void launch_mixmap_map(const uint64_t *best, uint64_t n, const MixValues &vals, 
 void launch_mixmap_select(const uint64_t *tally, const int32_t *v_status, const uint64_t *x_tally, const int32_t *x_status, uint64_t n,
                           const MixValues &vals, const uint8_t *records, uint32_t *rec_idx, uint32_t *chosen, uint64_t *cost, uint8_t *mixing,
                           cudaStream_t st);
+// literal speeds: the model pass (tally: the cost pass with literal halves) under per-stream speeds (EncodeParams::v_adapt), the
+// kernel that builds each stage's speeds, and the final choice (dv_encode.cu)
+void launch_encode_speeds(const EncodeParams &p, bool tally, uint32_t n_blocks, cudaStream_t st);
+void launch_encode_speeds_blend(const EncodeParams &p, bool tally, uint32_t n_blocks, cudaStream_t st);
+void launch_speeds_stage(int stage, uint64_t n, const SpeedValues &vals, const uint64_t *tally, const int32_t *v_status, const uint64_t *halves,
+                         uint32_t *sel, int *v_adapt, int *x_adapt, cudaStream_t st);
+void launch_speeds_select(uint64_t n, const SpeedValues &vals, bool tuned, const uint64_t *tally, const int32_t *v_status,
+                          const uint64_t *h_halves, const int32_t *h_status, const uint64_t *x_tally, const int32_t *x_status,
+                          const uint32_t *sel, int *x_adapt, uint32_t *chosen, uint64_t *cost, uint64_t *halves_out, cudaStream_t st);
 // decoding to command lists: the recording decoder (16 lanes per stream, either model) and the pack kernel that finishes the
 // blobs (dv_kernels.cu)
 void launch_decode_v2_rec(bool blend, const DecodeParams &p, const RecParams &r, uint32_t n_blocks, cudaStream_t st);

@@ -402,6 +402,60 @@ DivansResult divans_b200_encode_cmds_mixmap_batch_device(divans_b200_ctx *ctx, s
                                                          const int32_t *values, uint32_t n_values, uint32_t *d_chosen, uint8_t *d_mixing,
                                                          uint64_t *d_cost, uint64_t *d_bins, void *cuda_stream);
 
+/* ---- literal speeds ----
+ * literal_adaptation[4] is ordered stride-low, stride-high, cm-low, cm-high.  [0] adapts both nibbles' stride priors; [1] is
+ * coded in the stream and read by no literal; [2] and [3] adapt the context-map priors of the low and high nibble, which are read
+ * only with dynamic_context_mixing 2.  These calls choose each stream's speeds, by coding cost, from k candidate speeds v[0..k)
+ * under everything else the options say (mode, mixing value, maps).  For stream i:
+ *  1. Uniform passes: the cost walk under (v[c], v[c], v[c], v[c]) gives u[i][c] (T[freq], as encode_auto).  c* = argmin,
+ *     ties to the lowest c.
+ *  2. Only with opts->dynamic_context_mixing >= 2 and k > 1 (and u[i][c*] < UINT64_MAX): halves passes under
+ *     (v[c*], v[c*], v[d], v[d]) give lo[i][d] and hi[i][d], the cost of the literal low and high nibbles, both coders.  l* =
+ *     argmin lo, h* = argmin hi, ties to the lowest d; a failed pass takes no part (all failed: l* = h* = c*).  With dynamic
+ *     mixing 2 and S0 fixed, the low nibbles' cost depends on S2 alone and the high nibbles' on S3 alone, so each half is
+ *     chosen on its own; the command coder also codes the four speeds, so the total is checked:
+ *  3. Verify pass under (v[c*], v[c*], v[l*], v[h*]): x[i].  It is taken only if x[i] < u[i][c*].  When step 2 is skipped,
+ *     x[i] = u[i][c*].  chosen[i] = (a, b, c): (c*, l*, h*) when taken, else (c*, c*, c*).
+ *  4. Stream i's bytes, out_len and status equal divans_b200_encode_batch_host's with have_literal_adaptation = 1 and
+ *     literal_adaptation = {v[a], v[a], v[b], v[c]}; for command lists, divans_b200_encode_cmds_batch_host's (the speeds override
+ *     every record's, as opts->literal_adaptation does).  So no stream costs more than under its best uniform candidate.
+ *  5. A failed pass costs UINT64_MAX.  If every uniform pass fails, chosen = (0, 0, 0) and the stream fails; status 2 as in
+ *     encode_auto.
+ * opts->have_literal_adaptation and opts->literal_adaptation are ignored.  values: 1..16 int16_t[2] (inc, lim), each unchanged by
+ * the f8 round trip the stream codes speeds with and small enough that no literal prior can wrap its i16 counters (so the
+ * streams stay on the decoder's literal fast loops); anything else returns DIVANS_FAILURE before any work, and
+ * divans_b200_last_error names the entry.  Outputs, each may be NULL: chosen [n * 3]; cost [n * (k + 1)], row i = u[i][0..k)
+ * then x[i]; halves [n * k * 2], (lo, hi) of stream i under d at (i * k + d) * 2 (UINT64_MAX for a failed or skipped pass).
+ * Costs are in 1/65536 bit.  The call takes k cost walks (2k + 1 with the halves and verify passes) and the encode; the cost walks run
+ * on the fast literal loops.  Host calls are sub-batched like divans_b200_encode_auto_batch_host; n == 0 returns
+ * DIVANS_SUCCESS. */
+DivansResult divans_b200_encode_speeds_batch_host(divans_b200_ctx *ctx, size_t n, const uint8_t *in, const uint64_t *in_off,
+                                                  const uint64_t *in_len, uint8_t *out, const uint64_t *out_off, const uint64_t *out_cap,
+                                                  uint64_t *out_len, int32_t *status, const divans_b200_encode_options *opts,
+                                                  const int16_t *values, uint32_t n_values, uint32_t *chosen, uint64_t *cost,
+                                                  uint64_t *halves);
+/* Same with the buffers and outputs DEVICE pointers (values is a host array, read before the call returns); one launch sequence,
+ * no host sync; conventions of divans_b200_encode_auto_batch_device. */
+DivansResult divans_b200_encode_speeds_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_in, const uint64_t *d_in_off,
+                                                    const uint64_t *d_in_len, uint64_t max_in_len, uint8_t *d_out,
+                                                    const uint64_t *d_out_off, const uint64_t *d_out_cap, uint64_t *d_out_len,
+                                                    int32_t *d_status, const divans_b200_encode_options *opts, const int16_t *values,
+                                                    uint32_t n_values, uint32_t *d_chosen, uint64_t *d_cost, uint64_t *d_halves,
+                                                    void *cuda_stream);
+/* The same choice for command lists (DVCL blobs): the lists keep their records, commands, literal pool and window; the speeds
+ * override the records'.  Conventions of divans_b200_encode_cmds_auto_batch_host / _device. */
+DivansResult divans_b200_encode_cmds_speeds_batch_host(divans_b200_ctx *ctx, size_t n, const uint8_t *blobs, const uint64_t *blob_off,
+                                                       const uint64_t *blob_len, uint8_t *out, const uint64_t *out_off,
+                                                       const uint64_t *out_cap, uint64_t *out_len, int32_t *status,
+                                                       const divans_b200_encode_options *opts, const int16_t *values, uint32_t n_values,
+                                                       uint32_t *chosen, uint64_t *cost, uint64_t *halves);
+DivansResult divans_b200_encode_cmds_speeds_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_blobs, const uint64_t *d_blob_off,
+                                                         const uint64_t *d_blob_len, uint64_t max_blob_len, uint64_t max_raw_len,
+                                                         uint8_t *d_out, const uint64_t *d_out_off, const uint64_t *d_out_cap,
+                                                         uint64_t *d_out_len, int32_t *d_status, const divans_b200_encode_options *opts,
+                                                         const int16_t *values, uint32_t n_values, uint32_t *d_chosen, uint64_t *d_cost,
+                                                         uint64_t *d_halves, void *cuda_stream);
+
 /* ---- replaying command lists to raw bytes ----
  * Realise n command lists (DVCL blobs, below) as the bytes they describe: the reference's `recode` (src/bin/divans.rs:1108,
  * cmd_to_raw/mod.rs) on the GPU.  List i is blobs[blob_off[i] .. +blob_len[i]); its bytes go to out[out_off[i] .. +out_cap[i]).

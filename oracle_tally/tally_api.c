@@ -397,3 +397,77 @@ int dvo_encode_cmds_cov(const dvo_cmdlist *l, const dvo_options *o, uint32_t *co
     free(out);
     return rc;
 }
+
+/* ---- literal speeds ----
+ * The CPU reference of divans_b200_encode_speeds_* / encode_cmds_speeds_* (include/divans_b200.h, "literal speeds") for the list
+ * `l`, records kept: uniform passes, the halves passes (high = bins [0, 4096), low = bins [4096, 8192), the mixing-mask index of
+ * a high nibble being below 4096), the verify pass, and the encode under the chosen speeds.  values: k (inc, lim) pairs.
+ * Outputs: chosen[3]; cost[k + 1] and halves[k * 2] (lo, hi per d), each may be NULL. */
+static void dvt_set_speeds(dvo_options *o, const int16_t *values, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
+    const uint32_t idx[4] = {a, b, c, d};
+    o->have_literal_adaptation = 1;
+    for (int j = 0; j < 4; j++) { o->literal_adaptation[j].inc = values[2 * idx[j]]; o->literal_adaptation[j].lim = values[2 * idx[j] + 1]; }
+}
+
+static int dvt_speeds(const dvo_cmdlist *l, const dvo_options *o, const int16_t *values, uint32_t k, uint8_t *out, size_t cap,
+                      size_t *out_len, uint32_t *chosen, uint64_t *cost, uint64_t *halves) {
+    uint64_t *b = (uint64_t *)malloc(DVT_MIX * sizeof(uint64_t)), *lo = (uint64_t *)malloc(k * sizeof(uint64_t)),
+             *hi = (uint64_t *)malloc(k * sizeof(uint64_t));
+    int rc = DVO_FAILURE;
+    *out_len = 0;
+    if (!b || !lo || !hi) goto done;
+    dvo_options w = *o;
+    uint64_t u_best = UINT64_MAX; uint32_t cs = 0;
+    for (uint32_t c = 0; c < k; c++) {
+        uint64_t t = UINT64_MAX;
+        dvt_set_speeds(&w, values, c, c, c, c);
+        if (dvo_tally_cmds(l, &w, &t) != DVO_SUCCESS) t = UINT64_MAX;
+        if (cost) cost[c] = t;
+        if (t < u_best) { u_best = t; cs = c; }
+    }
+    const int tuned = o->dynamic_context_mixing >= 2 && k > 1 && u_best != UINT64_MAX;
+    uint32_t ls = cs, hs = cs;
+    uint64_t x = u_best;
+    if (tuned) {
+        uint64_t blo = UINT64_MAX, bhi = UINT64_MAX;
+        for (uint32_t d = 0; d < k; d++) {
+            uint64_t t = UINT64_MAX, nb = 0;
+            dvt_set_speeds(&w, values, cs, cs, d, d);
+            lo[d] = hi[d] = UINT64_MAX;
+            if (dvt_tally_bins(l, &w, &t, b, &nb) == DVO_SUCCESS) {
+                lo[d] = 0; hi[d] = 0;
+                for (uint32_t e = 0; e < DVT_MIX / 2; e++) { hi[d] += b[e]; lo[d] += b[DVT_MIX / 2 + e]; }
+                if (lo[d] < blo) { blo = lo[d]; ls = d; }
+                if (hi[d] < bhi) { bhi = hi[d]; hs = d; }
+            }
+        }
+        dvt_set_speeds(&w, values, cs, cs, ls, hs);
+        if (dvo_tally_cmds(l, &w, &x) != DVO_SUCCESS) x = UINT64_MAX;
+    }
+    for (uint32_t d = 0; d < k && halves; d++) {
+        halves[2 * d] = tuned ? lo[d] : UINT64_MAX;
+        halves[2 * d + 1] = tuned ? hi[d] : UINT64_MAX;
+    }
+    if (cost) cost[k] = x;
+    const int take = tuned && x < u_best;
+    chosen[0] = cs; chosen[1] = take ? ls : cs; chosen[2] = take ? hs : cs;
+    dvt_set_speeds(&w, values, chosen[0], chosen[0], chosen[1], chosen[2]);
+    rc = dvo_encode_cmds(l, &w, out, cap, out_len);
+done:
+    free(b); free(lo); free(hi);
+    return rc;
+}
+
+int dvo_encode_speeds(const uint8_t *in, size_t n, const dvo_options *o, int pred_mode, int mixing_value, const int16_t *values, uint32_t k,
+                      uint8_t *out, size_t cap, size_t *out_len, uint32_t *chosen, uint64_t *cost, uint64_t *halves) {
+    dvo_cmdlist l; dvo_cmdlist_init(&l);
+    dvt_raw_cmds(in, n, o->window_size, pred_mode, mixing_value, &l);
+    int rc = dvt_speeds(&l, o, values, k, out, cap, out_len, chosen, cost, halves);
+    dvo_cmdlist_free(&l);
+    return rc;
+}
+
+int dvo_encode_cmds_speeds(const dvo_cmdlist *l, const dvo_options *o, const int16_t *values, uint32_t k, uint8_t *out, size_t cap,
+                           size_t *out_len, uint32_t *chosen, uint64_t *cost, uint64_t *halves) {
+    return dvt_speeds(l, o, values, k, out, cap, out_len, chosen, cost, halves);
+}

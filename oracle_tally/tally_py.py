@@ -154,6 +154,9 @@ def lib(blend=False):
         L.dvo_encode_cmds_mixmap.argtypes = [vp, op, ctypes.c_int, vp, ctypes.c_uint32, vp, ctypes.c_size_t, szp,
                                              ctypes.POINTER(ctypes.c_uint32), vp, vp, vp]
         L.dvo_recode_blob.argtypes = [vp, ctypes.c_size_t, ctypes.c_int, vp, ctypes.c_size_t, szp]
+        L.dvo_encode_speeds.argtypes = [vp, ctypes.c_size_t, op, ctypes.c_int, ctypes.c_int, vp, ctypes.c_uint32, vp, ctypes.c_size_t, szp,
+                                        vp, vp, vp]
+        L.dvo_encode_cmds_speeds.argtypes = [vp, op, vp, ctypes.c_uint32, vp, ctypes.c_size_t, szp, vp, vp, vp]
         L.dvo_cmdlist_from_blob.argtypes = [vp, ctypes.c_size_t, vp]
         L.dvo_cov_size.restype = ctypes.c_size_t
         L.dvo_encode_cmds_cov.argtypes = [vp, op, vp]
@@ -397,3 +400,60 @@ def coverage_pairs(cov):
         t, typ, idx = prior_of(int(flat))
         out.setdefault((t, typ), {}).setdefault(idx, set()).add(int(nib))
     return out
+
+
+def _speed_to_u8(x):   # the stream's f8 speed code (probability/interface.rs), on an i16
+    u = x & 0xffff
+    length = u.bit_length()
+    mant = 0
+    if x != 0:
+        rem = ((x - (1 << (length - 1))) + 0x8000) % 0x10000 - 0x8000
+        r3 = (((rem << 3) & 0xffff) ^ 0x8000) - 0x8000
+        mant = (r3 >> (length - 1)) & 0xff
+    return ((length << 3) | mant) & 0xff
+
+
+def _u8_to_speed(d):
+    if d < 8:
+        return 0
+    lv = (d >> 3) - 1
+    rem = ((((d & 7) << lv) & 0xffff) ^ 0x8000) - 0x8000
+    return (((1 << lv) | (rem >> 3)) & 0xffff ^ 0x8000) - 0x8000
+
+
+def speed_ok(inc, lim):
+    """whether (inc, lim) is a speed the speeds calls accept: unchanged by the f8 round trip, and unable to wrap an i16 prior"""
+    rt = all(_u8_to_speed(_speed_to_u8(x)) == x for x in (inc, lim))
+    return rt and inc >= 0 and lim >= 0 and lim + inc + 16 <= 0x7fff and 4 * (inc + 16) <= 0x7fff
+
+
+def _speeds_args(values):
+    v = np.ascontiguousarray(values, np.int16).reshape(-1, 2)
+    if not 1 <= v.shape[0] <= 16 or not all(speed_ok(int(a), int(b)) for a, b in v):
+        raise ValueError("speeds: 1..16 speeds that survive the f8 round trip and cannot wrap an i16 prior are required")
+    k = v.shape[0]
+    return v, k, np.zeros(3, np.uint32), np.zeros(k + 1, np.uint64), np.zeros(2 * k, np.uint64)
+
+
+def encode_speeds(data, pred_mode, mixing_value, values, blend=False, **kw):
+    """(rc, stream or None, chosen [3], cost [k + 1], halves [k, 2]): the literal speeds of divans_b200_encode_speeds_batch_host for
+    one raw buffer under the literal model (pred_mode, mixing_value); ``values`` are (inc, lim) pairs"""
+    d = _u8(data)
+    v, k, ch, cost, halves = _speeds_args(values)
+    cap = len(data) + len(data) // 2 + 65536
+    out = np.empty(cap, np.uint8)
+    n = ctypes.c_size_t(0)
+    rc = lib(blend).dvo_encode_speeds(_p(d), len(data), ctypes.byref(options(blend, **kw)), pred_mode, mixing_value, _p(v), k, _p(out), cap,
+                                      ctypes.byref(n), _p(ch), _p(cost), _p(halves))
+    return rc, out[: n.value].tobytes() if rc == SUCCESS else None, ch, cost, halves.reshape(k, 2)
+
+
+def encode_cmds_speeds(cmds, values, blend=False, **kw):
+    """encode_speeds for the command list ``cmds`` (its records kept, the speeds overriding theirs)"""
+    v, k, ch, cost, halves = _speeds_args(values)
+    cap = int(cmds.c.n_lits) * 2 + int(cmds.c.n_cmds) * 16 + (1 << 20)
+    out = np.empty(cap, np.uint8)
+    n = ctypes.c_size_t(0)
+    rc = lib(blend).dvo_encode_cmds_speeds(ctypes.addressof(cmds.c), ctypes.byref(options(blend, **kw)), _p(v), k, _p(out), cap,
+                                           ctypes.byref(n), _p(ch), _p(cost), _p(halves))
+    return rc, out[: n.value].tobytes() if rc == SUCCESS else None, ch, cost, halves.reshape(k, 2)
