@@ -169,7 +169,8 @@ DivansResult divans_b200_decode_batch_host_wait(divans_b200_ctx *ctx, int32_t ti
  * status 3, never written out of bounds); `cuda_stream` is a cudaStream_t (NULL = the context's own stream).
  * Asynchronous: returns after enqueueing.  A context owns ONE set of scratch buffers: calls on the same context are
  * serialised (host mutex + an event that makes each launch set wait for the previous one, whatever stream it is on);
- * for concurrent batches create one context per batch in flight. */
+ * for concurrent batches create one context per batch in flight.  Regions are not cleared first: of region i only
+ * out[out_off[i] .. +out_len[i]) is written (with status 2, the bytes of the commands that fit), the rest holds what it held. */
 DivansResult divans_b200_decode_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_in, const uint64_t *d_in_off,
                                              const uint64_t *d_in_len, uint8_t *d_out, const uint64_t *d_out_off,
                                              const uint64_t *d_out_cap, uint64_t *d_out_len, int32_t *d_status,
@@ -193,7 +194,9 @@ DivansResult divans_b200_decode_cmds_batch_host(divans_b200_ctx *ctx, size_t n, 
                                                 const uint64_t *blob_cap, uint64_t *blob_len, int32_t *status, uint32_t flags);
 /* Same, all pointers are DEVICE pointers.  `in_total_bytes` and `cuda_stream` as for divans_b200_decode_batch_device; asynchronous
  * and serialised on the context exactly as that call.  Regions are not cleared first: past the lengths they hold what they held,
- * except that the records of a failed stream or of a region too small for its blob are zeroed. */
+ * except that the records of a failed stream or of a region too small for its blob are zeroed, and that in a blob region the
+ * bytes where the decoder staged the prediction-mode records (the region's last n_predmodes * PM_RECORD_BYTES) are zeroed past
+ * blob_len[i]. */
 DivansResult divans_b200_decode_cmds_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_in, const uint64_t *d_in_off,
                                                   const uint64_t *d_in_len, uint8_t *d_out, const uint64_t *d_out_off,
                                                   const uint64_t *d_out_cap, uint64_t *d_out_len, uint8_t *d_blobs,
@@ -228,7 +231,10 @@ typedef struct {
 void divans_b200_encode_options_default(divans_b200_encode_options *o);
 
 /* Encode n raw HOST buffers with the reference's internal literal-only command generator
- * (src/raw_to_cmd/mod.rs:105-181): one PredictionMode command + Literal commands. */
+ * (src/raw_to_cmd/mod.rs:105-181): one PredictionMode command + Literal commands.  Of region i only out[out_off[i] ..
+ * +out_len[i]) is written, and only with status 0: the rest of the region holds what it held, and a stream that fails or does
+ * not fit (status 2, out_len the size it needs) writes nothing.  Every encode call below, host or device, writes its regions
+ * the same way. */
 DivansResult divans_b200_encode_batch_host(divans_b200_ctx *ctx, size_t n, const uint8_t *in, const uint64_t *in_off,
                                            const uint64_t *in_len, uint8_t *out, const uint64_t *out_off,
                                            const uint64_t *out_cap, uint64_t *out_len, int32_t *status,
