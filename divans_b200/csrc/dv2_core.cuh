@@ -304,14 +304,53 @@ __device__ __forceinline__ void rans_pair_v2(uint64_t &a, uint64_t &b, const uin
     a = xa; b = xb;
 }
 
+// eager_refill of a split pair (rans_split16), in payload order: `a` takes the word in hand, `b` the one after it when `a`
+// refilled too.  The group's cursor moves exactly as two eager_refill calls move it.
+__device__ __forceinline__ void split_refill16(uint64_t &x, const bool need, const bool bl, const G2 g, FastK &f) {
+    const unsigned v = __ballot_sync(FULL, need);
+    uint32_t wb = f.wnext;
+    if ((v >> g.shift) & 1u) { f.wi = min(f.wi + 1, f.wmax); wb = ld_stream_u32(f.wbase + f.wi); }
+    if (need) x = (x << 32) | (uint64_t)(bl ? wb : f.wnext);
+    if ((v >> (g.shift + 8)) & 1u) { f.wi = min(f.wi + 1, f.wmax); f.wnext = ld_stream_u32(f.wbase + f.wi); }
+    else f.wnext = wb;
+}
+// The same byte at 16 lanes per stream with the two states split across the group: lanes 0-7 keep `a`, lanes 8-15 keep `b`
+// (`x`: this lane's state; `bl`: the lane keeps `b`; `hsel`: the PRMT selector of this lane's 16-bit half, 0x4432 on the `b`
+// lanes, else 0x4410).  Once both symbols are known the two steps are independent, so one set of instructions advances both.
+// Lane i packs element i of both priors (high nibble's in the low half) and each lane fetches its own state's elements sym and
+// sym - 1 with two shuffles.  The divides come after the shuffles, for the lane's own prior only: one reciprocal, two
+// quotients.  Element 15 of the packed word is max, so for sym = 0 the quotient of `lo` is 0x8000 and masks to 0, as in
+// rans_advance_v2.
+__device__ __forceinline__ void rans_split16(uint64_t &x, const uint32_t eh, const uint32_t mh, const int h, const uint32_t el,
+                                             const uint32_t ml, const int l, const bool bl, const uint32_t hsel, const G2 g, FastK &f) {
+    const uint32_t ep = __byte_perm(eh, el, 0x5410);
+    const int sym = bl ? l : h;
+    const uint32_t mv = bl ? ml : mh, inv = recip32(mv), nmv = 0u - mv;
+    // divq, with the remainder taken as n + q * (-max): one negation for both quotients
+    const auto quot = [inv, mv, nmv, hsel](const uint32_t w) {
+        const uint32_t n = __byte_perm(w, 0, hsel) << 15, q = __umulhi(n, inv);
+        return q + (n + q * nmv >= mv ? 1u : 0u);
+    };
+    const uint32_t hi = quot(__shfl_sync(FULL, ep, sym, 16)), lo = quot(__shfl_sync(FULL, ep, sym - 1, 16)) & 0x7fffu;
+    const uint32_t freq = hi - lo - 1, t = ((uint32_t)x & 0x7fffu) - lo - 1;   // (t = -1: see rans_advance_v2)
+    uint64_t nx = (uint64_t)freq * (x >> 15) + (uint64_t)(int64_t)(int32_t)t;
+    const bool need = nx < (1ull << 31);
+    if (__any_sync(FULL, need)) split_refill16(nx, need, bl, g, f);
+    x = nx;
+}
 // bin search: for a monotone CDF whose last element is max (> r) the number of elements with c[i] <= r is sym (the vote
 // counts it directly: no 16 - popc of the complement)
+// (`off`: the state's low 15 bits)
 template <int LPG>
-__device__ __forceinline__ int search_v2(const uint64_t st, const uint32_t ev, const uint32_t mv, const uint32_t bsel) {
-    const uint32_t rr = (((uint32_t)st & 0x7fffu) * mv) >> 15;              // probability/interface.rs:140
+__device__ __forceinline__ int search_off_v2(const uint32_t off, const uint32_t ev, const uint32_t mv, const uint32_t bsel) {
+    const uint32_t rr = (off * mv) >> 15;                                    // probability/interface.rs:140
     if (LPG == 16) return __popc(__ballot_sync(FULL, rr >= ev) & bsel);     // bsel: the group's 16 ballot bits
     const unsigned b0 = __ballot_sync(FULL, rr >= (ev & 0xffffu)), b1 = __ballot_sync(FULL, rr >= (ev >> 16));
     return __popc(__byte_perm(b0, b1, bsel)) >> 1;                          // bsel: PRMT selector [g, 4+g, g, 4+g]
+}
+template <int LPG>
+__device__ __forceinline__ int search_v2(const uint64_t st, const uint32_t ev, const uint32_t mv, const uint32_t bsel) {
+    return search_off_v2<LPG>((uint32_t)st & 0x7fffu, ev, mv, bsel);
 }
 
 // ---- dynamic context mixing >= 2 (codec/literal.rs:219-259), 16 lanes per stream: the stride prior `nb` (tagged literal table) is
@@ -478,8 +517,12 @@ __device__ __forceinline__ bool literal_plain_loop_v2(St &s, Next &nx, const G2 
     // eager-refill coder for the duration of the loop (coder_to_eager).  The literal coder codes nibbles in pairs: state `a`
     // serves every high nibble, `b` every low nibble (two rotations of ans.rs:240-243 are the identity), so the loop never
     // swaps them.
+    // 16 lanes per stream: inside the loop the pair is split (rans_split16), `x` is `a` on lanes 0-7 and `b` on lanes 8-15
     Coder k = s.cur;
     coder_to_eager(k, f, s.slot, active);
+    const bool bl = g.l16 >= 8;
+    const uint32_t hsel = bl ? 0x4432u : 0x4410u;
+    uint64_t x = bl ? k.b : k.a;
     uint32_t done = 0;
     while (done < n) {
         uint32_t m = n - done;
@@ -488,6 +531,7 @@ __device__ __forceinline__ bool literal_plain_loop_v2(St &s, Next &nx, const G2 
             else { k.a = k.b = 0; f.wi = f.wmax; }
             f.wnext = f.wbase[f.wi];
             k.sym_count = 0;
+            x = bl ? k.b : k.a;
         }
         m = min(m, (NUM_SYMBOLS_BEFORE_FLUSH - k.sym_count) >> 1);
         if (LPG == 8) m = min(m, __shfl_xor_sync(FULL, m, 8));
@@ -505,13 +549,17 @@ __device__ __forceinline__ bool literal_plain_loop_v2(St &s, Next &nx, const G2 
         // per trip)
 #pragma unroll (LPG == 16 ? 1 : 2)
         for (uint32_t i = 0; i < m; i++) {
+            // -- the offsets (low 15 bits) of both states on every lane of the group (16 lanes: from the split pair)
+            const uint32_t xm = (uint32_t)x & 0x7fffu;
+            const uint32_t oa = LPG == 16 ? __shfl_sync(FULL, xm, 0, 16) : (uint32_t)k.a & 0x7fffu;
+            const uint32_t ob = LPG == 16 ? __shfl_sync(FULL, xm, 8, 16) : (uint32_t)k.b & 0x7fffu;
             // -- high nibble: search (speculative: the prior is almost always one this stream has written)
             uint32_t eh_v = eh & ~tbits, mh_v = mh & 0x7fffu;
-            int h = search_v2<LPG>(k.a, eh_v, mh_v, bsel);
+            int h = search_off_v2<LPG>(oa, eh_v, mh_v, bsel);
             if (__builtin_expect(!__all_sync(FULL, ((eh ^ f.mytag) & tchk) == 0), 0)) {   // some group met a prior of an older
                 const unsigned okh = __ballot_sync(FULL, ((eh ^ f.mytag) & tchk) == 0);      // stream: default CDF
                 if ((okh & gm) != gm) { eh_v = defe; mh_v = 64u; }
-                h = search_v2<LPG>(k.a, eh_v, mh_v, bsel);
+                h = search_off_v2<LPG>(oa, eh_v, mh_v, bsel);
             }
             // -- low nibble: prior
             const char *const pl = mk_ptr(lo_tab + lit_index_lo(which, ((uint32_t)h & fc) + cl, ib) * 32u, slot_hi);
@@ -521,11 +569,11 @@ __device__ __forceinline__ bool literal_plain_loop_v2(St &s, Next &nx, const G2 
             blend_store_v2<LPG>(eh_v, mh_v, h, ph, g, f);
             // -- low nibble: search
             uint32_t el_v = el & ~tbits, ml_v = ml & 0x7fffu;
-            int l = search_v2<LPG>(k.b, el_v, ml_v, bsel);
+            int l = search_off_v2<LPG>(ob, el_v, ml_v, bsel);
             if (__builtin_expect(!__all_sync(FULL, ((el ^ f.mytag) & tchk) == 0), 0)) {
                 const unsigned okl = __ballot_sync(FULL, ((el ^ f.mytag) & tchk) == 0);
                 if ((okl & gm) != gm) { el_v = defe; ml_v = 64u; }
-                l = search_v2<LPG>(k.b, el_v, ml_v, bsel);
+                l = search_off_v2<LPG>(ob, el_v, ml_v, bsel);
             }
             const uint32_t cur = ((uint32_t)l | ((uint32_t)h << 4)) & 0xffu;
             l8 = (l8 >> 8) | ((unsigned long long)cur << 56);              // push_literal_byte, codec/interface.rs:280-284
@@ -541,11 +589,13 @@ __device__ __forceinline__ bool literal_plain_loop_v2(St &s, Next &nx, const G2 
             cl = (ctx & o1) << 4; ib = (mm & ssb) | ((~mm & 0xffu) & ctx);
             // -- low nibble: blend; then the rANS steps of both nibbles (state a before b: the order of the payload words)
             blend_store_v2<LPG>(el_v, ml_v, l, pl, g, f);
-            rans_pair_v2<LPG>(k.a, k.b, eh_v, mh_v, h, el_v, ml_v, l, f);
+            if (LPG == 16) rans_split16(x, eh_v, mh_v, h, el_v, ml_v, l, bl, hsel, g, f);
+            else rans_pair_v2<LPG>(k.a, k.b, eh_v, mh_v, h, el_v, ml_v, l, f);
         }
         done += m;
         if (active) k.sym_count += 2 * m;
     }
+    if (LPG == 16) { k.a = __shfl_sync(FULL, x, 0, 16); k.b = __shfl_sync(FULL, x, 8, 16); }
     if (!active) return true;
     // the bytes after the last aligned 8-byte store are still only in l8
     if (g.store0) {

@@ -103,8 +103,8 @@ def source_map(csrc):
     for i in range(fn, fn_end):
         if "__builtin_expect(" in src[i]:
             rare.update(range(i + 2, block_end(src, i) + 2))
-    er = next(i for i, s in enumerate(src) if re.search(r"\bvoid eager_refill\(", s))
-    rare.update(range(er + 1, block_end(src, er) + 2))
+    for er in (i for i, s in enumerate(src) if re.search(r"\bvoid (eager_refill|split_refill16)\(", s)):
+        rare.update(range(er + 1, block_end(src, er) + 2))
     return src, body, call, rare
 
 
