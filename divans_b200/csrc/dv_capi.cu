@@ -988,6 +988,16 @@ static bool mixmap_cands(divans_b200_ctx *ctx, const int32_t *values, uint32_t k
     return true;
 }
 
+// The raw calls that build their record from opts (plain and speeds; auto and mixmap check their own candidates): raw_record keeps
+// the mode's low byte, so 256 would code as LSB6 and 4..255 as a record the encoder can only fail on.
+static bool raw_mode_ok(divans_b200_ctx *ctx, int raw_mode, const divans_b200_encode_options *o, const AutoSel *sel) {
+    if (!raw_mode || (sel && !sel->speeds) || (o->literal_pred_mode >= 0 && o->literal_pred_mode <= 3)) return true;
+    char buf[200];
+    snprintf(buf, sizeof buf, "encode: opts->literal_pred_mode %d is outside 0..3", (int)o->literal_pred_mode);
+    ctx->err = buf;
+    return false;
+}
+
 // The four device encode calls: raw buffers (max_raw_len = max_in_len) or command lists (raw_mode 0), each plain or, with
 // `sel` (device chosen / cost), coded under the cheapest candidate literal model.  Host marshalling (the candidates' records,
 // the error strings) may throw, and no C++ exception may cross the C boundary.
@@ -997,6 +1007,7 @@ static DivansResult encode_device_common(divans_b200_ctx *ctx, size_t n, int raw
                                          const divans_b200_encode_options *opts, void *cuda_stream, const AutoSel *sel) try {
     if (!ctx || !opts) return DIVANS_FAILURE;
     if (sel && !sel->speeds && !check_cands(ctx, sel->cands, sel->n_cands, !raw_mode)) return DIVANS_FAILURE;
+    if (!raw_mode_ok(ctx, raw_mode, opts, sel)) return DIVANS_FAILURE;
     if (n == 0) return DIVANS_SUCCESS;
     if (sel && !sel->mixmap && !sel->speeds && !sel->chosen) { ctx->err = raw_mode ? "encode_auto: d_chosen is required" : "encode_cmds_auto: d_chosen is required"; return DIVANS_FAILURE; }
     if (sel && sel->mixmap && n > 0x7fffffffull) { ctx->err = "batch too large"; return DIVANS_FAILURE; }   // (one block per stream)
@@ -1090,6 +1101,7 @@ static DivansResult encode_host_common(divans_b200_ctx *ctx, size_t n, int raw_m
                                        const AutoSel *sel) try {
     if (!ctx || !opts) return DIVANS_FAILURE;
     if (sel && !sel->speeds && !check_cands(ctx, sel->cands, sel->n_cands, !raw_mode)) return DIVANS_FAILURE;
+    if (!raw_mode_ok(ctx, raw_mode, opts, sel)) return DIVANS_FAILURE;
     if (n == 0) return DIVANS_SUCCESS;
     if (sel && !sel->mixmap && !sel->speeds && !sel->chosen) { ctx->err = raw_mode ? "encode_auto: chosen is required" : "encode_cmds_auto: chosen is required"; return DIVANS_FAILURE; }
     if (sel && (uint64_t)n * sel->n_cands > 0xffffffffull) { ctx->err = "batch too large"; return DIVANS_FAILURE; }
@@ -1708,7 +1720,10 @@ extern "C" DivansResult divans_set_option(DivansCompressorState *s, DivansOption
     case DIVANS_OPTION_Q9_5: case DIVANS_OPTION_IR_OPTIMIZER:
         return DIVANS_SUCCESS;   // command-selection knobs of the brotli crate: accepted, no effect on the entropy half
     case DIVANS_OPTION_WINDOW_SIZE: o.window_size = (int32_t)value; return DIVANS_SUCCESS;
-    case DIVANS_OPTION_DYNAMIC_CONTEXT_MIXING: o.dynamic_context_mixing = (int32_t)(value & 0xff); return DIVANS_SUCCESS;
+    // the reference keeps the low byte (`value as u8`) of the next three.  It cannot code a mixing value of 8 or more (it asserts
+    // the value fits the nibble's low 3 bits), a prior depth above 15 or a mode above 3: refused here (include/divans_b200.h,
+    // section 1)
+    case DIVANS_OPTION_DYNAMIC_CONTEXT_MIXING: if ((value & 0xff) > 7) return DIVANS_FAILURE; o.dynamic_context_mixing = (int32_t)(value & 0xff); return DIVANS_SUCCESS;
     case DIVANS_OPTION_USE_BROTLI_COMMAND_SELECTION: if (value > 2) return DIVANS_FAILURE; s->use_brotli = (int)value; return DIVANS_SUCCESS;
     case DIVANS_OPTION_USE_BROTLI_BITSTREAM: if (value != 1) return DIVANS_FAILURE; s->use_brotli = 2; return DIVANS_SUCCESS;
     case DIVANS_OPTION_USE_CONTEXT_MAP: if (value > 1) return DIVANS_FAILURE; o.use_context_map = (int32_t)value; return DIVANS_SUCCESS;
@@ -1717,8 +1732,8 @@ extern "C" DivansResult divans_set_option(DivansCompressorState *s, DivansOption
     case DIVANS_OPTION_LITERAL_ADAPTATION_CM_HIGH: return set_adapt(3);
     case DIVANS_OPTION_LITERAL_ADAPTATION_STRIDE_LOW: return set_adapt(0);
     case DIVANS_OPTION_LITERAL_ADAPTATION_CM_LOW: return set_adapt(2);
-    case DIVANS_OPTION_PRIOR_DEPTH: o.prior_depth = (int32_t)(value & 0xff); return DIVANS_SUCCESS;
-    case DIVANS_OPTION_FORCE_LITERAL_CONTEXT_MODE: o.literal_pred_mode = (int32_t)(value & 0xff); return DIVANS_SUCCESS;
+    case DIVANS_OPTION_PRIOR_DEPTH: if ((value & 0xff) > 15) return DIVANS_FAILURE; o.prior_depth = (int32_t)(value & 0xff); return DIVANS_SUCCESS;
+    case DIVANS_OPTION_FORCE_LITERAL_CONTEXT_MODE: if ((value & 0xff) > 3) return DIVANS_FAILURE; o.literal_pred_mode = (int32_t)(value & 0xff); return DIVANS_SUCCESS;
     default: return DIVANS_FAILURE;
     }
 }

@@ -70,7 +70,17 @@ struct DivansDecompressorState *divans_new_decompressor_with_custom_alloc(struct
 /* reference: src/ffi/mod.rs:236-262.  Streaming contract: offsets are cursors that are advanced; any call may
  * return NEEDS_MORE_INPUT / NEEDS_MORE_OUTPUT and be resumed at byte granularity.  Implementation: input is
  * buffered until the stream's 8-byte trailer has been seen, then the stream is decoded as a batch of one on
- * the GPU and the output is streamed back out. */
+ * the GPU and the output is streamed back out.
+ *  - A bad magic number or a window byte outside 10..24 fails the call that completes the 16-byte header; a record header
+ *    whose size code is above 3, or an end-of-stream marker other than ff fe ff, fails the call that delivers it (the whole
+ *    marker).  The reference's demuxer checks neither (src/mux.rs: it reads a broken marker's next byte as a record header and
+ *    sizes any code as 1024 << 2k); these refusals are the oracle's.  After a DIVANS_FAILURE every later call returns
+ *    DIVANS_FAILURE.
+ *  - Input is taken up to the end of the trailer and no further: *input_offset stops there when more bytes follow, as in the
+ *    reference.  Once all output has been handed out every call returns DIVANS_SUCCESS and writes nothing.
+ *  - The stream does not state its decoded size.  The first attempt decodes into 8 x the stream's size + 64 KiB and each
+ *    NEEDS_MORE_OUTPUT retries at 4 x that, up to DIVANS_B200_MAX_OUTPUT bytes (environment, read once per process; default
+ *    2^32).  A stream that decodes to more fails with DIVANS_FAILURE (so does one the allocator cannot hold). */
 DivansResult divans_decode(struct DivansDecompressorState *state, const uint8_t *input_buf_ptr, size_t input_size,
                            size_t *input_offset, uint8_t *output_buf_ptr, size_t output_size, size_t *output_offset);
 void divans_free_decompressor(struct DivansDecompressorState *mfd);          /* src/ffi/mod.rs:312-323 */
@@ -82,7 +92,28 @@ void divans_decompressor_free_usize(struct DivansDecompressorState *s, size_t *p
 struct DivansCompressorState *divans_new_compressor(void);                                     /* :18-27 */
 struct DivansCompressorState *divans_new_compressor_with_custom_alloc(struct CAllocator alloc); /* :38-52 */
 DivansResult divans_set_option(struct DivansCompressorState *state, DivansOptionSelect selector, uint32_t value); /* :58-67 */
-/* :70-91.  Input is buffered; the stream is produced by the GPU encoder at flush. */
+/* Options map to divans_b200_encode_options as in the reference (src/ffi/compressor.rs:63-166), starting from its defaults
+ * (src/interface.rs:462-484: window 22, dynamic context mixing 1, context map on, stride from the command):
+ *  - WINDOW_SIZE: any value, taken as an i32 and clamped to 10..24 (so 2^31 and above give 10).
+ *  - the four LITERAL_ADAPTATION_*: a palette index 0..14 (Speed::ENCODER_DEFAULT_PALETTE).  The first of them sets all four
+ *    speeds, later ones only their own: STRIDE_LOW [0], STRIDE_HIGH [1], CM_LOW [2], CM_HIGH [3].
+ *  - FORCE_STRIDE_VALUE 0..8; USE_CONTEXT_MAP 0 or 1.
+ *  - DYNAMIC_CONTEXT_MIXING and PRIOR_DEPTH keep the low byte of the value, FORCE_LITERAL_CONTEXT_MODE (LSB6=0 MSB6=1 UTF8=2
+ *    SIGN=3, the mode of the literal-only record) too.
+ *  - USE_BROTLI_COMMAND_SELECTION 0..2 and USE_BROTLI_BITSTREAM 1 are accepted, as are any value of QUALITY, LGBLOCK,
+ *    STRIDE_DETECTION_QUALITY, PRIOR_BITMASK_DETECTION, SPEED_DETECTION_QUALITY, BROTLI_LITERAL_BYTE_SCORE, Q9_5 and
+ *    IR_OPTIMIZER.  None of them changes the output: the encoder always codes the literal-only command list (see
+ *    divans_b200_encode_batch_host), where the reference would select commands with the brotli crate.
+ *  - Other values and selectors, and any call after the first divans_encode or divans_encode_flush, return DIVANS_FAILURE.
+ * Departures: this library refuses at divans_set_option three kinds of value the reference accepts there but cannot code:
+ *  - DYNAMIC_CONTEXT_MIXING with a low byte of 8 or more: the reference panics when encoding starts (the value must fit the
+ *    low 3 bits of its PredictionMode nibble, codec/interface.rs:360, codec/context_map.rs:192);
+ *  - PRIOR_DEPTH with a low byte above 15: the reference codes it as a nibble it does not fit, and fails (with the default
+ *    probability model its stream does not decode back; a blend build indexes past the CDF);
+ *  - FORCE_LITERAL_CONTEXT_MODE with a low byte above 3: only the reference's brotli command selection reads it, as SIGN; the
+ *    mode here is the PredictionMode record's, which the decoder refuses above 3. */
+/* :70-91.  Input is buffered; the stream is produced by the GPU encoder at flush.  After the flush, divans_encode returns
+ * DIVANS_FAILURE, and a flush call once all output has been handed out returns DIVANS_SUCCESS and writes nothing. */
 DivansResult divans_encode(struct DivansCompressorState *state, const uint8_t *input_buf_ptr, size_t input_size,
                            size_t *input_offset, uint8_t *output_buf_ptr, size_t output_size, size_t *output_offset);
 DivansResult divans_encode_flush(struct DivansCompressorState *state, uint8_t *output_buf_ptr, size_t output_size,
@@ -223,7 +254,8 @@ typedef struct {
     int32_t force_stride;           /* 0..8, 9 = take the stride from the command */
     int32_t have_literal_adaptation;
     int16_t literal_adaptation[4][2];
-    int32_t literal_pred_mode;      /* internal literal-only compressor: LSB6=0 MSB6=1 UTF8=2 SIGN=3 */
+    int32_t literal_pred_mode;      /* internal literal-only compressor: LSB6=0 MSB6=1 UTF8=2 SIGN=3; the raw calls that build
+                                       their record from it (plain and speeds) return DIVANS_FAILURE for anything else */
     int32_t literal_mixing_value;   /* internal literal-only compressor: value of all 8192 mixing entries (reference: 4) */
     int32_t model_rev;              /* DIVANS_B200_MODEL_CURRENT (default) or DIVANS_B200_MODEL_WASM_2018 */
     int32_t cdf_model;              /* DIVANS_B200_CDF_FREQUENTIST (default) or DIVANS_B200_CDF_BLEND */

@@ -1429,11 +1429,13 @@ static void internal_predmode(dvo_predmode *pm, int pred_mode, int mixing_value)
     pm->dist_map_len = 4; for (int i = 0; i < 4; i++) pm->dist_map[i] = (uint8_t)(i & 3);
     memset(pm->mixing, mixing_value, 8192);
 }
-int dvo_encode_raw(const uint8_t *in, size_t n, const dvo_options *o, uint8_t *out, size_t cap, size_t *out_len) {
+/* the literal-only list under the PredictionMode record of (pred_mode, mixing_value); dvo_encode_raw's is (LSB6, 4) */
+static int encode_raw_record(const uint8_t *in, size_t n, const dvo_options *o, int pred_mode, int mixing_value, uint8_t *out, size_t cap,
+                             size_t *out_len) {
     dvo_cmdlist l; dvo_cmdlist_init(&l);
     int window = o->window_size < 10 ? 10 : (o->window_size > 24 ? 24 : o->window_size);
     dvo_cmd *c = cl_add(&l); c->type = DVO_CMD_PREDMODE; c->a = 0;
-    internal_predmode(cl_add_pm(&l), 0, 4);
+    internal_predmode(cl_add_pm(&l), pred_mode, mixing_value);
     size_t ring = (size_t)1 << window;
     for (size_t pos = 0; pos < n;) { /* one Literal per ring-buffer fill, raw_to_cmd/mod.rs:55-104,144-181 */
         size_t chunk = n - pos < ring ? n - pos : ring;
@@ -1444,6 +1446,9 @@ int dvo_encode_raw(const uint8_t *in, size_t n, const dvo_options *o, uint8_t *o
     int rc = dvo_encode_cmds(&l, o, out, cap, out_len);
     dvo_cmdlist_free(&l);
     return rc;
+}
+int dvo_encode_raw(const uint8_t *in, size_t n, const dvo_options *o, uint8_t *out, size_t cap, size_t *out_len) {
+    return encode_raw_record(in, n, o, 0, 4, out, cap, out_len);
 }
 
 /* deterministic greedy hash-chain LZ77 (ours; SURVEY 8d "Z" streams): min match 4, max match 2^16, no dictionary */
@@ -1631,15 +1636,11 @@ static void *batch_worker(void *arg) {
         if (i >= j->n) break;
         size_t ol = 0; int rc;
         if (j->mode == 0) rc = dvo_decode(j->in + j->in_off[i], j->in_len[i], j->out + j->out_off[i], j->out_cap[i], &ol, j->skip_crc);
-        else if (!j->lz77 && j->pred_mode == 0 && j->mixing_value == 4) rc = dvo_encode_raw(j->in + j->in_off[i], j->in_len[i], j->o, j->out + j->out_off[i], j->out_cap[i], &ol);
+        else if (!j->lz77)
+            rc = encode_raw_record(j->in + j->in_off[i], j->in_len[i], j->o, j->pred_mode, j->mixing_value, j->out + j->out_off[i], j->out_cap[i], &ol);
         else {
             dvo_cmdlist l; dvo_cmdlist_init(&l);
-            if (j->lz77) dvo_lz77_cmds(j->in + j->in_off[i], j->in_len[i], j->o->window_size, j->pred_mode, j->mixing_value, &l);
-            else {
-                dvo_cmd *c = cl_add(&l); c->type = DVO_CMD_PREDMODE; c->a = 0; internal_predmode(cl_add_pm(&l), j->pred_mode, j->mixing_value);
-                size_t off = cl_add_lit(&l, j->in + j->in_off[i], j->in_len[i]);
-                if (j->in_len[i]) { c = cl_add(&l); c->type = DVO_CMD_LITERAL; c->a = (uint32_t)off; c->b = (uint32_t)j->in_len[i]; }
-            }
+            dvo_lz77_cmds(j->in + j->in_off[i], j->in_len[i], j->o->window_size, j->pred_mode, j->mixing_value, &l);
             rc = dvo_encode_cmds(&l, j->o, j->out + j->out_off[i], j->out_cap[i], &ol);
             dvo_cmdlist_free(&l);
         }

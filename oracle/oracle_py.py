@@ -311,6 +311,22 @@ def decode_batch(blob, in_off, in_len, out_off, out_cap, n_threads=1, skip_crc=F
     return out, out_len, status
 
 
+def encode_raw_list(raws, opts=None, pred_mode=0, mixing_value=4):
+    """(status, stream or None) per raw byte string: the literal-only encode under the PredictionMode record of (pred_mode,
+    mixing_value), status 3 where the encoder refuses a symbol (dvo_encode_raw_batch)"""
+    blob = np.frombuffer(b"".join(raws) or b"\0", np.uint8)
+    in_len = np.array([len(r) for r in raws], np.uint64)
+    in_off = np.concatenate([[0], np.cumsum(in_len)[:-1]]).astype(np.uint64)
+    cap = in_len * np.uint64(2) + np.uint64(70000)
+    out_off = np.concatenate([[0], np.cumsum(cap)[:-1]]).astype(np.uint64)
+    out = np.zeros(int(cap.sum()), np.uint8)
+    out_len, status = np.zeros(len(raws), np.uint64), np.zeros(len(raws), np.int32)
+    o = opts or options()
+    lib().dvo_encode_raw_batch(_ptr(blob), _ptr(in_off), _ptr(in_len), _ptr(out), _ptr(out_off), _ptr(cap), _ptr(out_len), _ptr(status),
+                               len(raws), 1, ctypes.byref(o), 0, pred_mode, mixing_value)
+    return [(int(s), out[int(a):int(a) + int(n)].tobytes() if s == 0 else None) for s, a, n in zip(status, out_off, out_len)]
+
+
 def encode_batch(blob, in_off, in_len, opts=None, n_threads=1, lz77=False, pred_mode=0, mixing_value=4):
     blob = _as_u8(blob)
     in_off, in_len = np.ascontiguousarray(in_off, np.uint64), np.ascontiguousarray(in_len, np.uint64)

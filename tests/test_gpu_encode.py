@@ -237,19 +237,7 @@ def _oracle_cmds(cl, oracle, kw):
 
 def _oracle_raw(oracle, raws, kw, pred_mode, mixing_value):
     """(status, stream) per raw input of the oracle's raw-mode encoder with a literal prediction mode and mixing value"""
-    import ctypes
-    blob = np.frombuffer(b"".join(raws), np.uint8)
-    in_len = np.array([len(r) for r in raws], np.uint64)
-    in_off = np.concatenate([[0], np.cumsum(in_len)[:-1]]).astype(np.uint64)
-    cap = in_len * np.uint64(2) + np.uint64(70000)
-    out_off = np.concatenate([[0], np.cumsum(cap)[:-1]]).astype(np.uint64)
-    out = np.zeros(int(cap.sum()), np.uint8)
-    out_len, status = np.zeros(len(raws), np.uint64), np.zeros(len(raws), np.int32)
-    p = lambda a: a.ctypes.data_as(ctypes.c_void_p)
-    o = oracle.options(**kw)
-    oracle.lib().dvo_encode_raw_batch(p(blob), p(in_off), p(in_len), p(out), p(out_off), p(cap), p(out_len), p(status), len(raws), 1,
-                                      ctypes.byref(o), 0, pred_mode, mixing_value)
-    return [(int(s), out[int(a):int(a) + int(n)].tobytes() if s == 0 else None) for s, a, n in zip(status, out_off, out_len)]
+    return oracle.encode_raw_list(raws, oracle.options(**kw), pred_mode, mixing_value)
 
 
 def _compare(got, ref, what):
