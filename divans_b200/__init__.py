@@ -157,36 +157,14 @@ def load_library():
     L.divans_b200_encode_cmds_batch_device.argtypes = [vp, sz, vp, vp, vp, ctypes.c_uint64, ctypes.c_uint64, vp, vp, vp, vp, vp,
                                                        ctypes.POINTER(EncodeOptions), vp]
     L.divans_b200_encode_cmds_batch_device.restype = ctypes.c_uint8
-    L.divans_b200_encode_auto_batch_host.argtypes = batch + [ctypes.POINTER(EncodeOptions), vp, ctypes.c_uint32, vp, vp]
-    L.divans_b200_encode_auto_batch_host.restype = ctypes.c_uint8
-    L.divans_b200_encode_auto_batch_device.argtypes = [vp, sz, vp, vp, vp, ctypes.c_uint64, vp, vp, vp, vp, vp, ctypes.POINTER(EncodeOptions),
-                                                       vp, ctypes.c_uint32, vp, vp, vp]
-    L.divans_b200_encode_auto_batch_device.restype = ctypes.c_uint8
-    L.divans_b200_encode_cmds_auto_batch_host.argtypes = batch + [ctypes.POINTER(EncodeOptions), vp, ctypes.c_uint32, vp, vp]
-    L.divans_b200_encode_cmds_auto_batch_host.restype = ctypes.c_uint8
-    L.divans_b200_encode_cmds_auto_batch_device.argtypes = [vp, sz, vp, vp, vp, ctypes.c_uint64, ctypes.c_uint64, vp, vp, vp, vp, vp,
-                                                            ctypes.POINTER(EncodeOptions), vp, ctypes.c_uint32, vp, vp, vp]
-    L.divans_b200_encode_cmds_auto_batch_device.restype = ctypes.c_uint8
-    L.divans_b200_encode_mixmap_batch_host.argtypes = batch + [ctypes.POINTER(EncodeOptions), vp, ctypes.c_uint32, vp, vp, vp, vp]
-    L.divans_b200_encode_mixmap_batch_host.restype = ctypes.c_uint8
-    L.divans_b200_encode_cmds_mixmap_batch_host.argtypes = batch + [ctypes.POINTER(EncodeOptions), vp, ctypes.c_uint32, vp, vp, vp, vp]
-    L.divans_b200_encode_cmds_mixmap_batch_host.restype = ctypes.c_uint8
-    L.divans_b200_encode_mixmap_batch_device.argtypes = [vp, sz, vp, vp, vp, ctypes.c_uint64, vp, vp, vp, vp, vp, ctypes.POINTER(EncodeOptions),
-                                                         vp, ctypes.c_uint32, vp, vp, vp, vp, vp]
-    L.divans_b200_encode_mixmap_batch_device.restype = ctypes.c_uint8
-    L.divans_b200_encode_cmds_mixmap_batch_device.argtypes = [vp, sz, vp, vp, vp, ctypes.c_uint64, ctypes.c_uint64, vp, vp, vp, vp, vp,
-                                                              ctypes.POINTER(EncodeOptions), vp, ctypes.c_uint32, vp, vp, vp, vp, vp]
-    L.divans_b200_encode_cmds_mixmap_batch_device.restype = ctypes.c_uint8
-    L.divans_b200_encode_speeds_batch_host.argtypes = batch + [ctypes.POINTER(EncodeOptions), vp, ctypes.c_uint32, vp, vp, vp]
-    L.divans_b200_encode_speeds_batch_host.restype = ctypes.c_uint8
-    L.divans_b200_encode_cmds_speeds_batch_host.argtypes = batch + [ctypes.POINTER(EncodeOptions), vp, ctypes.c_uint32, vp, vp, vp]
-    L.divans_b200_encode_cmds_speeds_batch_host.restype = ctypes.c_uint8
-    L.divans_b200_encode_speeds_batch_device.argtypes = [vp, sz, vp, vp, vp, ctypes.c_uint64, vp, vp, vp, vp, vp, ctypes.POINTER(EncodeOptions),
-                                                         vp, ctypes.c_uint32, vp, vp, vp, vp]
-    L.divans_b200_encode_speeds_batch_device.restype = ctypes.c_uint8
-    L.divans_b200_encode_cmds_speeds_batch_device.argtypes = [vp, sz, vp, vp, vp, ctypes.c_uint64, ctypes.c_uint64, vp, vp, vp, vp, vp,
-                                                              ctypes.POINTER(EncodeOptions), vp, ctypes.c_uint32, vp, vp, vp, vp]
-    L.divans_b200_encode_cmds_speeds_batch_device.restype = ctypes.c_uint8
+    # the selection calls: a batch, the options and k candidates, then the selection's outputs (device calls: and the CUDA stream)
+    for stem, n_outs in (("auto", 2), ("mixmap", 4), ("speeds", 3)):
+        sel = [ctypes.POINTER(EncodeOptions), vp, ctypes.c_uint32] + [vp] * n_outs
+        for cmds in (False, True):
+            name = "divans_b200_encode_%s%s_batch_" % ("cmds_" if cmds else "", stem)
+            getattr(L, name + "host").argtypes = batch + sel
+            getattr(L, name + "device").argtypes = [vp, sz, vp, vp, vp] + [ctypes.c_uint64] * (2 if cmds else 1) + [vp] * 5 + sel + [vp]
+            getattr(L, name + "host").restype = getattr(L, name + "device").restype = ctypes.c_uint8
     L.divans_b200_replay_cmds_batch_host.argtypes = batch + [ctypes.c_int32]
     L.divans_b200_replay_cmds_batch_host.restype = ctypes.c_uint8
     L.divans_b200_replay_cmds_batch_device.argtypes = batch + [ctypes.c_int32, vp]
@@ -514,13 +492,13 @@ class Engine:
             idx = [i for i, x in enumerate(wins) if x == w]
             ow = EncodeOptions.from_buffer_copy(o)
             ow.window_size = w
-            st, outs, ch, co = self._encode_lists([dec[i][2] for i in idx], ow, True, auto, candidates)
+            st, outs, *sel = self._encode_lists([dec[i][2] for i in idx], ow, True, *((self._auto_host, candidates) if auto else ()))
             if (st != 0).any():
                 raise DivansError("encode failed for streams %s" % np.array(idx)[np.nonzero(st)[0][:8]])
             for k, i in enumerate(idx):
                 res[i] = outs[k]
             if auto:
-                chosen[idx], cost[idx] = ch, co
+                chosen[idx], cost[idx] = sel
         return (res, chosen, cost) if auto else res
 
     def encode_batch_host(self, in_blob, in_off, in_len, out, out_off, out_cap, opts=None, cmds=False):
@@ -551,19 +529,32 @@ class Engine:
             arr[i].literal_pred_mode, arr[i].literal_mixing_value = int(pm), int(mv)
         return arr, len(cs)
 
-    def _auto_host(self, cmds, in_blob, in_off, in_len, out, out_off, out_cap, opts, candidates):
+    def _select_host(self, stem, cmds, in_blob, in_off, in_len, out, out_off, out_cap, opts, cands, k, outs):
+        """The host call of selection ``stem`` (auto, mixmap or speeds; ``cmds``: its command-list call) with the candidates
+        ``cands`` (a pointer), ``k`` of them, and the output arrays ``outs`` (None: not wanted).  Returns (out_len, status)."""
+        name = "encode_%s%s" % ("cmds_" if cmds else "", stem)
         n = len(in_off)
         in_off, in_len, out_off, out_cap, out_len, status = _host_batch(in_off, in_len, out_off, out_cap)
-        cands, nc = self._cands(candidates, cmds)
-        chosen = np.zeros(n, np.uint32)
-        cost = np.zeros((n, nc), np.uint64)
-        o = opts or encode_options()
-        fn = self._L.divans_b200_encode_cmds_auto_batch_host if cmds else self._L.divans_b200_encode_auto_batch_host
-        rc = fn(self._h, n, _ptr(in_blob), _ptr(in_off), _ptr(in_len), _ptr(out), _ptr(out_off), _ptr(out_cap), _ptr(out_len), _ptr(status),
-                ctypes.byref(o), ctypes.addressof(cands), nc, _ptr(chosen), _ptr(cost))
+        rc = getattr(self._L, "divans_b200_%s_batch_host" % name)(
+            self._h, n, _ptr(in_blob), _ptr(in_off), _ptr(in_len), _ptr(out), _ptr(out_off), _ptr(out_cap), _ptr(out_len), _ptr(status),
+            ctypes.byref(opts or encode_options()), cands, k, *(None if a is None else _ptr(a) for a in outs))
         if rc != DIVANS_SUCCESS:
-            raise DivansError("%s_batch_host: %s" % ("encode_cmds_auto" if cmds else "encode_auto", self._err()))
-        return out_len, status, chosen, cost
+            raise DivansError("%s_batch_host: %s" % (name, self._err()))
+        return out_len, status
+
+    def _select_device(self, stem, cmds, batch, opts, cands, k, outs, stream):
+        """The device call of selection ``stem`` on ``batch`` (its arguments from n to d_status) with device outputs ``outs``."""
+        name = "encode_%s%s" % ("cmds_" if cmds else "", stem)
+        rc = getattr(self._L, "divans_b200_%s_batch_device" % name)(self._h, *batch, ctypes.byref(opts or encode_options()), cands, k, *outs,
+                                                                    stream)
+        if rc != DIVANS_SUCCESS:
+            raise DivansError("%s_batch_device: %s" % (name, self._err()))
+
+    def _auto_host(self, cmds, in_blob, in_off, in_len, out, out_off, out_cap, opts, candidates):
+        cands, nc = self._cands(candidates, cmds)
+        chosen, cost = np.zeros(len(in_off), np.uint32), np.zeros((len(in_off), nc), np.uint64)
+        return self._select_host("auto", cmds, in_blob, in_off, in_len, out, out_off, out_cap, opts, ctypes.addressof(cands), nc,
+                                 (chosen, cost)) + (chosen, cost)
 
     def encode_auto_batch_host(self, in_blob, in_off, in_len, out, out_off, out_cap, opts=None, candidates=None):
         """encode_batch_host with each stream's literal model chosen among ``candidates`` ((pred_mode, mixing_value) pairs,
@@ -583,48 +574,41 @@ class Engine:
         """encode_auto_batch_host with raw device pointers (ints; d_chosen u32 [n], d_cost u64 [n * C] or None).  Asynchronous
         on ``stream``."""
         cands, nc = self._cands(candidates)
-        o = opts or encode_options()
-        rc = self._L.divans_b200_encode_auto_batch_device(self._h, n, d_in, d_in_off, d_in_len, int(max_in_len), d_out, d_out_off, d_out_cap,
-                                                          d_out_len, d_status, ctypes.byref(o), ctypes.addressof(cands), nc, d_chosen,
-                                                          d_cost, stream)
-        if rc != DIVANS_SUCCESS:
-            raise DivansError("encode_auto_batch_device: " + self._err())
+        self._select_device("auto", False, (n, d_in, d_in_off, d_in_len, int(max_in_len), d_out, d_out_off, d_out_cap, d_out_len, d_status), opts,
+                            ctypes.addressof(cands), nc, (d_chosen, d_cost), stream)
 
     def encode_cmds_auto_batch_device(self, n, d_blobs, d_blob_off, d_blob_len, max_blob_len, max_raw_len, d_out, d_out_off, d_out_cap,
                                       d_out_len, d_status, d_chosen, d_cost=None, opts=None, candidates=None, stream=None):
         """encode_cmds_batch_device with each list coded under the cheapest of ``candidates`` (as encode_cmds_auto_batch_host;
         d_chosen u32 [n], d_cost u64 [n * C] or None).  Asynchronous on ``stream``."""
         cands, nc = self._cands(candidates, cmds=True)
-        o = opts or encode_options()
-        rc = self._L.divans_b200_encode_cmds_auto_batch_device(self._h, n, d_blobs, d_blob_off, d_blob_len, int(max_blob_len), int(max_raw_len),
-                                                               d_out, d_out_off, d_out_cap, d_out_len, d_status, ctypes.byref(o),
-                                                               ctypes.addressof(cands), nc, d_chosen, d_cost, stream)
-        if rc != DIVANS_SUCCESS:
-            raise DivansError("encode_cmds_auto_batch_device: " + self._err())
+        self._select_device("auto", True, (n, d_blobs, d_blob_off, d_blob_len, int(max_blob_len), int(max_raw_len), d_out, d_out_off, d_out_cap,
+                                           d_out_len, d_status), opts, ctypes.addressof(cands), nc, (d_chosen, d_cost), stream)
 
-    def _encode_lists(self, bufs, opts, cmds, auto, candidates=None):
-        """Byte strings (raw, or command lists with ``cmds``) through encode_batch_host, or with ``auto`` through
-        encode_auto / encode_cmds_auto: (status, list of bytes or None, chosen, cost), chosen and cost None without ``auto``."""
+    def _encode_lists(self, bufs, opts, cmds, host=None, *args):
+        """Byte strings (raw, or command lists with ``cmds``) through encode_batch_host, or through the selection's host call
+        ``host`` (_auto_host, _mixmap_host or _speeds_host, with ``args`` after the options): (status, list of bytes or None,
+        then the selection's other results)."""
         blob, in_off, in_len = _pack(bufs)
         out_cap = _encoded_cap(in_len)
         out_off, out_total = _regions(out_cap)
         out = np.zeros(out_total, np.uint8)
-        if auto:
-            out_len, status, chosen, cost = self._auto_host(cmds, blob, in_off, in_len, out, out_off, out_cap, opts, candidates)
+        if host is None:
+            out_len, status, *rest = self.encode_batch_host(blob, in_off, in_len, out, out_off, out_cap, opts, cmds)
         else:
-            (out_len, status), chosen, cost = self.encode_batch_host(blob, in_off, in_len, out, out_off, out_cap, opts, cmds), None, None
-        return status, [out[int(o):int(o) + int(n)].tobytes() if s == DIVANS_SUCCESS else None for s, o, n in zip(status, out_off, out_len)], \
-            chosen, cost
+            out_len, status, *rest = host(cmds, blob, in_off, in_len, out, out_off, out_cap, opts, *args)
+        return (status, [out[int(o):int(o) + int(n)].tobytes() if s == DIVANS_SUCCESS else None for s, o, n in zip(status, out_off, out_len)],
+                *rest)
 
     def encode_auto(self, raws, opts=None, candidates=None):
         """Convenience: list of raw byte strings -> list of (status, .divans bytes or None, chosen candidate index)."""
-        status, outs, chosen, _ = self._encode_lists(raws, opts, False, True, candidates)
+        status, outs, chosen, _ = self._encode_lists(raws, opts, False, self._auto_host, candidates)
         return [(int(s), b, int(c)) for s, b, c in zip(status, outs, chosen)]
 
     def encode_cmds_auto(self, blobs, opts=None, candidates=None):
         """Convenience: list of DVCL command-list blobs -> list of (status, .divans bytes or None, chosen candidate index), each
         list coded under the cheapest of ``candidates`` (encode_cmds_auto_batch_host)."""
-        status, outs, chosen, _ = self._encode_lists(blobs, opts, True, True, candidates)
+        status, outs, chosen, _ = self._encode_lists(blobs, opts, True, self._auto_host, candidates)
         return [(int(s), b, int(c)) for s, b, c in zip(status, outs, chosen)]
 
     # ---- per-context mixing values (include/divans_b200.h) ----
@@ -635,19 +619,11 @@ class Engine:
 
     def _mixmap_host(self, cmds, in_blob, in_off, in_len, out, out_off, out_cap, opts, values, want_bins):
         n = len(in_off)
-        in_off, in_len, out_off, out_cap, out_len, status = _host_batch(in_off, in_len, out_off, out_cap)
         v, k = self._values(values)
-        chosen = np.zeros(n, np.uint32)
-        mixing = np.zeros((n, MIX_ENTRIES), np.uint8)
-        cost = np.zeros((n, k + 1), np.uint64)
+        chosen, mixing, cost = np.zeros(n, np.uint32), np.zeros((n, MIX_ENTRIES), np.uint8), np.zeros((n, k + 1), np.uint64)
         bins = np.zeros((n, k, MIX_ENTRIES), np.uint64) if want_bins else None
-        o = opts or encode_options()
-        fn = self._L.divans_b200_encode_cmds_mixmap_batch_host if cmds else self._L.divans_b200_encode_mixmap_batch_host
-        rc = fn(self._h, n, _ptr(in_blob), _ptr(in_off), _ptr(in_len), _ptr(out), _ptr(out_off), _ptr(out_cap), _ptr(out_len), _ptr(status),
-                ctypes.byref(o), _ptr(v), k, _ptr(chosen), _ptr(mixing), _ptr(cost), _ptr(bins) if want_bins else None)
-        if rc != DIVANS_SUCCESS:
-            raise DivansError("%s_batch_host: %s" % ("encode_cmds_mixmap" if cmds else "encode_mixmap", self._err()))
-        return out_len, status, chosen, mixing, cost, bins
+        return self._select_host("mixmap", cmds, in_blob, in_off, in_len, out, out_off, out_cap, opts, _ptr(v), k,
+                                 (chosen, mixing, cost, bins)) + (chosen, mixing, cost, bins)
 
     def encode_mixmap_batch_host(self, in_blob, in_off, in_len, out, out_off, out_cap, opts=None, values=None, bins=False):
         """encode_batch_host with each stream's mixing values chosen per literal context among ``values`` (default
@@ -663,42 +639,27 @@ class Engine:
                                    d_chosen=None, d_mixing=None, d_cost=None, d_bins=None, opts=None, values=None, stream=None):
         """encode_mixmap_batch_host with raw device pointers (ints, or None for an output not wanted).  Asynchronous."""
         v, k = self._values(values)
-        o = opts or encode_options()
-        rc = self._L.divans_b200_encode_mixmap_batch_device(self._h, n, d_in, d_in_off, d_in_len, int(max_in_len), d_out, d_out_off, d_out_cap,
-                                                            d_out_len, d_status, ctypes.byref(o), _ptr(v), k, d_chosen, d_mixing, d_cost,
-                                                            d_bins, stream)
-        if rc != DIVANS_SUCCESS:
-            raise DivansError("encode_mixmap_batch_device: " + self._err())
+        self._select_device("mixmap", False, (n, d_in, d_in_off, d_in_len, int(max_in_len), d_out, d_out_off, d_out_cap, d_out_len, d_status),
+                            opts, _ptr(v), k, (d_chosen, d_mixing, d_cost, d_bins), stream)
 
     def encode_cmds_mixmap_batch_device(self, n, d_blobs, d_blob_off, d_blob_len, max_blob_len, max_raw_len, d_out, d_out_off, d_out_cap,
                                         d_out_len, d_status, d_chosen=None, d_mixing=None, d_cost=None, d_bins=None, opts=None, values=None,
                                         stream=None):
         """encode_cmds_mixmap_batch_host with raw device pointers (ints, or None for an output not wanted).  Asynchronous."""
         v, k = self._values(values)
-        o = opts or encode_options()
-        rc = self._L.divans_b200_encode_cmds_mixmap_batch_device(self._h, n, d_blobs, d_blob_off, d_blob_len, int(max_blob_len),
-                                                                 int(max_raw_len), d_out, d_out_off, d_out_cap, d_out_len, d_status,
-                                                                 ctypes.byref(o), _ptr(v), k, d_chosen, d_mixing, d_cost, d_bins, stream)
-        if rc != DIVANS_SUCCESS:
-            raise DivansError("encode_cmds_mixmap_batch_device: " + self._err())
-
-    def _mixmap_lists(self, bufs, opts, cmds, values):
-        blob, in_off, in_len = _pack(bufs)
-        out_cap = _encoded_cap(in_len)
-        out_off, out_total = _regions(out_cap)
-        out = np.zeros(out_total, np.uint8)
-        out_len, status, chosen, _, _, _ = self._mixmap_host(cmds, blob, in_off, in_len, out, out_off, out_cap, opts, values, False)
-        return [(int(s), out[int(o):int(o) + int(n)].tobytes() if s == DIVANS_SUCCESS else None, int(c))
-                for s, o, n, c in zip(status, out_off, out_len, chosen)]
+        self._select_device("mixmap", True, (n, d_blobs, d_blob_off, d_blob_len, int(max_blob_len), int(max_raw_len), d_out, d_out_off, d_out_cap,
+                                             d_out_len, d_status), opts, _ptr(v), k, (d_chosen, d_mixing, d_cost, d_bins), stream)
 
     def encode_mixmap(self, raws, opts=None, values=None):
         """Convenience: list of raw byte strings -> list of (status, .divans bytes or None, chosen): chosen < k is the uniform
         value values[chosen], k the per-context record (encode_mixmap_batch_host)."""
-        return self._mixmap_lists(raws, opts, False, values)
+        status, outs, chosen, _, _, _ = self._encode_lists(raws, opts, False, self._mixmap_host, values, False)
+        return [(int(s), b, int(c)) for s, b, c in zip(status, outs, chosen)]
 
     def encode_cmds_mixmap(self, blobs, opts=None, values=None):
         """Convenience: encode_mixmap for DVCL command-list blobs (encode_cmds_mixmap_batch_host)."""
-        return self._mixmap_lists(blobs, opts, True, values)
+        status, outs, chosen, _, _, _ = self._encode_lists(blobs, opts, True, self._mixmap_host, values, False)
+        return [(int(s), b, int(c)) for s, b, c in zip(status, outs, chosen)]
 
     # ---- literal speeds (include/divans_b200.h) ----
     @staticmethod
@@ -708,18 +669,10 @@ class Engine:
 
     def _speeds_host(self, cmds, in_blob, in_off, in_len, out, out_off, out_cap, opts, values):
         n = len(in_off)
-        in_off, in_len, out_off, out_cap, out_len, status = _host_batch(in_off, in_len, out_off, out_cap)
         v, k = self._speeds(values)
-        chosen = np.zeros((n, 3), np.uint32)
-        cost = np.zeros((n, k + 1), np.uint64)
-        halves = np.zeros((n, k, 2), np.uint64)
-        o = opts or encode_options()
-        fn = self._L.divans_b200_encode_cmds_speeds_batch_host if cmds else self._L.divans_b200_encode_speeds_batch_host
-        rc = fn(self._h, n, _ptr(in_blob), _ptr(in_off), _ptr(in_len), _ptr(out), _ptr(out_off), _ptr(out_cap), _ptr(out_len), _ptr(status),
-                ctypes.byref(o), _ptr(v), k, _ptr(chosen), _ptr(cost), _ptr(halves))
-        if rc != DIVANS_SUCCESS:
-            raise DivansError("%s_batch_host: %s" % ("encode_cmds_speeds" if cmds else "encode_speeds", self._err()))
-        return out_len, status, chosen, cost, halves
+        chosen, cost, halves = np.zeros((n, 3), np.uint32), np.zeros((n, k + 1), np.uint64), np.zeros((n, k, 2), np.uint64)
+        return self._select_host("speeds", cmds, in_blob, in_off, in_len, out, out_off, out_cap, opts, _ptr(v), k,
+                                 (chosen, cost, halves)) + (chosen, cost, halves)
 
     def encode_speeds_batch_host(self, in_blob, in_off, in_len, out, out_off, out_cap, opts=None, values=None):
         """encode_batch_host with each stream's literal speeds chosen among ``values`` ((inc, lim) pairs, default
@@ -735,35 +688,23 @@ class Engine:
                                    d_chosen=None, d_cost=None, d_halves=None, opts=None, values=None, stream=None):
         """encode_speeds_batch_host with raw device pointers (ints, or None for an output not wanted).  Asynchronous."""
         v, k = self._speeds(values)
-        o = opts or encode_options()
-        rc = self._L.divans_b200_encode_speeds_batch_device(self._h, n, d_in, d_in_off, d_in_len, int(max_in_len), d_out, d_out_off, d_out_cap,
-                                                            d_out_len, d_status, ctypes.byref(o), _ptr(v), k, d_chosen, d_cost, d_halves, stream)
-        if rc != DIVANS_SUCCESS:
-            raise DivansError("encode_speeds_batch_device: " + self._err())
+        self._select_device("speeds", False, (n, d_in, d_in_off, d_in_len, int(max_in_len), d_out, d_out_off, d_out_cap, d_out_len, d_status),
+                            opts, _ptr(v), k, (d_chosen, d_cost, d_halves), stream)
 
     def encode_cmds_speeds_batch_device(self, n, d_blobs, d_blob_off, d_blob_len, max_blob_len, max_raw_len, d_out, d_out_off, d_out_cap,
                                         d_out_len, d_status, d_chosen=None, d_cost=None, d_halves=None, opts=None, values=None, stream=None):
         """encode_cmds_speeds_batch_host with raw device pointers (ints, or None for an output not wanted).  Asynchronous."""
         v, k = self._speeds(values)
-        o = opts or encode_options()
-        rc = self._L.divans_b200_encode_cmds_speeds_batch_device(self._h, n, d_blobs, d_blob_off, d_blob_len, int(max_blob_len),
-                                                                 int(max_raw_len), d_out, d_out_off, d_out_cap, d_out_len, d_status,
-                                                                 ctypes.byref(o), _ptr(v), k, d_chosen, d_cost, d_halves, stream)
-        if rc != DIVANS_SUCCESS:
-            raise DivansError("encode_cmds_speeds_batch_device: " + self._err())
+        self._select_device("speeds", True, (n, d_blobs, d_blob_off, d_blob_len, int(max_blob_len), int(max_raw_len), d_out, d_out_off, d_out_cap,
+                                             d_out_len, d_status), opts, _ptr(v), k, (d_chosen, d_cost, d_halves), stream)
 
     def _speeds_lists(self, bufs, opts, cmds, values):
-        blob, in_off, in_len = _pack(bufs)
-        out_cap = _encoded_cap(in_len)
-        out_off, out_total = _regions(out_cap)
-        out = np.zeros(out_total, np.uint8)
-        out_len, status, chosen, cost, _ = self._speeds_host(cmds, blob, in_off, in_len, out, out_off, out_cap, opts, values)
+        status, outs, chosen, cost, _ = self._encode_lists(bufs, opts, cmds, self._speeds_host, values)
         v, _ = self._speeds(values)
         res = []
-        for i, (s, o, n) in enumerate(zip(status, out_off, out_len)):
-            a, b, c = (int(x) for x in chosen[i])
-            sp = [tuple(int(x) for x in v[j]) for j in (a, a, b, c)]
-            res.append((int(s), out[int(o):int(o) + int(n)].tobytes() if s == DIVANS_SUCCESS else None, sp, [int(x) for x in cost[i]]))
+        for i, (s, b) in enumerate(zip(status, outs)):
+            a, b2, c = (int(x) for x in chosen[i])
+            res.append((int(s), b, [tuple(int(x) for x in v[j]) for j in (a, a, b2, c)], [int(x) for x in cost[i]]))
         return res
 
     def encode_speeds(self, raws, opts=None, values=None):
@@ -1022,7 +963,7 @@ class Engine:
 
     def encode(self, raws, opts=None, cmds=False):
         """Convenience: list of raw byte strings (or DVCL command-list blobs with cmds=True) -> list of .divans bytes."""
-        status, outs, _, _ = self._encode_lists(raws, opts, cmds, False)
+        status, outs = self._encode_lists(raws, opts, cmds)
         if (status != 0).any():
             raise DivansError("encode failed for streams %s" % np.nonzero(status)[0][:8])
         return outs

@@ -73,24 +73,23 @@ struct divans_b200_ctx {
     uint32_t *d_sf = nullptr; size_t sf_cap = 0;               // encoder: symbol logs
     uint8_t *d_replay = nullptr; size_t replay_cap = 0;
     uint32_t *d_enc_scratch = nullptr; size_t enc_scratch_cap = 0;
-    uint8_t *d_pm_internal = nullptr; std::vector<uint8_t> h_pm;
     uint64_t *d_rcp15 = nullptr;
-    // literal model selection (encode_auto_*): the candidates' PredictionMode records, the cost table, per (stream, candidate)
-    // scratch: offsets, lengths, record index, status and cost
-    uint8_t *d_pm_records = nullptr; uint32_t *d_cost_tab = nullptr;
+    // the PredictionMode records a raw stream starts with or a command list's are replaced by (stage_records): the options' or
+    // the LZ77 generator's record, a selection's candidates, and encode_mixmap's mixed records; and their host staging
+    uint8_t *d_records = nullptr; size_t records_cap = 0; std::vector<uint8_t> h_pm;
+    // cost selections (encode_auto_*, encode_mixmap_*, encode_speeds_*): the cost table, per (stream, candidate) scratch:
+    // offsets, lengths, record index, status and cost
+    uint32_t *d_cost_tab = nullptr;
     uint64_t *d_auto = nullptr; size_t auto_cap = 0;
-    // per-context mixing values (encode_mixmap_*): per-stream scratch (per-entry winners, mixed pass, record index), the k uniform
-    // and n mixed records, the binned cost pass's per-slot bins, and the host calls' staging of the mixing / bins outputs
+    // per-context mixing values (encode_mixmap_*): per-stream scratch (per-entry winners, mixed pass, record index) and the
+    // binned cost pass's per-slot bins
     uint64_t *d_mix = nullptr; size_t mix_cap = 0;
-    uint8_t *d_mix_records = nullptr; size_t mix_records_cap = 0;
     uint64_t *d_slot_bins = nullptr; size_t slot_bins_cap = 0;
-    uint64_t *d_mix_out = nullptr; size_t mix_out_cap = 0;
     // literal speeds (encode_speeds_*): the halves and verify passes' costs, statuses and halves, the per-pair and per-stream speeds
     uint64_t *d_speeds = nullptr; size_t speeds_cap = 0;
-    // LZ77 command generator (lz77_cmds_batch_device): per-warp head table + prev array, and the PredictionMode record it copies
+    // LZ77 command generator (lz77_cmds_batch_device): per-warp head table + prev array
     // (lz_scratch_asked: the request the allocation was made for, which free memory may have cut down to lz_scratch_words)
     int32_t *d_lz_scratch = nullptr; size_t lz_scratch_words = 0, lz_scratch_asked = 0;
-    uint8_t *d_lz_pm = nullptr;
     bool main_end_is_evm1 = false;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr, evm = nullptr, evm1 = nullptr;   // ev0 | frame kernel | evm | decode kernel | ev1
     cudaEvent_t ev_busy = nullptr; bool busy_recorded = false;                 // end of the most recent launch set on any stream
@@ -187,10 +186,10 @@ extern "C" void divans_b200_destroy(divans_b200_ctx *ctx) {
     if (ctx->evm) cudaEventDestroy(ctx->evm);
     if (ctx->evm1) cudaEventDestroy(ctx->evm1);
     if (ctx->ev_busy) cudaEventDestroy(ctx->ev_busy);
-    cudaFree(ctx->d_sf); cudaFree(ctx->d_replay); cudaFree(ctx->d_enc_scratch); cudaFree(ctx->d_pm_internal); cudaFree(ctx->d_rcp15);
-    cudaFree(ctx->d_pm_records); cudaFree(ctx->d_cost_tab); cudaFree(ctx->d_auto);
-    cudaFree(ctx->d_mix); cudaFree(ctx->d_mix_records); cudaFree(ctx->d_slot_bins); cudaFree(ctx->d_mix_out); cudaFree(ctx->d_speeds);
-    cudaFree(ctx->d_lz_scratch); cudaFree(ctx->d_lz_pm);
+    cudaFree(ctx->d_sf); cudaFree(ctx->d_replay); cudaFree(ctx->d_enc_scratch); cudaFree(ctx->d_records); cudaFree(ctx->d_rcp15);
+    cudaFree(ctx->d_cost_tab); cudaFree(ctx->d_auto);
+    cudaFree(ctx->d_mix); cudaFree(ctx->d_slot_bins); cudaFree(ctx->d_speeds);
+    cudaFree(ctx->d_lz_scratch);
     for (auto &ln : ctx->lane) {
         free_host_bufs(ln.bufs);
         if (ln.h_res) cudaFreeHost(ln.h_res);
@@ -594,58 +593,102 @@ static uint64_t stage_aligned(std::vector<uint8_t> &staged, const uint8_t *src, 
     return o;
 }
 
-// The EncodeParams fields the model pass and the cost pass share: the n streams at d_in[d_in_off[v] .. +d_in_len[v]), the
-// context's arena, tables and replay windows, the log capacities `caps` (sized for streams of up to max_in_len bytes), the
-// window (10..24, or 0 for each command list's own) and the options.  Every other field is zero.
-static EncodeParams encode_params(const divans_b200_ctx *ctx, size_t n, int raw_mode, const uint8_t *d_in, const uint64_t *d_in_off,
-                                  const uint64_t *d_in_len, uint64_t max_in_len, const LogCaps &caps, const divans_b200_encode_options *o,
-                                  int window) {
+// One encode launch set's streams: n streams at in[in_off[i] .. +in_len[i]) in HBM (raw buffers, or command lists with
+// raw_mode 0), the log capacities `caps` (sized for streams of up to max_in_len bytes), the outputs, the options, the window
+// (10..24, or 0 for each command list's own) and the CUDA stream the launches go to.
+struct EncBatch {
+    size_t n; int raw_mode;
+    const uint8_t *in; const uint64_t *in_off, *in_len; uint64_t max_in_len; LogCaps caps;
+    uint8_t *out; const uint64_t *out_off, *out_cap; uint64_t *out_len; int32_t *status;
+    const divans_b200_encode_options *o; int window; cudaStream_t st;
+};
+
+// The EncodeParams fields the model pass and the cost passes share: the batch's log capacities, window and options, the
+// context's arena, tables and replay windows, and n streams (or pairs of a selection) at in[in_off[v] .. +in_len[v]).  Every
+// other field is zero.
+static EncodeParams encode_params(const divans_b200_ctx *ctx, const EncBatch &b, size_t n, const uint64_t *in_off, const uint64_t *in_len) {
+    const divans_b200_encode_options *o = b.o;
     EncodeParams ep;
     memset(&ep, 0, sizeof ep);
-    ep.in = d_in; ep.in_off = d_in_off; ep.in_len = d_in_len; ep.raw_mode = raw_mode; ep.n_streams = (uint32_t)n;
+    ep.in = b.in; ep.in_off = in_off; ep.in_len = in_len; ep.raw_mode = b.raw_mode; ep.n_streams = (uint32_t)n;
     ep.work_counter = ctx->d_counter; ep.arena = ctx->d_arena; ep.tables = ctx->d_tables;
-    ep.replay = ctx->d_replay; ep.replay_stride = caps.replay;
-    ep.cmd_cap = (uint32_t)caps.cmd; ep.lit_cap = (uint32_t)caps.lit;
-    ep.window_size = window; ep.max_in_len = max_in_len; ep.dynamic_context_mixing = o->dynamic_context_mixing & 0xff; ep.prior_depth = o->prior_depth & 0xff;
+    ep.replay = ctx->d_replay; ep.replay_stride = b.caps.replay;
+    ep.cmd_cap = (uint32_t)b.caps.cmd; ep.lit_cap = (uint32_t)b.caps.lit;
+    ep.window_size = b.window; ep.max_in_len = b.max_in_len; ep.dynamic_context_mixing = o->dynamic_context_mixing & 0xff; ep.prior_depth = o->prior_depth & 0xff;
     ep.use_context_map = o->use_context_map; ep.force_stride = o->force_stride; ep.have_literal_adaptation = o->have_literal_adaptation;
     for (int k = 0; k < 4; k++) ep.literal_adaptation[k] = pack_speed(o->literal_adaptation[k]);
     ep.model_rev = o->model_rev == DIVANS_B200_MODEL_WASM_2018 ? 1 : 0;
     return ep;
 }
+// a cost pass (no logs: cmd_cap / lit_cap are the final encode's capacities, which a pass must fit to be chosen): each of the n
+// streams or pairs sums its cost into tally[v] and ends with status[v]
+static EncodeParams cost_params(const divans_b200_ctx *ctx, const EncBatch &b, size_t n, const uint64_t *in_off, const uint64_t *in_len,
+                                int32_t *status, uint64_t *tally) {
+    EncodeParams ep = encode_params(ctx, b, n, in_off, in_len);
+    ep.cost_tab = ctx->d_cost_tab; ep.status = status; ep.tally = tally;
+    return ep;
+}
 
-// One launch set over n streams whose inputs/outputs already sit in HBM, with the log capacities `caps`.  Like every launch
-// sequence of a context, it waits for the previous call's last kernel (`ev_busy`, on whatever stream) before its first write to
-// the context's scratch.  `d_pm_records`: the caller's records (encode_auto_device_nolock), else raw streams start with the
-// record of the options.
-static DivansResult encode_device_internal(divans_b200_ctx *ctx, size_t n, int raw_mode, const uint8_t *d_in, const uint64_t *d_in_off,
-                                           const uint64_t *d_in_len, uint64_t max_in_len, const LogCaps &caps, uint8_t *d_out,
-                                           const uint64_t *d_out_off, const uint64_t *d_out_cap, uint64_t *d_out_len, int32_t *d_status,
-                                           const divans_b200_encode_options *o, int window, cudaStream_t st,
-                                           const uint8_t *d_pm_records = nullptr, const uint32_t *d_pm_index = nullptr, uint32_t pm_keep = 0,
-                                           const int *d_adapt = nullptr) {
-    const size_t slots = encode_slots(ctx, n);
-    const uint32_t blocks = (uint32_t)(slots / ENCODE_GROUPS_PER_BLOCK);
+// DIVANS_B200_LITERAL_MODEL_KEEP: a command list's own PredictionMode records (command-list calls only)
+static bool is_keep(const divans_b200_literal_model &c) { return c.literal_pred_mode == -1 && c.literal_mixing_value == -1; }
+
+// Records [0, k) of the context's records buffer, which is grown to hold k + extra (at least one): the raw record of each
+// candidate, or with `keep` a zero hole for each KEEP candidate (bit c of *keep), which the model pass never reads.  Like every
+// write of a call to the context's scratch, the upload waits for the previous call's last kernel (`ev_busy`, on any stream).
+static DivansResult stage_records(divans_b200_ctx *ctx, const divans_b200_literal_model *cands, uint32_t k, size_t extra, cudaStream_t st,
+                                  uint32_t *keep = nullptr) {
+    if (!grow(ctx, &ctx->d_records, &ctx->records_cap, std::max<size_t>(k + extra, 1) * PM_RECORD_BYTES)) return DIVANS_FAILURE;
+    std::vector<uint8_t> &pm = ctx->h_pm;
+    pm.assign((size_t)k * PM_RECORD_BYTES, 0);
+    if (keep) *keep = 0;
+    for (uint32_t c = 0; c < k; c++) {
+        if (keep && is_keep(cands[c])) *keep |= 1u << c;
+        else raw_record(pm.data() + (size_t)c * PM_RECORD_BYTES, cands[c].literal_pred_mode, cands[c].literal_mixing_value);
+    }
+    if (ctx->busy_recorded) CK(cudaStreamWaitEvent(st, ctx->ev_busy, 0));
+    if (k) CK(cudaMemcpyAsync(ctx->d_records, pm.data(), pm.size(), cudaMemcpyHostToDevice, st));
+    return DIVANS_SUCCESS;
+}
+
+// One pass of the model walk `w` over the p.n_streams streams or pairs, which it pulls from the context's work counter (reset
+// first), on as many encoder slots as they fill, under the options' CDF model.  `timed`: the encode's own model pass, which
+// last_kernel_ms and last_main_kernel_ms time from here.
+static DivansResult model_pass(divans_b200_ctx *ctx, const EncBatch &b, EncodeWalk w, const EncodeParams &p, const BinParams &bp = BinParams(),
+                               bool timed = false) {
+    const uint32_t blocks = (uint32_t)(encode_slots(ctx, p.n_streams) / ENCODE_GROUPS_PER_BLOCK);
+    CK(cudaMemsetAsync(ctx->d_counter, 0, 4, b.st));
+    if (timed) { CK(cudaEventRecord(ctx->ev0, b.st)); CK(cudaEventRecord(ctx->evm, b.st)); }
+    if (b.o->cdf_model == DIVANS_B200_CDF_BLEND) launch_encode_walk<true>(w, p, bp, blocks, b.st);
+    else launch_encode_walk<false>(w, p, bp, blocks, b.st);
+    ctx->launches += 1;
+    return DIVANS_SUCCESS;
+}
+
+// The launch set that encodes the batch: the model pass, then the flush, pack and mux passes.  Raw streams start with record
+// pm_index[i] (nullptr: record 0) of `records`, by default the options' record; command lists keep their own records unless
+// pm_index replaces them (pm_keep: the candidates that keep them).  `adapt`: each stream's literal speeds (encode_speeds).
+static DivansResult encode_device_internal(divans_b200_ctx *ctx, const EncBatch &b, const uint8_t *records = nullptr,
+                                           const uint32_t *pm_index = nullptr, uint32_t pm_keep = 0, const int *adapt = nullptr) {
+    const size_t n = b.n, slots = encode_slots(ctx, n);
     if (ensure_arena(ctx, slots) != DIVANS_SUCCESS) return DIVANS_FAILURE;
-    const uint32_t cmd_cap = (uint32_t)caps.cmd, lit_cap = (uint32_t)caps.lit;
+    const uint32_t cmd_cap = (uint32_t)b.caps.cmd, lit_cap = (uint32_t)b.caps.lit;
     const uint32_t cmd_chunks = (cmd_cap + NUM_SYMBOLS_BEFORE_FLUSH - 1) / NUM_SYMBOLS_BEFORE_FLUSH;
     const uint32_t lit_chunks = (lit_cap + NUM_SYMBOLS_BEFORE_FLUSH - 1) / NUM_SYMBOLS_BEFORE_FLUSH;
     const uint32_t max_chunks = cmd_chunks + lit_chunks;
     if (!grow(ctx, &ctx->d_sf, &ctx->sf_cap, n * ((size_t)cmd_cap + lit_cap))) return DIVANS_FAILURE;
-    if (!grow(ctx, &ctx->d_replay, &ctx->replay_cap, slots * (size_t)caps.replay)) return DIVANS_FAILURE;
+    if (!grow(ctx, &ctx->d_replay, &ctx->replay_cap, slots * (size_t)b.caps.replay)) return DIVANS_FAILURE;
     // small per-stream scratch: counts [2n] | window [n] | dummy [slots] | chunk_w [n*max_chunks] | chunk_state [16*n*max_chunks]
     size_t words = 3 * n + slots + n * (size_t)max_chunks + 4 * n * (size_t)max_chunks + 16 + 2 * n * (size_t)max_chunks * (NUM_SYMBOLS_BEFORE_FLUSH / 64);
     if (!grow(ctx, &ctx->d_enc_scratch, &ctx->enc_scratch_cap, words)) return DIVANS_FAILURE;
-    if (!ctx->d_pm_internal) CK(cudaMalloc((void **)&ctx->d_pm_internal, PM_RECORD_BYTES));
-    if (ctx->busy_recorded) CK(cudaStreamWaitEvent(st, ctx->ev_busy, 0));
-    if (!ctx->d_rcp15) { CK(cudaMalloc((void **)&ctx->d_rcp15, 32768 * sizeof(uint64_t))); launch_rcp15_init(ctx->d_rcp15, st); ctx->launches += 1; }
-    if (raw_mode && !d_pm_records) {
-        std::vector<uint8_t> &pm = ctx->h_pm;
-        pm.assign(PM_RECORD_BYTES, 0);
-        raw_record(pm.data(), o->literal_pred_mode, o->literal_mixing_value);
-        CK(cudaMemcpyAsync(ctx->d_pm_internal, pm.data(), PM_RECORD_BYTES, cudaMemcpyHostToDevice, st));
+    if (ctx->busy_recorded) CK(cudaStreamWaitEvent(b.st, ctx->ev_busy, 0));
+    if (!ctx->d_rcp15) { CK(cudaMalloc((void **)&ctx->d_rcp15, 32768 * sizeof(uint64_t))); launch_rcp15_init(ctx->d_rcp15, b.st); ctx->launches += 1; }
+    if (!records) {   // the options' record (command lists: none)
+        const divans_b200_literal_model opt = {b.o->literal_pred_mode, b.o->literal_mixing_value};
+        if (stage_records(ctx, &opt, b.raw_mode ? 1 : 0, 0, b.st) != DIVANS_SUCCESS) return DIVANS_FAILURE;
+        records = ctx->d_records;
     }
-    EncodeParams ep = encode_params(ctx, n, raw_mode, d_in, d_in_off, d_in_len, max_in_len, caps, o, window);
-    ep.pm_internal = d_pm_records ? d_pm_records : ctx->d_pm_internal; ep.pm_index = d_pm_index; ep.pm_keep = pm_keep;
+    EncodeParams ep = encode_params(ctx, b, n, b.in_off, b.in_len);
+    ep.pm_internal = records; ep.pm_index = pm_index; ep.pm_keep = pm_keep;
     ep.sf = ctx->d_sf;
     uint32_t *w = ctx->d_enc_scratch;
     ep.sf_counts = w; w += 2 * n;
@@ -657,36 +700,18 @@ static DivansResult encode_device_internal(divans_b200_ctx *ctx, size_t n, int r
     ep.emit_bits = w + 4 * n * (size_t)max_chunks;
     ep.rcp15 = ctx->d_rcp15;
     ep.max_chunks = max_chunks; ep.cmd_chunks = cmd_chunks;
-    ep.out = d_out; ep.out_off = d_out_off; ep.out_cap = d_out_cap; ep.out_len = d_out_len; ep.status = d_status;
-    ep.v_adapt = d_adapt;
-    CK(cudaMemsetAsync(ctx->d_counter, 0, 4, st));
-    CK(cudaEventRecord(ctx->ev0, st));
-    CK(cudaEventRecord(ctx->evm, st));
-    const bool blend = o->cdf_model == DIVANS_B200_CDF_BLEND;
-    if (d_adapt) { if (blend) launch_encode_speeds_blend(ep, false, blocks, st); else launch_encode_speeds(ep, false, blocks, st); }
-    else if (blend) launch_encode_model_blend(ep, blocks, st);
-    else launch_encode_model(ep, blocks, st);
-    CK(cudaEventRecord(ctx->evm1, st));
-    launch_encode_flush_mux(ep, st);
-    CK(cudaEventRecord(ctx->ev1, st));
-    CK(cudaEventRecord(ctx->ev_busy, st)); ctx->busy_recorded = true;
+    ep.out = b.out; ep.out_off = b.out_off; ep.out_cap = b.out_cap; ep.out_len = b.out_len; ep.status = b.status;
+    ep.v_adapt = adapt;
+    if (model_pass(ctx, b, adapt ? EncodeWalk::SPEEDS_MODEL : EncodeWalk::MODEL, ep, BinParams(), true) != DIVANS_SUCCESS) return DIVANS_FAILURE;
+    CK(cudaEventRecord(ctx->evm1, b.st));
+    launch_encode_flush_mux(ep, b.st);
+    CK(cudaEventRecord(ctx->ev1, b.st));
+    CK(cudaEventRecord(ctx->ev_busy, b.st)); ctx->busy_recorded = true;
     ctx->main_end_is_evm1 = true;
-    ctx->launches += 4;
+    ctx->launches += 3;
     CK(cudaGetLastError());
     return DIVANS_SUCCESS;
 }
-
-// literal model selection of a batch (encode_host_common, encode_device_common): the candidates, and where chosen / cost go.
-// mixmap (divans_b200_encode_mixmap_*): the candidates are (opts->literal_pred_mode, v[c]); chosen may be NULL, cost has k + 1
-// columns, and mixing / bins are the optional per-context outputs.
-struct AutoSel {
-    const divans_b200_literal_model *cands; uint32_t n_cands;
-    uint32_t *chosen; uint64_t *cost;
-    bool mixmap = false; uint8_t *mixing = nullptr; uint64_t *bins = nullptr;
-    // speeds (divans_b200_encode_speeds_*): the k = n_cands candidate speeds (cands unused); chosen has 3 columns, cost k + 1,
-    // halves [n * k * 2] is optional
-    const SpeedValues *speeds = nullptr; uint64_t *halves = nullptr;
-};
 
 // ---- literal model selection ----
 // Cost of coding a nibble of frequency f (1..32767 of 32768) in 1/65536 bit: 65536 * (15 - log2 f), the 16 fraction bits of
@@ -706,8 +731,6 @@ static uint32_t freq_cost(uint32_t f) {
     return (15u << 16) - ((e << 16) | frac);
 }
 
-// DIVANS_B200_LITERAL_MODEL_KEEP: a command list's own PredictionMode records (command-list calls only)
-static bool is_keep(const divans_b200_literal_model &c) { return c.literal_pred_mode == -1 && c.literal_mixing_value == -1; }
 
 // `cmds`: the candidates of a command-list call, which may also be KEEP
 static bool check_cands(divans_b200_ctx *ctx, const divans_b200_literal_model *cands, uint32_t n_cands, bool cmds) {
@@ -739,192 +762,164 @@ static bool ensure_cost_tab(divans_b200_ctx *ctx, cudaStream_t st) {
     return ck(ctx, cudaMemcpyAsync(ctx->d_cost_tab, tab, sizeof tab, cudaMemcpyHostToDevice, st), "cudaMemcpyAsync(cost table)");
 }
 
-// One launch sequence over n streams in HBM (raw buffers, or command lists with raw_mode 0): fan out to n * C virtual streams
-// (dv_encode.cu: candidate-major), the cost-only model pass over all of them, the per-stream argmin into d_chosen, then the
-// encoder pipeline with stream i coded under candidate d_chosen[i] (raw: its starting record; command lists: the record that
-// replaces each of the list's own, unless the candidate is KEEP).  The cost pass pulls virtual streams from the work counter
-// like the model pass, so however many there are, the context's encoder slots code them as many at a time as they hold.
-// caps / window: those of the plain call over the same n streams.
-static DivansResult encode_auto_device_nolock(divans_b200_ctx *ctx, size_t n, int raw_mode, const uint8_t *d_in, const uint64_t *d_in_off,
-                                              const uint64_t *d_in_len, uint64_t max_in_len, const LogCaps &caps, uint8_t *d_out,
-                                              const uint64_t *d_out_off, const uint64_t *d_out_cap, uint64_t *d_out_len, int32_t *d_status,
-                                              const divans_b200_encode_options *o, int window, const divans_b200_literal_model *cands,
-                                              uint32_t n_cands, uint32_t *d_chosen, uint64_t *d_cost, cudaStream_t st) {
-    const uint64_t nv = (uint64_t)n * n_cands;
-    const size_t vslots = encode_slots(ctx, nv);
-    if (ensure_arena(ctx, vslots) != DIVANS_SUCCESS) return DIVANS_FAILURE;
-    if (!grow(ctx, &ctx->d_replay, &ctx->replay_cap, vslots * (size_t)caps.replay)) return DIVANS_FAILURE;
-    // v_off [nv] | v_len [nv] | tally [nv] | v_pm u32 [nv] | v_status i32 [nv]
-    if (!grow(ctx, &ctx->d_auto, &ctx->auto_cap, 4 * nv + 2)) return DIVANS_FAILURE;
-    uint64_t *v_off = ctx->d_auto, *v_len = v_off + nv, *tally = v_len + nv;
-    uint32_t *v_pm = reinterpret_cast<uint32_t *>(tally + nv);
-    int32_t *v_status = reinterpret_cast<int32_t *>(v_pm + nv);
-    if (!ctx->d_pm_records) CK(cudaMalloc((void **)&ctx->d_pm_records, 16 * (size_t)PM_RECORD_BYTES));
-    if (ctx->busy_recorded) CK(cudaStreamWaitEvent(st, ctx->ev_busy, 0));
-    if (!ensure_cost_tab(ctx, st)) return DIVANS_FAILURE;
-    std::vector<uint8_t> &pm = ctx->h_pm;
-    pm.assign((size_t)n_cands * PM_RECORD_BYTES, 0);
-    uint32_t keep = 0;   // bit c: candidate c is KEEP (its record stays zero and is never read)
-    for (uint32_t c = 0; c < n_cands; c++) {
-        if (is_keep(cands[c])) keep |= 1u << c;
-        else raw_record(pm.data() + (size_t)c * PM_RECORD_BYTES, cands[c].literal_pred_mode, cands[c].literal_mixing_value);
-    }
-    CK(cudaMemcpyAsync(ctx->d_pm_records, pm.data(), pm.size(), cudaMemcpyHostToDevice, st));
-    launch_auto_fanout(d_in_off, d_in_len, n, n_cands, v_off, v_len, v_pm, st);
-
-    // no logs: cmd_cap / lit_cap are the final encode's capacities, which a pair must fit to be chosen
-    EncodeParams tp = encode_params(ctx, nv, raw_mode, d_in, v_off, v_len, max_in_len, caps, o, window);
-    tp.pm_internal = ctx->d_pm_records; tp.pm_index = v_pm; tp.pm_keep = keep;
-    tp.status = v_status; tp.cost_tab = ctx->d_cost_tab; tp.tally = tally;
-    CK(cudaMemsetAsync(ctx->d_counter, 0, 4, st));
-    const uint32_t blocks = (uint32_t)(vslots / ENCODE_GROUPS_PER_BLOCK);
-    if (o->cdf_model == DIVANS_B200_CDF_BLEND) launch_encode_tally_blend(tp, blocks, st); else launch_encode_tally(tp, blocks, st);
-    launch_auto_select(tally, v_status, n, n_cands, d_chosen, d_cost, st);
-    ctx->launches += 3;
-    CK(cudaGetLastError());
-    return encode_device_internal(ctx, n, raw_mode, d_in, d_in_off, d_in_len, max_in_len, caps, d_out, d_out_off, d_out_cap, d_out_len,
-                                  d_status, o, window, st, ctx->d_pm_records, d_chosen, keep);
+// ---- cost selections ----
+// What a call chooses per stream by coding cost among k candidates, the caller's candidates and where the choice goes (host
+// or device arrays, as the call).  SEL_NONE: the plain encode.
+//  * SEL_AUTO (divans_b200_encode_[cmds_]auto_*): literal models; chosen [n] (required), cost [n * k].
+//  * SEL_MIXMAP (divans_b200_encode_[cmds_]mixmap_*): mixing values under opts->literal_pred_mode, chosen per context;
+//    chosen [n], cost [n * (k + 1)], mixing [n * 8192], bins [n * k * 8192].
+//  * SEL_SPEEDS (divans_b200_encode_[cmds_]speeds_*): literal speeds; chosen [n * 3], cost [n * (k + 1)], halves [n * k * 2].
+// Outputs other than auto's chosen may be NULL.
+enum SelKind { SEL_NONE, SEL_AUTO, SEL_MIXMAP, SEL_SPEEDS };
+struct Selection {
+    SelKind kind = SEL_NONE;
+    uint32_t k = 0;
+    const divans_b200_literal_model *models = nullptr; const int32_t *mix_values = nullptr; const int16_t *speed_values = nullptr;
+    uint32_t *chosen = nullptr; uint64_t *cost = nullptr; uint8_t *mixing = nullptr; uint64_t *bins = nullptr; uint64_t *halves = nullptr;
+    // the candidates once check_selection has accepted them: the literal models (auto, mixmap) or the speeds
+    divans_b200_literal_model cands[16]; SpeedValues speeds;
+};
+static Selection sel_auto(const divans_b200_literal_model *cands, uint32_t k, uint32_t *chosen, uint64_t *cost) {
+    Selection s; s.kind = SEL_AUTO; s.k = k; s.models = cands; s.chosen = chosen; s.cost = cost;
+    return s;
+}
+static Selection sel_mixmap(const int32_t *values, uint32_t k, uint32_t *chosen, uint8_t *mixing, uint64_t *cost, uint64_t *bins) {
+    Selection s; s.kind = SEL_MIXMAP; s.k = k; s.mix_values = values; s.chosen = chosen; s.mixing = mixing; s.cost = cost; s.bins = bins;
+    return s;
+}
+static Selection sel_speeds(const int16_t *values, uint32_t k, uint32_t *chosen, uint64_t *cost, uint64_t *halves) {
+    Selection s; s.kind = SEL_SPEEDS; s.k = k; s.speed_values = values; s.chosen = chosen; s.cost = cost; s.halves = halves;
+    return s;
 }
 
-// Per-context mixing values: one launch sequence over n streams in HBM.  Records [0, k) are R(p, v[c]), records [k, k + n) the
-// streams' mixed records M_i.
-//  1. the binned cost pass over the n * k pairs (fan-out as encode_auto): totals u[i][c], per-entry winners best[i][e]
+// The n * k pairs of a selection, candidate-major: pair v = c * n + i codes stream i under candidate c, at in[v_off[v] ..
+// +v_len[v]) (dv_encode.cu), with record v_pm[v] = c; a cost pass sums its cost into tally[v] and ends with v_status[v].
+struct Pairs {
+    uint64_t nv;
+    uint64_t *v_off, *v_len, *tally; uint32_t *v_pm; int32_t *v_status;
+};
+// Slots and replay windows for the pairs, their scratch, and after the previous call's last kernel the cost table and the
+// fan-out.  The cost passes pull pairs from the work counter like the model pass, so however many there are, the context's
+// encoder slots code them as many at a time as they hold.
+static DivansResult fan_out(divans_b200_ctx *ctx, const EncBatch &b, uint32_t k, Pairs &p) {
+    p.nv = (uint64_t)b.n * k;
+    const size_t slots = encode_slots(ctx, p.nv);
+    if (ensure_arena(ctx, slots) != DIVANS_SUCCESS) return DIVANS_FAILURE;
+    if (!grow(ctx, &ctx->d_replay, &ctx->replay_cap, slots * (size_t)b.caps.replay)) return DIVANS_FAILURE;
+    // v_off [nv] | v_len [nv] | tally [nv] | v_pm u32 [nv] | v_status i32 [nv]
+    if (!grow(ctx, &ctx->d_auto, &ctx->auto_cap, 4 * p.nv + 2)) return DIVANS_FAILURE;
+    p.v_off = ctx->d_auto; p.v_len = p.v_off + p.nv; p.tally = p.v_len + p.nv;
+    p.v_pm = reinterpret_cast<uint32_t *>(p.tally + p.nv);
+    p.v_status = reinterpret_cast<int32_t *>(p.v_pm + p.nv);
+    if (ctx->busy_recorded) CK(cudaStreamWaitEvent(b.st, ctx->ev_busy, 0));
+    if (!ensure_cost_tab(ctx, b.st)) return DIVANS_FAILURE;
+    launch_auto_fanout(b.in_off, b.in_len, b.n, k, p.v_off, p.v_len, p.v_pm, b.st);
+    ctx->launches += 1;
+    return DIVANS_SUCCESS;
+}
+
+// Literal models: the cost pass over the pairs, the per-stream argmin into chosen, then the encode with stream i coded under
+// candidate chosen[i] (raw: its starting record; command lists: the record that replaces each of the list's own, unless the
+// candidate is KEEP).
+static DivansResult encode_auto_device_nolock(divans_b200_ctx *ctx, const EncBatch &b, const Selection &sel) {
+    Pairs p;
+    uint32_t keep;
+    if (fan_out(ctx, b, sel.k, p) != DIVANS_SUCCESS || stage_records(ctx, sel.cands, sel.k, 0, b.st, &keep) != DIVANS_SUCCESS)
+        return DIVANS_FAILURE;
+    EncodeParams tp = cost_params(ctx, b, p.nv, p.v_off, p.v_len, p.v_status, p.tally);
+    tp.pm_internal = ctx->d_records; tp.pm_index = p.v_pm; tp.pm_keep = keep;
+    if (model_pass(ctx, b, EncodeWalk::TALLY, tp) != DIVANS_SUCCESS) return DIVANS_FAILURE;
+    launch_auto_select(p.tally, p.v_status, b.n, sel.k, sel.chosen, sel.cost, b.st);
+    ctx->launches += 1;
+    CK(cudaGetLastError());
+    return encode_device_internal(ctx, b, ctx->d_records, sel.chosen, keep);
+}
+
+// Per-context mixing values.  Records [0, k) are R(p, v[c]), records [k, k + n) the streams' mixed records M_i.
+//  1. the binned cost pass over the pairs: totals u[i][c], per-entry winners best[i][e]
 //  2. mixmap_map_kernel builds M_i;  3. the cost pass of every stream under M_i: x[i]
-//  4. mixmap_select_kernel: record c* or k + i per stream;  5. the plain pipeline from that record.
+//  4. mixmap_select_kernel: record c* or k + i per stream;  5. the encode from that record.
 // Command lists: every record of a list is replaced (pm_keep 0).  The record index of a mixed stream, k + i, can exceed 31; the
 // model pass tests it against pm_keep with a 32-bit shift (shr.u32 yields 0 for counts of 32 or more), so it still reads as "replace".
-static DivansResult encode_mixmap_device_nolock(divans_b200_ctx *ctx, size_t n, int raw_mode, const uint8_t *d_in, const uint64_t *d_in_off,
-                                                const uint64_t *d_in_len, uint64_t max_in_len, const LogCaps &caps, uint8_t *d_out,
-                                                const uint64_t *d_out_off, const uint64_t *d_out_cap, uint64_t *d_out_len, int32_t *d_status,
-                                                const divans_b200_encode_options *o, int window, const divans_b200_literal_model *cands,
-                                                uint32_t k, uint32_t *d_chosen, uint64_t *d_cost, uint8_t *d_mixing, uint64_t *d_bins,
-                                                cudaStream_t st) {
-    const uint64_t nv = (uint64_t)n * k;
-    const size_t vslots = encode_slots(ctx, nv);
-    if (ensure_arena(ctx, vslots) != DIVANS_SUCCESS) return DIVANS_FAILURE;
-    if (!grow(ctx, &ctx->d_replay, &ctx->replay_cap, vslots * (size_t)caps.replay)) return DIVANS_FAILURE;
-    // v_off [nv] | v_len [nv] | tally [nv] | v_pm u32 [nv] | v_status i32 [nv]
-    if (!grow(ctx, &ctx->d_auto, &ctx->auto_cap, 4 * nv + 2)) return DIVANS_FAILURE;
-    uint64_t *v_off = ctx->d_auto, *v_len = v_off + nv, *tally = v_len + nv;
-    uint32_t *v_pm = reinterpret_cast<uint32_t *>(tally + nv);
-    int32_t *v_status = reinterpret_cast<int32_t *>(v_pm + nv);
+static DivansResult encode_mixmap_device_nolock(divans_b200_ctx *ctx, const EncBatch &b, const Selection &sel) {
+    const size_t n = b.n;
+    const uint32_t k = sel.k;
     // best [n * 8192] | x_tally [n] | x_status i32 [n] | mix_idx u32 [n] | rec_idx u32 [n]
-    if (!grow(ctx, &ctx->d_mix, &ctx->mix_cap, (size_t)n * MIX_ENTRIES + 3 * n)) return DIVANS_FAILURE;
-    uint64_t *best = ctx->d_mix, *x_tally = best + (size_t)n * MIX_ENTRIES;
+    if (!grow(ctx, &ctx->d_mix, &ctx->mix_cap, n * MIX_ENTRIES + 3 * n)) return DIVANS_FAILURE;
+    uint64_t *best = ctx->d_mix, *x_tally = best + n * MIX_ENTRIES;
     int32_t *x_status = reinterpret_cast<int32_t *>(x_tally + n);
     uint32_t *mix_idx = reinterpret_cast<uint32_t *>(x_status + n), *rec_idx = mix_idx + n;
-    if (!grow(ctx, &ctx->d_mix_records, &ctx->mix_records_cap, (k + n) * (size_t)PM_RECORD_BYTES)) return DIVANS_FAILURE;
-    if (!grow(ctx, &ctx->d_slot_bins, &ctx->slot_bins_cap, vslots * (size_t)MIX_ENTRIES)) return DIVANS_FAILURE;
-    if (ctx->busy_recorded) CK(cudaStreamWaitEvent(st, ctx->ev_busy, 0));
-    if (!ensure_cost_tab(ctx, st)) return DIVANS_FAILURE;
-    std::vector<uint8_t> &pm = ctx->h_pm;
-    pm.assign((size_t)k * PM_RECORD_BYTES, 0);
+    if (!grow(ctx, &ctx->d_slot_bins, &ctx->slot_bins_cap, encode_slots(ctx, (uint64_t)n * k) * (size_t)MIX_ENTRIES)) return DIVANS_FAILURE;
+    Pairs p;
+    if (fan_out(ctx, b, k, p) != DIVANS_SUCCESS || stage_records(ctx, sel.cands, k, n, b.st) != DIVANS_SUCCESS) return DIVANS_FAILURE;
+    CK(cudaMemsetAsync(best, 0xff, n * MIX_ENTRIES * 8, b.st));
     MixValues vals; memset(&vals, 0, sizeof vals); vals.k = k;
-    for (uint32_t c = 0; c < k; c++) {
-        raw_record(pm.data() + (size_t)c * PM_RECORD_BYTES, cands[c].literal_pred_mode, cands[c].literal_mixing_value);
-        vals.v[c] = (uint8_t)cands[c].literal_mixing_value;
-    }
-    CK(cudaMemcpyAsync(ctx->d_mix_records, pm.data(), pm.size(), cudaMemcpyHostToDevice, st));
-    CK(cudaMemsetAsync(best, 0xff, (size_t)n * MIX_ENTRIES * 8, st));
-    launch_auto_fanout(d_in_off, d_in_len, n, k, v_off, v_len, v_pm, st);
-
+    for (uint32_t c = 0; c < k; c++) vals.v[c] = (uint8_t)sel.cands[c].literal_mixing_value;
     // 1. uniform passes, binned
-    EncodeParams tp = encode_params(ctx, nv, raw_mode, d_in, v_off, v_len, max_in_len, caps, o, window);
-    tp.pm_internal = ctx->d_mix_records; tp.pm_index = v_pm; tp.pm_keep = 0;
-    tp.status = v_status; tp.cost_tab = ctx->d_cost_tab; tp.tally = tally;
+    EncodeParams tp = cost_params(ctx, b, p.nv, p.v_off, p.v_len, p.v_status, p.tally);
+    tp.pm_internal = ctx->d_records; tp.pm_index = p.v_pm;
     BinParams bp;
-    bp.slot_bins = ctx->d_slot_bins; bp.best = best; bp.bins_out = d_bins; bp.n = (uint32_t)n; bp.k = k;
-    CK(cudaMemsetAsync(ctx->d_counter, 0, 4, st));
-    if (o->cdf_model == DIVANS_B200_CDF_BLEND) launch_encode_bins_blend(tp, bp, (uint32_t)(vslots / ENCODE_GROUPS_PER_BLOCK), st);
-    else launch_encode_bins(tp, bp, (uint32_t)(vslots / ENCODE_GROUPS_PER_BLOCK), st);
+    bp.slot_bins = ctx->d_slot_bins; bp.best = best; bp.bins_out = sel.bins; bp.n = (uint32_t)n; bp.k = k;
+    if (model_pass(ctx, b, EncodeWalk::BINS, tp, bp) != DIVANS_SUCCESS) return DIVANS_FAILURE;
     // 2. mixed records;  3. the mixed pass, the plain cost pass (a mixed record is not uniform, so its literals take the per-nibble loop)
-    launch_mixmap_map(best, n, vals, ctx->d_mix_records, mix_idx, st);
-    EncodeParams xp = encode_params(ctx, n, raw_mode, d_in, d_in_off, d_in_len, max_in_len, caps, o, window);
-    xp.pm_internal = ctx->d_mix_records; xp.pm_index = mix_idx; xp.pm_keep = 0;
-    xp.status = x_status; xp.cost_tab = ctx->d_cost_tab; xp.tally = x_tally;
-    CK(cudaMemsetAsync(ctx->d_counter, 0, 4, st));
-    const uint32_t xblocks = (uint32_t)(encode_slots(ctx, n) / ENCODE_GROUPS_PER_BLOCK);
-    if (o->cdf_model == DIVANS_B200_CDF_BLEND) launch_encode_tally_blend(xp, xblocks, st); else launch_encode_tally(xp, xblocks, st);
+    launch_mixmap_map(best, n, vals, ctx->d_records, mix_idx, b.st);
+    EncodeParams xp = cost_params(ctx, b, n, b.in_off, b.in_len, x_status, x_tally);
+    xp.pm_internal = ctx->d_records; xp.pm_index = mix_idx;
+    if (model_pass(ctx, b, EncodeWalk::TALLY, xp) != DIVANS_SUCCESS) return DIVANS_FAILURE;
     // 4. choice
-    launch_mixmap_select(tally, v_status, x_tally, x_status, n, vals, ctx->d_mix_records, rec_idx, d_chosen, d_cost, d_mixing, st);
-    ctx->launches += 5;
+    launch_mixmap_select(p.tally, p.v_status, x_tally, x_status, n, vals, ctx->d_records, rec_idx, sel.chosen, sel.cost, sel.mixing, b.st);
+    ctx->launches += 2;   // map, select
     CK(cudaGetLastError());
-    return encode_device_internal(ctx, n, raw_mode, d_in, d_in_off, d_in_len, max_in_len, caps, d_out, d_out_off, d_out_cap, d_out_len,
-                                  d_status, o, window, st, ctx->d_mix_records, rec_idx, 0);
+    return encode_device_internal(ctx, b, ctx->d_records, rec_idx, 0);
 }
 
-// Literal speeds: one launch sequence over n streams in HBM, k candidate speeds, pairs candidate-major (v = c * n + i), every
-// pass on encode_speeds_kernel (the stream's speeds from v_adapt):
-//  1. uniform passes over the n * k pairs under (v[c], v[c], v[c], v[c]): u[i][c]
+// Literal speeds, every pass on encode_speeds_kernel (the stream's speeds from v_adapt):
+//  1. uniform passes over the pairs under (v[c], v[c], v[c], v[c]): u[i][c]
 //  2. with dynamic context mixing >= 2 and k > 1: halves passes under (v[c*], v[c*], v[d], v[d]), whose literal low / high
 //     nibble costs give l*, h*; then the verify pass of each stream under (v[c*], v[c*], v[l*], v[h*]): x[i]
-//  3. speeds_select_kernel: the chosen speeds per stream;  4. the plain pipeline under them.
+//  3. speeds_select_kernel: the chosen speeds per stream;  4. the encode under them.
 // Raw streams start with the options' record; command lists keep their records.
-static DivansResult encode_speeds_device_nolock(divans_b200_ctx *ctx, size_t n, int raw_mode, const uint8_t *d_in, const uint64_t *d_in_off,
-                                                const uint64_t *d_in_len, uint64_t max_in_len, const LogCaps &caps, uint8_t *d_out,
-                                                const uint64_t *d_out_off, const uint64_t *d_out_cap, uint64_t *d_out_len, int32_t *d_status,
-                                                const divans_b200_encode_options *o, int window, const SpeedValues &vals,
-                                                uint32_t *d_chosen, uint64_t *d_cost, uint64_t *d_halves, cudaStream_t st) {
-    const uint32_t k = vals.k;
+static DivansResult encode_speeds_device_nolock(divans_b200_ctx *ctx, const EncBatch &b, const Selection &sel) {
+    const size_t n = b.n;
+    const uint32_t k = sel.k;
     const uint64_t nv = (uint64_t)n * k;
-    const size_t vslots = encode_slots(ctx, nv);
-    if (ensure_arena(ctx, vslots) != DIVANS_SUCCESS) return DIVANS_FAILURE;
-    if (!grow(ctx, &ctx->d_replay, &ctx->replay_cap, vslots * (size_t)caps.replay)) return DIVANS_FAILURE;
-    // v_off [nv] | v_len [nv] | tally [nv] | v_pm u32 [nv] | v_status i32 [nv]
-    if (!grow(ctx, &ctx->d_auto, &ctx->auto_cap, 4 * nv + 2)) return DIVANS_FAILURE;
-    uint64_t *v_off = ctx->d_auto, *v_len = v_off + nv, *tally = v_len + nv;
-    uint32_t *v_pm = reinterpret_cast<uint32_t *>(tally + nv);
-    int32_t *v_status = reinterpret_cast<int32_t *>(v_pm + nv);
+    const SpeedValues &vals = sel.speeds;
     // h_tally [nv] | h_halves [2nv] | x_tally [n] | x_halves [2n] | h_status i32 [nv] | x_status i32 [n] | sel u32 [3n] |
     // v_adapt i32 [4nv] | x_adapt i32 [4n]
     if (!grow(ctx, &ctx->d_speeds, &ctx->speeds_cap, 6 * nv + 7 * n + 4)) return DIVANS_FAILURE;
     uint64_t *h_tally = ctx->d_speeds, *h_halves = h_tally + nv, *x_tally = h_halves + 2 * nv, *x_halves = x_tally + n;
     int32_t *h_status = reinterpret_cast<int32_t *>(x_halves + 2 * n), *x_status = h_status + nv;
-    uint32_t *sel = reinterpret_cast<uint32_t *>(x_status + n);
-    int *v_adapt = reinterpret_cast<int *>(sel + 3 * n), *x_adapt = v_adapt + 4 * nv;
-    if (!ctx->d_pm_internal) CK(cudaMalloc((void **)&ctx->d_pm_internal, PM_RECORD_BYTES));
-    if (ctx->busy_recorded) CK(cudaStreamWaitEvent(st, ctx->ev_busy, 0));
-    if (!ensure_cost_tab(ctx, st)) return DIVANS_FAILURE;
-    if (raw_mode) {
-        std::vector<uint8_t> &pm = ctx->h_pm;
-        pm.assign(PM_RECORD_BYTES, 0);
-        raw_record(pm.data(), o->literal_pred_mode, o->literal_mixing_value);
-        CK(cudaMemcpyAsync(ctx->d_pm_internal, pm.data(), PM_RECORD_BYTES, cudaMemcpyHostToDevice, st));
-    }
-    const bool blend = o->cdf_model == DIVANS_B200_CDF_BLEND;
-    launch_auto_fanout(d_in_off, d_in_len, n, k, v_off, v_len, v_pm, st);
-    launch_speeds_stage(0, n, vals, tally, v_status, h_halves, sel, v_adapt, x_adapt, st);
+    uint32_t *pick = reinterpret_cast<uint32_t *>(x_status + n);
+    int *v_adapt = reinterpret_cast<int *>(pick + 3 * n), *x_adapt = v_adapt + 4 * nv;
+    Pairs p;
+    const divans_b200_literal_model opt = {b.o->literal_pred_mode, b.o->literal_mixing_value};
+    if (fan_out(ctx, b, k, p) != DIVANS_SUCCESS || stage_records(ctx, &opt, b.raw_mode ? 1 : 0, 0, b.st) != DIVANS_SUCCESS)
+        return DIVANS_FAILURE;
+    launch_speeds_stage(0, n, vals, p.tally, p.v_status, h_halves, pick, v_adapt, x_adapt, b.st);
+    ctx->launches += 1;
     // 1. uniform passes
-    EncodeParams tp = encode_params(ctx, nv, raw_mode, d_in, v_off, v_len, max_in_len, caps, o, window);
-    tp.pm_internal = ctx->d_pm_internal; tp.cost_tab = ctx->d_cost_tab;
-    tp.status = v_status; tp.tally = tally; tp.v_adapt = v_adapt; tp.halves = h_halves;
-    const uint32_t vblocks = (uint32_t)(vslots / ENCODE_GROUPS_PER_BLOCK);
-    CK(cudaMemsetAsync(ctx->d_counter, 0, 4, st));
-    if (blend) launch_encode_speeds_blend(tp, true, vblocks, st); else launch_encode_speeds(tp, true, vblocks, st);
-    ctx->launches += 3;
+    EncodeParams tp = cost_params(ctx, b, nv, p.v_off, p.v_len, p.v_status, p.tally);
+    tp.pm_internal = ctx->d_records; tp.v_adapt = v_adapt; tp.halves = h_halves;
+    if (model_pass(ctx, b, EncodeWalk::SPEEDS, tp) != DIVANS_SUCCESS) return DIVANS_FAILURE;
     // 2. halves passes and the verify pass
-    const bool tuned = o->dynamic_context_mixing >= 2 && k > 1;
+    const bool tuned = b.o->dynamic_context_mixing >= 2 && k > 1;
     if (tuned) {
-        launch_speeds_stage(1, n, vals, tally, v_status, h_halves, sel, v_adapt, x_adapt, st);
+        launch_speeds_stage(1, n, vals, p.tally, p.v_status, h_halves, pick, v_adapt, x_adapt, b.st);
         EncodeParams hp = tp;
         hp.status = h_status; hp.tally = h_tally;
-        CK(cudaMemsetAsync(ctx->d_counter, 0, 4, st));
-        if (blend) launch_encode_speeds_blend(hp, true, vblocks, st); else launch_encode_speeds(hp, true, vblocks, st);
-        launch_speeds_stage(2, n, vals, tally, h_status, h_halves, sel, v_adapt, x_adapt, st);
-        EncodeParams xp = encode_params(ctx, n, raw_mode, d_in, d_in_off, d_in_len, max_in_len, caps, o, window);
-        xp.pm_internal = ctx->d_pm_internal; xp.cost_tab = ctx->d_cost_tab;
-        xp.status = x_status; xp.tally = x_tally; xp.v_adapt = x_adapt; xp.halves = x_halves;
-        const uint32_t xblocks = (uint32_t)(encode_slots(ctx, n) / ENCODE_GROUPS_PER_BLOCK);
-        CK(cudaMemsetAsync(ctx->d_counter, 0, 4, st));
-        if (blend) launch_encode_speeds_blend(xp, true, xblocks, st); else launch_encode_speeds(xp, true, xblocks, st);
-        ctx->launches += 4;
+        if (model_pass(ctx, b, EncodeWalk::SPEEDS, hp) != DIVANS_SUCCESS) return DIVANS_FAILURE;
+        launch_speeds_stage(2, n, vals, p.tally, h_status, h_halves, pick, v_adapt, x_adapt, b.st);
+        EncodeParams xp = cost_params(ctx, b, n, b.in_off, b.in_len, x_status, x_tally);
+        xp.pm_internal = ctx->d_records; xp.v_adapt = x_adapt; xp.halves = x_halves;
+        if (model_pass(ctx, b, EncodeWalk::SPEEDS, xp) != DIVANS_SUCCESS) return DIVANS_FAILURE;
+        ctx->launches += 2;   // stages 1 and 2
     }
     // 3. choice
-    launch_speeds_select(n, vals, tuned, tally, v_status, h_halves, h_status, x_tally, x_status, sel, x_adapt, d_chosen, d_cost, d_halves, st);
+    launch_speeds_select(n, vals, tuned, p.tally, p.v_status, h_halves, h_status, x_tally, x_status, pick, x_adapt, sel.chosen, sel.cost,
+                         sel.halves, b.st);
     ctx->launches += 1;
     CK(cudaGetLastError());
-    return encode_device_internal(ctx, n, raw_mode, d_in, d_in_off, d_in_len, max_in_len, caps, d_out, d_out_off, d_out_cap, d_out_len,
-                                  d_status, o, window, st, nullptr, nullptr, 0, x_adapt);
+    return encode_device_internal(ctx, b, ctx->d_records, nullptr, 0, x_adapt);
 }
 
 // host twins of the stream's f8 speed codec (dv_engine.cuh: speed_to_u8_i16, u8_to_speed) and of speed_is_small
@@ -987,31 +982,72 @@ static bool mixmap_cands(divans_b200_ctx *ctx, const int32_t *values, uint32_t k
     }
     return true;
 }
-
-// The raw calls that build their record from opts (plain and speeds; auto and mixmap check their own candidates): raw_record keeps
-// the mode's low byte, so 256 would code as LSB6 and 4..255 as a record the encoder can only fail on.
-static bool raw_mode_ok(divans_b200_ctx *ctx, int raw_mode, const divans_b200_encode_options *o, const AutoSel *sel) {
-    if (!raw_mode || (sel && !sel->speeds) || (o->literal_pred_mode >= 0 && o->literal_pred_mode <= 3)) return true;
+// The entry check of a call's candidates, after its null checks and before any other: false (and the error) for candidates
+// its kind does not take, else the accepted candidates in sel.cands / sel.speeds.  The raw calls that build their record from
+// opts (plain and speeds) also check its mode: raw_record keeps the mode's low byte, so 256 would code as LSB6 and 4..255 as a
+// record the encoder can only fail on.
+static bool check_selection(divans_b200_ctx *ctx, int raw_mode, const divans_b200_encode_options *o, Selection &sel) {
+    switch (sel.kind) {
+    case SEL_AUTO:
+        if (!check_cands(ctx, sel.models, sel.k, !raw_mode)) return false;
+        std::copy(sel.models, sel.models + sel.k, sel.cands);
+        break;
+    case SEL_MIXMAP: if (!mixmap_cands(ctx, sel.mix_values, sel.k, o, sel.cands)) return false; break;
+    case SEL_SPEEDS: if (!speed_values(ctx, sel.speed_values, sel.k, sel.speeds)) return false; break;
+    case SEL_NONE: break;
+    }
+    if (!raw_mode || sel.kind == SEL_AUTO || sel.kind == SEL_MIXMAP || (o->literal_pred_mode >= 0 && o->literal_pred_mode <= 3)) return true;
     char buf[200];
     snprintf(buf, sizeof buf, "encode: opts->literal_pred_mode %d is outside 0..3", (int)o->literal_pred_mode);
     ctx->err = buf;
     return false;
 }
 
-// The four device encode calls: raw buffers (max_raw_len = max_in_len) or command lists (raw_mode 0), each plain or, with
-// `sel` (device chosen / cost), coded under the cheapest candidate literal model.  Host marshalling (the candidates' records,
-// the error strings) may throw, and no C++ exception may cross the C boundary.
+// The encode of a batch under its selection, in HBM
+static DivansResult encode_nolock(divans_b200_ctx *ctx, const EncBatch &b, const Selection &sel) {
+    switch (sel.kind) {
+    case SEL_AUTO: return encode_auto_device_nolock(ctx, b, sel);
+    case SEL_MIXMAP: return encode_mixmap_device_nolock(ctx, b, sel);
+    case SEL_SPEEDS: return encode_speeds_device_nolock(ctx, b, sel);
+    case SEL_NONE: break;
+    }
+    return encode_device_internal(ctx, b);
+}
+
+// What a selection needs per stream of a host call: its output columns (chosen u32, cost, halves u64, mixing bytes, bins u64;
+// the optional ones counted whether asked for or not, except bins), and the device scratch of its drivers in bytes per pair, per
+// slot of the pairs (next to the replay window) and per stream (mixmap: the winners, mixed record and mixing output).
+struct SelLayout {
+    size_t chosen_cols, cost_cols, halves_cols, mixing_bytes, bins_cols;
+    uint64_t pair_bytes, slot_bytes, stream_bytes;
+};
+static SelLayout sel_layout(const Selection &sel) {
+    const bool none = sel.kind == SEL_NONE, mix = sel.kind == SEL_MIXMAP, spd = sel.kind == SEL_SPEEDS;
+    SelLayout l;
+    l.chosen_cols = none ? 0 : spd ? 3 : 1;
+    l.cost_cols = none ? 0 : sel.k + (mix || spd ? 1 : 0);
+    l.halves_cols = spd ? 2 * (size_t)sel.k : 0;
+    l.mixing_bytes = mix ? MIX_ENTRIES : 0;
+    l.bins_cols = mix && sel.bins ? (size_t)sel.k * MIX_ENTRIES : 0;
+    l.pair_bytes = spd ? 96 : 0;
+    l.slot_bytes = mix ? MIX_ENTRIES * 8 : 0;
+    l.stream_bytes = mix ? MIX_ENTRIES * 9 + PM_RECORD_BYTES + l.bins_cols * 8 : 0;
+    return l;
+}
+
+// The device encode calls: raw buffers (max_raw_len = max_in_len) or command lists (raw_mode 0), each plain or under a
+// selection whose outputs are device arrays.  Host marshalling (the candidates' records, the error strings) may throw, and no
+// C++ exception may cross the C boundary.
 static DivansResult encode_device_common(divans_b200_ctx *ctx, size_t n, int raw_mode, const uint8_t *d_in, const uint64_t *d_in_off,
                                          const uint64_t *d_in_len, uint64_t max_in_len, uint64_t max_raw_len, uint8_t *d_out,
                                          const uint64_t *d_out_off, const uint64_t *d_out_cap, uint64_t *d_out_len, int32_t *d_status,
-                                         const divans_b200_encode_options *opts, void *cuda_stream, const AutoSel *sel) try {
+                                         const divans_b200_encode_options *opts, void *cuda_stream, Selection sel) try {
     if (!ctx || !opts) return DIVANS_FAILURE;
-    if (sel && !sel->speeds && !check_cands(ctx, sel->cands, sel->n_cands, !raw_mode)) return DIVANS_FAILURE;
-    if (!raw_mode_ok(ctx, raw_mode, opts, sel)) return DIVANS_FAILURE;
+    if (!check_selection(ctx, raw_mode, opts, sel)) return DIVANS_FAILURE;
     if (n == 0) return DIVANS_SUCCESS;
-    if (sel && !sel->mixmap && !sel->speeds && !sel->chosen) { ctx->err = raw_mode ? "encode_auto: d_chosen is required" : "encode_cmds_auto: d_chosen is required"; return DIVANS_FAILURE; }
-    if (sel && sel->mixmap && n > 0x7fffffffull) { ctx->err = "batch too large"; return DIVANS_FAILURE; }   // (one block per stream)
-    const uint64_t nv = (uint64_t)n * (sel ? sel->n_cands : 1);
+    if (sel.kind == SEL_AUTO && !sel.chosen) { ctx->err = raw_mode ? "encode_auto: d_chosen is required" : "encode_cmds_auto: d_chosen is required"; return DIVANS_FAILURE; }
+    if (sel.kind == SEL_MIXMAP && n > 0x7fffffffull) { ctx->err = "batch too large"; return DIVANS_FAILURE; }   // (one block per stream)
+    const uint64_t nv = (uint64_t)n * (sel.kind == SEL_NONE ? 1 : sel.k);
     if (nv > 0xffffffffull || max_in_len > 0x7fff0000ull || max_raw_len > 0x7fff0000ull) { ctx->err = "batch too large"; return DIVANS_FAILURE; }
     const int window = !raw_mode && opts->window_size == 0 ? 0 : clamp_window(opts->window_size);
     const LogCaps caps = raw_mode ? raw_log_caps(max_in_len, window) : cmds_log_caps(max_in_len, max_raw_len);
@@ -1040,17 +1076,8 @@ static DivansResult encode_device_common(divans_b200_ctx *ctx, size_t n, int raw
             ctx->sf_cap = words;
         }
     }
-    if (sel && sel->speeds)
-        return encode_speeds_device_nolock(ctx, n, raw_mode, d_in, d_in_off, d_in_len, max_in_len, caps, d_out, d_out_off, d_out_cap, d_out_len,
-                                           d_status, opts, window, *sel->speeds, sel->chosen, sel->cost, sel->halves, st);
-    if (sel && sel->mixmap)
-        return encode_mixmap_device_nolock(ctx, n, raw_mode, d_in, d_in_off, d_in_len, max_in_len, caps, d_out, d_out_off, d_out_cap, d_out_len,
-                                           d_status, opts, window, sel->cands, sel->n_cands, sel->chosen, sel->cost, sel->mixing, sel->bins, st);
-    if (sel)
-        return encode_auto_device_nolock(ctx, n, raw_mode, d_in, d_in_off, d_in_len, max_in_len, caps, d_out, d_out_off, d_out_cap, d_out_len,
-                                         d_status, opts, window, sel->cands, sel->n_cands, sel->chosen, sel->cost, st);
-    return encode_device_internal(ctx, n, raw_mode, d_in, d_in_off, d_in_len, max_in_len, caps, d_out, d_out_off, d_out_cap, d_out_len,
-                                  d_status, opts, window, st);
+    const EncBatch b = {n, raw_mode, d_in, d_in_off, d_in_len, max_in_len, caps, d_out, d_out_off, d_out_cap, d_out_len, d_status, opts, window, st};
+    return encode_nolock(ctx, b, sel);
 } catch (...) {
     if (ctx) ctx->err = "divans_b200: out of host memory";
     return DIVANS_FAILURE;
@@ -1061,7 +1088,7 @@ extern "C" DivansResult divans_b200_encode_batch_device(divans_b200_ctx *ctx, si
                                                         const uint64_t *d_out_off, const uint64_t *d_out_cap, uint64_t *d_out_len,
                                                         int32_t *d_status, const divans_b200_encode_options *opts, void *cuda_stream) {
     return encode_device_common(ctx, n, 1, d_in, d_in_off, d_in_len, max_in_len, max_in_len, d_out, d_out_off, d_out_cap, d_out_len,
-                                d_status, opts, cuda_stream, nullptr);
+                                d_status, opts, cuda_stream, Selection());
 }
 extern "C" DivansResult divans_b200_encode_auto_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_in, const uint64_t *d_in_off,
                                                              const uint64_t *d_in_len, uint64_t max_in_len, uint8_t *d_out,
@@ -1069,9 +1096,8 @@ extern "C" DivansResult divans_b200_encode_auto_batch_device(divans_b200_ctx *ct
                                                              int32_t *d_status, const divans_b200_encode_options *opts,
                                                              const divans_b200_literal_model *cands, uint32_t n_cands, uint32_t *d_chosen,
                                                              uint64_t *d_cost, void *cuda_stream) {
-    const AutoSel sel = {cands, n_cands, d_chosen, d_cost};
     return encode_device_common(ctx, n, 1, d_in, d_in_off, d_in_len, max_in_len, max_in_len, d_out, d_out_off, d_out_cap, d_out_len,
-                                d_status, opts, cuda_stream, &sel);
+                                d_status, opts, cuda_stream, sel_auto(cands, n_cands, d_chosen, d_cost));
 }
 extern "C" DivansResult divans_b200_encode_cmds_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_blobs, const uint64_t *d_blob_off,
                                                              const uint64_t *d_blob_len, uint64_t max_blob_len, uint64_t max_raw_len,
@@ -1079,7 +1105,7 @@ extern "C" DivansResult divans_b200_encode_cmds_batch_device(divans_b200_ctx *ct
                                                              uint64_t *d_out_len, int32_t *d_status, const divans_b200_encode_options *opts,
                                                              void *cuda_stream) {
     return encode_device_common(ctx, n, 0, d_blobs, d_blob_off, d_blob_len, max_blob_len, max_raw_len, d_out, d_out_off, d_out_cap,
-                                d_out_len, d_status, opts, cuda_stream, nullptr);
+                                d_out_len, d_status, opts, cuda_stream, Selection());
 }
 extern "C" DivansResult divans_b200_encode_cmds_auto_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_blobs,
                                                                   const uint64_t *d_blob_off, const uint64_t *d_blob_len,
@@ -1088,23 +1114,20 @@ extern "C" DivansResult divans_b200_encode_cmds_auto_batch_device(divans_b200_ct
                                                                   int32_t *d_status, const divans_b200_encode_options *opts,
                                                                   const divans_b200_literal_model *cands, uint32_t n_cands,
                                                                   uint32_t *d_chosen, uint64_t *d_cost, void *cuda_stream) {
-    const AutoSel sel = {cands, n_cands, d_chosen, d_cost};
     return encode_device_common(ctx, n, 0, d_blobs, d_blob_off, d_blob_len, max_blob_len, max_raw_len, d_out, d_out_off, d_out_cap,
-                                d_out_len, d_status, opts, cuda_stream, &sel);
+                                d_out_len, d_status, opts, cuda_stream, sel_auto(cands, n_cands, d_chosen, d_cost));
 }
 
-// The four host encode calls: marshal, split into sub-batches whose symbol logs fit in HBM, run, copy back.  Host marshalling
-// uses std::vector sized by the caller's arguments, and no C++ exception may cross the C boundary.
+// The host encode calls: marshal, split into sub-batches whose symbol logs (and selection scratch) fit in HBM, run, copy back.
+// Host marshalling uses std::vector sized by the caller's arguments, and no C++ exception may cross the C boundary.
 static DivansResult encode_host_common(divans_b200_ctx *ctx, size_t n, int raw_mode, const uint8_t *in, const uint64_t *in_off,
                                        const uint64_t *in_len, uint8_t *out, const uint64_t *out_off, const uint64_t *out_cap,
-                                       uint64_t *out_len, int32_t *status, const divans_b200_encode_options *opts,
-                                       const AutoSel *sel) try {
+                                       uint64_t *out_len, int32_t *status, const divans_b200_encode_options *opts, Selection sel) try {
     if (!ctx || !opts) return DIVANS_FAILURE;
-    if (sel && !sel->speeds && !check_cands(ctx, sel->cands, sel->n_cands, !raw_mode)) return DIVANS_FAILURE;
-    if (!raw_mode_ok(ctx, raw_mode, opts, sel)) return DIVANS_FAILURE;
+    if (!check_selection(ctx, raw_mode, opts, sel)) return DIVANS_FAILURE;
     if (n == 0) return DIVANS_SUCCESS;
-    if (sel && !sel->mixmap && !sel->speeds && !sel->chosen) { ctx->err = raw_mode ? "encode_auto: chosen is required" : "encode_cmds_auto: chosen is required"; return DIVANS_FAILURE; }
-    if (sel && (uint64_t)n * sel->n_cands > 0xffffffffull) { ctx->err = "batch too large"; return DIVANS_FAILURE; }
+    if (sel.kind == SEL_AUTO && !sel.chosen) { ctx->err = raw_mode ? "encode_auto: chosen is required" : "encode_cmds_auto: chosen is required"; return DIVANS_FAILURE; }
+    if (sel.kind != SEL_NONE && (uint64_t)n * sel.k > 0xffffffffull) { ctx->err = "batch too large"; return DIVANS_FAILURE; }
     std::lock_guard<std::mutex> lk(ctx->mu);
     CK(cudaSetDevice(ctx->device));
     const int window = clamp_window(opts->window_size);
@@ -1136,21 +1159,17 @@ static DivansResult encode_host_common(divans_b200_ctx *ctx, size_t n, int raw_m
     if (!grow(ctx, &b.d_in, &b.d_in_cap, (size_t)in_end + 64)) return DIVANS_FAILURE;
     cudaStream_t st = ctx->stream;
     CK(cudaMemcpyAsync(b.d_in, src, in_end, cudaMemcpyHostToDevice, st));
+    const SelLayout lay = sel_layout(sel);
     size_t i0 = 0;
     while (i0 < n) {
-        // grow the sub-batch while its uniform-capacity logs fit
+        // grow the sub-batch while its uniform-capacity logs fit, with a selection's replay windows and scratch for its m * k pairs
         LogCaps mc = {0, 0, 0};
         uint64_t mx = 0; size_t i1 = i0;
         while (i1 < n) {
             const LogCaps c = {std::max(need[i1].cmd, mc.cmd), std::max(need[i1].lit, mc.lit), std::max(need[i1].replay, mc.replay)};
-            // encode_auto: the cost pass also holds a replay window per slot for up to m * C pairs.  encode_mixmap: and 64 KiB of
-            // bins per slot, and per stream its winners, mixed record, mixing output and (when asked for) C x 64 KiB of bins
-            const uint64_t vs = sel ? (uint64_t)encode_slots(ctx, (i1 - i0 + 1) * (size_t)sel->n_cands) : 0;
-            uint64_t rep = vs * c.replay;
-            if (sel && sel->mixmap)
-                rep += vs * MIX_ENTRIES * 8 + (uint64_t)(i1 - i0 + 1) * (MIX_ENTRIES * 9 + PM_RECORD_BYTES + (sel->bins ? sel->n_cands * MIX_ENTRIES * 8ull : 0));
-            if (sel && sel->speeds) rep += (uint64_t)(i1 - i0 + 1) * sel->n_cands * 96;   // encode_speeds: scratch and halves, per pair
-            if (i1 > i0 && (c.cmd + c.lit) * 4 * (uint64_t)(i1 - i0 + 1) + rep > budget) break;
+            const uint64_t m = i1 - i0 + 1, vs = sel.kind == SEL_NONE ? 0 : (uint64_t)encode_slots(ctx, m * sel.k);
+            const uint64_t rep = vs * (c.replay + lay.slot_bytes) + m * lay.stream_bytes + m * sel.k * lay.pair_bytes;
+            if (i1 > i0 && (c.cmd + c.lit) * 4 * m + rep > budget) break;
             mc = c;
             if (in_len[i1] > mx) mx = in_len[i1];
             i1++;
@@ -1160,20 +1179,10 @@ static DivansResult encode_host_common(divans_b200_ctx *ctx, size_t n, int raw_m
         uint64_t out_lo, out_hi;
         regions_span(m, out_off + i0, out_cap + i0, out_lo, out_hi);
         if (!grow(ctx, &b.d_out, &b.d_out_cap, (size_t)(out_hi - out_lo) + 64)) return DIVANS_FAILURE;
-        // in_off | in_len | out_off | out_cap | out_len | status (+ encode_auto: chosen | cost [m * C]; encode_mixmap: cost [m * (C + 1)];
-        // encode_speeds: chosen [3m u32] | cost [m * (C + 1)] | halves [m * C * 2])
-        const bool spd = sel && sel->speeds;
-        const size_t cost_cols = sel ? sel->n_cands + (sel->mixmap || spd ? 1 : 0) : 0;
-        const size_t chosen_words = spd ? 2 * m : m, halves_words = spd ? 2 * m * (size_t)sel->n_cands : 0;
-        if (!grow(ctx, &b.d_meta, &b.d_meta_cap, m * 6 + (sel ? chosen_words + m * cost_cols + halves_words : 0))) return DIVANS_FAILURE;
-        // encode_mixmap: mixing [m * 8192 bytes] | bins [m * C * 8192]
-        uint8_t *d_mixing = nullptr; uint64_t *d_bins = nullptr;
-        if (sel && sel->mixmap) {
-            const size_t bw = sel->bins ? m * (size_t)sel->n_cands * MIX_ENTRIES : 0;
-            if (!grow(ctx, &ctx->d_mix_out, &ctx->mix_out_cap, m * (size_t)MIX_ENTRIES / 8 + bw)) return DIVANS_FAILURE;
-            if (sel->mixing) d_mixing = reinterpret_cast<uint8_t *>(ctx->d_mix_out);
-            if (sel->bins) d_bins = ctx->d_mix_out + m * (size_t)MIX_ENTRIES / 8;
-        }
+        // in_off | in_len | out_off | out_cap | out_len | status, then the selection's outputs: chosen | cost | halves | mixing | bins
+        const size_t chosen_words = (lay.chosen_cols + 1) / 2;
+        if (!grow(ctx, &b.d_meta, &b.d_meta_cap,
+                  m * (6 + chosen_words + lay.cost_cols + lay.halves_cols + lay.mixing_bytes / 8 + lay.bins_cols))) return DIVANS_FAILURE;
         std::vector<uint64_t> rel(m);
         for (size_t i = 0; i < m; i++) rel[i] = out_off[i0 + i] - out_lo;
         uint64_t *mm = b.d_meta;
@@ -1182,28 +1191,22 @@ static DivansResult encode_host_common(divans_b200_ctx *ctx, size_t n, int raw_m
         CK(cudaMemcpyAsync(mm + 2 * m, rel.data(), m * 8, cudaMemcpyHostToDevice, st));
         CK(cudaMemcpyAsync(mm + 3 * m, out_cap + i0, m * 8, cudaMemcpyHostToDevice, st));
         int32_t *d_status = reinterpret_cast<int32_t *>(mm + 5 * m);
-        uint32_t *d_chosen = reinterpret_cast<uint32_t *>(mm + 6 * m);
-        uint64_t *d_cost = mm + 6 * m + chosen_words, *d_halves = spd && sel->halves ? d_cost + m * cost_cols : nullptr;
-        DivansResult r = spd
-                             ? encode_speeds_device_nolock(ctx, m, raw_mode, b.d_in, mm, mm + m, mx, mc, b.d_out, mm + 2 * m, mm + 3 * m, mm + 4 * m,
-                                                           d_status, opts, window, *sel->speeds, d_chosen, d_cost, d_halves, st)
-                         : sel && sel->mixmap
-                             ? encode_mixmap_device_nolock(ctx, m, raw_mode, b.d_in, mm, mm + m, mx, mc, b.d_out, mm + 2 * m, mm + 3 * m, mm + 4 * m,
-                                                           d_status, opts, window, sel->cands, sel->n_cands, d_chosen, d_cost, d_mixing, d_bins, st)
-                         : sel ? encode_auto_device_nolock(ctx, m, raw_mode, b.d_in, mm, mm + m, mx, mc, b.d_out, mm + 2 * m, mm + 3 * m,
-                                                           mm + 4 * m, d_status, opts, window, sel->cands, sel->n_cands, d_chosen, d_cost, st)
-                               : encode_device_internal(ctx, m, raw_mode, b.d_in, mm, mm + m, mx, mc, b.d_out, mm + 2 * m, mm + 3 * m,
-                                                        mm + 4 * m, d_status, opts, window, st);
+        // the selection with its outputs in d_meta: chosen and cost always, the others where the caller asked for them
+        Selection ds = sel;
+        uint64_t *w = mm + 6 * m;
+        ds.chosen = reinterpret_cast<uint32_t *>(w); w += m * chosen_words;
+        ds.cost = w; w += m * lay.cost_cols;
+        ds.halves = sel.halves ? w : nullptr; w += m * lay.halves_cols;
+        ds.mixing = sel.mixing ? reinterpret_cast<uint8_t *>(w) : nullptr; w += m * lay.mixing_bytes / 8;
+        ds.bins = sel.bins ? w : nullptr;
+        const EncBatch eb = {m, raw_mode, b.d_in, mm, mm + m, mx, mc, b.d_out, mm + 2 * m, mm + 3 * m, mm + 4 * m, d_status, opts, window, st};
+        DivansResult r = encode_nolock(ctx, eb, ds);
         if (r != DIVANS_SUCCESS) return r;
-        if (sel) {
-            const size_t ccols = spd ? 3 : 1;
-            if (sel->chosen) CK(cudaMemcpyAsync(sel->chosen + i0 * ccols, d_chosen, m * ccols * 4, cudaMemcpyDeviceToHost, st));
-            if (d_halves) CK(cudaMemcpyAsync(sel->halves + i0 * 2 * (size_t)sel->n_cands, d_halves, halves_words * 8, cudaMemcpyDeviceToHost, st));
-            if (sel->cost) CK(cudaMemcpyAsync(sel->cost + i0 * cost_cols, d_cost, m * cost_cols * 8, cudaMemcpyDeviceToHost, st));
-            if (d_mixing) CK(cudaMemcpyAsync(sel->mixing + i0 * (size_t)MIX_ENTRIES, d_mixing, m * (size_t)MIX_ENTRIES, cudaMemcpyDeviceToHost, st));
-            if (d_bins) CK(cudaMemcpyAsync(sel->bins + i0 * (size_t)sel->n_cands * MIX_ENTRIES, d_bins, m * (size_t)sel->n_cands * MIX_ENTRIES * 8,
-                                           cudaMemcpyDeviceToHost, st));
-        }
+        if (sel.chosen) CK(cudaMemcpyAsync(sel.chosen + i0 * lay.chosen_cols, ds.chosen, m * lay.chosen_cols * 4, cudaMemcpyDeviceToHost, st));
+        if (sel.halves) CK(cudaMemcpyAsync(sel.halves + i0 * lay.halves_cols, ds.halves, m * lay.halves_cols * 8, cudaMemcpyDeviceToHost, st));
+        if (sel.cost) CK(cudaMemcpyAsync(sel.cost + i0 * lay.cost_cols, ds.cost, m * lay.cost_cols * 8, cudaMemcpyDeviceToHost, st));
+        if (sel.mixing) CK(cudaMemcpyAsync(sel.mixing + i0 * lay.mixing_bytes, ds.mixing, m * lay.mixing_bytes, cudaMemcpyDeviceToHost, st));
+        if (sel.bins) CK(cudaMemcpyAsync(sel.bins + i0 * lay.bins_cols, ds.bins, m * lay.bins_cols * 8, cudaMemcpyDeviceToHost, st));
         CK(cudaMemcpyAsync(out_len + i0, mm + 4 * m, m * 8, cudaMemcpyDeviceToHost, st));
         CK(cudaMemcpyAsync(status + i0, d_status, m * 4, cudaMemcpyDeviceToHost, st));
         CK(cudaStreamSynchronize(st));
@@ -1222,29 +1225,27 @@ extern "C" DivansResult divans_b200_encode_batch_host(divans_b200_ctx *ctx, size
                                                       const uint64_t *in_len, uint8_t *out, const uint64_t *out_off,
                                                       const uint64_t *out_cap, uint64_t *out_len, int32_t *status,
                                                       const divans_b200_encode_options *opts) {
-    return encode_host_common(ctx, n, 1, in, in_off, in_len, out, out_off, out_cap, out_len, status, opts, nullptr);
+    return encode_host_common(ctx, n, 1, in, in_off, in_len, out, out_off, out_cap, out_len, status, opts, Selection());
 }
 extern "C" DivansResult divans_b200_encode_auto_batch_host(divans_b200_ctx *ctx, size_t n, const uint8_t *in, const uint64_t *in_off,
                                                            const uint64_t *in_len, uint8_t *out, const uint64_t *out_off, const uint64_t *out_cap,
                                                            uint64_t *out_len, int32_t *status, const divans_b200_encode_options *opts,
                                                            const divans_b200_literal_model *cands, uint32_t n_cands, uint32_t *chosen,
                                                            uint64_t *cost) {
-    const AutoSel sel = {cands, n_cands, chosen, cost};
-    return encode_host_common(ctx, n, 1, in, in_off, in_len, out, out_off, out_cap, out_len, status, opts, &sel);
+    return encode_host_common(ctx, n, 1, in, in_off, in_len, out, out_off, out_cap, out_len, status, opts, sel_auto(cands, n_cands, chosen, cost));
 }
 extern "C" DivansResult divans_b200_encode_cmds_batch_host(divans_b200_ctx *ctx, size_t n, const uint8_t *blobs, const uint64_t *blob_off,
                                                            const uint64_t *blob_len, uint8_t *out, const uint64_t *out_off,
                                                            const uint64_t *out_cap, uint64_t *out_len, int32_t *status,
                                                            const divans_b200_encode_options *opts) {
-    return encode_host_common(ctx, n, 0, blobs, blob_off, blob_len, out, out_off, out_cap, out_len, status, opts, nullptr);
+    return encode_host_common(ctx, n, 0, blobs, blob_off, blob_len, out, out_off, out_cap, out_len, status, opts, Selection());
 }
 extern "C" DivansResult divans_b200_encode_cmds_auto_batch_host(divans_b200_ctx *ctx, size_t n, const uint8_t *blobs, const uint64_t *blob_off,
                                                                 const uint64_t *blob_len, uint8_t *out, const uint64_t *out_off,
                                                                 const uint64_t *out_cap, uint64_t *out_len, int32_t *status,
                                                                 const divans_b200_encode_options *opts, const divans_b200_literal_model *cands,
                                                                 uint32_t n_cands, uint32_t *chosen, uint64_t *cost) {
-    const AutoSel sel = {cands, n_cands, chosen, cost};
-    return encode_host_common(ctx, n, 0, blobs, blob_off, blob_len, out, out_off, out_cap, out_len, status, opts, &sel);
+    return encode_host_common(ctx, n, 0, blobs, blob_off, blob_len, out, out_off, out_cap, out_len, status, opts, sel_auto(cands, n_cands, chosen, cost));
 }
 
 // ---- per-context mixing values ----
@@ -1253,10 +1254,8 @@ extern "C" DivansResult divans_b200_encode_mixmap_batch_host(divans_b200_ctx *ct
                                                              uint64_t *out_len, int32_t *status, const divans_b200_encode_options *opts,
                                                              const int32_t *values, uint32_t n_values, uint32_t *chosen, uint8_t *mixing,
                                                              uint64_t *cost, uint64_t *bins) {
-    divans_b200_literal_model cands[16];
-    if (!ctx || !opts || !mixmap_cands(ctx, values, n_values, opts, cands)) return DIVANS_FAILURE;
-    const AutoSel sel = {cands, n_values, chosen, cost, true, mixing, bins};
-    return encode_host_common(ctx, n, 1, in, in_off, in_len, out, out_off, out_cap, out_len, status, opts, &sel);
+    return encode_host_common(ctx, n, 1, in, in_off, in_len, out, out_off, out_cap, out_len, status, opts,
+                              sel_mixmap(values, n_values, chosen, mixing, cost, bins));
 }
 extern "C" DivansResult divans_b200_encode_mixmap_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_in, const uint64_t *d_in_off,
                                                                const uint64_t *d_in_len, uint64_t max_in_len, uint8_t *d_out,
@@ -1264,21 +1263,16 @@ extern "C" DivansResult divans_b200_encode_mixmap_batch_device(divans_b200_ctx *
                                                                int32_t *d_status, const divans_b200_encode_options *opts, const int32_t *values,
                                                                uint32_t n_values, uint32_t *d_chosen, uint8_t *d_mixing, uint64_t *d_cost,
                                                                uint64_t *d_bins, void *cuda_stream) {
-    divans_b200_literal_model cands[16];
-    if (!ctx || !opts || !mixmap_cands(ctx, values, n_values, opts, cands)) return DIVANS_FAILURE;
-    const AutoSel sel = {cands, n_values, d_chosen, d_cost, true, d_mixing, d_bins};
     return encode_device_common(ctx, n, 1, d_in, d_in_off, d_in_len, max_in_len, max_in_len, d_out, d_out_off, d_out_cap, d_out_len,
-                                d_status, opts, cuda_stream, &sel);
+                                d_status, opts, cuda_stream, sel_mixmap(values, n_values, d_chosen, d_mixing, d_cost, d_bins));
 }
 extern "C" DivansResult divans_b200_encode_cmds_mixmap_batch_host(divans_b200_ctx *ctx, size_t n, const uint8_t *blobs, const uint64_t *blob_off,
                                                                   const uint64_t *blob_len, uint8_t *out, const uint64_t *out_off,
                                                                   const uint64_t *out_cap, uint64_t *out_len, int32_t *status,
                                                                   const divans_b200_encode_options *opts, const int32_t *values, uint32_t n_values,
                                                                   uint32_t *chosen, uint8_t *mixing, uint64_t *cost, uint64_t *bins) {
-    divans_b200_literal_model cands[16];
-    if (!ctx || !opts || !mixmap_cands(ctx, values, n_values, opts, cands)) return DIVANS_FAILURE;
-    const AutoSel sel = {cands, n_values, chosen, cost, true, mixing, bins};
-    return encode_host_common(ctx, n, 0, blobs, blob_off, blob_len, out, out_off, out_cap, out_len, status, opts, &sel);
+    return encode_host_common(ctx, n, 0, blobs, blob_off, blob_len, out, out_off, out_cap, out_len, status, opts,
+                              sel_mixmap(values, n_values, chosen, mixing, cost, bins));
 }
 extern "C" DivansResult divans_b200_encode_cmds_mixmap_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_blobs,
                                                                     const uint64_t *d_blob_off, const uint64_t *d_blob_len,
@@ -1287,11 +1281,8 @@ extern "C" DivansResult divans_b200_encode_cmds_mixmap_batch_device(divans_b200_
                                                                     int32_t *d_status, const divans_b200_encode_options *opts,
                                                                     const int32_t *values, uint32_t n_values, uint32_t *d_chosen,
                                                                     uint8_t *d_mixing, uint64_t *d_cost, uint64_t *d_bins, void *cuda_stream) {
-    divans_b200_literal_model cands[16];
-    if (!ctx || !opts || !mixmap_cands(ctx, values, n_values, opts, cands)) return DIVANS_FAILURE;
-    const AutoSel sel = {cands, n_values, d_chosen, d_cost, true, d_mixing, d_bins};
     return encode_device_common(ctx, n, 0, d_blobs, d_blob_off, d_blob_len, max_blob_len, max_raw_len, d_out, d_out_off, d_out_cap,
-                                d_out_len, d_status, opts, cuda_stream, &sel);
+                                d_out_len, d_status, opts, cuda_stream, sel_mixmap(values, n_values, d_chosen, d_mixing, d_cost, d_bins));
 }
 
 // ---- literal speeds ----
@@ -1300,11 +1291,8 @@ extern "C" DivansResult divans_b200_encode_speeds_batch_host(divans_b200_ctx *ct
                                                              uint64_t *out_len, int32_t *status, const divans_b200_encode_options *opts,
                                                              const int16_t *values, uint32_t n_values, uint32_t *chosen, uint64_t *cost,
                                                              uint64_t *halves) {
-    SpeedValues vals;
-    if (!ctx || !opts || !speed_values(ctx, values, n_values, vals)) return DIVANS_FAILURE;
-    AutoSel sel = {nullptr, n_values, chosen, cost};
-    sel.speeds = &vals; sel.halves = halves;
-    return encode_host_common(ctx, n, 1, in, in_off, in_len, out, out_off, out_cap, out_len, status, opts, &sel);
+    return encode_host_common(ctx, n, 1, in, in_off, in_len, out, out_off, out_cap, out_len, status, opts,
+                              sel_speeds(values, n_values, chosen, cost, halves));
 }
 extern "C" DivansResult divans_b200_encode_speeds_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_in, const uint64_t *d_in_off,
                                                                const uint64_t *d_in_len, uint64_t max_in_len, uint8_t *d_out,
@@ -1312,23 +1300,16 @@ extern "C" DivansResult divans_b200_encode_speeds_batch_device(divans_b200_ctx *
                                                                int32_t *d_status, const divans_b200_encode_options *opts, const int16_t *values,
                                                                uint32_t n_values, uint32_t *d_chosen, uint64_t *d_cost, uint64_t *d_halves,
                                                                void *cuda_stream) {
-    SpeedValues vals;
-    if (!ctx || !opts || !speed_values(ctx, values, n_values, vals)) return DIVANS_FAILURE;
-    AutoSel sel = {nullptr, n_values, d_chosen, d_cost};
-    sel.speeds = &vals; sel.halves = d_halves;
     return encode_device_common(ctx, n, 1, d_in, d_in_off, d_in_len, max_in_len, max_in_len, d_out, d_out_off, d_out_cap, d_out_len,
-                                d_status, opts, cuda_stream, &sel);
+                                d_status, opts, cuda_stream, sel_speeds(values, n_values, d_chosen, d_cost, d_halves));
 }
 extern "C" DivansResult divans_b200_encode_cmds_speeds_batch_host(divans_b200_ctx *ctx, size_t n, const uint8_t *blobs, const uint64_t *blob_off,
                                                                   const uint64_t *blob_len, uint8_t *out, const uint64_t *out_off,
                                                                   const uint64_t *out_cap, uint64_t *out_len, int32_t *status,
                                                                   const divans_b200_encode_options *opts, const int16_t *values, uint32_t n_values,
                                                                   uint32_t *chosen, uint64_t *cost, uint64_t *halves) {
-    SpeedValues vals;
-    if (!ctx || !opts || !speed_values(ctx, values, n_values, vals)) return DIVANS_FAILURE;
-    AutoSel sel = {nullptr, n_values, chosen, cost};
-    sel.speeds = &vals; sel.halves = halves;
-    return encode_host_common(ctx, n, 0, blobs, blob_off, blob_len, out, out_off, out_cap, out_len, status, opts, &sel);
+    return encode_host_common(ctx, n, 0, blobs, blob_off, blob_len, out, out_off, out_cap, out_len, status, opts,
+                              sel_speeds(values, n_values, chosen, cost, halves));
 }
 extern "C" DivansResult divans_b200_encode_cmds_speeds_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_blobs,
                                                                     const uint64_t *d_blob_off, const uint64_t *d_blob_len,
@@ -1337,12 +1318,8 @@ extern "C" DivansResult divans_b200_encode_cmds_speeds_batch_device(divans_b200_
                                                                     int32_t *d_status, const divans_b200_encode_options *opts,
                                                                     const int16_t *values, uint32_t n_values, uint32_t *d_chosen,
                                                                     uint64_t *d_cost, uint64_t *d_halves, void *cuda_stream) {
-    SpeedValues vals;
-    if (!ctx || !opts || !speed_values(ctx, values, n_values, vals)) return DIVANS_FAILURE;
-    AutoSel sel = {nullptr, n_values, d_chosen, d_cost};
-    sel.speeds = &vals; sel.halves = d_halves;
     return encode_device_common(ctx, n, 0, d_blobs, d_blob_off, d_blob_len, max_blob_len, max_raw_len, d_out, d_out_off, d_out_cap,
-                                d_out_len, d_status, opts, cuda_stream, &sel);
+                                d_out_len, d_status, opts, cuda_stream, sel_speeds(values, n_values, d_chosen, d_cost, d_halves));
 }
 
 // ---- replaying command lists to raw bytes ----
@@ -1462,17 +1439,13 @@ extern "C" DivansResult divans_b200_lz77_cmds_batch_device(divans_b200_ctx *ctx,
         ctx->lz_scratch_asked = want;
     }
     warps = std::min<uint64_t>(warps, ctx->lz_scratch_words / stride);
-    if (!ctx->d_lz_pm) CK(cudaMalloc((void **)&ctx->d_lz_pm, PM_RECORD_BYTES));
-    if (ctx->busy_recorded) CK(cudaStreamWaitEvent(st, ctx->ev_busy, 0));
     // the record of lz77_blob: pred_mode and mixing_value stored as bytes
-    std::vector<uint8_t> &pm = ctx->h_pm;
-    pm.assign(PM_RECORD_BYTES, 0);
-    raw_record(pm.data(), pred_mode, mixing_value);
-    CK(cudaMemcpyAsync(ctx->d_lz_pm, pm.data(), PM_RECORD_BYTES, cudaMemcpyHostToDevice, st));
+    const divans_b200_literal_model rec = {pred_mode, mixing_value};
+    if (stage_records(ctx, &rec, 1, 0, st) != DIVANS_SUCCESS) return DIVANS_FAILURE;
     Lz77Params lp;
     lp.in = d_in; lp.in_off = d_in_off; lp.in_len = d_in_len; lp.max_in_len = max_in_len;
     lp.blobs = d_blobs; lp.blob_off = d_blob_off; lp.blob_cap = d_blob_cap; lp.blob_len = d_blob_len; lp.status = d_status;
-    lp.pm = ctx->d_lz_pm; lp.n_streams = (uint32_t)n; lp.window = window;
+    lp.pm = ctx->d_records; lp.n_streams = (uint32_t)n; lp.window = window;
     lp.work_counter = ctx->d_counter; lp.scratch = ctx->d_lz_scratch; lp.stride = stride; lp.n_warps = (uint32_t)warps;
     CK(cudaMemsetAsync(ctx->d_counter, 0, 4, st));
     CK(cudaEventRecord(ctx->ev0, st));

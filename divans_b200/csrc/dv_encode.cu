@@ -465,42 +465,22 @@ __global__ void __launch_bounds__(128) encode_mux_kernel(EncodeParams p) {
 
 #endif  // !DV_BLEND
 
+template <bool BLEND>
+void launch_encode_walk(EncodeWalk w, const EncodeParams &p, const BinParams &b, uint32_t n_blocks, cudaStream_t st) {
+    const size_t smem = (size_t)(DECODE_BLOCK_THREADS / 16) * SMEM_BYTES_PER_GROUP;
+    switch (w) {
+    case EncodeWalk::MODEL: encode_model_kernel<BLEND, false><<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p); break;
+    case EncodeWalk::TALLY: encode_model_kernel<BLEND, true><<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p); break;
+    case EncodeWalk::BINS: encode_bins_kernel<BLEND><<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p, b); break;
+    case EncodeWalk::SPEEDS_MODEL: encode_speeds_kernel<BLEND, false><<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p); break;
+    case EncodeWalk::SPEEDS: encode_speeds_kernel<BLEND, true><<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p); break;
+    }
+}
+
 #ifdef DV_BLEND
-void launch_encode_model_blend(const EncodeParams &p, uint32_t n_blocks, cudaStream_t st) {
-    size_t smem = (size_t)(DECODE_BLOCK_THREADS / 16) * SMEM_BYTES_PER_GROUP;
-    encode_model_kernel<true, false><<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p);
-}
-void launch_encode_tally_blend(const EncodeParams &p, uint32_t n_blocks, cudaStream_t st) {
-    size_t smem = (size_t)(DECODE_BLOCK_THREADS / 16) * SMEM_BYTES_PER_GROUP;
-    encode_model_kernel<true, true><<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p);
-}
-void launch_encode_bins_blend(const EncodeParams &p, const BinParams &b, uint32_t n_blocks, cudaStream_t st) {
-    size_t smem = (size_t)(DECODE_BLOCK_THREADS / 16) * SMEM_BYTES_PER_GROUP;
-    encode_bins_kernel<true><<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p, b);
-}
-void launch_encode_speeds_blend(const EncodeParams &p, bool tally, uint32_t n_blocks, cudaStream_t st) {
-    size_t smem = (size_t)(DECODE_BLOCK_THREADS / 16) * SMEM_BYTES_PER_GROUP;
-    if (tally) encode_speeds_kernel<true, true><<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p);
-    else encode_speeds_kernel<true, false><<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p);
-}
+template void launch_encode_walk<true>(EncodeWalk, const EncodeParams &, const BinParams &, uint32_t, cudaStream_t);
 #else
-void launch_encode_model(const EncodeParams &p, uint32_t n_blocks, cudaStream_t st) {
-    size_t smem = (size_t)(DECODE_BLOCK_THREADS / 16) * SMEM_BYTES_PER_GROUP;
-    encode_model_kernel<false, false><<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p);
-}
-void launch_encode_tally(const EncodeParams &p, uint32_t n_blocks, cudaStream_t st) {
-    size_t smem = (size_t)(DECODE_BLOCK_THREADS / 16) * SMEM_BYTES_PER_GROUP;
-    encode_model_kernel<false, true><<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p);
-}
-void launch_encode_bins(const EncodeParams &p, const BinParams &b, uint32_t n_blocks, cudaStream_t st) {
-    size_t smem = (size_t)(DECODE_BLOCK_THREADS / 16) * SMEM_BYTES_PER_GROUP;
-    encode_bins_kernel<false><<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p, b);
-}
-void launch_encode_speeds(const EncodeParams &p, bool tally, uint32_t n_blocks, cudaStream_t st) {
-    size_t smem = (size_t)(DECODE_BLOCK_THREADS / 16) * SMEM_BYTES_PER_GROUP;
-    if (tally) encode_speeds_kernel<false, true><<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p);
-    else encode_speeds_kernel<false, false><<<n_blocks, DECODE_BLOCK_THREADS, smem, st>>>(p);
-}
+template void launch_encode_walk<false>(EncodeWalk, const EncodeParams &, const BinParams &, uint32_t, cudaStream_t);
 
 // ---------------------------------------------------------------------------------------------------------------
 // literal speeds (divans_b200_encode_speeds_*): n streams x k candidate speeds v[0..k), pairs candidate-major (v = c * n + i)

@@ -22,32 +22,27 @@ void launch_decode_v2(int lanes_per_stream, bool blend, const DecodeParams &p, u
 void launch_decode_blend(const DecodeParams &p, const RecParams *r, uint32_t n_blocks, cudaStream_t st);   // its blend kernels (r: recording)
 int decode_max_blocks_per_sm_v2(int lanes_per_stream);
 int decode_groups_per_block_v2(int lanes_per_stream);
-void launch_encode_model(const EncodeParams &p, uint32_t n_blocks, cudaStream_t st);   // groups of 16 lanes
+// The encoder's model walks on n_blocks blocks of groups of 16 lanes: the model pass, which logs (SPEEDS_MODEL: under each
+// stream's speeds, EncodeParams::v_adapt), and the cost passes (no logs: EncodeParams::cost_tab / tally) of the selections:
+// TALLY, BINS (per-context mixing values, BinParams) and SPEEDS (each stream's speeds, with literal halves).  BLEND: under the
+// blend model.  dv_encode.cu instantiates BLEND = false, and built with DV_BLEND, true.
+enum class EncodeWalk { MODEL, TALLY, BINS, SPEEDS_MODEL, SPEEDS };
+template <bool BLEND> void launch_encode_walk(EncodeWalk w, const EncodeParams &p, const BinParams &b, uint32_t n_blocks, cudaStream_t st);
 void launch_encode_flush_mux(const EncodeParams &p, cudaStream_t st);                  // reverse rANS + mux/CRC (2 launches)
 int encode_max_blocks_per_sm();
-// the encoder's model pass under the blend model (dv_encode.cu built with DV_BLEND)
-void launch_encode_model_blend(const EncodeParams &p, uint32_t n_blocks, cudaStream_t st);
 void launch_rcp15_init(uint64_t *tab, cudaStream_t st);
-// model selection: the cost-only model passes (no logs: EncodeParams::cost_tab / tally), the fan-out of n streams to n x C
-// virtual streams (candidate-major) and the per-stream argmin
-void launch_encode_tally(const EncodeParams &p, uint32_t n_blocks, cudaStream_t st);
-void launch_encode_tally_blend(const EncodeParams &p, uint32_t n_blocks, cudaStream_t st);
+// model selection: the fan-out of n streams to n x C virtual streams (candidate-major) and the per-stream argmin
 void launch_auto_fanout(const uint64_t *in_off, const uint64_t *in_len, uint64_t n, uint32_t n_cands, uint64_t *v_off, uint64_t *v_len,
                         uint32_t *v_pm, cudaStream_t st);
 void launch_auto_select(const uint64_t *tally, const int32_t *v_status, uint64_t n, uint32_t n_cands, uint32_t *chosen, uint64_t *cost,
                         cudaStream_t st);
-// per-context mixing values: the binned cost pass over the n x k fan-out (BinParams), the kernel that builds each stream's
-// mixed record from the per-entry winners, and the choice between the best uniform record and the mixed one (dv_encode.cu)
-void launch_encode_bins(const EncodeParams &p, const BinParams &b, uint32_t n_blocks, cudaStream_t st);
-void launch_encode_bins_blend(const EncodeParams &p, const BinParams &b, uint32_t n_blocks, cudaStream_t st);
+// per-context mixing values: the kernel that builds each stream's mixed record from the per-entry winners, and the choice
+// between the best uniform record and the mixed one (dv_encode.cu)
 void launch_mixmap_map(const uint64_t *best, uint64_t n, const MixValues &vals, uint8_t *records, uint32_t *mix_idx, cudaStream_t st);
 void launch_mixmap_select(const uint64_t *tally, const int32_t *v_status, const uint64_t *x_tally, const int32_t *x_status, uint64_t n,
                           const MixValues &vals, const uint8_t *records, uint32_t *rec_idx, uint32_t *chosen, uint64_t *cost, uint8_t *mixing,
                           cudaStream_t st);
-// literal speeds: the model pass (tally: the cost pass with literal halves) under per-stream speeds (EncodeParams::v_adapt), the
-// kernel that builds each stage's speeds, and the final choice (dv_encode.cu)
-void launch_encode_speeds(const EncodeParams &p, bool tally, uint32_t n_blocks, cudaStream_t st);
-void launch_encode_speeds_blend(const EncodeParams &p, bool tally, uint32_t n_blocks, cudaStream_t st);
+// literal speeds: the kernel that builds each stage's speeds, and the final choice (dv_encode.cu)
 void launch_speeds_stage(int stage, uint64_t n, const SpeedValues &vals, const uint64_t *tally, const int32_t *v_status, const uint64_t *halves,
                          uint32_t *sel, int *v_adapt, int *x_adapt, cudaStream_t st);
 void launch_speeds_select(uint64_t n, const SpeedValues &vals, bool tuned, const uint64_t *tally, const int32_t *v_status,

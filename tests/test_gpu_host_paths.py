@@ -114,8 +114,9 @@ def test_host_encode_writes_only_the_returned_bytes(engine, call):
 
 
 def test_launch_count_of_each_entry_point():
-    """Launches per small call: decode 4, decode to command lists 5, encode 4, encode_auto / encode_cmds_auto 7, and one more
-    on a context's first encode (its reciprocal table).  Host and device variants alike."""
+    """Launches per small call: decode 4, decode to command lists 5, encode 4, encode_auto / encode_cmds_auto 7, encode_mixmap
+    9, encode_speeds 8, or 12 with its halves passes (dynamic context mixing 2, more than one speed), and one more on a
+    context's first encode (its reciprocal table).  Raw and command lists, host and device variants alike."""
     import torch
     eng = divans_b200.Engine(0, 64, 16)
     try:
@@ -138,6 +139,11 @@ def test_launch_count_of_each_entry_point():
         assert delta(lambda: eng.encode(lists, cmds=True)) == 4
         assert delta(lambda: eng.encode_auto(raws)) == 7
         assert delta(lambda: eng.encode_cmds_auto(lists)) == 7
+        halves = divans_b200.encode_options(dynamic_context_mixing=2)
+        for cmds, items in ((False, raws), (True, lists)):
+            assert delta(lambda: eng.encode_cmds_mixmap(items) if cmds else eng.encode_mixmap(items)) == 9
+            assert delta(lambda: eng.encode_cmds_speeds(items) if cmds else eng.encode_speeds(items)) == 8
+            assert delta(lambda: eng.encode_cmds_speeds(items, halves) if cmds else eng.encode_speeds(items, halves)) == 12
 
         n = len(raws)
         d_out, d_len, d_st, d_ch = (torch.zeros(e_total, dtype=torch.uint8, device="cuda"), torch.zeros(n, dtype=torch.int64, device="cuda"),
@@ -153,6 +159,14 @@ def test_launch_count_of_each_entry_point():
         assert delta(lambda: eng.encode_auto_batch_device(*raw_in, *outs, d_ch.data_ptr())) == 7
         assert delta(lambda: eng.encode_cmds_auto_batch_device(*lst_in, *outs, d_ch.data_ptr())) == 7
         assert (d_st.cpu().numpy() == 0).all()
+        for ins, mixmap, speeds in ((raw_in, eng.encode_mixmap_batch_device, eng.encode_speeds_batch_device),
+                                    (lst_in, eng.encode_cmds_mixmap_batch_device, eng.encode_cmds_speeds_batch_device)):
+            assert delta(lambda: mixmap(*ins, *outs)) == 9
+            assert (d_st.cpu().numpy() == 0).all()
+            assert delta(lambda: speeds(*ins, *outs)) == 8
+            assert (d_st.cpu().numpy() == 0).all()
+            assert delta(lambda: speeds(*ins, *outs, opts=halves)) == 12
+            assert (d_st.cpu().numpy() == 0).all()
 
         sblob, s_off, s_len = _pack(streams)
         d_cap = np.array([len(r) for r in raws], np.uint64)
