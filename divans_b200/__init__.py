@@ -52,6 +52,7 @@ BATCH_SYMBOLS = [
     "divans_b200_encode_speeds_batch_device",
     "divans_b200_encode_cmds_speeds_batch_host",
     "divans_b200_encode_cmds_speeds_batch_device",
+    "divans_b200_lz77_cmds_batch_parse", "divans_b200_lz77_cmds_batch_device_parse", "divans_b200_encode_cmds_choose_batch_device",
 ]
 PM_RECORD_BYTES = 32 + 16384 + 1024 + 8192   # one prediction-mode record of a DVCL blob (include/divans_b200.h)
 
@@ -97,6 +98,17 @@ LITERAL_SPEED_PALETTE = [(0, 1024), (2, 1024), (1, 128), (1, 16384), (2, 2048), 
 # encode_speeds' default candidates: MUD (16, 8192), the speed every stream is coded with otherwise, first, then the palette
 # speeds the real-text survey picks (DESIGN.md section 4, "Literal speeds").
 DEFAULT_LITERAL_SPEEDS = [(16, 8192), (32, 4096), (64, 16384), (128, 16384), (512, 16384), (1664, 16384)]
+
+
+class Lz77Parse(ctypes.Structure):
+    """divans_b200_lz77_parse: the LZ77 generator's minimum copy (4..32) and lazy lookahead steps (0..2)"""
+    _fields_ = [("min_match", ctypes.c_int32), ("lazy", ctypes.c_int32)]
+
+
+# compress_device's default parses, (min_match, lazy): (4, 0), the generator's own parse, first, so no stream costs more than
+# under it; then the parses a greedy survey of the corpora picks (tools/lz77_parse_probe.py --survey, DESIGN.md section 4,
+# "Choosing the LZ77 parse").
+DEFAULT_LZ77_PARSES = [(4, 0), (7, 2), (10, 2), (6, 2)]
 
 
 class CAllocator(ctypes.Structure):
@@ -176,6 +188,13 @@ def load_library():
     L.divans_b200_lz77_cmds_batch_device.argtypes = [vp, sz, vp, vp, vp, ctypes.c_uint64, ctypes.c_int32, ctypes.c_int32, ctypes.c_int32, vp, vp,
                                                      vp, vp, vp, vp]
     L.divans_b200_lz77_cmds_batch_device.restype = ctypes.c_uint8
+    L.divans_b200_lz77_cmds_batch_parse.argtypes = L.divans_b200_lz77_cmds_batch.argtypes + [ctypes.POINTER(Lz77Parse)]
+    L.divans_b200_lz77_cmds_batch_parse.restype = ctypes.c_uint8
+    L.divans_b200_lz77_cmds_batch_device_parse.argtypes = L.divans_b200_lz77_cmds_batch_device.argtypes[:-1] + [ctypes.POINTER(Lz77Parse), vp]
+    L.divans_b200_lz77_cmds_batch_device_parse.restype = ctypes.c_uint8
+    L.divans_b200_encode_cmds_choose_batch_device.argtypes = [vp, sz, ctypes.c_uint32, vp, vp, vp, ctypes.c_uint64, ctypes.c_uint64, vp, vp, vp,
+                                                              vp, vp, ctypes.POINTER(EncodeOptions), vp, vp, vp]
+    L.divans_b200_encode_cmds_choose_batch_device.restype = ctypes.c_uint8
     # reference FFI
     L.divans_new_decompressor.restype = vp
     L.divans_new_serial_decompressor.restype = vp
@@ -260,23 +279,36 @@ def kernel_version():
     return load_library().divans_b200_kernel_version().decode()
 
 
-def lz77_cmds_batch(blob, in_off, in_len, window=16, pred_mode=2, mixing_value=4, n_threads=None):
+def _parse(parse):
+    """(min_match, lazy) -> a Lz77Parse (the C calls refuse one outside min_match 4..32, lazy 0..2)"""
+    mm, lz = parse
+    return Lz77Parse(int(mm), int(lz))
+
+
+def lz77_cmds_batch(blob, in_off, in_len, window=16, pred_mode=2, mixing_value=4, n_threads=None, parse=None):
     """Raw buffers -> DVCL command lists by the library's greedy LZ77 (divans_b200_lz77_cmds_batch): returns
-    (blobs uint8 array, blob_off, blob_len) ready for Engine.encode_batch_host(..., cmds=True)."""
+    (blobs uint8 array, blob_off, blob_len) ready for Engine.encode_batch_host(..., cmds=True).  ``parse`` (min_match, lazy):
+    the parse of divans_b200_lz77_cmds_batch_parse (include/divans_b200.h); None is (4, 0)."""
     L = load_library()
+    if parse is not None:
+        ps = _parse(parse)
+        if not (4 <= ps.min_match <= 32 and 0 <= ps.lazy <= 2):
+            raise ValueError("lz77_cmds_batch: parse (%d, %d) is outside min_match 4..32, lazy 0..2" % (ps.min_match, ps.lazy))
+        fn = lambda *a: L.divans_b200_lz77_cmds_batch_parse(*a, ctypes.byref(ps))
+    else:
+        fn = L.divans_b200_lz77_cmds_batch
     blob = _u8(blob)
     in_off, in_len = np.ascontiguousarray(in_off, np.uint64), np.ascontiguousarray(in_len, np.uint64)
     n = len(in_off)
     boff, blen = np.zeros(n, np.uint64), np.zeros(n, np.uint64)
     total = ctypes.c_size_t(0)
     nt = int(n_threads or os.cpu_count() or 1)
-    rc = L.divans_b200_lz77_cmds_batch(n, _ptr(blob), _ptr(in_off), _ptr(in_len), window, pred_mode, mixing_value, None, 0, _ptr(boff), _ptr(blen),
-                                       ctypes.byref(total), nt)
+    rc = fn(n, _ptr(blob), _ptr(in_off), _ptr(in_len), window, pred_mode, mixing_value, None, 0, _ptr(boff), _ptr(blen), ctypes.byref(total), nt)
     if rc != DIVANS_NEEDS_MORE_OUTPUT and not (rc == DIVANS_SUCCESS and total.value == 0):
         raise ValueError("lz77_cmds_batch failed")
     out = np.zeros(max(1, total.value), np.uint8)
-    rc = L.divans_b200_lz77_cmds_batch(n, _ptr(blob), _ptr(in_off), _ptr(in_len), window, pred_mode, mixing_value, _ptr(out), out.size, _ptr(boff),
-                                       _ptr(blen), ctypes.byref(total), nt)
+    rc = fn(n, _ptr(blob), _ptr(in_off), _ptr(in_len), window, pred_mode, mixing_value, _ptr(out), out.size, _ptr(boff), _ptr(blen),
+            ctypes.byref(total), nt)
     if rc != DIVANS_SUCCESS:
         raise ValueError("lz77_cmds_batch failed")
     return out, boff, blen
@@ -822,18 +854,35 @@ class Engine:
 
     # -- generating LZ77 command lists on the GPU (include/divans_b200.h, divans_b200_lz77_cmds_batch_device)
     def lz77_cmds_batch_device(self, n, d_in, d_in_off, d_in_len, max_in_len, window, pred_mode, mixing_value, d_blobs, d_blob_off,
-                               d_blob_cap, d_blob_len, d_status, stream=None):
+                               d_blob_cap, d_blob_len, d_status, stream=None, parse=None):
         """lz77_cmds_batch on the GPU, with raw device pointers (ints): the blob of stream i goes to d_blobs[d_blob_off[i] ..
         +d_blob_cap[i]) (4-byte aligned; lz77_blob_cap always suffices).  Status 0: d_blob_len[i] bytes equal to lz77_cmds_batch's
         blob; 2: the region is too small and d_blob_len[i] is the size needed; 3: refused (misaligned region, in_len > max_in_len
-        or >= 2**31).  Asynchronous on ``stream``; regions are not cleared first."""
-        rc = self._L.divans_b200_lz77_cmds_batch_device(self._h, n, d_in, d_in_off, d_in_len, int(max_in_len), int(window), int(pred_mode),
-                                                        int(mixing_value), d_blobs, d_blob_off, d_blob_cap, d_blob_len, d_status, stream)
+        or >= 2**31).  Asynchronous on ``stream``; regions are not cleared first.  ``parse`` (min_match, lazy) as for
+        lz77_cmds_batch (divans_b200_lz77_cmds_batch_device_parse); None is (4, 0)."""
+        args = (self._h, n, d_in, d_in_off, d_in_len, int(max_in_len), int(window), int(pred_mode), int(mixing_value), d_blobs, d_blob_off,
+                d_blob_cap, d_blob_len, d_status)
+        if parse is None:
+            rc = self._L.divans_b200_lz77_cmds_batch_device(*args, stream)
+        else:
+            rc = self._L.divans_b200_lz77_cmds_batch_device_parse(*args, ctypes.byref(_parse(parse)), stream)
         if rc != DIVANS_SUCCESS:
             raise DivansError("lz77_cmds_batch_device: " + self._err())
 
+    def encode_cmds_choose_batch_device(self, n, k, d_blobs, d_blob_off, d_blob_len, max_blob_len, max_raw_len, d_out, d_out_off, d_out_cap,
+                                        d_out_len, d_status, d_chosen, d_cost=None, opts=None, stream=None):
+        """divans_b200_encode_cmds_choose_batch_device with raw device pointers (ints): k command lists per stream, list c of
+        stream i at d_blob_off[c * n + i] / d_blob_len[c * n + i]; each stream is encoded from the list that costs least under its
+        own records (d_chosen u32 [n], d_cost u64 [n * k] or None), exactly as encode_cmds_batch_device encodes that list.
+        d_out None: the choice only.  Asynchronous on ``stream``."""
+        rc = self._L.divans_b200_encode_cmds_choose_batch_device(self._h, n, int(k), d_blobs, d_blob_off, d_blob_len, int(max_blob_len),
+                                                                 int(max_raw_len), d_out, d_out_off, d_out_cap, d_out_len, d_status,
+                                                                 ctypes.byref(opts or encode_options()), d_chosen, d_cost, stream)
+        if rc != DIVANS_SUCCESS:
+            raise DivansError("encode_cmds_choose_batch_device: " + self._err())
+
     def compress_device(self, d_in, in_off, in_len, window=16, pred_mode=2, mixing_value=4, opts=None, candidates=None, stream=None,
-                        sub_batch=None):
+                        sub_batch=None, parses=None):
         """Compress raw buffers held in HBM with copy commands, without leaving the GPU: ``d_in`` is a CUDA uint8 tensor, buffer
         i at in_off[i] .. +in_len[i] (host arrays).  lz77_cmds_batch_device (``window``, ``pred_mode``, ``mixing_value`` as for
         lz77_cmds_batch) into regions of lz77_blob_cap, one synchronisation to read the blob lengths, then
@@ -844,11 +893,17 @@ class Engine:
         of a launch are one allocation, so the lists are encoded in as many sub-batches as memory needs: at most ``sub_batch``
         streams each (default all), halved while the encoder cannot allocate them.  Returns (d_new, new_off, new_len, status):
         status[i] is the generator's status where that failed (the list then reaches the encoder with length 0), else the
-        encoder's."""
+        encoder's.
+        With ``parses`` (a list of 1..16 (min_match, lazy) pairs, e.g. DEFAULT_LZ77_PARSES) the generator makes one list per
+        parse and stream, and encode_cmds_choose_batch_device encodes each stream from the list that codes cheapest under its own
+        record; with ``candidates`` too, the literal model is then chosen on that list (encode_cmds_auto_batch_device).  The call
+        then also returns chosen_parse [n] (an index into ``parses``) and parse_cost [n, k] last."""
         import torch
         n = len(in_off)
         in_off, in_len = np.ascontiguousarray(in_off, np.uint64).reshape(n), np.ascontiguousarray(in_len, np.uint64).reshape(n)
         o = opts if opts is not None else encode_options(window_size=0)
+        if parses is not None:
+            return self._compress_parses(d_in, in_off, in_len, window, pred_mode, mixing_value, o, candidates, stream, sub_batch, list(parses))
         auto = candidates is not None
         nc = len(candidates) if auto else 0
         dev = d_in.device
@@ -913,6 +968,94 @@ class Engine:
             cost = r[2 * n:(2 + nc) * n].view(np.uint64).reshape(n, nc).copy()
             return d_new, new_off, new_len, status, chosen, cost
         return d_new, new_off, new_len, status
+
+    def _compress_parses(self, d_in, in_off, in_len, window, pred_mode, mixing_value, o, candidates, stream, sub_batch, parses):
+        """compress_device with ``parses``: k lists per stream, candidate-major (list c of stream i is list v = c * n + i), in
+        regions of lz77_blob_cap each; one synchronisation reads their lengths; then each sub-batch chooses and encodes."""
+        import torch
+        n, k = len(in_off), len(parses)
+        if not 1 <= k <= 16:
+            raise ValueError("compress_device: 1..16 parses are required")
+        auto = candidates is not None
+        nc = len(candidates) if auto else 0
+        dev = d_in.device
+        if n == 0:
+            empty = torch.zeros(0, dtype=torch.uint8, device=dev), np.zeros(0, np.uint64), np.zeros(0, np.uint64), np.zeros(0, np.int32)
+            return empty + ((np.zeros(0, np.uint32), np.zeros((0, nc), np.uint64)) if auto else ()) + \
+                (np.zeros(0, np.uint32), np.zeros((0, k), np.uint64))
+        caller = stream if stream is not None else torch.cuda.current_stream(dev)
+        s = torch.cuda.Stream(dev)
+        s.wait_stream(caller)
+        u64 = lambda a: torch.from_numpy(np.ascontiguousarray(a, np.uint64).view(np.int64)).to(dev, non_blocking=False)
+        max_in = int(in_len.max())
+        bcap = np.tile(lz77_blob_cap(in_len), k)
+        blob_off, blob_total = _regions(bcap)
+        with torch.cuda.stream(s):
+            d_meta = u64(np.concatenate([in_off, in_len, blob_off, bcap]))
+            d_in_off, d_in_len, d_boff, d_bcap = d_meta[:n], d_meta[n:2 * n], d_meta[2 * n:2 * n + k * n], d_meta[2 * n + k * n:]
+            d_blobs = torch.empty(blob_total, dtype=torch.uint8, device=dev)
+            d_gen = torch.zeros(2 * k * n, dtype=torch.int64, device=dev)   # blob_len [k * n] | status (int32 pairs)
+            for c, ps in enumerate(parses):
+                v = c * n
+                self.lz77_cmds_batch_device(n, d_in.data_ptr(), d_in_off.data_ptr(), d_in_len.data_ptr(), max_in, window, pred_mode, mixing_value,
+                                            d_blobs.data_ptr(), d_boff[v:].data_ptr(), d_bcap[v:].data_ptr(), d_gen[v:].data_ptr(),
+                                            d_gen[k * n:].data_ptr() + 4 * v, s.cuda_stream, parse=ps)
+            g = d_gen.cpu().numpy()   # (the synchronisation that reads the blob lengths)
+        gen_st = g[k * n:].view(np.int32)[:k * n].reshape(k, n)
+        blob_len = np.where(gen_st == 0, g[:k * n].view(np.uint64).reshape(k, n), np.uint64(0))
+        gen_st = np.where((gen_st != 0).any(axis=0), gen_st.max(axis=0), 0).astype(np.int32)   # (a refusal refuses every parse)
+        new_cap = _encoded_cap(blob_len.max(axis=0))
+        new_off, new_total = _regions(new_cap)
+        max_blob = int(blob_len.max())
+        boff2 = blob_off.reshape(k, n)
+        with torch.cuda.stream(s):
+            d_enc = u64(np.concatenate([new_off, new_cap]))
+            d_new = torch.empty(new_total, dtype=torch.uint8, device=dev)
+            # new_len | status | parse cost [n * k] | chosen parse (| candidates: cost [n * C] | chosen)
+            d_res = torch.zeros((2 + k + 1 + (nc + 1 if auto else 0)) * n, dtype=torch.int64, device=dev)
+            d_pcost, d_pch = d_res[2 * n:(2 + k) * n], d_res[(2 + k) * n:(3 + k) * n]
+            d_cost, d_ch = d_res[(3 + k) * n:(3 + k + nc) * n], d_res[(3 + k + nc) * n:]
+            m = n if sub_batch is None else max(1, int(sub_batch))
+            i0 = 0
+            self.last_compress_sub_batches = 0
+            while i0 < n:
+                kk = min(m, n - i0)
+                at = lambda t, esz=8: t.data_ptr() + i0 * esz
+                # the sub-batch's lists, candidate-major
+                d_sub = u64(np.concatenate([boff2[:, i0:i0 + kk].reshape(-1), blob_len[:, i0:i0 + kk].reshape(-1)]))
+                try:
+                    if auto:
+                        self.encode_cmds_choose_batch_device(kk, k, d_blobs.data_ptr(), d_sub.data_ptr(), d_sub[k * kk:].data_ptr(), max_blob, max_in,
+                                                             None, None, None, None, None, at(d_pch, 4), at(d_pcost, 8 * k), o, s.cuda_stream)
+                        ch = d_pch.view(torch.int32)[i0:i0 + kk].long()
+                        d_pick = torch.cat([d_sub[:k * kk].view(k, kk).gather(0, ch[None])[0], d_sub[k * kk:].view(k, kk).gather(0, ch[None])[0]])
+                        self.encode_cmds_auto_batch_device(kk, d_blobs.data_ptr(), d_pick.data_ptr(), d_pick[kk:].data_ptr(), max_blob, max_in,
+                                                           d_new.data_ptr(), at(d_enc[:n]), at(d_enc[n:]), at(d_res), at(d_res[n:], 4), at(d_ch, 4),
+                                                           at(d_cost, 8 * nc), o, candidates, s.cuda_stream)
+                    else:
+                        self.encode_cmds_choose_batch_device(kk, k, d_blobs.data_ptr(), d_sub.data_ptr(), d_sub[k * kk:].data_ptr(), max_blob, max_in,
+                                                             d_new.data_ptr(), at(d_enc[:n]), at(d_enc[n:]), at(d_res), at(d_res[n:], 4),
+                                                             at(d_pch, 4), at(d_pcost, 8 * k), o, s.cuda_stream)
+                except DivansError as e:
+                    if kk == 1 or not ("cannot allocate" in str(e) or "out of memory" in str(e)):
+                        raise
+                    m = kk // 2   # the logs of kk streams (and the slots of their kk * k pairs) did not fit next to what the GPU holds
+                    continue
+                i0 += kk
+                self.last_compress_sub_batches += 1
+            r = d_res.cpu().numpy()
+        enc_st = r[n:2 * n].view(np.int32)[:n]
+        status = np.where(gen_st != 0, gen_st, enc_st).astype(np.int32)
+        new_len = r[:n].view(np.uint64).copy()
+        caller.wait_stream(s)
+        d_new.record_stream(caller)   # (allocated on the private stream, used on the caller's from here on)
+        chosen_parse = r[(2 + k) * n:(3 + k) * n].view(np.uint32)[:n].copy()
+        parse_cost = r[2 * n:(2 + k) * n].view(np.uint64).reshape(n, k).copy()
+        if auto:
+            chosen = r[(3 + k + nc) * n:].view(np.uint32)[:n].copy()
+            cost = r[(3 + k) * n:(3 + k + nc) * n].view(np.uint64).reshape(n, nc).copy()
+            return d_new, new_off, new_len, status, chosen, cost, chosen_parse, parse_cost
+        return d_new, new_off, new_len, status, chosen_parse, parse_cost
 
     # -- replaying command lists to raw bytes (include/divans_b200.h, divans_b200_replay_cmds_batch_*)
     def replay_cmds_batch_host(self, blobs, blob_off, blob_len, out, out_off, out_cap, window_size=0):

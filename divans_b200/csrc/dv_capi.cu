@@ -769,8 +769,10 @@ static bool ensure_cost_tab(divans_b200_ctx *ctx, cudaStream_t st) {
 //  * SEL_MIXMAP (divans_b200_encode_[cmds_]mixmap_*): mixing values under opts->literal_pred_mode, chosen per context;
 //    chosen [n], cost [n * (k + 1)], mixing [n * 8192], bins [n * k * 8192].
 //  * SEL_SPEEDS (divans_b200_encode_[cmds_]speeds_*): literal speeds; chosen [n * 3], cost [n * (k + 1)], halves [n * k * 2].
-// Outputs other than auto's chosen may be NULL.
-enum SelKind { SEL_NONE, SEL_AUTO, SEL_MIXMAP, SEL_SPEEDS };
+//  * SEL_LISTS (divans_b200_encode_cmds_choose_batch_device): one of k command lists per stream, each under its own records;
+//    the batch's in_off / in_len are the n * k lists, candidate-major; chosen [n] (required), cost [n * k].
+// Outputs other than auto's and lists' chosen may be NULL.
+enum SelKind { SEL_NONE, SEL_AUTO, SEL_MIXMAP, SEL_SPEEDS, SEL_LISTS };
 struct Selection {
     SelKind kind = SEL_NONE;
     uint32_t k = 0;
@@ -833,6 +835,38 @@ static DivansResult encode_auto_device_nolock(divans_b200_ctx *ctx, const EncBat
     ctx->launches += 1;
     CK(cudaGetLastError());
     return encode_device_internal(ctx, b, ctx->d_records, sel.chosen, keep);
+}
+
+// Command lists: the cost pass over the n * k lists themselves (pair v = c * n + i is list c of stream i, the batch's in_off[v] /
+// in_len[v]), each under its own records; the per-stream argmin into chosen; then, unless the batch has no output, the encode of
+// each stream's chosen list, whose offset and length choose_pick_kernel gathers.
+static DivansResult encode_lists_device_nolock(divans_b200_ctx *ctx, const EncBatch &b, const Selection &sel) {
+    const size_t n = b.n;
+    const uint64_t nv = (uint64_t)n * sel.k;
+    const size_t slots = encode_slots(ctx, nv);
+    if (ensure_arena(ctx, slots) != DIVANS_SUCCESS) return DIVANS_FAILURE;
+    if (!grow(ctx, &ctx->d_replay, &ctx->replay_cap, slots * (size_t)b.caps.replay)) return DIVANS_FAILURE;
+    // tally [nv] | pick_off [n] | pick_len [n] | v_status i32 [nv]
+    if (!grow(ctx, &ctx->d_auto, &ctx->auto_cap, nv + 2 * n + (nv + 1) / 2)) return DIVANS_FAILURE;
+    uint64_t *tally = ctx->d_auto, *pick_off = tally + nv, *pick_len = pick_off + n;
+    int32_t *v_status = reinterpret_cast<int32_t *>(pick_len + n);
+    if (ctx->busy_recorded) CK(cudaStreamWaitEvent(b.st, ctx->ev_busy, 0));
+    if (!ensure_cost_tab(ctx, b.st)) return DIVANS_FAILURE;
+    EncodeParams tp = cost_params(ctx, b, nv, b.in_off, b.in_len, v_status, tally);   // (no pm_index: each list keeps its records)
+    if (model_pass(ctx, b, EncodeWalk::TALLY, tp) != DIVANS_SUCCESS) return DIVANS_FAILURE;
+    launch_auto_select(tally, v_status, n, sel.k, sel.chosen, sel.cost, b.st);
+    ctx->launches += 1;
+    if (!b.out) {   // the choice only
+        CK(cudaEventRecord(ctx->ev_busy, b.st)); ctx->busy_recorded = true;
+        CK(cudaGetLastError());
+        return DIVANS_SUCCESS;
+    }
+    launch_choose_pick(b.in_off, b.in_len, n, sel.chosen, pick_off, pick_len, b.st);
+    ctx->launches += 1;
+    CK(cudaGetLastError());
+    EncBatch e = b;
+    e.in_off = pick_off; e.in_len = pick_len;
+    return encode_device_internal(ctx, e);
 }
 
 // Per-context mixing values.  Records [0, k) are R(p, v[c]), records [k, k + n) the streams' mixed records M_i.
@@ -994,6 +1028,9 @@ static bool check_selection(divans_b200_ctx *ctx, int raw_mode, const divans_b20
         break;
     case SEL_MIXMAP: if (!mixmap_cands(ctx, sel.mix_values, sel.k, o, sel.cands)) return false; break;
     case SEL_SPEEDS: if (!speed_values(ctx, sel.speed_values, sel.k, sel.speeds)) return false; break;
+    case SEL_LISTS:
+        if (sel.k < 1 || sel.k > 16) { ctx->err = "encode_cmds_choose: 1..16 command lists per stream are required"; return false; }
+        break;
     case SEL_NONE: break;
     }
     if (!raw_mode || sel.kind == SEL_AUTO || sel.kind == SEL_MIXMAP || (o->literal_pred_mode >= 0 && o->literal_pred_mode <= 3)) return true;
@@ -1009,6 +1046,7 @@ static DivansResult encode_nolock(divans_b200_ctx *ctx, const EncBatch &b, const
     case SEL_AUTO: return encode_auto_device_nolock(ctx, b, sel);
     case SEL_MIXMAP: return encode_mixmap_device_nolock(ctx, b, sel);
     case SEL_SPEEDS: return encode_speeds_device_nolock(ctx, b, sel);
+    case SEL_LISTS: return encode_lists_device_nolock(ctx, b, sel);
     case SEL_NONE: break;
     }
     return encode_device_internal(ctx, b);
@@ -1046,6 +1084,7 @@ static DivansResult encode_device_common(divans_b200_ctx *ctx, size_t n, int raw
     if (!check_selection(ctx, raw_mode, opts, sel)) return DIVANS_FAILURE;
     if (n == 0) return DIVANS_SUCCESS;
     if (sel.kind == SEL_AUTO && !sel.chosen) { ctx->err = raw_mode ? "encode_auto: d_chosen is required" : "encode_cmds_auto: d_chosen is required"; return DIVANS_FAILURE; }
+    if (sel.kind == SEL_LISTS && !sel.chosen) { ctx->err = "encode_cmds_choose: d_chosen is required"; return DIVANS_FAILURE; }
     if (sel.kind == SEL_MIXMAP && n > 0x7fffffffull) { ctx->err = "batch too large"; return DIVANS_FAILURE; }   // (one block per stream)
     const uint64_t nv = (uint64_t)n * (sel.kind == SEL_NONE ? 1 : sel.k);
     if (nv > 0xffffffffull || max_in_len > 0x7fff0000ull || max_raw_len > 0x7fff0000ull) { ctx->err = "batch too large"; return DIVANS_FAILURE; }
@@ -1116,6 +1155,17 @@ extern "C" DivansResult divans_b200_encode_cmds_auto_batch_device(divans_b200_ct
                                                                   uint32_t *d_chosen, uint64_t *d_cost, void *cuda_stream) {
     return encode_device_common(ctx, n, 0, d_blobs, d_blob_off, d_blob_len, max_blob_len, max_raw_len, d_out, d_out_off, d_out_cap,
                                 d_out_len, d_status, opts, cuda_stream, sel_auto(cands, n_cands, d_chosen, d_cost));
+}
+
+extern "C" DivansResult divans_b200_encode_cmds_choose_batch_device(divans_b200_ctx *ctx, size_t n, uint32_t k, const uint8_t *d_blobs,
+                                                                    const uint64_t *d_blob_off, const uint64_t *d_blob_len,
+                                                                    uint64_t max_blob_len, uint64_t max_raw_len, uint8_t *d_out,
+                                                                    const uint64_t *d_out_off, const uint64_t *d_out_cap, uint64_t *d_out_len,
+                                                                    int32_t *d_status, const divans_b200_encode_options *opts,
+                                                                    uint32_t *d_chosen, uint64_t *d_cost, void *cuda_stream) {
+    Selection sel; sel.kind = SEL_LISTS; sel.k = k; sel.chosen = d_chosen; sel.cost = d_cost;
+    return encode_device_common(ctx, n, 0, d_blobs, d_blob_off, d_blob_len, max_blob_len, max_raw_len, d_out, d_out_off, d_out_cap,
+                                d_out_len, d_status, opts, cuda_stream, sel);
 }
 
 // The host encode calls: marshal, split into sub-batches whose symbol logs (and selection scratch) fit in HBM, run, copy back.
@@ -1399,12 +1449,21 @@ extern "C" DivansResult divans_b200_replay_cmds_batch_host(divans_b200_ctx *ctx,
 // One launch (dv_lz77.cu) over n raw buffers in HBM: the blobs of divans_b200_lz77_cmds_batch.  Like the replay call it uses the
 // context's work counter and timing events only, and its own scratch: 2^15 + max_in_len int32 per warp, kept and grown on demand.
 // The warps are the fewest of n, the context's max_resident and what the scratch allocation holds.
-extern "C" DivansResult divans_b200_lz77_cmds_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_in, const uint64_t *d_in_off,
-                                                           const uint64_t *d_in_len, uint64_t max_in_len, int32_t window, int32_t pred_mode,
-                                                           int32_t mixing_value, uint8_t *d_blobs, const uint64_t *d_blob_off,
-                                                           const uint64_t *d_blob_cap, uint64_t *d_blob_len, int32_t *d_status,
-                                                           void *cuda_stream) try {
+// The parse (include/divans_b200.h) selects the kernel's lazy steps and its minimum copy; {4, 0} is the plain call.
+extern "C" DivansResult divans_b200_lz77_cmds_batch_device_parse(divans_b200_ctx *ctx, size_t n, const uint8_t *d_in, const uint64_t *d_in_off,
+                                                                 const uint64_t *d_in_len, uint64_t max_in_len, int32_t window,
+                                                                 int32_t pred_mode, int32_t mixing_value, uint8_t *d_blobs,
+                                                                 const uint64_t *d_blob_off, const uint64_t *d_blob_cap, uint64_t *d_blob_len,
+                                                                 int32_t *d_status, const divans_b200_lz77_parse *parse, void *cuda_stream) try {
     if (!ctx) return DIVANS_FAILURE;
+    if (!parse) { ctx->err = "lz77_cmds_batch_device: a parse is required"; return DIVANS_FAILURE; }
+    if (parse->min_match < 4 || parse->min_match > 32 || parse->lazy < 0 || parse->lazy > 2) {
+        char buf[200];
+        snprintf(buf, sizeof buf, "lz77_cmds_batch_device: parse (min_match %d, lazy %d) is outside min_match 4..32, lazy 0..2",
+                 (int)parse->min_match, (int)parse->lazy);
+        ctx->err = buf;
+        return DIVANS_FAILURE;
+    }
     if (window < 10 || window > 24) { ctx->err = "lz77_cmds_batch_device: window must be 10..24"; return DIVANS_FAILURE; }
     if (n > 0xffffffffull) { ctx->err = "lz77_cmds_batch_device: too many streams"; return DIVANS_FAILURE; }
     if (n == 0) return DIVANS_SUCCESS;
@@ -1445,7 +1504,7 @@ extern "C" DivansResult divans_b200_lz77_cmds_batch_device(divans_b200_ctx *ctx,
     Lz77Params lp;
     lp.in = d_in; lp.in_off = d_in_off; lp.in_len = d_in_len; lp.max_in_len = max_in_len;
     lp.blobs = d_blobs; lp.blob_off = d_blob_off; lp.blob_cap = d_blob_cap; lp.blob_len = d_blob_len; lp.status = d_status;
-    lp.pm = ctx->d_records; lp.n_streams = (uint32_t)n; lp.window = window;
+    lp.pm = ctx->d_records; lp.n_streams = (uint32_t)n; lp.window = window; lp.min_match = parse->min_match; lp.lazy = parse->lazy;
     lp.work_counter = ctx->d_counter; lp.scratch = ctx->d_lz_scratch; lp.stride = stride; lp.n_warps = (uint32_t)warps;
     CK(cudaMemsetAsync(ctx->d_counter, 0, 4, st));
     CK(cudaEventRecord(ctx->ev0, st));
@@ -1460,6 +1519,15 @@ extern "C" DivansResult divans_b200_lz77_cmds_batch_device(divans_b200_ctx *ctx,
 } catch (...) {
     if (ctx) ctx->err = "divans_b200: out of host memory";
     return DIVANS_FAILURE;
+}
+extern "C" DivansResult divans_b200_lz77_cmds_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_in, const uint64_t *d_in_off,
+                                                           const uint64_t *d_in_len, uint64_t max_in_len, int32_t window, int32_t pred_mode,
+                                                           int32_t mixing_value, uint8_t *d_blobs, const uint64_t *d_blob_off,
+                                                           const uint64_t *d_blob_cap, uint64_t *d_blob_len, int32_t *d_status,
+                                                           void *cuda_stream) {
+    const divans_b200_lz77_parse greedy = DIVANS_B200_LZ77_PARSE_DEFAULT;
+    return divans_b200_lz77_cmds_batch_device_parse(ctx, n, d_in, d_in_off, d_in_len, max_in_len, window, pred_mode, mixing_value, d_blobs,
+                                                    d_blob_off, d_blob_cap, d_blob_len, d_status, &greedy, cuda_stream);
 }
 
 // =================================================================================================================

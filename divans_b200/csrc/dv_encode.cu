@@ -679,6 +679,19 @@ void launch_auto_select(const uint64_t *tally, const int32_t *v_status, uint64_t
                         cudaStream_t st) {
     auto_select_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(tally, v_status, n, n_cands, chosen, cost);
 }
+// one of k command lists per stream (divans_b200_encode_cmds_choose_batch_device): stream i's chosen list, from the
+// candidate-major descriptors (list c of stream i at v = c * n + i)
+__global__ void choose_pick_kernel(const uint64_t *v_off, const uint64_t *v_len, uint64_t n, const uint32_t *chosen, uint64_t *off,
+                                   uint64_t *len) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint64_t v = (uint64_t)chosen[i] * n + i;
+    off[i] = v_off[v]; len[i] = v_len[v];
+}
+void launch_choose_pick(const uint64_t *v_off, const uint64_t *v_len, uint64_t n, const uint32_t *chosen, uint64_t *off, uint64_t *len,
+                        cudaStream_t st) {
+    choose_pick_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(v_off, v_len, n, chosen, off, len);
+}
 // M[f] = floor((2^64 - 1) / f), f = 1..32767 (entry 0 unused)
 __global__ void rcp15_init_kernel(uint64_t *tab) {
     const uint32_t f = blockIdx.x * blockDim.x + threadIdx.x;

@@ -183,8 +183,8 @@ extern "C" DivansResult divans_b200_ir_to_cmds(const char *ir_text, size_t ir_le
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// Command generator for benchmarks and tools (ours, not a reference component): a deterministic greedy hash-chain LZ77
-// (minimum match 4, window 2^window - 16, no dictionary words) that turns raw bytes into a DVCL command list -- one
+// Command generator for benchmarks and tools (ours, not a reference component): a deterministic hash-chain LZ77 (by default
+// greedy with minimum match 4; window 2^window - 16, no dictionary words) that turns raw bytes into a DVCL command list -- one
 // PredictionMode command (64-entry identity context map, one mixing value, like raw_to_cmd/mod.rs:116-143), then Literal /
 // Copy commands.  SURVEY 8d calls the resulting population "Z": copy-dominated streams like the reference's default
 // (brotli-driven) compressor produces.  The command SELECTION of the brotli crate stays out of scope.
@@ -193,7 +193,10 @@ extern "C" DivansResult divans_b200_ir_to_cmds(const char *ir_text, size_t ir_le
 #include <thread>
 
 namespace {
-size_t lz77_blob(const uint8_t *in, size_t n, int window, int pred_mode, int mixing_value, std::vector<uint8_t> &blob) {
+// The parse (include/divans_b200.h, "the LZ77 parse"): best(j) needs every position below j inserted and j not yet, so the
+// chain is filled up to j on demand; the (at most three) positions the parse looks at around i are kept in a small cache.
+size_t lz77_blob(const uint8_t *in, size_t n, int window, int pred_mode, int mixing_value, const divans_b200_lz77_parse &parse,
+                 std::vector<uint8_t> &blob) {
     std::vector<Cmd> cmds;
     cmds.push_back({7, 0, 0, 0, 0});
     const int HB = 15;
@@ -203,11 +206,15 @@ size_t lz77_blob(const uint8_t *in, size_t n, int window, int pred_mode, int mix
         uint32_t v; memcpy(&v, in + i, 4);
         return (v * 2654435761u) >> (32 - HB);
     };
-    size_t i = 0, lit_start = 0;
+    size_t ins = 0;   // positions below `ins` are in the chain
     auto insert = [&](size_t at) { if (at + 4 <= n) { const uint32_t hh = h4(at); prev[at] = head[hh]; head[hh] = (int32_t)at; } };
-    while (i < n) {
-        size_t best_len = 0, best_dist = 0;
+    size_t c_pos[4] = {SIZE_MAX, SIZE_MAX, SIZE_MAX, SIZE_MAX}, c_len[4] = {0}, c_dist[4] = {0};
+    auto best = [&](size_t i, size_t &best_dist) -> size_t {
+        if (c_pos[i & 3] == i) { best_dist = c_dist[i & 3]; return c_len[i & 3]; }
+        size_t best_len = 0;
+        best_dist = 0;
         if (i + 4 <= n) {
+            while (ins < i) insert(ins++);
             int chain = 16;
             for (int32_t c = head[h4(i)]; c >= 0 && chain-- > 0 && i - (size_t)c <= maxdist; c = prev[c]) {
                 size_t l = 0, lim = std::min<size_t>(n - i, 65535);
@@ -215,12 +222,23 @@ size_t lz77_blob(const uint8_t *in, size_t n, int window, int pred_mode, int mix
                 if (l > best_len) { best_len = l; best_dist = i - (size_t)c; }
             }
         }
-        if (best_len >= 4) {
+        c_pos[i & 3] = i; c_len[i & 3] = best_len; c_dist[i & 3] = best_dist;
+        return best_len;
+    };
+    const size_t min_match = (size_t)parse.min_match;
+    size_t i = 0, lit_start = 0, d1;
+    while (i < n) {
+        size_t best_dist;
+        const size_t L = best(i, best_dist);
+        bool take = L >= min_match;
+        if (take && parse.lazy >= 1 && L < 32)
+            take = !(best(i + 1, d1) > L || (parse.lazy == 2 && best(i + 2, d1) > L + 1));
+        if (take) {
             if (i > lit_start) cmds.push_back({3, (uint32_t)lit_start, (uint32_t)(i - lit_start), 0, 0});
-            cmds.push_back({1, (uint32_t)best_dist, (uint32_t)best_len, 0, 0});
-            for (size_t k = 0; k < best_len; k++) insert(i++);
+            cmds.push_back({1, (uint32_t)best_dist, (uint32_t)L, 0, 0});
+            i += L;
             lit_start = i;
-        } else insert(i++);
+        } else i++;
     }
     if (n > lit_start) cmds.push_back({3, (uint32_t)lit_start, (uint32_t)(n - lit_start), 0, 0});
     constexpr size_t PM_BYTES = 32 + 16384 + 1024 + 8192;
@@ -241,15 +259,18 @@ size_t lz77_blob(const uint8_t *in, size_t n, int window, int pred_mode, int mix
 
 // n raw buffers -> n DVCL blobs written back to back at blob_off[i] (16-byte aligned) of `out`; blob_len[i] receives the sizes.
 // With out == NULL or out_cap too small the call returns DIVANS_NEEDS_MORE_OUTPUT and *total receives the size needed.
-extern "C" DivansResult divans_b200_lz77_cmds_batch(size_t n, const uint8_t *in, const uint64_t *in_off, const uint64_t *in_len, int32_t window,
-                                                    int32_t pred_mode, int32_t mixing_value, uint8_t *out, size_t out_cap, uint64_t *blob_off,
-                                                    uint64_t *blob_len, size_t *total, int32_t n_threads) {
+// `parse` NULL or outside min_match 4..32, lazy 0..2: DIVANS_FAILURE, nothing written.
+extern "C" DivansResult divans_b200_lz77_cmds_batch_parse(size_t n, const uint8_t *in, const uint64_t *in_off, const uint64_t *in_len, int32_t window,
+                                                          int32_t pred_mode, int32_t mixing_value, uint8_t *out, size_t out_cap, uint64_t *blob_off,
+                                                          uint64_t *blob_len, size_t *total, int32_t n_threads, const divans_b200_lz77_parse *parse) {
     if (!in || !in_off || !in_len || !blob_off || !blob_len || !total || window < 10 || window > 24) return DIVANS_FAILURE;
+    if (!parse || parse->min_match < 4 || parse->min_match > 32 || parse->lazy < 0 || parse->lazy > 2) return DIVANS_FAILURE;
+    const divans_b200_lz77_parse ps = *parse;
     std::vector<std::vector<uint8_t>> blobs(n);
     if (n_threads < 1) n_threads = 1;
     std::vector<std::thread> th;
     for (int t = 0; t < n_threads; t++)
-        th.emplace_back([&, t]() { for (size_t i = (size_t)t; i < n; i += (size_t)n_threads) lz77_blob(in + in_off[i], (size_t)in_len[i], window, pred_mode, mixing_value, blobs[i]); });
+        th.emplace_back([&, t]() { for (size_t i = (size_t)t; i < n; i += (size_t)n_threads) lz77_blob(in + in_off[i], (size_t)in_len[i], window, pred_mode, mixing_value, ps, blobs[i]); });
     for (auto &x : th) x.join();
     size_t pos = 0;
     for (size_t i = 0; i < n; i++) { blob_off[i] = pos; blob_len[i] = blobs[i].size(); pos += (blobs[i].size() + 15) & ~(size_t)15; }
@@ -257,4 +278,12 @@ extern "C" DivansResult divans_b200_lz77_cmds_batch(size_t n, const uint8_t *in,
     if (!out || out_cap < pos) return DIVANS_NEEDS_MORE_OUTPUT;
     for (size_t i = 0; i < n; i++) memcpy(out + blob_off[i], blobs[i].data(), blobs[i].size());
     return DIVANS_SUCCESS;
+}
+
+extern "C" DivansResult divans_b200_lz77_cmds_batch(size_t n, const uint8_t *in, const uint64_t *in_off, const uint64_t *in_len, int32_t window,
+                                                    int32_t pred_mode, int32_t mixing_value, uint8_t *out, size_t out_cap, uint64_t *blob_off,
+                                                    uint64_t *blob_len, size_t *total, int32_t n_threads) {
+    const divans_b200_lz77_parse greedy = DIVANS_B200_LZ77_PARSE_DEFAULT;
+    return divans_b200_lz77_cmds_batch_parse(n, in, in_off, in_len, window, pred_mode, mixing_value, out, out_cap, blob_off, blob_len, total,
+                                             n_threads, &greedy);
 }

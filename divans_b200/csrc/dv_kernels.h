@@ -36,6 +36,9 @@ void launch_auto_fanout(const uint64_t *in_off, const uint64_t *in_len, uint64_t
                         uint32_t *v_pm, cudaStream_t st);
 void launch_auto_select(const uint64_t *tally, const int32_t *v_status, uint64_t n, uint32_t n_cands, uint32_t *chosen, uint64_t *cost,
                         cudaStream_t st);
+// one of k command lists per stream: off[i] / len[i] = the descriptors of list chosen[i] of stream i (candidate-major v_off / v_len)
+void launch_choose_pick(const uint64_t *v_off, const uint64_t *v_len, uint64_t n, const uint32_t *chosen, uint64_t *off, uint64_t *len,
+                        cudaStream_t st);
 // per-context mixing values: the kernel that builds each stream's mixed record from the per-entry winners, and the choice
 // between the best uniform record and the mixed one (dv_encode.cu)
 void launch_mixmap_map(const uint64_t *best, uint64_t n, const MixValues &vals, uint8_t *records, uint32_t *mix_idx, cudaStream_t st);

@@ -1,10 +1,12 @@
-// dv_lz77.cu -- sm_90a kernel of divans_b200_lz77_cmds_batch_device: the library's greedy hash-chain LZ77 (dv_ir.cpp,
-// lz77_blob) run next to raw buffers in HBM.  Every blob is byte for byte the one the host generator writes for the same input
-// and arguments.  The host's rules:
+// dv_lz77.cu -- sm_90a kernel of divans_b200_lz77_cmds_batch_device[_parse]: the library's hash-chain LZ77 (dv_ir.cpp,
+// lz77_blob) run next to raw buffers in HBM.  Every blob is byte for byte the one the host generator writes for the same input,
+// arguments and parse.  The host's rules:
 //   h4(i) = (le32(in + i) * 2654435761) >> 17, for positions with i + 4 <= n only; every such position is inserted, in order,
 //   copies included.  The candidates of position i are the (at most 16) most recent earlier positions of the same hash, walked
 //   newest first and up to the first farther than 2^window - 16.  The longest match of at most min(n - i, 65535) bytes wins, a
-//   tie going to the newer candidate; a match of 4 or more bytes is a copy, anything shorter leaves the byte a literal.
+//   tie going to the newer candidate.  The parse (include/divans_b200.h): a match of min_match or more bytes is a copy unless
+//   a lazy lookahead defers it (L < 32 and len(i + 1) > L, or with lazy 2 len(i + 2) > L + 1); anything else leaves the byte
+//   a literal.  The default parse is min_match 4, lazy 0.
 //
 // One warp per stream; persistent warps pull stream indices from the work counter, so any n runs in one launch.  Each warp owns
 // a head table (2^15 entries) and prev[max_in_len] in global memory.  Per stream:
@@ -13,8 +15,11 @@
 //     __match_any_sync; a lane's prev is the nearest lower lane of its group, or head[h]; the highest lane of a group writes
 //     head[h].  The head table is reset for every stream: a stale entry would be a candidate from another stream.
 //  2. Parse, 32 positions per window.  Lane t walks the chain of position p + t and compares every candidate up to LZ_CAP
-//     bytes, word by word.  The warp then replays the greedy parse over the window from the ballot of lanes with a match of
-//     4 or more: literal bytes up to the next such lane, its copy, and on from the copy's end while it stays in the window.  A
+//     bytes, word by word.  The warp then replays the parse over the window from the ballot of lanes with a match of
+//     min_match or more: literal bytes up to the next such lane, its copy, and on from the copy's end while it stays in the
+//     window.  A lazy parse reads the lookahead lanes' capped lengths (exact for the L < 32 it compares, as 32 < LZ_CAP); when a
+//     lookahead lane lies past the window (and the stream goes on), the window ends before that position and the next one
+//     starts there, so every deferral is decided with both lengths in hand.  A
 //     copy whose capped length reached LZ_CAP (and could be longer) is measured exactly, by the whole warp, for each candidate
 //     that reached the cap, in chain order: only those can be the longest.  So per window a lane spends at most 16 capped
 //     compares, and exact lengths are measured only where the parse lands.
@@ -32,7 +37,7 @@ constexpr unsigned LZ_FULL = 0xffffffffu;
 constexpr int LZ_CHAIN = 16;           // candidates per position
 constexpr int32_t LZ_CAP = 64;         // bytes of the capped compare
 constexpr int32_t LZ_MAX_COPY = 65535;
-constexpr uint32_t LZ_MIN_COPY = 4;
+constexpr int32_t LZ_LAZY_BELOW = 32;   // a lazy parse looks ahead only from matches shorter than this
 
 // The four bytes at p (p < end) as a little-endian word, from the aligned words that hold them.  The second word is read only
 // when it starts below `end`: no word without a byte of the stream is read.
@@ -95,6 +100,8 @@ __device__ __noinline__ int2 lz_extend(const uint8_t *in, const uint8_t *end, co
 }
 
 // (launch bounds: 16 blocks, 32 warps per SM, the most a context's max_resident asks for; without the minimum ptxas spilled)
+// LAZY: the parse's lazy steps (0..2); min_match is p.min_match
+template <int LAZY>
 __global__ void __launch_bounds__(LZ_BLOCK_THREADS, 16) lz77_cmds_kernel(Lz77Params p) {
     const int lane = threadIdx.x & 31;
     const uint32_t warp = blockIdx.x * LZ_WARPS + (threadIdx.x >> 5);
@@ -157,7 +164,7 @@ __global__ void __launch_bounds__(LZ_BLOCK_THREADS, 16) lz77_cmds_kernel(Lz77Par
                 lim = min(n - q, LZ_MAX_COPY);
                 best = lz_capped(in, end, prev, q, lim, maxdist, dist, hits);
             }
-            const uint32_t copies = __ballot_sync(LZ_FULL, best >= (int32_t)LZ_MIN_COPY);
+            const uint32_t copies = __ballot_sync(LZ_FULL, best >= p.min_match);
             const int32_t wend = pos + span;
             int32_t at = pos;   // the parse position in this window
             while (at < wend) {
@@ -169,6 +176,13 @@ __global__ void __launch_bounds__(LZ_BLOCK_THREADS, 16) lz77_cmds_kernel(Lz77Par
                 int32_t len = __shfl_sync(LZ_FULL, best, t), d = __shfl_sync(LZ_FULL, dist, t);
                 const int32_t lt = __shfl_sync(LZ_FULL, lim, t);
                 const uint32_t ht = __shfl_sync(LZ_FULL, hits, t);
+                if (LAZY > 0 && len < LZ_LAZY_BELOW) {
+                    // lanes past the stream's end hold 0, the length there; a lookahead past a window that the stream goes on
+                    // after is decided by the next window, which starts at cq
+                    if (t + LAZY >= span && wend < n) { at = cq; break; }
+                    const int32_t l1 = __shfl_sync(LZ_FULL, best, (t + 1) & 31), l2 = __shfl_sync(LZ_FULL, best, (t + 2) & 31);
+                    if ((t + 1 < 32 && l1 > len) || (LAZY == 2 && t + 2 < 32 && l2 > len + 1)) { at = cq + 1; continue; }
+                }
                 if (len == LZ_CAP && lt > LZ_CAP) {
                     const int2 e = lz_extend(in, end, prev, cq, lt, ht);
                     len = e.x; d = e.y;
@@ -203,7 +217,9 @@ __global__ void __launch_bounds__(LZ_BLOCK_THREADS, 16) lz77_cmds_kernel(Lz77Par
 
 void launch_lz77_cmds(const Lz77Params &p, cudaStream_t st) {
     const unsigned blocks = (p.n_warps + LZ_WARPS - 1) / LZ_WARPS;
-    lz77_cmds_kernel<<<blocks, LZ_BLOCK_THREADS, 0, st>>>(p);
+    if (p.lazy == 2) lz77_cmds_kernel<2><<<blocks, LZ_BLOCK_THREADS, 0, st>>>(p);
+    else if (p.lazy == 1) lz77_cmds_kernel<1><<<blocks, LZ_BLOCK_THREADS, 0, st>>>(p);
+    else lz77_cmds_kernel<0><<<blocks, LZ_BLOCK_THREADS, 0, st>>>(p);
 }
 
 }  // namespace dv

@@ -16,8 +16,9 @@ struct Lz77Params {
     const uint8_t *in; const uint64_t *in_off, *in_len; uint64_t max_in_len;
     uint8_t *blobs; const uint64_t *blob_off, *blob_cap; uint64_t *blob_len; int32_t *status;
     const uint8_t *pm; uint32_t n_streams; int32_t window;
+    int32_t min_match, lazy;   // the parse (include/divans_b200.h): min_match 4..32, lazy 0..2
     uint32_t *work_counter; int32_t *scratch; uint64_t stride; uint32_t n_warps;
 };
-void launch_lz77_cmds(const Lz77Params &p, cudaStream_t st);   // one launch, n_warps persistent warps
+void launch_lz77_cmds(const Lz77Params &p, cudaStream_t st);   // one launch, n_warps persistent warps (a kernel per lazy 0..2)
 
 }  // namespace dv

@@ -564,6 +564,61 @@ DivansResult divans_b200_lz77_cmds_batch_device(divans_b200_ctx *ctx, size_t n, 
                                                 const uint64_t *d_in_len, uint64_t max_in_len, int32_t window, int32_t pred_mode,
                                                 int32_t mixing_value, uint8_t *d_blobs, const uint64_t *d_blob_off,
                                                 const uint64_t *d_blob_cap, uint64_t *d_blob_len, int32_t *d_status, void *cuda_stream);
+/* ---- the LZ77 parse ----
+ * How the generator above walks the positions of a stream of n bytes.  best(i) = (len(i), dist(i)) is the longest match at
+ * position i exactly as above: the (at most 16) most recent earlier positions of the same hash, up to the first farther than
+ * 2^window - 16, each compared up to min(n - i, 65535) bytes, ties to the most recent candidate, and len(i) = 0 where i + 4 > n
+ * or i >= n.  Every position is inserted into the chain in order, copies included, so best(i) is a function of i alone, not of
+ * the parse.  The parse starts at i = 0 with an empty literal run, and while i < n, with L = len(i):
+ *  - it defers when lazy >= 1 and L < 32 and either len(i + 1) > L, or lazy == 2 and len(i + 2) > L + 1;
+ *  - if L >= min_match and it does not defer, it emits the pending literal run (if any), then Copy(dist(i), L), and i += L;
+ *  - otherwise byte i joins the literal run and i += 1.
+ * The last literal run is emitted at the end.  Domain: min_match 4..32 and lazy 0..2; a parse outside it fails the call
+ * (DIVANS_FAILURE) with nothing written.  {4, 0} is the parse of the two calls above, byte for byte.  Every copy is at least
+ * 4 bytes long, so the region bound of divans_b200_lz77_cmds_batch_device (divans_b200.lz77_blob_cap) holds for every parse.
+ * (The L < 32 guard keeps each comparison of lengths below the GPU generator's 64-byte capped compare, which is exact there.) */
+typedef struct {
+    int32_t min_match;   /* 4..32: the shortest match emitted as a copy */
+    int32_t lazy;        /* 0..2: positions looked ahead before a match shorter than 32 bytes is taken */
+} divans_b200_lz77_parse;
+#define DIVANS_B200_LZ77_PARSE_DEFAULT { 4, 0 }
+/* divans_b200_lz77_cmds_batch under `parse` (NULL or out of the domain: DIVANS_FAILURE, nothing written). */
+DivansResult divans_b200_lz77_cmds_batch_parse(size_t n, const uint8_t *in, const uint64_t *in_off, const uint64_t *in_len, int32_t window,
+                                               int32_t pred_mode, int32_t mixing_value, uint8_t *out, size_t out_cap, uint64_t *blob_off,
+                                               uint64_t *blob_len, size_t *total, int32_t n_threads, const divans_b200_lz77_parse *parse);
+/* divans_b200_lz77_cmds_batch_device under `parse`: every blob byte for byte divans_b200_lz77_cmds_batch_parse's, with every
+ * other rule of that call (statuses, regions, refusals, scratch).  A parse that is NULL or outside the domain fails the call
+ * (DIVANS_FAILURE, divans_b200_last_error says why) before any work.  The GPU walks 32 positions per step; a deferral whose
+ * lookahead (i + 1 or i + 2) falls past those 32 is not decided there: the step ends before position i, and the next starts
+ * at it.  So a lazy parse may take a few more steps than the greedy one. */
+DivansResult divans_b200_lz77_cmds_batch_device_parse(divans_b200_ctx *ctx, size_t n, const uint8_t *d_in, const uint64_t *d_in_off,
+                                                      const uint64_t *d_in_len, uint64_t max_in_len, int32_t window, int32_t pred_mode,
+                                                      int32_t mixing_value, uint8_t *d_blobs, const uint64_t *d_blob_off,
+                                                      const uint64_t *d_blob_cap, uint64_t *d_blob_len, int32_t *d_status,
+                                                      const divans_b200_lz77_parse *parse, void *cuda_stream);
+/* ---- choosing one of k command lists per stream by coding cost ----
+ * n streams, each with k (1..16) candidate DVCL command lists already in HBM, candidate-major: list c of stream i is
+ * d_blobs[d_blob_off[c * n + i] .. +d_blob_len[c * n + i]) (4-byte aligned).  The lists of a stream should replay to the same
+ * bytes (several parses of one input, say), but any lists are accepted: host-generated, from the GPU generator, from IR.
+ *  1. The cost pass of divans_b200_encode_cmds_auto_batch_device runs over the n * k (stream, list) pairs, each list under its
+ *     own PredictionMode records: the sum of T[freq] over every coded nibble of both coders, in 1/65536 bit.  A pair whose pass
+ *     fails (status 2 or 3, or a list that would outgrow the logs) costs UINT64_MAX.
+ *  2. d_chosen[i] = the list of the lowest cost, ties to the lowest index; d_cost (may be NULL) = the n * k costs, row per stream
+ *     (d_cost[i * k + c]).  When every list of a stream fails, d_chosen[i] = 0.
+ *  3. Stream i is encoded from list d_chosen[i]: its bytes, out_len and status are exactly divans_b200_encode_cmds_batch_device's
+ *     for that list (so a stream whose lists all fail fails as the plain call does on list 0).  With d_out == NULL the call
+ *     stops after step 2, and d_out_off, d_out_cap, d_out_len and d_status are not read.
+ * Every convention of divans_b200_encode_cmds_batch_device holds, with max_blob_len >= every list's length and max_raw_len >=
+ * every list's decoded length: window_size 0 = each list's header window, status 2 and 3, no sub-batching.  One launch
+ * sequence, no host synchronisation; the pairs run through the context's encoder slots in waves, each slot holding a replay
+ * window of max_raw_len bytes.  k outside 1..16 or a NULL d_chosen returns DIVANS_FAILURE before any work; n == 0 returns
+ * DIVANS_SUCCESS. */
+DivansResult divans_b200_encode_cmds_choose_batch_device(divans_b200_ctx *ctx, size_t n, uint32_t k, const uint8_t *d_blobs,
+                                                         const uint64_t *d_blob_off, const uint64_t *d_blob_len, uint64_t max_blob_len,
+                                                         uint64_t max_raw_len, uint8_t *d_out, const uint64_t *d_out_off,
+                                                         const uint64_t *d_out_cap, uint64_t *d_out_len, int32_t *d_status,
+                                                         const divans_b200_encode_options *opts, uint32_t *d_chosen, uint64_t *d_cost,
+                                                         void *cuda_stream);
 /*
  * command list blob ("DVCL", little endian) -- the binary form of the reference's IR (src/bin/divans.rs:191-483):
  *   u32 magic 0x4c435644, u32 version 1, u32 n_cmds, u32 n_predmodes, u32 n_literal_bytes, u32 window, u32[2] 0

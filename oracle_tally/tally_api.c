@@ -471,3 +471,82 @@ int dvo_encode_cmds_speeds(const dvo_cmdlist *l, const dvo_options *o, const int
                            size_t *out_len, uint32_t *chosen, uint64_t *cost, uint64_t *halves) {
     return dvt_speeds(l, o, values, k, out, cap, out_len, chosen, cost, halves);
 }
+
+/* ---- LZ77 parses, and choosing one of k command lists by cost ----
+ * dvo_lz77_cmds_parse: dvo_lz77_cmds under the parse of include/divans_b200.h ("the LZ77 parse"): best(i) is dvo_lz77_cmds's
+ * match at i (the chain holds every position below i, none above), and the walk takes it when it is at least min_match long and
+ * no lookahead defers it.  {4, 0} is dvo_lz77_cmds.  Outside min_match 4..32, lazy 0..2: DVO_FAILURE and `l` untouched. */
+typedef struct { const uint8_t *in; size_t n, maxdist, ins; int32_t *head, *prev; size_t pos[4], len[4], dist[4]; } dvt_lz;
+
+static uint32_t dvt_h4(const uint8_t *p) {
+    return (((uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24)) * 2654435761u) >> 17;
+}
+
+static size_t dvt_lz_best(dvt_lz *z, size_t i, size_t *dist) {
+    if (z->pos[i & 3] == i) { *dist = z->dist[i & 3]; return z->len[i & 3]; }
+    size_t best = 0, bd = 0;
+    if (i + 4 <= z->n) {
+        for (; z->ins < i; z->ins++)
+            if (z->ins + 4 <= z->n) { uint32_t h = dvt_h4(z->in + z->ins); z->prev[z->ins] = z->head[h]; z->head[h] = (int32_t)z->ins; }
+        int32_t cand = z->head[dvt_h4(z->in + i)]; int chain = 16;
+        while (cand >= 0 && chain-- > 0 && i - (size_t)cand <= z->maxdist) {
+            size_t m = 0, lim = z->n - i; if (lim > 65535) lim = 65535;
+            while (m < lim && z->in[cand + m] == z->in[i + m]) m++;
+            if (m > best) { best = m; bd = i - (size_t)cand; }
+            cand = z->prev[cand];
+        }
+    }
+    z->pos[i & 3] = i; z->len[i & 3] = best; z->dist[i & 3] = bd;
+    *dist = bd;
+    return best;
+}
+
+int dvo_lz77_cmds_parse(const uint8_t *in, size_t n, int window, int pred_mode, int mixing_value, int min_match, int lazy, dvo_cmdlist *l) {
+    if (min_match < 4 || min_match > 32 || lazy < 0 || lazy > 2) return DVO_FAILURE;
+    dvt_lz z; memset(&z, 0, sizeof z);
+    z.in = in; z.n = n; z.maxdist = ((size_t)1 << window) - 16;
+    z.head = (int32_t *)malloc(((size_t)1 << 15) * sizeof(int32_t)); z.prev = (int32_t *)malloc((n + 1) * sizeof(int32_t));
+    if (!z.head || !z.prev) { free(z.head); free(z.prev); return DVO_FAILURE; }
+    for (size_t k = 0; k < ((size_t)1 << 15); k++) z.head[k] = -1;
+    for (int k = 0; k < 4; k++) z.pos[k] = SIZE_MAX;
+    dvo_cmd *c = cl_add(l); c->type = DVO_CMD_PREDMODE; c->a = (uint32_t)l->n_pms;
+    internal_predmode(cl_add_pm(l), pred_mode, mixing_value);
+    size_t i = 0, lit_start = 0, d, d1;
+    while (i < n) {
+        const size_t L = dvt_lz_best(&z, i, &d);
+        int take = L >= (size_t)min_match;
+        if (take && lazy >= 1 && L < 32)
+            take = !(dvt_lz_best(&z, i + 1, &d1) > L || (lazy == 2 && dvt_lz_best(&z, i + 2, &d1) > L + 1));
+        if (!take) { i++; continue; }
+        if (i > lit_start) {
+            size_t off = cl_add_lit(l, in + lit_start, i - lit_start);
+            c = cl_add(l); c->type = DVO_CMD_LITERAL; c->a = (uint32_t)off; c->b = (uint32_t)(i - lit_start);
+        }
+        c = cl_add(l); c->type = DVO_CMD_COPY; c->a = (uint32_t)d; c->b = (uint32_t)L;
+        i += L;
+        lit_start = i;
+    }
+    if (n > lit_start) {
+        size_t off = cl_add_lit(l, in + lit_start, n - lit_start);
+        c = cl_add(l); c->type = DVO_CMD_LITERAL; c->a = (uint32_t)off; c->b = (uint32_t)(n - lit_start);
+    }
+    free(z.head); free(z.prev);
+    return DVO_SUCCESS;
+}
+
+/* The CPU reference of divans_b200_encode_cmds_choose_batch_device for one stream: costs[c] = dvo_tally_cmds of lists[c], each
+ * under its own records (UINT64_MAX where the encoder refuses it), *chosen = their argmin (ties to the lowest index; 0 when all
+ * fail), and lists[*chosen] encoded into out. */
+int dvo_encode_cmds_choose(const dvo_cmdlist *const *lists, uint32_t k, const dvo_options *o, uint8_t *out, size_t cap, size_t *out_len,
+                           uint32_t *chosen, uint64_t *costs) {
+    uint64_t best = UINT64_MAX; uint32_t arg = 0;
+    for (uint32_t c = 0; c < k; c++) {
+        uint64_t t = UINT64_MAX;
+        if (dvo_tally_cmds(lists[c], o, &t) != DVO_SUCCESS) t = UINT64_MAX;
+        if (costs) costs[c] = t;
+        if (t < best) { best = t; arg = c; }
+    }
+    *chosen = arg;
+    *out_len = 0;
+    return dvo_encode_cmds(lists[arg], o, out, cap, out_len);
+}

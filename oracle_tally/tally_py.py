@@ -10,7 +10,8 @@ the record's type ends the walk, and a walk that fails after a forged nibble is 
 followed by tally_api.c, and compiles it twice, with the reference's default probability model and with feature="blend", as
 the oracle's own Makefile does.  Every function of the oracle is in these libraries unchanged while no forged encode runs; only
 the tally entry points, dvo_cmdlist_set_mixing (a test's own mixing values in a list), dvo_recode_blob (the CPU reference of
-the library's command-list replay, on the serialised blob), dvo_cmdlist_from_blob and dvo_encode_cmds_forged are new.
+the library's command-list replay, on the serialised blob), dvo_cmdlist_from_blob, dvo_encode_cmds_forged, dvo_lz77_cmds_parse
+(the LZ77 generator under a parse) and dvo_encode_cmds_choose (one of k command lists chosen by cost) are new.
 """
 import ctypes
 import os
@@ -161,6 +162,9 @@ def lib(blend=False):
         L.dvo_cov_size.restype = ctypes.c_size_t
         L.dvo_encode_cmds_cov.argtypes = [vp, op, vp]
         L.dvo_encode_cmds_forged.argtypes = [vp, op, vp, vp, ctypes.c_size_t, vp, ctypes.c_size_t, szp, u64p]
+        L.dvo_tally_cmds.argtypes = [vp, op, u64p]
+        L.dvo_lz77_cmds_parse.argtypes = [vp, ctypes.c_size_t, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, vp]
+        L.dvo_encode_cmds_choose.argtypes = [vp, ctypes.c_uint32, op, vp, ctypes.c_size_t, szp, ctypes.POINTER(ctypes.c_uint32), vp]
         assert L.dvo_feature_blend() == int(blend)
         _libs[blend] = L
     return _libs[blend]
@@ -457,3 +461,35 @@ def encode_cmds_speeds(cmds, values, blend=False, **kw):
     rc = lib(blend).dvo_encode_cmds_speeds(ctypes.addressof(cmds.c), ctypes.byref(options(blend, **kw)), _p(v), k, _p(out), cap,
                                            ctypes.byref(n), _p(ch), _p(cost), _p(halves))
     return rc, out[: n.value].tobytes() if rc == SUCCESS else None, ch, cost, halves.reshape(k, 2)
+
+
+# ---- LZ77 parses (include/divans_b200.h, "the LZ77 parse") and the choice among k command lists ----
+def tally_cmds(cmds, blend=False, **kw):
+    """(rc, cost): the cost-only walk of the oracle's encoder over the command list ``cmds`` under its own records (dvo_tally_cmds;
+    TALLY_FAILED where the encoder refuses it)"""
+    c = ctypes.c_uint64(0)
+    rc = lib(blend).dvo_tally_cmds(ctypes.addressof(cmds.c), ctypes.byref(options(blend, **kw)), ctypes.byref(c))
+    return rc, c.value
+
+
+def lz77_parse(oracle, data, min_match=4, lazy=0, window=16, pred_mode=2, mixing_value=4):
+    """the oracle_py Commands of dvo_lz77_cmds_parse for ``data`` under the parse (min_match, lazy), or None for a parse outside
+    min_match 4..32, lazy 0..2 (the list is then untouched)"""
+    cl = oracle.Commands()
+    d = _u8(data)
+    rc = lib().dvo_lz77_cmds_parse(_p(d), len(data), window, pred_mode, mixing_value, min_match, lazy, ctypes.addressof(cl.c))
+    return cl if rc == SUCCESS else None
+
+
+def encode_cmds_choose(lists, blend=False, **kw):
+    """(rc, stream or None, chosen, costs [k]): the command list of ``lists`` (oracle_py Commands) that costs least under its own
+    records, ties to the lowest index, encoded (dvo_encode_cmds_choose)"""
+    k = len(lists)
+    ptrs = (ctypes.c_void_p * k)(*[ctypes.addressof(c.c) for c in lists])
+    costs = np.zeros(k, np.uint64)
+    cap = max(int(c.c.n_lits) * 2 + int(c.c.n_cmds) * 16 for c in lists) + (1 << 20)
+    out = np.empty(cap, np.uint8)
+    n, ch = ctypes.c_size_t(0), ctypes.c_uint32(0)
+    rc = lib(blend).dvo_encode_cmds_choose(ptrs, k, ctypes.byref(options(blend, **kw)), _p(out), cap, ctypes.byref(n), ctypes.byref(ch),
+                                           _p(costs))
+    return rc, out[: n.value].tobytes() if rc == SUCCESS else None, ch.value, costs
