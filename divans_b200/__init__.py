@@ -53,6 +53,7 @@ BATCH_SYMBOLS = [
     "divans_b200_encode_cmds_speeds_batch_host",
     "divans_b200_encode_cmds_speeds_batch_device",
     "divans_b200_lz77_cmds_batch_parse", "divans_b200_lz77_cmds_batch_device_parse", "divans_b200_encode_cmds_choose_batch_device",
+    "divans_b200_lz77_cmds_batch_dict", "divans_b200_lz77_cmds_batch_device_dict",
 ]
 PM_RECORD_BYTES = 32 + 16384 + 1024 + 8192   # one prediction-mode record of a DVCL blob (include/divans_b200.h)
 
@@ -109,6 +110,16 @@ class Lz77Parse(ctypes.Structure):
 # under it; then the parses a greedy survey of the corpora picks (tools/lz77_parse_probe.py --survey, DESIGN.md section 4,
 # "Choosing the LZ77 parse").
 DEFAULT_LZ77_PARSES = [(4, 0), (7, 2), (10, 2), (6, 2)]
+
+
+class Lz77DictParse(ctypes.Structure):
+    """divans_b200_lz77_dict_parse: Lz77Parse plus the shortest dictionary word taken (0: none, else 4..32)"""
+    _fields_ = [("min_match", ctypes.c_int32), ("lazy", ctypes.c_int32), ("dict_min", ctypes.c_int32), ("reserved", ctypes.c_int32)]
+
+
+# DEFAULT_LZ77_PARSES, then the (min_match, lazy, dict_min) parses with dictionary words that a greedy survey of exact oracle
+# sizes adds (tools/lz77_dict_probe.py --survey, DESIGN.md section 4, "Dictionary words in the LZ77 parse").
+DEFAULT_LZ77_DICT_PARSES = DEFAULT_LZ77_PARSES + [(7, 2, 4), (10, 2, 4)]
 
 
 class CAllocator(ctypes.Structure):
@@ -192,6 +203,10 @@ def load_library():
     L.divans_b200_lz77_cmds_batch_parse.restype = ctypes.c_uint8
     L.divans_b200_lz77_cmds_batch_device_parse.argtypes = L.divans_b200_lz77_cmds_batch_device.argtypes[:-1] + [ctypes.POINTER(Lz77Parse), vp]
     L.divans_b200_lz77_cmds_batch_device_parse.restype = ctypes.c_uint8
+    L.divans_b200_lz77_cmds_batch_dict.argtypes = L.divans_b200_lz77_cmds_batch.argtypes + [ctypes.POINTER(Lz77DictParse)]
+    L.divans_b200_lz77_cmds_batch_dict.restype = ctypes.c_uint8
+    L.divans_b200_lz77_cmds_batch_device_dict.argtypes = L.divans_b200_lz77_cmds_batch_device.argtypes[:-1] + [ctypes.POINTER(Lz77DictParse), vp]
+    L.divans_b200_lz77_cmds_batch_device_dict.restype = ctypes.c_uint8
     L.divans_b200_encode_cmds_choose_batch_device.argtypes = [vp, sz, ctypes.c_uint32, vp, vp, vp, ctypes.c_uint64, ctypes.c_uint64, vp, vp, vp,
                                                               vp, vp, ctypes.POINTER(EncodeOptions), vp, vp, vp]
     L.divans_b200_encode_cmds_choose_batch_device.restype = ctypes.c_uint8
@@ -280,21 +295,35 @@ def kernel_version():
 
 
 def _parse(parse):
-    """(min_match, lazy) -> a Lz77Parse (the C calls refuse one outside min_match 4..32, lazy 0..2)"""
+    """(min_match, lazy) -> a Lz77Parse, (min_match, lazy, dict_min) -> a Lz77DictParse (the C calls refuse one outside
+    min_match 4..32, lazy 0..2, dict_min 0 or 4..32)"""
+    if len(parse) == 3:
+        mm, lz, dm = parse
+        return Lz77DictParse(int(mm), int(lz), int(dm), 0)
     mm, lz = parse
     return Lz77Parse(int(mm), int(lz))
+
+
+def _parse_ok(ps):
+    ok = 4 <= ps.min_match <= 32 and 0 <= ps.lazy <= 2
+    return ok and (not isinstance(ps, Lz77DictParse) or ps.dict_min == 0 or 4 <= ps.dict_min <= 32)
 
 
 def lz77_cmds_batch(blob, in_off, in_len, window=16, pred_mode=2, mixing_value=4, n_threads=None, parse=None):
     """Raw buffers -> DVCL command lists by the library's greedy LZ77 (divans_b200_lz77_cmds_batch): returns
     (blobs uint8 array, blob_off, blob_len) ready for Engine.encode_batch_host(..., cmds=True).  ``parse`` (min_match, lazy):
-    the parse of divans_b200_lz77_cmds_batch_parse (include/divans_b200.h); None is (4, 0)."""
+    the parse of divans_b200_lz77_cmds_batch_parse (include/divans_b200.h); None is (4, 0).  (min_match, lazy, dict_min): the
+    parse with dictionary words of divans_b200_lz77_cmds_batch_dict."""
     L = load_library()
     if parse is not None:
         ps = _parse(parse)
-        if not (4 <= ps.min_match <= 32 and 0 <= ps.lazy <= 2):
+        if not _parse_ok(ps):
+            if isinstance(ps, Lz77DictParse):
+                raise ValueError("lz77_cmds_batch: parse (%d, %d, %d) is outside min_match 4..32, lazy 0..2, dict_min 0 or 4..32"
+                                 % (ps.min_match, ps.lazy, ps.dict_min))
             raise ValueError("lz77_cmds_batch: parse (%d, %d) is outside min_match 4..32, lazy 0..2" % (ps.min_match, ps.lazy))
-        fn = lambda *a: L.divans_b200_lz77_cmds_batch_parse(*a, ctypes.byref(ps))
+        f = L.divans_b200_lz77_cmds_batch_dict if isinstance(ps, Lz77DictParse) else L.divans_b200_lz77_cmds_batch_parse
+        fn = lambda *a: f(*a, ctypes.byref(ps))
     else:
         fn = L.divans_b200_lz77_cmds_batch
     blob = _u8(blob)
@@ -859,13 +888,16 @@ class Engine:
         +d_blob_cap[i]) (4-byte aligned; lz77_blob_cap always suffices).  Status 0: d_blob_len[i] bytes equal to lz77_cmds_batch's
         blob; 2: the region is too small and d_blob_len[i] is the size needed; 3: refused (misaligned region, in_len > max_in_len
         or >= 2**31).  Asynchronous on ``stream``; regions are not cleared first.  ``parse`` (min_match, lazy) as for
-        lz77_cmds_batch (divans_b200_lz77_cmds_batch_device_parse); None is (4, 0)."""
+        lz77_cmds_batch (divans_b200_lz77_cmds_batch_device_parse); None is (4, 0).  (min_match, lazy, dict_min): with dictionary
+        words (divans_b200_lz77_cmds_batch_device_dict)."""
         args = (self._h, n, d_in, d_in_off, d_in_len, int(max_in_len), int(window), int(pred_mode), int(mixing_value), d_blobs, d_blob_off,
                 d_blob_cap, d_blob_len, d_status)
         if parse is None:
             rc = self._L.divans_b200_lz77_cmds_batch_device(*args, stream)
         else:
-            rc = self._L.divans_b200_lz77_cmds_batch_device_parse(*args, ctypes.byref(_parse(parse)), stream)
+            ps = _parse(parse)
+            f = self._L.divans_b200_lz77_cmds_batch_device_dict if isinstance(ps, Lz77DictParse) else self._L.divans_b200_lz77_cmds_batch_device_parse
+            rc = f(*args, ctypes.byref(ps), stream)
         if rc != DIVANS_SUCCESS:
             raise DivansError("lz77_cmds_batch_device: " + self._err())
 
@@ -894,9 +926,9 @@ class Engine:
         streams each (default all), halved while the encoder cannot allocate them.  Returns (d_new, new_off, new_len, status):
         status[i] is the generator's status where that failed (the list then reaches the encoder with length 0), else the
         encoder's.
-        With ``parses`` (a list of 1..16 (min_match, lazy) pairs, e.g. DEFAULT_LZ77_PARSES) the generator makes one list per
-        parse and stream, and encode_cmds_choose_batch_device encodes each stream from the list that codes cheapest under its own
-        record; with ``candidates`` too, the literal model is then chosen on that list (encode_cmds_auto_batch_device).  The call
+        With ``parses`` (a list of 1..16 (min_match, lazy) pairs or (min_match, lazy, dict_min) triples, e.g. DEFAULT_LZ77_PARSES
+        or DEFAULT_LZ77_DICT_PARSES) the generator makes one list per parse and stream, and encode_cmds_choose_batch_device
+        encodes each stream from the list that codes cheapest under its own record; with ``candidates`` too, the literal model is then chosen on that list (encode_cmds_auto_batch_device).  The call
         then also returns chosen_parse [n] (an index into ``parses``) and parse_cost [n, k] last."""
         import torch
         n = len(in_off)

@@ -184,18 +184,37 @@ extern "C" DivansResult divans_b200_ir_to_cmds(const char *ir_text, size_t ir_le
 
 // ---------------------------------------------------------------------------------------------------------------
 // Command generator for benchmarks and tools (ours, not a reference component): a deterministic hash-chain LZ77 (by default
-// greedy with minimum match 4; window 2^window - 16, no dictionary words) that turns raw bytes into a DVCL command list -- one
-// PredictionMode command (64-entry identity context map, one mixing value, like raw_to_cmd/mod.rs:116-143), then Literal /
-// Copy commands.  SURVEY 8d calls the resulting population "Z": copy-dominated streams like the reference's default
+// greedy with minimum match 4; window 2^window - 16; dictionary words only when the parse asks for them) that turns raw bytes
+// into a DVCL command list -- one PredictionMode command (64-entry identity context map, one mixing value, like
+// raw_to_cmd/mod.rs:116-143), then Literal / Copy / Dictionary commands.  SURVEY 8d calls the resulting population "Z": copy-dominated streams like the reference's default
 // (brotli-driven) compressor produces.  The command SELECTION of the brotli crate stays out of scope.
 // ---------------------------------------------------------------------------------------------------------------
 #include <algorithm>
+#include <memory>
 #include <thread>
+
+#include "dv_dict.h"
+
+extern "C" const uint8_t dv_tables_blob[];   // brotli_tables.bin, embedded by dv_capi.cu
+
+namespace dv {
+// The dictionary index, built once per process on first use (the GPU generator uploads this copy).  NULL if the tables do not
+// have the shape the index assumes.
+const DictIndex *host_dict_index() {
+    static const std::unique_ptr<DictIndex> x = [] {
+        std::unique_ptr<DictIndex> d(new DictIndex());
+        if (!dict_index_build(dv_tables_blob, *d)) d.reset();
+        return d;
+    }();
+    return x.get();
+}
+}  // namespace dv
 
 namespace {
 // The parse (include/divans_b200.h, "the LZ77 parse"): best(j) needs every position below j inserted and j not yet, so the
 // chain is filled up to j on demand; the (at most three) positions the parse looks at around i are kept in a small cache.
-size_t lz77_blob(const uint8_t *in, size_t n, int window, int pred_mode, int mixing_value, const divans_b200_lz77_parse &parse,
+// With dict_min != 0, dict(i) (dv_dict.h) is looked up at every position the parse reaches and does not defer.
+size_t lz77_blob(const uint8_t *in, size_t n, int window, int pred_mode, int mixing_value, const divans_b200_lz77_dict_parse &parse,
                  std::vector<uint8_t> &blob) {
     std::vector<Cmd> cmds;
     cmds.push_back({7, 0, 0, 0, 0});
@@ -233,6 +252,17 @@ size_t lz77_blob(const uint8_t *in, size_t n, int window, int pred_mode, int mix
         bool take = L >= min_match;
         if (take && parse.lazy >= 1 && L < 32)
             take = !(best(i + 1, d1) > L || (parse.lazy == 2 && best(i + 2, d1) > L + 1));
+        if (parse.dict_min && (take || L < min_match)) {   // (not deferred)
+            const uint32_t k = dv::dict_match(*dv::host_dict_index(), dv_tables_blob + dv::DICT_TB_DICT, in + i, (uint32_t)std::min<size_t>(n - i, 64));
+            const size_t Ld = dv::dict_len(k);
+            if (Ld >= (size_t)parse.dict_min && Ld > (take ? L : 0)) {
+                if (i > lit_start) cmds.push_back({3, (uint32_t)lit_start, (uint32_t)(i - lit_start), 0, 0});
+                cmds.push_back({2, dv::dict_id(k), dv::dict_size(k), dv::dict_transform(k), (uint32_t)Ld});
+                i += Ld;
+                lit_start = i;
+                continue;
+            }
+        }
         if (take) {
             if (i > lit_start) cmds.push_back({3, (uint32_t)lit_start, (uint32_t)(i - lit_start), 0, 0});
             cmds.push_back({1, (uint32_t)best_dist, (uint32_t)L, 0, 0});
@@ -259,13 +289,15 @@ size_t lz77_blob(const uint8_t *in, size_t n, int window, int pred_mode, int mix
 
 // n raw buffers -> n DVCL blobs written back to back at blob_off[i] (16-byte aligned) of `out`; blob_len[i] receives the sizes.
 // With out == NULL or out_cap too small the call returns DIVANS_NEEDS_MORE_OUTPUT and *total receives the size needed.
-// `parse` NULL or outside min_match 4..32, lazy 0..2: DIVANS_FAILURE, nothing written.
-extern "C" DivansResult divans_b200_lz77_cmds_batch_parse(size_t n, const uint8_t *in, const uint64_t *in_off, const uint64_t *in_len, int32_t window,
-                                                          int32_t pred_mode, int32_t mixing_value, uint8_t *out, size_t out_cap, uint64_t *blob_off,
-                                                          uint64_t *blob_len, size_t *total, int32_t n_threads, const divans_b200_lz77_parse *parse) {
+// `parse` NULL or outside min_match 4..32, lazy 0..2, dict_min 0 or 4..32, reserved 0: DIVANS_FAILURE, nothing written.
+extern "C" DivansResult divans_b200_lz77_cmds_batch_dict(size_t n, const uint8_t *in, const uint64_t *in_off, const uint64_t *in_len, int32_t window,
+                                                         int32_t pred_mode, int32_t mixing_value, uint8_t *out, size_t out_cap, uint64_t *blob_off,
+                                                         uint64_t *blob_len, size_t *total, int32_t n_threads, const divans_b200_lz77_dict_parse *parse) {
     if (!in || !in_off || !in_len || !blob_off || !blob_len || !total || window < 10 || window > 24) return DIVANS_FAILURE;
     if (!parse || parse->min_match < 4 || parse->min_match > 32 || parse->lazy < 0 || parse->lazy > 2) return DIVANS_FAILURE;
-    const divans_b200_lz77_parse ps = *parse;
+    if ((parse->dict_min != 0 && (parse->dict_min < 4 || parse->dict_min > 32)) || parse->reserved != 0) return DIVANS_FAILURE;
+    if (parse->dict_min && !dv::host_dict_index()) return DIVANS_FAILURE;
+    const divans_b200_lz77_dict_parse ps = *parse;
     std::vector<std::vector<uint8_t>> blobs(n);
     if (n_threads < 1) n_threads = 1;
     std::vector<std::thread> th;
@@ -278,6 +310,15 @@ extern "C" DivansResult divans_b200_lz77_cmds_batch_parse(size_t n, const uint8_
     if (!out || out_cap < pos) return DIVANS_NEEDS_MORE_OUTPUT;
     for (size_t i = 0; i < n; i++) memcpy(out + blob_off[i], blobs[i].data(), blobs[i].size());
     return DIVANS_SUCCESS;
+}
+
+extern "C" DivansResult divans_b200_lz77_cmds_batch_parse(size_t n, const uint8_t *in, const uint64_t *in_off, const uint64_t *in_len, int32_t window,
+                                                          int32_t pred_mode, int32_t mixing_value, uint8_t *out, size_t out_cap, uint64_t *blob_off,
+                                                          uint64_t *blob_len, size_t *total, int32_t n_threads, const divans_b200_lz77_parse *parse) {
+    if (!parse) return DIVANS_FAILURE;
+    const divans_b200_lz77_dict_parse dp = {parse->min_match, parse->lazy, 0, 0};
+    return divans_b200_lz77_cmds_batch_dict(n, in, in_off, in_len, window, pred_mode, mixing_value, out, out_cap, blob_off, blob_len, total,
+                                            n_threads, &dp);
 }
 
 extern "C" DivansResult divans_b200_lz77_cmds_batch(size_t n, const uint8_t *in, const uint64_t *in_off, const uint64_t *in_len, int32_t window,

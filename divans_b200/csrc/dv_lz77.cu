@@ -1,4 +1,4 @@
-// dv_lz77.cu -- sm_90a kernel of divans_b200_lz77_cmds_batch_device[_parse]: the library's hash-chain LZ77 (dv_ir.cpp,
+// dv_lz77.cu -- sm_90a kernels of divans_b200_lz77_cmds_batch_device[_parse|_dict]: the library's hash-chain LZ77 (dv_ir.cpp,
 // lz77_blob) run next to raw buffers in HBM.  Every blob is byte for byte the one the host generator writes for the same input,
 // arguments and parse.  The host's rules:
 //   h4(i) = (le32(in + i) * 2654435761) >> 17, for positions with i + 4 <= n only; every such position is inserted, in order,
@@ -6,7 +6,8 @@
 //   newest first and up to the first farther than 2^window - 16.  The longest match of at most min(n - i, 65535) bytes wins, a
 //   tie going to the newer candidate.  The parse (include/divans_b200.h): a match of min_match or more bytes is a copy unless
 //   a lazy lookahead defers it (L < 32 and len(i + 1) > L, or with lazy 2 len(i + 2) > L + 1); anything else leaves the byte
-//   a literal.  The default parse is min_match 4, lazy 0.
+//   a literal.  The default parse is min_match 4, lazy 0.  With dict_min != 0, a position the parse reaches and does not defer
+//   takes the dictionary word dict(i) (dv_dict.h) when it has dict_min or more bytes and is longer than the copy there.
 //
 // One warp per stream; persistent warps pull stream indices from the work counter, so any n runs in one launch.  Each warp owns
 // a head table (2^15 entries) and prev[max_in_len] in global memory.  Per stream:
@@ -22,7 +23,9 @@
 //     starts there, so every deferral is decided with both lengths in hand.  A
 //     copy whose capped length reached LZ_CAP (and could be longer) is measured exactly, by the whole warp, for each candidate
 //     that reached the cap, in chain order: only those can be the longest.  So per window a lane spends at most 16 capped
-//     compares, and exact lengths are measured only where the parse lands.
+//     compares, and exact lengths are measured only where the parse lands.  With the dictionary step (lz77_dict_kernel), lane t
+//     also looks up dict(p + t) in the dictionary index, and the lanes with a copy or a word make the ballot.  A word has at most
+//     31 bytes, so comparing it with a capped copy length (LZ_CAP = 64) is exact.
 //  3. Emit.  Records go out as they are found, at blob + 32 + 20k, while they fit the region; then the header, the
 //     PredictionMode record (built once per call on the host) and the literal pool, which is the raw stream.  A blob that
 //     does not fit is still parsed to the end, so its exact size is reported.
@@ -99,10 +102,9 @@ __device__ __noinline__ int2 lz_extend(const uint8_t *in, const uint8_t *end, co
     return make_int2(best, dist);
 }
 
-// (launch bounds: 16 blocks, 32 warps per SM, the most a context's max_resident asks for; without the minimum ptxas spilled)
-// LAZY: the parse's lazy steps (0..2); min_match is p.min_match
-template <int LAZY>
-__global__ void __launch_bounds__(LZ_BLOCK_THREADS, 16) lz77_cmds_kernel(Lz77Params p) {
+// LAZY: the parse's lazy steps (0..2); min_match is p.min_match.  DICT: the dictionary step, dc.dict_min 4..32 (dc unread without it).
+template <int LAZY, bool DICT>
+__device__ __forceinline__ void lz77_cmds_body(const Lz77Params &p, const Lz77Dict &dc) {
     const int lane = threadIdx.x & 31;
     const uint32_t warp = blockIdx.x * LZ_WARPS + (threadIdx.x >> 5);
     if (warp >= p.n_warps) return;
@@ -153,18 +155,28 @@ __global__ void __launch_bounds__(LZ_BLOCK_THREADS, 16) lz77_cmds_kernel(Lz77Par
                 reinterpret_cast<uint32_t *>(blob + 32 + 20ull * n_cmds)[lane] = lane == 0 ? type : lane == 1 ? a : lane == 2 ? b : 0u;
             n_cmds++;
         };
+        auto emit_word = [&](uint32_t k) {   // Dictionary(id, size, transform, length) of a packed dict_match
+            if (32ull + 20ull * (n_cmds + 1) <= cap && lane < 5)
+                reinterpret_cast<uint32_t *>(blob + 32 + 20ull * n_cmds)[lane] =
+                    lane == 0 ? 2u : lane == 1 ? dict_id(k) : lane == 2 ? dict_size(k) : lane == 3 ? dict_transform(k) : dict_len(k);
+            n_cmds++;
+        };
         emit(7, 0, 0);   // the PredictionMode command: record 0
         int32_t pos = 0, lit_start = 0;
         while (pos < n) {
             const int32_t span = min(32, n - pos);   // the window: positions pos .. pos + span - 1, all below n
             const int32_t q = lane < span ? pos + lane : n;
             int32_t best = 0, dist = 0, lim = 0;
-            uint32_t hits = 0;
+            uint32_t hits = 0, word = 0;
             if (q < nh) {
                 lim = min(n - q, LZ_MAX_COPY);
                 best = lz_capped(in, end, prev, q, lim, maxdist, dist, hits);
+                if (DICT) {
+                    word = dict_match(*dc.index, dc.words, in + q, (uint32_t)min(n - q, LZ_CAP));
+                    if (dict_len(word) < (uint32_t)dc.dict_min) word = 0;
+                }
             }
-            const uint32_t copies = __ballot_sync(LZ_FULL, best >= p.min_match);
+            const uint32_t copies = __ballot_sync(LZ_FULL, best >= p.min_match || (DICT && word != 0));
             const int32_t wend = pos + span;
             int32_t at = pos;   // the parse position in this window
             while (at < wend) {
@@ -176,12 +188,23 @@ __global__ void __launch_bounds__(LZ_BLOCK_THREADS, 16) lz77_cmds_kernel(Lz77Par
                 int32_t len = __shfl_sync(LZ_FULL, best, t), d = __shfl_sync(LZ_FULL, dist, t);
                 const int32_t lt = __shfl_sync(LZ_FULL, lim, t);
                 const uint32_t ht = __shfl_sync(LZ_FULL, hits, t);
-                if (LAZY > 0 && len < LZ_LAZY_BELOW) {
+                const bool is_copy = !DICT || len >= p.min_match;   // (with DICT the lane may hold a word only)
+                if (LAZY > 0 && is_copy && len < LZ_LAZY_BELOW) {
                     // lanes past the stream's end hold 0, the length there; a lookahead past a window that the stream goes on
                     // after is decided by the next window, which starts at cq
                     if (t + LAZY >= span && wend < n) { at = cq; break; }
                     const int32_t l1 = __shfl_sync(LZ_FULL, best, (t + 1) & 31), l2 = __shfl_sync(LZ_FULL, best, (t + 2) & 31);
                     if ((t + 1 < 32 && l1 > len) || (LAZY == 2 && t + 2 < 32 && l2 > len + 1)) { at = cq + 1; continue; }
+                }
+                if (DICT) {
+                    const uint32_t wt = __shfl_sync(LZ_FULL, word, t);
+                    if ((int32_t)dict_len(wt) > (is_copy ? len : 0)) {   // (a capped len of LZ_CAP is longer than any word)
+                        if (cq > lit_start) emit(3, (uint32_t)lit_start, (uint32_t)(cq - lit_start));
+                        emit_word(wt);
+                        at = cq + (int32_t)dict_len(wt);
+                        lit_start = at;
+                        continue;
+                    }
                 }
                 if (len == LZ_CAP && lt > LZ_CAP) {
                     const int2 e = lz_extend(in, end, prev, cq, lt, ht);
@@ -215,9 +238,21 @@ __global__ void __launch_bounds__(LZ_BLOCK_THREADS, 16) lz77_cmds_kernel(Lz77Par
     }
 }
 
-void launch_lz77_cmds(const Lz77Params &p, cudaStream_t st) {
+// (launch bounds: 16 blocks, 32 warps per SM, the most a context's max_resident asks for; without the minimum ptxas spilled)
+template <int LAZY>
+__global__ void __launch_bounds__(LZ_BLOCK_THREADS, 16) lz77_cmds_kernel(Lz77Params p) { lz77_cmds_body<LAZY, false>(p, Lz77Dict{}); }
+template <int LAZY>
+__global__ void __launch_bounds__(LZ_BLOCK_THREADS, 16) lz77_dict_kernel(Lz77Params p, Lz77Dict d) {
+    lz77_cmds_body<LAZY, true>(p, d);
+}
+
+void launch_lz77_cmds(const Lz77Params &p, const Lz77Dict &d, cudaStream_t st) {
     const unsigned blocks = (p.n_warps + LZ_WARPS - 1) / LZ_WARPS;
-    if (p.lazy == 2) lz77_cmds_kernel<2><<<blocks, LZ_BLOCK_THREADS, 0, st>>>(p);
+    if (d.dict_min) {
+        if (p.lazy == 2) lz77_dict_kernel<2><<<blocks, LZ_BLOCK_THREADS, 0, st>>>(p, d);
+        else if (p.lazy == 1) lz77_dict_kernel<1><<<blocks, LZ_BLOCK_THREADS, 0, st>>>(p, d);
+        else lz77_dict_kernel<0><<<blocks, LZ_BLOCK_THREADS, 0, st>>>(p, d);
+    } else if (p.lazy == 2) lz77_cmds_kernel<2><<<blocks, LZ_BLOCK_THREADS, 0, st>>>(p);
     else if (p.lazy == 1) lz77_cmds_kernel<1><<<blocks, LZ_BLOCK_THREADS, 0, st>>>(p);
     else lz77_cmds_kernel<0><<<blocks, LZ_BLOCK_THREADS, 0, st>>>(p);
 }

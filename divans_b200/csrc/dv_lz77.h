@@ -3,6 +3,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "dv_dict.h"
+
 namespace dv {
 
 constexpr uint32_t LZ_HEAD_ENTRIES = 1u << 15;   // the hash table of the host generator (dv_ir.cpp, lz77_blob): 15-bit hashes
@@ -19,6 +21,12 @@ struct Lz77Params {
     int32_t min_match, lazy;   // the parse (include/divans_b200.h): min_match 4..32, lazy 0..2
     uint32_t *work_counter; int32_t *scratch; uint64_t stride; uint32_t n_warps;
 };
-void launch_lz77_cmds(const Lz77Params &p, cudaStream_t st);   // one launch, n_warps persistent warps (a kernel per lazy 0..2)
+// The dictionary step (include/divans_b200.h, "dictionary words in the LZ77 parse"): dict_min 0 (off) or 4..32, the index and
+// the dictionary bytes.  A parameter of its own: the kernels without the step keep Lz77Params, and with it their code.
+struct Lz77Dict {
+    const DictIndex *index; const uint8_t *words; int32_t dict_min;
+};
+// one launch, n_warps persistent warps (a kernel per lazy 0..2, with the dictionary step when d.dict_min != 0)
+void launch_lz77_cmds(const Lz77Params &p, const Lz77Dict &d, cudaStream_t st);
 
 }  // namespace dv

@@ -596,6 +596,48 @@ DivansResult divans_b200_lz77_cmds_batch_device_parse(divans_b200_ctx *ctx, size
                                                       int32_t mixing_value, uint8_t *d_blobs, const uint64_t *d_blob_off,
                                                       const uint64_t *d_blob_cap, uint64_t *d_blob_len, int32_t *d_status,
                                                       const divans_b200_lz77_parse *parse, void *cuda_stream);
+/* ---- dictionary words in the LZ77 parse ----
+ * The parse above with one more step: RFC 7932 static-dictionary words, emitted as Dictionary commands (DVCL type 2).
+ *  - The transform set: the transforms whose prefix is empty and whose type is identity (0), so their output is word + suffix.
+ *    It is derived from the RFC 7932 tables at load time; it has 44 members, 0 (""), 1 (" "), 5 (" the "), 8 (" of "), ...
+ *  - dict(i) = (Ld, word id, word size, transform).  Among every word of size 4..24 with id below 2^size_bits_by_length[size],
+ *    under every transform of the set, with transformed bytes w, i + |w| <= n and in[i .. i + |w|) == w: the longest |w|, ties
+ *    to the lowest transform id, then the shortest word size, then the lowest word id.  Ld = 0 where none matches.  Like best(i),
+ *    dict(i) is a function of i alone.  |w| is at most 24 + 7 = 31 bytes.
+ *  - With dict_min = 0 the parse is exactly the one above.  With dict_min 4..32, at a position the parse reaches and does not
+ *    defer, let Lc = len(i) if it is at least min_match (else 0) and Ld = dict(i)'s length if it is at least dict_min (else 0).
+ *    If Ld > Lc the parse emits the pending literal run (if any), then Dictionary(a = word id, b = word size, c = transform,
+ *    d = Ld), and i += Ld.  Otherwise it goes on exactly as above.
+ *  - Deferral keeps its rule on copy lengths alone: a position deferred because len(i + 1) or len(i + 2) is longer becomes a
+ *    literal even when a dictionary word starts there.  A deferral needs L = len(i) >= min_match, so a position with no copy
+ *    is never deferred and may always take a word.
+ *  - Every position is still inserted into the hash chain in order, so best(i) does not move.
+ *  - Region bound: a Dictionary command covers |w| >= 4 bytes, as a Copy covers at least 4, and literal runs stay maximal.  So
+ *    the proof of divans_b200_lz77_cmds_batch_device holds with "Copy" read as "Copy or Dictionary", and lz77_blob_cap holds
+ *    every list of every parse.
+ * Domain: min_match 4..32, lazy 0..2, dict_min 0 or 4..32, reserved 0. */
+typedef struct {
+    int32_t min_match;   /* 4..32: the shortest match emitted as a copy */
+    int32_t lazy;        /* 0..2: positions looked ahead before a match shorter than 32 bytes is taken */
+    int32_t dict_min;    /* 0 (no dictionary words) or 4..32: the shortest transformed word emitted as a Dictionary command */
+    int32_t reserved;    /* 0 */
+} divans_b200_lz77_dict_parse;
+/* divans_b200_lz77_cmds_batch_parse under a parse with dictionary words (NULL or out of the domain: DIVANS_FAILURE, nothing
+ * written).  dict_min = 0 writes divans_b200_lz77_cmds_batch_parse's blobs for {min_match, lazy}, byte for byte. */
+DivansResult divans_b200_lz77_cmds_batch_dict(size_t n, const uint8_t *in, const uint64_t *in_off, const uint64_t *in_len, int32_t window,
+                                              int32_t pred_mode, int32_t mixing_value, uint8_t *out, size_t out_cap, uint64_t *blob_off,
+                                              uint64_t *blob_len, size_t *total, int32_t n_threads, const divans_b200_lz77_dict_parse *parse);
+/* divans_b200_lz77_cmds_batch_device_parse under a parse with dictionary words: every blob byte for byte
+ * divans_b200_lz77_cmds_batch_dict's, with every other rule of that call (statuses, regions, refusals, scratch, the step end
+ * before a deferral whose lookahead falls past the 32 positions).  A parse that is NULL or outside the domain fails the call
+ * (DIVANS_FAILURE, divans_b200_last_error says why) before any work.  With dict_min != 0 the first call on a context uploads a
+ * dictionary index of 174,344 bytes next to the RFC 7932 tables (122,784 dictionary bytes) the decoder already holds; it stays
+ * until the context is destroyed. */
+DivansResult divans_b200_lz77_cmds_batch_device_dict(divans_b200_ctx *ctx, size_t n, const uint8_t *d_in, const uint64_t *d_in_off,
+                                                     const uint64_t *d_in_len, uint64_t max_in_len, int32_t window, int32_t pred_mode,
+                                                     int32_t mixing_value, uint8_t *d_blobs, const uint64_t *d_blob_off,
+                                                     const uint64_t *d_blob_cap, uint64_t *d_blob_len, int32_t *d_status,
+                                                     const divans_b200_lz77_dict_parse *parse, void *cuda_stream);
 /* ---- choosing one of k command lists per stream by coding cost ----
  * n streams, each with k (1..16) candidate DVCL command lists already in HBM, candidate-major: list c of stream i is
  * d_blobs[d_blob_off[c * n + i] .. +d_blob_len[c * n + i]) (4-byte aligned).  The lists of a stream should replay to the same

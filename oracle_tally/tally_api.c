@@ -501,8 +501,38 @@ static size_t dvt_lz_best(dvt_lz *z, size_t i, size_t *dist) {
     return best;
 }
 
-int dvo_lz77_cmds_parse(const uint8_t *in, size_t n, int window, int pred_mode, int mixing_value, int min_match, int lazy, dvo_cmdlist *l) {
+/* dict(i) of include/divans_b200.h ("dictionary words in the LZ77 parse"), restated without an index: every word of size 4..24
+ * and id below 2^size_bits_by_length[size] is compared with the input; where one matches, every transform with an empty prefix
+ * and the identity type is built by dvo_dict_word and compared.  The best is kept under the rule's order: longest, then lowest
+ * transform, shortest size, lowest id.  Returns the length (0: none). */
+static size_t dvt_dict_at(const uint8_t *in, size_t n, size_t i, uint32_t *id, uint32_t *size, uint32_t *transform) {
+    size_t best = 0;
+    uint8_t w[64];
+    for (uint32_t s = 4; s <= 24; s++) {
+        if (i + s > n) break;
+        for (uint32_t wid = 0; wid < (1u << TB_SIZE_BITS[s]); wid++) {
+            if (memcmp(TB_DICT + TB_OFFSETS[s] + (size_t)wid * s, in + i, s) != 0) continue;
+            for (uint32_t t = 0; t < 121; t++) {
+                const uint8_t *tr = TB_TRANSFORMS + 3 * t;
+                if (TB_PS[TB_PSMAP[tr[0]]] != 0 || tr[1] != 0) continue;
+                const int len = dvo_dict_word(s, wid, t, w);
+                if (len < 0 || i + (size_t)len > n || memcmp(w, in + i, (size_t)len) != 0) continue;
+                const int better = (size_t)len > best
+                    || ((size_t)len == best && (t < *transform || (t == *transform && (s < *size || (s == *size && wid < *id)))));
+                if (better) { best = (size_t)len; *id = wid; *size = s; *transform = t; }
+            }
+        }
+    }
+    return best;
+}
+
+/* dvo_lz77_cmds_parse with dictionary words (dict_min 0 or 4..32; 0 is dvo_lz77_cmds_parse).  At a position the walk reaches and
+ * does not defer, a word of dict_min or more bytes that is longer than the copy there (0 below min_match) is emitted as a
+ * Dictionary command. */
+int dvo_lz77_cmds_dict_parse(const uint8_t *in, size_t n, int window, int pred_mode, int mixing_value, int min_match, int lazy, int dict_min,
+                             dvo_cmdlist *l) {
     if (min_match < 4 || min_match > 32 || lazy < 0 || lazy > 2) return DVO_FAILURE;
+    if (dict_min != 0 && (dict_min < 4 || dict_min > 32)) return DVO_FAILURE;
     dvt_lz z; memset(&z, 0, sizeof z);
     z.in = in; z.n = n; z.maxdist = ((size_t)1 << window) - 16;
     z.head = (int32_t *)malloc(((size_t)1 << 15) * sizeof(int32_t)); z.prev = (int32_t *)malloc((n + 1) * sizeof(int32_t));
@@ -514,16 +544,22 @@ int dvo_lz77_cmds_parse(const uint8_t *in, size_t n, int window, int pred_mode, 
     size_t i = 0, lit_start = 0, d, d1;
     while (i < n) {
         const size_t L = dvt_lz_best(&z, i, &d);
-        int take = L >= (size_t)min_match;
-        if (take && lazy >= 1 && L < 32)
-            take = !(dvt_lz_best(&z, i + 1, &d1) > L || (lazy == 2 && dvt_lz_best(&z, i + 2, &d1) > L + 1));
-        if (!take) { i++; continue; }
+        int take = L >= (size_t)min_match, deferred = 0;
+        if (take && lazy >= 1 && L < 32) {
+            deferred = dvt_lz_best(&z, i + 1, &d1) > L || (lazy == 2 && dvt_lz_best(&z, i + 2, &d1) > L + 1);
+            take = !deferred;
+        }
+        uint32_t wid = 0, ws = 0, wt = 0;
+        const size_t Ld = dict_min && !deferred ? dvt_dict_at(in, n, i, &wid, &ws, &wt) : 0;
+        const int word = Ld >= (size_t)dict_min && Ld > (take ? L : 0);
+        if (!take && !word) { i++; continue; }
         if (i > lit_start) {
             size_t off = cl_add_lit(l, in + lit_start, i - lit_start);
             c = cl_add(l); c->type = DVO_CMD_LITERAL; c->a = (uint32_t)off; c->b = (uint32_t)(i - lit_start);
         }
-        c = cl_add(l); c->type = DVO_CMD_COPY; c->a = (uint32_t)d; c->b = (uint32_t)L;
-        i += L;
+        c = cl_add(l);
+        if (word) { c->type = DVO_CMD_DICT; c->a = wid; c->b = ws; c->c = wt; c->d = (uint32_t)Ld; i += Ld; }
+        else { c->type = DVO_CMD_COPY; c->a = (uint32_t)d; c->b = (uint32_t)L; i += L; }
         lit_start = i;
     }
     if (n > lit_start) {
@@ -532,6 +568,10 @@ int dvo_lz77_cmds_parse(const uint8_t *in, size_t n, int window, int pred_mode, 
     }
     free(z.head); free(z.prev);
     return DVO_SUCCESS;
+}
+
+int dvo_lz77_cmds_parse(const uint8_t *in, size_t n, int window, int pred_mode, int mixing_value, int min_match, int lazy, dvo_cmdlist *l) {
+    return dvo_lz77_cmds_dict_parse(in, n, window, pred_mode, mixing_value, min_match, lazy, 0, l);
 }
 
 /* The CPU reference of divans_b200_encode_cmds_choose_batch_device for one stream: costs[c] = dvo_tally_cmds of lists[c], each
