@@ -274,6 +274,71 @@ def _host_batch(*desc):
     return [np.ascontiguousarray(a, np.uint64) for a in desc] + [np.zeros(n, np.uint64), np.full(n, DIVANS_FAILURE, np.int32)]
 
 
+# -- the plumbing of the pipelines that keep their data in HBM (Engine.transcode_device, Engine.compress_device)
+def _private_stream(dev, stream):
+    """(caller, s): the caller's CUDA stream (``stream``, default the current one) and a stream of the pipeline's own, ordered
+    after the work already queued on the caller's.  A default stream has no handle the library could take: NULL would mean
+    the context's stream."""
+    import torch
+    caller = stream if stream is not None else torch.cuda.current_stream(dev)
+    s = torch.cuda.Stream(dev)
+    s.wait_stream(caller)
+    return caller, s
+
+
+def _hand_back(caller, s, d_new):
+    """Order the caller's stream after the pipeline's, which allocated ``d_new``: the caller uses it from here on."""
+    caller.wait_stream(s)
+    d_new.record_stream(caller)
+
+
+def _u64(a, dev):
+    """A host array of uint64 values -> a device int64 tensor of the same bits (a synchronous upload)."""
+    import torch
+    return torch.from_numpy(np.ascontiguousarray(a, np.uint64).view(np.int64)).to(dev, non_blocking=False)
+
+
+def _columns(t, n, widths):
+    """The columns of ``t``, a device tensor of n-slot columns or its host copy: {name: slots} for each name of ``widths`` in
+    order, widths[name] * n slots each.  An int32 or uint32 column of n values takes the first half of its n int64 slots."""
+    cols, i = {}, 0
+    for name, w in widths.items():
+        cols[name] = t[i * n:(i + w) * n]
+        i += w
+    return cols
+
+
+def _empty_result(dev, *choices):
+    """What a pipeline returns for no streams: (d_new, new_off, new_len, status), then (chosen, cost [0, c]) for each c of
+    ``choices`` that is not None."""
+    import torch
+    res = torch.zeros(0, dtype=torch.uint8, device=dev), np.zeros(0, np.uint64), np.zeros(0, np.uint64), np.zeros(0, np.int32)
+    for c in choices:
+        if c is not None:
+            res += (np.zeros(0, np.uint32), np.zeros((0, c), np.uint64))
+    return res
+
+
+def _sub_batches(n, sub_batch, step):
+    """Run step(i0, kk) over streams i0 .. i0 + kk of n, at most ``sub_batch`` streams at a time (None: all; less than 1: 1),
+    halving kk while the step raises a DivansError that it cannot allocate.  Any other error, and that one at kk = 1, is
+    raised.  Returns the number of sub-batches run."""
+    m = n if sub_batch is None else max(1, int(sub_batch))
+    i0 = runs = 0
+    while i0 < n:
+        kk = min(m, n - i0)
+        try:
+            step(i0, kk)
+        except DivansError as e:
+            if kk == 1 or not ("cannot allocate" in str(e) or "out of memory" in str(e)):
+                raise
+            m = kk // 2   # what kk streams need did not fit next to what the GPU holds
+            continue
+        i0 += kk
+        runs += 1
+    return runs
+
+
 def ir_to_cmds(text):
     """Reference IR text (src/bin/divans.rs:191-483) -> (DVCL command-list blob, window size).  Host-side parser of the
     C ABI (divans_b200_ir_to_cmds); feed the blob to ``Engine.encode(..., cmds=True)``."""
@@ -294,19 +359,26 @@ def kernel_version():
     return load_library().divans_b200_kernel_version().decode()
 
 
-def _parse(parse):
-    """(min_match, lazy) -> a Lz77Parse, (min_match, lazy, dict_min) -> a Lz77DictParse (the C calls refuse one outside
-    min_match 4..32, lazy 0..2, dict_min 0 or 4..32)"""
+def _lz77_call(L, parse, device):
+    """The LZ77 generator call ``parse`` selects and the arguments it takes after the batch's: None -> the plain call;
+    (min_match, lazy) -> the _parse call and a Lz77Parse; (min_match, lazy, dict_min) -> the _dict call and a Lz77DictParse.
+    The host call refuses a parse outside min_match 4..32, lazy 0..2, dict_min 0 or 4..32 here (ValueError); the device call
+    passes it on to the library, which refuses it."""
+    name = "divans_b200_lz77_cmds_batch" + ("_device" if device else "")
+    if parse is None:
+        return getattr(L, name), ()
     if len(parse) == 3:
         mm, lz, dm = parse
-        return Lz77DictParse(int(mm), int(lz), int(dm), 0)
-    mm, lz = parse
-    return Lz77Parse(int(mm), int(lz))
-
-
-def _parse_ok(ps):
-    ok = 4 <= ps.min_match <= 32 and 0 <= ps.lazy <= 2
-    return ok and (not isinstance(ps, Lz77DictParse) or ps.dict_min == 0 or 4 <= ps.dict_min <= 32)
+        ps, name = Lz77DictParse(int(mm), int(lz), int(dm), 0), name + "_dict"
+        ok = ps.dict_min == 0 or 4 <= ps.dict_min <= 32
+        what = "(%d, %d, %d) is outside min_match 4..32, lazy 0..2, dict_min 0 or 4..32" % (ps.min_match, ps.lazy, ps.dict_min)
+    else:
+        mm, lz = parse
+        ps, name, ok = Lz77Parse(int(mm), int(lz)), name + "_parse", True
+        what = "(%d, %d) is outside min_match 4..32, lazy 0..2" % (ps.min_match, ps.lazy)
+    if not device and not (ok and 4 <= ps.min_match <= 32 and 0 <= ps.lazy <= 2):
+        raise ValueError("lz77_cmds_batch: parse " + what)
+    return getattr(L, name), (ctypes.byref(ps),)
 
 
 def lz77_cmds_batch(blob, in_off, in_len, window=16, pred_mode=2, mixing_value=4, n_threads=None, parse=None):
@@ -314,18 +386,8 @@ def lz77_cmds_batch(blob, in_off, in_len, window=16, pred_mode=2, mixing_value=4
     (blobs uint8 array, blob_off, blob_len) ready for Engine.encode_batch_host(..., cmds=True).  ``parse`` (min_match, lazy):
     the parse of divans_b200_lz77_cmds_batch_parse (include/divans_b200.h); None is (4, 0).  (min_match, lazy, dict_min): the
     parse with dictionary words of divans_b200_lz77_cmds_batch_dict."""
-    L = load_library()
-    if parse is not None:
-        ps = _parse(parse)
-        if not _parse_ok(ps):
-            if isinstance(ps, Lz77DictParse):
-                raise ValueError("lz77_cmds_batch: parse (%d, %d, %d) is outside min_match 4..32, lazy 0..2, dict_min 0 or 4..32"
-                                 % (ps.min_match, ps.lazy, ps.dict_min))
-            raise ValueError("lz77_cmds_batch: parse (%d, %d) is outside min_match 4..32, lazy 0..2" % (ps.min_match, ps.lazy))
-        f = L.divans_b200_lz77_cmds_batch_dict if isinstance(ps, Lz77DictParse) else L.divans_b200_lz77_cmds_batch_parse
-        fn = lambda *a: f(*a, ctypes.byref(ps))
-    else:
-        fn = L.divans_b200_lz77_cmds_batch
+    f, ps = _lz77_call(load_library(), parse, False)
+    fn = lambda *a: f(*a, *ps)
     blob = _u8(blob)
     in_off, in_len = np.ascontiguousarray(in_off, np.uint64), np.ascontiguousarray(in_len, np.uint64)
     n = len(in_off)
@@ -806,18 +868,14 @@ class Engine:
         out_cap = np.array(out_caps, np.uint64).reshape(n)
         o = opts if opts is not None else encode_options(window_size=0)
         dev = d_in.device
-        # the calls run on a stream of their own, ordered after the work already queued on `stream` (a default stream has no
-        # handle the library could take: NULL would mean the context's stream)
-        caller = stream if stream is not None else torch.cuda.current_stream(dev)
-        s = torch.cuda.Stream(dev)
-        s.wait_stream(caller)
-        u64 = lambda a: torch.from_numpy(np.ascontiguousarray(a, np.uint64).view(np.int64)).to(dev, non_blocking=False)
         self.last_transcode_retried = 0
         auto = candidates is not None
         nc = len(candidates) if auto else 0
         if n == 0:
-            empty = torch.zeros(0, dtype=torch.uint8, device=dev), np.zeros(0, np.uint64), np.zeros(0, np.uint64), np.zeros(0, np.int32)
-            return empty + (np.zeros(0, np.uint32), np.zeros((0, nc), np.uint64)) if auto else empty
+            return _empty_result(dev, nc if auto else None)
+        caller, s = _private_stream(dev, stream)
+        # a pass's results; status holds the decode statuses, then the encode statuses
+        cols = dict(out_len=1, blob_len=1, new_len=1, status=1, **(dict(cost=nc, chosen=1) if auto else {}))
 
         def run(idx, blob_cap, d_new=None):
             """decode + encode of streams idx on the device, one synchronisation: (d_new, new_off, new_len, status, blob_len,
@@ -828,36 +886,34 @@ class Engine:
             new_cap = _encoded_cap(bcap)
             (out_off, out_total), (blob_off, blobs_total), (new_off, new_total) = _regions(ocap), _regions(bcap), _regions(new_cap)
             with torch.cuda.stream(s):
-                d_meta = u64(np.concatenate([in_off[idx], in_len[idx], out_off, ocap, blob_off, bcap, new_off, new_cap]))
+                d_meta = _u64(np.concatenate([in_off[idx], in_len[idx], out_off, ocap, blob_off, bcap, new_off, new_cap]), dev)
                 M = [d_meta[k * m:(k + 1) * m] for k in range(8)]
                 d_out = torch.empty(out_total, dtype=torch.uint8, device=dev)
                 d_blobs = torch.empty(blobs_total, dtype=torch.uint8, device=dev)
                 if d_new is None:
                     d_new = torch.empty(new_total, dtype=torch.uint8, device=dev)
-                # out_len | blob_len | new_len | both statuses (| candidates: cost [m * C] | chosen)
-                d_res = torch.zeros((4 + (nc + 1 if auto else 0)) * m, dtype=torch.int64, device=dev)
-                d_st = d_res[3 * m:4 * m].view(torch.int32)
+                d_res = torch.zeros(sum(cols.values()) * m, dtype=torch.int64, device=dev)
+                D = _columns(d_res, m, cols)
+                d_st = D["status"].view(torch.int32)
                 d_dec_st, d_enc_st = d_st[:m], d_st[m:]
                 self.decode_cmds_batch_device(d_in.data_ptr(), M[0].data_ptr(), M[1].data_ptr(), d_out.data_ptr(), M[2].data_ptr(), M[3].data_ptr(),
-                                              d_res.data_ptr(), d_blobs.data_ptr(), M[4].data_ptr(), M[5].data_ptr(), d_res[m:].data_ptr(),
-                                              d_dec_st.data_ptr(), m, int(in_len[idx].sum()), flags, s.cuda_stream)
+                                              D["out_len"].data_ptr(), d_blobs.data_ptr(), M[4].data_ptr(), M[5].data_ptr(),
+                                              D["blob_len"].data_ptr(), d_dec_st.data_ptr(), m, int(in_len[idx].sum()), flags, s.cuda_stream)
                 # a stream that did not decode reaches the encoder with no blob (status 2's blob_len is larger than its region)
-                d_enc_len = torch.where(d_dec_st == 0, d_res[m:2 * m], torch.zeros_like(d_res[m:2 * m]))
+                d_enc_len = torch.where(d_dec_st == 0, D["blob_len"], torch.zeros_like(D["blob_len"]))
                 enc = (m, d_blobs.data_ptr(), M[4].data_ptr(), d_enc_len.data_ptr(), int(bcap.max()), int(ocap.max()), d_new.data_ptr(),
-                       M[6].data_ptr(), M[7].data_ptr(), d_res[2 * m:].data_ptr(), d_enc_st.data_ptr())
+                       M[6].data_ptr(), M[7].data_ptr(), D["new_len"].data_ptr(), d_enc_st.data_ptr())
                 if auto:
-                    self.encode_cmds_auto_batch_device(*enc, d_res[(4 + nc) * m:].data_ptr(), d_res[4 * m:(4 + nc) * m].data_ptr(), o,
-                                                       candidates, s.cuda_stream)
+                    self.encode_cmds_auto_batch_device(*enc, D["chosen"].data_ptr(), D["cost"].data_ptr(), o, candidates, s.cuda_stream)
                 else:
                     self.encode_cmds_batch_device(*enc, o, s.cuda_stream)
-                res = d_res.cpu()   # (the one synchronisation of the pass)
-            r = res.numpy()
-            st = r[3 * m:4 * m].view(np.int32)
+                R = _columns(d_res.cpu().numpy(), m, cols)   # (the one synchronisation of the pass)
+            st = R["status"].view(np.int32)
             dec_st, enc_st = st[:m], st[m:]
-            chosen = r[(4 + nc) * m:].view(np.uint32)[:m].copy() if auto else None
-            cost = r[4 * m:(4 + nc) * m].view(np.uint64).reshape(m, nc).copy() if auto else None
-            return d_new, new_off, r[2 * m:3 * m].view(np.uint64).copy(), np.where(dec_st != 0, dec_st, enc_st).astype(np.int32), \
-                r[m:2 * m].view(np.uint64).copy(), dec_st.copy(), chosen, cost
+            chosen = R["chosen"].view(np.uint32)[:m].copy() if auto else None
+            cost = R["cost"].view(np.uint64).reshape(m, nc).copy() if auto else None
+            return d_new, new_off, R["new_len"].view(np.uint64).copy(), np.where(dec_st != 0, dec_st, enc_st).astype(np.int32), \
+                R["blob_len"].view(np.uint64).copy(), dec_st.copy(), chosen, cost
 
         cap1 = first_blob_cap(out_cap)
         d_new, new_off, new_len, status, blob_len, dec_st, chosen, cost = run(np.arange(n), cap1)
@@ -877,8 +933,7 @@ class Engine:
             new_len[retry], status[retry] = len2, st2
             if auto:
                 chosen[retry], cost[retry] = ch2, co2
-        caller.wait_stream(s)
-        d_new.record_stream(caller)   # (allocated on the private stream, used on the caller's from here on)
+        _hand_back(caller, s, d_new)
         return (d_new, new_off, new_len, status, chosen, cost) if auto else (d_new, new_off, new_len, status)
 
     # -- generating LZ77 command lists on the GPU (include/divans_b200.h, divans_b200_lz77_cmds_batch_device)
@@ -890,14 +945,9 @@ class Engine:
         or >= 2**31).  Asynchronous on ``stream``; regions are not cleared first.  ``parse`` (min_match, lazy) as for
         lz77_cmds_batch (divans_b200_lz77_cmds_batch_device_parse); None is (4, 0).  (min_match, lazy, dict_min): with dictionary
         words (divans_b200_lz77_cmds_batch_device_dict)."""
-        args = (self._h, n, d_in, d_in_off, d_in_len, int(max_in_len), int(window), int(pred_mode), int(mixing_value), d_blobs, d_blob_off,
-                d_blob_cap, d_blob_len, d_status)
-        if parse is None:
-            rc = self._L.divans_b200_lz77_cmds_batch_device(*args, stream)
-        else:
-            ps = _parse(parse)
-            f = self._L.divans_b200_lz77_cmds_batch_device_dict if isinstance(ps, Lz77DictParse) else self._L.divans_b200_lz77_cmds_batch_device_parse
-            rc = f(*args, ctypes.byref(ps), stream)
+        f, ps = _lz77_call(self._L, parse, True)
+        rc = f(self._h, n, d_in, d_in_off, d_in_len, int(max_in_len), int(window), int(pred_mode), int(mixing_value), d_blobs, d_blob_off,
+               d_blob_cap, d_blob_len, d_status, *ps, stream)
         if rc != DIVANS_SUCCESS:
             raise DivansError("lz77_cmds_batch_device: " + self._err())
 
@@ -934,160 +984,75 @@ class Engine:
         n = len(in_off)
         in_off, in_len = np.ascontiguousarray(in_off, np.uint64).reshape(n), np.ascontiguousarray(in_len, np.uint64).reshape(n)
         o = opts if opts is not None else encode_options(window_size=0)
-        if parses is not None:
-            return self._compress_parses(d_in, in_off, in_len, window, pred_mode, mixing_value, o, candidates, stream, sub_batch, list(parses))
-        auto = candidates is not None
-        nc = len(candidates) if auto else 0
-        dev = d_in.device
-        if n == 0:
-            empty = torch.zeros(0, dtype=torch.uint8, device=dev), np.zeros(0, np.uint64), np.zeros(0, np.uint64), np.zeros(0, np.int32)
-            return empty + (np.zeros(0, np.uint32), np.zeros((0, nc), np.uint64)) if auto else empty
-        caller = stream if stream is not None else torch.cuda.current_stream(dev)
-        s = torch.cuda.Stream(dev)
-        s.wait_stream(caller)
-        u64 = lambda a: torch.from_numpy(np.ascontiguousarray(a, np.uint64).view(np.int64)).to(dev, non_blocking=False)
-        max_in = int(in_len.max())
-        bcap = lz77_blob_cap(in_len)
-        blob_off, blob_total = _regions(bcap)
-        with torch.cuda.stream(s):
-            d_meta = u64(np.concatenate([in_off, in_len, blob_off, bcap]))
-            M = [d_meta[k * n:(k + 1) * n] for k in range(4)]
-            d_blobs = torch.empty(blob_total, dtype=torch.uint8, device=dev)
-            d_gen = torch.zeros(2 * n, dtype=torch.int64, device=dev)   # blob_len | status (int32 pairs)
-            self.lz77_cmds_batch_device(n, d_in.data_ptr(), M[0].data_ptr(), M[1].data_ptr(), max_in, window, pred_mode, mixing_value,
-                                        d_blobs.data_ptr(), M[2].data_ptr(), M[3].data_ptr(), d_gen.data_ptr(), d_gen[n:].data_ptr(),
-                                        s.cuda_stream)
-            g = d_gen.cpu().numpy()   # (the synchronisation that reads the blob lengths)
-        gen_st = g[n:].view(np.int32)[:n].copy()
-        blob_len = np.where(gen_st == 0, g[:n].view(np.uint64), np.uint64(0))
-        new_cap = _encoded_cap(blob_len)
-        new_off, new_total = _regions(new_cap)
-        max_blob = int(blob_len.max())
-        with torch.cuda.stream(s):
-            d_enc = u64(np.concatenate([blob_len, new_off, new_cap]))
-            d_new = torch.empty(new_total, dtype=torch.uint8, device=dev)
-            # new_len | status (| candidates: cost [n * C] | chosen)
-            d_res = torch.zeros((2 + (nc + 1 if auto else 0)) * n, dtype=torch.int64, device=dev)
-            m = n if sub_batch is None else max(1, int(sub_batch))
-            i0 = 0
-            self.last_compress_sub_batches = 0   # (encode launches of the most recent call)
-            while i0 < n:
-                k = min(m, n - i0)
-                at = lambda t, esz=8: t.data_ptr() + i0 * esz
-                enc = (k, d_blobs.data_ptr(), at(M[2]), at(d_enc[:n]), max_blob, max_in, d_new.data_ptr(), at(d_enc[n:2 * n]),
-                       at(d_enc[2 * n:]), at(d_res), at(d_res[n:], 4))
-                try:
-                    if auto:
-                        self.encode_cmds_auto_batch_device(*enc, at(d_res[(2 + nc) * n:], 4), at(d_res[2 * n:], 8 * nc), o, candidates,
-                                                           s.cuda_stream)
-                    else:
-                        self.encode_cmds_batch_device(*enc, o, s.cuda_stream)
-                except DivansError as e:
-                    if k == 1 or not ("cannot allocate" in str(e) or "out of memory" in str(e)):
-                        raise
-                    m = k // 2   # the logs of k streams did not fit next to what the GPU holds
-                    continue
-                i0 += k
-                self.last_compress_sub_batches += 1
-            r = d_res.cpu().numpy()
-        enc_st = r[n:2 * n].view(np.int32)[:n]
-        status = np.where(gen_st != 0, gen_st, enc_st).astype(np.int32)
-        new_len = r[:n].view(np.uint64).copy()
-        caller.wait_stream(s)
-        d_new.record_stream(caller)   # (allocated on the private stream, used on the caller's from here on)
-        if auto:
-            chosen = r[(2 + nc) * n:].view(np.uint32)[:n].copy()
-            cost = r[2 * n:(2 + nc) * n].view(np.uint64).reshape(n, nc).copy()
-            return d_new, new_off, new_len, status, chosen, cost
-        return d_new, new_off, new_len, status
-
-    def _compress_parses(self, d_in, in_off, in_len, window, pred_mode, mixing_value, o, candidates, stream, sub_batch, parses):
-        """compress_device with ``parses``: k lists per stream, candidate-major (list c of stream i is list v = c * n + i), in
-        regions of lz77_blob_cap each; one synchronisation reads their lengths; then each sub-batch chooses and encodes."""
-        import torch
-        n, k = len(in_off), len(parses)
+        choose, auto = parses is not None, candidates is not None
+        lists = list(parses) if choose else [None]   # a stream's lists: one per parse, or the generator's own
+        k, nc = len(lists), len(candidates) if auto else 0
         if not 1 <= k <= 16:
             raise ValueError("compress_device: 1..16 parses are required")
-        auto = candidates is not None
-        nc = len(candidates) if auto else 0
         dev = d_in.device
         if n == 0:
-            empty = torch.zeros(0, dtype=torch.uint8, device=dev), np.zeros(0, np.uint64), np.zeros(0, np.uint64), np.zeros(0, np.int32)
-            return empty + ((np.zeros(0, np.uint32), np.zeros((0, nc), np.uint64)) if auto else ()) + \
-                (np.zeros(0, np.uint32), np.zeros((0, k), np.uint64))
-        caller = stream if stream is not None else torch.cuda.current_stream(dev)
-        s = torch.cuda.Stream(dev)
-        s.wait_stream(caller)
-        u64 = lambda a: torch.from_numpy(np.ascontiguousarray(a, np.uint64).view(np.int64)).to(dev, non_blocking=False)
+            return _empty_result(dev, nc if auto else None, k if choose else None)
+        caller, s = _private_stream(dev, stream)
         max_in = int(in_len.max())
+        # k lists per stream, candidate-major (list c of stream i is list c * n + i), in regions of lz77_blob_cap each
         bcap = np.tile(lz77_blob_cap(in_len), k)
         blob_off, blob_total = _regions(bcap)
+        gen = dict(blob_len=k, status=k)
         with torch.cuda.stream(s):
-            d_meta = u64(np.concatenate([in_off, in_len, blob_off, bcap]))
-            d_in_off, d_in_len, d_boff, d_bcap = d_meta[:n], d_meta[n:2 * n], d_meta[2 * n:2 * n + k * n], d_meta[2 * n + k * n:]
+            M = _columns(_u64(np.concatenate([in_off, in_len, blob_off, bcap]), dev), n, dict(in_off=1, in_len=1, blob_off=k, blob_cap=k))
             d_blobs = torch.empty(blob_total, dtype=torch.uint8, device=dev)
-            d_gen = torch.zeros(2 * k * n, dtype=torch.int64, device=dev)   # blob_len [k * n] | status (int32 pairs)
-            for c, ps in enumerate(parses):
+            d_gen = torch.zeros(sum(gen.values()) * n, dtype=torch.int64, device=dev)
+            G = _columns(d_gen, n, gen)
+            for c, ps in enumerate(lists):
                 v = c * n
-                self.lz77_cmds_batch_device(n, d_in.data_ptr(), d_in_off.data_ptr(), d_in_len.data_ptr(), max_in, window, pred_mode, mixing_value,
-                                            d_blobs.data_ptr(), d_boff[v:].data_ptr(), d_bcap[v:].data_ptr(), d_gen[v:].data_ptr(),
-                                            d_gen[k * n:].data_ptr() + 4 * v, s.cuda_stream, parse=ps)
-            g = d_gen.cpu().numpy()   # (the synchronisation that reads the blob lengths)
-        gen_st = g[k * n:].view(np.int32)[:k * n].reshape(k, n)
-        blob_len = np.where(gen_st == 0, g[:k * n].view(np.uint64).reshape(k, n), np.uint64(0))
+                self.lz77_cmds_batch_device(n, d_in.data_ptr(), M["in_off"].data_ptr(), M["in_len"].data_ptr(), max_in, window, pred_mode,
+                                            mixing_value, d_blobs.data_ptr(), M["blob_off"][v:].data_ptr(), M["blob_cap"][v:].data_ptr(),
+                                            G["blob_len"][v:].data_ptr(), G["status"].data_ptr() + 4 * v, s.cuda_stream, parse=ps)
+            G = _columns(d_gen.cpu().numpy(), n, gen)   # (the synchronisation that reads the blob lengths)
+        gen_st = G["status"].view(np.int32)[:k * n].reshape(k, n)
+        blob_len = np.where(gen_st == 0, G["blob_len"].view(np.uint64).reshape(k, n), np.uint64(0))
         gen_st = np.where((gen_st != 0).any(axis=0), gen_st.max(axis=0), 0).astype(np.int32)   # (a refusal refuses every parse)
         new_cap = _encoded_cap(blob_len.max(axis=0))
         new_off, new_total = _regions(new_cap)
         max_blob = int(blob_len.max())
-        boff2 = blob_off.reshape(k, n)
+        cols = dict(new_len=1, status=1, **(dict(cost=nc, chosen=1) if auto else {}), **(dict(parse_cost=k, chosen_parse=1) if choose else {}))
         with torch.cuda.stream(s):
-            d_enc = u64(np.concatenate([new_off, new_cap]))
+            E = _columns(_u64(np.concatenate([blob_len.reshape(-1), new_off, new_cap]), dev), n, dict(blob_len=k, new_off=1, new_cap=1))
             d_new = torch.empty(new_total, dtype=torch.uint8, device=dev)
-            # new_len | status | parse cost [n * k] | chosen parse (| candidates: cost [n * C] | chosen)
-            d_res = torch.zeros((2 + k + 1 + (nc + 1 if auto else 0)) * n, dtype=torch.int64, device=dev)
-            d_pcost, d_pch = d_res[2 * n:(2 + k) * n], d_res[(2 + k) * n:(3 + k) * n]
-            d_cost, d_ch = d_res[(3 + k) * n:(3 + k + nc) * n], d_res[(3 + k + nc) * n:]
-            m = n if sub_batch is None else max(1, int(sub_batch))
-            i0 = 0
-            self.last_compress_sub_batches = 0
-            while i0 < n:
-                kk = min(m, n - i0)
+            d_res = torch.zeros(sum(cols.values()) * n, dtype=torch.int64, device=dev)
+            D = _columns(d_res, n, cols)
+
+            def step(i0, kk):
                 at = lambda t, esz=8: t.data_ptr() + i0 * esz
-                # the sub-batch's lists, candidate-major
-                d_sub = u64(np.concatenate([boff2[:, i0:i0 + kk].reshape(-1), blob_len[:, i0:i0 + kk].reshape(-1)]))
-                try:
-                    if auto:
-                        self.encode_cmds_choose_batch_device(kk, k, d_blobs.data_ptr(), d_sub.data_ptr(), d_sub[k * kk:].data_ptr(), max_blob, max_in,
-                                                             None, None, None, None, None, at(d_pch, 4), at(d_pcost, 8 * k), o, s.cuda_stream)
-                        ch = d_pch.view(torch.int32)[i0:i0 + kk].long()
-                        d_pick = torch.cat([d_sub[:k * kk].view(k, kk).gather(0, ch[None])[0], d_sub[k * kk:].view(k, kk).gather(0, ch[None])[0]])
-                        self.encode_cmds_auto_batch_device(kk, d_blobs.data_ptr(), d_pick.data_ptr(), d_pick[kk:].data_ptr(), max_blob, max_in,
-                                                           d_new.data_ptr(), at(d_enc[:n]), at(d_enc[n:]), at(d_res), at(d_res[n:], 4), at(d_ch, 4),
-                                                           at(d_cost, 8 * nc), o, candidates, s.cuda_stream)
-                    else:
-                        self.encode_cmds_choose_batch_device(kk, k, d_blobs.data_ptr(), d_sub.data_ptr(), d_sub[k * kk:].data_ptr(), max_blob, max_in,
-                                                             d_new.data_ptr(), at(d_enc[:n]), at(d_enc[n:]), at(d_res), at(d_res[n:], 4),
-                                                             at(d_pch, 4), at(d_pcost, 8 * k), o, s.cuda_stream)
-                except DivansError as e:
-                    if kk == 1 or not ("cannot allocate" in str(e) or "out of memory" in str(e)):
-                        raise
-                    m = kk // 2   # the logs of kk streams (and the slots of their kk * k pairs) did not fit next to what the GPU holds
-                    continue
-                i0 += kk
-                self.last_compress_sub_batches += 1
-            r = d_res.cpu().numpy()
-        enc_st = r[n:2 * n].view(np.int32)[:n]
-        status = np.where(gen_st != 0, gen_st, enc_st).astype(np.int32)
-        new_len = r[:n].view(np.uint64).copy()
-        caller.wait_stream(s)
-        d_new.record_stream(caller)   # (allocated on the private stream, used on the caller's from here on)
-        chosen_parse = r[(2 + k) * n:(3 + k) * n].view(np.uint32)[:n].copy()
-        parse_cost = r[2 * n:(2 + k) * n].view(np.uint64).reshape(n, k).copy()
+                # the sub-batch's lists, candidate-major: at k = 1, or in one sub-batch, views of the batch's
+                boff, blen = (t.view(k, n)[:, i0:i0 + kk].contiguous() for t in (M["blob_off"], E["blob_len"]))
+                out = (d_new.data_ptr(), at(E["new_off"]), at(E["new_cap"]), at(D["new_len"]), at(D["status"], 4))
+                if choose:
+                    pick = (at(D["chosen_parse"], 4), at(D["parse_cost"], 8 * k), o, s.cuda_stream)
+                    if not auto:
+                        self.encode_cmds_choose_batch_device(kk, k, d_blobs.data_ptr(), boff.data_ptr(), blen.data_ptr(), max_blob, max_in,
+                                                             *out, *pick)
+                        return
+                    # the choice only, then the literal model is chosen on each stream's chosen list
+                    self.encode_cmds_choose_batch_device(kk, k, d_blobs.data_ptr(), boff.data_ptr(), blen.data_ptr(), max_blob, max_in,
+                                                         None, None, None, None, None, *pick)
+                    ch = D["chosen_parse"].view(torch.int32)[i0:i0 + kk].long()[None]
+                    boff, blen = boff.gather(0, ch)[0], blen.gather(0, ch)[0]
+                enc = (kk, d_blobs.data_ptr(), boff.data_ptr(), blen.data_ptr(), max_blob, max_in, *out)
+                if auto:
+                    self.encode_cmds_auto_batch_device(*enc, at(D["chosen"], 4), at(D["cost"], 8 * nc), o, candidates, s.cuda_stream)
+                else:
+                    self.encode_cmds_batch_device(*enc, o, s.cuda_stream)
+
+            self.last_compress_sub_batches = _sub_batches(n, sub_batch, step)   # (encode launches of the most recent call)
+            R = _columns(d_res.cpu().numpy(), n, cols)
+        _hand_back(caller, s, d_new)
+        res = d_new, new_off, R["new_len"].view(np.uint64).copy(), np.where(gen_st != 0, gen_st, R["status"].view(np.int32)[:n]).astype(np.int32)
         if auto:
-            chosen = r[(3 + k + nc) * n:].view(np.uint32)[:n].copy()
-            cost = r[(3 + k) * n:(3 + k + nc) * n].view(np.uint64).reshape(n, nc).copy()
-            return d_new, new_off, new_len, status, chosen, cost, chosen_parse, parse_cost
-        return d_new, new_off, new_len, status, chosen_parse, parse_cost
+            res += (R["chosen"].view(np.uint32)[:n].copy(), R["cost"].view(np.uint64).reshape(n, nc).copy())
+        if choose:
+            res += (R["chosen_parse"].view(np.uint32)[:n].copy(), R["parse_cost"].view(np.uint64).reshape(n, k).copy())
+        return res
 
     # -- replaying command lists to raw bytes (include/divans_b200.h, divans_b200_replay_cmds_batch_*)
     def replay_cmds_batch_host(self, blobs, blob_off, blob_len, out, out_off, out_cap, window_size=0):
