@@ -659,7 +659,8 @@ __device__ __forceinline__ bool literal_fast_v2(St &s, Next &nx, const G2 g, con
 //     symbol 65534 and moves that of symbol 65535 behind its own words (ans.rs:230-244).
 // The run proper, out of line: the command path that shares the kernel is instruction-fetch bound (DESIGN section 4), and the
 // loop inlined into the main loop made LZ77 command streams slower.  Everything crosses the call by value, so that the caller's
-// St stays in registers.  Returns the coder (lazy form) and the next mixing value.
+// St stays in registers.  Returns the coder (lazy form) and the next mixing value.  mixval_run_v2 is the loop of 8 lanes per
+// stream; 16 lanes per stream take mixval_run16 (below).
 struct MixvalRun { Coder k; uint32_t f1; };
 template <int LPG>
 static __device__ __noinline__ MixvalRun mixval_run_v2(Coder k, const uint32_t f1, const uint32_t n, uint8_t *const slot, const bool rev,
@@ -717,6 +718,85 @@ static __device__ __noinline__ MixvalRun mixval_run_v2(Coder k, const uint32_t f
     coder_from_eager(k, f);
     return MixvalRun{k, f1 + n};
 }
+// The same run at 16 lanes per stream, in trips of at most 16 values:
+//   * the states are split as in the literal loops (rans_split16): `x` is `a` on lanes 0-7 and `b` on lanes 8-15, and one
+//     split step advances a pair of values, 2j on `a` (its prior) and 2j + 1 on `b` (the prior after the first blend);
+//   * where the run ends is found once per trip: lane j of a group loads the mixing value of value i + 1 + j, and one ballot
+//     gives the first value, in any group, whose prior is not the run's;
+//   * lanes 2j and 2j + 1 keep the symbols of pair j of the trip, and the group stores the trip's values with one byte store
+//     per lane;
+//   * the prior stays in registers for the whole run and is stored once, when the run ends (nothing else reads it meanwhile).
+// The trip reads mixing values 240 to 255 values behind the value being coded; only the trip's own values (at most 16) are
+// still in registers, so every byte it reads has been stored.
+constexpr uint32_t MV_TRIP = 16;
+static_assert(MV_TRIP <= 16 && 2 * MV_TRIP < 256, "one lane per value of a trip; the lookahead must not reach a value still in registers");
+static __device__ __noinline__ MixvalRun mixval_run16(Coder k, const uint32_t f1, const uint32_t n, uint8_t *const slot, const bool rev,
+                                                      const G2 g, const bool active) {
+    const int li = g.l16;
+    FastK f;
+    f.inc = (int)(short)(SPK_PLANE & 0xffff); f.lim = SPK_PLANE >> 16;
+    f.incp = 0; f.kp = (uint32_t)(li + 1); f.mytag = 0;
+    const uint32_t bsel = 0xffffu << g.shift;
+    const uint32_t slot_lo = (uint32_t)(uintptr_t)slot, slot_hi = (uint32_t)((uintptr_t)slot >> 32);
+    const uint32_t pbase = slot_lo + (uint32_t)OFF_MISC + (uint32_t)(MI_PRED + PM_MIXING_VALUE) * CDF_BYTES, mixb = slot_lo + (uint32_t)OFF_MIX;
+    const auto mix = [slot_hi, mixb](uint32_t v) { return ld_u8g(mk_ptr(mixb + v, slot_hi)); };
+    // element 15 after a blend: the new max (lane 15's blend_v2)
+    const auto next_max = [&f](const uint32_t mv) {
+        uint32_t nm = mv + (uint32_t)f.inc;
+        if ((int)nm >= f.lim) { const uint32_t u = nm + 16u; nm = u - (u >> 2); }
+        return nm;
+    };
+    coder_to_eager(k, f, slot, active);
+    if (g.store0 && active && f1 == 0) reinterpret_cast<uint32_t *>(slot + OFF_HDR)[3] = 1u;   // the mask is about to hold this stream's values
+    const bool bl = li >= 8;
+    const uint32_t hsel = bl ? 0x4432u : 0x4410u;
+    uint64_t x = bl ? k.b : k.a;
+    uint32_t i = 0;
+    while (i < n) {
+        const uint32_t pi = mixval_prior(f1 + i, rev, mix);
+        const uint32_t pa = pbase + pi * CDF_BYTES;
+        __syncwarp();                                                    // (the other lanes' stores: mixing values, the prior)
+        const char *const pe = mk_ptr(pa + 2u * li, slot_hi);
+        uint32_t ev = ld_u16g(pe), mv = ld_u16g(mk_ptr(pa + 30u, slot_hi));
+        bool more;
+        do {
+            const unsigned c = __ballot_sync(FULL, mixval_prior(f1 + i + 1 + li, rev, mix) != pi);
+            const uint32_t cg = (c | (c >> 16)) & 0xffffu;               // first set bit j: value i + 1 + j takes another prior
+            const uint32_t m = min((uint32_t)__ffs(cg | (1u << (MV_TRIP - 1))), n - i);   // (no bit below: a whole trip)
+            more = cg == 0 && i + m < n;
+            uint32_t ms = 0;
+            for (uint32_t j = 0; 2 * j + 1 < m; j++) {
+                const uint32_t xm = (uint32_t)x & 0x7fffu;
+                const uint32_t oa = __shfl_sync(FULL, xm, 0, 16), ob = __shfl_sync(FULL, xm, 8, 16);
+                const int sa = search_off_v2<16>(oa, ev, mv, bsel);
+                const uint32_t e1 = blend_v2<16>(ev, mv, sa, g, f), m1 = next_max(mv);
+                const int sb = search_off_v2<16>(ob, e1, m1, bsel);
+                const uint32_t e2 = blend_v2<16>(e1, m1, sb, g, f), m2 = next_max(m1);
+                rans_split16(x, ev, mv, sa, e1, m1, sb, bl, hsel, g, f);
+                if ((uint32_t)(li >> 1) == j) ms = (uint32_t)sa | ((uint32_t)sb << 8);   // (the lane's byte is taken at the store)
+                ev = e2; mv = m2;
+            }
+            if (m & 1) {   // the run ends after an odd number of values: the last one on `a`, then the two states swap
+                const uint64_t xs = __shfl_xor_sync(FULL, x, 8), ka = __shfl_sync(FULL, x, 0, 16);
+                const int sa = search_v2<16>(ka, ev, mv, bsel);
+                uint64_t xa = rans_advance_v2<16>(ka, ev, mv, sa);
+                const bool rf = xa < (1ull << 31);
+                if (__any_sync(FULL, rf)) { if (rf) eager_refill(xa, f); }
+                x = bl ? xa : xs;
+                if ((uint32_t)(li >> 1) == (m >> 1)) ms = (uint32_t)sa;
+                ev = blend_v2<16>(ev, mv, sa, g, f); mv = next_max(mv);
+            }
+            if (active && (uint32_t)li < m) st_u8(mk_ptr(mixb + f1 + i + li, slot_hi), ms >> (8 * (li & 1)));
+            __syncwarp();
+            i += m;
+        } while (more);
+        store_elems<16>(pe, 0, ev);                                      // element 15 is the max
+    }
+    k.a = __shfl_sync(FULL, x, 0, 16); k.b = __shfl_sync(FULL, x, 8, 16);
+    k.sym_count += n;
+    coder_from_eager(k, f);
+    return MixvalRun{k, f1 + n};
+}
 // Returns false (nothing done) when some group has fewer than 8 values to go before one of them.
 template <int LPG>
 __device__ __forceinline__ bool mixval_fast_v2(St &s, Next &nx, const G2 g, const bool active) {
@@ -726,7 +806,9 @@ __device__ __forceinline__ bool mixval_fast_v2(St &s, Next &nx, const G2 g, cons
     n = min(n, __shfl_xor_sync(FULL, n, 16));
     if (n < 8) return false;
     // a dummy codes against slot 16 of its own slot
-    const MixvalRun r = mixval_run_v2<LPG>(s.cur, active ? s.f1 : 0u, n, s.slot, !active || s.c->model_rev, g, active);
+    MixvalRun r;
+    if constexpr (LPG == 16) r = mixval_run16(s.cur, active ? s.f1 : 0u, n, s.slot, !active || s.c->model_rev, g, active);
+    else r = mixval_run_v2<LPG>(s.cur, active ? s.f1 : 0u, n, s.slot, !active || s.c->model_rev, g, active);
     if (!active) return true;
     s.cur = r.k; s.f1 = r.f1;
     enter_pm_mixval<false>(s, nx);

@@ -1,8 +1,9 @@
-"""Account for every instruction of the 16-lane T2S plain literal loop of the v2 decoder.
+"""Account for every instruction of the 16-lane T2S plain literal loop, or of the 16-lane mixing-value loop, of the v2 decoder.
 
     python tools/loop_sass.py                 # compiles divans_b200/csrc/dv2_kernels.cu for sm_90a with -lineinfo
     python tools/loop_sass.py --cubin K.cubin # or reads a cubin built from the same sources
     python tools/loop_sass.py --list          # also prints the hot path, one instruction per line
+    python tools/loop_sass.py --mixval        # the pair loop of mixval_run16 instead (two mixing values per iteration)
 
 The loop is `literal_plain_loop_v2<16, true>` (dv2_core.cuh): the plain loop with the context read from T2S in shared
 memory, which the flagship text batch runs for nearly all of its time.  The tool finds it in the SASS of
@@ -11,6 +12,10 @@ loop when one of its frames is a line of the loop's `for` body inlined at the ca
 loop's region runs from the target of its back edge to the back edge.  Inside it, a forward branch that skips code of a
 rare case (a block under `__builtin_expect`, or the eager refill of a rANS state) leaves that code off the hot path: the
 hot path is what one byte costs when every prior carries the stream's tag and neither state needs a payload word.
+
+With --mixval the loop is the pair loop of `mixval_run16`, the out-of-line mixing-value run that `decode_kernel_v2<16>` calls:
+its instructions carry the loop's lines as their outermost frame (the function is not inlined), and its hot path is one pair
+of mixing values with no refill.
 
 It prints the hot path's instruction count per byte, the count per source line of the loop and per opcode class, the
 size of each rare block, and the kernel's registers, stack and local-memory accesses.  Needs only the CUDA toolkit.
@@ -91,14 +96,22 @@ def block_end(src, start):
     raise ValueError("unbalanced braces after line %d" % (start + 1))
 
 
-def source_map(csrc):
-    """1-based lines of dv2_core.cuh: the loop's `for` body, the call that instantiates the T2S loop, the rare lines"""
+# the loops: (function definition, its `for` line, the call that instantiates it -- None: an out-of-line function)
+LOOPS = {
+    "t2s": (r"\bbool literal_plain_loop_v2\(", r"for \(uint32_t i = 0; i < m; i\+\+\)", "literal_plain_loop_v2<LPG, LPG == 16>("),
+    "mixval": (r"\bMixvalRun mixval_run16\(", r"for \(uint32_t j = 0; 2 \* j \+ 1 < m; j\+\+\)", None),
+}
+
+
+def source_map(csrc, loop):
+    """1-based lines of dv2_core.cuh: the loop's `for` body, the call that instantiates it (None: not inlined), the rare lines"""
+    fn_re, for_re, call_s = LOOPS[loop]
     src = open(os.path.join(csrc, CORE)).read().splitlines()
-    fn = next(i for i, s in enumerate(src) if re.search(r"\bbool literal_plain_loop_v2\(", s))
+    fn = next(i for i, s in enumerate(src) if re.search(fn_re, s))
     fn_end = block_end(src, fn)
-    fo = next(i for i in range(fn, fn_end) if re.search(r"for \(uint32_t i = 0; i < m; i\+\+\)", src[i]))
+    fo = next(i for i in range(fn, fn_end) if re.search(for_re, src[i]))
     body = range(fo + 1, block_end(src, fo) + 2)                          # 1-based: the `for` line and its body
-    call = next(i for i, s in enumerate(src) if "literal_plain_loop_v2<LPG, LPG == 16>(" in s) + 1
+    call = next(i for i, s in enumerate(src) if call_s in s) + 1 if call_s else None
     rare = set()
     for i in range(fn, fn_end):
         if "__builtin_expect(" in src[i]:
@@ -111,7 +124,7 @@ def source_map(csrc):
 def loop_frame(frames, body, call):
     """the line of the loop body this instruction is charged to, or None"""
     for f, ln, caller in frames:
-        if f == CORE and ln in body and caller == (CORE, call):
+        if f == CORE and ln in body and caller == ((CORE, call) if call else None):
             return ln
     return None
 
@@ -142,7 +155,9 @@ def main():
     ap.add_argument("--cubin", help="a cubin of dv2_kernels.cu built with -lineinfo (default: compile one)")
     ap.add_argument("--csrc", default=CSRC, help="the sources the cubin is built from (default: this tree's)")
     ap.add_argument("--list", action="store_true", help="print the hot path")
+    ap.add_argument("--mixval", action="store_true", help="the mixing-value pair loop (mixval_run16) instead of the T2S loop")
     a = ap.parse_args()
+    loop = "mixval" if a.mixval else "t2s"
     with tempfile.TemporaryDirectory() as tmp:
         cubin = a.cubin
         if not cubin:
@@ -151,11 +166,11 @@ def main():
         ins, labels = disassemble(cubin)
         res = subprocess.run([os.path.join(CUDA, "bin", "cuobjdump"), "-res-usage", cubin], check=True, capture_output=True,
                              text=True).stdout
-    src, body, call, rare = source_map(a.csrc)
+    src, body, call, rare = source_map(a.csrc, loop)
     idx = {addr: i for i, (addr, _, _) in enumerate(ins)}
     mine = [loop_frame(fr, body, call) is not None for _, _, fr in ins]
     if not any(mine):
-        sys.exit("no instruction of the T2S loop found: was the cubin built with -lineinfo from these sources?")
+        sys.exit("no instruction of the %s loop found: was the cubin built with -lineinfo from these sources?" % loop)
     # the back edge: the shortest backward branch charged to the `for` line itself (the out-of-line divergent paths of the
     # loop's votes and shuffles branch back into it too, but from the lines of those votes)
     best = None
@@ -167,7 +182,7 @@ def main():
         if best is None or i - lo < best[1] - best[0]:
             best = (lo, i)
     if best is None:
-        sys.exit("the back edge of the T2S loop was not found")
+        sys.exit("the back edge of the %s loop was not found" % loop)
     lo, hi = best
     # forward branches that skip a rare block
     skipped, blocks = set(), []
@@ -184,9 +199,15 @@ def main():
             blocks.append((ins[i][0], len(span), sorted({loop_frame(ins[k][2], body, call) or 0 for k in span} - {0})))
     hot = [k for k in range(lo, hi + 1) if k not in skipped]
 
-    print("decode_kernel_v2<16>, T2S plain loop (literal_plain_loop_v2<16, true>): region 0x%04x-0x%04x, %d instructions"
-          % (ins[lo][0], ins[hi][0], hi - lo + 1))
-    print("hot path (tags match, no refill): %d warp instructions per byte (two streams per warp)" % len(hot))
+    if loop == "mixval":
+        print("decode_kernel_v2<16>, mixing-value pair loop (mixval_run16): region 0x%04x-0x%04x, %d instructions"
+              % (ins[lo][0], ins[hi][0], hi - lo + 1))
+        print("hot path (no refill): %d warp instructions per pair of values, %.1f per value (two streams per warp)"
+              % (len(hot), len(hot) / 2))
+    else:
+        print("decode_kernel_v2<16>, T2S plain loop (literal_plain_loop_v2<16, true>): region 0x%04x-0x%04x, %d instructions"
+              % (ins[lo][0], ins[hi][0], hi - lo + 1))
+        print("hot path (tags match, no refill): %d warp instructions per byte (two streams per warp)" % len(hot))
     for addr, n, lines in blocks:
         print("  rare block after the branch at 0x%04x: %3d instructions (loop lines %s)" % (addr, n, ", ".join(map(str, lines))))
     print()
