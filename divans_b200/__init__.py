@@ -54,6 +54,7 @@ BATCH_SYMBOLS = [
     "divans_b200_encode_cmds_speeds_batch_device",
     "divans_b200_lz77_cmds_batch_parse", "divans_b200_lz77_cmds_batch_device_parse", "divans_b200_encode_cmds_choose_batch_device",
     "divans_b200_lz77_cmds_batch_dict", "divans_b200_lz77_cmds_batch_device_dict",
+    "divans_b200_lz77_cmds_batch_words", "divans_b200_lz77_cmds_batch_device_words",
 ]
 PM_RECORD_BYTES = 32 + 16384 + 1024 + 8192   # one prediction-mode record of a DVCL blob (include/divans_b200.h)
 
@@ -120,6 +121,16 @@ class Lz77DictParse(ctypes.Structure):
 # DEFAULT_LZ77_PARSES, then the (min_match, lazy, dict_min) parses with dictionary words that a greedy survey of exact oracle
 # sizes adds (tools/lz77_dict_probe.py --survey, DESIGN.md section 4, "Dictionary words in the LZ77 parse").
 DEFAULT_LZ77_DICT_PARSES = DEFAULT_LZ77_PARSES + [(7, 2, 4), (10, 2, 4)]
+
+
+class Lz77WordsParse(ctypes.Structure):
+    """divans_b200_lz77_words_parse: Lz77DictParse with its candidate transforms (0: the 44-member set, 1: all 121)"""
+    _fields_ = [("min_match", ctypes.c_int32), ("lazy", ctypes.c_int32), ("dict_min", ctypes.c_int32), ("transforms", ctypes.c_int32)]
+
+
+# DEFAULT_LZ77_DICT_PARSES, then the (min_match, lazy, dict_min, transforms) parses a greedy survey of exact oracle sizes adds
+# (tools/lz77_words_probe.py --survey, DESIGN.md section 4, "Dictionary words under every transform").
+DEFAULT_LZ77_WORD_PARSES = DEFAULT_LZ77_DICT_PARSES + [(4, 0, 4, 1), (10, 2, 4, 1)]
 
 
 class CAllocator(ctypes.Structure):
@@ -207,6 +218,10 @@ def load_library():
     L.divans_b200_lz77_cmds_batch_dict.restype = ctypes.c_uint8
     L.divans_b200_lz77_cmds_batch_device_dict.argtypes = L.divans_b200_lz77_cmds_batch_device.argtypes[:-1] + [ctypes.POINTER(Lz77DictParse), vp]
     L.divans_b200_lz77_cmds_batch_device_dict.restype = ctypes.c_uint8
+    L.divans_b200_lz77_cmds_batch_words.argtypes = L.divans_b200_lz77_cmds_batch.argtypes + [ctypes.POINTER(Lz77WordsParse)]
+    L.divans_b200_lz77_cmds_batch_words.restype = ctypes.c_uint8
+    L.divans_b200_lz77_cmds_batch_device_words.argtypes = L.divans_b200_lz77_cmds_batch_device.argtypes[:-1] + [ctypes.POINTER(Lz77WordsParse), vp]
+    L.divans_b200_lz77_cmds_batch_device_words.restype = ctypes.c_uint8
     L.divans_b200_encode_cmds_choose_batch_device.argtypes = [vp, sz, ctypes.c_uint32, vp, vp, vp, ctypes.c_uint64, ctypes.c_uint64, vp, vp, vp,
                                                               vp, vp, ctypes.POINTER(EncodeOptions), vp, vp, vp]
     L.divans_b200_encode_cmds_choose_batch_device.restype = ctypes.c_uint8
@@ -361,13 +376,20 @@ def kernel_version():
 
 def _lz77_call(L, parse, device):
     """The LZ77 generator call ``parse`` selects and the arguments it takes after the batch's: None -> the plain call;
-    (min_match, lazy) -> the _parse call and a Lz77Parse; (min_match, lazy, dict_min) -> the _dict call and a Lz77DictParse.
-    The host call refuses a parse outside min_match 4..32, lazy 0..2, dict_min 0 or 4..32 here (ValueError); the device call
-    passes it on to the library, which refuses it."""
+    (min_match, lazy) -> the _parse call and a Lz77Parse; (min_match, lazy, dict_min) -> the _dict call and a Lz77DictParse;
+    (min_match, lazy, dict_min, transforms) -> the _words call and a Lz77WordsParse.  The host call refuses a parse outside
+    min_match 4..32, lazy 0..2, dict_min 0 or 4..32, transforms 0 or 1 here (ValueError); the device call passes it on to the
+    library, which refuses it."""
     name = "divans_b200_lz77_cmds_batch" + ("_device" if device else "")
     if parse is None:
         return getattr(L, name), ()
-    if len(parse) == 3:
+    if len(parse) == 4:
+        mm, lz, dm, tf = parse
+        ps, name = Lz77WordsParse(int(mm), int(lz), int(dm), int(tf)), name + "_words"
+        ok = (ps.dict_min == 0 or 4 <= ps.dict_min <= 32) and ps.transforms in (0, 1)
+        what = "(%d, %d, %d, %d) is outside min_match 4..32, lazy 0..2, dict_min 0 or 4..32, transforms 0 or 1" % (
+            ps.min_match, ps.lazy, ps.dict_min, ps.transforms)
+    elif len(parse) == 3:
         mm, lz, dm = parse
         ps, name = Lz77DictParse(int(mm), int(lz), int(dm), 0), name + "_dict"
         ok = ps.dict_min == 0 or 4 <= ps.dict_min <= 32
@@ -385,7 +407,8 @@ def lz77_cmds_batch(blob, in_off, in_len, window=16, pred_mode=2, mixing_value=4
     """Raw buffers -> DVCL command lists by the library's greedy LZ77 (divans_b200_lz77_cmds_batch): returns
     (blobs uint8 array, blob_off, blob_len) ready for Engine.encode_batch_host(..., cmds=True).  ``parse`` (min_match, lazy):
     the parse of divans_b200_lz77_cmds_batch_parse (include/divans_b200.h); None is (4, 0).  (min_match, lazy, dict_min): the
-    parse with dictionary words of divans_b200_lz77_cmds_batch_dict."""
+    parse with dictionary words of divans_b200_lz77_cmds_batch_dict.  (min_match, lazy, dict_min, transforms): the parse of
+    divans_b200_lz77_cmds_batch_words, with transforms 1 dictionary words under every transform."""
     f, ps = _lz77_call(load_library(), parse, False)
     fn = lambda *a: f(*a, *ps)
     blob = _u8(blob)
@@ -944,7 +967,7 @@ class Engine:
         blob; 2: the region is too small and d_blob_len[i] is the size needed; 3: refused (misaligned region, in_len > max_in_len
         or >= 2**31).  Asynchronous on ``stream``; regions are not cleared first.  ``parse`` (min_match, lazy) as for
         lz77_cmds_batch (divans_b200_lz77_cmds_batch_device_parse); None is (4, 0).  (min_match, lazy, dict_min): with dictionary
-        words (divans_b200_lz77_cmds_batch_device_dict)."""
+        words (divans_b200_lz77_cmds_batch_device_dict); (min_match, lazy, dict_min, transforms): divans_b200_lz77_cmds_batch_device_words."""
         f, ps = _lz77_call(self._L, parse, True)
         rc = f(self._h, n, d_in, d_in_off, d_in_len, int(max_in_len), int(window), int(pred_mode), int(mixing_value), d_blobs, d_blob_off,
                d_blob_cap, d_blob_len, d_status, *ps, stream)
@@ -976,8 +999,8 @@ class Engine:
         streams each (default all), halved while the encoder cannot allocate them.  Returns (d_new, new_off, new_len, status):
         status[i] is the generator's status where that failed (the list then reaches the encoder with length 0), else the
         encoder's.
-        With ``parses`` (a list of 1..16 (min_match, lazy) pairs or (min_match, lazy, dict_min) triples, e.g. DEFAULT_LZ77_PARSES
-        or DEFAULT_LZ77_DICT_PARSES) the generator makes one list per parse and stream, and encode_cmds_choose_batch_device
+        With ``parses`` (a list of 1..16 (min_match, lazy) pairs, (min_match, lazy, dict_min) triples or (min_match, lazy,
+        dict_min, transforms) 4-tuples, e.g. DEFAULT_LZ77_PARSES, DEFAULT_LZ77_DICT_PARSES or DEFAULT_LZ77_WORD_PARSES) the generator makes one list per parse and stream, and encode_cmds_choose_batch_device
         encodes each stream from the list that codes cheapest under its own record; with ``candidates`` too, the literal model is then chosen on that list (encode_cmds_auto_batch_device).  The call
         then also returns chosen_parse [n] (an index into ``parses``) and parse_cost [n, k] last."""
         import torch

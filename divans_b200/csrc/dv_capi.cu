@@ -91,6 +91,7 @@ struct divans_b200_ctx {
     // (lz_scratch_asked: the request the allocation was made for, which free memory may have cut down to lz_scratch_words)
     int32_t *d_lz_scratch = nullptr; size_t lz_scratch_words = 0, lz_scratch_asked = 0;
     DictIndex *d_dict_index = nullptr;   // the LZ77 generator's dictionary index (dv_dict.h), uploaded by its first dictionary call
+    WordIndex *d_words_index = nullptr;  // its index of every transform (dv_dict.h), uploaded by its first call that needs it
     bool main_end_is_evm1 = false;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr, evm = nullptr, evm1 = nullptr;   // ev0 | frame kernel | evm | decode kernel | ev1
     cudaEvent_t ev_busy = nullptr; bool busy_recorded = false;                 // end of the most recent launch set on any stream
@@ -190,7 +191,7 @@ extern "C" void divans_b200_destroy(divans_b200_ctx *ctx) {
     cudaFree(ctx->d_sf); cudaFree(ctx->d_replay); cudaFree(ctx->d_enc_scratch); cudaFree(ctx->d_records); cudaFree(ctx->d_rcp15);
     cudaFree(ctx->d_cost_tab); cudaFree(ctx->d_auto);
     cudaFree(ctx->d_mix); cudaFree(ctx->d_slot_bins); cudaFree(ctx->d_speeds);
-    cudaFree(ctx->d_lz_scratch); cudaFree(ctx->d_dict_index);
+    cudaFree(ctx->d_lz_scratch); cudaFree(ctx->d_dict_index); cudaFree(ctx->d_words_index);
     for (auto &ln : ctx->lane) {
         free_host_bufs(ln.bufs);
         if (ln.h_res) cudaFreeHost(ln.h_res);
@@ -1450,25 +1451,32 @@ extern "C" DivansResult divans_b200_replay_cmds_batch_host(divans_b200_ctx *ctx,
 // One launch (dv_lz77.cu) over n raw buffers in HBM: the blobs of divans_b200_lz77_cmds_batch.  Like the replay call it uses the
 // context's work counter and timing events only, and its own scratch: 2^15 + max_in_len int32 per warp, kept and grown on demand.
 // The warps are the fewest of n, the context's max_resident and what the scratch allocation holds.
-// The parse (include/divans_b200.h) selects the kernel's lazy steps, its minimum copy and whether it runs the dictionary step;
-// {4, 0, 0} is the plain call.  The dictionary index is built on the host (dv_ir.cpp) and uploaded once per context.
-extern "C" DivansResult divans_b200_lz77_cmds_batch_device_dict(divans_b200_ctx *ctx, size_t n, const uint8_t *d_in, const uint64_t *d_in_off,
-                                                                const uint64_t *d_in_len, uint64_t max_in_len, int32_t window,
-                                                                int32_t pred_mode, int32_t mixing_value, uint8_t *d_blobs,
-                                                                const uint64_t *d_blob_off, const uint64_t *d_blob_cap, uint64_t *d_blob_len,
-                                                                int32_t *d_status, const divans_b200_lz77_dict_parse *parse, void *cuda_stream) try {
+// The parse (include/divans_b200.h) selects the kernel's lazy steps, its minimum copy, whether it runs the dictionary step and
+// under which transforms; {4, 0, 0, 0} is the plain call.  Each dictionary index is built on the host (dv_ir.cpp) and uploaded
+// once per context, by the first call that needs it.
+extern "C" DivansResult divans_b200_lz77_cmds_batch_device_words(divans_b200_ctx *ctx, size_t n, const uint8_t *d_in, const uint64_t *d_in_off,
+                                                                 const uint64_t *d_in_len, uint64_t max_in_len, int32_t window,
+                                                                 int32_t pred_mode, int32_t mixing_value, uint8_t *d_blobs,
+                                                                 const uint64_t *d_blob_off, const uint64_t *d_blob_cap, uint64_t *d_blob_len,
+                                                                 int32_t *d_status, const divans_b200_lz77_words_parse *parse, void *cuda_stream) try {
     if (!ctx) return DIVANS_FAILURE;
     if (!parse) { ctx->err = "lz77_cmds_batch_device: a parse is required"; return DIVANS_FAILURE; }
     if (parse->min_match < 4 || parse->min_match > 32 || parse->lazy < 0 || parse->lazy > 2 ||
-        (parse->dict_min != 0 && (parse->dict_min < 4 || parse->dict_min > 32)) || parse->reserved != 0) {
+        (parse->dict_min != 0 && (parse->dict_min < 4 || parse->dict_min > 32)) || parse->transforms < 0 || parse->transforms > 1) {
         char buf[240];
-        snprintf(buf, sizeof buf, "lz77_cmds_batch_device: parse (min_match %d, lazy %d, dict_min %d, reserved %d) is outside min_match 4..32, "
-                 "lazy 0..2, dict_min 0 or 4..32, reserved 0", (int)parse->min_match, (int)parse->lazy, (int)parse->dict_min, (int)parse->reserved);
+        snprintf(buf, sizeof buf, "lz77_cmds_batch_device: parse (min_match %d, lazy %d, dict_min %d, transforms %d) is outside min_match 4..32, "
+                 "lazy 0..2, dict_min 0 or 4..32, transforms 0 or 1", (int)parse->min_match, (int)parse->lazy, (int)parse->dict_min,
+                 (int)parse->transforms);
         ctx->err = buf;
         return DIVANS_FAILURE;
     }
-    const DictIndex *host_dict = parse->dict_min ? host_dict_index() : nullptr;
-    if (parse->dict_min && !host_dict) { ctx->err = "lz77_cmds_batch_device: the dictionary index cannot be built from the tables"; return DIVANS_FAILURE; }
+    const bool all = parse->dict_min && parse->transforms;
+    const DictIndex *host_dict = parse->dict_min && !all ? host_dict_index() : nullptr;
+    const WordIndex *host_words = all ? host_words_index() : nullptr;
+    if (parse->dict_min && !host_dict && !host_words) {
+        ctx->err = "lz77_cmds_batch_device: the dictionary index cannot be built from the tables";
+        return DIVANS_FAILURE;
+    }
     if (window < 10 || window > 24) { ctx->err = "lz77_cmds_batch_device: window must be 10..24"; return DIVANS_FAILURE; }
     if (n > 0xffffffffull) { ctx->err = "lz77_cmds_batch_device: too many streams"; return DIVANS_FAILURE; }
     if (n == 0) return DIVANS_SUCCESS;
@@ -1512,6 +1520,15 @@ extern "C" DivansResult divans_b200_lz77_cmds_batch_device_dict(divans_b200_ctx 
         }
         CK(cudaMemcpy(ctx->d_dict_index, host_dict, sizeof(DictIndex), cudaMemcpyHostToDevice));
     }
+    if (host_words && !ctx->d_words_index) {
+        if (cudaMalloc((void **)&ctx->d_words_index, sizeof(WordIndex)) != cudaSuccess) {
+            cudaGetLastError();
+            ctx->d_words_index = nullptr;
+            ctx->err = "divans_b200: cannot allocate the LZ77 dictionary index of every transform";
+            return DIVANS_FAILURE;
+        }
+        CK(cudaMemcpy(ctx->d_words_index, host_words, sizeof(WordIndex), cudaMemcpyHostToDevice));
+    }
     // the record of lz77_blob: pred_mode and mixing_value stored as bytes
     const divans_b200_literal_model rec = {pred_mode, mixing_value};
     if (stage_records(ctx, &rec, 1, 0, st) != DIVANS_SUCCESS) return DIVANS_FAILURE;
@@ -1524,7 +1541,8 @@ extern "C" DivansResult divans_b200_lz77_cmds_batch_device_dict(divans_b200_ctx 
     CK(cudaMemsetAsync(ctx->d_counter, 0, 4, st));
     CK(cudaEventRecord(ctx->ev0, st));
     CK(cudaEventRecord(ctx->evm, st));
-    launch_lz77_cmds(lp, ld, st);
+    if (all) launch_lz77_words(lp, Lz77Words{ctx->d_words_index, parse->dict_min}, st);
+    else launch_lz77_cmds(lp, ld, st);
     CK(cudaEventRecord(ctx->ev1, st));
     CK(cudaEventRecord(ctx->ev_busy, st)); ctx->busy_recorded = true;
     ctx->main_end_is_evm1 = false;
@@ -1534,6 +1552,25 @@ extern "C" DivansResult divans_b200_lz77_cmds_batch_device_dict(divans_b200_ctx 
 } catch (...) {
     if (ctx) ctx->err = "divans_b200: out of host memory";
     return DIVANS_FAILURE;
+}
+extern "C" DivansResult divans_b200_lz77_cmds_batch_device_dict(divans_b200_ctx *ctx, size_t n, const uint8_t *d_in, const uint64_t *d_in_off,
+                                                                const uint64_t *d_in_len, uint64_t max_in_len, int32_t window,
+                                                                int32_t pred_mode, int32_t mixing_value, uint8_t *d_blobs,
+                                                                const uint64_t *d_blob_off, const uint64_t *d_blob_cap, uint64_t *d_blob_len,
+                                                                int32_t *d_status, const divans_b200_lz77_dict_parse *parse, void *cuda_stream) {
+    if (!ctx) return DIVANS_FAILURE;
+    if (!parse) { ctx->err = "lz77_cmds_batch_device: a parse is required"; return DIVANS_FAILURE; }
+    if (parse->min_match < 4 || parse->min_match > 32 || parse->lazy < 0 || parse->lazy > 2 ||
+        (parse->dict_min != 0 && (parse->dict_min < 4 || parse->dict_min > 32)) || parse->reserved != 0) {
+        char buf[240];
+        snprintf(buf, sizeof buf, "lz77_cmds_batch_device: parse (min_match %d, lazy %d, dict_min %d, reserved %d) is outside min_match 4..32, "
+                 "lazy 0..2, dict_min 0 or 4..32, reserved 0", (int)parse->min_match, (int)parse->lazy, (int)parse->dict_min, (int)parse->reserved);
+        ctx->err = buf;
+        return DIVANS_FAILURE;
+    }
+    const divans_b200_lz77_words_parse wp = {parse->min_match, parse->lazy, parse->dict_min, 0};
+    return divans_b200_lz77_cmds_batch_device_words(ctx, n, d_in, d_in_off, d_in_len, max_in_len, window, pred_mode, mixing_value, d_blobs,
+                                                    d_blob_off, d_blob_cap, d_blob_len, d_status, &wp, cuda_stream);
 }
 extern "C" DivansResult divans_b200_lz77_cmds_batch_device_parse(divans_b200_ctx *ctx, size_t n, const uint8_t *d_in, const uint64_t *d_in_off,
                                                                  const uint64_t *d_in_len, uint64_t max_in_len, int32_t window,

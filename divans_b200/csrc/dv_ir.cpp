@@ -208,13 +208,22 @@ const DictIndex *host_dict_index() {
     }();
     return x.get();
 }
+const WordIndex *host_words_index() {
+    static const std::unique_ptr<WordIndex> x = [] {
+        std::unique_ptr<WordIndex> d(new WordIndex());
+        if (!words_index_build(dv_tables_blob, *d)) d.reset();
+        return d;
+    }();
+    return x.get();
+}
 }  // namespace dv
 
 namespace {
 // The parse (include/divans_b200.h, "the LZ77 parse"): best(j) needs every position below j inserted and j not yet, so the
 // chain is filled up to j on demand; the (at most three) positions the parse looks at around i are kept in a small cache.
-// With dict_min != 0, dict(i) (dv_dict.h) is looked up at every position the parse reaches and does not defer.
-size_t lz77_blob(const uint8_t *in, size_t n, int window, int pred_mode, int mixing_value, const divans_b200_lz77_dict_parse &parse,
+// With dict_min != 0, dict(i) (dv_dict.h: dict_match, or words_match under transforms 1) is looked up at every position the
+// parse reaches and does not defer.
+size_t lz77_blob(const uint8_t *in, size_t n, int window, int pred_mode, int mixing_value, const divans_b200_lz77_words_parse &parse,
                  std::vector<uint8_t> &blob) {
     std::vector<Cmd> cmds;
     cmds.push_back({7, 0, 0, 0, 0});
@@ -253,7 +262,9 @@ size_t lz77_blob(const uint8_t *in, size_t n, int window, int pred_mode, int mix
         if (take && parse.lazy >= 1 && L < 32)
             take = !(best(i + 1, d1) > L || (parse.lazy == 2 && best(i + 2, d1) > L + 1));
         if (parse.dict_min && (take || L < min_match)) {   // (not deferred)
-            const uint32_t k = dv::dict_match(*dv::host_dict_index(), dv_tables_blob + dv::DICT_TB_DICT, in + i, (uint32_t)std::min<size_t>(n - i, 64));
+            const uint32_t avail = (uint32_t)std::min<size_t>(n - i, 64);
+            const uint32_t k = parse.transforms ? dv::words_match(*dv::host_words_index(), in + i, avail)
+                                                : dv::dict_match(*dv::host_dict_index(), dv_tables_blob + dv::DICT_TB_DICT, in + i, avail);
             const size_t Ld = dv::dict_len(k);
             if (Ld >= (size_t)parse.dict_min && Ld > (take ? L : 0)) {
                 if (i > lit_start) cmds.push_back({3, (uint32_t)lit_start, (uint32_t)(i - lit_start), 0, 0});
@@ -289,15 +300,16 @@ size_t lz77_blob(const uint8_t *in, size_t n, int window, int pred_mode, int mix
 
 // n raw buffers -> n DVCL blobs written back to back at blob_off[i] (16-byte aligned) of `out`; blob_len[i] receives the sizes.
 // With out == NULL or out_cap too small the call returns DIVANS_NEEDS_MORE_OUTPUT and *total receives the size needed.
-// `parse` NULL or outside min_match 4..32, lazy 0..2, dict_min 0 or 4..32, reserved 0: DIVANS_FAILURE, nothing written.
-extern "C" DivansResult divans_b200_lz77_cmds_batch_dict(size_t n, const uint8_t *in, const uint64_t *in_off, const uint64_t *in_len, int32_t window,
-                                                         int32_t pred_mode, int32_t mixing_value, uint8_t *out, size_t out_cap, uint64_t *blob_off,
-                                                         uint64_t *blob_len, size_t *total, int32_t n_threads, const divans_b200_lz77_dict_parse *parse) {
+// `parse` NULL or outside min_match 4..32, lazy 0..2, dict_min 0 or 4..32, transforms 0 or 1: DIVANS_FAILURE, nothing written.
+extern "C" DivansResult divans_b200_lz77_cmds_batch_words(size_t n, const uint8_t *in, const uint64_t *in_off, const uint64_t *in_len, int32_t window,
+                                                          int32_t pred_mode, int32_t mixing_value, uint8_t *out, size_t out_cap, uint64_t *blob_off,
+                                                          uint64_t *blob_len, size_t *total, int32_t n_threads, const divans_b200_lz77_words_parse *parse) {
     if (!in || !in_off || !in_len || !blob_off || !blob_len || !total || window < 10 || window > 24) return DIVANS_FAILURE;
     if (!parse || parse->min_match < 4 || parse->min_match > 32 || parse->lazy < 0 || parse->lazy > 2) return DIVANS_FAILURE;
-    if ((parse->dict_min != 0 && (parse->dict_min < 4 || parse->dict_min > 32)) || parse->reserved != 0) return DIVANS_FAILURE;
-    if (parse->dict_min && !dv::host_dict_index()) return DIVANS_FAILURE;
-    const divans_b200_lz77_dict_parse ps = *parse;
+    if ((parse->dict_min != 0 && (parse->dict_min < 4 || parse->dict_min > 32)) || parse->transforms < 0 || parse->transforms > 1)
+        return DIVANS_FAILURE;
+    if (parse->dict_min && !(parse->transforms ? (const void *)dv::host_words_index() : (const void *)dv::host_dict_index())) return DIVANS_FAILURE;
+    const divans_b200_lz77_words_parse ps = *parse;
     std::vector<std::vector<uint8_t>> blobs(n);
     if (n_threads < 1) n_threads = 1;
     std::vector<std::thread> th;
@@ -310,6 +322,15 @@ extern "C" DivansResult divans_b200_lz77_cmds_batch_dict(size_t n, const uint8_t
     if (!out || out_cap < pos) return DIVANS_NEEDS_MORE_OUTPUT;
     for (size_t i = 0; i < n; i++) memcpy(out + blob_off[i], blobs[i].data(), blobs[i].size());
     return DIVANS_SUCCESS;
+}
+
+extern "C" DivansResult divans_b200_lz77_cmds_batch_dict(size_t n, const uint8_t *in, const uint64_t *in_off, const uint64_t *in_len, int32_t window,
+                                                         int32_t pred_mode, int32_t mixing_value, uint8_t *out, size_t out_cap, uint64_t *blob_off,
+                                                         uint64_t *blob_len, size_t *total, int32_t n_threads, const divans_b200_lz77_dict_parse *parse) {
+    if (!parse || parse->reserved != 0) return DIVANS_FAILURE;
+    const divans_b200_lz77_words_parse wp = {parse->min_match, parse->lazy, parse->dict_min, 0};
+    return divans_b200_lz77_cmds_batch_words(n, in, in_off, in_len, window, pred_mode, mixing_value, out, out_cap, blob_off, blob_len, total,
+                                             n_threads, &wp);
 }
 
 extern "C" DivansResult divans_b200_lz77_cmds_batch_parse(size_t n, const uint8_t *in, const uint64_t *in_off, const uint64_t *in_len, int32_t window,

@@ -1,4 +1,4 @@
-// dv_lz77.cu -- sm_90a kernels of divans_b200_lz77_cmds_batch_device[_parse|_dict]: the library's hash-chain LZ77 (dv_ir.cpp,
+// dv_lz77.cu -- sm_90a kernels of divans_b200_lz77_cmds_batch_device[_parse|_dict|_words]: the library's hash-chain LZ77 (dv_ir.cpp,
 // lz77_blob) run next to raw buffers in HBM.  Every blob is byte for byte the one the host generator writes for the same input,
 // arguments and parse.  The host's rules:
 //   h4(i) = (le32(in + i) * 2654435761) >> 17, for positions with i + 4 <= n only; every such position is inserted, in order,
@@ -25,7 +25,8 @@
 //     that reached the cap, in chain order: only those can be the longest.  So per window a lane spends at most 16 capped
 //     compares, and exact lengths are measured only where the parse lands.  With the dictionary step (lz77_dict_kernel), lane t
 //     also looks up dict(p + t) in the dictionary index, and the lanes with a copy or a word make the ballot.  A word has at most
-//     31 bytes, so comparing it with a capped copy length (LZ_CAP = 64) is exact.
+//     31 bytes, so comparing it with a capped copy length (LZ_CAP = 64) is exact.  lz77_words_kernel looks up dict(p + t) under
+//     every transform instead (words_match); those words have at most 37 bytes, so the same holds.
 //  3. Emit.  Records go out as they are found, at blob + 32 + 20k, while they fit the region; then the header, the
 //     PredictionMode record (built once per call on the host) and the literal pool, which is the raw stream.  A blob that
 //     does not fit is still parsed to the end, so its exact size is reported.
@@ -41,6 +42,9 @@ constexpr int LZ_CHAIN = 16;           // candidates per position
 constexpr int32_t LZ_CAP = 64;         // bytes of the capped compare
 constexpr int32_t LZ_MAX_COPY = 65535;
 constexpr int32_t LZ_LAZY_BELOW = 32;   // a lazy parse looks ahead only from matches shorter than this
+// A capped copy length of LZ_CAP is longer than any dictionary word, so a word and a copy compare exactly without the copy's
+// full length.
+static_assert(DICT_MAX_MATCH < (uint32_t)LZ_CAP && WORDS_MAX_MATCH < (uint32_t)LZ_CAP, "a word must be shorter than LZ_CAP");
 
 // The four bytes at p (p < end) as a little-endian word, from the aligned words that hold them.  The second word is read only
 // when it starts below `end`: no word without a byte of the stream is read.
@@ -102,9 +106,14 @@ __device__ __noinline__ int2 lz_extend(const uint8_t *in, const uint8_t *end, co
     return make_int2(best, dist);
 }
 
-// LAZY: the parse's lazy steps (0..2); min_match is p.min_match.  DICT: the dictionary step, dc.dict_min 4..32 (dc unread without it).
-template <int LAZY, bool DICT>
-__device__ __forceinline__ void lz77_cmds_body(const Lz77Params &p, const Lz77Dict &dc) {
+// dict(q) of the dictionary step a kernel runs, packed (dv_dict.h)
+__device__ __forceinline__ uint32_t lz_dict(const Lz77Dict &d, const uint8_t *p, uint32_t avail) { return dict_match(*d.index, d.words, p, avail); }
+__device__ __forceinline__ uint32_t lz_dict(const Lz77Words &d, const uint8_t *p, uint32_t avail) { return words_match(*d.index, p, avail); }
+
+// LAZY: the parse's lazy steps (0..2); min_match is p.min_match.  DICT: the dictionary step, dc.dict_min 4..32 (dc unread without
+// it); D: Lz77Dict (the 44-member set) or Lz77Words (every transform).
+template <int LAZY, bool DICT, class D>
+__device__ __forceinline__ void lz77_cmds_body(const Lz77Params &p, const D &dc) {
     const int lane = threadIdx.x & 31;
     const uint32_t warp = blockIdx.x * LZ_WARPS + (threadIdx.x >> 5);
     if (warp >= p.n_warps) return;
@@ -172,7 +181,7 @@ __device__ __forceinline__ void lz77_cmds_body(const Lz77Params &p, const Lz77Di
                 lim = min(n - q, LZ_MAX_COPY);
                 best = lz_capped(in, end, prev, q, lim, maxdist, dist, hits);
                 if (DICT) {
-                    word = dict_match(*dc.index, dc.words, in + q, (uint32_t)min(n - q, LZ_CAP));
+                    word = lz_dict(dc, in + q, (uint32_t)min(n - q, LZ_CAP));
                     if (dict_len(word) < (uint32_t)dc.dict_min) word = 0;
                 }
             }
@@ -245,6 +254,10 @@ template <int LAZY>
 __global__ void __launch_bounds__(LZ_BLOCK_THREADS, 16) lz77_dict_kernel(Lz77Params p, Lz77Dict d) {
     lz77_cmds_body<LAZY, true>(p, d);
 }
+template <int LAZY>
+__global__ void __launch_bounds__(LZ_BLOCK_THREADS, 16) lz77_words_kernel(Lz77Params p, Lz77Words w) {
+    lz77_cmds_body<LAZY, true>(p, w);
+}
 
 void launch_lz77_cmds(const Lz77Params &p, const Lz77Dict &d, cudaStream_t st) {
     const unsigned blocks = (p.n_warps + LZ_WARPS - 1) / LZ_WARPS;
@@ -255,6 +268,13 @@ void launch_lz77_cmds(const Lz77Params &p, const Lz77Dict &d, cudaStream_t st) {
     } else if (p.lazy == 2) lz77_cmds_kernel<2><<<blocks, LZ_BLOCK_THREADS, 0, st>>>(p);
     else if (p.lazy == 1) lz77_cmds_kernel<1><<<blocks, LZ_BLOCK_THREADS, 0, st>>>(p);
     else lz77_cmds_kernel<0><<<blocks, LZ_BLOCK_THREADS, 0, st>>>(p);
+}
+
+void launch_lz77_words(const Lz77Params &p, const Lz77Words &w, cudaStream_t st) {
+    const unsigned blocks = (p.n_warps + LZ_WARPS - 1) / LZ_WARPS;
+    if (p.lazy == 2) lz77_words_kernel<2><<<blocks, LZ_BLOCK_THREADS, 0, st>>>(p, w);
+    else if (p.lazy == 1) lz77_words_kernel<1><<<blocks, LZ_BLOCK_THREADS, 0, st>>>(p, w);
+    else lz77_words_kernel<0><<<blocks, LZ_BLOCK_THREADS, 0, st>>>(p, w);
 }
 
 }  // namespace dv

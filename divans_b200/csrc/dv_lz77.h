@@ -26,7 +26,14 @@ struct Lz77Params {
 struct Lz77Dict {
     const DictIndex *index; const uint8_t *words; int32_t dict_min;
 };
+// The dictionary step under every transform (include/divans_b200.h, "dictionary words under every transform in the LZ77
+// parse"): dict_min 4..32 and the index, which holds the dictionary bytes it reads.
+struct Lz77Words {
+    const WordIndex *index; int32_t dict_min;
+};
 // one launch, n_warps persistent warps (a kernel per lazy 0..2, with the dictionary step when d.dict_min != 0)
 void launch_lz77_cmds(const Lz77Params &p, const Lz77Dict &d, cudaStream_t st);
+// the same with the dictionary step under every transform (w.dict_min 4..32)
+void launch_lz77_words(const Lz77Params &p, const Lz77Words &w, cudaStream_t st);
 
 }  // namespace dv

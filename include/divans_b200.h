@@ -638,6 +638,42 @@ DivansResult divans_b200_lz77_cmds_batch_device_dict(divans_b200_ctx *ctx, size_
                                                      int32_t mixing_value, uint8_t *d_blobs, const uint64_t *d_blob_off,
                                                      const uint64_t *d_blob_cap, uint64_t *d_blob_len, int32_t *d_status,
                                                      const divans_b200_lz77_dict_parse *parse, void *cuda_stream);
+/* ---- dictionary words under every transform in the LZ77 parse ----
+ * The parse with dictionary words above, with a larger candidate set when transforms = 1.  Everything else is that parse's:
+ * deferral on copy lengths only, Ld > Lc, every position inserted into the hash chain, the window rule.
+ *  - transforms = 0: the 44-member set above; the lists are divans_b200_lz77_cmds_batch_dict's, byte for byte.
+ *  - transforms = 1: every word of size 4..24 (id below 2^size_bits_by_length[size]) under every transform t of 0..120.  w is
+ *    exactly what the decoder's dictionary step writes for (id, size, t): the prefix, then the core (the word after the
+ *    transform's omission, with its case transform applied, by the decoder's UTF-8 uppercase rule), then the suffix.  Types:
+ *    0 identity, 1..9 omit the last 1..9 bytes, 10 uppercase the first character, 11 uppercase all, 12..20 omit the first 1..9.
+ *  - A candidate counts only when its core has at least 4 bytes.  Then each candidate is found by one 4-byte key at the core's
+ *    start: the first 4 bytes of the core after the case transform, which depend on the core's first 4 bytes alone.
+ *  - dict(i) is the longest w with i + |w| <= n and in[i .. i + |w|) == w; ties to the lowest transform, then the shortest word
+ *    size, then the lowest word id (the order of the 44-member set).  There are 9 distinct prefixes and a prefix and suffix
+ *    together have at most 13 bytes, so |w| <= 24 + 13 = 37: the GPU generator's capped copy compare of 64 bytes still orders a
+ *    word against a copy exactly.  dict_min >= 4 keeps Ld >= 4, so lz77_blob_cap still holds every list.
+ * Domain: min_match 4..32, lazy 0..2, dict_min 0 or 4..32, transforms 0 or 1. */
+typedef struct {
+    int32_t min_match;   /* 4..32: the shortest match emitted as a copy */
+    int32_t lazy;        /* 0..2: positions looked ahead before a match shorter than 32 bytes is taken */
+    int32_t dict_min;    /* 0 (no dictionary words) or 4..32: the shortest transformed word emitted as a Dictionary command */
+    int32_t transforms;  /* 0: the 44 transforms with an empty prefix and the identity type; 1: all 121 */
+} divans_b200_lz77_words_parse;
+/* divans_b200_lz77_cmds_batch_dict under a words parse (NULL or out of the domain: DIVANS_FAILURE, nothing written).
+ * transforms = 0 writes divans_b200_lz77_cmds_batch_dict's blobs for {min_match, lazy, dict_min, 0}, byte for byte. */
+DivansResult divans_b200_lz77_cmds_batch_words(size_t n, const uint8_t *in, const uint64_t *in_off, const uint64_t *in_len, int32_t window,
+                                               int32_t pred_mode, int32_t mixing_value, uint8_t *out, size_t out_cap, uint64_t *blob_off,
+                                               uint64_t *blob_len, size_t *total, int32_t n_threads, const divans_b200_lz77_words_parse *parse);
+/* divans_b200_lz77_cmds_batch_device_dict under a words parse: every blob byte for byte divans_b200_lz77_cmds_batch_words's, with
+ * every other rule of that call (statuses, regions, refusals, scratch, the step end before a deferral whose lookahead falls past
+ * the 32 positions).  A parse that is NULL or outside the domain fails the call (DIVANS_FAILURE, divans_b200_last_error says
+ * why) before any work.  With dict_min != 0 and transforms = 1 the first call on a context uploads the index of every transform
+ * (1,427,612 bytes, the dictionary bytes and their two uppercase forms included); it stays until the context is destroyed. */
+DivansResult divans_b200_lz77_cmds_batch_device_words(divans_b200_ctx *ctx, size_t n, const uint8_t *d_in, const uint64_t *d_in_off,
+                                                      const uint64_t *d_in_len, uint64_t max_in_len, int32_t window, int32_t pred_mode,
+                                                      int32_t mixing_value, uint8_t *d_blobs, const uint64_t *d_blob_off,
+                                                      const uint64_t *d_blob_cap, uint64_t *d_blob_len, int32_t *d_status,
+                                                      const divans_b200_lz77_words_parse *parse, void *cuda_stream);
 /* ---- choosing one of k command lists per stream by coding cost ----
  * n streams, each with k (1..16) candidate DVCL command lists already in HBM, candidate-major: list c of stream i is
  * d_blobs[d_blob_off[c * n + i] .. +d_blob_len[c * n + i]) (4-byte aligned).  The lists of a stream should replay to the same

@@ -526,11 +526,14 @@ static size_t dvt_dict_at(const uint8_t *in, size_t n, size_t i, uint32_t *id, u
     return best;
 }
 
-/* dvo_lz77_cmds_parse with dictionary words (dict_min 0 or 4..32; 0 is dvo_lz77_cmds_parse).  At a position the walk reaches and
- * does not defer, a word of dict_min or more bytes that is longer than the copy there (0 below min_match) is emitted as a
- * Dictionary command. */
-int dvo_lz77_cmds_dict_parse(const uint8_t *in, size_t n, int window, int pred_mode, int mixing_value, int min_match, int lazy, int dict_min,
-                             dvo_cmdlist *l) {
+typedef size_t (*dvt_dict_fn)(const uint8_t *in, size_t n, size_t i, uint32_t *id, uint32_t *size, uint32_t *transform);
+static size_t dvt_words_at(const uint8_t *in, size_t n, size_t i, uint32_t *id, uint32_t *size, uint32_t *transform);
+
+/* dvo_lz77_cmds_parse with dictionary words (dict_min 0 or 4..32; 0 is dvo_lz77_cmds_parse), found by dict_at.  At a position
+ * the walk reaches and does not defer, a word of dict_min or more bytes that is longer than the copy there (0 below min_match)
+ * is emitted as a Dictionary command. */
+static int dvt_lz77_cmds(const uint8_t *in, size_t n, int window, int pred_mode, int mixing_value, int min_match, int lazy, int dict_min,
+                         dvt_dict_fn dict_at, dvo_cmdlist *l) {
     if (min_match < 4 || min_match > 32 || lazy < 0 || lazy > 2) return DVO_FAILURE;
     if (dict_min != 0 && (dict_min < 4 || dict_min > 32)) return DVO_FAILURE;
     dvt_lz z; memset(&z, 0, sizeof z);
@@ -550,7 +553,7 @@ int dvo_lz77_cmds_dict_parse(const uint8_t *in, size_t n, int window, int pred_m
             take = !deferred;
         }
         uint32_t wid = 0, ws = 0, wt = 0;
-        const size_t Ld = dict_min && !deferred ? dvt_dict_at(in, n, i, &wid, &ws, &wt) : 0;
+        const size_t Ld = dict_min && !deferred ? dict_at(in, n, i, &wid, &ws, &wt) : 0;
         const int word = Ld >= (size_t)dict_min && Ld > (take ? L : 0);
         if (!take && !word) { i++; continue; }
         if (i > lit_start) {
@@ -570,8 +573,71 @@ int dvo_lz77_cmds_dict_parse(const uint8_t *in, size_t n, int window, int pred_m
     return DVO_SUCCESS;
 }
 
+int dvo_lz77_cmds_dict_parse(const uint8_t *in, size_t n, int window, int pred_mode, int mixing_value, int min_match, int lazy, int dict_min,
+                             dvo_cmdlist *l) {
+    return dvt_lz77_cmds(in, n, window, pred_mode, mixing_value, min_match, lazy, dict_min, dvt_dict_at, l);
+}
+
 int dvo_lz77_cmds_parse(const uint8_t *in, size_t n, int window, int pred_mode, int mixing_value, int min_match, int lazy, dvo_cmdlist *l) {
     return dvo_lz77_cmds_dict_parse(in, n, window, pred_mode, mixing_value, min_match, lazy, 0, l);
+}
+
+/* dict(i) of include/divans_b200.h ("dictionary words under every transform in the LZ77 parse"), restated without an index:
+ * every word of size 4..24 under every transform 0..120 whose prefix matches at i is built by dvo_dict_word and compared, when
+ * its core (the word after the transform's omission) has 4 or more bytes.  Before the build, a word is filtered on where its
+ * core starts, i + |prefix|: the core's first four bytes are the word's (from the omitted start on) unless a case transform
+ * applies, and a case transform leaves a first byte below 0xc0 as its ASCII uppercase and any other as it is.  Returns the
+ * length (0: none). */
+static size_t dvt_words_at(const uint8_t *in, size_t n, size_t i, uint32_t *id, uint32_t *size, uint32_t *transform) {
+    size_t best = 0;
+    uint8_t w[64];
+    int pre_ok[121];
+    size_t pre_len[121], cores[121];   /* where the cores may start: i + the length of a prefix that matches */
+    uint32_t n_cores = 0;
+    for (uint32_t t = 0; t < 121; t++) {
+        const uint8_t *prefix = TB_PS + TB_PSMAP[TB_TRANSFORMS[3 * t]];
+        pre_len[t] = prefix[0];
+        pre_ok[t] = i + prefix[0] + 4 <= n && memcmp(prefix + 1, in + i, prefix[0]) == 0;
+        uint32_t k = 0;
+        while (pre_ok[t] && k < n_cores && cores[k] != i + prefix[0]) k++;
+        if (pre_ok[t] && k == n_cores) cores[n_cores++] = i + prefix[0];
+    }
+    for (uint32_t s = 4; s <= 24; s++) {
+        for (uint32_t wid = 0; wid < (1u << TB_SIZE_BITS[s]); wid++) {
+            const uint8_t *word = TB_DICT + TB_OFFSETS[s] + (size_t)wid * s;
+            int any = 0;   /* the filter below, for any transform: skip the word when no core of it can start anywhere */
+            for (uint32_t k = 0; k < n_cores && !any; k++) {
+                const uint8_t *c = in + cores[k];
+                any = (word[0] < 0xc0 && word[0] >= 'a' && word[0] <= 'z' ? word[0] ^ 32 : word[0]) == c[0];
+                for (uint32_t skip = 0; skip <= 9 && skip + 4 <= s && !any; skip++) any = memcmp(word + skip, c, 4) == 0;
+            }
+            if (!any) continue;
+            for (uint32_t t = 0; t < 121; t++) {
+                if (!pre_ok[t]) continue;
+                const uint32_t type = TB_TRANSFORMS[3 * t + 1];
+                const uint32_t skip = type >= 12 ? type - 11 : 0, core = s - skip - (type <= 9 ? type : 0);
+                const uint8_t *c = in + i + pre_len[t];
+                if (skip > s || (int)core < 4) continue;
+                if (type == 10 || type == 11) {
+                    if ((word[0] < 0xc0 && word[0] >= 'a' && word[0] <= 'z' ? word[0] ^ 32 : word[0]) != c[0]) continue;
+                } else if (memcmp(word + skip, c, 4) != 0) continue;
+                const int len = dvo_dict_word(s, wid, t, w);
+                if (len < 0 || i + (size_t)len > n || memcmp(w, in + i, (size_t)len) != 0) continue;
+                const int better = (size_t)len > best
+                    || ((size_t)len == best && (t < *transform || (t == *transform && (s < *size || (s == *size && wid < *id)))));
+                if (better) { best = (size_t)len; *id = wid; *size = s; *transform = t; }
+            }
+        }
+    }
+    return best;
+}
+
+/* dvo_lz77_cmds_dict_parse with the candidate set of `transforms`: 0 the 44-member set (dvo_lz77_cmds_dict_parse), 1 every
+ * transform (dvt_words_at). */
+int dvo_lz77_cmds_words_parse(const uint8_t *in, size_t n, int window, int pred_mode, int mixing_value, int min_match, int lazy, int dict_min,
+                              int transforms, dvo_cmdlist *l) {
+    if (transforms != 0 && transforms != 1) return DVO_FAILURE;
+    return dvt_lz77_cmds(in, n, window, pred_mode, mixing_value, min_match, lazy, dict_min, transforms ? dvt_words_at : dvt_dict_at, l);
 }
 
 /* The CPU reference of divans_b200_encode_cmds_choose_batch_device for one stream: costs[c] = dvo_tally_cmds of lists[c], each

@@ -11,8 +11,8 @@ followed by tally_api.c, and compiles it twice, with the reference's default pro
 the oracle's own Makefile does.  Every function of the oracle is in these libraries unchanged while no forged encode runs; only
 the tally entry points, dvo_cmdlist_set_mixing (a test's own mixing values in a list), dvo_recode_blob (the CPU reference of
 the library's command-list replay, on the serialised blob), dvo_cmdlist_from_blob, dvo_encode_cmds_forged, dvo_lz77_cmds_parse
-(the LZ77 generator under a parse), dvo_lz77_cmds_dict_parse (the same with dictionary words) and dvo_encode_cmds_choose (one of
-k command lists chosen by cost) are new.
+(the LZ77 generator under a parse), dvo_lz77_cmds_dict_parse (the same with dictionary words), dvo_lz77_cmds_words_parse (with
+dictionary words under every transform) and dvo_encode_cmds_choose (one of k command lists chosen by cost) are new.
 """
 import ctypes
 import os
@@ -166,6 +166,7 @@ def lib(blend=False):
         L.dvo_tally_cmds.argtypes = [vp, op, u64p]
         L.dvo_lz77_cmds_parse.argtypes = [vp, ctypes.c_size_t, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, vp]
         L.dvo_lz77_cmds_dict_parse.argtypes = [vp, ctypes.c_size_t] + [ctypes.c_int] * 6 + [vp]
+        L.dvo_lz77_cmds_words_parse.argtypes = [vp, ctypes.c_size_t] + [ctypes.c_int] * 7 + [vp]
         L.dvo_encode_cmds_choose.argtypes = [vp, ctypes.c_uint32, op, vp, ctypes.c_size_t, szp, ctypes.POINTER(ctypes.c_uint32), vp]
         assert L.dvo_feature_blend() == int(blend)
         _libs[blend] = L
@@ -489,6 +490,16 @@ def lz77_dict_parse(oracle, data, min_match=4, lazy=0, dict_min=0, window=16, pr
     cl = oracle.Commands()
     d = _u8(data)
     rc = lib().dvo_lz77_cmds_dict_parse(_p(d), len(data), window, pred_mode, mixing_value, min_match, lazy, dict_min, ctypes.addressof(cl.c))
+    return cl if rc == SUCCESS else None
+
+
+def lz77_words_parse(oracle, data, min_match=4, lazy=0, dict_min=0, transforms=0, window=16, pred_mode=2, mixing_value=4):
+    """the oracle_py Commands of dvo_lz77_cmds_words_parse for ``data`` under the parse (min_match, lazy, dict_min, transforms),
+    or None for a parse outside min_match 4..32, lazy 0..2, dict_min 0 or 4..32, transforms 0 or 1 (the list is then untouched)"""
+    cl = oracle.Commands()
+    d = _u8(data)
+    rc = lib().dvo_lz77_cmds_words_parse(_p(d), len(data), window, pred_mode, mixing_value, min_match, lazy, dict_min, transforms,
+                                         ctypes.addressof(cl.c))
     return cl if rc == SUCCESS else None
 
 
