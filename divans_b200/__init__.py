@@ -55,6 +55,7 @@ BATCH_SYMBOLS = [
     "divans_b200_lz77_cmds_batch_parse", "divans_b200_lz77_cmds_batch_device_parse", "divans_b200_encode_cmds_choose_batch_device",
     "divans_b200_lz77_cmds_batch_dict", "divans_b200_lz77_cmds_batch_device_dict",
     "divans_b200_lz77_cmds_batch_words", "divans_b200_lz77_cmds_batch_device_words",
+    "divans_b200_bill_batch_host", "divans_b200_bill_batch_device", "divans_b200_bill_cmds_batch_host", "divans_b200_bill_cmds_batch_device",
 ]
 PM_RECORD_BYTES = 32 + 16384 + 1024 + 8192   # one prediction-mode record of a DVCL blob (include/divans_b200.h)
 
@@ -131,6 +132,40 @@ class Lz77WordsParse(ctypes.Structure):
 # DEFAULT_LZ77_DICT_PARSES, then the (min_match, lazy, dict_min, transforms) parses a greedy survey of exact oracle sizes adds
 # (tools/lz77_words_probe.py --survey, DESIGN.md section 4, "Dictionary words under every transform").
 DEFAULT_LZ77_WORD_PARSES = DEFAULT_LZ77_DICT_PARSES + [(4, 0, 4, 1), (10, 2, 4, 1)]
+
+
+# The rows of a stream's bill (Engine.bill), in the order of include/divans_b200.h ("billing each stream's coding cost by coder
+# state"): one per nibble-coding state of the encoder's command state machine.
+BILL_STATES = [
+    "CMD_TYPE", "LIT_HI", "LIT_LO",
+    "LL_COUNT_SMALL", "LL_SIZE_BEG", "LL_SIZE_LAST", "LL_MANT",
+    "CP_COUNT_SMALL", "CP_COUNT_BEG", "CP_COUNT_LAST", "CP_COUNT_MANT",
+    "CP_MNEMONIC", "CP_DIST_BEG", "CP_DIST_LAST", "CP_DIST_MANT",
+    "DC_SIZE_BEG", "DC_SIZE_LAST", "DC_INDEX", "DC_TR_HI", "DC_TR_LO",
+    "BT_MNEMONIC", "BT_FIRST", "BT_SECOND", "BT_STRIDE",
+    "PM_MODE", "PM_MIX", "PM_DEPTH", "PM_SPEED", "PM_MAP_MNEMONIC", "PM_MAP_FIRST", "PM_MAP_SECOND", "PM_MIXVAL",
+]
+# bill_summary's coarse groups, after the reference's billing build (the BillingDesignation kinds, with copies split into lengths
+# and distances and the PredictionMode command's mixing values apart from the rest of it)
+BILL_GROUPS = [
+    ("command selection", ["CMD_TYPE"]),
+    ("literal lengths", ["LL_COUNT_SMALL", "LL_SIZE_BEG", "LL_SIZE_LAST", "LL_MANT"]),
+    ("literals", ["LIT_HI", "LIT_LO"]),
+    ("copy lengths", ["CP_COUNT_SMALL", "CP_COUNT_BEG", "CP_COUNT_LAST", "CP_COUNT_MANT"]),
+    ("copy distances", ["CP_MNEMONIC", "CP_DIST_BEG", "CP_DIST_LAST", "CP_DIST_MANT"]),
+    ("dictionary", ["DC_SIZE_BEG", "DC_SIZE_LAST", "DC_INDEX", "DC_TR_HI", "DC_TR_LO"]),
+    ("block switches", ["BT_MNEMONIC", "BT_FIRST", "BT_SECOND", "BT_STRIDE"]),
+    ("prediction mode", ["PM_MODE", "PM_MIX", "PM_DEPTH", "PM_SPEED", "PM_MAP_MNEMONIC", "PM_MAP_FIRST", "PM_MAP_SECOND"]),
+    ("mixing values", ["PM_MIXVAL"]),
+]
+
+
+def bill_summary(rows):
+    """Fold bill rows ([BILL_STATES, 2] of one stream, or [..., BILL_STATES, 2] summed over the leading axes) into BILL_GROUPS:
+    a list of (group, cost in 1/65536 bit, nibbles)."""
+    r = np.asarray(rows, np.uint64).reshape(-1, len(BILL_STATES), 2).sum(axis=0, dtype=np.uint64)
+    return [(name, int(sum(int(r[BILL_STATES.index(k), 0]) for k in keys)), int(sum(int(r[BILL_STATES.index(k), 1]) for k in keys)))
+            for name, keys in BILL_GROUPS]
 
 
 class CAllocator(ctypes.Structure):
@@ -222,6 +257,12 @@ def load_library():
     L.divans_b200_lz77_cmds_batch_words.restype = ctypes.c_uint8
     L.divans_b200_lz77_cmds_batch_device_words.argtypes = L.divans_b200_lz77_cmds_batch_device.argtypes[:-1] + [ctypes.POINTER(Lz77WordsParse), vp]
     L.divans_b200_lz77_cmds_batch_device_words.restype = ctypes.c_uint8
+    eo = ctypes.POINTER(EncodeOptions)
+    L.divans_b200_bill_batch_host.argtypes = L.divans_b200_bill_cmds_batch_host.argtypes = [vp, sz, vp, vp, vp, eo, vp, vp]
+    L.divans_b200_bill_batch_device.argtypes = [vp, sz, vp, vp, vp, ctypes.c_uint64, eo, vp, vp, vp]
+    L.divans_b200_bill_cmds_batch_device.argtypes = [vp, sz, vp, vp, vp, ctypes.c_uint64, ctypes.c_uint64, eo, vp, vp, vp]
+    for name in ("bill_batch_host", "bill_batch_device", "bill_cmds_batch_host", "bill_cmds_batch_device"):
+        getattr(L, "divans_b200_" + name).restype = ctypes.c_uint8
     L.divans_b200_encode_cmds_choose_batch_device.argtypes = [vp, sz, ctypes.c_uint32, vp, vp, vp, ctypes.c_uint64, ctypes.c_uint64, vp, vp, vp,
                                                               vp, vp, ctypes.POINTER(EncodeOptions), vp, vp, vp]
     L.divans_b200_encode_cmds_choose_batch_device.restype = ctypes.c_uint8
@@ -756,6 +797,33 @@ class Engine:
         list coded under the cheapest of ``candidates`` (encode_cmds_auto_batch_host)."""
         status, outs, chosen, _ = self._encode_lists(blobs, opts, True, self._auto_host, candidates)
         return [(int(s), b, int(c)) for s, b, c in zip(status, outs, chosen)]
+
+    # ---- billing by coder state (include/divans_b200.h) ----
+    def bill(self, items, opts=None, cmds=False):
+        """Each stream's coding cost billed by the encoder state that coded each nibble: raw byte strings (coded as encode
+        codes them), or DVCL command lists with ``cmds`` (under their own records).  Returns (bill [n, len(BILL_STATES), 2]
+        uint64 of (cost in 1/65536 bit, nibbles) per row, status [n]); a stream whose pass failed has an all-zero bill."""
+        blob, off, ln = _pack(items)
+        n = len(ln)
+        bill, status = np.zeros((n, len(BILL_STATES), 2), np.uint64), np.full(n, DIVANS_FAILURE, np.int32)
+        fn = self._L.divans_b200_bill_cmds_batch_host if cmds else self._L.divans_b200_bill_batch_host
+        rc = fn(self._h, n, _ptr(blob), _ptr(off), _ptr(ln), ctypes.byref(opts or encode_options()), _ptr(bill), _ptr(status))
+        if rc != DIVANS_SUCCESS:
+            raise DivansError("bill: " + self._err())
+        return bill, status
+
+    def bill_device(self, n, d_in, d_in_off, d_in_len, max_in_len, d_bill, d_status, opts=None, cmds=False, max_raw_len=None, stream=None):
+        """Engine.bill with raw device pointers (ints): d_bill u64 [n * len(BILL_STATES) * 2], d_status i32 [n].  With ``cmds``
+        the inputs are 4-byte aligned DVCL command lists of at most ``max_in_len`` bytes replaying at most ``max_raw_len``
+        bytes.  Asynchronous on ``stream``."""
+        o = ctypes.byref(opts or encode_options())
+        if cmds:
+            rc = self._L.divans_b200_bill_cmds_batch_device(self._h, n, d_in, d_in_off, d_in_len, int(max_in_len), int(max_raw_len), o, d_bill,
+                                                            d_status, stream)
+        else:
+            rc = self._L.divans_b200_bill_batch_device(self._h, n, d_in, d_in_off, d_in_len, int(max_in_len), o, d_bill, d_status, stream)
+        if rc != DIVANS_SUCCESS:
+            raise DivansError("bill_device: " + self._err())
 
     # ---- per-context mixing values (include/divans_b200.h) ----
     @staticmethod

@@ -654,13 +654,16 @@ static DivansResult stage_records(divans_b200_ctx *ctx, const divans_b200_litera
 
 // One pass of the model walk `w` over the p.n_streams streams or pairs, which it pulls from the context's work counter (reset
 // first), on as many encoder slots as they fill, under the options' CDF model.  `timed`: the encode's own model pass, which
-// last_kernel_ms and last_main_kernel_ms time from here.
+// last_kernel_ms and last_main_kernel_ms time from here.  With `bill` the pass is the cost pass billed by coder state
+// (encode_bill_kernel) instead of `w`.
 static DivansResult model_pass(divans_b200_ctx *ctx, const EncBatch &b, EncodeWalk w, const EncodeParams &p, const BinParams &bp = BinParams(),
-                               bool timed = false) {
+                               bool timed = false, uint64_t *bill = nullptr) {
     const uint32_t blocks = (uint32_t)(encode_slots(ctx, p.n_streams) / ENCODE_GROUPS_PER_BLOCK);
     CK(cudaMemsetAsync(ctx->d_counter, 0, 4, b.st));
     if (timed) { CK(cudaEventRecord(ctx->ev0, b.st)); CK(cudaEventRecord(ctx->evm, b.st)); }
-    if (b.o->cdf_model == DIVANS_B200_CDF_BLEND) launch_encode_walk<true>(w, p, bp, blocks, b.st);
+    const bool blend = b.o->cdf_model == DIVANS_B200_CDF_BLEND;
+    if (bill) { if (blend) launch_encode_bill<true>(p, bill, blocks, b.st); else launch_encode_bill<false>(p, bill, blocks, b.st); }
+    else if (blend) launch_encode_walk<true>(w, p, bp, blocks, b.st);
     else launch_encode_walk<false>(w, p, bp, blocks, b.st);
     ctx->launches += 1;
     return DIVANS_SUCCESS;
@@ -773,13 +776,17 @@ static bool ensure_cost_tab(divans_b200_ctx *ctx, cudaStream_t st) {
 //  * SEL_SPEEDS (divans_b200_encode_[cmds_]speeds_*): literal speeds; chosen [n * 3], cost [n * (k + 1)], halves [n * k * 2].
 //  * SEL_LISTS (divans_b200_encode_cmds_choose_batch_device): one of k command lists per stream, each under its own records;
 //    the batch's in_off / in_len are the n * k lists, candidate-major; chosen [n] (required), cost [n * k].
+//  * SEL_BILL (divans_b200_bill_[cmds_]batch_*): no choice and no encode, the cost pass alone, billed by coder state;
+//    bill [n * BILL_COLS] (required).  The batch has no output regions.
 // Outputs other than auto's and lists' chosen may be NULL.
-enum SelKind { SEL_NONE, SEL_AUTO, SEL_MIXMAP, SEL_SPEEDS, SEL_LISTS };
+enum SelKind { SEL_NONE, SEL_AUTO, SEL_MIXMAP, SEL_SPEEDS, SEL_LISTS, SEL_BILL };
+constexpr size_t BILL_COLS = 2 * DIVANS_B200_BILL_STATES;
 struct Selection {
     SelKind kind = SEL_NONE;
     uint32_t k = 0;
     const divans_b200_literal_model *models = nullptr; const int32_t *mix_values = nullptr; const int16_t *speed_values = nullptr;
     uint32_t *chosen = nullptr; uint64_t *cost = nullptr; uint8_t *mixing = nullptr; uint64_t *bins = nullptr; uint64_t *halves = nullptr;
+    uint64_t *bill = nullptr;
     // the candidates once check_selection has accepted them: the literal models (auto, mixmap) or the speeds
     divans_b200_literal_model cands[16]; SpeedValues speeds;
 };
@@ -793,6 +800,10 @@ static Selection sel_mixmap(const int32_t *values, uint32_t k, uint32_t *chosen,
 }
 static Selection sel_speeds(const int16_t *values, uint32_t k, uint32_t *chosen, uint64_t *cost, uint64_t *halves) {
     Selection s; s.kind = SEL_SPEEDS; s.k = k; s.speed_values = values; s.chosen = chosen; s.cost = cost; s.halves = halves;
+    return s;
+}
+static Selection sel_bill(uint64_t *bill) {
+    Selection s; s.kind = SEL_BILL; s.k = 1; s.bill = bill;
     return s;
 }
 
@@ -869,6 +880,29 @@ static DivansResult encode_lists_device_nolock(divans_b200_ctx *ctx, const EncBa
     EncBatch e = b;
     e.in_off = pick_off; e.in_len = pick_len;
     return encode_device_internal(ctx, e);
+}
+
+// Billing: the cost pass over the n streams on encode_bill_kernel, each coded nibble's cost and count added to the row of the
+// state that coded it; the rows to sel.bill, the status to b.status, and nothing encoded.  Raw streams start with the options'
+// record, command lists keep their own.  last_kernel_ms times the pass.
+static DivansResult bill_device_nolock(divans_b200_ctx *ctx, const EncBatch &b, const Selection &sel) {
+    const size_t n = b.n, slots = encode_slots(ctx, n);
+    if (ensure_arena(ctx, slots) != DIVANS_SUCCESS) return DIVANS_FAILURE;
+    if (!grow(ctx, &ctx->d_replay, &ctx->replay_cap, slots * (size_t)b.caps.replay)) return DIVANS_FAILURE;
+    if (!grow(ctx, &ctx->d_auto, &ctx->auto_cap, n)) return DIVANS_FAILURE;   // tally [n]: the pass's totals (the bill's row sums)
+    if (ctx->busy_recorded) CK(cudaStreamWaitEvent(b.st, ctx->ev_busy, 0));
+    if (!ensure_cost_tab(ctx, b.st)) return DIVANS_FAILURE;
+    const divans_b200_literal_model opt = {b.o->literal_pred_mode, b.o->literal_mixing_value};
+    if (stage_records(ctx, &opt, b.raw_mode ? 1 : 0, 0, b.st) != DIVANS_SUCCESS) return DIVANS_FAILURE;
+    EncodeParams tp = cost_params(ctx, b, n, b.in_off, b.in_len, b.status, ctx->d_auto);
+    tp.pm_internal = ctx->d_records;
+    if (model_pass(ctx, b, EncodeWalk::TALLY, tp, BinParams(), true, sel.bill) != DIVANS_SUCCESS) return DIVANS_FAILURE;
+    CK(cudaEventRecord(ctx->evm1, b.st));
+    CK(cudaEventRecord(ctx->ev1, b.st));
+    CK(cudaEventRecord(ctx->ev_busy, b.st)); ctx->busy_recorded = true;
+    ctx->main_end_is_evm1 = true;
+    CK(cudaGetLastError());
+    return DIVANS_SUCCESS;
 }
 
 // Per-context mixing values.  Records [0, k) are R(p, v[c]), records [k, k + n) the streams' mixed records M_i.
@@ -1033,7 +1067,7 @@ static bool check_selection(divans_b200_ctx *ctx, int raw_mode, const divans_b20
     case SEL_LISTS:
         if (sel.k < 1 || sel.k > 16) { ctx->err = "encode_cmds_choose: 1..16 command lists per stream are required"; return false; }
         break;
-    case SEL_NONE: break;
+    case SEL_BILL: case SEL_NONE: break;
     }
     if (!raw_mode || sel.kind == SEL_AUTO || sel.kind == SEL_MIXMAP || (o->literal_pred_mode >= 0 && o->literal_pred_mode <= 3)) return true;
     char buf[200];
@@ -1049,6 +1083,7 @@ static DivansResult encode_nolock(divans_b200_ctx *ctx, const EncBatch &b, const
     case SEL_MIXMAP: return encode_mixmap_device_nolock(ctx, b, sel);
     case SEL_SPEEDS: return encode_speeds_device_nolock(ctx, b, sel);
     case SEL_LISTS: return encode_lists_device_nolock(ctx, b, sel);
+    case SEL_BILL: return bill_device_nolock(ctx, b, sel);
     case SEL_NONE: break;
     }
     return encode_device_internal(ctx, b);
@@ -1058,20 +1093,21 @@ static DivansResult encode_nolock(divans_b200_ctx *ctx, const EncBatch &b, const
 // the optional ones counted whether asked for or not, except bins), and the device scratch of its drivers in bytes per pair, per
 // slot of the pairs (next to the replay window) and per stream (mixmap: the winners, mixed record and mixing output).
 struct SelLayout {
-    size_t chosen_cols, cost_cols, halves_cols, mixing_bytes, bins_cols;
+    size_t chosen_cols, cost_cols, halves_cols, mixing_bytes, bins_cols, bill_cols;
     uint64_t pair_bytes, slot_bytes, stream_bytes;
 };
 static SelLayout sel_layout(const Selection &sel) {
-    const bool none = sel.kind == SEL_NONE, mix = sel.kind == SEL_MIXMAP, spd = sel.kind == SEL_SPEEDS;
+    const bool none = sel.kind == SEL_NONE, mix = sel.kind == SEL_MIXMAP, spd = sel.kind == SEL_SPEEDS, bill = sel.kind == SEL_BILL;
     SelLayout l;
-    l.chosen_cols = none ? 0 : spd ? 3 : 1;
-    l.cost_cols = none ? 0 : sel.k + (mix || spd ? 1 : 0);
+    l.chosen_cols = none || bill ? 0 : spd ? 3 : 1;
+    l.cost_cols = none || bill ? 0 : sel.k + (mix || spd ? 1 : 0);
+    l.bill_cols = bill ? BILL_COLS : 0;
     l.halves_cols = spd ? 2 * (size_t)sel.k : 0;
     l.mixing_bytes = mix ? MIX_ENTRIES : 0;
     l.bins_cols = mix && sel.bins ? (size_t)sel.k * MIX_ENTRIES : 0;
     l.pair_bytes = spd ? 96 : 0;
     l.slot_bytes = mix ? MIX_ENTRIES * 8 : 0;
-    l.stream_bytes = mix ? MIX_ENTRIES * 9 + PM_RECORD_BYTES + l.bins_cols * 8 : 0;
+    l.stream_bytes = mix ? MIX_ENTRIES * 9 + PM_RECORD_BYTES + l.bins_cols * 8 : bill ? BILL_COLS * 8 : 0;
     return l;
 }
 
@@ -1087,6 +1123,7 @@ static DivansResult encode_device_common(divans_b200_ctx *ctx, size_t n, int raw
     if (n == 0) return DIVANS_SUCCESS;
     if (sel.kind == SEL_AUTO && !sel.chosen) { ctx->err = raw_mode ? "encode_auto: d_chosen is required" : "encode_cmds_auto: d_chosen is required"; return DIVANS_FAILURE; }
     if (sel.kind == SEL_LISTS && !sel.chosen) { ctx->err = "encode_cmds_choose: d_chosen is required"; return DIVANS_FAILURE; }
+    if (sel.kind == SEL_BILL && !sel.bill) { ctx->err = "bill: the bill array is required"; return DIVANS_FAILURE; }
     if (sel.kind == SEL_MIXMAP && n > 0x7fffffffull) { ctx->err = "batch too large"; return DIVANS_FAILURE; }   // (one block per stream)
     const uint64_t nv = (uint64_t)n * (sel.kind == SEL_NONE ? 1 : sel.k);
     if (nv > 0xffffffffull || max_in_len > 0x7fff0000ull || max_raw_len > 0x7fff0000ull) { ctx->err = "batch too large"; return DIVANS_FAILURE; }
@@ -1097,7 +1134,7 @@ static DivansResult encode_device_common(divans_b200_ctx *ctx, size_t n, int raw
     std::lock_guard<std::mutex> lk(ctx->mu);
     CK(cudaSetDevice(ctx->device));
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream;
-    if (!raw_mode) {
+    if (!raw_mode && sel.kind != SEL_BILL) {   // (billing keeps no logs)
         // the slots first, as in the host call: the logs are sized from what is left, and a failure names them.  (The cost pass of
         // the n * C pairs has no logs; it runs in as many slots as the pairs fill.)
         if (ensure_arena(ctx, encode_slots(ctx, nv)) != DIVANS_SUCCESS) return DIVANS_FAILURE;
@@ -1171,6 +1208,7 @@ extern "C" DivansResult divans_b200_encode_cmds_choose_batch_device(divans_b200_
 }
 
 // The host encode calls: marshal, split into sub-batches whose symbol logs (and selection scratch) fit in HBM, run, copy back.
+// The billing calls (SEL_BILL) have no output regions (out, out_off, out_cap and out_len NULL) and keep no logs.
 // Host marshalling uses std::vector sized by the caller's arguments, and no C++ exception may cross the C boundary.
 static DivansResult encode_host_common(divans_b200_ctx *ctx, size_t n, int raw_mode, const uint8_t *in, const uint64_t *in_off,
                                        const uint64_t *in_len, uint8_t *out, const uint64_t *out_off, const uint64_t *out_cap,
@@ -1179,6 +1217,7 @@ static DivansResult encode_host_common(divans_b200_ctx *ctx, size_t n, int raw_m
     if (!check_selection(ctx, raw_mode, opts, sel)) return DIVANS_FAILURE;
     if (n == 0) return DIVANS_SUCCESS;
     if (sel.kind == SEL_AUTO && !sel.chosen) { ctx->err = raw_mode ? "encode_auto: chosen is required" : "encode_cmds_auto: chosen is required"; return DIVANS_FAILURE; }
+    if (sel.kind == SEL_BILL && !sel.bill) { ctx->err = "bill: the bill array is required"; return DIVANS_FAILURE; }
     if (sel.kind != SEL_NONE && (uint64_t)n * sel.k > 0xffffffffull) { ctx->err = "batch too large"; return DIVANS_FAILURE; }
     std::lock_guard<std::mutex> lk(ctx->mu);
     CK(cudaSetDevice(ctx->device));
@@ -1189,7 +1228,7 @@ static DivansResult encode_host_common(divans_b200_ctx *ctx, size_t n, int raw_m
     std::vector<uint8_t> staged;   // command lists are re-based to 4-byte aligned offsets
     uint64_t in_end = 0;
     for (size_t i = 0; i < n; i++) {
-        status[i] = DIVANS_FAILURE; out_len[i] = 0;
+        status[i] = DIVANS_FAILURE; if (out_len) out_len[i] = 0;
         if (raw_mode) {
             if (in_len[i] > 0x7fff0000ull) { ctx->err = "stream too large"; return DIVANS_FAILURE; }
             s_off[i] = in_off[i];
@@ -1221,27 +1260,32 @@ static DivansResult encode_host_common(divans_b200_ctx *ctx, size_t n, int raw_m
             const LogCaps c = {std::max(need[i1].cmd, mc.cmd), std::max(need[i1].lit, mc.lit), std::max(need[i1].replay, mc.replay)};
             const uint64_t m = i1 - i0 + 1, vs = sel.kind == SEL_NONE ? 0 : (uint64_t)encode_slots(ctx, m * sel.k);
             const uint64_t rep = vs * (c.replay + lay.slot_bytes) + m * lay.stream_bytes + m * sel.k * lay.pair_bytes;
-            if (i1 > i0 && (c.cmd + c.lit) * 4 * m + rep > budget) break;
+            const uint64_t logs = sel.kind == SEL_BILL ? 0 : (c.cmd + c.lit) * 4 * m;
+            if (i1 > i0 && logs + rep > budget) break;
             mc = c;
             if (in_len[i1] > mx) mx = in_len[i1];
             i1++;
         }
         if (mc.cmd + mc.lit > 0xffffffffull) { ctx->err = "stream too large"; return DIVANS_FAILURE; }   // (the kernels' 32-bit log stride)
         const size_t m = i1 - i0;
-        uint64_t out_lo, out_hi;
-        regions_span(m, out_off + i0, out_cap + i0, out_lo, out_hi);
-        if (!grow(ctx, &b.d_out, &b.d_out_cap, (size_t)(out_hi - out_lo) + 64)) return DIVANS_FAILURE;
-        // in_off | in_len | out_off | out_cap | out_len | status, then the selection's outputs: chosen | cost | halves | mixing | bins
+        uint64_t out_lo = 0, out_hi = 0;
+        if (out) {
+            regions_span(m, out_off + i0, out_cap + i0, out_lo, out_hi);
+            if (!grow(ctx, &b.d_out, &b.d_out_cap, (size_t)(out_hi - out_lo) + 64)) return DIVANS_FAILURE;
+        }
+        // in_off | in_len | out_off | out_cap | out_len | status, then the selection's outputs: chosen | cost | halves | mixing | bins | bill
         const size_t chosen_words = (lay.chosen_cols + 1) / 2;
         if (!grow(ctx, &b.d_meta, &b.d_meta_cap,
-                  m * (6 + chosen_words + lay.cost_cols + lay.halves_cols + lay.mixing_bytes / 8 + lay.bins_cols))) return DIVANS_FAILURE;
-        std::vector<uint64_t> rel(m);
-        for (size_t i = 0; i < m; i++) rel[i] = out_off[i0 + i] - out_lo;
+                  m * (6 + chosen_words + lay.cost_cols + lay.halves_cols + lay.mixing_bytes / 8 + lay.bins_cols + lay.bill_cols))) return DIVANS_FAILURE;
+        std::vector<uint64_t> rel(out ? m : 0);
+        for (size_t i = 0; i < rel.size(); i++) rel[i] = out_off[i0 + i] - out_lo;
         uint64_t *mm = b.d_meta;
         CK(cudaMemcpyAsync(mm, s_off.data() + i0, m * 8, cudaMemcpyHostToDevice, st));
         CK(cudaMemcpyAsync(mm + m, in_len + i0, m * 8, cudaMemcpyHostToDevice, st));
-        CK(cudaMemcpyAsync(mm + 2 * m, rel.data(), m * 8, cudaMemcpyHostToDevice, st));
-        CK(cudaMemcpyAsync(mm + 3 * m, out_cap + i0, m * 8, cudaMemcpyHostToDevice, st));
+        if (out) {
+            CK(cudaMemcpyAsync(mm + 2 * m, rel.data(), m * 8, cudaMemcpyHostToDevice, st));
+            CK(cudaMemcpyAsync(mm + 3 * m, out_cap + i0, m * 8, cudaMemcpyHostToDevice, st));
+        }
         int32_t *d_status = reinterpret_cast<int32_t *>(mm + 5 * m);
         // the selection with its outputs in d_meta: chosen and cost always, the others where the caller asked for them
         Selection ds = sel;
@@ -1250,8 +1294,10 @@ static DivansResult encode_host_common(divans_b200_ctx *ctx, size_t n, int raw_m
         ds.cost = w; w += m * lay.cost_cols;
         ds.halves = sel.halves ? w : nullptr; w += m * lay.halves_cols;
         ds.mixing = sel.mixing ? reinterpret_cast<uint8_t *>(w) : nullptr; w += m * lay.mixing_bytes / 8;
-        ds.bins = sel.bins ? w : nullptr;
-        const EncBatch eb = {m, raw_mode, b.d_in, mm, mm + m, mx, mc, b.d_out, mm + 2 * m, mm + 3 * m, mm + 4 * m, d_status, opts, window, st};
+        ds.bins = sel.bins ? w : nullptr; w += m * lay.bins_cols;
+        ds.bill = sel.bill ? w : nullptr;
+        const EncBatch eb = {m, raw_mode, b.d_in, mm, mm + m, mx, mc, out ? b.d_out : nullptr, mm + 2 * m, mm + 3 * m, mm + 4 * m, d_status, opts,
+                             window, st};
         DivansResult r = encode_nolock(ctx, eb, ds);
         if (r != DIVANS_SUCCESS) return r;
         if (sel.chosen) CK(cudaMemcpyAsync(sel.chosen + i0 * lay.chosen_cols, ds.chosen, m * lay.chosen_cols * 4, cudaMemcpyDeviceToHost, st));
@@ -1259,10 +1305,11 @@ static DivansResult encode_host_common(divans_b200_ctx *ctx, size_t n, int raw_m
         if (sel.cost) CK(cudaMemcpyAsync(sel.cost + i0 * lay.cost_cols, ds.cost, m * lay.cost_cols * 8, cudaMemcpyDeviceToHost, st));
         if (sel.mixing) CK(cudaMemcpyAsync(sel.mixing + i0 * lay.mixing_bytes, ds.mixing, m * lay.mixing_bytes, cudaMemcpyDeviceToHost, st));
         if (sel.bins) CK(cudaMemcpyAsync(sel.bins + i0 * lay.bins_cols, ds.bins, m * lay.bins_cols * 8, cudaMemcpyDeviceToHost, st));
-        CK(cudaMemcpyAsync(out_len + i0, mm + 4 * m, m * 8, cudaMemcpyDeviceToHost, st));
+        if (sel.bill) CK(cudaMemcpyAsync(sel.bill + i0 * lay.bill_cols, ds.bill, m * lay.bill_cols * 8, cudaMemcpyDeviceToHost, st));
+        if (out_len) CK(cudaMemcpyAsync(out_len + i0, mm + 4 * m, m * 8, cudaMemcpyDeviceToHost, st));
         CK(cudaMemcpyAsync(status + i0, d_status, m * 4, cudaMemcpyDeviceToHost, st));
         CK(cudaStreamSynchronize(st));
-        for (size_t i = i0; i < i1; i++) {
+        for (size_t i = i0; i < i1 && out; i++) {
             if (status[i] == DIVANS_SUCCESS && out_len[i]) CK(cudaMemcpyAsync(out + out_off[i], b.d_out + (out_off[i] - out_lo), out_len[i], cudaMemcpyDeviceToHost, st));
         }
         CK(cudaStreamSynchronize(st));
@@ -1298,6 +1345,31 @@ extern "C" DivansResult divans_b200_encode_cmds_auto_batch_host(divans_b200_ctx 
                                                                 const divans_b200_encode_options *opts, const divans_b200_literal_model *cands,
                                                                 uint32_t n_cands, uint32_t *chosen, uint64_t *cost) {
     return encode_host_common(ctx, n, 0, blobs, blob_off, blob_len, out, out_off, out_cap, out_len, status, opts, sel_auto(cands, n_cands, chosen, cost));
+}
+
+// ---- billing by coder state ----
+extern "C" DivansResult divans_b200_bill_batch_host(divans_b200_ctx *ctx, size_t n, const uint8_t *in, const uint64_t *in_off,
+                                                    const uint64_t *in_len, const divans_b200_encode_options *opts, uint64_t *bill,
+                                                    int32_t *status) {
+    return encode_host_common(ctx, n, 1, in, in_off, in_len, nullptr, nullptr, nullptr, nullptr, status, opts, sel_bill(bill));
+}
+extern "C" DivansResult divans_b200_bill_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_in, const uint64_t *d_in_off,
+                                                      const uint64_t *d_in_len, uint64_t max_in_len, const divans_b200_encode_options *opts,
+                                                      uint64_t *d_bill, int32_t *d_status, void *cuda_stream) {
+    return encode_device_common(ctx, n, 1, d_in, d_in_off, d_in_len, max_in_len, max_in_len, nullptr, nullptr, nullptr, nullptr, d_status,
+                                opts, cuda_stream, sel_bill(d_bill));
+}
+extern "C" DivansResult divans_b200_bill_cmds_batch_host(divans_b200_ctx *ctx, size_t n, const uint8_t *blobs, const uint64_t *blob_off,
+                                                         const uint64_t *blob_len, const divans_b200_encode_options *opts, uint64_t *bill,
+                                                         int32_t *status) {
+    return encode_host_common(ctx, n, 0, blobs, blob_off, blob_len, nullptr, nullptr, nullptr, nullptr, status, opts, sel_bill(bill));
+}
+extern "C" DivansResult divans_b200_bill_cmds_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_blobs, const uint64_t *d_blob_off,
+                                                           const uint64_t *d_blob_len, uint64_t max_blob_len, uint64_t max_raw_len,
+                                                           const divans_b200_encode_options *opts, uint64_t *d_bill, int32_t *d_status,
+                                                           void *cuda_stream) {
+    return encode_device_common(ctx, n, 0, d_blobs, d_blob_off, d_blob_len, max_blob_len, max_raw_len, nullptr, nullptr, nullptr, nullptr,
+                                d_status, opts, cuda_stream, sel_bill(d_bill));
 }
 
 // ---- per-context mixing values ----

@@ -15,8 +15,25 @@
 //   3. encode_mux_kernel    one warp per stream: header, the record chain of Mux::serialize_close with everything
 //                           still buffered (mux.rs:478-561), EOF marker, CRC32C and trailer (codec/mod.rs:493-560).
 #include "dv_core.cuh"
+#include "../../include/divans_b200.h"
 
 namespace dv {
+
+// BILL: row r of a stream's bill is state r + S_CMD_TYPE (include/divans_b200.h, "billing each stream's coding cost by coder state")
+constexpr uint32_t BILL_WORDS = 2 * DIVANS_B200_BILL_STATES;   // (cost, nibbles) per row
+static_assert(S_PM_MIXVAL - S_CMD_TYPE + 1 == DIVANS_B200_BILL_STATES && S_DICT_EMIT == S_PM_MIXVAL + 1,
+              "the bill has one row per nibble-coding state");
+static_assert(S_LIT_HI - S_CMD_TYPE == 1 && S_LL_COUNT_SMALL - S_CMD_TYPE == 3 && S_CP_COUNT_SMALL - S_CMD_TYPE == 7 &&
+              S_CP_MNEMONIC - S_CMD_TYPE == 11 && S_DC_SIZE_BEG - S_CMD_TYPE == 15 && S_BT_MNEMONIC - S_CMD_TYPE == 20 &&
+              S_PM_MODE - S_CMD_TYPE == 24 && S_PM_MAP_MNEMONIC - S_CMD_TYPE == 28, "the states in the order of the header's row table");
+// the rows of each group in dynamic shared memory, after the groups' cold states
+constexpr size_t BILL_SMEM_BYTES = (size_t)(DECODE_BLOCK_THREADS / 16) * (SMEM_BYTES_PER_GROUP + BILL_WORDS * 8);
+
+// BILL: the end of stream v (status `ok`): its bill is the group's rows, or zeros for a stream that failed
+__device__ __forceinline__ void fold_bill(const G2 g, const uint64_t *rows, uint64_t *bill, uint32_t v, bool ok) {
+    __syncwarp(g.gmask);   // the group's store lane added the last nibble
+    for (uint32_t e = (uint32_t)g.l16; e < BILL_WORDS; e += 16) bill[(uint64_t)v * BILL_WORDS + e] = ok ? rows[e] : 0ull;
+}
 
 // BINS: the end of pair v (status `ok`): fold the slot's bins into stream i's per-entry minimum (cost << 4) | c; a failed pair
 // takes no part and reports UINT64_MAX bins
@@ -35,8 +52,11 @@ __device__ __forceinline__ void fold_bins(const G2 g, const uint64_t *sbins, con
 // loops do not track the mixing-mask index.
 // SPEEDS (encode_speeds_kernel): each stream codes with its own literal speeds, p.v_adapt; with TALLY the pass also sums the
 // cost of the literal high nibbles and of all literal nibbles (LitHalves), on the fast loops as on the generic path.
-template <bool BLEND, bool TALLY, bool BINS, bool SPEEDS>
-__device__ __forceinline__ void encode_model_walk(const EncodeParams &p, const BinParams &bp) {
+// BILL (encode_bill_kernel: TALLY as well) adds each coded nibble's cost and count to the group's row of the state that coded
+// it, in shared memory, and writes the rows to bill[v] when stream v ends.  The literal fast loops keep running: they split
+// their cost into the high and low nibbles (LitHalves), and the bytes they coded are the count of both rows.
+template <bool BLEND, bool TALLY, bool BINS, bool SPEEDS, bool BILL = false>
+__device__ __forceinline__ void encode_model_walk(const EncodeParams &p, const BinParams &bp, uint64_t *bill = nullptr) {
     extern __shared__ __align__(16) uint8_t smem[];
     const int lane = threadIdx.x & 31;
     const int group_in_block = (threadIdx.x >> 5) * 2 + (lane >> 4);
@@ -69,6 +89,8 @@ __device__ __forceinline__ void encode_model_walk(const EncodeParams &p, const B
     bool exhausted = false;
     const uint32_t per_stream = p.cmd_cap + p.lit_cap;
     uint64_t *const sbins = BINS ? bp.slot_bins + (uint64_t)slot * MIX_ENTRIES : nullptr;
+    uint64_t *const rows = BILL ? reinterpret_cast<uint64_t *>(smem + (DECODE_BLOCK_THREADS / 16) * SMEM_BYTES_PER_GROUP) + group_in_block * BILL_WORDS
+                                : nullptr;
     // Every cost pass under SPEEDS tallies the halves; only the halves passes' are read (at dynamic mixing 2, where the records'
     // literals take the mixing loop).  One kernel for all cost passes keeps the uniform, halves and verify walks identical.
     constexpr bool HALVES = SPEEDS && TALLY;
@@ -139,9 +161,14 @@ __device__ __forceinline__ void encode_model_walk(const EncodeParams &p, const B
                             if constexpr (TALLY) p.tally[v] = 0; else { p.sf_counts[2 * v] = 0; p.sf_counts[2 * v + 1] = 0; }
                         }
                         if constexpr (BINS) fold_bins(g, sbins, bp, v, false);
+                        if constexpr (BILL) fold_bill(g, rows, bill, v, false);
                     } else if constexpr (TALLY) {
                         if constexpr (BINS) {
                             for (uint32_t e = (uint32_t)g.l16; e < MIX_ENTRIES; e += 16) sbins[e] = 0;
+                            __syncwarp(g.gmask);
+                        }
+                        if constexpr (BILL) {
+                            for (uint32_t e = (uint32_t)g.l16; e < BILL_WORDS; e += 16) rows[e] = 0;
                             __syncwarp(g.gmask);
                         }
                         if constexpr (HALVES) hv = LitHalves{0, 0};
@@ -166,6 +193,7 @@ __device__ __forceinline__ void encode_model_walk(const EncodeParams &p, const B
             if (g.store0 && TALLY) { p.status[v] = s.status; p.tally[v] = s.cur.a + s.c->oth.a; }
             if constexpr (HALVES) if (g.store0) { p.halves[2ull * v] = hv.lit - hv.hi; p.halves[2ull * v + 1] = hv.hi; }
             if constexpr (BINS) fold_bins(g, sbins, bp, v, s.status == ST_OK);
+            if constexpr (BILL) fold_bill(g, rows, bill, v, s.status == ST_OK);
             if (g.store0 && !TALLY) {
                 p.status[v] = s.status;
                 const uint32_t nc = s.c->cur_is_lit ? s.c->oth.left : s.cur.left, nl = s.c->cur_is_lit ? s.cur.left : s.c->oth.left;
@@ -177,8 +205,16 @@ __device__ __forceinline__ void encode_model_walk(const EncodeParams &p, const B
         };
         if (!BLEND && !BINS && __all_sync(FULL, s.state == S_LIT_HI)) {
             const uint64_t a_in = s.cur.a;
-            literal_fast_enc<TALLY, HALVES>(s, nx, g, &hv);
+            const uint32_t left_in = s.lit_left;
+            if constexpr (BILL) hv.hi = 0;
+            literal_fast_enc<TALLY, HALVES || BILL>(s, nx, g, &hv);
             if constexpr (HALVES) hv.lit += s.cur.a - a_in;
+            if constexpr (BILL) if (g.store0) {   // the bytes the loop coded: as many high as low nibbles
+                const uint64_t n = left_in - s.lit_left;
+                uint64_t *const hi = rows + 2 * (S_LIT_HI - S_CMD_TYPE), *const lo = rows + 2 * (S_LIT_LO - S_CMD_TYPE);
+                hi[0] += hv.hi; hi[1] += n;
+                lo[0] += s.cur.a - a_in - hv.hi; lo[1] += n;
+            }
             if (s.lit_left == 0 && s.status == ST_OK) { swap_coders(s, g); s.c->in.pos++; enter_cmd_type<true>(s, nx); }
             if (s.status != ST_OK) finish();   // a symbol the loop could not code (enc_log): the stream ends here
             continue;
@@ -195,7 +231,10 @@ __device__ __forceinline__ void encode_model_walk(const EncodeParams &p, const B
             lit_hi = s.state == S_LIT_HI; lit_nib = lit_hi || s.state == S_LIT_LO;
             a0 = s.cur.a;
         }
+        const int st0 = s.state;
+        if constexpr (BILL) a0 = s.cur.a;
         int sym = core_dispatch<BLEND, TALLY>(s, nx, g);
+        if constexpr (BILL) if (busy && g.store0) { uint64_t *const r = rows + 2 * (st0 - S_CMD_TYPE); r[0] += s.cur.a - a0; r[1] += 1; }
         if constexpr (BINS) if (lit_nib && g.store0) sbins[mmi] += s.cur.a - a0;
         if constexpr (HALVES) if (lit_nib) { const uint64_t d = s.cur.a - a0; hv.lit += d; if (lit_hi) hv.hi += d; }
         if (!busy) s.cur.left = 0;
@@ -224,6 +263,11 @@ __global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) encode_bins_kernel(En
 template <bool BLEND, bool TALLY>
 __global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) encode_speeds_kernel(EncodeParams p) {
     encode_model_walk<BLEND, TALLY, false, true>(p, BinParams{});
+}
+// the cost pass with each stream's cost billed by coder state (divans_b200_bill_*): bill [n_streams * BILL_WORDS]
+template <bool BLEND>
+__global__ void __launch_bounds__(DECODE_BLOCK_THREADS, 8) encode_bill_kernel(EncodeParams p, uint64_t *bill) {
+    encode_model_walk<BLEND, true, false, false, true>(p, BinParams{}, bill);
 }
 
 #ifndef DV_BLEND   // (the rANS / mux passes do not depend on the probability model: they live in the default translation unit)
@@ -477,10 +521,17 @@ void launch_encode_walk(EncodeWalk w, const EncodeParams &p, const BinParams &b,
     }
 }
 
+template <bool BLEND>
+void launch_encode_bill(const EncodeParams &p, uint64_t *bill, uint32_t n_blocks, cudaStream_t st) {
+    encode_bill_kernel<BLEND><<<n_blocks, DECODE_BLOCK_THREADS, BILL_SMEM_BYTES, st>>>(p, bill);
+}
+
 #ifdef DV_BLEND
 template void launch_encode_walk<true>(EncodeWalk, const EncodeParams &, const BinParams &, uint32_t, cudaStream_t);
+template void launch_encode_bill<true>(const EncodeParams &, uint64_t *, uint32_t, cudaStream_t);
 #else
 template void launch_encode_walk<false>(EncodeWalk, const EncodeParams &, const BinParams &, uint32_t, cudaStream_t);
+template void launch_encode_bill<false>(const EncodeParams &, uint64_t *, uint32_t, cudaStream_t);
 
 // ---------------------------------------------------------------------------------------------------------------
 // literal speeds (divans_b200_encode_speeds_*): n streams x k candidate speeds v[0..k), pairs candidate-major (v = c * n + i)

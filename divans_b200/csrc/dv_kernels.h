@@ -28,6 +28,8 @@ int decode_groups_per_block_v2(int lanes_per_stream);
 // blend model.  dv_encode.cu instantiates BLEND = false, and built with DV_BLEND, true.
 enum class EncodeWalk { MODEL, TALLY, BINS, SPEEDS_MODEL, SPEEDS };
 template <bool BLEND> void launch_encode_walk(EncodeWalk w, const EncodeParams &p, const BinParams &b, uint32_t n_blocks, cudaStream_t st);
+// the cost pass of p (TALLY) billed by coder state into bill [p.n_streams * 2 * DIVANS_B200_BILL_STATES] (include/divans_b200.h)
+template <bool BLEND> void launch_encode_bill(const EncodeParams &p, uint64_t *bill, uint32_t n_blocks, cudaStream_t st);
 void launch_encode_flush_mux(const EncodeParams &p, cudaStream_t st);                  // reverse rANS + mux/CRC (2 launches)
 int encode_max_blocks_per_sm();
 void launch_rcp15_init(uint64_t *tab, cudaStream_t st);

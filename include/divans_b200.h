@@ -697,6 +697,78 @@ DivansResult divans_b200_encode_cmds_choose_batch_device(divans_b200_ctx *ctx, s
                                                          const uint64_t *d_out_cap, uint64_t *d_out_len, int32_t *d_status,
                                                          const divans_b200_encode_options *opts, uint32_t *d_chosen, uint64_t *d_cost,
                                                          void *cuda_stream);
+/* ---- billing each stream's coding cost by coder state ----
+ * The cost pass (encode_auto's cost, encode_cmds_choose's d_cost) gives one number per stream.  The bill splits that number by
+ * the state of the encoder's command state machine that coded each nibble, as the reference's billing build does
+ * (BillingDesignation, src/interface.rs:328-346; there the mantissa nibble states are folded together, here they are rows).
+ *  - A stream's bill has DIVANS_B200_BILL_STATES rows, one per nibble-coding state, in the order of the table below (row index,
+ *    name, the reference substate).  The order is part of the interface.
+ *  - Each row holds two uint64_t: cost, the sum of T[freq] (1/65536 bit, as encode_auto) over every nibble coded in that state
+ *    by either coder; nibbles, how many nibbles were coded in it.
+ *  - A nibble's state is the state the encoder was in when it coded that nibble.  A literal byte is one LIT_HI and one LIT_LO
+ *    nibble; the end-of-stream nibble is a CMD_TYPE nibble.
+ *  - The sum of a stream's cost column equals, to the unit, the cost the cost pass gives the same stream under the same options
+ *    and list: encode_auto's cost for that candidate, encode_cmds_choose's d_cost for that list.
+ *  - A stream whose pass fails has status 3 (or 2, a command list that replays past max_raw_len) and an all-zero bill: the
+ *    failures for which the cost pass gives UINT64_MAX (a refused record, a speed that wraps, a list that outgrows the logs).
+ *  - Nothing is encoded and no output stream is written.
+ * Rows (index  name              reference substate):
+ *    0 CMD_TYPE          CrossCommandBilling::FullSelection: command type, end-of-stream nibble         codec/mod.rs:662-688
+ *    1 LIT_HI            LiteralSubstate::LiteralNibbleIndex                                            codec/literal.rs:261-394
+ *    2 LIT_LO            LiteralSubstate::LiteralNibbleLowerHalf
+ *    3 LL_COUNT_SMALL    LiteralSubstate::LiteralCountSmall                                             codec/literal.rs:565-661
+ *    4 LL_SIZE_BEG       LiteralSubstate::LiteralCountFirst
+ *    5 LL_SIZE_LAST      LiteralSubstate::LiteralCountLengthGreater14Less25
+ *    6 LL_MANT           LiteralSubstate::LiteralCountMantissaNibbles
+ *    7 CP_COUNT_SMALL    CopySubstate::CountSmall                                                       codec/copy.rs:87-162
+ *    8 CP_COUNT_BEG      CopySubstate::CountLengthFirst
+ *    9 CP_COUNT_LAST     CopySubstate::CountLengthGreater18Less25
+ *   10 CP_COUNT_MANT     CopySubstate::CountMantissaNibbles
+ *   11 CP_MNEMONIC       CopySubstate::DistanceLengthMnemonic                                           codec/copy.rs:166-280
+ *   12 CP_DIST_BEG       CopySubstate::DistanceLengthFirst
+ *   13 CP_DIST_LAST      CopySubstate::DistanceLengthGreater14Less25
+ *   14 CP_DIST_MANT      CopySubstate::DistanceMantissaNibbles
+ *   15 DC_SIZE_BEG       DictSubstate::WordSizeFirst                                                    codec/dict.rs:81-170
+ *   16 DC_SIZE_LAST      DictSubstate::WordSizeGreater18Less25
+ *   17 DC_INDEX          DictSubstate::WordIndexMantissa
+ *   18 DC_TR_HI          DictSubstate::TransformHigh
+ *   19 DC_TR_LO          DictSubstate::TransformLow
+ *   20 BT_MNEMONIC       BlockTypeState::Begin                                                          codec/block_type.rs:61-110
+ *   21 BT_FIRST          BlockTypeState::TwoNibbleType
+ *   22 BT_SECOND         BlockTypeState::FinalNibble
+ *   23 BT_STRIDE         LiteralBlockSwitch's stride nibble                                             codec/block_type.rs:170-190
+ *   24 PM_MODE           PredictionModeSubstate::Begin                                                  context_map.rs:172-425
+ *   25 PM_MIX            PredictionModeSubstate::DynamicContextMixing
+ *   26 PM_DEPTH          PredictionModeSubstate::PriorDepth
+ *   27 PM_SPEED          PredictionModeSubstate::AdaptationSpeed
+ *   28 PM_MAP_MNEMONIC   PredictionModeSubstate::ContextMapMnemonic
+ *   29 PM_MAP_FIRST      PredictionModeSubstate::ContextMapFirstNibble
+ *   30 PM_MAP_SECOND     PredictionModeSubstate::ContextMapSecondNibble
+ *   31 PM_MIXVAL         PredictionModeSubstate::MixingValues
+ * (32 rows in all; see DIVANS_B200_BILL_STATES.) */
+#define DIVANS_B200_BILL_STATES 32
+/* Raw buffers, coded as divans_b200_encode_batch_host codes them: the literal-only list with the record of
+ * opts->literal_pred_mode and literal_mixing_value.  bill [n * DIVANS_B200_BILL_STATES * 2]: (cost, nibbles) of stream i, row r
+ * at (i * DIVANS_B200_BILL_STATES + r) * 2; status [n].  Sub-batched like divans_b200_encode_auto_batch_host.  Options apply as
+ * in the encoders, both probability models and DIVANS_B200_MODEL_WASM_2018 included.  n == 0 returns DIVANS_SUCCESS. */
+DivansResult divans_b200_bill_batch_host(divans_b200_ctx *ctx, size_t n, const uint8_t *in, const uint64_t *in_off,
+                                         const uint64_t *in_len, const divans_b200_encode_options *opts, uint64_t *bill,
+                                         int32_t *status);
+/* Same with the buffers, d_bill and d_status DEVICE pointers: one launch sequence, no host synchronisation, asynchronous on
+ * cuda_stream and serialised on the context; divans_b200_last_kernel_ms times the billing pass afterwards. */
+DivansResult divans_b200_bill_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_in, const uint64_t *d_in_off,
+                                           const uint64_t *d_in_len, uint64_t max_in_len, const divans_b200_encode_options *opts,
+                                           uint64_t *d_bill, int32_t *d_status, void *cuda_stream);
+/* DVCL command lists under their own records, with every convention of divans_b200_encode_cmds_batch_host / _device:
+ * window_size 0 = each list's header window; device blobs 4-byte aligned, at most max_blob_len bytes, replaying at most
+ * max_raw_len bytes (else status 3, or 2 past max_raw_len).  Outputs and synchronisation as the raw calls. */
+DivansResult divans_b200_bill_cmds_batch_host(divans_b200_ctx *ctx, size_t n, const uint8_t *blobs, const uint64_t *blob_off,
+                                              const uint64_t *blob_len, const divans_b200_encode_options *opts, uint64_t *bill,
+                                              int32_t *status);
+DivansResult divans_b200_bill_cmds_batch_device(divans_b200_ctx *ctx, size_t n, const uint8_t *d_blobs, const uint64_t *d_blob_off,
+                                                const uint64_t *d_blob_len, uint64_t max_blob_len, uint64_t max_raw_len,
+                                                const divans_b200_encode_options *opts, uint64_t *d_bill, int32_t *d_status,
+                                                void *cuda_stream);
 /*
  * command list blob ("DVCL", little endian) -- the binary form of the reference's IR (src/bin/divans.rs:191-483):
  *   u32 magic 0x4c435644, u32 version 1, u32 n_cmds, u32 n_predmodes, u32 n_literal_bytes, u32 window, u32[2] 0

@@ -656,3 +656,28 @@ int dvo_encode_cmds_choose(const dvo_cmdlist *const *lists, uint32_t k, const dv
     *out_len = 0;
     return dvo_encode_cmds(lists[arg], o, out, cap, out_len);
 }
+
+/* ---- billing by coder state (include/divans_b200.h, "billing each stream's coding cost by coder state") ----
+ * While dvt_rows is set, ans_enc_put also adds each symbol's cost and a count of one to row dvt_row of the bill: tally_py.py makes
+ * every nibble-coding call of the encoder name the row of its own substate just before it codes, and ans_enc_put clears it.  A
+ * nibble coded where no call named a row goes to row DVT_BILL_ROWS, and a walk with any such nibble is refused.  rows
+ * [DVT_BILL_ROWS * 2]: (cost, nibbles) per row, all zero when the walk fails; *cost as dvo_tally_cmds. */
+int dvo_bill_cmds(const dvo_cmdlist *l, const dvo_options *o, uint64_t *cost, uint64_t *rows) {
+    uint64_t r[2 * (DVT_BILL_ROWS + 1)];
+    memset(r, 0, sizeof r);
+    dvt_rows = r; dvt_row = -1;
+    int rc = dvo_tally_cmds(l, o, cost);
+    dvt_rows = NULL; dvt_row = -1;
+    if (rc == DVO_SUCCESS && r[2 * DVT_BILL_ROWS + 1] != 0) { rc = DVO_FAILURE; *cost = UINT64_MAX; }
+    if (rc != DVO_SUCCESS) memset(r, 0, sizeof r);
+    memcpy(rows, r, 2 * DVT_BILL_ROWS * sizeof *rows);
+    return rc;
+}
+
+int dvo_bill_raw(const uint8_t *in, size_t n, const dvo_options *o, int pred_mode, int mixing_value, uint64_t *cost, uint64_t *rows) {
+    dvo_cmdlist l; dvo_cmdlist_init(&l);
+    dvt_raw_cmds(in, n, o->window_size, pred_mode, mixing_value, &l);
+    int rc = dvo_bill_cmds(&l, o, cost, rows);
+    dvo_cmdlist_free(&l);
+    return rc;
+}

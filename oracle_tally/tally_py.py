@@ -5,6 +5,8 @@ TEST INFRASTRUCTURE: imported only by tests/ and tools/.  Nothing under divans_b
 build() writes oracle_tally/_build/divans_oracle_tally.c: oracle/divans_oracle.c (read, never modified) with one hook in
 ans_enc_put -- while a tally is running, each symbol adds the cost of its frequency to the tally instead of being recorded --
 and a second one at the literal nibble's mixing-mask read -- the index becomes the bin of that nibble's cost --
+and the billing hook -- each nibble-coding call of the encoder names its row of the bill (BILL_ROWS) just before it codes, and
+ans_enc_put adds the symbol's cost to that row --
 and three forging hooks -- every command nibble the encoder codes passes through dvt_forge_nib, a command-type nibble other than
 the record's type ends the walk, and a walk that fails after a forged nibble is still flushed and framed --
 followed by tally_api.c, and compiles it twice, with the reference's default probability model and with feature="blend", as
@@ -12,7 +14,8 @@ the oracle's own Makefile does.  Every function of the oracle is in these librar
 the tally entry points, dvo_cmdlist_set_mixing (a test's own mixing values in a list), dvo_recode_blob (the CPU reference of
 the library's command-list replay, on the serialised blob), dvo_cmdlist_from_blob, dvo_encode_cmds_forged, dvo_lz77_cmds_parse
 (the LZ77 generator under a parse), dvo_lz77_cmds_dict_parse (the same with dictionary words), dvo_lz77_cmds_words_parse (with
-dictionary words under every transform) and dvo_encode_cmds_choose (one of k command lists chosen by cost) are new.
+dictionary words under every transform), dvo_encode_cmds_choose (one of k command lists chosen by cost) and dvo_bill_cmds /
+dvo_bill_raw (the cost billed by coder state) are new.
 """
 import ctypes
 import os
@@ -38,7 +41,8 @@ _PUT_TALLIED = _PUT + ("    if (dvt_tally) {   /* (oracle_tally) */\n"
                        "        const uint32_t dvt_c = dvt_freq_cost((uint32_t)freq);\n"
                        "        *dvt_tally += dvt_c;\n"
                        "        if (dvt_bins) { if (dvt_bin >= 0) dvt_bins[dvt_bin] += dvt_c; else *dvt_nobin += dvt_c; }\n"
-                       "        dvt_bin = -1; e->n_syms++; return;\n"
+                       "        if (dvt_rows) { const int32_t r = dvt_row >= 0 ? dvt_row : DVT_BILL_ROWS; dvt_rows[2 * r] += dvt_c; dvt_rows[2 * r + 1]++; }\n"
+                       "        dvt_bin = -1; dvt_row = -1; e->n_syms++; return;\n"
                        "    }\n")
 # the second hook: a literal nibble's mixing-mask index becomes the bin of the nibble coded next (ans_enc_put clears it)
 _MM = "    uint8_t mm_opts = s->mixing_mask[mmi];\n"
@@ -83,7 +87,50 @@ _PREFIX = ("/* generated by oracle_tally/tally_py.py from oracle/divans_oracle.c
            "static __thread uint32_t *dvt_cov;   /* set: every coded command nibble counts in dvt_cov[flat prior * 16 + nibble] */\n"
            "static __thread void *dvt_codec;   /* the codec of the running encode */\n"
            "static void dvt_cov_add(const void *cdf, uint8_t nib);\n"
+           "#define DVT_BILL_ROWS %d   /* the bill's rows; one more collects a nibble coded where no call named its row */\n"
+           "static __thread uint64_t *dvt_rows;   /* set: each cost also goes to row dvt_row of the bill (cost, nibbles) */\n"
+           "static __thread int32_t dvt_row = -1;   /* the row of the nibble being coded, named by its coding call, or -1 */\n"
            "#line 1 \"oracle/divans_oracle.c\"\n")
+
+
+# The bill's rows (include/divans_b200.h, "billing each stream's coding cost by coder state"), and which of the oracle's nibble-coding
+# calls codes each: its own prior types (the P() type of a code_and_blend call of the command coder) mapped onto the rows.  A call
+# whose prior names no row, or two, stops the build.
+BILL_ROWS = ["CMD_TYPE", "LIT_HI", "LIT_LO", "LL_COUNT_SMALL", "LL_SIZE_BEG", "LL_SIZE_LAST", "LL_MANT", "CP_COUNT_SMALL", "CP_COUNT_BEG",
+             "CP_COUNT_LAST", "CP_COUNT_MANT", "CP_MNEMONIC", "CP_DIST_BEG", "CP_DIST_LAST", "CP_DIST_MANT", "DC_SIZE_BEG", "DC_SIZE_LAST",
+             "DC_INDEX", "DC_TR_HI", "DC_TR_LO", "BT_MNEMONIC", "BT_FIRST", "BT_SECOND", "BT_STRIDE", "PM_MODE", "PM_MIX", "PM_DEPTH",
+             "PM_SPEED", "PM_MAP_MNEMONIC", "PM_MAP_FIRST", "PM_MAP_SECOND", "PM_MIXVAL"]
+_ROW_OF_PRIOR = {
+    "CC_FullSelection,": "CMD_TYPE",
+    "LL_CountSmall,": "LL_COUNT_SMALL", "LL_SizeBegNib,": "LL_SIZE_BEG", "LL_SizeLastNib,": "LL_SIZE_LAST", "LL_SizeMantissaNib,": "LL_MANT",
+    "CP_CountSmall,": "CP_COUNT_SMALL", "CP_CountBegNib,": "CP_COUNT_BEG", "CP_CountLastNib,": "CP_COUNT_LAST",
+    "CP_CountMantissaNib,": "CP_COUNT_MANT", "CP_DistanceMnemonic,": "CP_MNEMONIC", "CP_DistanceBegNib,": "CP_DIST_BEG",
+    "CP_DistanceLastNib,": "CP_DIST_LAST", "CP_DistanceMantissaNib,": "CP_DIST_MANT",
+    "DC_SizeBegNib,": "DC_SIZE_BEG", "DC_SizeLastNib,": "DC_SIZE_LAST", "DC_Index,": "DC_INDEX",
+    "DC_Transform, 0,": "DC_TR_HI", "DC_Transform, 1,": "DC_TR_LO",
+    "BT_Mnemonic,": "BT_MNEMONIC", "BT_FirstNibble,": "BT_FIRST", "BT_SecondNibble,": "BT_SECOND", "BT_StrideNibble,": "BT_STRIDE",
+    "PM_Only,": "PM_MODE", "PM_DynamicContextMixingSpeed,": "PM_MIX", "PM_PriorDepth,": "PM_DEPTH", "PM_ContextMapSpeedPalette,": "PM_SPEED",
+    "mn_prior,": "PM_MAP_MNEMONIC", "PM_FirstNibble,": "PM_MAP_FIRST", "PM_SecondNibble,": "PM_MAP_SECOND",
+    "PM_PriorMixingValue,": "PM_MIXVAL",
+}
+_CMD_CALL = "code_and_blend(&s->cmd, "
+_LIT_CALL = "code_nibble(&s->lit, "   # the literal nibbles (code_lit_nibble): high or low by its is_high
+
+
+def _bill_hooked(src):
+    """``src`` with every nibble-coding call of the encoder naming its bill row first: code_and_blend((dvt_row = r, &s->cmd), ...)"""
+    out = []
+    for line in src.split("\n"):
+        if _CMD_CALL in line:
+            assert line.count(_CMD_CALL) == 1, line
+            rows = {r for k, r in _ROW_OF_PRIOR.items() if k in line.split(_CMD_CALL, 1)[1]}
+            if len(rows) != 1:
+                raise RuntimeError("oracle_tally: no single bill row for the oracle's call: " + line.strip())
+            line = line.replace(_CMD_CALL, "code_and_blend((dvt_row = %d, &s->cmd), " % BILL_ROWS.index(rows.pop()))
+        elif _LIT_CALL in line:
+            line = line.replace(_LIT_CALL, "code_nibble((dvt_row = is_high ? %d : %d, &s->lit), " % (BILL_ROWS.index("LIT_HI"), BILL_ROWS.index("LIT_LO")))
+        out.append(line)
+    return "\n".join(out)
 
 
 def _lib_path(blend):
@@ -108,8 +155,11 @@ def build(force=False):
     os.makedirs(_BUILD, exist_ok=True)
     hooked = oracle.replace(_PUT, _PUT_TALLIED).replace(_MM, _MM_TALLIED)
     hooked = hooked.replace(_CAB, _CAB_FORGED).replace(_TYPE, _TYPE_FORGED).replace(_FLUSH, _FLUSH_FORGED).replace(_LIT, _LIT_FORGED).replace(_INIT, _INIT_COV)
+    if hooked.count(_LIT_CALL) != 2:
+        raise RuntimeError("oracle_tally: the literal nibbles of oracle/divans_oracle.c are not the ones the billing hook was written for")
+    hooked = _bill_hooked(hooked)
     with open(_SRC + ".tmp", "w") as f:
-        f.write(_PREFIX + hooked + '\n#line 1 "oracle_tally/tally_api.c"\n' + open(_API_C).read())
+        f.write(_PREFIX % len(BILL_ROWS) + hooked + '\n#line 1 "oracle_tally/tally_api.c"\n' + open(_API_C).read())
     os.replace(_SRC + ".tmp", _SRC)
     cc = os.environ.get("CC", "gcc")
     flags = ["-O3", "-march=x86-64-v2", "-fwrapv", "-fPIC", "-Wall", "-Wextra", "-Wno-unused-parameter", "-pthread", "-shared",
@@ -164,6 +214,8 @@ def lib(blend=False):
         L.dvo_encode_cmds_cov.argtypes = [vp, op, vp]
         L.dvo_encode_cmds_forged.argtypes = [vp, op, vp, vp, ctypes.c_size_t, vp, ctypes.c_size_t, szp, u64p]
         L.dvo_tally_cmds.argtypes = [vp, op, u64p]
+        L.dvo_bill_cmds.argtypes = [vp, op, u64p, vp]
+        L.dvo_bill_raw.argtypes = [vp, ctypes.c_size_t, op, ctypes.c_int, ctypes.c_int, u64p, vp]
         L.dvo_lz77_cmds_parse.argtypes = [vp, ctypes.c_size_t, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, vp]
         L.dvo_lz77_cmds_dict_parse.argtypes = [vp, ctypes.c_size_t] + [ctypes.c_int] * 6 + [vp]
         L.dvo_lz77_cmds_words_parse.argtypes = [vp, ctypes.c_size_t] + [ctypes.c_int] * 7 + [vp]
@@ -515,3 +567,22 @@ def encode_cmds_choose(lists, blend=False, **kw):
     rc = lib(blend).dvo_encode_cmds_choose(ptrs, k, ctypes.byref(options(blend, **kw)), _p(out), cap, ctypes.byref(n), ctypes.byref(ch),
                                            _p(costs))
     return rc, out[: n.value].tobytes() if rc == SUCCESS else None, ch.value, costs
+
+
+# ---- billing by coder state (include/divans_b200.h) ----
+def bill_cmds(cmds, blend=False, **kw):
+    """(rc, cost, rows [len(BILL_ROWS), 2] u64): tally_cmds with each nibble's cost and a count of one added to the row of the
+    encoder substate that coded it (dvo_bill_cmds); rows.sum(axis=0)[0] == cost, and all zeros where the encoder refuses the list"""
+    c = ctypes.c_uint64(0)
+    rows = np.zeros((len(BILL_ROWS), 2), np.uint64)
+    rc = lib(blend).dvo_bill_cmds(ctypes.addressof(cmds.c), ctypes.byref(options(blend, **kw)), ctypes.byref(c), _p(rows))
+    return rc, c.value, rows
+
+
+def bill_raw(data, pred_mode=0, mixing_value=4, blend=False, **kw):
+    """bill_cmds for the raw buffer ``data`` coded as tally_raw codes it (dvo_bill_raw)"""
+    d = _u8(data)
+    c = ctypes.c_uint64(0)
+    rows = np.zeros((len(BILL_ROWS), 2), np.uint64)
+    rc = lib(blend).dvo_bill_raw(_p(d), len(data), ctypes.byref(options(blend, **kw)), pred_mode, mixing_value, ctypes.byref(c), _p(rows))
+    return rc, c.value, rows
